@@ -53,12 +53,14 @@ if ROOT not in sys.path:
 import workloads  # noqa: E402
 
 METRIC = "weight-sync GB/s (state_dict bytes / wall s)"
-NVLINK_MEASURED_GBPS = 770.0  # peer copy per direction per GPU, B200_PROFILING.md
-NVLINK_NOMINAL_GBPS = 900.0
-# measured with both directions busy (tools/p2p_bidir.py, profiles/r2_p2p_bidirectional.json): two GPUs pulling 4 GiB from each
-# other at once, HBM otherwise idle -- the read requests of one direction share the wire with the responses of the other
-# (ncu: 0.19 B of request traffic per payload byte with the TMA ring, 0.25 with LDG.128).  One-way the same pull runs at 790.
-NVLINK_BIDIR_MEASURED_GBPS = 676.0
+# H100 SXM data sheet: NVLink 4 moves 900 GB/s per GPU counting both directions, 450 GB/s each way.  The
+# peer-copy rate reached on an H100 box has not been measured, so the NVLink roofline uses the nominal figure.
+NVLINK_NOMINAL_GBPS = 450.0
+# device-to-device copy of 4 GiB, read + write bytes over time (tools/hbm_copy_peak.py), measured on an
+# H100 80GB HBM3 (SXM) at a 400 W power limit; the data sheet's 3.35 TB/s is for 700 W
+HBM_COPY_MEASURED_GBPS = 3026.0
+# --dump-outputs writes at most this many bytes in all (every rank together)
+DUMP_BUDGET_BYTES = 64 << 20
 
 
 # =================================================================================================
@@ -69,17 +71,7 @@ def load_peaks():
     if os.path.exists(path):
         with open(path) as f:
             return json.load(f), "measured (MEASURED_PEAKS.json)"
-    return {"hbm_gbs": 6650.0}, "fallback (B200_PROFILING.md)"
-
-
-def load_traffic(n: int):
-    """Per-launch DRAM / NVLink bytes of the dominant kernel from the committed ncu captures
-    (profiles/ncu_traffic.json, regenerated by tools/ncu_traffic.py -- never edited by hand)."""
-    path = os.path.join(ROOT, "profiles", "ncu_traffic.json")
-    try:
-        return json.load(open(path)).get(str(n))
-    except Exception:
-        return None
+    return {"hbm_gbs": HBM_COPY_MEASURED_GBPS}, "measured D2D copy peak (H100 80GB HBM3, 400 W power limit)"
 
 
 class ClockSampler:
@@ -194,7 +186,7 @@ def cpu_reference_run(n_ranks: int, steps: int, warmup: int, budget_s: float = 2
     get = every stored rectangle that intersects the wanted slice copied segment -> destination
     (shared_memory.py:473-476, client.py:284-314).  Byte movement by oracle/copy_rects_ref.c with
     all host threads; Python/RPC/pickle overhead of the real reference is NOT included (favours it;
-    profiles/r1_port_vs_reference_cpu*.json calibrates the port against the real reference).
+    oracle/calibrate_port.py calibrates the port against the real reference).
 
     Workload: the Llama-3-8B FSDP(n)->TP(n) sync, all n source and n destination ranks emulated in
     one address space -- the FULL 291-tensor layout when host RAM allows (3 x 16 GB), else the first
@@ -321,7 +313,7 @@ def cpu_reference_run(n_ranks: int, steps: int, warmup: int, budget_s: float = 2
         "kind": "port",
         "full_layout": use_full,
         "sample_bytes": sample_bytes,
-        # measured in the build container against the UNMODIFIED reference (profiles/r1_port_vs_reference_cpu*.json):
+        # measured on the host CPU against the UNMODIFIED reference (oracle/calibrate_port.py):
         # the port moves bytes 1.3-2.6x faster than the reference's Python/pickle/asyncio path
         "port_over_reference": [1.3, 2.6],
         "sample": (f"{what} ({sample_bytes} B of bf16, {len(put_list)} put copies + {len(get_specs)} get rectangles) "
@@ -574,6 +566,27 @@ def verify_flat(ctx: Ctx, sh, tag: str):
         raise SystemExit(f"[rank {ctx.rank}] PARITY FAILURE after {tag}: {bad[:5]} ({len(bad)} tensors differ bitwise)")
 
 
+def dump_outputs(ctx: Ctx, tensors: dict, out_dir: str):
+    """Write what the timed path delivered: every destination tensor as DIR/<name>.npy in float32
+    (rank<r>.<name>.npy when N > 1).  A tensor larger than its share of the budget is sampled at a
+    fixed, seeded set of element positions, so two builds run with the same arguments can be compared
+    file for file."""
+    import numpy as np
+
+    torch = ctx.torch
+    os.makedirs(out_dir, exist_ok=True)
+    header = 128  # .npy header of a 1-D array
+    per_tensor = (DUMP_BUDGET_BYTES // ctx.world // max(1, len(tensors)) - header) // 4
+    prefix = f"rank{ctx.rank}." if ctx.world > 1 else ""
+    for i, (name, t) in enumerate(tensors.items()):
+        flat = t.reshape(-1)
+        if flat.numel() > per_tensor:
+            gen = torch.Generator().manual_seed(i)
+            idx = torch.randint(0, flat.numel(), (per_tensor,), generator=gen).sort().values
+            flat = flat[idx.to(flat.device)]
+        np.save(os.path.join(out_dir, f"{prefix}{name}.npy"), flat.float().cpu().numpy())
+
+
 def full_box(name, shape, tp):
     return (0,) * len(shape), tuple(shape)
 
@@ -623,31 +636,25 @@ async def timed_steps(ctx: Ctx, step, kernel_ms_of, zero=None):
                 launches=int(ctx.allsum(launches)), clocks=clocks)
 
 
-def roofline_for(n_remote_bound: bool, info, kern_ms, n_for_traffic):
+def roofline_for(n_remote_bound: bool, info, kern_ms):
     """HBM-bound launches: bytes read locally + bytes written, vs the measured HBM copy peak.
-    NVLink-bound launches: bytes pulled from peers vs the measured per-direction peer-copy rate."""
+    NVLink-bound launches: bytes pulled from peers vs the nominal per-direction NVLink rate.
+    `traffic` (DRAM bytes counted by the hardware) is not measured: null."""
     peaks, peak_src = load_peaks()
     local_read = info["src_bytes"] - info["remote_src_bytes"]
     algo_hbm = local_read + info["payload_bytes"]
     kern_s = max(kern_ms, 1e-9) / 1e3
-    tr = load_traffic(n_for_traffic)
-    traffic = tr.get("dram_bytes") if isinstance(tr, dict) else tr
     if not n_remote_bound:
         return {"bound": "hbm", "achieved": algo_hbm / kern_s / 1e9, "peak": peaks["hbm_gbs"], "unit": "GB/s",
-                "frac": algo_hbm / kern_s / 1e9 / peaks["hbm_gbs"], "traffic": traffic,
-                "traffic_source": tr.get("source") if isinstance(tr, dict) else None,
+                "frac": algo_hbm / kern_s / 1e9 / peaks["hbm_gbs"], "traffic": None, "traffic_source": "not measured",
                 "peak_source": peak_src, "kernel": "copy_rects_kernel<KIND_B16>",
                 "algorithmic_bytes_per_launch": algo_hbm, "kernel_ms_avg": kern_ms}
     nvl = info["remote_src_bytes"] / kern_s / 1e9
     # this GPU's HBM also serves the peers' reads of its shards (symmetric plans: as many bytes out as in)
     hbm_bytes = algo_hbm + info["remote_src_bytes"]
-    return {"bound": "nvlink", "achieved": nvl, "peak": NVLINK_MEASURED_GBPS, "unit": "GB/s",
-            "frac": nvl / NVLINK_MEASURED_GBPS, "traffic": traffic,
-            # symmetric jobs pull in both directions at once: the measured two-way peer-pull rate is the tighter bound
-            "bidirectional_peak": NVLINK_BIDIR_MEASURED_GBPS, "frac_of_bidirectional_peak": nvl / NVLINK_BIDIR_MEASURED_GBPS,
-            "nvlink_traffic": tr.get("nvlrx_bytes") if isinstance(tr, dict) else None,
-            "traffic_source": tr.get("source") if isinstance(tr, dict) else None,
-            "peak_source": "measured peer copy 770 GB/s/dir (B200_PROFILING.md); nominal 900",
+    return {"bound": "nvlink", "achieved": nvl, "peak": NVLINK_NOMINAL_GBPS, "unit": "GB/s",
+            "frac": nvl / NVLINK_NOMINAL_GBPS, "traffic": None, "nvlink_traffic": None, "traffic_source": "not measured",
+            "peak_source": "nominal NVLink 4 per direction (H100 SXM data sheet); peer-copy rate not measured",
             "kernel": "copy_rects_kernel<KIND_B16> (copy warps: local HBM; link warp: TMA bulk over NVLink)",
             "algorithmic_bytes_per_launch": info["remote_src_bytes"], "kernel_ms_avg": kern_ms,
             "hbm": {"achieved": hbm_bytes / kern_s / 1e9, "peak": peaks["hbm_gbs"],
@@ -782,6 +789,8 @@ async def cfg_headline(ctx: Ctx):
 
     timed = await timed_steps(ctx, step, lambda: dest_sync.last_pull_ms[ctx.local_rank], zero=lambda: dst_flat.zero_())
     verify_flat(ctx, sh, "timed steps")
+    if args.dump_outputs:
+        dump_outputs(ctx, sh["dst"], args.dump_outputs)
     if rank == 0 and os.environ.get("TSB_BENCH_LIST_CONTEXTS"):
         # evidence that no rank holds a stray CUDA context on another rank's GPU (round-1 DeviceGuard bug)
         try:
@@ -899,7 +908,7 @@ async def cfg_headline(ctx: Ctx):
     steps = args.steps
     value = sd_bytes * steps / (timed["dev_ms"] / 1e3) / 1e9
     e2e = sd_bytes * steps / (e2e_ms / 1e3) / 1e9 if e2e_ms else None
-    roofline = roofline_for(n > 1, info, timed["kern_avg"], n)
+    roofline = roofline_for(n > 1, info, timed["kern_avg"])
     return base_line(
         ctx, value, timed["dev_ms"] / steps,
         f"llama3-8b bf16 state_dict ({len(layout)} tensors) FSDP({n}) Shard(0) -> TP({n}) direct_weight_sync via "
@@ -1009,7 +1018,7 @@ async def cfg_disjoint(ctx: Ctx):
         return None
     steps = args.steps
     value = sd_bytes * steps / (timed["dev_ms"] / 1e3) / 1e9
-    roofline = roofline_for(True, info, timed["kern_avg"], f"4p_{n}")
+    roofline = roofline_for(True, info, timed["kern_avg"])
     return base_line(
         ctx, value, timed["dev_ms"] / steps,
         f"llama3-8b bf16 state_dict FSDP({half}) on GPUs 0..{half - 1} -> TP({half}) on GPUs {half}..{n - 1} "
@@ -1074,7 +1083,7 @@ async def cfg_flat2(ctx: Ctx):
     timed, info = results["bf16"]
     itimed, _ = results["int32"]
     value = nbytes * steps / (timed["dev_ms"] / 1e3) / 1e9
-    roofline = roofline_for(True, info, timed["kern_avg"], "2")
+    roofline = roofline_for(True, info, timed["kern_avg"])
     return base_line(
         ctx, value, timed["dev_ms"] / steps,
         "direct_weight_sync of one flat 4 GiB bf16 tensor GPU0 -> GPU1, same placement (single exact-match op)",
@@ -1150,10 +1159,10 @@ async def cfg_replicated(ctx: Ctx, all_readers: bool):
     readers = n if all_readers else 1
     remote_in = sd_bytes * (n - 1) // n  # bytes each reader ingests over NVLink
     if info is not None:
-        roofline = roofline_for(n > 1, info, timed["kern_avg"], f"3{'b' if all_readers else 'a'}_{n}")
+        roofline = roofline_for(n > 1, info, timed["kern_avg"])
     else:
         nvl = remote_in / (timed["kern_avg"] / 1e3) / 1e9
-        roofline = {"bound": "nvlink", "achieved": nvl, "peak": NVLINK_MEASURED_GBPS, "unit": "GB/s", "frac": nvl / NVLINK_MEASURED_GBPS,
+        roofline = {"bound": "nvlink", "achieved": nvl, "peak": NVLINK_NOMINAL_GBPS, "unit": "GB/s", "frac": nvl / NVLINK_NOMINAL_GBPS,
                     "traffic": None, "kernel": "ncclAllGather (library collective, 291 calls)", "kernel_ms_avg": timed["kern_avg"],
                     "algorithmic_bytes_per_launch": remote_in}
     return base_line(
@@ -1379,7 +1388,12 @@ def main():
     ap.add_argument("--profiler-range", action="store_true",
                     help="cudaProfilerStart/Stop around the timed steps (for ncu --profile-from-start off)")
     ap.add_argument("--no-e2e", action="store_true", help="skip the host-input leg (profiling runs)")
+    ap.add_argument("--dump-outputs", metavar="DIR",
+                    help="config 4: after the timed steps, write the destination state dict of the last step as DIR/<name>.npy "
+                         "(float32; tensors over their share of 64 MiB in all are a fixed seeded sample of elements)")
     args = ap.parse_args()
+    if args.dump_outputs and (args.impl != "ours" or args.config != "4"):
+        ap.error("--dump-outputs applies to the default config 4 of --impl ours")
     args.warmup = max(args.warmup, 3) if args.impl == "ours" else args.warmup
     capture_stdout()
     if args.impl == "reference":

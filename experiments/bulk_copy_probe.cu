@@ -2,11 +2,10 @@
 //
 // Question for round 2: does a TMA bulk pipeline (cp.async.bulk global->shared->global driven by one
 // thread per CTA, mbarrier-signalled) move contiguous bytes faster than the product's LDG.128/STG.128
-// path (a) inside one GPU's HBM and (b) when the source is a peer GPU over NVLink?  Round-1 numbers
-// for the LDG path: 6.8 TB/s r+w local (1.04x the measured copy peak), 788 GB/s peer pull.
+// path (a) inside one GPU's HBM and (b) when the source is a peer GPU over NVLink?
 //
-// Build:  nvcc -gencode arch=compute_100a,code=sm_100a -O3 -lineinfo -o gpurun_out/bulk_probe experiments/bulk_copy_probe.cu
-// Run:    gpurun_out/bulk_probe [peer]        (peer: source on GPU 0, kernel on GPU 1)
+// Build:  nvcc -gencode arch=compute_90a,code=sm_90a -O3 -lineinfo -o experiments/bulk_probe.bin experiments/bulk_copy_probe.cu
+// Run:    experiments/bulk_probe.bin [peer]        (peer: source on GPU 0, kernel on GPU 1)
 #include <cuda_runtime.h>
 
 #include <cstdint>

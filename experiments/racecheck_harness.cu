@@ -1,7 +1,7 @@
 // experiments/racecheck_harness.cu -- torch-free driver for compute-sanitizer (racecheck / memcheck /
 // synccheck) of the copy_rects kernel through the C-ABI.  Not part of the product library.
 //
-// Build: nvcc -gencode arch=compute_100a,code=sm_100a -O2 -o experiments/racecheck_harness.bin \
+// Build: nvcc -gencode arch=compute_90a,code=sm_90a -O2 -o experiments/racecheck_harness.bin \
 //          experiments/racecheck_harness.cu -Iinclude -Ltorchstore_b200/lib -ltstore_b200 \
 //          -Xlinker -rpath -Xlinker '$ORIGIN/../torchstore_b200/lib'
 // Run:   compute-sanitizer --tool racecheck experiments/racecheck_harness.bin

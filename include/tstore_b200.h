@@ -1,5 +1,5 @@
 /*
- * tstore_b200.h -- C-ABI of libtstore_b200.so: the B200-native data plane behind torchstore's
+ * tstore_b200.h -- C-ABI of libtstore_b200.so: the H100-native data plane behind torchstore's
  * weight-sync hot path (ts.put/ts.get, put_state_dict/get_state_dict, direct_weight_sync).
  *
  * The reference (meta-pytorch/torchstore) is 100% Python and reaches native code only through

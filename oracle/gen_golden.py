@@ -1,7 +1,8 @@
 """TEST INFRASTRUCTURE ONLY -- generate tests/golden/* by executing the UNMODIFIED reference.
 
-Run in the build container (needs /root/reference):   python oracle/gen_golden.py
-The outputs are committed; nothing under tests/ or bench.py reads /root/reference at run time.
+Run where the reference tree is present (TORCHSTORE_REFERENCE_ROOT):
+    python oracle/gen_golden.py [fixture ...]      (no argument: regenerate every fixture)
+The outputs are committed; nothing under tests/ or bench.py reads the reference at run time.
 
 Fixtures (all produced by reference code, not by the oracle or the product):
   slice_math.json     get_slice_intersection / get_destination_view / assemble_tensor /
@@ -15,6 +16,8 @@ Fixtures (all produced by reference code, not by the oracle or the product):
                       put shards / reshard-get for the mesh pairs of tests/test_resharding_basic.py,
                       tests/test_resharding_ext.py and tests/test_tensor_slice.py (sha256 of results)
   cast_vectors.npz    torch CPU .to() bit patterns for the dtype pairs the cast kernel implements
+  reference_dropin.json  the reference's DirectWeightSyncDest._build_plan op lists for the product's
+                      NvlinkBuffer handles, and the RDMAWeightHandle / rdma_buffer duck-type surface
 """
 
 from __future__ import annotations
@@ -489,19 +492,106 @@ def gen_cast_vectors():
                 f32_to_f64=f32_to_f64)
 
 
-def main():
+# ------------------------------------------------------------------------------------------------
+DROPIN_CASES = [
+    # (global shape, n source ranks, source placement, n dest ranks, dest placement)
+    ((512, 512), 2, ("S", 0), 2, ("S", 0)),   # exact
+    ((512, 512), 4, ("S", 0), 2, ("S", 1)),   # reshard
+    ((96, 40), 4, ("S", 0), 3, ("S", 1)),     # uneven
+    ((64,), 4, ("R",), 2, ("R",)),            # replicated dedup
+    ((128, 64), 8, ("S", 0), 1, ("R",)),      # replicated reader (config 3)
+]
+
+
+def dropin_case_id(case):
+    shape, n_src, sp, n_dst, dp = case
+    return f"{tuple(shape)}-{n_src}{tuple(sp)}->{n_dst}{tuple(dp)}"
+
+
+def gen_reference_dropin():
+    """The reference's DirectWeightSyncDest._build_plan run on handles whose rdma_buffer is the product's
+    NvlinkBuffer (descriptor only, as a destination process sees it after unpickling): per case and
+    destination rank, the op list (source rank, exact/partial, slices, receive-buffer shape); plus the
+    RDMAWeightHandle fields and the rdma_buffer methods the reference calls."""
+    import dataclasses
+    import inspect
+    import re
+
+    import torchstore.direct_weight_sync as ref
+    from torchstore.transport.types import TensorSlice as RefSlice
+
+    import workloads
+    from torchstore_b200 import direct_weight_sync as ours
+    from torchstore_b200.planner import HbmDescriptor
+
+    def fake_buffer(shape, device):
+        stride, s = [], 1
+        for e in reversed(shape):
+            stride.append(s)
+            s *= e
+        desc = HbmDescriptor(region=bytes(120), shape=tuple(shape), stride=tuple(reversed(stride)), dtype=torch.float32, device=device)
+        return ours.NvlinkBuffer(descriptor=desc)
+
+    def mk_slice(shape, n, r, placement):
+        off, shp = workloads.shard_box(shape, n, r, placement) if placement[0] == "S" else ((0,) * len(shape), tuple(shape))
+        return RefSlice(offsets=tuple(off), coordinates=(r,), global_shape=tuple(shape), local_shape=tuple(shp), mesh_shape=(n,))
+
+    cases = {}
+    saved = ref._request_to_slice
+    try:
+        for case in DROPIN_CASES:
+            shape, n_src, sp, n_dst, dp = case
+            per_rank = {}
+            for drank in range(n_dst):
+                handles, rank_of = [], {}
+                for r in range(n_src):
+                    rs = mk_slice(shape, n_src, r, sp)
+                    if 0 in rs.local_shape:
+                        continue
+                    buf = fake_buffer(rs.local_shape, r)
+                    rank_of[id(buf)] = r
+                    handles.append(ref.RDMAWeightHandle(rdma_buffer=buf, tensor_slice=rs, source_rank=r))
+                ds = mk_slice(shape, n_dst, drank, dp)
+                if 0 in ds.local_shape:
+                    continue
+                dest = torch.zeros(ds.local_shape, dtype=torch.float32)
+                ref._request_to_slice = lambda req, param, _s=ds: _s
+                ops = ref.DirectWeightSyncDest()._build_plan({"w": handles}, {"w": dest})
+                per_rank[str(drank)] = [{
+                    "source_rank": rank_of[id(op.rdma_buffer)],
+                    "exact": op.dest_tensor is None,
+                    "src_slices": None if op.dest_tensor is None else [[s.start, s.stop] for s in op.src_slices],
+                    "dest_slices": None if op.dest_tensor is None else [[s.start, s.stop] for s in op.dest_slices],
+                    "recv_shape": None if op.dest_tensor is None else list(op.recv_buffer.shape),
+                } for op in ops]
+            cases[dropin_case_id(case)] = per_rank
+    finally:
+        ref._request_to_slice = saved
+    return {
+        "cases": cases,
+        "handle_fields": [f.name for f in dataclasses.fields(ref.RDMAWeightHandle)],
+        "buffer_methods_called": sorted(set(re.findall(r"rdma_buffer\.(\w+)\(", inspect.getsource(ref)))),
+    }
+
+
+def main(only=None):
     ref_harness.import_reference()
     os.makedirs(GOLDEN, exist_ok=True)
     meta = {"reference_commit": "ed2ddb67", "torch": torch.__version__, "generator": "oracle/gen_golden.py"}
-    for name, fn in (("slice_math", gen_slice_math), ("direct_plan", gen_direct_plan), ("store_reshard", gen_store_reshard)):
+    for name, fn in (("slice_math", gen_slice_math), ("direct_plan", gen_direct_plan), ("store_reshard", gen_store_reshard),
+                     ("reference_dropin", gen_reference_dropin)):
+        if only and name not in only:
+            continue
         data = fn()
         data["_meta"] = meta
         with open(os.path.join(GOLDEN, name + ".json"), "w") as f:
             json.dump(data, f, separators=(",", ":"))
         print(name, os.path.getsize(os.path.join(GOLDEN, name + ".json")), "bytes")
+    if only and "cast_vectors" not in only:
+        return
     np.savez_compressed(os.path.join(GOLDEN, "cast_vectors.npz"), **gen_cast_vectors())
     print("cast_vectors", os.path.getsize(os.path.join(GOLDEN, "cast_vectors.npz")), "bytes")
 
 
 if __name__ == "__main__":
-    main()
+    main(sys.argv[1:] or None)

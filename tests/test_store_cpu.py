@@ -136,7 +136,7 @@ def test_other_transports_are_rejected(kind):
     async def main():
         await ts.initialize(num_storage_volumes=1, strategy=ts.ControllerStorageVolumes(getattr(ts.TransportType, kind)))
         try:
-            with pytest.raises(RuntimeError, match="not part of the B200 build"):
+            with pytest.raises(RuntimeError, match="not part of the torchstore_b200 build"):
                 await ts.put("x", 1)
         finally:
             await ts.shutdown()

@@ -1,4 +1,4 @@
-"""torchstore_b200 -- B200-native weight-sync path behind torchstore's API.
+"""torchstore_b200 -- H100-native weight-sync path behind torchstore's API.
 
 ``import torchstore_b200 as ts`` gives the reference package's public names (torchstore/__init__.py:47-69):
 store lifecycle (initialize, initialize_spmd, shutdown, client, reset_client), key/value calls (put, get, put_batch,

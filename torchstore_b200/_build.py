@@ -1,4 +1,4 @@
-"""In-tree build of libtstore_b200.so (nvcc, sm_100a).  No torch extension machinery: the
+"""In-tree build of libtstore_b200.so (nvcc, sm_90a: H100).  No torch extension machinery: the
 library is a plain C-ABI shared object loaded with ctypes (see ``_native.py``)."""
 
 from __future__ import annotations
@@ -17,7 +17,7 @@ HEADERS = [os.path.join(CSRC, "tsb_internal.h"), os.path.join(REPO_ROOT, "includ
 
 NVCC_FLAGS = [
     "-gencode",
-    "arch=compute_100a,code=sm_100a",
+    "arch=compute_90a,code=sm_90a",
     "-lineinfo",
     "-O3",
     "-std=c++17",

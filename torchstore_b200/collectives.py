@@ -12,10 +12,9 @@ The reference has no equivalent: each reader fetches all N shards itself
 (``client.py:292-314``).  This module is device-agnostic plumbing around the collective, so its
 logic is exercised by a world-size-2 gloo test on the CPU; the GPU hot path is NCCL's.
 
-Status (round 2): measured against the P2P path through ``bench.py --config 3b [--allgather]``
-(profiles/r2_bench_*cfg3b*.json): the one-sided pulls win (one copy_rects launch per reader vs one
-NCCL collective per tensor), so the route stays **off by default**; TORCHSTORE_B200_ALLGATHER=1
-selects it.  ``tests/test_gpu_multi.py`` runs it over NCCL on two GPUs.
+Status: the one-sided pulls need one copy_rects launch per reader where this route needs one NCCL
+collective per tensor, so the route stays **off by default** (compare with ``bench.py --config 3b
+[--allgather]``; not measured on H100); TORCHSTORE_B200_ALLGATHER=1 selects it.  ``tests/test_gpu_multi.py`` runs it over NCCL on two GPUs.
 """
 
 from __future__ import annotations

@@ -1,4 +1,4 @@
-// copy_rects: the reshard kernel of libtstore_b200 (sm_100a).
+// copy_rects: the reshard kernel of libtstore_b200 (sm_90a, H100).
 //
 // One persistent launch moves every rectangle of a compiled plan: local-shard slice -> (peer or
 // local) gather into the destination shard, with the optional dtype cast fused into the store.

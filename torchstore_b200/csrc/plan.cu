@@ -117,9 +117,9 @@ constexpr uint64_t kMaxUnitsPerRow = 1ull << 30;
 
 struct Tuning {
   uint32_t tile_units = 4096;       // copy queue: 64 KiB tiles
-  // link queue: one ring stage per tile.  3 stages x 4 KiB (8 KiB of loads in flight per CTA, 3.5 MB
-  // per GPU) measured best on the 2-GPU emulation of the FSDP(8/4/2)->TP syncs: deeper rings only
-  // lengthen the queues at the source GPU, whose HBM is busy with its own copy (profiles/r2_sweep_x2_*)
+  // link queue: one ring stage per tile.  3 stages x 4 KiB (8 KiB of loads in flight per CTA): deeper
+  // rings only lengthen the queues at a source GPU whose HBM is busy with its own copy.  The multi-GPU
+  // ring geometry has not been re-measured on H100; TSB_LINK_STAGES / TSB_LINK_STAGE_BYTES override it.
   uint32_t link_tile_units = 256;
   uint32_t link_stages = 3;
   bool link_stages_auto = true;     // no TSB_LINK_STAGES: pick the depth from the number of source GPUs
@@ -395,9 +395,9 @@ int compile(int device, const tsb_rect_t* rects, uint64_t n, uint32_t flags, con
   for (uint32_t t : c.rect_tiles) total += t;
   if (total >= (1ull << 32)) return fail(TSB_ERR_UNSUPPORTED, "plan has more than 2^32 tiles");
   if (c.tune.link_stages_auto) {
-    // Ring depth by fan-in, measured on the real jobs (profiles/r2_bench_8gpu_sweep_n{4,8}.json): with 7 source
-    // GPUs each NVSwitch path carries 1/7 of the stream and 6 stages win (0.815 vs 0.851 ms at N=8); with
-    // <= 3 sources the deeper ring only lengthens the queues at the busy sources (1.56 vs 1.48 ms at N=4).
+    // Ring depth by fan-in: with many source GPUs each NVSwitch path carries a small share of the stream and
+    // a deeper ring keeps enough bytes in flight; with <= 3 sources the deeper ring only lengthens the
+    // queues at the busy sources.
     std::set<int32_t> sources;
     for (size_t i = 0; i < c.rects.size(); ++i)
       if (c.rects[i].link) sources.insert(c.rect_src_device[i]);

@@ -397,7 +397,7 @@ class DirectWeightSyncDest:
                 )
             if not isinstance(op.rdma_buffer, NvlinkBuffer):
                 raise TypeError(
-                    f"handle for '{op.name}' carries a {type(op.rdma_buffer).__name__}; the B200 path needs NvlinkBuffer handles"
+                    f"handle for '{op.name}' carries a {type(op.rdma_buffer).__name__}; the direct path needs NvlinkBuffer handles"
                 )
             dev = dest.device.index
             per_device[dev].append(self.op_windows(op, op.rdma_buffer.window(dev)))

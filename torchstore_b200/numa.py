@@ -1,7 +1,7 @@
 """NUMA placement of host staging memory.
 
 On an 8-GPU box the GPUs hang off two CPU sockets; a pinned host buffer that lives on the other
-socket's DRAM halves the H2D rate of a rank (SCALE_r01: 54 GB/s per GPU at N<=4, 30 GB/s at N=8).
+socket's DRAM lowers the H2D rate of a rank.
 The reference pins its shm segments with ``cudaHostRegister`` wherever the kernel happened to
 place them (transport/shared_memory.py:55-96); here the staging buffer of a rank is first-touched by
 a thread bound to the cores of the GPU's own NUMA node and only then page-locked.

@@ -1,4 +1,4 @@
-"""Transport registry.  The B200 build ships two data tiers: the NVLink/HBM transport
+"""Transport registry.  This build ships two data tiers: the NVLink/HBM transport
 (``transport/hbm.py``, the default wherever a CUDA device exists) and the host tier
 (``transport/host.py``: POSIX shm volumes for CPU clients and GPU-less boxes, the reference's
 ``TransportType.SharedMemory``), plus the by-value ``TransportType.MonarchRPC`` transport
@@ -55,7 +55,7 @@ def create_transport_buffer(storage_volume_ref: "StorageVolumeRef") -> Transport
 
         return ActorRpcTransportBuffer(storage_volume_ref)
     raise RuntimeError(
-        f"transport {transport_type.name} is not part of the B200 build; use TransportType.NVLink (HBM volumes), "
+        f"transport {transport_type.name} is not part of the torchstore_b200 build; use TransportType.NVLink (HBM volumes), "
         "TransportType.SharedMemory (host tier), TransportType.MonarchRPC (by value through the actor RPC) or leave "
         "default_transport_type unset"
     )

@@ -1,4 +1,4 @@
-"""NVLink / HBM transport: the storage-volume data plane of the B200 build.
+"""NVLink / HBM transport: the storage-volume data plane of this build.
 
 Implements the ``TransportBuffer`` contract (transport/buffers.py) the way the reference's
 ``SharedMemoryTransportBuffer`` does (transport/shared_memory.py:263-483), with HBM instead of
