@@ -313,6 +313,42 @@ def test_fast_lane_replays_put_and_get_and_invalidates_on_layout_change():
     run(main())
 
 
+def test_failed_recorded_get_batch_destroys_its_plans(monkeypatch):
+    """A recorded in-place get_batch that fails after its transports compiled their native plans
+    leaves no recording behind and destroys every plan it created."""
+    from torchstore_b200.client import LocalClient
+
+    async def main():
+        await ts.initialize()
+        try:
+            cl = await ts.client()
+            src = {f"w{i}": torch.randn(65, 33, device=DEV) for i in range(3)}
+            await ts.put_batch(src)
+            created = []
+            real_create = _native.plan_create
+
+            def plan_create(*args, **kwargs):
+                created.append(real_create(*args, **kwargs))
+                return created[-1]
+
+            async def assemble_fails(self, *args):
+                raise RuntimeError("assemble failed")
+
+            monkeypatch.setattr(_native, "plan_create", plan_create)
+            monkeypatch.setattr(LocalClient, "_assemble_results", assemble_fails)
+            with pytest.raises(RuntimeError, match="assemble failed"):
+                await ts.get_batch({k: torch.zeros_like(v) for k, v in src.items()})
+            assert created and not cl._recordings
+            for plan in created:
+                with pytest.raises(_native.TsbError) as err:
+                    _native.plan_info(plan)
+                assert err.value.code == _native.TSB_ERR_NOTFOUND
+        finally:
+            await ts.shutdown()
+
+    run(main())
+
+
 def test_put_batch_wait_false_overlaps_and_completes():
     async def main():
         await ts.initialize()

@@ -313,12 +313,10 @@ def plan_launch(plan: int, caller_stream: int | None = None, fence_out: bool = T
                                       0 if fence_out else TSB_LAUNCH_NO_FENCE_OUT))
 
 
-_poll_flag = C.c_int(0)
-
-
 def plan_poll(plan: int) -> bool:
-    check(lib().tsb_plan_poll(plan, C.byref(_poll_flag)))
-    return bool(_poll_flag.value)
+    done = C.c_int(0)  # per call: ctypes drops the GIL, so threads may poll concurrently
+    check(lib().tsb_plan_poll(plan, C.byref(done)))
+    return bool(done.value)
 
 
 def plan_wait(plan: int) -> None:

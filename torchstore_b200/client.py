@@ -10,7 +10,6 @@ destination the bounding box is gathered on the GPU first and moved to the host 
 from __future__ import annotations
 
 import asyncio
-import collections
 from collections import defaultdict
 from dataclasses import dataclass
 from logging import getLogger
@@ -19,10 +18,13 @@ from typing import Any
 import torch
 from torch.distributed.tensor import DTensor
 
+from torchstore_b200 import _native
 from torchstore_b200.controller import ObjectType
+from torchstore_b200.launch import SessionLRU, wait_copy_stream
 from torchstore_b200.logging import LatencyTracker
 from torchstore_b200.strategy import TorchStoreStrategy
 from torchstore_b200.transport import Request, TensorSlice, create_transport_buffer
+from torchstore_b200.transport.hbm import get_result_device
 from torchstore_b200.utils import (
     assemble_tensor,
     get_destination_region,
@@ -79,6 +81,10 @@ class _GetSession:
     parts: list  # HbmSession per volume
     final: dict  # key -> the caller's destination object
 
+    def close(self) -> None:
+        for p in self.parts:
+            p.close()
+
 
 class LocalClient:
     MAX_GET_SESSIONS = 64
@@ -86,7 +92,7 @@ class LocalClient:
     def __init__(self, controller, strategy) -> None:
         self._controller = controller
         self.strategy: TorchStoreStrategy = strategy
-        self._get_sessions: "collections.OrderedDict[tuple, _GetSession]" = collections.OrderedDict()
+        self._get_sessions = SessionLRU(self.MAX_GET_SESSIONS)
         self._recordings: dict = {}  # signature of a get being recorded -> (controller epoch, transports)
         self.get_session_hits = 0
 
@@ -165,10 +171,13 @@ class LocalClient:
             if replay is not None:
                 tracker.track_e2e()
                 return replay
-        results = await self._fetch(requests, record_sig=sig)
-        tracker.track_step("fetch")
-        final = {r.key: self._apply_inplace(results[r.key], inplace.get(r.key), r) for r in requests}
-        self._finish_get_session(sig, requests, results, final)
+        results = final = None
+        try:
+            results = await self._fetch(requests, record_sig=sig)
+            tracker.track_step("fetch")
+            final = {r.key: self._apply_inplace(results[r.key], inplace.get(r.key), r) for r in requests}
+        finally:
+            self._finish_get_session(sig, requests, results, final)
         tracker.track_e2e()
         return final
 
@@ -198,13 +207,12 @@ class LocalClient:
         else:
             got = await asyncio.gather(self._controller.get_epoch.call_one(), *[p.valid() for p in sess.parts])
         if got[0] != sess.controller_epoch or not all(got[1:]):
-            self._drop_get_session(sig)
+            self._get_sessions.drop(sig)
             return None
-        self._get_sessions.move_to_end(sig)
         for p in sess.parts:
-            p.launch()
+            p.plans.launch()
         for p in sess.parts:
-            await p.wait()
+            await p.plans.wait()
         self.get_session_hits += 1
         return dict(sess.final)
 
@@ -216,35 +224,26 @@ class LocalClient:
 
         return epoch_board.attached(info[0])
 
-    def _drop_get_session(self, sig) -> None:
-        sess = self._get_sessions.pop(sig, None)
-        if sess is not None:
-            for p in sess.parts:
-                p.close()
-
     def _finish_get_session(self, sig, requests, results, final) -> None:
-        """Keep what a recorded fetch produced if (and only if) every result landed in place."""
+        """Keep what a recorded fetch produced if (and only if) it succeeded (``final`` is set) and
+        every result landed in place; otherwise close every plan it recorded."""
         recorded = self._recordings.pop(sig, None) if sig is not None else None
         if recorded is None:
             return
         epoch, transports = recorded
         parts = [t.take_session() for t in transports]
-        inplace_ok = all(results[r.key] is not None and isinstance(results[r.key], torch.Tensor)
-                         and results[r.key].data_ptr() == r.tensor_val.data_ptr() for r in requests)
+        inplace_ok = final is not None and all(
+            results[r.key] is not None and isinstance(results[r.key], torch.Tensor)
+            and results[r.key].data_ptr() == r.tensor_val.data_ptr() for r in requests)
         if epoch is None or not inplace_ok or any(p is None for p in parts):
             for p in parts:
                 if p is not None:
                     p.close()
             return
-        self._drop_get_session(sig)
-        self._get_sessions[sig] = _GetSession(epoch, parts, dict(final))
-        while len(self._get_sessions) > self.MAX_GET_SESSIONS:
-            old, _ = next(iter(self._get_sessions.items()))
-            self._drop_get_session(old)
+        self._get_sessions.put(sig, _GetSession(epoch, parts, dict(final)))
 
     def close_sessions(self) -> None:
-        for sig in list(self._get_sessions):
-            self._drop_get_session(sig)
+        self._get_sessions.clear()
         info = getattr(self.strategy, "epoch_board", None)
         if info:
             from torchstore_b200 import epoch_board
@@ -379,16 +378,13 @@ class LocalClient:
         return final
 
     async def _to_result_device(self, gathered: torch.Tensor) -> torch.Tensor:
-        from torchstore_b200 import _native
-        from torchstore_b200.transport.hbm import _wait, get_result_device
-
         if get_result_device() == "cuda" or not gathered.is_cuda:
             return gathered
         host = torch.empty(gathered.shape, dtype=gathered.dtype)
         dev = gathered.device.index
         _native.memcpy_async(dev, host.data_ptr(), gathered.data_ptr(), gathered.numel() * gathered.element_size(),
                              _native.TSB_D2H)
-        await _wait(dev)
+        await wait_copy_stream(dev)
         return host
 
     # ---- misc -----------------------------------------------------------------------------------

@@ -27,59 +27,20 @@ Typical usage is unchanged::
 
 from __future__ import annotations
 
-import asyncio
 import logging
-import threading
 from collections import defaultdict
 from dataclasses import dataclass
 
 import torch
 
-from torchstore_b200 import _native
-from torchstore_b200.planner import HbmDescriptor, StridedMem, build_rects
+from torchstore_b200.launch import Plans, copy_once, wait_copy_stream
+from torchstore_b200.planner import HbmDescriptor, StridedMem
 from torchstore_b200.transport.types import Request, TensorSlice
 from torchstore_b200.utils import get_slice_intersection, to_byte_view
 
 logger = logging.getLogger(__name__)
 
 RDMA_KEY_PREFIX = "policy_rdma"
-
-
-async def wait_event(event: "_native.Event") -> None:
-    """Await a CUDA event without blocking the actor's event loop (the reference awaits RDMA
-    completions the same way: everything on the path is a coroutine).  Every poll goes through the
-    loop's selector, which drops the GIL, so actor-server threads keep running."""
-    spins = 0
-    while not event.query():
-        spins += 1
-        await asyncio.sleep(0 if spins < 4000 else 0.0002)
-
-
-async def wait_plan(plan: int) -> None:
-    """Await the done event of the plan's last fenced launch (tsb_plan_poll).  (Polling the last
-    stretch without yielding was tried and measured no gain: 0.048 vs 0.049 ms of host time per sync.)"""
-    spins = 0
-    poll = _native.plan_poll
-    while not poll(plan):
-        spins += 1
-        await asyncio.sleep(0 if spins < 4000 else 0.0002)
-
-
-_fence_events = threading.local()
-
-
-def _fence_in(device: int) -> None:
-    """Copy stream waits for whatever torch has queued on the caller's current stream.  One reusable
-    event per (thread, device): cudaStreamWaitEvent snapshots the record it follows, so a later
-    record on the same event does not disturb earlier waits."""
-    cache = getattr(_fence_events, "by_device", None)
-    if cache is None:
-        cache = _fence_events.by_device = {}
-    ev = cache.get(device)
-    if ev is None:
-        ev = cache[device] = _native.Event(device)
-    ev.record(_native.torch_stream(device))
-    ev.wait_on(device, None)
 
 
 # ---------------------------------------------------------------------------------------------
@@ -148,12 +109,8 @@ class NvlinkBuffer:
         device = local_bytes.device.index
         remote = self.window(device).flat_bytes()
         local = StridedMem.from_tensor(local_bytes)
-        rects, n = build_rects([(remote, local) if read else (local, remote)])
-        _fence_in(device)
-        _native.copy_rects(device, rects, n)
-        done = _native.Event(device).record(None)
-        await wait_event(done)
-        done.close()
+        copy_once({device: [(remote, local) if read else (local, remote)]})
+        await wait_copy_stream(device)
 
     async def drop(self) -> None:
         try:
@@ -196,7 +153,7 @@ class DirectWeightSyncSource:
         self._handles: dict[str, RDMAWeightHandle] = {}
         # name -> (staging_buffer, source_local_tensor)
         self._staging: dict[str, tuple[torch.Tensor, torch.Tensor]] = {}
-        self._refresh_plans: dict[int, int] = {}  # device -> native plan id
+        self._refresh_plans = Plans()
         self._devices: tuple[int, ...] = ()  # devices holding registered memory (fence targets)
 
     def register(self, state_dict: dict[str, torch.Tensor], rank: int,
@@ -207,8 +164,9 @@ class DirectWeightSyncSource:
         ``tensor_slices`` (extension) gives the global rectangle of *plain* local shards for
         callers that do not wrap them in DTensors."""
         handles: dict[str, RDMAWeightHandle] = {}
-        self._drop_plans()
+        self._refresh_plans.close()
         self._staging = {}
+        casts: dict[int, list] = defaultdict(list)  # device -> (source, staging) windows of the refresh
         devices = set()
         for name, param in state_dict.items():
             req = Request.from_any(name, param, tensor_slices.get(name) if tensor_slices else None)
@@ -220,6 +178,7 @@ class DirectWeightSyncSource:
             if transfer_dtype is not None:
                 staging = torch.empty(local.shape, dtype=transfer_dtype, device=local.device)
                 self._staging[name] = (staging, local)
+                casts[local.device.index].append((StridedMem.from_tensor(local), StridedMem.from_tensor(staging)))
                 buf = staging
             else:
                 assert local.is_contiguous(), f"Expected contiguous tensor for key={name}, strides={local.stride()}"
@@ -228,7 +187,7 @@ class DirectWeightSyncSource:
         self._handles = handles
         self._devices = tuple(sorted(devices))
         if self._staging:
-            self._build_refresh_plans()
+            self._refresh_plans = Plans.build(casts)
             self.refresh()
         else:
             # make sure the weights the handles point at are materialised before anyone reads them
@@ -238,24 +197,14 @@ class DirectWeightSyncSource:
                     len(handles) - len(self._staging))
         return handles
 
-    def _build_refresh_plans(self) -> None:
-        per_device: dict[int, list] = defaultdict(list)
-        for staging, src in self._staging.values():
-            per_device[src.device.index].append((StridedMem.from_tensor(src), StridedMem.from_tensor(staging)))
-        for dev, pairs in per_device.items():
-            rects, n = build_rects(pairs)
-            self._refresh_plans[dev] = _native.plan_create(dev, rects, n)
-
     def refresh(self) -> int:
         """Re-cast the source params into their staging buffers (no-op without transfer_dtype).
         Returns the number of staging buffers refreshed.  Blocks until the cast has landed so the
         caller may publish/notify right after, like the reference's synchronous copy loop."""
         if not self._refresh_plans:
             return 0
-        for dev, plan in self._refresh_plans.items():
-            _native.plan_launch(plan, _native.torch_stream(dev))
-        for plan in self._refresh_plans.values():
-            _native.plan_wait(plan)
+        self._refresh_plans.launch()
+        self._refresh_plans.synchronize()
         return len(self._staging)
 
     def fence(self) -> None:
@@ -265,20 +214,12 @@ class DirectWeightSyncSource:
         for dev in self._devices:
             torch.cuda.current_stream(dev).synchronize()
 
-    def _drop_plans(self) -> None:
-        for plan in self._refresh_plans.values():
-            try:
-                _native.plan_destroy(plan)
-            except Exception as e:
-                logger.warning("plan_destroy failed: %s", e)
-        self._refresh_plans = {}
-
     async def cleanup(self) -> None:
         for handle in self._handles.values():
             await handle.rdma_buffer.drop()
         self._handles.clear()
         self._staging.clear()
-        self._drop_plans()
+        self._refresh_plans.close()
 
 
 # ---------------------------------------------------------------------------------------------
@@ -313,7 +254,7 @@ class DirectWeightSyncDest:
         self._plan_ids: tuple | None = None  # id() of the destination objects the plan was built for
         self._plan_refs: list | None = None  # ...kept alive, so those ids cannot be recycled
         self._plan_dict: dict | None = None  # the dict object they came in (identity short-cut of the next pull)
-        self._native_plans: dict[int, int] = {}  # device -> plan id
+        self._native_plans = Plans()  # the compiled plan, one native plan per destination device
         self.last_pull_ms: dict[int, float] = {}  # device -> kernel time of the last pull
 
     # -- planning (host, metadata only) ----------------------------------------------------------
@@ -401,12 +342,10 @@ class DirectWeightSyncDest:
                 )
             dev = dest.device.index
             per_device[dev].append(self.op_windows(op, op.rdma_buffer.window(dev)))
-        for dev, pairs in per_device.items():
-            rects, n = build_rects(pairs)
-            self._native_plans[dev] = _native.plan_create(dev, rects, n)
+        self._native_plans = Plans.build(per_device)
 
     def plan_info(self) -> dict[int, dict]:
-        return {dev: _native.plan_info(p).as_dict() for dev, p in self._native_plans.items()}
+        return self._native_plans.info()
 
     # -- execution ---------------------------------------------------------------------------------
     async def pull(self, all_handles: dict[str, list[RDMAWeightHandle]],
@@ -460,21 +399,14 @@ class DirectWeightSyncDest:
         stream on both sides (later work on that stream sees the new weights without a host wait)."""
         if self._plan is None:
             raise RuntimeError("pull() must build the plan first")
-        for dev, plan in self._native_plans.items():
-            _native.plan_launch(plan, _native.torch_stream(dev))
+        self._native_plans.launch()
 
     async def wait(self) -> None:
-        for dev, plan in self._native_plans.items():
-            await wait_plan(plan)
-            self.last_pull_ms[dev] = _native.plan_elapsed_ms(plan)
+        await self._native_plans.wait()
+        self.last_pull_ms.update(self._native_plans.elapsed_ms())
 
     def close(self) -> None:
-        for plan in self._native_plans.values():
-            try:
-                _native.plan_destroy(plan)
-            except Exception as e:
-                logger.warning("plan_destroy failed: %s", e)
-        self._native_plans = {}
+        self._native_plans.close()
         self._plan = None
         self._plan_ids = self._plan_refs = self._plan_dict = None
 

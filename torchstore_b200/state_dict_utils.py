@@ -53,7 +53,7 @@ def reset_direct_cache(store=None) -> None:
             for d in cache.dests.values():
                 d.close()
             for src in cache.sources.values():
-                src._drop_plans()
+                src._refresh_plans.close()
 
 
 async def put_state_dict(store, state_dict, key, direct_rdma=False, transfer_dtype=None):

@@ -20,7 +20,6 @@ GET  1. volume   handle_get_request: descriptor (exported region + layout) of ea
 
 from __future__ import annotations
 
-import collections
 import logging
 import os
 import time
@@ -31,8 +30,9 @@ from typing import TYPE_CHECKING, Any
 import torch
 
 from torchstore_b200 import _native
+from torchstore_b200.launch import Plans, SessionLRU, copy_once, wait_copy_stream
 from torchstore_b200.logging import LatencyTracker
-from torchstore_b200.planner import HbmDescriptor, StridedMem, build_rects
+from torchstore_b200.planner import HbmDescriptor, StridedMem
 from torchstore_b200.transport.buffers import TransportBuffer, TransportCache
 from torchstore_b200.transport.types import Request
 
@@ -166,7 +166,7 @@ class HbmSession:
     were built under.  While the volume's epoch is unchanged no key of the batch has moved, so the
     next identical batch is ONE small RPC (the epoch check) + one launch per device."""
 
-    plans: dict  # device -> native plan id
+    plans: Plans
     epoch: int
     volume_ref: Any
     board: Any = None   # (EpochBoard, slot): read the volume's epoch from shared memory instead of by RPC
@@ -176,25 +176,8 @@ class HbmSession:
             return self.board[0].read(self.board[1]) == self.epoch
         return await self.volume_ref.volume.epoch.call_one() == self.epoch
 
-    def launch(self, fence_out: bool = True) -> None:
-        """fence_out=False (puts): the caller's stream may run ahead of the copy -- the source is only
-        read, and completion is observed on the host before the put is reported done."""
-        for dev, plan in self.plans.items():
-            _native.plan_launch(plan, _native.torch_stream(dev), fence_out=fence_out)
-
-    async def wait(self) -> None:
-        from torchstore_b200.direct_weight_sync import wait_plan
-
-        for plan in self.plans.values():
-            await wait_plan(plan)
-
     def close(self) -> None:
-        for plan in self.plans.values():
-            try:
-                _native.plan_destroy(plan)
-            except Exception as e:
-                logger.warning("plan_destroy failed: %s", e)
-        self.plans = {}
+        self.plans.close()
 
 
 class HbmClientCache(TransportCache):
@@ -207,32 +190,10 @@ class HbmClientCache(TransportCache):
 
     def __init__(self) -> None:
         self.mapped = 0
-        self.put_sessions: "collections.OrderedDict[tuple, HbmSession]" = collections.OrderedDict()
+        self.put_sessions = SessionLRU(self.MAX_SESSIONS)
         self.hits = self.misses = 0
 
-    def lookup(self, sig) -> HbmSession | None:
-        sess = self.put_sessions.get(sig)
-        if sess is not None:
-            self.put_sessions.move_to_end(sig)
-        return sess
-
-    def remember(self, sig, sess: HbmSession) -> None:
-        old = self.put_sessions.pop(sig, None)
-        if old is not None:
-            old.close()
-        self.put_sessions[sig] = sess
-        while len(self.put_sessions) > self.MAX_SESSIONS:
-            _, victim = self.put_sessions.popitem(last=False)
-            victim.close()
-
-    def forget(self, sig) -> None:
-        sess = self.put_sessions.pop(sig, None)
-        if sess is not None:
-            sess.close()
-
     def clear(self) -> None:
-        for sess in self.put_sessions.values():
-            sess.close()
         self.put_sessions.clear()
         try:
             _native.release_all()
@@ -273,14 +234,6 @@ class _PutSpec:
     dtype: torch.dtype
 
 
-async def _wait(device: int) -> None:
-    from torchstore_b200.direct_weight_sync import wait_event
-
-    done = _native.Event(device).record(None)
-    await wait_event(done)
-    done.close()
-
-
 class HbmTransportBuffer(TransportBuffer):
     supports_inplace_resharding = True
     supports_batch_puts = True
@@ -299,9 +252,9 @@ class HbmTransportBuffer(TransportBuffer):
         # identifies THIS put on the volume between handshake and put (two clients may put the same
         # key concurrently; each must get back the landing buffer it wrote into)
         self._nonce = os.urandom(8).hex()
-        self._epoch = None            # volume layout epoch seen by the volume half of a get
+        self._epoch = None            # volume layout epoch seen by the volume half of a get, or after a put
         self._record = False          # client: compile cached plans instead of one-shot copies
-        self._recorded_plans: dict[int, int] = {}
+        self._recorded_plans: Plans | None = None
         self.fast_path_hit = False    # last put was served by a cached session (no handshake, no notify)
 
     def __getstate__(self) -> dict[str, Any]:
@@ -333,37 +286,34 @@ class HbmTransportBuffer(TransportBuffer):
         """Store path fast lane: a batch that was put before (same keys, same source pointers) and
         whose landing buffers have not moved (volume epoch unchanged) replays its compiled plan --
         one epoch RPC + one launch per device, no handshake, no per-key work.  With ``wait=False`` the
-        launch is returned un-awaited (an :class:`HbmSession`; ``await sess.wait()`` completes the
-        put), so the copy runs on the side stream while the caller's compute continues."""
+        launch is returned un-awaited (the session's :class:`Plans`; ``await plans.wait()`` completes
+        the put), so the copy runs on the side stream while the caller's compute continues."""
         self._needs_handshake = True
         self.fast_path_hit = False
         cache: HbmClientCache = self.storage_volume_ref.transport_context.get(HbmClientCache)
         sig = self._put_signature(requests) if os.environ.get("TORCHSTORE_B200_FAST_LANE", "1") == "1" else None
         if sig is not None:
-            sess = cache.lookup(sig)
+            sess = cache.put_sessions.get(sig)
             if sess is not None:
                 if await sess.valid():
                     cache.hits += 1
-                    sess.launch(fence_out=False)
+                    sess.plans.launch(fence_out=False)
                     self.fast_path_hit = True
                     if not wait:
-                        return sess
-                    await sess.wait()
+                        return sess.plans
+                    await sess.plans.wait()
                     return None
-                cache.forget(sig)
+                cache.put_sessions.drop(sig)
             cache.misses += 1
             self._record = True
         try:
             await super().put_to_storage_volume(requests)
-            if self._record and self._recorded_plans and self._volume_epoch is not None:
-                cache.remember(sig, HbmSession(self._recorded_plans, int(self._volume_epoch), self.storage_volume_ref,
-                                               _board_slot(self.storage_volume_ref)))
-                self._recorded_plans = {}
+            self._epoch = self._volume_epoch
         finally:
-            for plan in self._recorded_plans.values():  # failed before the session was stored
-                _native.plan_destroy(plan)
-            self._recorded_plans = {}
+            sess = self.take_session()  # a failed put has no epoch: its recorded plans are closed
             self._record = False
+        if sess is not None:
+            cache.put_sessions.put(sig, sess)
         return None
 
     async def recv_handshake(self, ctx: "TransportContext", entries: list[tuple[Request, Any]]) -> list[Any]:
@@ -409,20 +359,7 @@ class HbmTransportBuffer(TransportBuffer):
                 keep.append(src)
                 host_copies.append((src, desc))
         tracker.track_step("plan")
-        from torchstore_b200.direct_weight_sync import _fence_in
-
-        devices = set()
-        record = self._record and not host_copies
-        for dev, pairs in per_device.items():
-            rects, n = build_rects(pairs)
-            if record:
-                # fast lane: keep the compiled tables; the next identical batch replays them
-                plan = self._recorded_plans[dev] = _native.plan_create(dev, rects, n)
-                _native.plan_launch(plan, _native.torch_stream(dev), fence_out=False)
-            else:
-                _fence_in(dev)
-                _native.copy_rects(dev, rects, n)
-            devices.add(dev)
+        devices = self._copy(per_device, record=self._record and not host_copies, fence_out=False)
         for src, desc in host_copies:
             dev = desc.device if _same_process(desc) else torch.cuda.current_device()
             dst = desc.resolve(dev)
@@ -430,8 +367,17 @@ class HbmTransportBuffer(TransportBuffer):
             devices.add(dev)
         tracker.track_step("alloc_and_copy")
         for dev in devices:
-            await _wait(dev)
+            await wait_copy_stream(dev)
         tracker.track_step("cuda_synchronize")
+
+    def _copy(self, per_device: dict[int, list], record: bool, fence_out: bool) -> set[int]:
+        """One launch per device; a recorded batch keeps its compiled plans for the next identical
+        batch to replay.  Returns the devices to wait on."""
+        if not (record and per_device):
+            return copy_once(per_device)
+        self._recorded_plans = Plans.build(per_device)
+        self._recorded_plans.launch(fence_out)
+        return set(per_device)
 
     async def handle_put_request(self, ctx: "TransportContext", entries: list[tuple[Request, Any]]) -> list[Any]:
         results = []
@@ -492,22 +438,9 @@ class HbmTransportBuffer(TransportBuffer):
                 results[i] = out
             else:
                 d2h.append((i, desc, None))
-        from torchstore_b200.direct_weight_sync import _fence_in
-
-        devices = set()
-        record = self._record and not d2h
         self._epoch = transport_buffer._epoch
-        for dev, pairs in per_device.items():
-            rects, n = build_rects(pairs)
-            if record:
-                plan = self._recorded_plans[dev] = _native.plan_create(dev, rects, n)
-                _native.plan_launch(plan, _native.torch_stream(dev))
-            else:
-                _fence_in(dev)
-                _native.copy_rects(dev, rects, n)
-            devices.add(dev)
-        if not record:
-            self._record = False  # something in this batch is not replayable (host / object results)
+        # a batch with host results is not replayable
+        devices = self._copy(per_device, record=self._record and not d2h, fence_out=True)
         staged = []
         for i, desc, dest in d2h:
             dev = desc.device if _same_process(desc) else torch.cuda.current_device()
@@ -516,8 +449,7 @@ class HbmTransportBuffer(TransportBuffer):
             # then one D2H copy
             if not src.is_contiguous():
                 bounce = torch.empty(desc.shape, dtype=desc.dtype, device=torch.device("cuda", dev))
-                rects, n = build_rects([(src, StridedMem.from_tensor(bounce))])
-                _native.copy_rects(dev, rects, n)
+                copy_once({dev: [(src, StridedMem.from_tensor(bounce))]}, fence=False)
                 src_ptr = bounce.data_ptr()
             else:
                 bounce, src_ptr = None, src.ptr
@@ -532,7 +464,7 @@ class HbmTransportBuffer(TransportBuffer):
             devices.add(dev)
             staged.append((i, dest, host, bounce))
         for dev in devices:
-            await _wait(dev)
+            await wait_copy_stream(dev)
         for i, dest, host, _bounce in staged:
             if dest is not None and host is not dest:
                 dest.copy_(host)  # non-contiguous host destination: host-side scatter of host data
@@ -542,15 +474,14 @@ class HbmTransportBuffer(TransportBuffer):
         return results
 
     def take_session(self) -> HbmSession | None:
-        """Client, after a recorded get: the replayable session of this volume's part (or None)."""
-        if not self._record or not self._recorded_plans or self._epoch is None:
-            for plan in self._recorded_plans.values():
-                _native.plan_destroy(plan)
-            self._recorded_plans = {}
+        """Client, after a recorded put or get: the replayable session of this volume's part, or None
+        with the recorded plans closed."""
+        plans, self._recorded_plans = self._recorded_plans, None
+        if plans is None or self._epoch is None:
+            if plans is not None:
+                plans.close()
             return None
-        sess = HbmSession(self._recorded_plans, int(self._epoch), self.storage_volume_ref, _board_slot(self.storage_volume_ref))
-        self._recorded_plans = {}
-        return sess
+        return HbmSession(plans, int(self._epoch), self.storage_volume_ref, _board_slot(self.storage_volume_ref))
 
     async def drop(self) -> None:
         self._contexts = []

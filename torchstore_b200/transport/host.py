@@ -31,6 +31,7 @@ from typing import TYPE_CHECKING, Any
 import torch
 
 from torchstore_b200 import _native
+from torchstore_b200.launch import fence_in, wait_copy_stream
 from torchstore_b200.planner import StridedMem, build_rects
 from torchstore_b200.transport.buffers import TransportBuffer, TransportCache
 from torchstore_b200.transport.types import Request
@@ -297,20 +298,15 @@ class HostShmTransportBuffer(TransportBuffer):
                 seg = cache.attach(desc, request.key)
                 seg.pin()
                 dev = tensor.device.index
-                from torchstore_b200.direct_weight_sync import _fence_in
-
-                _fence_in(dev)
+                fence_in(dev)
                 _native.memcpy_async(dev, landing.data_ptr(), src.data_ptr(), desc.nbytes, _native.TSB_D2H)
                 devices.add(dev)
                 self._keep = getattr(self, "_keep", []) + [src]
             else:
                 host_pairs.append((tensor, landing))
         _host_move(host_pairs)
-        if devices:
-            from torchstore_b200.transport.hbm import _wait
-
-            for dev in devices:
-                await _wait(dev)  # polled from the loop, like the HBM transport
+        for dev in devices:
+            await wait_copy_stream(dev)  # polled from the loop, like the HBM transport
         self._keep = []
 
     async def handle_put_request(self, ctx: "TransportContext", entries: list[tuple[Request, Any]]) -> list[Any]:
@@ -384,11 +380,8 @@ class HostShmTransportBuffer(TransportBuffer):
                 self._keep = getattr(self, "_keep", []) + [src]
             else:
                 dest.copy_(src)
-        if devices:
-            from torchstore_b200.transport.hbm import _wait
-
-            for dev in devices:
-                await _wait(dev)
+        for dev in devices:
+            await wait_copy_stream(dev)
         self._keep = []
         return results
 
