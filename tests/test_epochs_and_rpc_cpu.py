@@ -228,28 +228,3 @@ def test_epoch_board_also_serves_the_default_single_volume_store():
             await ts.shutdown()
 
     run(main())
-
-
-def test_session_lru_closes_what_it_replaces_evicts_drops_and_clears():
-    """The fast lane's put and get sessions hold native plans: every session leaving the cache is closed."""
-    from torchstore_b200.launch import SessionLRU
-
-    class Sess:
-        closed = False
-
-        def close(self):
-            self.closed = True
-
-    lru = SessionLRU(2)
-    a, b, c, a2 = Sess(), Sess(), Sess(), Sess()
-    lru.put("a", a)
-    lru.put("b", b)
-    assert lru.get("a") is a                 # a becomes the most recently used
-    lru.put("c", c)                          # over the cap: b, the least recently used, goes
-    assert b.closed and not a.closed and not c.closed and len(lru) == 2 and lru.get("b") is None
-    lru.put("a", a2)                         # replacing a signature closes the old session
-    assert a.closed and lru.get("a") is a2
-    lru.drop("c")
-    assert c.closed and len(lru) == 1
-    lru.clear()
-    assert a2.closed and len(lru) == 0

@@ -258,38 +258,36 @@ def test_volume_memory_is_hbm_arena_and_freed_on_delete():
     run(main())
 
 
-def test_fast_lane_replays_put_and_get_and_invalidates_on_layout_change():
+def test_client_fast_lane_replays_put_and_get_and_invalidates_on_layout_change():
     """Store-path fast lane: an identical put_batch / in-place get_batch replays its compiled plan
     (no handshake, no per-key RPC payload); any change of the volume layout (delete, reallocation)
     or of the index drops the session and the slow path takes over -- results stay bit-exact."""
-    from torchstore_b200.transport.hbm import HbmClientCache
-
     async def main():
         await ts.initialize()
         try:
             cl = await ts.client()
-            cache = cl.strategy.transport_context.get(HbmClientCache)
+            lane = cl.fast_lane
             src = {f"w{i}": torch.randn(257, 129, device=DEV) for i in range(6)}
             dst = {k: torch.zeros_like(v) for k, v in src.items()}
             await ts.put_batch(src)                       # slow path, records a session
-            assert cache.misses == 1 and cache.hits == 0 and len(cache.put_sessions) == 1
+            assert lane.put_misses == 1 and lane.put_hits == 0 and len(lane.put_sessions) == 1
             before = _native.launch_count()
             for k in src:
                 src[k].add_(1.0)
             await ts.put_batch(src)                       # replay
-            assert cache.hits == 1 and _native.launch_count() == before + 1
+            assert lane.put_hits == 1 and _native.launch_count() == before + 1
             await ts.get_batch(dst)                       # slow get, records
-            assert all(torch.equal(dst[k], src[k]) for k in src) and cl.get_session_hits == 0
+            assert all(torch.equal(dst[k], src[k]) for k in src) and lane.get_hits == 0
             for k in src:
                 src[k].mul_(-2.0)
             await ts.put_batch(src)
             out = await ts.get_batch(dst)                 # replayed get: one launch, returns the caller's objects
-            assert cl.get_session_hits == 1 and all(out[k] is dst[k] for k in dst)
+            assert lane.get_hits == 1 and all(out[k] is dst[k] for k in dst)
             assert all(torch.equal(dst[k], src[k]) for k in src)
             # a different destination set is a different session (not a false hit)
             dst2 = {k: torch.zeros_like(v) for k, v in src.items()}
             await ts.get_batch(dst2)
-            assert cl.get_session_hits == 1 and all(torch.equal(dst2[k], src[k]) for k in src)
+            assert lane.get_hits == 1 and all(torch.equal(dst2[k], src[k]) for k in src)
             # layout change: delete one key, put it back with another shape -> sessions are stale
             await ts.delete("w0")
             with pytest.raises(Exception):
@@ -299,9 +297,9 @@ def test_fast_lane_replays_put_and_get_and_invalidates_on_layout_change():
             await ts.put_batch(src)                       # new signature + stale old session
             await ts.get_batch(dst)
             assert all(torch.equal(dst[k], src[k]) for k in src)
-            hits = cache.hits
+            hits = lane.put_hits
             await ts.put_batch(src)                       # and the new batch replays again
-            assert cache.hits == hits + 1
+            assert lane.put_hits == hits + 1
             # same keys, same shapes, but the volume reallocated (dtype change) -> epoch moved
             src["w1"] = src["w1"].to(torch.float16)
             await ts.put_batch(src)
@@ -313,9 +311,9 @@ def test_fast_lane_replays_put_and_get_and_invalidates_on_layout_change():
     run(main())
 
 
-def test_failed_recorded_get_batch_destroys_its_plans(monkeypatch):
+def test_failed_recorded_get_batch_caches_no_session_and_destroys_its_plans(monkeypatch):
     """A recorded in-place get_batch that fails after its transports compiled their native plans
-    leaves no recording behind and destroys every plan it created."""
+    caches no get session and destroys every plan it created."""
     from torchstore_b200.client import LocalClient
 
     async def main():
@@ -338,11 +336,47 @@ def test_failed_recorded_get_batch_destroys_its_plans(monkeypatch):
             monkeypatch.setattr(LocalClient, "_assemble_results", assemble_fails)
             with pytest.raises(RuntimeError, match="assemble failed"):
                 await ts.get_batch({k: torch.zeros_like(v) for k, v in src.items()})
-            assert created and not cl._recordings
+            assert created and len(cl.fast_lane.get_sessions) == 0
             for plan in created:
                 with pytest.raises(_native.TsbError) as err:
                     _native.plan_info(plan)
                 assert err.value.code == _native.TSB_ERR_NOTFOUND
+        finally:
+            await ts.shutdown()
+
+    run(main())
+
+
+def test_put_batch_whose_notify_fails_records_no_session(monkeypatch):
+    """A put_batch whose notify_put_batch raises leaves its data in the volume but its keys unindexed.
+    It must not leave a put session behind: a replay skips the notify, so the identical retry has to
+    take the slow path and index the keys."""
+    from torchstore_b200 import rpc
+
+    async def main():
+        await ts.initialize()
+        try:
+            cl = await ts.client()
+            ctrl = rpc._lookup("torchstore/controller")[0]
+            real_notify = ctrl.notify_put_batch
+            failed = []
+
+            @rpc.endpoint
+            async def notify_fails_once(*args, **kwargs):
+                if not failed:
+                    failed.append(True)
+                    raise RuntimeError("notify lost")
+                return await real_notify(*args, **kwargs)
+
+            monkeypatch.setattr(ctrl, "notify_put_batch", notify_fails_once)
+            src = {f"n{i}": torch.randn(65, 33, device=DEV) for i in range(3)}
+            with pytest.raises(Exception, match="notify lost"):
+                await ts.put_batch(src)
+            assert cl.fast_lane.put_misses == 1 and len(cl.fast_lane.put_sessions) == 0
+            await ts.put_batch(src)                       # slow path again: notifies this time
+            assert cl.fast_lane.put_misses == 2 and cl.fast_lane.put_hits == 0
+            for k, v in src.items():
+                assert torch.equal(await ts.get(k), v.cpu())
         finally:
             await ts.shutdown()
 

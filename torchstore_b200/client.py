@@ -11,7 +11,6 @@ from __future__ import annotations
 
 import asyncio
 from collections import defaultdict
-from dataclasses import dataclass
 from logging import getLogger
 from typing import Any
 
@@ -20,7 +19,8 @@ from torch.distributed.tensor import DTensor
 
 from torchstore_b200 import _native
 from torchstore_b200.controller import ObjectType
-from torchstore_b200.launch import SessionLRU, wait_copy_stream
+from torchstore_b200.fast_lane import FastLane, Recording, signature
+from torchstore_b200.launch import wait_copy_stream
 from torchstore_b200.logging import LatencyTracker
 from torchstore_b200.strategy import TorchStoreStrategy
 from torchstore_b200.transport import Request, TensorSlice, create_transport_buffer
@@ -72,29 +72,11 @@ class PendingPut:
             self.done = True
 
 
-@dataclass
-class _GetSession:
-    """A replayable in-place get_batch: per-volume transport sessions plus the controller epoch the
-    volume map was read under (see HbmSession)."""
-
-    controller_epoch: int
-    parts: list  # HbmSession per volume
-    final: dict  # key -> the caller's destination object
-
-    def close(self) -> None:
-        for p in self.parts:
-            p.close()
-
-
 class LocalClient:
-    MAX_GET_SESSIONS = 64
-
     def __init__(self, controller, strategy) -> None:
         self._controller = controller
         self.strategy: TorchStoreStrategy = strategy
-        self._get_sessions = SessionLRU(self.MAX_GET_SESSIONS)
-        self._recordings: dict = {}  # signature of a get being recorded -> (controller epoch, transports)
-        self.get_session_hits = 0
+        self.fast_lane = FastLane(controller, strategy)
 
     async def _locate_volumes(self, keys: list[str]):
         try:
@@ -124,19 +106,29 @@ class LocalClient:
         volume_ref = self.strategy.select_storage_volume()
         transport = create_transport_buffer(volume_ref)
         tracker.track_step("create transport buffer")
-        if getattr(transport, "supports_fast_lane", False):
-            inflight = await transport.put_to_storage_volume(requests, wait=wait)
-        else:
-            inflight = await transport.put_to_storage_volume(requests)
-        tracker.track_step("put_to_storage_volume")
-        if not getattr(transport, "fast_path_hit", False):
-            # a replayed batch overwrote indexed keys in place: the index is already right
+        sig = signature(requests, volume_ref.volume_id) if transport.supports_fast_lane else None
+        rec = None
+        if sig is not None:
+            replay = await self.fast_lane.replay_put(sig)
+            if replay is not None:  # keys overwritten in place: the index is already right, no notify
+                if wait:
+                    await replay.wait()
+                tracker.track_e2e()
+                return None if wait else PendingPut(replay.wait)
+            rec = Recording(sig)
+            rec.attach([transport])
+        ok = False
+        try:
+            await transport.put_to_storage_volume(requests)
+            tracker.track_step("put_to_storage_volume")
             await self._controller.notify_put_batch.call([r.meta_only() for r in requests], volume_ref.volume_id)
             tracker.track_step("notify_put_batch")
+            ok = True
+        finally:
+            if rec is not None:
+                self.fast_lane.commit(rec, ok)
         tracker.track_e2e()
-        if not wait:
-            return PendingPut(inflight.wait if inflight is not None else None)
-        return None
+        return None if wait else PendingPut()
 
     # ---- get ------------------------------------------------------------------------------------
     @torch.no_grad
@@ -165,90 +157,27 @@ class LocalClient:
         else:
             raise TypeError(f"get_batch expects list[str] or dict, got {type(keys)}")
         requests = [Request.from_any(k, inplace.get(k)) for k in keys]
-        sig = self._get_signature(requests)
+        sig = signature(requests)
+        rec = None
         if sig is not None:
-            replay = await self._replay_get(sig)
+            replay = await self.fast_lane.replay_get(sig)
             if replay is not None:
                 tracker.track_e2e()
                 return replay
+            rec = await self.fast_lane.record_get(sig)
         results = final = None
         try:
-            results = await self._fetch(requests, record_sig=sig)
+            results = await self._fetch(requests, rec)
             tracker.track_step("fetch")
             final = {r.key: self._apply_inplace(results[r.key], inplace.get(r.key), r) for r in requests}
         finally:
-            self._finish_get_session(sig, requests, results, final)
+            if rec is not None:
+                self.fast_lane.finish_get(rec, requests, results, final)
         tracker.track_e2e()
         return final
 
-    # ---- get fast lane ---------------------------------------------------------------------------
-    def _get_signature(self, requests: list[Request]):
-        """Identity of an in-place get batch (keys, wanted slices, destination memory); None when a
-        request has no GPU destination (nothing to replay into)."""
-        import os
-
-        if os.environ.get("TORCHSTORE_B200_FAST_LANE", "1") != "1":
-            return None
-        sig = []
-        for r in requests:
-            t = r.tensor_val
-            if t is None or not t.is_cuda:
-                return None
-            sig.append((r.key, r.tensor_slice, t.data_ptr(), tuple(t.shape), tuple(t.stride()), t.dtype))
-        return tuple(sig)
-
-    async def _replay_get(self, sig):
-        sess = self._get_sessions.get(sig)
-        if sess is None:
-            return None
-        board = self._epoch_board()
-        if board is not None:
-            got = [board.read(0)] + [await p.valid() for p in sess.parts]  # memory loads, no RPC
-        else:
-            got = await asyncio.gather(self._controller.get_epoch.call_one(), *[p.valid() for p in sess.parts])
-        if got[0] != sess.controller_epoch or not all(got[1:]):
-            self._get_sessions.drop(sig)
-            return None
-        for p in sess.parts:
-            p.plans.launch()
-        for p in sess.parts:
-            await p.plans.wait()
-        self.get_session_hits += 1
-        return dict(sess.final)
-
-    def _epoch_board(self):
-        info = getattr(self.strategy, "epoch_board", None)
-        if not info:
-            return None
-        from torchstore_b200 import epoch_board
-
-        return epoch_board.attached(info[0])
-
-    def _finish_get_session(self, sig, requests, results, final) -> None:
-        """Keep what a recorded fetch produced if (and only if) it succeeded (``final`` is set) and
-        every result landed in place; otherwise close every plan it recorded."""
-        recorded = self._recordings.pop(sig, None) if sig is not None else None
-        if recorded is None:
-            return
-        epoch, transports = recorded
-        parts = [t.take_session() for t in transports]
-        inplace_ok = final is not None and all(
-            results[r.key] is not None and isinstance(results[r.key], torch.Tensor)
-            and results[r.key].data_ptr() == r.tensor_val.data_ptr() for r in requests)
-        if epoch is None or not inplace_ok or any(p is None for p in parts):
-            for p in parts:
-                if p is not None:
-                    p.close()
-            return
-        self._get_sessions.put(sig, _GetSession(epoch, parts, dict(final)))
-
     def close_sessions(self) -> None:
-        self._get_sessions.clear()
-        info = getattr(self.strategy, "epoch_board", None)
-        if info:
-            from torchstore_b200 import epoch_board
-
-            epoch_board.forget(info[0])
+        self.fast_lane.clear()
 
     def _apply_inplace(self, fetched: Any, inplace_tensor, request: Request) -> Any:
         """Always hand back the caller's object; copy only if the fetch could not land in place."""
@@ -257,25 +186,13 @@ class LocalClient:
             return inplace_tensor
         return inplace_tensor if inplace_tensor is not None else fetched
 
-    async def _fetch(self, requests: list[Request], record_sig=None) -> dict[str, Any]:
-        epoch = None
-        if record_sig is not None:
-            # read BEFORE the volume map: if the index changes in between, the session is born stale
-            # (and is dropped on its first replay) rather than wrongly valid
-            try:
-                board = self._epoch_board()
-                epoch = board.read(0) if board is not None else await self._controller.get_epoch.call_one()
-            except Exception:
-                record_sig = None
+    async def _fetch(self, requests: list[Request], recording: Recording | None = None) -> dict[str, Any]:
         volume_maps = await self._locate_volumes([r.key for r in requests])
         volume_ids = {vid for vm in volume_maps.values() for vid in vm}
         transports = {vid: create_transport_buffer(self.strategy.get_storage_volume(vid)) for vid in volume_ids}
         volume_requests, whole_keys, gathers = self._build_volume_requests(requests, volume_maps, transports)
-        used = [transports[v] for v in volume_requests]
-        if record_sig is not None and all(getattr(t, "supports_fast_lane", False) for t in used):
-            for t in used:
-                t._record = True
-            self._recordings[record_sig] = (epoch, used)
+        if recording is not None:
+            recording.attach([transports[v] for v in volume_requests])
         pairs = await self._fetch_results(volume_requests, transports)
         return await self._assemble_results(requests, pairs, whole_keys, gathers)
 
@@ -291,7 +208,7 @@ class LocalClient:
         for request in requests:
             volume_map = volume_maps[request.key]
             inplace_ok = all(transports[v].supports_inplace_resharding for v in volume_map)
-            strided_ok = all(getattr(transports[v], "supports_strided_inplace", False) for v in volume_map)
+            strided_ok = all(transports[v].supports_strided_inplace for v in volume_map)
             use_inplace = (
                 inplace_ok
                 and request.tensor_val is not None

@@ -1,7 +1,7 @@
 """Epoch board: the controller's index epoch and every volume's layout epoch in ONE page of POSIX
 shared memory, so a client on the same box validates a replayable put/get session with two memory
 loads instead of two RPC round trips (storage_volume.py ``InMemoryStore.epoch``, controller.py
-``Controller.epoch``; see transport/hbm.py ``HbmSession``).
+``Controller.epoch``; see fast_lane.py).
 
 Slot 0 belongs to the controller, slot 1+i to volume i.  Each slot has exactly one writer (the process
 that owns the controller / the volume), which stores the new value *inside* the endpoint that changes

@@ -5,7 +5,6 @@ the package calls these instead of the plan and copy entry points of ``_native``
 from __future__ import annotations
 
 import asyncio
-import collections
 import functools
 import logging
 import threading
@@ -110,37 +109,3 @@ class Plans(dict):
             except Exception as e:
                 logger.warning("plan_destroy failed: %s", e)
         self.clear()
-
-
-class SessionLRU:
-    """Replayable sessions keyed by signature, least recently used first.  A session is closed when
-    it is replaced, dropped, evicted past ``cap`` or cleared."""
-
-    def __init__(self, cap: int) -> None:
-        self.cap = cap
-        self._by_sig: "collections.OrderedDict[object, object]" = collections.OrderedDict()
-
-    def __len__(self) -> int:
-        return len(self._by_sig)
-
-    def get(self, sig):
-        sess = self._by_sig.get(sig)
-        if sess is not None:
-            self._by_sig.move_to_end(sig)
-        return sess
-
-    def put(self, sig, sess) -> None:
-        self.drop(sig)
-        self._by_sig[sig] = sess
-        while len(self._by_sig) > self.cap:
-            self._by_sig.popitem(last=False)[1].close()
-
-    def drop(self, sig) -> None:
-        sess = self._by_sig.pop(sig, None)
-        if sess is not None:
-            sess.close()
-
-    def clear(self) -> None:
-        for sess in self._by_sig.values():
-            sess.close()
-        self._by_sig.clear()

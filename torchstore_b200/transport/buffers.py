@@ -70,6 +70,8 @@ class TransportBuffer:
     supports_inplace_resharding: bool = True
     supports_batch_puts: bool = False
     supports_batch_gets: bool = False
+    supports_strided_inplace: bool = False  # in-place destinations may be non-contiguous views
+    supports_fast_lane: bool = False        # has a ``record`` flag and ``take_recorded`` (fast_lane.py)
 
     def __init__(self, storage_volume_ref: "StorageVolumeRef"):
         self.storage_volume_ref = storage_volume_ref

@@ -30,7 +30,7 @@ from typing import TYPE_CHECKING, Any
 import torch
 
 from torchstore_b200 import _native
-from torchstore_b200.launch import Plans, SessionLRU, copy_once, wait_copy_stream
+from torchstore_b200.launch import Plans, copy_once, wait_copy_stream
 from torchstore_b200.logging import LatencyTracker
 from torchstore_b200.planner import HbmDescriptor, StridedMem
 from torchstore_b200.transport.buffers import TransportBuffer, TransportCache
@@ -159,63 +159,16 @@ class HbmVolumeCache(TransportCache):
             self._pool = None
 
 
-@dataclass
-class HbmSession:
-    """A replayable put or get of one key batch against one volume: the compiled native plans
-    (device tables with resolved source/destination pointers) and the volume layout epoch they
-    were built under.  While the volume's epoch is unchanged no key of the batch has moved, so the
-    next identical batch is ONE small RPC (the epoch check) + one launch per device."""
-
-    plans: Plans
-    epoch: int
-    volume_ref: Any
-    board: Any = None   # (EpochBoard, slot): read the volume's epoch from shared memory instead of by RPC
-
-    async def valid(self) -> bool:
-        if self.board is not None:
-            return self.board[0].read(self.board[1]) == self.epoch
-        return await self.volume_ref.volume.epoch.call_one() == self.epoch
-
-    def close(self) -> None:
-        self.plans.close()
-
-
 class HbmClientCache(TransportCache):
     """Client-side long-lived state.  Region mappings are cached natively per
     (exporter, allocation); clearing the context drops them all
-    (reference SharedMemoryCache.clear, shared_memory.py:246-250).  Also holds the replayable
-    sessions of the store path's fast lane (LRU)."""
-
-    MAX_SESSIONS = int(os.environ.get("TORCHSTORE_B200_MAX_SESSIONS", "64"))
-
-    def __init__(self) -> None:
-        self.mapped = 0
-        self.put_sessions = SessionLRU(self.MAX_SESSIONS)
-        self.hits = self.misses = 0
+    (reference SharedMemoryCache.clear, shared_memory.py:246-250)."""
 
     def clear(self) -> None:
-        self.put_sessions.clear()
         try:
             _native.release_all()
         except Exception as e:
             logger.warning("release_all failed: %s", e)
-
-
-def _board_slot(volume_ref):
-    """(EpochBoard, slot) of a volume when the controller published an epoch board, else None."""
-    info = getattr(volume_ref, "epoch_board", None)
-    if not info:
-        return None
-    from torchstore_b200 import epoch_board
-
-    name, slots = info
-    board = epoch_board.attached(name)
-    slot = slots.get(volume_ref.volume_id)
-    return (board, slot) if board is not None and slot is not None else None
-
-
-def tensor_sig(t: torch.Tensor) -> tuple:
-    return (t.data_ptr(), tuple(t.shape), tuple(t.stride()), t.dtype)
 
 
 # ---------------------------------------------------------------------------------------------
@@ -241,7 +194,6 @@ class HbmTransportBuffer(TransportBuffer):
     # the reshard kernel writes strided destination rectangles directly, so the client may hand
     # non-contiguous in-place views (the reference restricts to contiguous ones, utils.py:94-96)
     supports_strided_inplace = True
-    # replayable put/get sessions (see HbmSession): LocalClient keys get sessions, this class put sessions
     supports_fast_lane = True
 
     def __init__(self, storage_volume_ref: "StorageVolumeRef"):
@@ -253,9 +205,8 @@ class HbmTransportBuffer(TransportBuffer):
         # key concurrently; each must get back the landing buffer it wrote into)
         self._nonce = os.urandom(8).hex()
         self._epoch = None            # volume layout epoch seen by the volume half of a get, or after a put
-        self._record = False          # client: compile cached plans instead of one-shot copies
+        self.record = False           # client: compile Plans for the fast lane instead of one-shot copies
         self._recorded_plans: Plans | None = None
-        self.fast_path_hit = False    # last put was served by a cached session (no handshake, no notify)
 
     def __getstate__(self) -> dict[str, Any]:
         state = self.__dict__.copy()
@@ -271,50 +222,10 @@ class HbmTransportBuffer(TransportBuffer):
         ]
         return True
 
-    def _put_signature(self, requests: list[Request]):
-        """Identity of a put batch for the fast lane: same keys, same source memory, same layout.
-        None when the batch is not replayable (objects, host tensors)."""
-        sig = [self.storage_volume_ref.volume_id]
-        for r in requests:
-            t = r.tensor_val
-            if r.is_object or t is None or not t.is_cuda:
-                return None
-            sig.append((r.key, None if r.tensor_slice is None else r.tensor_slice.coordinates, *tensor_sig(t)))
-        return tuple(sig)
-
-    async def put_to_storage_volume(self, requests: list[Request], wait: bool = True):
-        """Store path fast lane: a batch that was put before (same keys, same source pointers) and
-        whose landing buffers have not moved (volume epoch unchanged) replays its compiled plan --
-        one epoch RPC + one launch per device, no handshake, no per-key work.  With ``wait=False`` the
-        launch is returned un-awaited (the session's :class:`Plans`; ``await plans.wait()`` completes
-        the put), so the copy runs on the side stream while the caller's compute continues."""
+    async def put_to_storage_volume(self, requests: list[Request]) -> None:
         self._needs_handshake = True
-        self.fast_path_hit = False
-        cache: HbmClientCache = self.storage_volume_ref.transport_context.get(HbmClientCache)
-        sig = self._put_signature(requests) if os.environ.get("TORCHSTORE_B200_FAST_LANE", "1") == "1" else None
-        if sig is not None:
-            sess = cache.put_sessions.get(sig)
-            if sess is not None:
-                if await sess.valid():
-                    cache.hits += 1
-                    sess.plans.launch(fence_out=False)
-                    self.fast_path_hit = True
-                    if not wait:
-                        return sess.plans
-                    await sess.plans.wait()
-                    return None
-                cache.put_sessions.drop(sig)
-            cache.misses += 1
-            self._record = True
-        try:
-            await super().put_to_storage_volume(requests)
-            self._epoch = self._volume_epoch
-        finally:
-            sess = self.take_session()  # a failed put has no epoch: its recorded plans are closed
-            self._record = False
-        if sess is not None:
-            cache.put_sessions.put(sig, sess)
-        return None
+        await super().put_to_storage_volume(requests)
+        self._epoch = self._volume_epoch
 
     async def recv_handshake(self, ctx: "TransportContext", entries: list[tuple[Request, Any]]) -> list[Any]:
         """Volume: hand out where each tensor must be written."""
@@ -359,7 +270,7 @@ class HbmTransportBuffer(TransportBuffer):
                 keep.append(src)
                 host_copies.append((src, desc))
         tracker.track_step("plan")
-        devices = self._copy(per_device, record=self._record and not host_copies, fence_out=False)
+        devices = self._copy(per_device, record=self.record and not host_copies, fence_out=False)
         for src, desc in host_copies:
             dev = desc.device if _same_process(desc) else torch.cuda.current_device()
             dst = desc.resolve(dev)
@@ -440,7 +351,7 @@ class HbmTransportBuffer(TransportBuffer):
                 d2h.append((i, desc, None))
         self._epoch = transport_buffer._epoch
         # a batch with host results is not replayable
-        devices = self._copy(per_device, record=self._record and not d2h, fence_out=True)
+        devices = self._copy(per_device, record=self.record and not d2h, fence_out=True)
         staged = []
         for i, desc, dest in d2h:
             dev = desc.device if _same_process(desc) else torch.cuda.current_device()
@@ -473,15 +384,14 @@ class HbmTransportBuffer(TransportBuffer):
                 results[i] = host
         return results
 
-    def take_session(self) -> HbmSession | None:
-        """Client, after a recorded put or get: the replayable session of this volume's part, or None
-        with the recorded plans closed."""
+    def take_recorded(self) -> tuple[Plans, int] | None:
+        """Client, after a recorded put or get: the compiled plans and the volume epoch they were built
+        under, or None with the plans closed when the request never got an epoch (it failed)."""
         plans, self._recorded_plans = self._recorded_plans, None
-        if plans is None or self._epoch is None:
-            if plans is not None:
-                plans.close()
-            return None
-        return HbmSession(plans, int(self._epoch), self.storage_volume_ref, _board_slot(self.storage_volume_ref))
+        if plans is not None and self._epoch is None:
+            plans.close()
+            plans = None
+        return None if plans is None else (plans, int(self._epoch))
 
     async def drop(self) -> None:
         self._contexts = []
