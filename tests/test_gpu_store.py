@@ -458,3 +458,27 @@ def test_host_tier_stages_gpu_tensors_like_the_reference():
             await ts.shutdown()
 
     run(main())
+
+
+def test_host_tier_get_into_cuda_lands_after_the_callers_queued_writes():
+    """A host-tier get into a contiguous CUDA destination is an H2D copy on the copy stream.  It is
+    fenced in behind the caller's stream, so a write the caller queued on the destination before the
+    get (a fill behind a sleep) lands first and the fetched data is what remains."""
+    from torchstore_b200.transport import TransportType
+
+    async def main():
+        await ts.initialize(num_storage_volumes=1, strategy=ts.LocalRankStrategy(TransportType.SharedMemory))
+        try:
+            t = torch.randn(1024, 1024)
+            await ts.put("t", t)
+            dest = torch.zeros(1024, 1024, device=DEV)
+            torch.cuda.synchronize()
+            torch.cuda._sleep(60_000_000)  # clock cycles: ~30 ms on an H100
+            dest.fill_(-1)
+            out = await ts.get("t", dest)
+            torch.cuda.synchronize()
+            assert out is dest and torch.equal(dest.cpu(), t)
+        finally:
+            await ts.shutdown()
+
+    run(main())

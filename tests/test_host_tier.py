@@ -360,3 +360,81 @@ def test_segments_of_dead_processes_are_reaped():
     finally:
         _native.shm_detach(ptr, 4096)
         _native.shm_unlink(mine)
+
+
+# ---- the landing-buffer put protocol (transport/buffers.py) on the host tier ----------------------------
+async def _handshake_only(ref, key, value):
+    """The first phase of a put: the volume hands out (and parks) a landing segment, the client fills it."""
+    buf = create_transport_buffer(ref)
+    reqs = [Request.from_tensor(key, value)]
+    meta = [r.meta_only() for r in reqs]
+    assert buf.requires_handshake(reqs)
+    await buf.perform_handshake(reqs, meta)
+    return buf, meta
+
+
+def test_concurrent_puts_of_one_key_each_store_their_own_landing_segment():
+    """Two puts of the same key both handshake before either one puts: the volume parks each landing
+    segment under the put's own nonce, so each put stores the segment its own handshake handed out."""
+    import gc
+
+    from torchstore_b200.transport.host import HostVolumeCache
+
+    async def main():
+        await ts.initialize(num_storage_volumes=1, strategy=host_strategy())
+        try:
+            cl = await ts.client()
+            ref = cl.strategy.select_storage_volume()
+            store = ts.api.rpc._lookup("torchstore/volume/0")[0].store
+            values = [torch.full((64, 32), 1.0), torch.full((64, 32), 2.0)]
+            puts = []
+            for v in values:
+                before = _segments()
+                buf, meta = await _handshake_only(ref, "k", v)
+                puts.append((buf, meta, v, _segments() - before))
+            assert all(len(seg) == 1 for *_, seg in puts) and puts[0][3] != puts[1][3]
+            for buf, meta, v, seg in puts:
+                await ref.volume.put.call(buf, meta)
+                stored = store.kv["k"]
+                assert torch.equal(stored, v)
+                assert {"/dev/shm" + store.transport_context.get(HostVolumeCache).describe(stored).name} == seg
+            gc.collect()
+            assert _segments() == puts[1][3]  # the first put's segment went with its overwritten value
+        finally:
+            await ts.shutdown()
+
+    run(main())
+    assert not _segments()
+
+
+def test_abandoned_put_releases_its_landing_segment_after_the_ttl(monkeypatch):
+    """A put that handshakes and never puts (its client failed in between) leaves a parked landing
+    segment; the first handshake after the TTL releases it, one before the TTL does not, and a reset
+    drops whatever is still parked."""
+    import gc
+
+    from torchstore_b200.transport import buffers
+
+    async def main():
+        await ts.initialize(num_storage_volumes=1, strategy=host_strategy())
+        try:
+            cl = await ts.client()
+            ref = cl.strategy.select_storage_volume()
+            await _handshake_only(ref, "lost", torch.ones(128, 64))
+            abandoned = _segments()
+            assert len(abandoned) == 1
+            await ts.put("k", torch.zeros(8))               # a handshake within the TTL keeps it
+            gc.collect()
+            assert abandoned <= _segments()
+            now = buffers.monotonic()
+            monkeypatch.setattr(buffers, "monotonic", lambda: now + buffers.LANDING_TTL_S + 1)
+            await ts.put("k", torch.ones(8))                # the next handshake after the TTL releases it
+            gc.collect()
+            assert not abandoned & _segments()
+            assert torch.equal(await ts.get("k"), torch.ones(8))
+            await _handshake_only(ref, "lost", torch.ones(128, 64))  # parked until the reset below
+        finally:
+            await ts.shutdown()
+
+    run(main())
+    assert not _segments()

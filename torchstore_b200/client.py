@@ -20,7 +20,7 @@ from torch.distributed.tensor import DTensor
 from torchstore_b200 import _native
 from torchstore_b200.controller import ObjectType
 from torchstore_b200.fast_lane import FastLane, Recording, signature
-from torchstore_b200.launch import wait_copy_stream
+from torchstore_b200.launch import staging_copy, wait_copy_stream
 from torchstore_b200.logging import LatencyTracker
 from torchstore_b200.strategy import TorchStoreStrategy
 from torchstore_b200.transport import Request, TensorSlice, create_transport_buffer
@@ -207,13 +207,8 @@ class LocalClient:
         gathers: dict[str, torch.Tensor] = {}
         for request in requests:
             volume_map = volume_maps[request.key]
-            inplace_ok = all(transports[v].supports_inplace_resharding for v in volume_map)
             strided_ok = all(transports[v].supports_strided_inplace for v in volume_map)
-            use_inplace = (
-                inplace_ok
-                and request.tensor_val is not None
-                and (strided_ok or request.tensor_val.is_contiguous())
-            )
+            use_inplace = request.tensor_val is not None and (strided_ok or request.tensor_val.is_contiguous())
             sharded: list[tuple[str, TensorSlice]] = []
             for volume_id, info in volume_map.items():
                 if info.object_type == ObjectType.OBJECT:
@@ -299,8 +294,7 @@ class LocalClient:
             return gathered
         host = torch.empty(gathered.shape, dtype=gathered.dtype)
         dev = gathered.device.index
-        _native.memcpy_async(dev, host.data_ptr(), gathered.data_ptr(), gathered.numel() * gathered.element_size(),
-                             _native.TSB_D2H)
+        staging_copy(dev, host.data_ptr(), gathered.data_ptr(), gathered.numel() * gathered.element_size(), _native.TSB_D2H)
         await wait_copy_stream(dev)
         return host
 

@@ -1,6 +1,7 @@
 """Work on the library's per-device copy stream: fencing it behind the caller's stream, one-shot
-copies, compiled plans and their lifetime, and awaiting completion from an event loop.  The rest of
-the package calls these instead of the plan and copy entry points of ``_native``."""
+copies, host<->device staging copies, compiled plans and their lifetime, and awaiting completion
+from an event loop.  The rest of the package calls these instead of the plan and copy entry points
+of ``_native``."""
 
 from __future__ import annotations
 
@@ -41,6 +42,14 @@ def fence_in(device: int) -> None:
         ev = cache[device] = _native.Event(device)
     ev.record(_native.torch_stream(device))
     ev.wait_on(device, None)
+
+
+def staging_copy(device: int, dst: int, src: int, nbytes: int, kind: int) -> None:
+    """Async host<->device copy of ``nbytes`` (``kind``: ``_native.TSB_H2D`` or ``TSB_D2H``) on
+    ``device``'s copy stream, fenced in behind the caller's stream: it reads what the caller queued
+    before it, and a write the caller queued on the destination cannot land after it."""
+    fence_in(device)
+    _native.memcpy_async(device, dst, src, nbytes, kind)
 
 
 async def wait_copy_stream(device: int) -> None:

@@ -169,7 +169,7 @@ class InMemoryStore(StorageImpl):
         # the HBM transport's volume half allocates stored tensors from this volume's arenas
         from torchstore_b200.transport.hbm import HbmVolumeCache
 
-        self.transport_context.get(HbmVolumeCache).configure(self.device, self)
+        self.transport_context.get(HbmVolumeCache).configure(self.device)
 
     def stats(self) -> dict:
         from torchstore_b200.transport.hbm import HbmVolumeCache
@@ -264,6 +264,8 @@ class InMemoryStore(StorageImpl):
             if request.key not in self.kv:
                 raise KeyError(f"Key '{request.key}' not found. {list(self.kv.keys())=}")
             entries.append((request, self._get_data(request)))
+        # the layout epoch the client's fast lane files a get's plans under (StorageVolume.put returns it)
+        transport_buffer._volume_epoch = self.epoch
         await transport_buffer.handle_get_request(self.transport_context, entries)
         return transport_buffer
 

@@ -25,7 +25,6 @@ if TYPE_CHECKING:
 
 
 class ActorRpcTransportBuffer(TransportBuffer):
-    supports_inplace_resharding = True
     supports_batch_puts = True
     supports_batch_gets = True
     supports_strided_inplace = True  # Tensor.copy_ into any view
@@ -36,8 +35,7 @@ class ActorRpcTransportBuffer(TransportBuffer):
         self._inplace: list[torch.Tensor | None] = []
 
     def __getstate__(self) -> dict[str, Any]:
-        state = self.__dict__.copy()
-        state["storage_volume_ref"] = None
+        state = super().__getstate__()
         state["_inplace"] = []                 # destinations never travel
         return state
 

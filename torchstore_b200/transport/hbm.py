@@ -2,16 +2,16 @@
 
 Implements the ``TransportBuffer`` contract (transport/buffers.py) the way the reference's
 ``SharedMemoryTransportBuffer`` does (transport/shared_memory.py:263-483), with HBM instead of
-POSIX shm and the copy_rects kernel instead of ``Tensor.copy_``:
+POSIX shm and the copy_rects kernel instead of ``Tensor.copy_``.  The landing-buffer put protocol
+is ``LandingBufferTransport``'s; this module supplies the HBM memory and the copies:
 
-PUT  1. client   requires_handshake: any tensor in the batch -> yes; records (shape, dtype) per entry
-     2. volume   recv_handshake: descriptor of the existing stored tensor when shape/dtype match
-                 (overwrite in place), else allocate from the volume's HBM arena; objects -> None
-     3. client   _post_handshake: ONE copy_rects launch pushes every tensor of the batch into the
+PUT  1. volume   recv_handshake: the stored CUDA tensor when shape, dtype and contiguity match
+                 (overwrite in place), else a new one from the volume's HBM arena; objects -> None
+     2. client   _post_handshake: ONE copy_rects launch pushes every tensor of the batch into the
                  volume's memory (local D2D when the volume is on the caller's GPU, P2P stores over
                  NVLink otherwise; host tensors go through an async H2D copy); awaits completion
-     4. volume   handle_put_request: returns the stored tensors / objects, aligned with entries
-GET  1. volume   handle_get_request: descriptor (exported region + layout) of each stored view
+     3. volume   handle_put_request: stores the landing buffers / objects
+GET  1. volume   handle_get_request: descriptor (exported region + layout) of each stored CUDA view
      2. client   _handle_storage_volume_response: ONE copy_rects launch gathers every requested
                  rectangle straight into the caller's tensors (strided destinations included);
                  without a destination the result is materialised on the host like the reference
@@ -22,18 +22,16 @@ from __future__ import annotations
 
 import logging
 import os
-import time
 import weakref
-from dataclasses import dataclass
 from typing import TYPE_CHECKING, Any
 
 import torch
 
 from torchstore_b200 import _native
-from torchstore_b200.launch import Plans, copy_once, wait_copy_stream
+from torchstore_b200.launch import Plans, copy_once, staging_copy, wait_copy_stream
 from torchstore_b200.logging import LatencyTracker
 from torchstore_b200.planner import HbmDescriptor, StridedMem
-from torchstore_b200.transport.buffers import TransportBuffer, TransportCache
+from torchstore_b200.transport.buffers import EntryContext, LandingBufferTransport, TransportBuffer, TransportCache
 from torchstore_b200.transport.types import Request
 
 if TYPE_CHECKING:
@@ -132,13 +130,8 @@ class HbmVolumeCache(TransportCache):
         self.device: int | None = None
         self._pool: HbmPool | None = None
 
-    def configure(self, device: int | None, store=None) -> None:
+    def configure(self, device: int | None) -> None:
         self.device = device
-        self._store = store
-
-    def epoch_of_store(self) -> int | None:
-        store = getattr(self, "_store", None)
-        return None if store is None else store.epoch
 
     def allocate(self, shape, dtype: torch.dtype) -> torch.Tensor:
         if self.device is None:
@@ -171,26 +164,7 @@ class HbmClientCache(TransportCache):
             logger.warning("release_all failed: %s", e)
 
 
-# ---------------------------------------------------------------------------------------------
-# per-entry state carried inside the pickled buffer
-# ---------------------------------------------------------------------------------------------
-@dataclass
-class HbmContext:
-    descriptor: HbmDescriptor | None = None
-    objects: Any = None
-    use_rpc: bool = False  # objects (and anything that is not an HBM tensor) ride in the RPC
-
-
-@dataclass
-class _PutSpec:
-    shape: tuple
-    dtype: torch.dtype
-
-
-class HbmTransportBuffer(TransportBuffer):
-    supports_inplace_resharding = True
-    supports_batch_puts = True
-    supports_batch_gets = True
+class HbmTransportBuffer(LandingBufferTransport):
     # the reshard kernel writes strided destination rectangles directly, so the client may hand
     # non-contiguous in-place views (the reference restricts to contiguous ones, utils.py:94-96)
     supports_strided_inplace = True
@@ -198,55 +172,18 @@ class HbmTransportBuffer(TransportBuffer):
 
     def __init__(self, storage_volume_ref: "StorageVolumeRef"):
         super().__init__(storage_volume_ref)
-        self._needs_handshake = False
-        self._contexts: list[HbmContext] = []
-        self._put_specs: list[_PutSpec | None] = []
-        # identifies THIS put on the volume between handshake and put (two clients may put the same
-        # key concurrently; each must get back the landing buffer it wrote into)
-        self._nonce = os.urandom(8).hex()
-        self._epoch = None            # volume layout epoch seen by the volume half of a get, or after a put
         self.record = False           # client: compile Plans for the fast lane instead of one-shot copies
         self._recorded_plans: Plans | None = None
 
-    def __getstate__(self) -> dict[str, Any]:
-        state = self.__dict__.copy()
-        state["storage_volume_ref"] = None  # process-local handle
-        return state
+    # ---- volume memory: HBM arenas --------------------------------------------------------------
+    def _describe(self, ctx: "TransportContext", tensor: torch.Tensor) -> HbmDescriptor | None:
+        return HbmDescriptor.from_tensor(tensor) if tensor.is_cuda else None
+
+    def _allocate(self, ctx: "TransportContext", shape: tuple, dtype: torch.dtype) -> tuple[torch.Tensor, HbmDescriptor]:
+        tensor = ctx.get(HbmVolumeCache).allocate(shape, dtype)
+        return tensor, HbmDescriptor.from_tensor(tensor)
 
     # ---- PUT ------------------------------------------------------------------------------------
-    def requires_handshake(self, requests: list[Request]) -> bool:
-        if not self._needs_handshake:
-            return False
-        self._put_specs = [
-            None if r.is_object else _PutSpec(tuple(r.tensor_val.shape), r.tensor_val.dtype) for r in requests
-        ]
-        return True
-
-    async def put_to_storage_volume(self, requests: list[Request]) -> None:
-        self._needs_handshake = True
-        await super().put_to_storage_volume(requests)
-        self._epoch = self._volume_epoch
-
-    async def recv_handshake(self, ctx: "TransportContext", entries: list[tuple[Request, Any]]) -> list[Any]:
-        """Volume: hand out where each tensor must be written."""
-        vol = ctx.get(HbmVolumeCache)
-        out: list[HbmDescriptor | None] = []
-        pending = _pending(ctx)
-        _purge_stale(pending)
-        for idx, ((request, current), spec) in enumerate(zip(entries, self._put_specs, strict=True)):
-            if spec is None:
-                out.append(None)
-                continue
-            if isinstance(current, torch.Tensor) and tuple(current.shape) == spec.shape and current.dtype == spec.dtype \
-                    and current.is_contiguous():
-                target = current  # overwrite in place (reference storage_volume.py:161-207)
-            else:
-                target = vol.allocate(spec.shape, spec.dtype)
-            # keep new allocations alive until handle_put_request stores them
-            pending[(self._nonce, idx)] = (time.monotonic(), target)
-            out.append(HbmDescriptor.from_tensor(target))
-        return out
-
     async def _post_handshake(self, handshake_results: list[Any], requests: list[Request]) -> None:
         """Client: move the batch into the volume's HBM with one launch (+ H2D for host tensors)."""
         tracker = LatencyTracker("post_handshake")
@@ -257,11 +194,11 @@ class HbmTransportBuffer(TransportBuffer):
         keep = []
         for request, desc in zip(requests, handshake_results, strict=True):
             if request.is_object:
-                self._contexts.append(HbmContext(objects=request.objects, use_rpc=True))
+                self._contexts.append(EntryContext(objects=request.objects, use_rpc=True))
                 continue
             tensor = request.tensor_val
             assert tensor is not None and desc is not None
-            self._contexts.append(HbmContext(descriptor=desc))
+            self._contexts.append(EntryContext(descriptor=desc))
             if tensor.is_cuda:
                 dev = tensor.device.index
                 per_device.setdefault(dev, []).append((StridedMem.from_tensor(tensor), desc.resolve(dev)))
@@ -274,7 +211,7 @@ class HbmTransportBuffer(TransportBuffer):
         for src, desc in host_copies:
             dev = desc.device if _same_process(desc) else torch.cuda.current_device()
             dst = desc.resolve(dev)
-            _native.memcpy_async(dev, dst.ptr, src.data_ptr(), src.numel() * src.element_size(), _native.TSB_H2D)
+            staging_copy(dev, dst.ptr, src.data_ptr(), src.numel() * src.element_size(), _native.TSB_H2D)
             devices.add(dev)
         tracker.track_step("alloc_and_copy")
         for dev in devices:
@@ -290,30 +227,7 @@ class HbmTransportBuffer(TransportBuffer):
         self._recorded_plans.launch(fence_out)
         return set(per_device)
 
-    async def handle_put_request(self, ctx: "TransportContext", entries: list[tuple[Request, Any]]) -> list[Any]:
-        results = []
-        pending = _pending(ctx)
-        for idx, ((request, current), hctx) in enumerate(zip(entries, self._contexts, strict=True)):
-            if hctx.use_rpc:
-                results.append(hctx.objects)
-                continue
-            entry = pending.pop((self._nonce, idx), None)
-            assert entry is not None, f"No landing buffer for {request.key}: put without a matching handshake"
-            results.append(entry[1])
-        return results
-
     # ---- GET ------------------------------------------------------------------------------------
-    async def handle_get_request(self, ctx: "TransportContext", entries: list[tuple[Request, Any]]) -> None:
-        self._contexts = []
-        self._epoch = ctx.get(HbmVolumeCache).epoch_of_store()
-        for request, data in entries:
-            if request.is_object or not isinstance(data, torch.Tensor):
-                self._contexts.append(HbmContext(objects=data, use_rpc=True))
-            elif data.is_cuda:
-                self._contexts.append(HbmContext(descriptor=HbmDescriptor.from_tensor(data)))
-            else:
-                self._contexts.append(HbmContext(objects=data, use_rpc=True))
-
     async def _handle_storage_volume_response(self, requests: list[Request], transport_buffer: "TransportBuffer") -> list[Any]:
         self.storage_volume_ref.transport_context.get(HbmClientCache)
         results: list[Any] = [None] * len(requests)
@@ -349,7 +263,7 @@ class HbmTransportBuffer(TransportBuffer):
                 results[i] = out
             else:
                 d2h.append((i, desc, None))
-        self._epoch = transport_buffer._epoch
+        self._volume_epoch = transport_buffer._volume_epoch
         # a batch with host results is not replayable
         devices = self._copy(per_device, record=self.record and not d2h, fence_out=True)
         staged = []
@@ -371,7 +285,7 @@ class HbmTransportBuffer(TransportBuffer):
             direct = dest is not None and dest.is_contiguous() and dest.dtype == desc.dtype and \
                 dest.numel() * dest.element_size() == desc.nbytes
             host = dest if direct else torch.empty(desc.shape, dtype=desc.dtype)
-            _native.memcpy_async(dev, host.data_ptr(), src_ptr, desc.nbytes, _native.TSB_D2H)
+            staging_copy(dev, host.data_ptr(), src_ptr, desc.nbytes, _native.TSB_D2H)
             devices.add(dev)
             staged.append((i, dest, host, bounce))
         for dev in devices:
@@ -388,35 +302,10 @@ class HbmTransportBuffer(TransportBuffer):
         """Client, after a recorded put or get: the compiled plans and the volume epoch they were built
         under, or None with the plans closed when the request never got an epoch (it failed)."""
         plans, self._recorded_plans = self._recorded_plans, None
-        if plans is not None and self._epoch is None:
+        if plans is not None and self._volume_epoch is None:
             plans.close()
             plans = None
-        return None if plans is None else (plans, int(self._epoch))
-
-    async def drop(self) -> None:
-        self._contexts = []
-        self._put_specs = []
-
-
-# volume-side scratch: landing buffers between handshake and put, kept on the volume cache object
-def _pending(ctx: "TransportContext") -> dict:
-    vol = ctx.get(HbmVolumeCache)
-    if not hasattr(vol, "_pending"):
-        vol._pending = {}
-    return vol._pending
-
-
-_PENDING_TTL_S = 300.0
-
-
-def _purge_stale(pending: dict) -> None:
-    """Landing buffers of puts that failed between handshake and put (the client's drop() cannot
-    reach the volume) go back to the arena after a grace period."""
-    if not pending:
-        return
-    now = time.monotonic()
-    for k in [k for k, (t, _) in pending.items() if now - t > _PENDING_TTL_S]:
-        pending.pop(k, None)
+        return None if plans is None else (plans, int(self._volume_epoch))
 
 
 def _same_process(desc: HbmDescriptor) -> bool:

@@ -8,8 +8,9 @@ It is a tier, not a fallback: on a GPU box the default stays the NVLink/HBM tran
 put through THIS transport are staged with explicit D2H/H2D copies like the reference does
 (:374,:475), and nothing in the HBM path ever routes here.
 
-PUT  handshake: the volume allocates (or reuses, when shape/dtype match: in-place overwrite,
-     storage_volume.py:161-207) one shm segment per tensor and returns its descriptor; the client
+PUT  handshake (``LandingBufferTransport``, shared with the HBM transport): the volume allocates one
+     shm segment per tensor (or reuses the stored one when shape, dtype and contiguity match:
+     in-place overwrite, storage_volume.py:161-207) and returns its descriptor; the client
      attaches (cached) and moves the bytes in with ONE threaded ``tsb_host_copy_rects`` call for
      all CPU tensors of the batch (strided sources included) and async D2H copies for CUDA tensors.
 GET  the volume returns descriptors of the stored views; the client copies segment -> destination
@@ -31,13 +32,12 @@ from typing import TYPE_CHECKING, Any
 import torch
 
 from torchstore_b200 import _native
-from torchstore_b200.launch import fence_in, wait_copy_stream
+from torchstore_b200.launch import staging_copy, wait_copy_stream
 from torchstore_b200.planner import StridedMem, build_rects
-from torchstore_b200.transport.buffers import TransportBuffer, TransportCache
+from torchstore_b200.transport.buffers import EntryContext, LandingBufferTransport, TransportBuffer, TransportCache
 from torchstore_b200.transport.types import Request
 
 if TYPE_CHECKING:
-    from torchstore_b200.strategy import StorageVolumeRef
     from torchstore_b200.transport.buffers import TransportContext
 
 logger = logging.getLogger(__name__)
@@ -112,7 +112,6 @@ class HostVolumeCache(TransportCache):
     def __init__(self) -> None:
         self.segments: dict[str, _Segment] = {}
         self._storage_refs: dict[str, weakref.ref] = {}  # segment name -> weakref on the stored tensor's storage
-        self._pending: dict = {}
         self._starts: list[int] = []                     # sorted base addresses of our segments (describe() bisects)
         self._by_start: dict[int, _Segment] = {}
         from torchstore_b200.epoch_board import reap_stale_segments
@@ -169,7 +168,6 @@ class HostVolumeCache(TransportCache):
         return ShmDescriptor(seg.name, seg.nbytes, tuple(tensor.shape), tuple(tensor.stride()), tensor.dtype, off)
 
     def clear(self) -> None:
-        self._pending.clear()
         self._storage_refs.clear()
         for seg in self.segments.values():
             seg.close()
@@ -214,13 +212,6 @@ class HostClientCache(TransportCache):
         self._by_key.clear()
 
 
-@dataclass
-class _Ctx:
-    descriptor: ShmDescriptor | None = None
-    objects: Any = None
-    use_rpc: bool = False
-
-
 def _host_move(pairs: list[tuple[torch.Tensor, torch.Tensor]]) -> None:
     """(src, dst) CPU tensor pairs of equal shape and dtype -> one threaded native call."""
     if not pairs:
@@ -232,65 +223,28 @@ def _host_move(pairs: list[tuple[torch.Tensor, torch.Tensor]]) -> None:
     _native.host_copy_rects(rects, n, _COPY_THREADS)
 
 
-class HostShmTransportBuffer(TransportBuffer):
-    supports_inplace_resharding = True
-    supports_batch_puts = True
-    supports_batch_gets = True
+class HostShmTransportBuffer(LandingBufferTransport):
     supports_strided_inplace = True  # the host mover writes strided destination rectangles directly
 
-    def __init__(self, storage_volume_ref: "StorageVolumeRef"):
-        super().__init__(storage_volume_ref)
-        self._needs_handshake = False
-        self._contexts: list[_Ctx] = []
-        self._put_specs: list[tuple | None] = []
-        self._nonce = os.urandom(8).hex()
+    # ---- volume memory: POSIX shm segments ------------------------------------------------------
+    def _describe(self, ctx: "TransportContext", tensor: torch.Tensor) -> ShmDescriptor | None:
+        return None if tensor.is_cuda else ctx.get(HostVolumeCache).describe(tensor)
 
-    def __getstate__(self) -> dict[str, Any]:
-        state = self.__dict__.copy()
-        state["storage_volume_ref"] = None
-        return state
+    def _allocate(self, ctx: "TransportContext", shape: tuple, dtype: torch.dtype) -> tuple[torch.Tensor, ShmDescriptor]:
+        return ctx.get(HostVolumeCache).allocate(shape, dtype)
 
     # ---- PUT ------------------------------------------------------------------------------------
-    def requires_handshake(self, requests: list[Request]) -> bool:
-        if not self._needs_handshake:
-            return False
-        self._put_specs = [None if r.is_object else (tuple(r.tensor_val.shape), r.tensor_val.dtype) for r in requests]
-        return True
-
-    async def put_to_storage_volume(self, requests: list[Request]) -> None:
-        self._needs_handshake = True
-        await super().put_to_storage_volume(requests)
-
-    async def recv_handshake(self, ctx: "TransportContext", entries: list[tuple[Request, Any]]) -> list[Any]:
-        vol = ctx.get(HostVolumeCache)
-        out: list[ShmDescriptor | None] = []
-        for idx, ((request, current), spec) in enumerate(zip(entries, self._put_specs, strict=True)):
-            if spec is None:
-                out.append(None)
-                continue
-            shape, dtype = spec
-            desc = None
-            if isinstance(current, torch.Tensor) and not current.is_cuda and tuple(current.shape) == shape \
-                    and current.dtype == dtype and current.is_contiguous():
-                desc = vol.describe(current)  # overwrite in place
-                target = current
-            if desc is None:
-                target, desc = vol.allocate(shape, dtype)
-            vol._pending[(self._nonce, idx)] = target
-            out.append(desc)
-        return out
-
     async def _post_handshake(self, handshake_results: list[Any], requests: list[Request]) -> None:
         cache: HostClientCache = self.storage_volume_ref.transport_context.get(HostClientCache)
         self._contexts = []
-        host_pairs, devices = [], set()
+        host_pairs, devices, keep = [], set(), []
         for request, desc in zip(requests, handshake_results, strict=True):
             if request.is_object:
-                self._contexts.append(_Ctx(objects=request.objects, use_rpc=True))
+                self._contexts.append(EntryContext(objects=request.objects, use_rpc=True))
                 continue
             tensor = request.tensor_val
             assert tensor is not None and desc is not None
-            self._contexts.append(_Ctx(descriptor=desc))
+            self._contexts.append(EntryContext(descriptor=desc))
             landing = cache.view(desc, request.key)
             if tensor.is_cuda:
                 # D2H into the (pinned) segment, like the reference's shm_tensor.copy_(tensor) (:374)
@@ -298,48 +252,20 @@ class HostShmTransportBuffer(TransportBuffer):
                 seg = cache.attach(desc, request.key)
                 seg.pin()
                 dev = tensor.device.index
-                fence_in(dev)
-                _native.memcpy_async(dev, landing.data_ptr(), src.data_ptr(), desc.nbytes, _native.TSB_D2H)
+                staging_copy(dev, landing.data_ptr(), src.data_ptr(), desc.nbytes, _native.TSB_D2H)
                 devices.add(dev)
-                self._keep = getattr(self, "_keep", []) + [src]
+                keep.append(src)
             else:
                 host_pairs.append((tensor, landing))
         _host_move(host_pairs)
         for dev in devices:
             await wait_copy_stream(dev)  # polled from the loop, like the HBM transport
-        self._keep = []
-
-    async def handle_put_request(self, ctx: "TransportContext", entries: list[tuple[Request, Any]]) -> list[Any]:
-        vol = ctx.get(HostVolumeCache)
-        results = []
-        for idx, ((request, current), hctx) in enumerate(zip(entries, self._contexts, strict=True)):
-            if hctx.use_rpc:
-                results.append(hctx.objects)
-                continue
-            target = vol._pending.pop((self._nonce, idx), None)
-            assert target is not None, f"No landing segment for {request.key}: put without a matching handshake"
-            results.append(target)
-        return results
 
     # ---- GET ------------------------------------------------------------------------------------
-    async def handle_get_request(self, ctx: "TransportContext", entries: list[tuple[Request, Any]]) -> None:
-        vol = ctx.get(HostVolumeCache)
-        self._contexts = []
-        for request, data in entries:
-            if request.is_object or not isinstance(data, torch.Tensor):
-                self._contexts.append(_Ctx(objects=data, use_rpc=True))
-                continue
-            desc = None if data.is_cuda else vol.describe(data)
-            if desc is None:
-                # stored by another tier (HBM volume): by value, on the host
-                self._contexts.append(_Ctx(objects=data.detach().cpu(), use_rpc=True))
-            else:
-                self._contexts.append(_Ctx(descriptor=desc))
-
     async def _handle_storage_volume_response(self, requests: list[Request], transport_buffer: "TransportBuffer") -> list[Any]:
         cache: HostClientCache = self.storage_volume_ref.transport_context.get(HostClientCache)
         results: list[Any] = [None] * len(requests)
-        host_pairs, h2d, devices = [], [], set()
+        host_pairs, h2d, devices, keep = [], [], set(), []
         for i, (request, hctx) in enumerate(zip(requests, transport_buffer._contexts, strict=True)):
             dest = request.tensor_val
             if hctx.use_rpc:
@@ -375,16 +301,11 @@ class HostShmTransportBuffer(TransportBuffer):
             src = stored if stored.is_contiguous() else stored.contiguous()
             if dest.is_contiguous() and dest.dtype == desc.dtype:
                 cache.attach(desc).pin()
-                _native.memcpy_async(dev, dest.data_ptr(), src.data_ptr(), desc.nbytes, _native.TSB_H2D)
+                staging_copy(dev, dest.data_ptr(), src.data_ptr(), desc.nbytes, _native.TSB_H2D)
                 devices.add(dev)
-                self._keep = getattr(self, "_keep", []) + [src]
+                keep.append(src)
             else:
                 dest.copy_(src)
         for dev in devices:
             await wait_copy_stream(dev)
-        self._keep = []
         return results
-
-    async def drop(self) -> None:
-        self._contexts = []
-        self._put_specs = []
