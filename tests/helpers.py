@@ -88,6 +88,184 @@ def random_case(rng: random.Random, cast: bool = False, max_elems: int = 1 << 16
     return RectCase(s_alloc, d_alloc, sdt, ddt, s_view, d_view)
 
 
+# ---- edge-biased workloads ----------------------------------------------------------------------------
+# Windows aimed at the copy_rects kernel's boundaries for a given copy tile size (in units): rows of
+# exactly k tiles and one unit either side, narrow rects whose row count is not a multiple of their
+# rows-per-tile, one-unit rows (magic 0), rows one unit short of a tile, wide rows under several
+# strided outer dims, 5-D and 6-D windows, and cast windows on both sides of the vector rule.
+VECTOR_CAST_PAIRS = [p for p in CAST_PAIRS if torch.float64 not in p]
+EDGE_KINDS = ("wide_exact", "wide_minus", "wide_plus", "narrow_ragged", "unit_row", "tile_minus_one",
+              "wide_nd", "deep_nd", "aligned", "cast_vector", "cast_scalar")
+
+
+def _edge_window(rng: random.Random, shape, itemsize: int, aligned: bool, pad_outer: bool):
+    """(base shape, window index) of a window of `shape` whose innermost dim is contiguous and never
+    merges with the dim above it.  aligned: the window's start and every row pitch are multiples of
+    16 bytes (given a 16-byte aligned base); otherwise the window starts one element off alignment."""
+    q = max(1, 16 // itemsize)  # elements per 16 bytes
+    if aligned:
+        start_in = q * rng.randint(0, 2)
+        inner = -(-(start_in + shape[-1] + 1) // q) * q + q * rng.randint(0, 1)
+    else:
+        start_in = 1
+        inner = start_in + shape[-1] + rng.randint(1, 5)
+    base, starts = [], []
+    for d, s in enumerate(shape[:-1]):
+        # pad_outer: one spare row in every outer dim but the outermost, so no two outer dims merge
+        pad = (1 if d else rng.choice([0, 1])) if pad_outer else rng.choice([0, 1])
+        base.append(s + pad)
+        starts.append(rng.randint(0, pad))
+    base.append(inner)
+    starts.append(start_in)
+    return tuple(base), tuple(slice(a, a + s) for a, s in zip(starts, shape))
+
+
+def _edge_outer(rng: random.Random, rows: int, n_dims: int):
+    """Split `rows` over n_dims outer extents (each > 1 where possible, product == rows)."""
+    dims = []
+    for _ in range(n_dims - 1):
+        f = next((d for d in (2, 3, 5, 7) if rows % d == 0 and rows // d > 1), None)
+        if f is None:
+            break
+        dims.append(f)
+        rows //= f
+    dims.append(rows)
+    rng.shuffle(dims)
+    return dims
+
+
+def edge_case(rng: random.Random, tile_units: int, kind: str, uniform: str | None = None) -> RectCase:
+    """One window of `kind` (see EDGE_KINDS) for copy tiles of `tile_units` units.
+
+    uniform="b16": a same-dtype window of 16-byte units, so a workload of them compiles to KIND_B16;
+    uniform="f32_bf16": a vector fp32->bf16 window, so a workload of them compiles to KIND_F32_BF16."""
+    T = tile_units
+    if uniform == "b16":
+        sdt = ddt = rng.choice(SAME_DTYPES)
+        aligned, vec_cast = True, False
+    elif uniform == "f32_bf16":
+        sdt, ddt = torch.float32, torch.bfloat16
+        aligned, vec_cast = True, True
+    elif kind == "cast_vector":
+        sdt, ddt = rng.choice(VECTOR_CAST_PAIRS)
+        aligned, vec_cast = True, True
+    elif kind == "cast_scalar":
+        sdt, ddt = rng.choice(CAST_PAIRS)
+        aligned, vec_cast = False, False
+    else:
+        sdt = ddt = rng.choice(SAME_DTYPES)
+        aligned, vec_cast = kind == "aligned" or rng.random() < 0.5, False
+    cast = sdt != ddt
+    big = T >= 4096  # keep the largest tile sizes to a few tens of MiB per workload
+    # elements per unit: 8 for a vector cast, 16 bytes for an aligned byte move, one element otherwise
+    epu = 8 if vec_cast else (16 // sdt.itemsize if aligned and not cast else 1)
+
+    n_outer = 0
+    if kind in ("wide_exact", "wide_minus", "wide_plus"):
+        k = rng.choice([1, 2])
+        units = k * T + {"wide_exact": 0, "wide_minus": -1, "wide_plus": 1}[kind]
+        rows, n_outer = rng.choice([1, 2, 3]), rng.choice([0, 1, 2])
+    elif kind == "narrow_ragged":
+        units = rng.choice([max(1, T // 3), max(1, T // 4 + 1), rng.randint(1, 7)])
+        split = max(1, T // units)
+        if split == 1:
+            units, split = max(1, T // 3), max(1, T // max(1, T // 3))
+        rows = split * rng.randint(1, 2) + rng.randint(1, max(1, split - 1))
+        n_outer = rng.choice([1, 2])
+    elif kind == "unit_row":
+        units, rows, n_outer = 1, rng.randint(2, 3 * T + 7), rng.choice([1, 2, 3])
+    elif kind == "tile_minus_one":
+        units, rows, n_outer = T - 1, rng.randint(2, 7), rng.choice([1, 2])
+    elif kind == "wide_nd":
+        n_outer = rng.randint(2, 3 if big else 5)
+        units = T + rng.choice([0, 1, 7] if big else [0, 1, 7, T // 2])
+        rows = 2 ** n_outer * (1 if big else rng.choice([1, 1, 3]))
+    elif kind == "deep_nd":
+        n_outer = rng.choice([4, 5])
+        units = rng.choice([1, 3, T // 2, T + 1]) if not big else rng.choice([1, 3, 100])
+        rows = 2 ** n_outer * rng.choice([1, 3])
+    else:  # aligned / cast_vector / cast_scalar: a random N-D window
+        n_outer = rng.choice([0, 1, 2, 3])
+        units = rng.choice([1, 2, 5, 31, T // 2, T, T + 3])
+        rows = max(1, rng.choice([1, 3, 8, 17]) * max(1, n_outer))
+    units = max(1, units)
+    outer = _edge_outer(rng, rows, n_outer) if n_outer else []
+    if not outer and rows > 1:
+        outer = [rows]
+    shape = outer + [units * epu]
+    pad_outer = kind in ("wide_nd", "deep_nd") or rng.random() < 0.7
+    sbase, sidx = _edge_window(rng, shape, sdt.itemsize, aligned, pad_outer)
+    dbase, didx = _edge_window(rng, shape, ddt.itemsize, aligned, pad_outer)
+    if not aligned and cast and rng.random() < 0.5:
+        # misalign only one side: still no vector mode, but the other side is a clean pitch
+        dbase, didx = _edge_window(rng, shape, ddt.itemsize, True, pad_outer)
+    return RectCase(sbase, dbase, sdt, ddt, lambda b, i=sidx: b[i], lambda b, i=didx: b[i])
+
+
+def edge_workload(rng: random.Random, tile_units: int, uniform: str | None = None, cast: bool | None = None,
+                  extra: int = 6) -> list:
+    """Every edge kind at least once (casts only where `cast` allows), plus `extra` more, shuffled.
+    cast=None mixes copies and casts; uniform= as in edge_case (all windows of one mode)."""
+    if uniform is not None or cast is False:
+        kinds = [k for k in EDGE_KINDS if not k.startswith("cast")]
+    elif cast:
+        kinds = [k for k in EDGE_KINDS if k.startswith("cast")] * 3
+    else:
+        kinds = list(EDGE_KINDS)
+    kinds = kinds + [rng.choice(kinds) for _ in range(extra)]
+    rng.shuffle(kinds)
+    if cast:
+        return [edge_case(rng, tile_units, k) for k in kinds] + [
+            edge_case(rng, tile_units, k, uniform="f32_bf16") for k in EDGE_KINDS if not k.startswith("cast")]
+    return [edge_case(rng, tile_units, k, uniform) for k in kinds]
+
+
+# ---- compiled plan tables -----------------------------------------------------------------------------
+# DevRect (csrc/tsb_internal.h) as a numpy record: 192 bytes per rect of a tsb_plan_compile_host table.
+DEV_RECT = np.dtype([
+    ("src", "<u8"), ("dst", "<u8"), ("src_stride", "<i8", (6,)), ("dst_stride", "<i8", (6,)), ("ext", "<u4", (6,)),
+    ("n_outer", "<u4"), ("rows", "<u4"), ("units_per_row", "<u4"), ("magic", "<u4"), ("wide", "<u4"), ("split", "<u4"),
+    ("mode", "<u4"), ("src_unit_bytes", "<u4"), ("dst_unit_bytes", "<u4"), ("tile_units", "<u4"), ("link", "<u4"),
+    ("pad_", "<u4", (3,)),
+])
+assert DEV_RECT.itemsize == 192
+MODE_B16, MODE_F32_BF16_V8 = 4, 8
+VECTOR_CAST_MODES = (8, 10, 12, 14, 16, 18)
+KIND_GENERIC, KIND_B16, KIND_F32_BF16 = 0, 1, 2
+
+
+def rect_fields(table: np.ndarray) -> np.ndarray:
+    """The rect table of _native.plan_compile_host as a record array with DevRect's field names."""
+    return np.ascontiguousarray(table).view(DEV_RECT)
+
+
+def plan_kind(fields: np.ndarray) -> int:
+    """The kernel specialisation a plan of these compiled rects launches (plan.cu Compiler::kind)."""
+    if len(fields) and (fields["mode"] == MODE_B16).all():
+        return KIND_B16
+    if len(fields) and (fields["mode"] == MODE_F32_BF16_V8).all():
+        return KIND_F32_BF16
+    return KIND_GENERIC
+
+
+def edge_coverage(fields: np.ndarray, tile_units: int) -> dict:
+    """Which of the kernel's tile boundaries the copy-queue rects of `fields` (tile size `tile_units`) reach."""
+    f = fields[fields["tile_units"] == tile_units]
+    T = tile_units
+    upr, wide, split, rows, n_outer = (f[k].astype(np.int64) for k in ("units_per_row", "wide", "split", "rows", "n_outer"))
+    return {
+        "rows_of_k_tiles": bool(((upr % T == 0) & (wide == 1)).any()),
+        "rows_of_k_tiles_plus_1": bool(((upr % T == 1) & (wide == 1)).any()),
+        "rows_of_k_tiles_minus_1": bool((upr % T == T - 1).any()),
+        "narrow_ragged": bool(((wide == 0) & (split > 1) & (rows % np.maximum(split, 1) != 0)).any()),
+        "one_unit_rows": bool(((upr == 1) & (f["magic"] == 0)).any()),
+        "tile_minus_one_rows": bool(((wide == 0) & (split == 1) & (upr == T - 1)).any()),
+        "wide_under_2_outer": bool(((wide == 1) & (n_outer >= 2)).any()),
+        "narrow_nd": bool(((wide == 0) & (n_outer >= 2)).any()),
+        "outer_4_or_more": bool((n_outer >= 4).any()),
+    }
+
+
 def materialise(cases, device, seed: int, finite_only: bool = False):
     """Allocate bases on `device` (filled from a seeded CPU generator so CPU and CUDA copies hold
     identical bytes) and return [(src_view, dst_view, dst_base)]."""

@@ -24,6 +24,9 @@ def _init():
 
 
 def run_product(pairs, device=0, flags=0):
+    # the plan runs on the library's copy stream, which is not ordered after torch's stream: the
+    # sources and destinations torch just wrote must be complete first
+    torch.cuda.synchronize()
     rects, n = rects_for(pairs)
     plan = _native.plan_create(device, rects, n, flags)
     info = _native.plan_info(plan)

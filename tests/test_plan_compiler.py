@@ -9,7 +9,8 @@ import pytest
 import torch
 
 from oracle import c_oracle
-from tests.helpers import bytes_of, materialise, random_case, rects_for
+from tests.helpers import (KIND_B16, KIND_F32_BF16, KIND_GENERIC, MODE_B16, VECTOR_CAST_MODES, bytes_of, edge_coverage,
+                           edge_workload, materialise, plan_kind, random_case, rect_fields, rects_for)
 from torchstore_b200 import _native
 
 
@@ -25,7 +26,7 @@ def _run(cases, seed, tile_units, flags=0):
     c_oracle.replay_plan(table, tiles, info.tile_bytes // 16, nan_mode=0)
     for (sa, da, dbase_a, _), (sb, db, dbase_b, _) in zip(a, b):
         assert np.array_equal(bytes_of(dbase_a), bytes_of(dbase_b))
-    return a, info
+    return a, info, table
 
 
 @pytest.mark.parametrize("tile_units", [64, 256, 4096])
@@ -40,11 +41,45 @@ def test_compiled_plan_replays_to_oracle_result(tile_units, cast, link, monkeypa
     _run(cases, seed=5, tile_units=tile_units)
 
 
+@pytest.mark.parametrize("tile_units", [64, 256, 4096, 32768])
+@pytest.mark.parametrize("workload", ["mixed", "cast", "b16", "f32_bf16"])
+@pytest.mark.parametrize("link", ["1", "2"])
+def test_edge_workloads_replay_to_oracle_result(tile_units, workload, link, monkeypatch):
+    """Edge-biased windows (tests/helpers.edge_workload) at every copy tile size the kernel is run
+    with: the compiled tables reach the boundaries they aim at and replay to the oracle's bytes."""
+    monkeypatch.setenv("TSB_LINK", link)
+    rng = random.Random(f"edge-{tile_units}-{workload}")
+    if workload in ("b16", "f32_bf16"):
+        cases = edge_workload(rng, tile_units, uniform=workload)
+    else:
+        cases = edge_workload(rng, tile_units, cast=workload == "cast")
+    _, info, table = _run(cases, seed=11, tile_units=tile_units)
+    f = rect_fields(table)
+    assert info.tile_bytes == tile_units * 16
+    if workload == "b16":
+        assert plan_kind(f) == KIND_B16
+    elif workload == "f32_bf16":
+        assert plan_kind(f) == KIND_F32_BF16
+    else:
+        assert plan_kind(f) == KIND_GENERIC
+    if workload == "cast":
+        assert set(f["mode"].tolist()) & set(VECTOR_CAST_MODES)
+        assert set(f["mode"].tolist()) & {9, 11, 13, 15, 17, 19, 20, 21}  # scalar casts
+    if workload == "mixed":
+        assert MODE_B16 in f["mode"] and (f["mode"] < MODE_B16).any()
+    if link == "1":
+        cov = edge_coverage(f, tile_units)
+        missing = sorted(k for k, hit in cov.items() if not hit)
+        assert not missing, missing
+    elif workload in ("mixed", "b16"):  # only 16-byte-unit moves ride the link warp
+        assert info.num_link_tiles > 0 and f["link"].any()
+
+
 def test_same_dtype_result_equals_torch_copy():
     """The oracle's rectangle copy is torch's dst.copy_(src) (what the reference executes)."""
     rng = random.Random(7)
     cases = [random_case(rng) for _ in range(40)]
-    a, _ = _run(cases, seed=9, tile_units=256)
+    a, _, _ = _run(cases, seed=9, tile_units=256)
     ref = materialise(cases, "cpu", 9)
     for (s, d, dbase, _), (rs, rd, rbase, _) in zip(a, ref):
         rd.copy_(rs)

@@ -433,6 +433,10 @@ int choose_grid(int device, uint32_t kind, const Compiled& cp, uint32_t* out_gri
   uint64_t work = std::max<uint64_t>(cp.tiles.size(), (cp.link_tiles.size() + kLinkBatch - 1) / kLinkBatch);
   uint64_t grid = static_cast<uint64_t>(sm) * per_sm;
   if (grid > work) grid = work;
+  // TSB_MAX_GRID caps the CTAs per launch (tests and ablations: a grid of 1 walks the whole queue in
+  // one CTA); 0 or unset means no cap
+  const uint32_t max_grid = env_u32("TSB_MAX_GRID", 0);
+  if (max_grid && grid > max_grid) grid = max_grid;
   if (grid == 0) grid = 1;
   *out_grid = static_cast<uint32_t>(grid);
   return TSB_OK;
