@@ -285,7 +285,9 @@ def rects_for(pairs):
 
 
 def bytes_of(t: torch.Tensor) -> np.ndarray:
-    return t.detach().cpu().contiguous().view(torch.uint8).numpy().copy()
+    if t.numel() == 0:
+        return np.zeros(0, dtype=np.uint8)
+    return t.detach().cpu().contiguous().reshape(-1).view(torch.uint8).numpy().copy()
 
 
 NAN_CHECK = {

@@ -438,3 +438,21 @@ def test_abandoned_put_releases_its_landing_segment_after_the_ttl(monkeypatch):
 
     run(main())
     assert not _segments()
+
+
+@pytest.mark.parametrize("seed", range(3))
+def test_store_matches_oracle_across_random_layouts_on_the_host_tier(seed):
+    """The differential store harness (tests/store_harness.py) over three host-tier volumes: random
+    layouts with uneven, empty and replicated shards, every dtype, and fresh, contiguous, strided and
+    converting CPU destinations, each compared with the oracle store; every coverage bucket is reached."""
+    from tests.store_harness import run_differential
+
+    async def main():
+        await ts.initialize(num_storage_volumes=3, strategy=host_strategy())
+        try:
+            h = await run_differential(1000 + seed, 40, devices=("cpu",), source_device="cpu")
+        finally:
+            await ts.shutdown()
+        h.assert_coverage()
+
+    run(main())

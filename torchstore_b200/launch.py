@@ -47,7 +47,10 @@ def fence_in(device: int) -> None:
 def staging_copy(device: int, dst: int, src: int, nbytes: int, kind: int) -> None:
     """Async host<->device copy of ``nbytes`` (``kind``: ``_native.TSB_H2D`` or ``TSB_D2H``) on
     ``device``'s copy stream, fenced in behind the caller's stream: it reads what the caller queued
-    before it, and a write the caller queued on the destination cannot land after it."""
+    before it, and a write the caller queued on the destination cannot land after it.  A copy of zero
+    bytes (an empty tensor, whose data pointer torch reports as null) is not issued."""
+    if nbytes == 0:
+        return
     fence_in(device)
     _native.memcpy_async(device, dst, src, nbytes, kind)
 

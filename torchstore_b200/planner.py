@@ -167,13 +167,16 @@ class _ExportCache:
         self.hits = self.misses = self.evictions = 0
 
     def export(self, t: torch.Tensor, nbytes: int) -> tuple[bytes, int]:
-        key = (t.data_ptr(), nbytes)
+        # torch reports a null data pointer for a tensor without elements (an empty shard, or an empty
+        # window of a stored tensor); its storage still has an address to describe, and no copy reads it
+        ptr = t.data_ptr() or t.untyped_storage().data_ptr()
+        key = (ptr, nbytes)
         hit = self._regions.get(key)
         if hit is not None:
             self.hits += 1
             return hit
         self.misses += 1
-        region = _native.export_region(t.data_ptr(), nbytes)
+        region = _native.export_region(ptr, nbytes)
         entry = (_native.region_to_bytes(region), int(region.device))
         try:
             ref = weakref.ref(t.untyped_storage(), lambda _r, _k=key: self._evict(_k))

@@ -13,7 +13,8 @@ PUT  1. volume   recv_handshake: the stored CUDA tensor when shape, dtype and co
      3. volume   handle_put_request: stores the landing buffers / objects
 GET  1. volume   handle_get_request: descriptor (exported region + layout) of each stored CUDA view
      2. client   _handle_storage_volume_response: ONE copy_rects launch gathers every requested
-                 rectangle straight into the caller's tensors (strided destinations included);
+                 rectangle straight into the caller's tensors (strided destinations included;
+                 a dtype pair the fused cast lacks lands in a temporary and is converted by copy_);
                  without a destination the result is materialised on the host like the reference
                  does (D2H), or on the GPU when TORCHSTORE_B200_GET_DEVICE=cuda
 """
@@ -233,6 +234,7 @@ class HbmTransportBuffer(LandingBufferTransport):
         results: list[Any] = [None] * len(requests)
         per_device: dict[int, list] = {}
         d2h = []
+        converts = []  # (CUDA destination, gathered stored-dtype temporary) for pairs the fused cast lacks
         for i, (request, hctx) in enumerate(zip(requests, transport_buffer._contexts, strict=True)):
             dest = request.tensor_val
             if hctx.use_rpc:
@@ -252,7 +254,13 @@ class HbmTransportBuffer(LandingBufferTransport):
                 assert tuple(dest.shape) == tuple(desc.shape), f"{tuple(dest.shape)} != {tuple(desc.shape)}"
                 if dest.is_cuda:
                     dev = dest.device.index
-                    per_device.setdefault(dev, []).append((desc.resolve(dev), StridedMem.from_tensor(dest)))
+                    target = dest
+                    if not _native.cast_supported(desc.dtype, dest.dtype):
+                        # no fused cast for this pair: gather the stored dtype in the same launch, then
+                        # convert like the reference's client_tensor.copy_(shm_tensor)
+                        target = torch.empty(desc.shape, dtype=desc.dtype, device=dest.device)
+                        converts.append((dest, target))
+                    per_device.setdefault(dev, []).append((desc.resolve(dev), StridedMem.from_tensor(target)))
                     results[i] = dest
                 else:
                     d2h.append((i, desc, dest))
@@ -264,8 +272,8 @@ class HbmTransportBuffer(LandingBufferTransport):
             else:
                 d2h.append((i, desc, None))
         self._volume_epoch = transport_buffer._volume_epoch
-        # a batch with host results is not replayable
-        devices = self._copy(per_device, record=self.record and not d2h, fence_out=True)
+        # a batch with host results, or one finished by a torch conversion after the plan, is not replayable
+        devices = self._copy(per_device, record=self.record and not d2h and not converts, fence_out=True)
         staged = []
         for i, desc, dest in d2h:
             dev = desc.device if _same_process(desc) else torch.cuda.current_device()
@@ -290,6 +298,8 @@ class HbmTransportBuffer(LandingBufferTransport):
             staged.append((i, dest, host, bounce))
         for dev in devices:
             await wait_copy_stream(dev)
+        for dest, gathered in converts:
+            dest.copy_(gathered)
         for i, dest, host, _bounce in staged:
             if dest is not None and host is not dest:
                 dest.copy_(host)  # non-contiguous host destination: host-side scatter of host data
