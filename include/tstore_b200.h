@@ -26,7 +26,7 @@
 extern "C" {
 #endif
 
-#define TSB_ABI_VERSION 2
+#define TSB_ABI_VERSION 3
 #define TSB_MAX_DIMS 6
 
 enum {
@@ -41,7 +41,7 @@ enum {
 /* element types understood by the copy/cast kernel (same-dtype copies are byte moves and accept
  * any of them; cross-dtype pairs are listed in tsb_cast_supported) */
 enum {
-  TSB_U8 = 0,  /* also used for "opaque bytes": int8, bool, fp8 ... */
+  TSB_U8 = 0,  /* also used for "opaque bytes": int8, bool, and fp8 when it is only moved */
   TSB_U16 = 1, /* opaque 2-byte (int16) */
   TSB_U32 = 2, /* opaque 4-byte (int32) */
   TSB_U64 = 3, /* opaque 8-byte (int64, complex64) */
@@ -49,6 +49,8 @@ enum {
   TSB_BF16 = 5,
   TSB_F32 = 6,
   TSB_F64 = 7,
+  TSB_F8E4M3 = 8, /* float8_e4m3fn: one side of a cast (a same-dtype fp8 move is TSB_U8) */
+  TSB_F8E5M2 = 9, /* float8_e5m2: likewise */
 };
 
 /* ------------------------------------------------------------------------------------------ */
@@ -158,7 +160,14 @@ typedef struct tsb_plan_info {
   uint32_t link_stages;       /* ring depth */
 } tsb_plan_info_t;
 
-/* Is (src_dtype -> dst_dtype) implemented?  Same dtype is always supported. */
+/* Is (src_dtype -> dst_dtype) implemented?  Same dtype is always supported.  The fused casts, all
+ * bit-exact with torch's .to():
+ *   f32 <-> bf16, f32 <-> f16, bf16 <-> f16, f64 <-> f32
+ *   {f32, bf16, f16} -> {f8e4m3, f8e5m2}: round to nearest even; e4m3fn has no Inf, so |x| > 464,
+ *     +-Inf and NaN give 0x7F|sign; e5m2 gives +-Inf (0x7C|sign) for |x| >= 61440 and 0x7F|sign for NaN
+ *     (an f16 NaN gives 0x7F: its widening to f32 on the GPU drops the sign, as in torch's CUDA .to())
+ *   {f8e4m3, f8e5m2} -> {f32, bf16, f16}: exact
+ * Casts run on the GPU only (tsb_host_copy_rects moves bytes). */
 int tsb_cast_supported(uint32_t src_dtype, uint32_t dst_dtype);
 
 /* Compile a list of rects into a device-resident tile table for `device` (the cached transfer

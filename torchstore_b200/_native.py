@@ -16,11 +16,11 @@ import torch
 from torchstore_b200._build import LIB_PATH
 
 TSB_MAX_DIMS = 6
-TSB_ABI_VERSION = 2
+TSB_ABI_VERSION = 3
 
 TSB_OK, TSB_ERR_INVALID, TSB_ERR_CUDA, TSB_ERR_UNSUPPORTED, TSB_ERR_NOMEM, TSB_ERR_NOTFOUND = range(6)
 
-TSB_U8, TSB_U16, TSB_U32, TSB_U64, TSB_F16, TSB_BF16, TSB_F32, TSB_F64 = range(8)
+TSB_U8, TSB_U16, TSB_U32, TSB_U64, TSB_F16, TSB_BF16, TSB_F32, TSB_F64, TSB_F8E4M3, TSB_F8E5M2 = range(10)
 TSB_H2D, TSB_D2H, TSB_D2D = 1, 2, 3
 TSB_PLAN_DEFAULT, TSB_PLAN_NO_INTERLEAVE = 0, 1
 
@@ -201,6 +201,8 @@ _FLOAT_CODES = {
     torch.float32: TSB_F32,
     torch.float64: TSB_F64,
 }
+# fp8 has a code only as one side of a cast: moved as itself it is an opaque byte (dtype_code -> TSB_U8)
+_CAST_CODES = {**_FLOAT_CODES, torch.float8_e4m3fn: TSB_F8E4M3, torch.float8_e5m2: TSB_F8E5M2}
 _OPAQUE_BY_SIZE = {1: TSB_U8, 2: TSB_U16, 4: TSB_U32, 8: TSB_U64}
 
 
@@ -218,12 +220,20 @@ def dtype_code(dtype: torch.dtype) -> int:
     raise TypeError(f"unsupported dtype {dtype}")
 
 
+def cast_code(dtype: torch.dtype) -> int:
+    """TSB_* code of `dtype` as one side of a fused cast (fp8 included)."""
+    code = _CAST_CODES.get(dtype)
+    if code is None:
+        raise TypeError(f"no cast code for {dtype}")
+    return code
+
+
 def cast_supported(src: torch.dtype, dst: torch.dtype) -> bool:
     if src == dst:
         return True
-    if src not in _FLOAT_CODES or dst not in _FLOAT_CODES:
+    if src not in _CAST_CODES or dst not in _CAST_CODES:
         return False
-    return bool(lib().tsb_cast_supported(_FLOAT_CODES[src], _FLOAT_CODES[dst]))
+    return bool(lib().tsb_cast_supported(_CAST_CODES[src], _CAST_CODES[dst]))
 
 
 # ------------------------------------------------------------------------------------------------

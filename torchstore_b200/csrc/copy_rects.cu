@@ -9,7 +9,8 @@
 //   * local.to(transfer_dtype) / staging.copy_(src)        direct_weight_sync.py:133,167-168
 //
 // Work decomposition (built on the host by plan.cu):
-//   rect  -> rows x units   (unit = 16 B for byte moves, 8 elements for vector casts)
+//   rect  -> rows x units   (unit = 16 B for byte moves, 8 elements for vector casts, 16 elements
+//            for vector fp8 casts: the fp8 side of every unit is one 16-byte access)
 //   tile  = <= tile_units units: either a segment of one wide row or a group of whole narrow rows
 //   tiles are listed in an order that round-robins over source GPUs (NVSwitch port fairness)
 //   CTA b processes tiles b, b+grid, b+2*grid, ...; the next tile's rect header is staged into
@@ -27,6 +28,7 @@
 #include <cuda_fp16.h>
 
 #include <atomic>
+#include <type_traits>
 
 #include "tsb_internal.h"
 
@@ -142,6 +144,136 @@ struct CastHalfV8 {
   static __device__ __forceinline__ void st(char* p, const Reg& v) {
     uint4 o{cv(v.x), cv(v.y), cv(v.z), cv(v.w)};
     stg16(p, o);
+  }
+};
+
+// ---- fp8 (float8_e4m3fn, float8_e5m2) ------------------------------------------------------------
+// Storage tags of the fp8 side of a scalar cast (the vector movers handle raw bytes).
+struct F8E4M3 { unsigned char x; };
+struct F8E5M2 { unsigned char x; };
+
+// The narrowing cvt exists only in .satfinite form: values past the largest finite one and +-Inf
+// saturate to it, and every NaN becomes one canonical NaN.  torch's .to() instead rounds to nearest
+// even all the way: e4m3fn has no Inf, so whatever rounds past 448 (|x| > 464), +-Inf and NaN become
+// 0x7F|sign; e5m2 overflows to +-Inf (0x7C|sign) from |x| >= 61440 on, and a NaN keeps its sign
+// (0x7F|sign).  fp8_fix replaces the cvt's byte for exactly those inputs; below the thresholds the
+// cvt already rounds like torch (subnormals included).  An f16 source is widened with cvt.f32.f16 like
+// torch's CUDA .to() does, which makes every NaN positive: a negative f16 NaN gives 0x7F, as in torch.
+template <bool kE4M3>
+__device__ __forceinline__ uint32_t fp8_fix(uint32_t cvt_byte, uint32_t f32_bits) {
+  const uint32_t a = f32_bits & 0x7fffffffu;
+  const uint32_t sign = (f32_bits >> 24) & 0x80u;
+  if (kE4M3) return a > 0x43e80000u /* 464.0f */ ? (0x7fu | sign) : cvt_byte;
+  return a >= 0x47700000u /* 61440.0f */ ? ((a > 0x7f800000u ? 0x7fu : 0x7cu) | sign) : cvt_byte;
+}
+// two f32 bit patterns -> two fp8 bytes (lo in bits 0..7, hi in bits 8..15)
+template <bool kE4M3>
+__device__ __forceinline__ uint32_t f32x2_to_fp8x2(uint32_t lo, uint32_t hi) {
+  unsigned short r;
+  if (kE4M3)
+    asm("cvt.rn.satfinite.e4m3x2.f32 %0, %1, %2;" : "=h"(r) : "f"(__uint_as_float(hi)), "f"(__uint_as_float(lo)));
+  else
+    asm("cvt.rn.satfinite.e5m2x2.f32 %0, %1, %2;" : "=h"(r) : "f"(__uint_as_float(hi)), "f"(__uint_as_float(lo)));
+  return fp8_fix<kE4M3>(r & 0xffu, lo) | (fp8_fix<kE4M3>(static_cast<uint32_t>(r) >> 8, hi) << 8);
+}
+// two fp8 bytes (bits 0..15) -> f16x2 (exact: every fp8 value is an f16 value)
+template <bool kE4M3>
+__device__ __forceinline__ uint32_t fp8x2_to_f16x2(uint32_t two) {
+  uint32_t r;
+  const unsigned short b = static_cast<unsigned short>(two);
+  if (kE4M3) asm("cvt.rn.f16x2.e4m3x2 %0, %1;" : "=r"(r) : "h"(b));
+  else asm("cvt.rn.f16x2.e5m2x2 %0, %1;" : "=r"(r) : "h"(b));
+  return r;
+}
+__device__ __forceinline__ float f16_bits_to_float(uint32_t bits16) {
+  unsigned short b = static_cast<unsigned short>(bits16);
+  return __half2float(*reinterpret_cast<__half*>(&b));
+}
+__device__ __forceinline__ uint32_t float_to_bf16_bits(float f) {
+  __nv_bfloat16 h = __float2bfloat16_rn(f);
+  return *reinterpret_cast<unsigned short*>(&h);
+}
+
+template <> __device__ __forceinline__ F8E4M3 convert<float, F8E4M3>(float v) { return F8E4M3{static_cast<unsigned char>(f32x2_to_fp8x2<true>(__float_as_uint(v), 0u))}; }
+template <> __device__ __forceinline__ F8E5M2 convert<float, F8E5M2>(float v) { return F8E5M2{static_cast<unsigned char>(f32x2_to_fp8x2<false>(__float_as_uint(v), 0u))}; }
+template <> __device__ __forceinline__ F8E4M3 convert<__nv_bfloat16, F8E4M3>(__nv_bfloat16 v) { return convert<float, F8E4M3>(__bfloat162float(v)); }
+template <> __device__ __forceinline__ F8E5M2 convert<__nv_bfloat16, F8E5M2>(__nv_bfloat16 v) { return convert<float, F8E5M2>(__bfloat162float(v)); }
+template <> __device__ __forceinline__ F8E4M3 convert<__half, F8E4M3>(__half v) { return convert<float, F8E4M3>(__half2float(v)); }
+template <> __device__ __forceinline__ F8E5M2 convert<__half, F8E5M2>(__half v) { return convert<float, F8E5M2>(__half2float(v)); }
+template <> __device__ __forceinline__ float convert<F8E4M3, float>(F8E4M3 v) { return f16_bits_to_float(fp8x2_to_f16x2<true>(v.x)); }
+template <> __device__ __forceinline__ float convert<F8E5M2, float>(F8E5M2 v) { return f16_bits_to_float(fp8x2_to_f16x2<false>(v.x)); }
+template <> __device__ __forceinline__ __half convert<F8E4M3, __half>(F8E4M3 v) { return __float2half_rn(convert<F8E4M3, float>(v)); }
+template <> __device__ __forceinline__ __half convert<F8E5M2, __half>(F8E5M2 v) { return __float2half_rn(convert<F8E5M2, float>(v)); }
+template <> __device__ __forceinline__ __nv_bfloat16 convert<F8E4M3, __nv_bfloat16>(F8E4M3 v) { return __float2bfloat16_rn(convert<F8E4M3, float>(v)); }
+template <> __device__ __forceinline__ __nv_bfloat16 convert<F8E5M2, __nv_bfloat16>(F8E5M2 v) { return __float2bfloat16_rn(convert<F8E5M2, float>(v)); }
+
+__device__ __forceinline__ uint32_t word_of(const uint4& u, int i) { return i == 0 ? u.x : i == 1 ? u.y : i == 2 ? u.z : u.w; }
+
+// f32 bit patterns of elements (e, e+1) of a vector unit held as 32-bit words
+template <typename S>
+__device__ __forceinline__ void f32_pair(const uint4* q, int e, uint32_t& a, uint32_t& b);
+template <> __device__ __forceinline__ void f32_pair<float>(const uint4* q, int e, uint32_t& a, uint32_t& b) {
+  a = word_of(q[e >> 2], e & 3);
+  b = word_of(q[(e + 1) >> 2], (e + 1) & 3);
+}
+template <> __device__ __forceinline__ void f32_pair<__nv_bfloat16>(const uint4* q, int e, uint32_t& a, uint32_t& b) {
+  const uint32_t w = word_of(q[e >> 3], (e >> 1) & 3);
+  a = w << 16;
+  b = w & 0xffff0000u;
+}
+template <> __device__ __forceinline__ void f32_pair<__half>(const uint4* q, int e, uint32_t& a, uint32_t& b) {
+  const uint32_t w = word_of(q[e >> 3], (e >> 1) & 3);
+  a = __float_as_uint(f16_bits_to_float(w & 0xffffu));
+  b = __float_as_uint(f16_bits_to_float(w >> 16));
+}
+
+// 16 elements per unit; f32/bf16/f16 -> fp8 (64 or 32 B in, one 16 B store out)
+template <typename S, bool kE4M3>
+struct CastToFp8V16 {
+  static constexpr int kLoads = static_cast<int>(sizeof(S));  // 16-byte loads per unit: 4 (f32) or 2
+  static constexpr int kUnroll = 2;
+  struct Reg { uint4 q[kLoads]; };
+  static __device__ __forceinline__ Reg ld(const char* p) {
+    Reg r;
+#pragma unroll
+    for (int i = 0; i < kLoads; ++i) r.q[i] = ldg16(p + 16 * i);
+    return r;
+  }
+  static __device__ __forceinline__ uint32_t quad(const Reg& v, int e) {  // elements e..e+3 -> 4 bytes
+    uint32_t a, b, c, d;
+    f32_pair<S>(v.q, e, a, b);
+    f32_pair<S>(v.q, e + 2, c, d);
+    return f32x2_to_fp8x2<kE4M3>(a, b) | (f32x2_to_fp8x2<kE4M3>(c, d) << 16);
+  }
+  static __device__ __forceinline__ void st(char* p, const Reg& v) {
+    uint4 o{quad(v, 0), quad(v, 4), quad(v, 8), quad(v, 12)};
+    stg16(p, o);
+  }
+};
+
+// 16 elements per unit; fp8 -> f32/bf16/f16 (one 16 B load in, 64 or 32 B out)
+template <typename D, bool kE4M3>
+struct CastFromFp8V16 {
+  static constexpr int kStores = static_cast<int>(sizeof(D));  // 16-byte stores per unit: 4 (f32) or 2
+  static constexpr int kUnroll = 4;
+  using Reg = uint4;
+  static __device__ __forceinline__ Reg ld(const char* p) { return ldg16(p); }
+  static __device__ __forceinline__ void st(char* p, const Reg& v) {
+    uint32_t o[4 * kStores];
+#pragma unroll
+    for (int j = 0; j < 8; ++j) {  // element pairs (2j, 2j+1)
+      const uint32_t h2 = fp8x2_to_f16x2<kE4M3>(word_of(v, j >> 1) >> (16 * (j & 1)));
+      if (sizeof(D) == 2 && std::is_same<D, __half>::value) {
+        o[j] = h2;
+      } else if (sizeof(D) == 2) {
+        o[j] = float_to_bf16_bits(f16_bits_to_float(h2 & 0xffffu)) | (float_to_bf16_bits(f16_bits_to_float(h2 >> 16)) << 16);
+      } else {
+        o[2 * j] = __float_as_uint(f16_bits_to_float(h2 & 0xffffu));
+        o[2 * j + 1] = __float_as_uint(f16_bits_to_float(h2 >> 16));
+      }
+    }
+#pragma unroll
+    for (int i = 0; i < kStores; ++i) stg16(p + 16 * i, uint4{o[4 * i], o[4 * i + 1], o[4 * i + 2], o[4 * i + 3]});
   }
 };
 
@@ -278,6 +410,8 @@ __device__ __forceinline__ void move_tile(const DevRect& r, uint32_t tile_in_rec
 //   KIND_GENERIC  any mix of modes (per-tile dispatch, out-of-line movers)
 //   KIND_B16      every rect moves 16-byte units: the weight-sync case, fully inlined
 //   KIND_F32_BF16 every rect is the vector fp32->bf16 cast (transfer_dtype=bf16), fully inlined
+//   KIND_BF16_E4M3 every rect is the vector bf16->e4m3fn cast (a bf16 trainer's refresh for an fp8
+//                 generator), fully inlined
 template <int KIND>
 __device__ __forceinline__ void process_tile(const DevRect& r, uint32_t tile_in_rect) {
   const uint32_t tile_units = r.tile_units;
@@ -287,6 +421,10 @@ __device__ __forceinline__ void process_tile(const DevRect& r, uint32_t tile_in_
   }
   if (KIND == KIND_F32_BF16) {
     move_tile<CastNarrowV8<__nv_bfloat16>, true>(r, tile_in_rect, tile_units);
+    return;
+  }
+  if (KIND == KIND_BF16_E4M3) {
+    move_tile<CastToFp8V16<__nv_bfloat16, true>, true>(r, tile_in_rect, tile_units);
     return;
   }
   switch (r.mode) {
@@ -309,6 +447,30 @@ __device__ __forceinline__ void process_tile(const DevRect& r, uint32_t tile_in_
     case MODE_F16_BF16_S: move_tile<CastScalar<__half, __nv_bfloat16>, false>(r, tile_in_rect, tile_units); break;
     case MODE_F64_F32_S: move_tile<CastScalar<double, float>, false>(r, tile_in_rect, tile_units); break;
     case MODE_F32_F64_S: move_tile<CastScalar<float, double>, false>(r, tile_in_rect, tile_units); break;
+    case MODE_F32_E4M3_V16: move_tile<CastToFp8V16<float, true>, false>(r, tile_in_rect, tile_units); break;
+    case MODE_F32_E4M3_S: move_tile<CastScalar<float, F8E4M3>, false>(r, tile_in_rect, tile_units); break;
+    case MODE_F32_E5M2_V16: move_tile<CastToFp8V16<float, false>, false>(r, tile_in_rect, tile_units); break;
+    case MODE_F32_E5M2_S: move_tile<CastScalar<float, F8E5M2>, false>(r, tile_in_rect, tile_units); break;
+    case MODE_BF16_E4M3_V16: move_tile<CastToFp8V16<__nv_bfloat16, true>, false>(r, tile_in_rect, tile_units); break;
+    case MODE_BF16_E4M3_S: move_tile<CastScalar<__nv_bfloat16, F8E4M3>, false>(r, tile_in_rect, tile_units); break;
+    case MODE_BF16_E5M2_V16: move_tile<CastToFp8V16<__nv_bfloat16, false>, false>(r, tile_in_rect, tile_units); break;
+    case MODE_BF16_E5M2_S: move_tile<CastScalar<__nv_bfloat16, F8E5M2>, false>(r, tile_in_rect, tile_units); break;
+    case MODE_F16_E4M3_V16: move_tile<CastToFp8V16<__half, true>, false>(r, tile_in_rect, tile_units); break;
+    case MODE_F16_E4M3_S: move_tile<CastScalar<__half, F8E4M3>, false>(r, tile_in_rect, tile_units); break;
+    case MODE_F16_E5M2_V16: move_tile<CastToFp8V16<__half, false>, false>(r, tile_in_rect, tile_units); break;
+    case MODE_F16_E5M2_S: move_tile<CastScalar<__half, F8E5M2>, false>(r, tile_in_rect, tile_units); break;
+    case MODE_E4M3_F32_V16: move_tile<CastFromFp8V16<float, true>, false>(r, tile_in_rect, tile_units); break;
+    case MODE_E4M3_F32_S: move_tile<CastScalar<F8E4M3, float>, false>(r, tile_in_rect, tile_units); break;
+    case MODE_E5M2_F32_V16: move_tile<CastFromFp8V16<float, false>, false>(r, tile_in_rect, tile_units); break;
+    case MODE_E5M2_F32_S: move_tile<CastScalar<F8E5M2, float>, false>(r, tile_in_rect, tile_units); break;
+    case MODE_E4M3_BF16_V16: move_tile<CastFromFp8V16<__nv_bfloat16, true>, false>(r, tile_in_rect, tile_units); break;
+    case MODE_E4M3_BF16_S: move_tile<CastScalar<F8E4M3, __nv_bfloat16>, false>(r, tile_in_rect, tile_units); break;
+    case MODE_E5M2_BF16_V16: move_tile<CastFromFp8V16<__nv_bfloat16, false>, false>(r, tile_in_rect, tile_units); break;
+    case MODE_E5M2_BF16_S: move_tile<CastScalar<F8E5M2, __nv_bfloat16>, false>(r, tile_in_rect, tile_units); break;
+    case MODE_E4M3_F16_V16: move_tile<CastFromFp8V16<__half, true>, false>(r, tile_in_rect, tile_units); break;
+    case MODE_E4M3_F16_S: move_tile<CastScalar<F8E4M3, __half>, false>(r, tile_in_rect, tile_units); break;
+    case MODE_E5M2_F16_V16: move_tile<CastFromFp8V16<__half, false>, false>(r, tile_in_rect, tile_units); break;
+    case MODE_E5M2_F16_S: move_tile<CastScalar<F8E5M2, __half>, false>(r, tile_in_rect, tile_units); break;
     default: break;
   }
 }
@@ -573,6 +735,7 @@ int max_ctas_per_sm(uint32_t kind, bool with_link, uint32_t link_smem_bytes, int
   switch (kind) {
     case KIND_B16: e = occupancy<KIND_B16>(with_link, smem, &n); break;
     case KIND_F32_BF16: e = occupancy<KIND_F32_BF16>(with_link, smem, &n); break;
+    case KIND_BF16_E4M3: e = occupancy<KIND_BF16_E4M3>(with_link, smem, &n); break;
     default: e = occupancy<KIND_GENERIC>(with_link, smem, &n); break;
   }
   if (e != cudaSuccess) return cuda_fail(e, "cudaOccupancyMaxActiveBlocksPerMultiprocessor");
@@ -592,6 +755,7 @@ int launch_copy_rects(const LaunchParams& p, uint32_t grid, cudaStream_t stream)
   switch (p.kind) {
     case KIND_B16: e = launch<KIND_B16>(p, grid, stream); break;
     case KIND_F32_BF16: e = launch<KIND_F32_BF16>(p, grid, stream); break;
+    case KIND_BF16_E4M3: e = launch<KIND_BF16_E4M3>(p, grid, stream); break;
     default: e = launch<KIND_GENERIC>(p, grid, stream); break;
   }
   if (e != cudaSuccess) return cuda_fail(e, "copy_rects_kernel launch");

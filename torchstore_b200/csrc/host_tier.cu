@@ -25,7 +25,7 @@ namespace {
 
 uint32_t host_dtype_size(uint32_t dt) {
   switch (dt) {
-    case TSB_U8: return 1;
+    case TSB_U8: case TSB_F8E4M3: case TSB_F8E5M2: return 1;
     case TSB_U16: case TSB_F16: case TSB_BF16: return 2;
     case TSB_U32: case TSB_F32: return 4;
     case TSB_U64: case TSB_F64: return 8;

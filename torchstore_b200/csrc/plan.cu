@@ -82,7 +82,7 @@ PlanRegistry& R() {
 
 uint32_t dtype_size(uint32_t dt) {
   switch (dt) {
-    case TSB_U8: return 1;
+    case TSB_U8: case TSB_F8E4M3: case TSB_F8E5M2: return 1;
     case TSB_U16: case TSB_F16: case TSB_BF16: return 2;
     case TSB_U32: case TSB_F32: return 4;
     case TSB_U64: case TSB_F64: return 8;
@@ -90,19 +90,26 @@ uint32_t dtype_size(uint32_t dt) {
   }
 }
 
-// (vector mode, scalar mode) for a cross-dtype pair, or false
-bool cast_modes(uint32_t s, uint32_t d, uint32_t* vmode, uint32_t* smode) {
-  struct Row { uint32_t s, d, v, sc; };
+// (vector mode, scalar mode, elements per vector unit) for a cross-dtype pair, or false
+bool cast_modes(uint32_t s, uint32_t d, uint32_t* vmode, uint32_t* smode, uint32_t* velems = nullptr) {
+  struct Row { uint32_t s, d, v, sc, ve; };
   static const Row table[] = {
-      {TSB_F32, TSB_BF16, MODE_F32_BF16_V8, MODE_F32_BF16_S}, {TSB_F32, TSB_F16, MODE_F32_F16_V8, MODE_F32_F16_S},
-      {TSB_BF16, TSB_F32, MODE_BF16_F32_V8, MODE_BF16_F32_S}, {TSB_F16, TSB_F32, MODE_F16_F32_V8, MODE_F16_F32_S},
-      {TSB_BF16, TSB_F16, MODE_BF16_F16_V8, MODE_BF16_F16_S}, {TSB_F16, TSB_BF16, MODE_F16_BF16_V8, MODE_F16_BF16_S},
-      {TSB_F64, TSB_F32, 0xffffffffu, MODE_F64_F32_S},        {TSB_F32, TSB_F64, 0xffffffffu, MODE_F32_F64_S},
+      {TSB_F32, TSB_BF16, MODE_F32_BF16_V8, MODE_F32_BF16_S, 8},         {TSB_F32, TSB_F16, MODE_F32_F16_V8, MODE_F32_F16_S, 8},
+      {TSB_BF16, TSB_F32, MODE_BF16_F32_V8, MODE_BF16_F32_S, 8},         {TSB_F16, TSB_F32, MODE_F16_F32_V8, MODE_F16_F32_S, 8},
+      {TSB_BF16, TSB_F16, MODE_BF16_F16_V8, MODE_BF16_F16_S, 8},         {TSB_F16, TSB_BF16, MODE_F16_BF16_V8, MODE_F16_BF16_S, 8},
+      {TSB_F64, TSB_F32, 0xffffffffu, MODE_F64_F32_S, 0},                {TSB_F32, TSB_F64, 0xffffffffu, MODE_F32_F64_S, 0},
+      {TSB_F32, TSB_F8E4M3, MODE_F32_E4M3_V16, MODE_F32_E4M3_S, 16},     {TSB_F32, TSB_F8E5M2, MODE_F32_E5M2_V16, MODE_F32_E5M2_S, 16},
+      {TSB_BF16, TSB_F8E4M3, MODE_BF16_E4M3_V16, MODE_BF16_E4M3_S, 16},  {TSB_BF16, TSB_F8E5M2, MODE_BF16_E5M2_V16, MODE_BF16_E5M2_S, 16},
+      {TSB_F16, TSB_F8E4M3, MODE_F16_E4M3_V16, MODE_F16_E4M3_S, 16},     {TSB_F16, TSB_F8E5M2, MODE_F16_E5M2_V16, MODE_F16_E5M2_S, 16},
+      {TSB_F8E4M3, TSB_F32, MODE_E4M3_F32_V16, MODE_E4M3_F32_S, 16},     {TSB_F8E5M2, TSB_F32, MODE_E5M2_F32_V16, MODE_E5M2_F32_S, 16},
+      {TSB_F8E4M3, TSB_BF16, MODE_E4M3_BF16_V16, MODE_E4M3_BF16_S, 16},  {TSB_F8E5M2, TSB_BF16, MODE_E5M2_BF16_V16, MODE_E5M2_BF16_S, 16},
+      {TSB_F8E4M3, TSB_F16, MODE_E4M3_F16_V16, MODE_E4M3_F16_S, 16},     {TSB_F8E5M2, TSB_F16, MODE_E5M2_F16_V16, MODE_E5M2_F16_S, 16},
   };
   for (const Row& r : table)
     if (r.s == s && r.d == d) {
       *vmode = r.v;
       *smode = r.sc;
+      if (velems) *velems = r.ve;
       return true;
     }
   return false;
@@ -228,7 +235,7 @@ struct Compiler {
     info.src_bytes += rows * units * sub;
     if (remote) info.remote_src_bytes += rows * units * sub;
     if (link) info.link_bytes += rows * units * sub;
-    if (mode == MODE_B16 || (mode >= MODE_F32_BF16_V8 && (mode % 2) == 0 && mode <= MODE_F16_BF16_V8)) info.num_vector_rects++;
+    if (is_vector_mode(mode)) info.num_vector_rects++;
   }
 
   int add(const tsb_rect_t& in, uint64_t index) {
@@ -236,9 +243,9 @@ struct Compiler {
     if (in.ndim < 1 || in.ndim > TSB_MAX_DIMS) return fail(TSB_ERR_INVALID, where + "ndim must be in [1, " + std::to_string(TSB_MAX_DIMS) + "]");
     const uint32_t es = dtype_size(in.src_dtype), ed = dtype_size(in.dst_dtype);
     if (!es || !ed) return fail(TSB_ERR_INVALID, where + "unknown dtype");
-    uint32_t vmode = 0, smode = 0;
+    uint32_t vmode = 0, smode = 0, velems = 0;
     const bool is_cast = in.src_dtype != in.dst_dtype;
-    if (is_cast && !cast_modes(in.src_dtype, in.dst_dtype, &vmode, &smode))
+    if (is_cast && !cast_modes(in.src_dtype, in.dst_dtype, &vmode, &smode, &velems))
       return fail(TSB_ERR_UNSUPPORTED, where + "dtype cast " + std::to_string(in.src_dtype) + " -> " + std::to_string(in.dst_dtype) + " is not implemented");
 
     std::vector<Dim> dims;
@@ -289,8 +296,9 @@ struct Compiler {
       if (in.src % es || in.dst % ed) return fail(TSB_ERR_INVALID, where + "src/dst not aligned to their element size");
       for (const Dim& d : dims)
         if (d.ss % static_cast<int64_t>(es) || d.ds % static_cast<int64_t>(ed)) return fail(TSB_ERR_INVALID, where + "stride not a multiple of the element size");
-      if (vmode != 0xffffffffu && all_aligned(16) && run % 8 == 0) {
-        emit(in.src, in.dst, dims, static_cast<uint64_t>(run) / 8, vmode, 8 * es, 8 * ed, in.src_device);
+      // vector unit: 8 elements (16-bit/32-bit pairs) or 16 (fp8 pairs: the fp8 side is one 16-byte access)
+      if (vmode != 0xffffffffu && all_aligned(16) && run % velems == 0) {
+        emit(in.src, in.dst, dims, static_cast<uint64_t>(run) / velems, vmode, velems * es, velems * ed, in.src_device);
       } else {
         emit(in.src, in.dst, dims, static_cast<uint64_t>(run), smode, es, ed, in.src_device);
       }
@@ -300,12 +308,13 @@ struct Compiler {
 
   uint32_t kind() const {
     if (rects.empty()) return KIND_GENERIC;
-    bool all_b16 = true, all_cast = true;
+    bool all_b16 = true, all_cast = true, all_fp8 = true;
     for (const DevRect& r : rects) {
       all_b16 = all_b16 && r.mode == MODE_B16;
       all_cast = all_cast && r.mode == MODE_F32_BF16_V8;
+      all_fp8 = all_fp8 && r.mode == MODE_BF16_E4M3_V16;
     }
-    return all_b16 ? KIND_B16 : all_cast ? KIND_F32_BF16 : KIND_GENERIC;
+    return all_b16 ? KIND_B16 : all_cast ? KIND_F32_BF16 : all_fp8 ? KIND_BF16_E4M3 : KIND_GENERIC;
   }
 
   // Tile order of one queue: proportional interleave over source devices, starting after the

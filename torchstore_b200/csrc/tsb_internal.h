@@ -65,7 +65,38 @@ enum : uint32_t {
   MODE_F16_BF16_S = 19,
   MODE_F64_F32_S = 20,
   MODE_F32_F64_S = 21,
+  // fp8 casts: unit = 16 elements (vector: the fp8 side is one 16-byte access) or 1 element (scalar)
+  MODE_F32_E4M3_V16 = 22,
+  MODE_F32_E4M3_S = 23,
+  MODE_F32_E5M2_V16 = 24,
+  MODE_F32_E5M2_S = 25,
+  MODE_BF16_E4M3_V16 = 26,
+  MODE_BF16_E4M3_S = 27,
+  MODE_BF16_E5M2_V16 = 28,
+  MODE_BF16_E5M2_S = 29,
+  MODE_F16_E4M3_V16 = 30,
+  MODE_F16_E4M3_S = 31,
+  MODE_F16_E5M2_V16 = 32,
+  MODE_F16_E5M2_S = 33,
+  MODE_E4M3_F32_V16 = 34,
+  MODE_E4M3_F32_S = 35,
+  MODE_E5M2_F32_V16 = 36,
+  MODE_E5M2_F32_S = 37,
+  MODE_E4M3_BF16_V16 = 38,
+  MODE_E4M3_BF16_S = 39,
+  MODE_E5M2_BF16_V16 = 40,
+  MODE_E5M2_BF16_S = 41,
+  MODE_E4M3_F16_V16 = 42,
+  MODE_E4M3_F16_S = 43,
+  MODE_E5M2_F16_V16 = 44,
+  MODE_E5M2_F16_S = 45,
 };
+
+// modes whose units are 16-byte accesses on both sides (plan info: num_vector_rects)
+constexpr bool is_vector_mode(uint32_t m) {
+  return m == MODE_B16 || (m >= MODE_F32_BF16_V8 && m <= MODE_F16_BF16_V8 && m % 2 == 0) ||
+         (m >= MODE_F32_E4M3_V16 && m <= MODE_E5M2_F16_V16 && m % 2 == 0);
+}
 
 constexpr int kMaxOuter = TSB_MAX_DIMS;  // outer (row) dims after splitting off the run
 
@@ -98,7 +129,7 @@ struct DevTile {
 };
 
 // kernel specialisations (see copy_rects.cu)
-enum : uint32_t { KIND_GENERIC = 0, KIND_B16 = 1, KIND_F32_BF16 = 2 };
+enum : uint32_t { KIND_GENERIC = 0, KIND_B16 = 1, KIND_F32_BF16 = 2, KIND_BF16_E4M3 = 3 };
 
 // Two work queues per plan (see copy_rects.cu):
 //   copy queue  tiles moved by the CTA's 8 copy warps with LDG.128/STG.128 (local HBM sources,

@@ -13,7 +13,8 @@ the data plane replaced:
   over NVLink (peer-mapped addresses) and stores coalesced into the destination shard;
 * ``transfer_dtype`` staging is refreshed by one batched fused-cast launch instead of one
   ``staging.copy_(src)`` per parameter (reference :158-169); if a handle's dtype differs from the
-  destination's, the cast is fused into the gather itself.
+  destination's, the cast is fused into the gather itself.  Pairs the fused cast does not cover
+  (an int64 buffer, float64 staging, ...) keep the reference's ``staging.copy_(src)``.
 
 Typical usage is unchanged::
 
@@ -33,6 +34,7 @@ from dataclasses import dataclass
 
 import torch
 
+from torchstore_b200 import _native
 from torchstore_b200.launch import Plans, copy_once, wait_copy_stream
 from torchstore_b200.planner import HbmDescriptor, StridedMem
 from torchstore_b200.transport.types import Request, TensorSlice
@@ -146,7 +148,9 @@ class DirectWeightSyncSource:
     """Registers live parameter memory (zero-copy) or dtype-cast staging buffers.
 
     With ``transfer_dtype`` every param gets an HBM staging buffer in that dtype; ``refresh()``
-    re-casts all of them with ONE fused-cast kernel launch per device.
+    re-casts all of them with ONE fused-cast kernel launch per device.  A param whose dtype has no
+    fused cast to ``transfer_dtype`` is refreshed like the reference does it, with
+    ``staging.copy_(source)`` on the caller's stream.
     """
 
     def __init__(self) -> None:
@@ -154,6 +158,7 @@ class DirectWeightSyncSource:
         # name -> (staging_buffer, source_local_tensor)
         self._staging: dict[str, tuple[torch.Tensor, torch.Tensor]] = {}
         self._refresh_plans = Plans()
+        self._copied: list[tuple[torch.Tensor, torch.Tensor]] = []  # (staging, source) refreshed with copy_
         self._devices: tuple[int, ...] = ()  # devices holding registered memory (fence targets)
 
     def register(self, state_dict: dict[str, torch.Tensor], rank: int,
@@ -166,6 +171,7 @@ class DirectWeightSyncSource:
         handles: dict[str, RDMAWeightHandle] = {}
         self._refresh_plans.close()
         self._staging = {}
+        self._copied = []
         casts: dict[int, list] = defaultdict(list)  # device -> (source, staging) windows of the refresh
         devices = set()
         for name, param in state_dict.items():
@@ -178,7 +184,10 @@ class DirectWeightSyncSource:
             if transfer_dtype is not None:
                 staging = torch.empty(local.shape, dtype=transfer_dtype, device=local.device)
                 self._staging[name] = (staging, local)
-                casts[local.device.index].append((StridedMem.from_tensor(local), StridedMem.from_tensor(staging)))
+                if fused_refresh(local.dtype, transfer_dtype):
+                    casts[local.device.index].append((StridedMem.from_tensor(local), StridedMem.from_tensor(staging)))
+                else:
+                    self._copied.append((staging, local))
                 buf = staging
             else:
                 assert local.is_contiguous(), f"Expected contiguous tensor for key={name}, strides={local.stride()}"
@@ -187,7 +196,8 @@ class DirectWeightSyncSource:
         self._handles = handles
         self._devices = tuple(sorted(devices))
         if self._staging:
-            self._refresh_plans = Plans.build(casts)
+            if casts:
+                self._refresh_plans = Plans.build(casts)
             self.refresh()
         else:
             # make sure the weights the handles point at are materialised before anyone reads them
@@ -201,10 +211,14 @@ class DirectWeightSyncSource:
         """Re-cast the source params into their staging buffers (no-op without transfer_dtype).
         Returns the number of staging buffers refreshed.  Blocks until the cast has landed so the
         caller may publish/notify right after, like the reference's synchronous copy loop."""
-        if not self._refresh_plans:
+        if not self._staging:
             return 0
         self._refresh_plans.launch()
+        for staging, local in self._copied:
+            staging.copy_(local)
         self._refresh_plans.synchronize()
+        for dev in {local.device.index for _, local in self._copied}:
+            torch.cuda.current_stream(dev).synchronize()
         return len(self._staging)
 
     def fence(self) -> None:
@@ -219,7 +233,14 @@ class DirectWeightSyncSource:
             await handle.rdma_buffer.drop()
         self._handles.clear()
         self._staging.clear()
+        self._copied.clear()
         self._refresh_plans.close()
+
+
+def fused_refresh(src_dtype: torch.dtype, transfer_dtype: torch.dtype) -> bool:
+    """Does a ``src_dtype`` param's ``transfer_dtype`` staging refresh in the batched fused-cast
+    launch?  Otherwise :meth:`DirectWeightSyncSource.refresh` uses ``staging.copy_(source)``."""
+    return _native.cast_supported(src_dtype, transfer_dtype)
 
 
 # ---------------------------------------------------------------------------------------------

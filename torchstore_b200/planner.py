@@ -128,8 +128,8 @@ def fill_rect(rect: "_native.Rect", src: StridedMem, dst: StridedMem) -> bool:
             raise NotImplementedError("16-byte elements are not supported")
         rect.src_dtype = rect.dst_dtype = code
     else:
-        rect.src_dtype = _native.dtype_code(src.dtype)
-        rect.dst_dtype = _native.dtype_code(dst.dtype)
+        rect.src_dtype = _native.cast_code(src.dtype)
+        rect.dst_dtype = _native.cast_code(dst.dtype)
     rect.src_device = src.device
     return True
 
