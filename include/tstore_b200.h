@@ -26,7 +26,7 @@
 extern "C" {
 #endif
 
-#define TSB_ABI_VERSION 3
+#define TSB_ABI_VERSION 4
 #define TSB_MAX_DIMS 6
 
 enum {
@@ -204,6 +204,39 @@ int tsb_plan_compile_host(int device, const tsb_rect_t* rects, uint64_t n, uint3
 int tsb_copy_rects(int device, const tsb_rect_t* rects, uint64_t n, uint32_t flags, void* stream);
 /* Table-pool counters (tests / diagnostics). */
 int tsb_pool_stats(uint64_t* out_blocks, uint64_t* out_allocs, uint64_t* out_reuses);
+
+/* ------------------------------------------------------------------------------------------ */
+/* block-scaled FP8 destinations (DeepSeek-V3 / vLLM weight_block_size=[128, 128] layout):      */
+/* the pull quantises while it gathers                                                          */
+/* ------------------------------------------------------------------------------------------ */
+
+/* One block-scaled destination: `batch` independent [rows, cols] matrices.  Every 128x128 block
+ * (anchored at (0, 0); edge blocks are partial) gets one scale:
+ *   amax = max |x| over the block (NaN if any x is NaN); amax_c = max(amax, 1e-4f) (NaN stays NaN)
+ *   dst[i, j] = e4m3fn(rn(x[i, j] * (448 / amax_c)))  with torch's .to(float8_e4m3fn) rounding
+ *   scale_inv[i / 128, j / 128] = amax_c / 448
+ * with correctly rounded f32 divisions and multiply, x widened exactly to f32. */
+typedef struct tsb_bq_target {
+  uint64_t dst;       /* float8_e4m3fn, contiguous [batch, rows, cols] */
+  uint64_t scale_inv; /* float32, contiguous [batch, ceil(rows/128), ceil(cols/128)] */
+  uint64_t batch, rows, cols;
+} tsb_bq_target_t;
+
+/* Compile a block-scaled pull: `rects` are ordinary source -> destination rectangles with
+ * src_dtype in {TSB_F32, TSB_BF16, TSB_F16}, dst_dtype == TSB_F8E4M3 and dst inside one target.
+ * Every element of every target must be written by exactly one rect (TSB_ERR_INVALID otherwise: a
+ * block's scale needs all of it).  The result is a plan like any other: tsb_plan_launch[_flags],
+ * _run, _poll, _wait, _elapsed_ms, _info and _destroy accept it.  flags: reserved, pass 0. */
+int tsb_block_fp8_plan_create(int device, const tsb_rect_t* rects, uint64_t n, const tsb_bq_target_t* targets,
+                              uint64_t n_targets, uint32_t flags, tsb_plan_t* out);
+/* Host-only (no CUDA call): compile and copy the kernel tables out.  out_blocks: records of 32 bytes
+ *   {u64 dst, u64 scale_inv, u32 dst_pitch, u16 rows, u16 cols, u32 first_piece, u16 n_pieces, u16 src_dtype}
+ * out_pieces: records of 32 bytes
+ *   {u64 src, i64 src_row_stride_bytes, u16 row0, u16 col0, u16 rows, u16 cols, u32 vector, u32 pad}
+ * (row0/col0 relative to the block; vector: 16-byte loads).  A NULL table only reports its count. */
+int tsb_block_fp8_compile_host(int device, const tsb_rect_t* rects, uint64_t n, const tsb_bq_target_t* targets,
+                               uint64_t n_targets, uint32_t flags, void* out_blocks, uint64_t block_cap,
+                               uint64_t* out_n_blocks, void* out_pieces, uint64_t piece_cap, uint64_t* out_n_pieces);
 
 /* ------------------------------------------------------------------------------------------ */
 /* streams and events (the await points of the reference's coroutines)                         */

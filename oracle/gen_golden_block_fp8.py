@@ -1,0 +1,48 @@
+"""TEST INFRASTRUCTURE ONLY -- records tests/golden/block_fp8_vectors.npz.
+
+The inputs are block_fp8_oracle.fixture_inputs(), rebuilt bit for bit from an integer hash wherever
+the tests run, so the fixture does not carry them: per case it keeps the dtype, the sha256 of the
+input bits (to catch a drifted generator), torch CPU's scale_inv in full and the sha256 of torch
+CPU's fp8 bytes (block_fp8_oracle.torch_quantize, tensor/tensor ops).  A case with non-finite blocks
+keeps its fp8 bytes in full instead: NaN bytes are platform-specific there, so the tests compare
+them NaN-agnostically.
+
+    python oracle/gen_golden_block_fp8.py
+"""
+
+from __future__ import annotations
+
+import os
+import sys
+
+import numpy as np
+import torch
+
+sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
+
+from oracle.block_fp8_oracle import bits_of, digest, fixture_inputs, torch_quantize  # noqa: E402
+
+OUT = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "tests", "golden", "block_fp8_vectors.npz")
+
+
+def main():
+    arrays = {}
+    names = []
+    for i, (name, x) in enumerate(fixture_inputs()):
+        q, s = torch_quantize(x)
+        q, s = q.view(torch.uint8).numpy(), s.numpy()
+        names.append(name)
+        arrays[f"dtype{i}"] = np.array(str(x.dtype).replace("torch.", ""))
+        arrays[f"x_sha{i}"] = np.array(digest(bits_of(x)))
+        arrays[f"s{i}"] = s
+        if np.isfinite(s).all():
+            arrays[f"q_sha{i}"] = np.array(digest(q))
+        else:
+            arrays[f"q{i}"] = q
+    arrays["names"] = np.array(names)
+    np.savez_compressed(OUT, **arrays)
+    print(f"wrote {len(names)} cases to {OUT}")
+
+
+if __name__ == "__main__":
+    main()

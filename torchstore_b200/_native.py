@@ -16,7 +16,7 @@ import torch
 from torchstore_b200._build import LIB_PATH
 
 TSB_MAX_DIMS = 6
-TSB_ABI_VERSION = 3
+TSB_ABI_VERSION = 4
 
 TSB_OK, TSB_ERR_INVALID, TSB_ERR_CUDA, TSB_ERR_UNSUPPORTED, TSB_ERR_NOMEM, TSB_ERR_NOTFOUND = range(6)
 
@@ -84,6 +84,18 @@ class PlanInfo(C.Structure):
         return {name: int(getattr(self, name)) for name, _ in self._fields_}
 
 
+class BqTarget(C.Structure):
+    """tsb_bq_target_t: one block-scaled fp8 destination."""
+
+    _fields_ = [
+        ("dst", C.c_uint64),
+        ("scale_inv", C.c_uint64),
+        ("batch", C.c_uint64),
+        ("rows", C.c_uint64),
+        ("cols", C.c_uint64),
+    ]
+
+
 class ArenaStats(C.Structure):
     _fields_ = [
         ("capacity", C.c_uint64),
@@ -126,6 +138,14 @@ _SIGNATURES = {
          _vp, C.c_uint64, C.POINTER(C.c_uint64), C.POINTER(PlanInfo)],
     ),
     "tsb_copy_rects": (C.c_int, [C.c_int, C.POINTER(Rect), C.c_uint64, C.c_uint32, _vp]),
+    "tsb_block_fp8_plan_create": (
+        C.c_int, [C.c_int, C.POINTER(Rect), C.c_uint64, C.POINTER(BqTarget), C.c_uint64, C.c_uint32, C.POINTER(C.c_uint64)],
+    ),
+    "tsb_block_fp8_compile_host": (
+        C.c_int,
+        [C.c_int, C.POINTER(Rect), C.c_uint64, C.POINTER(BqTarget), C.c_uint64, C.c_uint32, _vp, C.c_uint64,
+         C.POINTER(C.c_uint64), _vp, C.c_uint64, C.POINTER(C.c_uint64)],
+    ),
     "tsb_stream_create": (C.c_int, [C.c_int, C.POINTER(_vp)]),
     "tsb_stream_destroy": (C.c_int, [_vp]),
     "tsb_stream_sync": (C.c_int, [C.c_int, _vp]),
@@ -369,6 +389,38 @@ def plan_compile_host(device: int, rects, n: int, flags: int = 0, tile_units: in
                                   C.byref(n_rects), tile_buf.ctypes.data, n_tiles.value, C.byref(n_tiles),
                                   C.byref(info)))
     return rect_buf[: n_rects.value * 192], tile_buf[: n_tiles.value], info
+
+
+def make_target_array(n: int):
+    return (BqTarget * n)()
+
+
+def block_fp8_plan_create(device: int, rects, n: int, targets, n_targets: int) -> int:
+    out = C.c_uint64(0)
+    check(lib().tsb_block_fp8_plan_create(device, rects, n, targets, n_targets, 0, C.byref(out)))
+    return int(out.value)
+
+
+# record layouts of tsb_block_fp8_compile_host (include/tstore_b200.h)
+BQ_BLOCK_DTYPE = [("dst", "<u8"), ("scale_inv", "<u8"), ("pitch", "<u4"), ("rows", "<u2"), ("cols", "<u2"),
+                  ("piece0", "<u4"), ("n_pieces", "<u2"), ("src_dtype", "<u2")]
+BQ_PIECE_DTYPE = [("src", "<u8"), ("src_stride", "<i8"), ("row0", "<u2"), ("col0", "<u2"), ("rows", "<u2"),
+                  ("cols", "<u2"), ("vec", "<u4"), ("pad", "<u4")]
+
+
+def block_fp8_compile_host(device: int, rects, n: int, targets, n_targets: int):
+    """Host-only compilation of a block-scaled fp8 pull -> (blocks, pieces) numpy record arrays."""
+    import numpy as np
+
+    nb, npc = C.c_uint64(0), C.c_uint64(0)
+    L = lib()
+    check(L.tsb_block_fp8_compile_host(device, rects, n, targets, n_targets, 0, None, 0, C.byref(nb), None, 0,
+                                       C.byref(npc)))
+    blocks = np.zeros(max(1, nb.value), dtype=BQ_BLOCK_DTYPE)
+    pieces = np.zeros(max(1, npc.value), dtype=BQ_PIECE_DTYPE)
+    check(L.tsb_block_fp8_compile_host(device, rects, n, targets, n_targets, 0, blocks.ctypes.data, nb.value,
+                                       C.byref(nb), pieces.ctypes.data, npc.value, C.byref(npc)))
+    return blocks[: nb.value], pieces[: npc.value]
 
 
 CUDA_STREAM_LEGACY = 0x1  # cudaStreamLegacy: an explicit handle for the default stream

@@ -1,0 +1,493 @@
+// Block-scaled FP8 pulls (sm_90a, H100): gather bf16/f16/f32 source rectangles into float8_e4m3fn
+// destinations stored the way DeepSeek-V3 / vLLM (weight_block_size=[128, 128]) keep FP8 weights, one
+// float32 scale_inv per 128x128 block, quantising on the way.  Each source byte is read once.
+//
+// Host side: the plan compiler maps every rect onto its target's [batch, rows, cols] grid, cuts it
+// at block boundaries into pieces, sorts the pieces by block and checks that they tile every block
+// exactly (an uncovered element would leave the block's amax undefined).
+// Device side: one CTA of 256 threads per block.
+//   phase 1  the block's pieces (from any shard, local or peer-mapped) land in shared memory in their
+//            source dtype, 16-byte loads where address, stride and width allow it, and every thread
+//            folds |x| into a running max as the data arrives.  |x| is compared as an integer (sign
+//            bit cleared): for non-negative floats that orders finite < Inf < NaN, so a NaN anywhere
+//            makes the block's amax NaN (fmaxf would drop it).
+//   reduce   warp max, then one thread: amax_c = max(amax, 1e-4f), scale = 448 / amax_c and
+//            scale_inv = amax_c / 448, both correctly rounded (__fdiv_rn).
+//   phase 2  shared -> e4m3fn: x * scale (__fmul_rn), torch-exact narrowing (fp8_cvt.cuh), 16
+//            destination bytes per thread and step (one STG.128 when aligned, byte stores at ragged edges).
+
+#include <cuda_fp16.h>
+
+#include <algorithm>
+#include <atomic>
+#include <cstring>
+
+#include "fp8_cvt.cuh"
+#include "tsb_internal.h"
+
+namespace tsb {
+
+namespace {
+
+uint32_t src_elem_bytes(uint32_t dt) {
+  switch (dt) {
+    case TSB_F32: return 4;
+    case TSB_BF16: case TSB_F16: return 2;
+    default: return 0;
+  }
+}
+
+// A rect after mapping onto its target: a [er, ec] box at (b, r0, c0).
+struct Box {
+  uint64_t src;
+  int64_t row_stride;  // source bytes between rows (0 for a single row)
+  uint64_t target, b, r0, c0, er, ec;
+  uint32_t dtype;
+  int32_t src_device;
+};
+
+struct Dim {
+  int64_t e, ss, ds;
+};
+
+int rect_boxes(const tsb_rect_t& in, uint64_t index, const tsb_bq_target_t* targets, uint64_t n_targets,
+               std::vector<Box>* out) {
+  const std::string where = "rect " + std::to_string(index) + ": ";
+  if (in.ndim < 1 || in.ndim > TSB_MAX_DIMS) return fail(TSB_ERR_INVALID, where + "ndim must be in [1, 6]");
+  const uint32_t es = src_elem_bytes(in.src_dtype);
+  if (!es) return fail(TSB_ERR_UNSUPPORTED, where + "block-scaled fp8 reads f32, bf16 or f16 sources");
+  if (in.dst_dtype != TSB_F8E4M3) return fail(TSB_ERR_UNSUPPORTED, where + "block-scaled destinations are float8_e4m3fn");
+  std::vector<Dim> work;
+  for (uint32_t i = 0; i < in.ndim; ++i) {
+    if (in.extent[i] < 0) return fail(TSB_ERR_INVALID, where + "negative extent");
+    if (in.extent[i] == 0) return TSB_OK;
+    if (in.extent[i] > 1) work.push_back({in.extent[i], in.src_stride[i], in.dst_stride[i]});
+  }
+  if (in.src == 0 || in.dst == 0) return fail(TSB_ERR_INVALID, where + "NULL src/dst");
+  uint64_t t = 0;
+  while (t < n_targets && !(in.dst >= targets[t].dst && in.dst - targets[t].dst < targets[t].batch * targets[t].rows * targets[t].cols)) ++t;
+  if (t == n_targets) return fail(TSB_ERR_INVALID, where + "dst is inside no target");
+  const int64_t R = static_cast<int64_t>(targets[t].rows), C = static_cast<int64_t>(targets[t].cols);
+  const int64_t B = static_cast<int64_t>(targets[t].batch);
+  const uint64_t o = in.dst - targets[t].dst;
+  const int64_t b0 = static_cast<int64_t>(o / (R * C)), r0 = static_cast<int64_t>(o % (R * C)) / C, c0 = static_cast<int64_t>(o % C);
+  // Classify every dim by its destination step: columns (1), rows (C) or whole matrices (multiple of
+  // R*C).  A collapsed dim that runs past the end of a row (or of a matrix) is split back.
+  int64_t er = 1, ec = 1, row_ss = 0, col_ss = es;
+  bool have_row = false, have_col = false;
+  std::vector<Dim> batch;
+  const std::string bad = where + "its destination strides do not describe a box of the target";
+  while (!work.empty()) {
+    const Dim d = work.back();
+    work.pop_back();
+    if (d.ds == 1 && C > 1) {
+      if (c0 + d.e <= C) {
+        if (have_col) return fail(TSB_ERR_INVALID, bad);
+        have_col = true;
+        ec = d.e;
+        col_ss = d.ss;
+      } else if (c0 == 0 && d.e % C == 0) {
+        work.push_back({d.e / C, d.ss * C, C});
+        work.push_back({C, d.ss, 1});
+      } else {
+        return fail(TSB_ERR_INVALID, bad);
+      }
+    } else if (d.ds == C && R > 1) {
+      if (r0 + d.e <= R) {
+        if (have_row) return fail(TSB_ERR_INVALID, bad);
+        have_row = true;
+        er = d.e;
+        row_ss = d.ss;
+      } else if (r0 == 0 && d.e % R == 0) {
+        work.push_back({d.e / R, d.ss * R, R * C});
+        work.push_back({R, d.ss, C});
+      } else {
+        return fail(TSB_ERR_INVALID, bad);
+      }
+    } else if (d.ds > 0 && d.ds % (R * C) == 0) {
+      batch.push_back({d.e, d.ss, d.ds / (R * C)});
+    } else {
+      return fail(TSB_ERR_INVALID, bad);
+    }
+  }
+  int64_t b_last = b0;
+  for (const Dim& d : batch) b_last += (d.e - 1) * d.ds;
+  if (b_last >= B) return fail(TSB_ERR_INVALID, bad);
+  if (have_col && col_ss != static_cast<int64_t>(es))
+    return fail(TSB_ERR_UNSUPPORTED, where + "block-scaled pulls read contiguous source rows");
+  if (in.src % es || row_ss % es) return fail(TSB_ERR_INVALID, where + "source not aligned to its element size");
+  for (const Dim& d : batch)
+    if (d.ss % es) return fail(TSB_ERR_INVALID, where + "source not aligned to its element size");
+  // one box per combination of the batch dims
+  std::vector<int64_t> k(batch.size(), 0);
+  while (true) {
+    int64_t b = b0, so = 0;
+    for (size_t i = 0; i < batch.size(); ++i) {
+      b += k[i] * batch[i].ds;
+      so += k[i] * batch[i].ss;
+    }
+    out->push_back({in.src + static_cast<uint64_t>(so), row_ss, t, static_cast<uint64_t>(b), static_cast<uint64_t>(r0),
+                    static_cast<uint64_t>(c0), static_cast<uint64_t>(er), static_cast<uint64_t>(ec), in.src_dtype, in.src_device});
+    size_t i = batch.size();
+    while (i > 0 && ++k[i - 1] == batch[i - 1].e) k[--i] = 0;
+    if (i == 0) break;
+  }
+  return TSB_OK;
+}
+
+}  // namespace
+
+int block_fp8_compile(int device, const tsb_rect_t* rects, uint64_t n, const tsb_bq_target_t* targets, uint64_t n_targets,
+                      BqTables* out) {
+  if ((n && !rects) || (n_targets && !targets)) return fail(TSB_ERR_INVALID, "block_fp8: NULL rects or targets");
+  // block index of every target's first block
+  std::vector<uint64_t> base(n_targets + 1, 0);
+  for (uint64_t t = 0; t < n_targets; ++t) {
+    const tsb_bq_target_t& T = targets[t];
+    const std::string where = "target " + std::to_string(t) + ": ";
+    if (!T.dst || !T.scale_inv) return fail(TSB_ERR_INVALID, where + "NULL dst or scale_inv");
+    if (!T.batch || !T.rows || !T.cols) return fail(TSB_ERR_INVALID, where + "empty target");
+    if (T.scale_inv % 4) return fail(TSB_ERR_INVALID, where + "scale_inv is not 4-byte aligned");
+    if (T.cols >= (1ull << 31) || T.rows >= (1ull << 31) || T.batch >= (1ull << 31) ||
+        T.batch * T.rows >= (1ull << 40) / T.cols)
+      return fail(TSB_ERR_INVALID, where + "target too large");
+    const uint64_t nbr = (T.rows + kBqBlock - 1) / kBqBlock, nbc = (T.cols + kBqBlock - 1) / kBqBlock;
+    base[t + 1] = base[t] + T.batch * nbr * nbc;
+    out->payload_bytes += T.batch * T.rows * T.cols + 4 * T.batch * nbr * nbc;
+  }
+  if (base[n_targets] >= (1ull << 31)) return fail(TSB_ERR_UNSUPPORTED, "block_fp8: more than 2^31 blocks");
+  std::vector<Box> boxes;
+  for (uint64_t i = 0; i < n; ++i) {
+    int st = rect_boxes(rects[i], i, targets, n_targets, &boxes);
+    if (st) return st;
+  }
+  struct Keyed {
+    uint64_t block;
+    uint32_t dtype;
+    BqPiece piece;
+  };
+  std::vector<Keyed> pieces;
+  for (const Box& x : boxes) {
+    const tsb_bq_target_t& T = targets[x.target];
+    const uint64_t nbr = (T.rows + kBqBlock - 1) / kBqBlock, nbc = (T.cols + kBqBlock - 1) / kBqBlock;
+    const uint32_t es = src_elem_bytes(x.dtype);
+    for (uint64_t br = x.r0 / kBqBlock; br <= (x.r0 + x.er - 1) / kBqBlock; ++br) {
+      const uint64_t pr0 = std::max<uint64_t>(x.r0, br * kBqBlock), pr1 = std::min<uint64_t>(x.r0 + x.er, (br + 1) * kBqBlock);
+      for (uint64_t bc = x.c0 / kBqBlock; bc <= (x.c0 + x.ec - 1) / kBqBlock; ++bc) {
+        const uint64_t pc0 = std::max<uint64_t>(x.c0, bc * kBqBlock), pc1 = std::min<uint64_t>(x.c0 + x.ec, (bc + 1) * kBqBlock);
+        BqPiece p;
+        memset(&p, 0, sizeof(p));
+        p.src = x.src + (pr0 - x.r0) * x.row_stride + (pc0 - x.c0) * es;
+        p.src_stride = x.row_stride;
+        p.row0 = static_cast<uint16_t>(pr0 - br * kBqBlock);
+        p.col0 = static_cast<uint16_t>(pc0 - bc * kBqBlock);
+        p.rows = static_cast<uint16_t>(pr1 - pr0);
+        p.cols = static_cast<uint16_t>(pc1 - pc0);
+        p.vec = (p.src % 16 == 0 && (p.rows == 1 || p.src_stride % 16 == 0) && (p.cols * es) % 16 == 0 && (p.col0 * es) % 16 == 0) ? 1u : 0u;
+        pieces.push_back({base[x.target] + (x.b * nbr + br) * nbc + bc, x.dtype, p});
+        const uint64_t bytes = static_cast<uint64_t>(p.rows) * p.cols * es;
+        out->src_bytes += bytes;
+        if (x.src_device >= 0 && x.src_device != device) out->remote_src_bytes += bytes;
+        out->max_src_bytes = std::max(out->max_src_bytes, es);
+      }
+    }
+  }
+  std::stable_sort(pieces.begin(), pieces.end(), [](const Keyed& a, const Keyed& b) { return a.block < b.block; });
+  out->blocks.resize(base[n_targets]);
+  out->pieces.resize(pieces.size());
+  size_t pi = 0;
+  uint64_t t = 0;
+  for (uint64_t blk = 0; blk < base[n_targets]; ++blk) {
+    while (blk >= base[t + 1]) ++t;
+    const tsb_bq_target_t& T = targets[t];
+    const uint64_t nbr = (T.rows + kBqBlock - 1) / kBqBlock, nbc = (T.cols + kBqBlock - 1) / kBqBlock;
+    const uint64_t local = blk - base[t], b = local / (nbr * nbc), br = (local / nbc) % nbr, bc = local % nbc;
+    const uint32_t rows = static_cast<uint32_t>(std::min<uint64_t>(kBqBlock, T.rows - br * kBqBlock));
+    const uint32_t cols = static_cast<uint32_t>(std::min<uint64_t>(kBqBlock, T.cols - bc * kBqBlock));
+    const size_t first = pi;
+    uint64_t area = 0;
+    while (pi < pieces.size() && pieces[pi].block == blk) {
+      area += static_cast<uint64_t>(pieces[pi].piece.rows) * pieces[pi].piece.cols;
+      out->pieces[pi] = pieces[pi].piece;
+      ++pi;
+    }
+    const std::string where = "target " + std::to_string(t) + " block (" + std::to_string(b) + ", " + std::to_string(br) + ", " +
+                              std::to_string(bc) + "): ";
+    if (area != static_cast<uint64_t>(rows) * cols)
+      return fail(TSB_ERR_INVALID, where + "its elements are not all written exactly once (" + std::to_string(area) + " of " +
+                                       std::to_string(rows * cols) + ")");
+    for (size_t i = first + 1; i < pi; ++i)
+      if (pieces[i].dtype != pieces[first].dtype) return fail(TSB_ERR_UNSUPPORTED, where + "sources of different dtypes");
+    if (pi - first > 1) {  // equal area: exact tiling unless two pieces overlap
+      uint64_t mask[kBqBlock][2] = {};
+      for (size_t i = first; i < pi; ++i) {
+        const BqPiece& p = out->pieces[i];
+        uint64_t m[2] = {0, 0};
+        for (uint32_t c = p.col0; c < static_cast<uint32_t>(p.col0) + p.cols; ++c) m[c >> 6] |= 1ull << (c & 63);
+        for (uint32_t r = p.row0; r < static_cast<uint32_t>(p.row0) + p.rows; ++r) {
+          if ((mask[r][0] & m[0]) | (mask[r][1] & m[1]))
+            return fail(TSB_ERR_INVALID, where + "its elements are not all written exactly once (overlap)");
+          mask[r][0] |= m[0];
+          mask[r][1] |= m[1];
+        }
+      }
+    }
+    BqBlock& o = out->blocks[blk];
+    memset(&o, 0, sizeof(o));
+    o.dst = T.dst + b * T.rows * T.cols + br * kBqBlock * T.cols + bc * kBqBlock;
+    o.scale = T.scale_inv + 4 * ((b * nbr + br) * nbc + bc);
+    o.pitch = static_cast<uint32_t>(T.cols);
+    o.rows = static_cast<uint16_t>(rows);
+    o.cols = static_cast<uint16_t>(cols);
+    o.piece0 = static_cast<uint32_t>(first);
+    o.n_pieces = static_cast<uint16_t>(pi - first);
+    o.src_dtype = static_cast<uint16_t>(pieces[first].dtype);
+  }
+  return TSB_OK;
+}
+
+namespace {
+
+__device__ __forceinline__ uint4 ldg16(const char* p) {
+  uint4 v;
+  asm volatile("ld.global.nc.L1::no_allocate.v4.u32 {%0,%1,%2,%3}, [%4];"
+               : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w)
+               : "l"(p));
+  return v;
+}
+
+__device__ __forceinline__ float f16_bits_to_f32(uint32_t bits16) {
+  const unsigned short b = static_cast<unsigned short>(bits16);
+  return __half2float(*reinterpret_cast<const __half*>(&b));
+}
+
+// Source dtypes: element size and the exact widening of one element's bits to f32 bits.
+template <uint32_t DT> struct Src;
+template <> struct Src<TSB_F32> {
+  static constexpr uint32_t kBytes = 4;
+  static __device__ __forceinline__ uint32_t f32(uint32_t bits) { return bits; }
+};
+template <> struct Src<TSB_BF16> {
+  static constexpr uint32_t kBytes = 2;
+  static __device__ __forceinline__ uint32_t f32(uint32_t bits) { return bits << 16; }
+};
+template <> struct Src<TSB_F16> {
+  static constexpr uint32_t kBytes = 2;
+  static __device__ __forceinline__ uint32_t f32(uint32_t bits) { return __float_as_uint(f16_bits_to_f32(bits)); }
+};
+
+// |x| as an integer: finite < Inf < NaN
+__device__ __forceinline__ uint32_t abs_bits(uint32_t f32_bits) { return f32_bits & 0x7fffffffu; }
+
+template <uint32_t DT>
+__device__ __forceinline__ uint32_t fold_word(uint32_t m, uint32_t w) {
+  if (Src<DT>::kBytes == 4) return max(m, abs_bits(w));
+  return max(m, max(abs_bits(Src<DT>::f32(w & 0xffffu)), abs_bits(Src<DT>::f32(w >> 16))));
+}
+
+// 4 loads in flight per thread and 6 CTAs per SM (40 registers; a bf16 stage is 32 KiB): measured faster
+// on H100 than 8 loads at 4 CTAs per SM (64 registers), see DESIGN.md section 6.
+constexpr int kUnroll = 4;
+
+// Phase 1: pieces -> shared memory (source dtype, block row pitch 128 elements); returns this
+// thread's max |x| bits.
+template <uint32_t DT>
+__device__ __forceinline__ uint32_t stage_block(const BqBlock& blk, const BqPiece* __restrict__ pieces, unsigned char* smem) {
+  constexpr uint32_t es = Src<DT>::kBytes;
+  constexpr uint32_t spitch = kBqBlock * es;
+  uint32_t m = 0;
+  for (uint32_t q = 0; q < blk.n_pieces; ++q) {
+    const BqPiece p = pieces[blk.piece0 + q];
+    const char* src = reinterpret_cast<const char*>(p.src);
+    unsigned char* s0 = smem + p.row0 * spitch + p.col0 * es;
+    if (p.vec) {
+      const uint32_t upr = p.cols * es / 16;  // 16-byte units per row
+      const uint32_t total = p.rows * upr;
+      for (uint32_t i = threadIdx.x; i < total; i += kBqThreads * kUnroll) {
+        uint4 v[kUnroll];
+#pragma unroll
+        for (int k = 0; k < kUnroll; ++k) {
+          const uint32_t idx = i + k * kBqThreads;
+          if (idx < total) {
+            const uint32_t r = idx / upr, c = idx - r * upr;
+            v[k] = ldg16(src + static_cast<int64_t>(r) * p.src_stride + c * 16);
+          }
+        }
+#pragma unroll
+        for (int k = 0; k < kUnroll; ++k) {
+          const uint32_t idx = i + k * kBqThreads;
+          if (idx < total) {
+            const uint32_t r = idx / upr, c = idx - r * upr;
+            m = fold_word<DT>(fold_word<DT>(fold_word<DT>(fold_word<DT>(m, v[k].x), v[k].y), v[k].z), v[k].w);
+            *reinterpret_cast<uint4*>(s0 + r * spitch + c * 16) = v[k];
+          }
+        }
+      }
+    } else {
+      const uint32_t total = static_cast<uint32_t>(p.rows) * p.cols;
+      for (uint32_t idx = threadIdx.x; idx < total; idx += kBqThreads) {
+        const uint32_t r = idx / p.cols, c = idx - r * p.cols;
+        const char* a = src + static_cast<int64_t>(r) * p.src_stride + c * es;
+        unsigned char* s = s0 + r * spitch + c * es;
+        if (es == 4) {
+          const uint32_t w = __ldg(reinterpret_cast<const uint32_t*>(a));
+          m = max(m, abs_bits(w));
+          *reinterpret_cast<uint32_t*>(s) = w;
+        } else {
+          const unsigned short h = __ldg(reinterpret_cast<const unsigned short*>(a));
+          m = max(m, abs_bits(Src<DT>::f32(h)));
+          *reinterpret_cast<unsigned short*>(s) = h;
+        }
+      }
+    }
+  }
+  return m;
+}
+
+// f32 bits of element j of a 16-element chunk starting at `s` (shared memory)
+template <uint32_t DT>
+__device__ __forceinline__ uint32_t elem(const unsigned char* s, uint32_t j) {
+  if (Src<DT>::kBytes == 4) return *reinterpret_cast<const uint32_t*>(s + 4 * j);
+  return Src<DT>::f32(*reinterpret_cast<const unsigned short*>(s + 2 * j));
+}
+
+// Phase 2: shared memory -> e4m3fn, 16 destination bytes per thread and step.
+template <uint32_t DT>
+__device__ __forceinline__ void quantise_block(const BqBlock& blk, const unsigned char* smem, float scale) {
+  constexpr uint32_t es = Src<DT>::kBytes;
+  constexpr uint32_t spitch = kBqBlock * es;
+  const uint32_t cpr = (blk.cols + 15u) / 16u;
+  const uint32_t total = blk.rows * cpr;
+  for (uint32_t idx = threadIdx.x; idx < total; idx += kBqThreads) {
+    const uint32_t r = idx / cpr, c = (idx - r * cpr) * 16u;
+    const unsigned char* s = smem + r * spitch + c * es;
+    char* d = reinterpret_cast<char*>(blk.dst) + static_cast<uint64_t>(r) * blk.pitch + c;
+    const uint32_t nvalid = min(16u, static_cast<uint32_t>(blk.cols) - c);
+    uint32_t f[16];
+    if (nvalid == 16) {
+#pragma unroll
+      for (uint32_t i = 0; i < es; ++i) {
+        const uint4 w = reinterpret_cast<const uint4*>(s)[i];
+        const uint32_t words[4] = {w.x, w.y, w.z, w.w};
+#pragma unroll
+        for (uint32_t k = 0; k < 4; ++k) {
+          if constexpr (es == 4) {
+            f[4 * i + k] = words[k];
+          } else {
+            f[8 * i + 2 * k] = Src<DT>::f32(words[k] & 0xffffu);
+            f[8 * i + 2 * k + 1] = Src<DT>::f32(words[k] >> 16);
+          }
+        }
+      }
+    } else {
+#pragma unroll
+      for (uint32_t j = 0; j < 16; ++j) f[j] = j < nvalid ? elem<DT>(s, j) : 0u;
+    }
+    uint32_t o[4];
+#pragma unroll
+    for (uint32_t q = 0; q < 4; ++q) {
+      uint32_t x[4];
+#pragma unroll
+      for (uint32_t j = 0; j < 4; ++j) x[j] = __float_as_uint(__fmul_rn(__uint_as_float(f[4 * q + j]), scale));
+      o[q] = f32x2_to_fp8x2<true>(x[0], x[1]) | (f32x2_to_fp8x2<true>(x[2], x[3]) << 16);
+    }
+    if (nvalid == 16 && (reinterpret_cast<uintptr_t>(d) & 15u) == 0) {
+      asm volatile("st.global.v4.u32 [%0], {%1,%2,%3,%4};" ::"l"(d), "r"(o[0]), "r"(o[1]), "r"(o[2]), "r"(o[3]) : "memory");
+    } else {
+#pragma unroll
+      for (uint32_t j = 0; j < 16; ++j)
+        if (j < nvalid) d[j] = static_cast<char>((o[j >> 2] >> (8 * (j & 3))) & 0xffu);
+    }
+  }
+}
+
+template <uint32_t DT>
+__device__ __forceinline__ void run_block(const BqBlock& blk, const BqPiece* pieces, unsigned char* smem, uint32_t* s_red,
+                                          float* s_scale) {
+  uint32_t m = stage_block<DT>(blk, pieces, smem);
+  m = __reduce_max_sync(0xffffffffu, m);
+  if ((threadIdx.x & 31u) == 0) s_red[threadIdx.x >> 5] = m;
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    uint32_t a = s_red[0];
+#pragma unroll
+    for (uint32_t w = 1; w < kBqThreads / 32; ++w) a = max(a, s_red[w]);
+    float amax_c, scale, scale_inv;
+    if (a > 0x7f800000u) {  // a NaN in the block: NaN scale, every output NaN
+      amax_c = __uint_as_float(0x7fffffffu);
+      scale = amax_c;
+      scale_inv = amax_c;
+    } else {
+      amax_c = fmaxf(__uint_as_float(a), 1e-4f);
+      scale = __fdiv_rn(448.0f, amax_c);
+      scale_inv = __fdiv_rn(amax_c, 448.0f);
+    }
+    *s_scale = scale;
+    *reinterpret_cast<float*>(blk.scale) = scale_inv;
+  }
+  __syncthreads();
+  quantise_block<DT>(blk, smem, *s_scale);
+}
+
+__global__ void __launch_bounds__(kBqThreads, 6) block_fp8_kernel(const BqBlock* __restrict__ blocks, const BqPiece* __restrict__ pieces) {
+  extern __shared__ __align__(16) unsigned char stage[];
+  __shared__ uint32_t s_red[kBqThreads / 32];
+  __shared__ float s_scale;
+  const BqBlock blk = blocks[blockIdx.x];
+  switch (blk.src_dtype) {
+    case TSB_BF16: run_block<TSB_BF16>(blk, pieces, stage, s_red, &s_scale); break;
+    case TSB_F16: run_block<TSB_F16>(blk, pieces, stage, s_red, &s_scale); break;
+    default: run_block<TSB_F32>(blk, pieces, stage, s_red, &s_scale); break;
+  }
+}
+
+cudaError_t prepare() {
+  // an f32 stage (64 KiB) exceeds the 48 KiB default; the attribute is per device (context)
+  static std::atomic<uint64_t> prepared{0};
+  int dev = 0;
+  cudaError_t e = cudaGetDevice(&dev);
+  if (e != cudaSuccess) return e;
+  const uint64_t bit = 1ull << (dev & 63);
+  if (prepared.load(std::memory_order_acquire) & bit) return cudaSuccess;
+  e = cudaFuncSetAttribute(block_fp8_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(kBqBlock * kBqBlock * 4));
+  if (e == cudaSuccess) prepared.fetch_or(bit, std::memory_order_release);
+  return e;
+}
+
+}  // namespace
+
+int launch_block_fp8(const BqBlock* blocks, const BqPiece* pieces, uint32_t n_blocks, uint32_t max_src_bytes, cudaStream_t stream) {
+  if (n_blocks == 0) return TSB_OK;
+  cudaError_t e = prepare();
+  if (e == cudaSuccess) {
+    block_fp8_kernel<<<n_blocks, kBqThreads, kBqBlock * kBqBlock * max_src_bytes, stream>>>(blocks, pieces);
+    e = cudaGetLastError();
+  }
+  if (e != cudaSuccess) return cuda_fail(e, "block_fp8_kernel launch");
+  count_launch();
+  return TSB_OK;
+}
+
+}  // namespace tsb
+
+using namespace tsb;
+
+extern "C" int tsb_block_fp8_compile_host(int device, const tsb_rect_t* rects, uint64_t n, const tsb_bq_target_t* targets,
+                                          uint64_t n_targets, uint32_t flags, void* out_blocks, uint64_t block_cap,
+                                          uint64_t* out_n_blocks, void* out_pieces, uint64_t piece_cap, uint64_t* out_n_pieces) {
+  if (flags != 0) return fail(TSB_ERR_INVALID, "tsb_block_fp8_compile_host: flags must be 0");
+  BqTables tb;
+  int st = block_fp8_compile(device, rects, n, targets, n_targets, &tb);
+  if (st) return st;
+  if (out_n_blocks) *out_n_blocks = tb.blocks.size();
+  if (out_n_pieces) *out_n_pieces = tb.pieces.size();
+  if (out_blocks) {
+    if (tb.blocks.size() > block_cap) return fail(TSB_ERR_NOMEM, "out_blocks too small");
+    if (!tb.blocks.empty()) memcpy(out_blocks, tb.blocks.data(), tb.blocks.size() * sizeof(BqBlock));
+  }
+  if (out_pieces) {
+    if (tb.pieces.size() > piece_cap) return fail(TSB_ERR_NOMEM, "out_pieces too small");
+    if (!tb.pieces.empty()) memcpy(out_pieces, tb.pieces.data(), tb.pieces.size() * sizeof(BqPiece));
+  }
+  return TSB_OK;
+}

@@ -40,13 +40,20 @@ TableLayout table_layout(size_t n_rects, size_t n_tiles, size_t n_link) {
   return l;
 }
 
+// What a plan's tables drive: the copy_rects kernel, or the block-scaled fp8 quantiser
+// (d_block = {BqBlock table | BqPiece table}, num_tiles = blocks).
+enum : uint32_t { PLAN_COPY = 0, PLAN_BLOCK_FP8 = 1 };
+
 struct Plan {
   int device = 0;
+  uint32_t plan_kind = PLAN_COPY;
   char* d_block = nullptr;
   TableLayout layout;
   uint32_t num_tiles = 0;
   uint32_t num_link_tiles = 0;
   uint32_t kind = KIND_GENERIC;
+  size_t bq_pieces_off = 0;    // PLAN_BLOCK_FP8: byte offset of the piece table in d_block
+  uint32_t bq_src_bytes = 2;   // PLAN_BLOCK_FP8: largest source element size
   uint32_t link_stage_bytes = 0;
   uint32_t link_stages = 0;
   tsb_plan_info_t info{};
@@ -547,11 +554,49 @@ int find_plan(tsb_plan_t plan, Plan** out) {
 }
 
 int run_plan(Plan* p, cudaStream_t s) {
+  if (p->plan_kind == PLAN_BLOCK_FP8)
+    return launch_block_fp8(reinterpret_cast<const BqBlock*>(p->d_block), reinterpret_cast<const BqPiece*>(p->d_block + p->bq_pieces_off),
+                            p->num_tiles, p->bq_src_bytes, s);
   uint32_t kind = p->kind;
   if (getenv("TSB_FORCE_GENERIC")) kind = KIND_GENERIC;
   LaunchParams lp = make_params(p->d_block, p->layout, p->num_tiles, p->num_link_tiles, kind, p->link_stage_bytes, p->link_stages);
   if (getenv("TSB_STATIC_SCHED") && p->num_link_tiles == 0) lp.sched = nullptr;
   return launch_copy_rects(lp, p->info.grid, s);
+}
+
+// Upload a plan's serialised tables, create its launch events and register it; frees `p` on failure.
+int register_plan(Plan* p, const std::vector<char>& host, tsb_plan_t* out) {
+  int st;
+  {
+    // upload on the device's copy stream and wait for it: after this returns the tables are in
+    // HBM whatever stream the plan is later run on
+    cudaStream_t up;
+    if ((st = copy_stream(p->device, &up))) {
+      delete p;
+      return st;
+    }
+    DeviceGuard guard(p->device);
+    if (!guard.ok) { delete p; return cuda_fail(guard.err, "cudaSetDevice"); }
+    cudaError_t e = cudaMalloc(&p->d_block, host.size());
+    if (e == cudaSuccess) e = cudaMemcpyAsync(p->d_block, host.data(), host.size(), cudaMemcpyHostToDevice, up);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(up);
+    // the events of tsb_plan_launch belong to the plan and exist from the start (no lazy creation that
+    // two threads launching the same plan could race on)
+    if (e == cudaSuccess) e = cudaEventCreateWithFlags(&p->ev_fence, cudaEventDisableTiming);
+    if (e == cudaSuccess) e = cudaEventCreate(&p->ev_start);
+    if (e == cudaSuccess) e = cudaEventCreate(&p->ev_done);
+    if (e != cudaSuccess) {
+      cuda_fail(e, "plan upload");
+      free_plan(p);
+      return TSB_ERR_CUDA;
+    }
+  }
+  PlanRegistry& reg = R();
+  std::lock_guard<std::mutex> lk(reg.mu);
+  uint64_t id = reg.next_id++;
+  reg.plans[id] = p;
+  *out = id;
+  return TSB_OK;
 }
 
 }  // namespace
@@ -635,38 +680,36 @@ int tsb_plan_create(int device, const tsb_rect_t* rects, uint64_t n, uint32_t fl
     return st;
   }
   p->layout = table_layout(cp.c.rects.size(), cp.tiles.size(), cp.link_tiles.size());
-  {
-    // upload on the device's copy stream and wait for it: after this returns the tables are in
-    // HBM whatever stream the plan is later run on
-    cudaStream_t up;
-    if ((st = copy_stream(device, &up))) {
-      delete p;
-      return st;
-    }
-    DeviceGuard guard(device);
-    if (!guard.ok) { delete p; return cuda_fail(guard.err, "cudaSetDevice"); }
-    std::vector<char> host(p->layout.total);
-    fill_block(host.data(), p->layout, cp);
-    cudaError_t e = cudaMalloc(&p->d_block, p->layout.total);
-    if (e == cudaSuccess) e = cudaMemcpyAsync(p->d_block, host.data(), p->layout.total, cudaMemcpyHostToDevice, up);
-    if (e == cudaSuccess) e = cudaStreamSynchronize(up);
-    // the events of tsb_plan_launch belong to the plan and exist from the start (no lazy creation that
-    // two threads launching the same plan could race on)
-    if (e == cudaSuccess) e = cudaEventCreateWithFlags(&p->ev_fence, cudaEventDisableTiming);
-    if (e == cudaSuccess) e = cudaEventCreate(&p->ev_start);
-    if (e == cudaSuccess) e = cudaEventCreate(&p->ev_done);
-    if (e != cudaSuccess) {
-      cuda_fail(e, "plan upload");
-      free_plan(p);
-      return TSB_ERR_CUDA;
-    }
-  }
-  PlanRegistry& reg = R();
-  std::lock_guard<std::mutex> lk(reg.mu);
-  uint64_t id = reg.next_id++;
-  reg.plans[id] = p;
-  *out = id;
-  return TSB_OK;
+  std::vector<char> host(p->layout.total);
+  fill_block(host.data(), p->layout, cp);
+  return register_plan(p, host, out);
+}
+
+int tsb_block_fp8_plan_create(int device, const tsb_rect_t* rects, uint64_t n, const tsb_bq_target_t* targets,
+                              uint64_t n_targets, uint32_t flags, tsb_plan_t* out) {
+  if (!out) return fail(TSB_ERR_INVALID, "tsb_block_fp8_plan_create: NULL argument");
+  if (flags != 0) return fail(TSB_ERR_INVALID, "tsb_block_fp8_plan_create: flags must be 0");
+  BqTables tb;
+  int st = block_fp8_compile(device, rects, n, targets, n_targets, &tb);
+  if (st) return st;
+  Plan* p = new Plan();
+  p->device = device;
+  p->plan_kind = PLAN_BLOCK_FP8;
+  p->num_tiles = static_cast<uint32_t>(tb.blocks.size());
+  p->bq_src_bytes = tb.max_src_bytes;
+  p->bq_pieces_off = tb.blocks.size() * sizeof(BqBlock);
+  p->info.num_rects = n;
+  p->info.num_tiles = tb.blocks.size();
+  p->info.payload_bytes = tb.payload_bytes;
+  p->info.src_bytes = tb.src_bytes;
+  p->info.remote_src_bytes = tb.remote_src_bytes;
+  p->info.grid = static_cast<uint32_t>(tb.blocks.size());
+  p->info.block = kBqThreads;
+  p->info.tile_bytes = kBqBlock * kBqBlock;
+  std::vector<char> host(std::max<size_t>(16, p->bq_pieces_off + tb.pieces.size() * sizeof(BqPiece)));
+  if (!tb.blocks.empty()) memcpy(host.data(), tb.blocks.data(), p->bq_pieces_off);
+  if (!tb.pieces.empty()) memcpy(host.data() + p->bq_pieces_off, tb.pieces.data(), tb.pieces.size() * sizeof(BqPiece));
+  return register_plan(p, host, out);
 }
 
 int tsb_plan_info(tsb_plan_t plan, tsb_plan_info_t* out) {

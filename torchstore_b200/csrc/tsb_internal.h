@@ -5,6 +5,7 @@
 #include <stdint.h>
 
 #include <string>
+#include <vector>
 
 #include "tstore_b200.h"
 
@@ -157,5 +158,43 @@ constexpr uint32_t kLinkBatch = 8;  // link tiles claimed per atomic
 int launch_copy_rects(const LaunchParams& p, uint32_t grid, cudaStream_t stream);
 void count_launch();
 int max_ctas_per_sm(uint32_t kind, bool with_link, uint32_t link_smem_bytes, int* out);
+
+// ---- block-scaled fp8 (block_fp8.cu) ---------------------------------------------------------------
+constexpr uint32_t kBqBlock = 128;  // block edge (elements)
+constexpr uint32_t kBqThreads = 256;
+
+// One 128x128 (or partial edge) block of a target: CTA-sized unit of work.
+struct alignas(16) BqBlock {
+  uint64_t dst;          // fp8 element (0, 0) of the block
+  uint64_t scale;        // its float32 scale_inv
+  uint32_t pitch;        // destination row pitch (bytes == elements)
+  uint16_t rows, cols;   // real extent of the block
+  uint32_t piece0;       // first piece
+  uint16_t n_pieces;
+  uint16_t src_dtype;    // TSB_F32 / TSB_BF16 / TSB_F16, the same for every piece of the block
+};
+static_assert(sizeof(BqBlock) == 32, "BqBlock is part of tsb_block_fp8_compile_host's output");
+
+// A source rectangle inside one block.
+struct alignas(16) BqPiece {
+  uint64_t src;          // source element (row0, col0) of the piece
+  int64_t src_stride;    // bytes between source rows
+  uint16_t row0, col0;   // position inside the block
+  uint16_t rows, cols;
+  uint32_t vec;          // 1: source address, stride, column offset and width allow 16-byte accesses
+  uint32_t pad_;
+};
+static_assert(sizeof(BqPiece) == 32, "BqPiece is part of tsb_block_fp8_compile_host's output");
+
+struct BqTables {
+  std::vector<BqBlock> blocks;
+  std::vector<BqPiece> pieces;
+  uint32_t max_src_bytes = 2;  // largest source element size: sizes the shared-memory stage
+  uint64_t src_bytes = 0, remote_src_bytes = 0, payload_bytes = 0;
+};
+int block_fp8_compile(int device, const tsb_rect_t* rects, uint64_t n, const tsb_bq_target_t* targets, uint64_t n_targets,
+                      BqTables* out);
+int launch_block_fp8(const BqBlock* blocks, const BqPiece* pieces, uint32_t n_blocks, uint32_t max_src_bytes,
+                     cudaStream_t stream);
 
 }  // namespace tsb

@@ -91,6 +91,22 @@ class Plans(dict):
             raise
         return plans
 
+    @classmethod
+    def build_block_fp8(cls, per_device: dict[int, tuple[list, list]]) -> "Plans":
+        """Compile block-scaled fp8 pulls: ``{device: ([(src, dst) StridedMem windows], [BqTarget])}``."""
+        plans = cls()
+        try:
+            for dev, (pairs, targets) in per_device.items():
+                rects, n = build_rects(pairs)
+                arr = _native.make_target_array(max(1, len(targets)))
+                for i, t in enumerate(targets):
+                    arr[i] = t
+                plans[dev] = _native.block_fp8_plan_create(dev, rects, n, arr, len(targets))
+        except BaseException:
+            plans.close()
+            raise
+        return plans
+
     def launch(self, fence_out: bool = True) -> None:
         """Enqueue every plan on its device's copy stream, fenced in against the caller's current
         stream of that device.  ``fence_out=False``: the caller's stream is not made to wait for the
