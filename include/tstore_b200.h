@@ -26,7 +26,7 @@
 extern "C" {
 #endif
 
-#define TSB_ABI_VERSION 4
+#define TSB_ABI_VERSION 5
 #define TSB_MAX_DIMS 6
 
 enum {
@@ -237,6 +237,51 @@ int tsb_block_fp8_plan_create(int device, const tsb_rect_t* rects, uint64_t n, c
 int tsb_block_fp8_compile_host(int device, const tsb_rect_t* rects, uint64_t n, const tsb_bq_target_t* targets,
                                uint64_t n_targets, uint32_t flags, void* out_blocks, uint64_t block_cap,
                                uint64_t* out_n_blocks, void* out_pieces, uint64_t piece_cap, uint64_t* out_n_pieces);
+
+/* ------------------------------------------------------------------------------------------ */
+/* per-channel / per-tensor scaled FP8 destinations (compressed-tensors FP8, fbgemm-fp8, vLLM  */
+/* quantization="fp8"): the pull quantises while it gathers                                     */
+/* ------------------------------------------------------------------------------------------ */
+
+enum { TSB_SCALE_PER_CHANNEL = 1, TSB_SCALE_PER_TENSOR = 2 };
+
+/* One scaled destination: `batch` independent [rows, cols] matrices.  A group is one row
+ * (TSB_SCALE_PER_CHANNEL; scale_inv is float32 [batch, rows]) or one whole matrix
+ * (TSB_SCALE_PER_TENSOR; scale_inv is float32 [batch]).  Per group:
+ *   amax = max |x| over the group (NaN if any x is NaN); amax_c = max(amax, 1e-4f) (NaN stays NaN)
+ *   dst = e4m3fn(rn(x * (448 / amax_c)))  with torch's .to(float8_e4m3fn) rounding;  scale_inv = amax_c / 448
+ * with correctly rounded f32 divisions and multiply, x widened exactly to f32. */
+typedef struct tsb_sq_target {
+  uint64_t dst;       /* float8_e4m3fn, contiguous [batch, rows, cols] */
+  uint64_t scale_inv; /* float32, contiguous, one per group */
+  uint64_t batch, rows, cols;
+  uint32_t granularity; /* TSB_SCALE_PER_CHANNEL or TSB_SCALE_PER_TENSOR */
+  uint32_t pad;         /* 0 */
+} tsb_sq_target_t;
+
+/* Compile a scaled pull: rects as for tsb_block_fp8_plan_create; every element of every target must
+ * be written by exactly one rect, and every group read from one source dtype (TSB_ERR_INVALID
+ * naming the target and group otherwise).  A per-channel row of at most 32 KiB of source bytes is
+ * quantised from shared memory after one read; per-tensor groups and longer rows take two passes
+ * (amax, then quantise), reading the source twice.  The result is a plan like any other.
+ * flags: reserved, pass 0. */
+int tsb_scaled_fp8_plan_create(int device, const tsb_rect_t* rects, uint64_t n, const tsb_sq_target_t* targets,
+                               uint64_t n_targets, uint32_t flags, tsb_plan_t* out);
+/* Host-only (no CUDA call): compile and copy the kernel tables out.  A NULL table only reports its count.
+ * out_bands (row-staged path, one CTA each): records of 40 bytes
+ *   {u64 dst, u64 scale_inv_of_row0, u32 cols, u32 rows, u32 first_piece, u32 n_pieces, u32 src_dtype, u32 pad}
+ * out_pieces: records of 40 bytes
+ *   {u64 src, i64 src_row_stride_bytes, u32 row0, u32 col0, u32 rows, u32 cols, u32 vector, u32 pad}
+ *   (row0/col0 relative to the band; vector: 16-byte loads)
+ * out_tiles (two-pass path, one CTA per pass each): records of 56 bytes, sorted by group
+ *   {u64 src, i64 src_row_stride_bytes, u64 dst, u64 scale_inv_or_0, u32 dst_pitch, u32 rows, u32 cols,
+ *    u32 group, u32 src_dtype, u32 vector}
+ *   (scale_inv_or_0: non-zero in exactly one tile per group, the one that writes its scale)
+ * out_n_groups: the number of two-pass groups (amax words). */
+int tsb_scaled_fp8_compile_host(int device, const tsb_rect_t* rects, uint64_t n, const tsb_sq_target_t* targets,
+                                uint64_t n_targets, uint32_t flags, void* out_bands, uint64_t band_cap,
+                                uint64_t* out_n_bands, void* out_pieces, uint64_t piece_cap, uint64_t* out_n_pieces,
+                                void* out_tiles, uint64_t tile_cap, uint64_t* out_n_tiles, uint64_t* out_n_groups);
 
 /* ------------------------------------------------------------------------------------------ */
 /* streams and events (the await points of the reference's coroutines)                         */

@@ -16,7 +16,7 @@ import torch
 from torchstore_b200._build import LIB_PATH
 
 TSB_MAX_DIMS = 6
-TSB_ABI_VERSION = 4
+TSB_ABI_VERSION = 5
 
 TSB_OK, TSB_ERR_INVALID, TSB_ERR_CUDA, TSB_ERR_UNSUPPORTED, TSB_ERR_NOMEM, TSB_ERR_NOTFOUND = range(6)
 
@@ -96,6 +96,23 @@ class BqTarget(C.Structure):
     ]
 
 
+TSB_SCALE_PER_CHANNEL, TSB_SCALE_PER_TENSOR = 1, 2
+
+
+class SqTarget(C.Structure):
+    """tsb_sq_target_t: one per-channel or per-tensor scaled fp8 destination."""
+
+    _fields_ = [
+        ("dst", C.c_uint64),
+        ("scale_inv", C.c_uint64),
+        ("batch", C.c_uint64),
+        ("rows", C.c_uint64),
+        ("cols", C.c_uint64),
+        ("granularity", C.c_uint32),
+        ("pad", C.c_uint32),
+    ]
+
+
 class ArenaStats(C.Structure):
     _fields_ = [
         ("capacity", C.c_uint64),
@@ -145,6 +162,15 @@ _SIGNATURES = {
         C.c_int,
         [C.c_int, C.POINTER(Rect), C.c_uint64, C.POINTER(BqTarget), C.c_uint64, C.c_uint32, _vp, C.c_uint64,
          C.POINTER(C.c_uint64), _vp, C.c_uint64, C.POINTER(C.c_uint64)],
+    ),
+    "tsb_scaled_fp8_plan_create": (
+        C.c_int, [C.c_int, C.POINTER(Rect), C.c_uint64, C.POINTER(SqTarget), C.c_uint64, C.c_uint32, C.POINTER(C.c_uint64)],
+    ),
+    "tsb_scaled_fp8_compile_host": (
+        C.c_int,
+        [C.c_int, C.POINTER(Rect), C.c_uint64, C.POINTER(SqTarget), C.c_uint64, C.c_uint32, _vp, C.c_uint64,
+         C.POINTER(C.c_uint64), _vp, C.c_uint64, C.POINTER(C.c_uint64), _vp, C.c_uint64, C.POINTER(C.c_uint64),
+         C.POINTER(C.c_uint64)],
     ),
     "tsb_stream_create": (C.c_int, [C.c_int, C.POINTER(_vp)]),
     "tsb_stream_destroy": (C.c_int, [_vp]),
@@ -421,6 +447,43 @@ def block_fp8_compile_host(device: int, rects, n: int, targets, n_targets: int):
     check(L.tsb_block_fp8_compile_host(device, rects, n, targets, n_targets, 0, blocks.ctypes.data, nb.value,
                                        C.byref(nb), pieces.ctypes.data, npc.value, C.byref(npc)))
     return blocks[: nb.value], pieces[: npc.value]
+
+
+def make_sq_target_array(n: int):
+    return (SqTarget * n)()
+
+
+def scaled_fp8_plan_create(device: int, rects, n: int, targets, n_targets: int) -> int:
+    out = C.c_uint64(0)
+    check(lib().tsb_scaled_fp8_plan_create(device, rects, n, targets, n_targets, 0, C.byref(out)))
+    return int(out.value)
+
+
+# record layouts of tsb_scaled_fp8_compile_host (include/tstore_b200.h)
+SQ_BAND_DTYPE = [("dst", "<u8"), ("scale_inv", "<u8"), ("cols", "<u4"), ("rows", "<u4"), ("piece0", "<u4"),
+                 ("n_pieces", "<u4"), ("src_dtype", "<u4"), ("pad", "<u4")]
+SQ_PIECE_DTYPE = [("src", "<u8"), ("src_stride", "<i8"), ("row0", "<u4"), ("col0", "<u4"), ("rows", "<u4"),
+                  ("cols", "<u4"), ("vec", "<u4"), ("pad", "<u4")]
+SQ_TILE_DTYPE = [("src", "<u8"), ("src_stride", "<i8"), ("dst", "<u8"), ("scale_inv", "<u8"), ("pitch", "<u4"),
+                 ("rows", "<u4"), ("cols", "<u4"), ("group", "<u4"), ("src_dtype", "<u4"), ("vec", "<u4")]
+
+
+def scaled_fp8_compile_host(device: int, rects, n: int, targets, n_targets: int):
+    """Host-only compilation of a per-channel / per-tensor scaled fp8 pull -> (bands, pieces, tiles,
+    n_groups): numpy record arrays and the number of two-pass groups."""
+    import numpy as np
+
+    nb, npc, nt, ng = C.c_uint64(0), C.c_uint64(0), C.c_uint64(0), C.c_uint64(0)
+    L = lib()
+    check(L.tsb_scaled_fp8_compile_host(device, rects, n, targets, n_targets, 0, None, 0, C.byref(nb), None, 0,
+                                        C.byref(npc), None, 0, C.byref(nt), C.byref(ng)))
+    bands = np.zeros(max(1, nb.value), dtype=SQ_BAND_DTYPE)
+    pieces = np.zeros(max(1, npc.value), dtype=SQ_PIECE_DTYPE)
+    tiles = np.zeros(max(1, nt.value), dtype=SQ_TILE_DTYPE)
+    check(L.tsb_scaled_fp8_compile_host(device, rects, n, targets, n_targets, 0, bands.ctypes.data, nb.value,
+                                        C.byref(nb), pieces.ctypes.data, npc.value, C.byref(npc), tiles.ctypes.data,
+                                        nt.value, C.byref(nt), C.byref(ng)))
+    return bands[: nb.value], pieces[: npc.value], tiles[: nt.value], int(ng.value)
 
 
 CUDA_STREAM_LEGACY = 0x1  # cudaStreamLegacy: an explicit handle for the default stream

@@ -16,20 +16,16 @@
 //   phase 2  shared -> e4m3fn: x * scale (__fmul_rn), torch-exact narrowing (fp8_cvt.cuh), 16
 //            destination bytes per thread and step (one STG.128 when aligned, byte stores at ragged edges).
 
-#include <cuda_fp16.h>
-
 #include <algorithm>
 #include <atomic>
 #include <cstring>
 
-#include "fp8_cvt.cuh"
+#include "fp8_quant.cuh"
 #include "tsb_internal.h"
 
 namespace tsb {
 
-namespace {
-
-uint32_t src_elem_bytes(uint32_t dt) {
+uint32_t quant_src_bytes(uint32_t dt) {
   switch (dt) {
     case TSB_F32: return 4;
     case TSB_BF16: case TSB_F16: return 2;
@@ -37,26 +33,21 @@ uint32_t src_elem_bytes(uint32_t dt) {
   }
 }
 
-// A rect after mapping onto its target: a [er, ec] box at (b, r0, c0).
-struct Box {
-  uint64_t src;
-  int64_t row_stride;  // source bytes between rows (0 for a single row)
-  uint64_t target, b, r0, c0, er, ec;
-  uint32_t dtype;
-  int32_t src_device;
-};
+namespace {
 
 struct Dim {
   int64_t e, ss, ds;
 };
 
-int rect_boxes(const tsb_rect_t& in, uint64_t index, const tsb_bq_target_t* targets, uint64_t n_targets,
-               std::vector<Box>* out) {
+}  // namespace
+
+int rect_boxes(const tsb_rect_t& in, uint64_t index, const TargetGeom* targets, uint64_t n_targets,
+               std::vector<TargetBox>* out) {
   const std::string where = "rect " + std::to_string(index) + ": ";
   if (in.ndim < 1 || in.ndim > TSB_MAX_DIMS) return fail(TSB_ERR_INVALID, where + "ndim must be in [1, 6]");
-  const uint32_t es = src_elem_bytes(in.src_dtype);
-  if (!es) return fail(TSB_ERR_UNSUPPORTED, where + "block-scaled fp8 reads f32, bf16 or f16 sources");
-  if (in.dst_dtype != TSB_F8E4M3) return fail(TSB_ERR_UNSUPPORTED, where + "block-scaled destinations are float8_e4m3fn");
+  const uint32_t es = quant_src_bytes(in.src_dtype);
+  if (!es) return fail(TSB_ERR_UNSUPPORTED, where + "scaled fp8 pulls read f32, bf16 or f16 sources");
+  if (in.dst_dtype != TSB_F8E4M3) return fail(TSB_ERR_UNSUPPORTED, where + "scaled fp8 destinations are float8_e4m3fn");
   std::vector<Dim> work;
   for (uint32_t i = 0; i < in.ndim; ++i) {
     if (in.extent[i] < 0) return fail(TSB_ERR_INVALID, where + "negative extent");
@@ -114,7 +105,7 @@ int rect_boxes(const tsb_rect_t& in, uint64_t index, const tsb_bq_target_t* targ
   for (const Dim& d : batch) b_last += (d.e - 1) * d.ds;
   if (b_last >= B) return fail(TSB_ERR_INVALID, bad);
   if (have_col && col_ss != static_cast<int64_t>(es))
-    return fail(TSB_ERR_UNSUPPORTED, where + "block-scaled pulls read contiguous source rows");
+    return fail(TSB_ERR_UNSUPPORTED, where + "scaled fp8 pulls read contiguous source rows");
   if (in.src % es || row_ss % es) return fail(TSB_ERR_INVALID, where + "source not aligned to its element size");
   for (const Dim& d : batch)
     if (d.ss % es) return fail(TSB_ERR_INVALID, where + "source not aligned to its element size");
@@ -135,8 +126,6 @@ int rect_boxes(const tsb_rect_t& in, uint64_t index, const tsb_bq_target_t* targ
   return TSB_OK;
 }
 
-}  // namespace
-
 int block_fp8_compile(int device, const tsb_rect_t* rects, uint64_t n, const tsb_bq_target_t* targets, uint64_t n_targets,
                       BqTables* out) {
   if ((n && !rects) || (n_targets && !targets)) return fail(TSB_ERR_INVALID, "block_fp8: NULL rects or targets");
@@ -156,9 +145,11 @@ int block_fp8_compile(int device, const tsb_rect_t* rects, uint64_t n, const tsb
     out->payload_bytes += T.batch * T.rows * T.cols + 4 * T.batch * nbr * nbc;
   }
   if (base[n_targets] >= (1ull << 31)) return fail(TSB_ERR_UNSUPPORTED, "block_fp8: more than 2^31 blocks");
-  std::vector<Box> boxes;
+  std::vector<TargetGeom> geom(n_targets);
+  for (uint64_t t = 0; t < n_targets; ++t) geom[t] = {targets[t].dst, targets[t].batch, targets[t].rows, targets[t].cols};
+  std::vector<TargetBox> boxes;
   for (uint64_t i = 0; i < n; ++i) {
-    int st = rect_boxes(rects[i], i, targets, n_targets, &boxes);
+    int st = rect_boxes(rects[i], i, geom.data(), n_targets, &boxes);
     if (st) return st;
   }
   struct Keyed {
@@ -167,10 +158,10 @@ int block_fp8_compile(int device, const tsb_rect_t* rects, uint64_t n, const tsb
     BqPiece piece;
   };
   std::vector<Keyed> pieces;
-  for (const Box& x : boxes) {
+  for (const TargetBox& x : boxes) {
     const tsb_bq_target_t& T = targets[x.target];
     const uint64_t nbr = (T.rows + kBqBlock - 1) / kBqBlock, nbc = (T.cols + kBqBlock - 1) / kBqBlock;
-    const uint32_t es = src_elem_bytes(x.dtype);
+    const uint32_t es = quant_src_bytes(x.dtype);
     for (uint64_t br = x.r0 / kBqBlock; br <= (x.r0 + x.er - 1) / kBqBlock; ++br) {
       const uint64_t pr0 = std::max<uint64_t>(x.r0, br * kBqBlock), pr1 = std::min<uint64_t>(x.r0 + x.er, (br + 1) * kBqBlock);
       for (uint64_t bc = x.c0 / kBqBlock; bc <= (x.c0 + x.ec - 1) / kBqBlock; ++bc) {
@@ -248,43 +239,6 @@ int block_fp8_compile(int device, const tsb_rect_t* rects, uint64_t n, const tsb
 
 namespace {
 
-__device__ __forceinline__ uint4 ldg16(const char* p) {
-  uint4 v;
-  asm volatile("ld.global.nc.L1::no_allocate.v4.u32 {%0,%1,%2,%3}, [%4];"
-               : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w)
-               : "l"(p));
-  return v;
-}
-
-__device__ __forceinline__ float f16_bits_to_f32(uint32_t bits16) {
-  const unsigned short b = static_cast<unsigned short>(bits16);
-  return __half2float(*reinterpret_cast<const __half*>(&b));
-}
-
-// Source dtypes: element size and the exact widening of one element's bits to f32 bits.
-template <uint32_t DT> struct Src;
-template <> struct Src<TSB_F32> {
-  static constexpr uint32_t kBytes = 4;
-  static __device__ __forceinline__ uint32_t f32(uint32_t bits) { return bits; }
-};
-template <> struct Src<TSB_BF16> {
-  static constexpr uint32_t kBytes = 2;
-  static __device__ __forceinline__ uint32_t f32(uint32_t bits) { return bits << 16; }
-};
-template <> struct Src<TSB_F16> {
-  static constexpr uint32_t kBytes = 2;
-  static __device__ __forceinline__ uint32_t f32(uint32_t bits) { return __float_as_uint(f16_bits_to_f32(bits)); }
-};
-
-// |x| as an integer: finite < Inf < NaN
-__device__ __forceinline__ uint32_t abs_bits(uint32_t f32_bits) { return f32_bits & 0x7fffffffu; }
-
-template <uint32_t DT>
-__device__ __forceinline__ uint32_t fold_word(uint32_t m, uint32_t w) {
-  if (Src<DT>::kBytes == 4) return max(m, abs_bits(w));
-  return max(m, max(abs_bits(Src<DT>::f32(w & 0xffffu)), abs_bits(Src<DT>::f32(w >> 16))));
-}
-
 // 4 loads in flight per thread and 6 CTAs per SM (40 registers; a bf16 stage is 32 KiB): measured faster
 // on H100 than 8 loads at 4 CTAs per SM (64 registers), see DESIGN.md section 6.
 constexpr int kUnroll = 4;
@@ -318,7 +272,7 @@ __device__ __forceinline__ uint32_t stage_block(const BqBlock& blk, const BqPiec
           const uint32_t idx = i + k * kBqThreads;
           if (idx < total) {
             const uint32_t r = idx / upr, c = idx - r * upr;
-            m = fold_word<DT>(fold_word<DT>(fold_word<DT>(fold_word<DT>(m, v[k].x), v[k].y), v[k].z), v[k].w);
+            m = fold16<DT>(m, v[k]);
             *reinterpret_cast<uint4*>(s0 + r * spitch + c * 16) = v[k];
           }
         }
@@ -344,13 +298,6 @@ __device__ __forceinline__ uint32_t stage_block(const BqBlock& blk, const BqPiec
   return m;
 }
 
-// f32 bits of element j of a 16-element chunk starting at `s` (shared memory)
-template <uint32_t DT>
-__device__ __forceinline__ uint32_t elem(const unsigned char* s, uint32_t j) {
-  if (Src<DT>::kBytes == 4) return *reinterpret_cast<const uint32_t*>(s + 4 * j);
-  return Src<DT>::f32(*reinterpret_cast<const unsigned short*>(s + 2 * j));
-}
-
 // Phase 2: shared memory -> e4m3fn, 16 destination bytes per thread and step.
 template <uint32_t DT>
 __device__ __forceinline__ void quantise_block(const BqBlock& blk, const unsigned char* smem, float scale) {
@@ -363,41 +310,10 @@ __device__ __forceinline__ void quantise_block(const BqBlock& blk, const unsigne
     const unsigned char* s = smem + r * spitch + c * es;
     char* d = reinterpret_cast<char*>(blk.dst) + static_cast<uint64_t>(r) * blk.pitch + c;
     const uint32_t nvalid = min(16u, static_cast<uint32_t>(blk.cols) - c);
-    uint32_t f[16];
-    if (nvalid == 16) {
-#pragma unroll
-      for (uint32_t i = 0; i < es; ++i) {
-        const uint4 w = reinterpret_cast<const uint4*>(s)[i];
-        const uint32_t words[4] = {w.x, w.y, w.z, w.w};
-#pragma unroll
-        for (uint32_t k = 0; k < 4; ++k) {
-          if constexpr (es == 4) {
-            f[4 * i + k] = words[k];
-          } else {
-            f[8 * i + 2 * k] = Src<DT>::f32(words[k] & 0xffffu);
-            f[8 * i + 2 * k + 1] = Src<DT>::f32(words[k] >> 16);
-          }
-        }
-      }
-    } else {
-#pragma unroll
-      for (uint32_t j = 0; j < 16; ++j) f[j] = j < nvalid ? elem<DT>(s, j) : 0u;
-    }
-    uint32_t o[4];
-#pragma unroll
-    for (uint32_t q = 0; q < 4; ++q) {
-      uint32_t x[4];
-#pragma unroll
-      for (uint32_t j = 0; j < 4; ++j) x[j] = __float_as_uint(__fmul_rn(__uint_as_float(f[4 * q + j]), scale));
-      o[q] = f32x2_to_fp8x2<true>(x[0], x[1]) | (f32x2_to_fp8x2<true>(x[2], x[3]) << 16);
-    }
-    if (nvalid == 16 && (reinterpret_cast<uintptr_t>(d) & 15u) == 0) {
-      asm volatile("st.global.v4.u32 [%0], {%1,%2,%3,%4};" ::"l"(d), "r"(o[0]), "r"(o[1]), "r"(o[2]), "r"(o[3]) : "memory");
-    } else {
-#pragma unroll
-      for (uint32_t j = 0; j < 16; ++j)
-        if (j < nvalid) d[j] = static_cast<char>((o[j >> 2] >> (8 * (j & 3))) & 0xffu);
-    }
+    uint32_t f[16], o[4];
+    load16_shared<DT>(s, nvalid, f);
+    narrow16(f, scale, o);
+    store16(d, nvalid, o);
   }
 }
 
@@ -412,16 +328,8 @@ __device__ __forceinline__ void run_block(const BqBlock& blk, const BqPiece* pie
     uint32_t a = s_red[0];
 #pragma unroll
     for (uint32_t w = 1; w < kBqThreads / 32; ++w) a = max(a, s_red[w]);
-    float amax_c, scale, scale_inv;
-    if (a > 0x7f800000u) {  // a NaN in the block: NaN scale, every output NaN
-      amax_c = __uint_as_float(0x7fffffffu);
-      scale = amax_c;
-      scale_inv = amax_c;
-    } else {
-      amax_c = fmaxf(__uint_as_float(a), 1e-4f);
-      scale = __fdiv_rn(448.0f, amax_c);
-      scale_inv = __fdiv_rn(amax_c, 448.0f);
-    }
+    float scale, scale_inv;
+    scales_of_amax(a, &scale, &scale_inv);
     *s_scale = scale;
     *reinterpret_cast<float*>(blk.scale) = scale_inv;
   }

@@ -1,0 +1,131 @@
+// Device helpers of the scaled fp8 quantisers (block_fp8.cu: 128x128 blocks; scaled_fp8.cu: per-channel
+// and per-tensor scales): exact widening of bf16/f16/f32 source bits to f32, |x| as an ordered integer,
+// the folding 16-byte loads, and the 16-element narrowing x * scale -> e4m3fn with its stores.
+#pragma once
+
+#include <cuda_fp16.h>
+#include <stdint.h>
+
+#include "fp8_cvt.cuh"
+#include "tsb_internal.h"
+
+namespace tsb {
+
+__device__ __forceinline__ uint4 ldg16(const char* p) {
+  uint4 v;
+  asm volatile("ld.global.nc.L1::no_allocate.v4.u32 {%0,%1,%2,%3}, [%4];"
+               : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w)
+               : "l"(p));
+  return v;
+}
+
+__device__ __forceinline__ float f16_bits_to_f32(uint32_t bits16) {
+  const unsigned short b = static_cast<unsigned short>(bits16);
+  return __half2float(*reinterpret_cast<const __half*>(&b));
+}
+
+// Source dtypes: element size and the exact widening of one element's bits to f32 bits.
+template <uint32_t DT> struct Src;
+template <> struct Src<TSB_F32> {
+  static constexpr uint32_t kBytes = 4;
+  static __device__ __forceinline__ uint32_t f32(uint32_t bits) { return bits; }
+};
+template <> struct Src<TSB_BF16> {
+  static constexpr uint32_t kBytes = 2;
+  static __device__ __forceinline__ uint32_t f32(uint32_t bits) { return bits << 16; }
+};
+template <> struct Src<TSB_F16> {
+  static constexpr uint32_t kBytes = 2;
+  static __device__ __forceinline__ uint32_t f32(uint32_t bits) { return __float_as_uint(f16_bits_to_f32(bits)); }
+};
+
+// |x| as an integer: finite < Inf < NaN
+__device__ __forceinline__ uint32_t abs_bits(uint32_t f32_bits) { return f32_bits & 0x7fffffffu; }
+
+// fold the elements of one 32-bit source word into a running max of abs_bits
+template <uint32_t DT>
+__device__ __forceinline__ uint32_t fold_word(uint32_t m, uint32_t w) {
+  if (Src<DT>::kBytes == 4) return max(m, abs_bits(w));
+  return max(m, max(abs_bits(Src<DT>::f32(w & 0xffffu)), abs_bits(Src<DT>::f32(w >> 16))));
+}
+
+// fold one 16-byte load
+template <uint32_t DT>
+__device__ __forceinline__ uint32_t fold16(uint32_t m, const uint4& v) {
+  return fold_word<DT>(fold_word<DT>(fold_word<DT>(fold_word<DT>(m, v.x), v.y), v.z), v.w);
+}
+
+// f32 bits of element j of a chunk starting at `s` (any memory the thread may dereference)
+template <uint32_t DT>
+__device__ __forceinline__ uint32_t elem(const unsigned char* s, uint32_t j) {
+  if (Src<DT>::kBytes == 4) return *reinterpret_cast<const uint32_t*>(s + 4 * j);
+  return Src<DT>::f32(*reinterpret_cast<const unsigned short*>(s + 2 * j));
+}
+
+// the f32 bits of the 16 source words `w` (16 elements, 2 or 4 bytes each) in element order
+template <uint32_t DT>
+__device__ __forceinline__ void widen16(const uint4* w4, uint32_t f[16]) {
+  constexpr uint32_t es = Src<DT>::kBytes;
+#pragma unroll
+  for (uint32_t i = 0; i < es; ++i) {
+    const uint4 w = w4[i];
+    const uint32_t words[4] = {w.x, w.y, w.z, w.w};
+#pragma unroll
+    for (uint32_t k = 0; k < 4; ++k) {
+      if constexpr (es == 4) {
+        f[4 * i + k] = words[k];
+      } else {
+        f[8 * i + 2 * k] = Src<DT>::f32(words[k] & 0xffffu);
+        f[8 * i + 2 * k + 1] = Src<DT>::f32(words[k] >> 16);
+      }
+    }
+  }
+}
+
+// 16 elements from shared memory: `s` is 16-byte aligned when nvalid == 16; elements past nvalid are 0
+template <uint32_t DT>
+__device__ __forceinline__ void load16_shared(const unsigned char* s, uint32_t nvalid, uint32_t f[16]) {
+  if (nvalid == 16) {
+    widen16<DT>(reinterpret_cast<const uint4*>(s), f);
+  } else {
+#pragma unroll
+    for (uint32_t j = 0; j < 16; ++j) f[j] = j < nvalid ? elem<DT>(s, j) : 0u;
+  }
+}
+
+// x * scale (correctly rounded) -> e4m3fn with torch's .to() rounding, 4 bytes per word
+__device__ __forceinline__ void narrow16(const uint32_t f[16], float scale, uint32_t o[4]) {
+#pragma unroll
+  for (uint32_t q = 0; q < 4; ++q) {
+    uint32_t x[4];
+#pragma unroll
+    for (uint32_t j = 0; j < 4; ++j) x[j] = __float_as_uint(__fmul_rn(__uint_as_float(f[4 * q + j]), scale));
+    o[q] = f32x2_to_fp8x2<true>(x[0], x[1]) | (f32x2_to_fp8x2<true>(x[2], x[3]) << 16);
+  }
+}
+
+// the first nvalid of 16 fp8 bytes to global memory: one STG.128 when whole and aligned, else bytes
+__device__ __forceinline__ void store16(char* d, uint32_t nvalid, const uint32_t o[4]) {
+  if (nvalid == 16 && (reinterpret_cast<uintptr_t>(d) & 15u) == 0) {
+    asm volatile("st.global.v4.u32 [%0], {%1,%2,%3,%4};" ::"l"(d), "r"(o[0]), "r"(o[1]), "r"(o[2]), "r"(o[3]) : "memory");
+  } else {
+#pragma unroll
+    for (uint32_t j = 0; j < 16; ++j)
+      if (j < nvalid) d[j] = static_cast<char>((o[j >> 2] >> (8 * (j & 3))) & 0xffu);
+  }
+}
+
+// amax bits -> (scale, scale_inv): amax_c = max(amax, 1e-4f), scale = 448 / amax_c, scale_inv = amax_c / 448,
+// both correctly rounded; a NaN amax gives NaN for both
+__device__ __forceinline__ void scales_of_amax(uint32_t a, float* scale, float* scale_inv) {
+  if (a > 0x7f800000u) {
+    *scale = __uint_as_float(0x7fffffffu);
+    *scale_inv = *scale;
+  } else {
+    const float amax_c = fmaxf(__uint_as_float(a), 1e-4f);
+    *scale = __fdiv_rn(448.0f, amax_c);
+    *scale_inv = __fdiv_rn(amax_c, 448.0f);
+  }
+}
+
+}  // namespace tsb

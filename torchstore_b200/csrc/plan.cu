@@ -40,9 +40,10 @@ TableLayout table_layout(size_t n_rects, size_t n_tiles, size_t n_link) {
   return l;
 }
 
-// What a plan's tables drive: the copy_rects kernel, or the block-scaled fp8 quantiser
-// (d_block = {BqBlock table | BqPiece table}, num_tiles = blocks).
-enum : uint32_t { PLAN_COPY = 0, PLAN_BLOCK_FP8 = 1 };
+// What a plan's tables drive: the copy_rects kernel, the block-scaled fp8 quantiser
+// (d_block = {BqBlock table | BqPiece table}, num_tiles = blocks), or the per-channel / per-tensor
+// scaled fp8 quantisers (d_block = {SqBand table | SqPiece table | SqTile table | amax words}).
+enum : uint32_t { PLAN_COPY = 0, PLAN_BLOCK_FP8 = 1, PLAN_SCALED_FP8 = 2 };
 
 struct Plan {
   int device = 0;
@@ -54,6 +55,8 @@ struct Plan {
   uint32_t kind = KIND_GENERIC;
   size_t bq_pieces_off = 0;    // PLAN_BLOCK_FP8: byte offset of the piece table in d_block
   uint32_t bq_src_bytes = 2;   // PLAN_BLOCK_FP8: largest source element size
+  size_t sq_off[3] = {};       // PLAN_SCALED_FP8: byte offsets of the piece and tile tables and the amax words
+  SqLaunch sq{};               // PLAN_SCALED_FP8: counts (run_plan fills in the table pointers)
   uint32_t link_stage_bytes = 0;
   uint32_t link_stages = 0;
   tsb_plan_info_t info{};
@@ -557,6 +560,14 @@ int run_plan(Plan* p, cudaStream_t s) {
   if (p->plan_kind == PLAN_BLOCK_FP8)
     return launch_block_fp8(reinterpret_cast<const BqBlock*>(p->d_block), reinterpret_cast<const BqPiece*>(p->d_block + p->bq_pieces_off),
                             p->num_tiles, p->bq_src_bytes, s);
+  if (p->plan_kind == PLAN_SCALED_FP8) {
+    SqLaunch l = p->sq;
+    l.bands = reinterpret_cast<const SqBand*>(p->d_block);
+    l.pieces = reinterpret_cast<const SqPiece*>(p->d_block + p->sq_off[0]);
+    l.tiles = reinterpret_cast<const SqTile*>(p->d_block + p->sq_off[1]);
+    l.amax = reinterpret_cast<uint32_t*>(p->d_block + p->sq_off[2]);
+    return launch_scaled_fp8(l, s);
+  }
   uint32_t kind = p->kind;
   if (getenv("TSB_FORCE_GENERIC")) kind = KIND_GENERIC;
   LaunchParams lp = make_params(p->d_block, p->layout, p->num_tiles, p->num_link_tiles, kind, p->link_stage_bytes, p->link_stages);
@@ -709,6 +720,42 @@ int tsb_block_fp8_plan_create(int device, const tsb_rect_t* rects, uint64_t n, c
   std::vector<char> host(std::max<size_t>(16, p->bq_pieces_off + tb.pieces.size() * sizeof(BqPiece)));
   if (!tb.blocks.empty()) memcpy(host.data(), tb.blocks.data(), p->bq_pieces_off);
   if (!tb.pieces.empty()) memcpy(host.data() + p->bq_pieces_off, tb.pieces.data(), tb.pieces.size() * sizeof(BqPiece));
+  return register_plan(p, host, out);
+}
+
+int tsb_scaled_fp8_plan_create(int device, const tsb_rect_t* rects, uint64_t n, const tsb_sq_target_t* targets,
+                               uint64_t n_targets, uint32_t flags, tsb_plan_t* out) {
+  if (!out) return fail(TSB_ERR_INVALID, "tsb_scaled_fp8_plan_create: NULL argument");
+  if (flags != 0) return fail(TSB_ERR_INVALID, "tsb_scaled_fp8_plan_create: flags must be 0");
+  SqTables tb;
+  int st = scaled_fp8_compile(device, rects, n, targets, n_targets, &tb);
+  if (st) return st;
+  const size_t pieces_off = tb.bands.size() * sizeof(SqBand);
+  const size_t tiles_off = pieces_off + tb.pieces.size() * sizeof(SqPiece);
+  const size_t amax_off = tiles_off + tb.tiles.size() * sizeof(SqTile);
+  std::vector<char> host(std::max<size_t>(16, amax_off + 4ull * tb.n_groups), 0);
+  if (!tb.bands.empty()) memcpy(host.data(), tb.bands.data(), pieces_off);
+  if (!tb.pieces.empty()) memcpy(host.data() + pieces_off, tb.pieces.data(), tiles_off - pieces_off);
+  if (!tb.tiles.empty()) memcpy(host.data() + tiles_off, tb.tiles.data(), amax_off - tiles_off);
+  Plan* p = new Plan();
+  p->device = device;
+  p->plan_kind = PLAN_SCALED_FP8;
+  p->num_tiles = static_cast<uint32_t>(tb.bands.size() + tb.tiles.size());
+  p->info.num_rects = n;
+  p->info.num_tiles = p->num_tiles;
+  p->info.payload_bytes = tb.payload_bytes;
+  p->info.src_bytes = tb.src_bytes;
+  p->info.remote_src_bytes = tb.remote_src_bytes;
+  p->info.grid = p->num_tiles;
+  p->info.block = kSqThreads;
+  p->info.tile_bytes = kSqStageBytes;
+  p->sq_off[0] = pieces_off;
+  p->sq_off[1] = tiles_off;
+  p->sq_off[2] = amax_off;
+  p->sq.n_bands = static_cast<uint32_t>(tb.bands.size());
+  p->sq.n_tiles = static_cast<uint32_t>(tb.tiles.size());
+  p->sq.n_groups = tb.n_groups;
+  p->sq.stage_bytes = tb.stage_bytes;
   return register_plan(p, host, out);
 }
 

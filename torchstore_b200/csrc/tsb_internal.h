@@ -159,6 +159,24 @@ int launch_copy_rects(const LaunchParams& p, uint32_t grid, cudaStream_t stream)
 void count_launch();
 int max_ctas_per_sm(uint32_t kind, bool with_link, uint32_t link_smem_bytes, int* out);
 
+// ---- scaled fp8 destinations: the rect -> [batch, rows, cols] mapping (block_fp8.cu) ----------------
+// Where a quantised destination lives: `batch` contiguous [rows, cols] float8_e4m3fn matrices at dst.
+struct TargetGeom {
+  uint64_t dst, batch, rows, cols;
+};
+// A rect after mapping onto its target: an [er, ec] box of matrix b at (r0, c0), source rows contiguous.
+struct TargetBox {
+  uint64_t src;
+  int64_t row_stride;  // source bytes between rows (0 for a single row)
+  uint64_t target, b, r0, c0, er, ec;
+  uint32_t dtype;
+  int32_t src_device;
+};
+uint32_t quant_src_bytes(uint32_t dtype);  // 4 / 2 for TSB_F32 / TSB_BF16, TSB_F16; 0 otherwise
+// Append one box per combination of the rect's batch dims to `out` (nothing for an empty rect).
+int rect_boxes(const tsb_rect_t& in, uint64_t index, const TargetGeom* targets, uint64_t n_targets,
+               std::vector<TargetBox>* out);
+
 // ---- block-scaled fp8 (block_fp8.cu) ---------------------------------------------------------------
 constexpr uint32_t kBqBlock = 128;  // block edge (elements)
 constexpr uint32_t kBqThreads = 256;
@@ -196,5 +214,71 @@ int block_fp8_compile(int device, const tsb_rect_t* rects, uint64_t n, const tsb
                       BqTables* out);
 int launch_block_fp8(const BqBlock* blocks, const BqPiece* pieces, uint32_t n_blocks, uint32_t max_src_bytes,
                      cudaStream_t stream);
+
+// ---- per-channel / per-tensor scaled fp8 (scaled_fp8.cu) -------------------------------------------
+constexpr uint32_t kSqThreads = 256;
+// Shared-memory stage of the row-staged kernel: a per-channel row whose source bytes (rounded up to 16)
+// fit takes the one-read path.  32 KiB admits a bf16 row of K = 14336 (28 KiB) and four of K = 4096,
+// stays under the 48 KiB default (no opt-in), and leaves room for 6 CTAs of 256 threads per SM.
+constexpr uint32_t kSqStageBytes = 32768;
+constexpr uint32_t kSqBandRows = 256;      // most rows one CTA stages (one per thread in the reduction)
+constexpr uint32_t kSqTileElems = 16384;   // most elements of one two-pass tile (one CTA per pass)
+
+// Row-staged path: a band of whole rows of one per-channel matrix.
+struct alignas(8) SqBand {
+  uint64_t dst;          // fp8 element (0, 0) of the band
+  uint64_t scale;        // float32 scale_inv of its first row (one per row, contiguous)
+  uint32_t cols;         // row length (elements == destination pitch in bytes)
+  uint32_t rows;
+  uint32_t piece0, n_pieces;
+  uint32_t src_dtype;    // the same for every piece of the band
+  uint32_t pad_;
+};
+static_assert(sizeof(SqBand) == 40, "SqBand is part of tsb_scaled_fp8_compile_host's output");
+
+// A source rectangle inside one band.
+struct alignas(8) SqPiece {
+  uint64_t src;          // source element (row0, col0) of the piece
+  int64_t src_stride;    // bytes between source rows
+  uint32_t row0, col0;   // position inside the band
+  uint32_t rows, cols;
+  uint32_t vec;          // 1: source address, stride, column offset and width allow 16-byte accesses
+  uint32_t pad_;
+};
+static_assert(sizeof(SqPiece) == 40, "SqPiece is part of tsb_scaled_fp8_compile_host's output");
+
+// Two-pass path: a rectangle of one group (a per-tensor matrix or a long per-channel row), read once
+// per pass by one CTA.
+struct alignas(8) SqTile {
+  uint64_t src;          // source element (0, 0) of the tile
+  int64_t src_stride;    // bytes between source rows
+  uint64_t dst;          // its fp8 element (0, 0)
+  uint64_t scale;        // the group's float32 scale_inv if this tile writes it (one tile per group), else 0
+  uint32_t dst_pitch;    // destination row pitch (bytes == elements)
+  uint32_t rows, cols;
+  uint32_t group;        // index of the group's amax word
+  uint32_t src_dtype;
+  uint32_t vec;          // as SqPiece::vec
+};
+static_assert(sizeof(SqTile) == 56, "SqTile is part of tsb_scaled_fp8_compile_host's output");
+
+struct SqTables {
+  std::vector<SqBand> bands;
+  std::vector<SqPiece> pieces;
+  std::vector<SqTile> tiles;
+  uint32_t n_groups = 0;        // amax words of the two-pass path
+  uint32_t stage_bytes = 0;     // largest band stage (dynamic shared memory of the row-staged kernel)
+  uint64_t src_bytes = 0, remote_src_bytes = 0, payload_bytes = 0;
+};
+int scaled_fp8_compile(int device, const tsb_rect_t* rects, uint64_t n, const tsb_sq_target_t* targets,
+                       uint64_t n_targets, SqTables* out);
+struct SqLaunch {
+  const SqBand* bands;
+  const SqPiece* pieces;
+  const SqTile* tiles;
+  uint32_t* amax;  // n_groups words, cleared by the launch
+  uint32_t n_bands, n_tiles, n_groups, stage_bytes;
+};
+int launch_scaled_fp8(const SqLaunch& l, cudaStream_t stream);
 
 }  // namespace tsb

@@ -46,6 +46,13 @@ logger = logging.getLogger(__name__)
 RDMA_KEY_PREFIX = "policy_rdma"
 BLOCK = 128  # edge of a block-scaled fp8 block (elements)
 BLOCK_SOURCE_DTYPES = {torch.bfloat16, torch.float16, torch.float32}
+# the scale granularities of pull(): keyword -> (what its validation messages call the scale, the destination)
+SCALE_KINDS = {
+    "block_scales": ("block scale", "block-scaled"),
+    "channel_scales": ("channel scale", "channel-scaled"),
+    "tensor_scales": ("tensor scale", "tensor-scaled"),
+}
+_GRANULARITY = {"channel_scales": _native.TSB_SCALE_PER_CHANNEL, "tensor_scales": _native.TSB_SCALE_PER_TENSOR}
 
 
 # ---------------------------------------------------------------------------------------------
@@ -280,8 +287,9 @@ class DirectWeightSyncDest:
         self._plan_dict: dict | None = None  # the dict object they came in (identity short-cut of the next pull)
         self._native_plans = Plans()  # the compiled plan, one native plan per destination device
         self._block_plans = Plans()  # block-scaled fp8 names: one quantising plan per destination device
-        self._block_keys: frozenset = frozenset()  # names the cached plan quantises
-        self._plan_block_dict: dict | None = None  # the block_scales dict object of the last pull
+        self._scaled_plans = Plans()  # per-channel / per-tensor scaled fp8 names: likewise
+        self._scale_keys: frozenset = frozenset()  # (name, scale keyword) pairs the cached plan quantises
+        self._plan_scale_dicts: tuple | None = None  # the three scale dict objects of the last pull
         self.last_pull_ms: dict[int, float] = {}  # device -> kernel time of the last pull
 
     # -- planning (host, metadata only) ----------------------------------------------------------
@@ -349,52 +357,69 @@ class DirectWeightSyncDest:
         return src_window.sub(op.src_slices), dst_full.sub(op.dest_slices)
 
     @staticmethod
-    def _signature(dest_state_dict, block_scales=None) -> tuple:
+    def _signature(dest_state_dict, scales: tuple = ()) -> tuple:
         # data pointers only: ~35 us for 291 tensors; a new state_dict() wrapper around the same
         # memory keeps the plan, new memory invalidates it
         sig = tuple(getattr(p, "_local_tensor", p).data_ptr() for p in dest_state_dict.values())
-        return sig + tuple(s.data_ptr() for s in block_scales.values()) if block_scales else sig
+        for d in scales:
+            if d:
+                sig += tuple(s.data_ptr() for s in d.values())
+        return sig
 
     @staticmethod
-    def _ids(dest_state_dict, block_scales=None) -> tuple:
+    def _ids(dest_state_dict, scales: tuple = ()) -> tuple:
         ids = tuple(map(id, dest_state_dict.values()))
-        return ids + tuple(map(id, block_scales.values())) if block_scales else ids
+        for d in scales:
+            if d:
+                ids += tuple(map(id, d.values()))
+        return ids
 
     @staticmethod
-    def _check_block_scales(all_handles, dest_state_dict, block_scales) -> dict[str, tuple[torch.Tensor, torch.Tensor]]:
-        """Validate ``block_scales`` -> ``{name: (fp8 destination, scale_inv)}``.  Raises before anything
-        is compiled or launched."""
+    def _check_scales(all_handles, dest_state_dict, scales: dict[str, dict | None]) -> dict[str, tuple]:
+        """Validate the scale dicts of a pull (``{keyword: {name: scale}}``, keywords of SCALE_KINDS) ->
+        ``{name: (keyword, fp8 destination, scale)}``.  Raises before anything is compiled or launched."""
         out = {}
-        for name, scale in block_scales.items():
-            if name not in dest_state_dict:
-                raise ValueError(f"block_scales names '{name}', which is not in the destination state dict")
-            dest = getattr(dest_state_dict[name], "_local_tensor", dest_state_dict[name])
-            if not isinstance(scale, torch.Tensor):
-                raise TypeError(f"block scale of '{name}' is a {type(scale).__name__}, not a tensor")
-            if dest.dtype != torch.float8_e4m3fn:
-                raise TypeError(f"block-scaled destination '{name}' must be float8_e4m3fn, not {dest.dtype}")
-            if dest.dim() < 2 or dest.numel() == 0 or not dest.is_contiguous() or not dest.is_cuda:
-                raise ValueError(f"block-scaled destination '{name}' must be a non-empty contiguous CUDA tensor with at "
-                                 f"least 2 dims; got shape {tuple(dest.shape)}, strides {dest.stride()} on {dest.device}")
-            rows, cols = dest.shape[-2:]
-            want = tuple(dest.shape[:-2]) + (-(-rows // BLOCK), -(-cols // BLOCK))
-            if scale.dtype != torch.float32:
-                raise TypeError(f"block scale of '{name}' must be float32, not {scale.dtype}")
-            if tuple(scale.shape) != want or not scale.is_contiguous() or scale.device != dest.device:
-                raise ValueError(f"block scale of '{name}' must be a contiguous {want} tensor on {dest.device}; got "
-                                 f"{tuple(scale.shape)}, strides {scale.stride()} on {scale.device}")
-            handles = all_handles.get(name) or []
-            if not handles:
-                raise ValueError(f"no source handles for block-scaled destination '{name}': its blocks would not be covered")
-            dtypes = {h.rdma_buffer.dtype for h in handles}
-            if not dtypes <= BLOCK_SOURCE_DTYPES or len(dtypes) != 1:
-                raise TypeError(f"block-scaled pulls of '{name}' read bf16, f16 or f32 handles of one dtype; got {sorted(map(str, dtypes))}")
-            out[name] = (dest, scale)
+        for kw, by_name in scales.items():
+            what, kind = SCALE_KINDS[kw]
+            for name, scale in (by_name or {}).items():
+                if name not in dest_state_dict:
+                    raise ValueError(f"{kw} names '{name}', which is not in the destination state dict")
+                if name in out:
+                    raise ValueError(f"'{name}' is in both {out[name][0]} and {kw}: a destination has one scale layout")
+                dest = getattr(dest_state_dict[name], "_local_tensor", dest_state_dict[name])
+                if not isinstance(scale, torch.Tensor):
+                    raise TypeError(f"{what} of '{name}' is a {type(scale).__name__}, not a tensor")
+                if dest.dtype != torch.float8_e4m3fn:
+                    raise TypeError(f"{kind} destination '{name}' must be float8_e4m3fn, not {dest.dtype}")
+                if dest.dim() < 2 or dest.numel() == 0 or not dest.is_contiguous() or not dest.is_cuda:
+                    raise ValueError(f"{kind} destination '{name}' must be a non-empty contiguous CUDA tensor with at "
+                                     f"least 2 dims; got shape {tuple(dest.shape)}, strides {dest.stride()} on {dest.device}")
+                lead, (rows, cols) = tuple(dest.shape[:-2]), dest.shape[-2:]
+                if kw == "block_scales":
+                    wants = [lead + (-(-rows // BLOCK), -(-cols // BLOCK))]
+                elif kw == "channel_scales":
+                    wants = [lead + (rows, 1)]
+                else:
+                    wants = [lead, lead + (1,)]
+                if scale.dtype != torch.float32:
+                    raise TypeError(f"{what} of '{name}' must be float32, not {scale.dtype}")
+                if tuple(scale.shape) not in wants or not scale.is_contiguous() or scale.device != dest.device:
+                    want = " or ".join(map(str, wants))
+                    raise ValueError(f"{what} of '{name}' must be a contiguous {want} tensor on {dest.device}; got "
+                                     f"{tuple(scale.shape)}, strides {scale.stride()} on {scale.device}")
+                handles = all_handles.get(name) or []
+                if not handles:
+                    raise ValueError(f"no source handles for {kind} destination '{name}': its groups would not be covered")
+                dtypes = {h.rdma_buffer.dtype for h in handles}
+                if not dtypes <= BLOCK_SOURCE_DTYPES or len(dtypes) != 1:
+                    raise TypeError(f"{kind} pulls of '{name}' read bf16, f16 or f32 handles of one dtype; "
+                                    f"got {sorted(map(str, dtypes))}")
+                out[name] = (kw, dest, scale)
         return out
 
-    def _compile(self, blocked: dict | None = None) -> None:
+    def _compile(self, scaled: dict | None = None) -> None:
         per_device: dict[int, list] = defaultdict(list)
-        block_pairs: dict[int, list] = defaultdict(list)
+        quant_pairs: dict[tuple, list] = defaultdict(list)  # (device, block?) -> windows of the quantising plans
         for op in self._plan:
             dest = op.dest_local
             if not dest.is_cuda:
@@ -407,28 +432,43 @@ class DirectWeightSyncDest:
                     f"handle for '{op.name}' carries a {type(op.rdma_buffer).__name__}; the direct path needs NvlinkBuffer handles"
                 )
             dev = dest.device.index
-            (block_pairs if blocked and op.name in blocked else per_device)[dev].append(self.op_windows(op, op.rdma_buffer.window(dev)))
+            window = self.op_windows(op, op.rdma_buffer.window(dev))
+            if scaled and op.name in scaled:
+                quant_pairs[(dev, scaled[op.name][0] == "block_scales")].append(window)
+            else:
+                per_device[dev].append(window)
         self._native_plans = Plans.build(per_device)
-        if not blocked:
+        if not scaled:
             return
         try:
-            for dev in sorted({d.device.index for d, _ in blocked.values()}):
-                pairs = block_pairs.get(dev, [])
-                names = [n for n, (d, _) in blocked.items() if d.device.index == dev]
-                targets = []
-                for n in names:
-                    d, s = blocked[n]
-                    rows, cols = d.shape[-2:]
-                    targets.append(_native.BqTarget(d.data_ptr(), s.data_ptr(), d.numel() // (rows * cols), rows, cols))
-                try:
-                    self._block_plans.update(Plans.build_block_fp8({dev: (pairs, targets)}))
-                except _native.TsbError as e:
-                    m = re.search(r"target (\d+)", str(e))
-                    if e.code == _native.TSB_ERR_INVALID and m:
-                        raise ValueError(f"block-scaled pull of '{names[int(m.group(1))]}': {e}") from e
-                    raise
+            for block in (True, False):
+                for dev in sorted({d.device.index for kw, d, _ in scaled.values() if (kw == "block_scales") == block}):
+                    names = [n for n, (kw, d, _) in scaled.items()
+                             if d.device.index == dev and (kw == "block_scales") == block]
+                    targets = []
+                    for n in names:
+                        kw, d, s = scaled[n]
+                        rows, cols = d.shape[-2:]
+                        if block:
+                            targets.append(_native.BqTarget(d.data_ptr(), s.data_ptr(), d.numel() // (rows * cols), rows, cols))
+                        else:
+                            targets.append(_native.SqTarget(d.data_ptr(), s.data_ptr(), d.numel() // (rows * cols), rows, cols,
+                                                            _GRANULARITY[kw], 0))
+                    pairs = quant_pairs.get((dev, block), [])
+                    try:
+                        if block:
+                            self._block_plans.update(Plans.build_block_fp8({dev: (pairs, targets)}))
+                        else:
+                            self._scaled_plans.update(Plans.build_scaled_fp8({dev: (pairs, targets)}))
+                    except _native.TsbError as e:
+                        m = re.search(r"target (\d+)", str(e))
+                        if e.code == _native.TSB_ERR_INVALID and m:
+                            name = names[int(m.group(1))]
+                            raise ValueError(f"{SCALE_KINDS[scaled[name][0]][1]} pull of '{name}' ({scaled[name][0]}): {e}") from e
+                        raise
         except BaseException:
             self._block_plans.close()
+            self._scaled_plans.close()
             self._native_plans.close()
             raise
 
@@ -439,67 +479,79 @@ class DirectWeightSyncDest:
     async def pull(self, all_handles: dict[str, list[RDMAWeightHandle]],
                    dest_state_dict: dict[str, torch.Tensor],
                    dest_slices: dict[str, TensorSlice] | None = None, *,
-                   block_scales: dict[str, torch.Tensor] | None = None) -> None:
+                   block_scales: dict[str, torch.Tensor] | None = None,
+                   channel_scales: dict[str, torch.Tensor] | None = None,
+                   tensor_scales: dict[str, torch.Tensor] | None = None) -> None:
         """Pull every overlapping region into ``dest_state_dict`` (in place).  Returns when the
         bytes are in destination HBM (so the caller may tell the source it is done reading).
 
-        ``block_scales`` (extension) maps names to float32 ``scale_inv`` tensors: those destinations are
-        float8_e4m3fn weights in the 128x128 block-scaled layout of DeepSeek-V3 / vLLM
-        (``weight_block_size=[128, 128]``), quantised during the pull from bf16/f16/f32 handles (the
-        formula is in DESIGN.md section 4).  Every element of such a destination must be covered by
-        the handles.  The other names are pulled as without ``block_scales``.
+        Scaled fp8 destinations (extension): float8_e4m3fn weights quantised during the pull from
+        bf16/f16/f32 handles, each name in at most one of
+        * ``block_scales``: float32 ``scale_inv`` per 128x128 block, the layout of DeepSeek-V3 / vLLM
+          ``weight_block_size=[128, 128]`` (shape ``lead + (ceil(N/128), ceil(K/128))``);
+        * ``channel_scales``: one float32 scale per output row, compressed-tensors FP8 / fbgemm-fp8
+          ``weight_scale`` (shape ``lead + (N, 1)``);
+        * ``tensor_scales``: one float32 scale per [N, K] matrix, vLLM ``quantization="fp8"`` (shape
+          ``lead`` or ``lead + (1,)``).
+        ``lead`` is the destination's dims before the last two (MoE stacks quantise every matrix on its
+        own).  The formula is in DESIGN.md section 4.  Every element of such a destination must be
+        covered by the handles.  The other names are pulled as without scales.
 
         Steady state costs one native call to launch and a poll loop: the cached plan is checked
         against the destination OBJECTS first (their ids; the plan keeps them alive), the kernel
         is enqueued, and the data-pointer signature -- which catches ``param.data = new`` under an
         unchanged object -- is recomputed while the kernel runs."""
-        if self._plan is not None and (block_scales or self._block_keys) and frozenset(block_scales or ()) != self._block_keys:
-            logger.info("block_scales names changed; rebuilding the transfer plan")
+        scales = (block_scales, channel_scales, tensor_scales)
+        keys = frozenset((n, kw) for kw, d in zip(SCALE_KINDS, scales) for n in (d or ()))
+        if self._plan is not None and keys != self._scale_keys:
+            logger.info("scaled names or their granularity changed; rebuilding the transfer plan")
             self.close()
-        if self._plan is not None and dest_state_dict is self._plan_dict and block_scales is self._plan_block_dict:
+        if self._plan is not None and dest_state_dict is self._plan_dict and \
+                all(a is b for a, b in zip(scales, self._plan_scale_dicts)):
             # the very dict object of the last pull: launch first, validate it (object ids, then data pointers)
             # while the kernel runs -- a stale launch only fills memory the plan still references
             self.launch()
-            same = self._ids(dest_state_dict, block_scales) == self._plan_ids and \
-                self._signature(dest_state_dict, block_scales) == self._plan_signature
+            same = self._ids(dest_state_dict, scales) == self._plan_ids and \
+                self._signature(dest_state_dict, scales) == self._plan_signature
             await self.wait()
             if same:
                 return
             logger.info("destination dict was edited in place; rebuilding the transfer plan")
             self.close()
-        ids = self._ids(dest_state_dict, block_scales)
-        refs = list(dest_state_dict.values()) + (list(block_scales.values()) if block_scales else [])
+        ids = self._ids(dest_state_dict, scales)
+        refs = list(dest_state_dict.values()) + [t for d in scales if d for t in d.values()]
         verified = False
         if self._plan is not None and ids != self._plan_ids:
             # other wrapper objects: fine if they alias the same memory (e.g. a fresh state_dict())
-            if self._signature(dest_state_dict, block_scales) != self._plan_signature:
+            if self._signature(dest_state_dict, scales) != self._plan_signature:
                 logger.info("destination tensors changed; rebuilding the transfer plan")
                 self.close()
             else:
                 self._plan_ids, self._plan_refs, self._plan_dict = ids, refs, dest_state_dict
-                self._plan_block_dict = block_scales
+                self._plan_scale_dicts = scales
             verified = True
         if self._plan is None:
-            blocked = self._check_block_scales(all_handles, dest_state_dict, block_scales) if block_scales else None
+            scaled = self._check_scales(all_handles, dest_state_dict, dict(zip(SCALE_KINDS, scales))) if keys else None
             self._plan = self._build_plan(all_handles, dest_state_dict, dest_slices)
             try:
-                self._compile(blocked)
+                self._compile(scaled)
             except BaseException:
                 self._plan = None
                 raise
-            self._block_keys = frozenset(block_scales or ())
-            self._plan_signature = self._signature(dest_state_dict, block_scales)
+            self._scale_keys = keys
+            self._plan_signature = self._signature(dest_state_dict, scales)
             self._plan_ids, self._plan_refs, self._plan_dict = ids, refs, dest_state_dict
-            self._plan_block_dict = block_scales
+            self._plan_scale_dicts = scales
             verified = True
         self.launch()
-        stale = not verified and self._signature(dest_state_dict, block_scales) != self._plan_signature
+        stale = not verified and self._signature(dest_state_dict, scales) != self._plan_signature
         await self.wait()
         if stale:
             # the launch above filled the OLD memory (still referenced by the plan, so harmless)
             logger.info("destination storage changed under the same tensors; rebuilding the transfer plan")
             self.close()
-            await self.pull(all_handles, dest_state_dict, dest_slices, block_scales=block_scales)
+            await self.pull(all_handles, dest_state_dict, dest_slices, block_scales=block_scales,
+                            channel_scales=channel_scales, tensor_scales=tensor_scales)
 
     def launch(self) -> None:
         """Enqueue the cached plan on each device's copy stream, fenced against the caller's current
@@ -509,23 +561,27 @@ class DirectWeightSyncDest:
         self._native_plans.launch()
         if self._block_plans:
             self._block_plans.launch()
+        if self._scaled_plans:
+            self._scaled_plans.launch()
 
     async def wait(self) -> None:
         await self._native_plans.wait()
         ms = self._native_plans.elapsed_ms()
-        if self._block_plans:
-            # both plans of a device run back to back on its copy stream
-            await self._block_plans.wait()
-            for dev, t in self._block_plans.elapsed_ms().items():
-                ms[dev] = ms.get(dev, 0.0) + t
+        # the plans of a device run back to back on its copy stream
+        for plans in (self._block_plans, self._scaled_plans):
+            if plans:
+                await plans.wait()
+                for dev, t in plans.elapsed_ms().items():
+                    ms[dev] = ms.get(dev, 0.0) + t
         self.last_pull_ms.update(ms)
 
     def close(self) -> None:
         self._native_plans.close()
         self._block_plans.close()
-        self._block_keys = frozenset()
+        self._scaled_plans.close()
+        self._scale_keys = frozenset()
         self._plan = None
-        self._plan_ids = self._plan_refs = self._plan_dict = self._plan_block_dict = None
+        self._plan_ids = self._plan_refs = self._plan_dict = self._plan_scale_dicts = None
 
 
 def _contig(shape) -> tuple:

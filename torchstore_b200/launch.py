@@ -107,6 +107,23 @@ class Plans(dict):
             raise
         return plans
 
+    @classmethod
+    def build_scaled_fp8(cls, per_device: dict[int, tuple[list, list]]) -> "Plans":
+        """Compile per-channel / per-tensor scaled fp8 pulls: ``{device: ([(src, dst) StridedMem windows],
+        [SqTarget])}``."""
+        plans = cls()
+        try:
+            for dev, (pairs, targets) in per_device.items():
+                rects, n = build_rects(pairs)
+                arr = _native.make_sq_target_array(max(1, len(targets)))
+                for i, t in enumerate(targets):
+                    arr[i] = t
+                plans[dev] = _native.scaled_fp8_plan_create(dev, rects, n, arr, len(targets))
+        except BaseException:
+            plans.close()
+            raise
+        return plans
+
     def launch(self, fence_out: bool = True) -> None:
         """Enqueue every plan on its device's copy stream, fenced in against the caller's current
         stream of that device.  ``fence_out=False``: the caller's stream is not made to wait for the

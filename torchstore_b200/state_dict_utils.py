@@ -71,17 +71,22 @@ async def put_state_dict(store, state_dict, key, direct_rdma=False, transfer_dty
 
 
 async def get_state_dict(store, key, user_state_dict: dict | None = None, strict=True, direct_rdma=False,
-                         block_scales: dict | None = None):
+                         block_scales: dict | None = None, channel_scales: dict | None = None,
+                         tensor_scales: dict | None = None):
     """Fetch a state dict.  ``user_state_dict`` tensors are filled in place (and required in direct
     mode).  A missing mapping means no matching push finished: RuntimeError.  ``block_scales``
     (direct mode only) names float8_e4m3fn destinations quantised into the 128x128 block-scaled
-    layout during the pull (see ``DirectWeightSyncDest.pull``)."""
+    layout during the pull; ``channel_scales`` / ``tensor_scales`` likewise name destinations with one
+    float32 scale per row / per matrix (see ``DirectWeightSyncDest.pull``)."""
     if direct_rdma:
         assert user_state_dict is not None, "user_state_dict is required for direct_rdma mode"
-        await _get_state_dict_direct_rdma(store, key, user_state_dict, block_scales)
+        await _get_state_dict_direct_rdma(store, key, user_state_dict, block_scales, channel_scales, tensor_scales)
         return user_state_dict
     if block_scales:
         raise NotImplementedError("block_scales needs direct_rdma=True: the store path does not quantise into block-scaled fp8")
+    if channel_scales or tensor_scales:
+        raise NotImplementedError("channel_scales and tensor_scales need direct_rdma=True: the store path does not "
+                                  "quantise into scaled fp8")
     try:
         fetched_mapping = await store.get(f"{key}{DELIM}{MAPPING}")
     except Exception as e:
@@ -135,10 +140,10 @@ async def _put_state_dict_direct_rdma(store, state_dict, key, transfer_dtype=Non
         cache.source.fence()
 
 
-def _try_all_gather(cache: _DirectRDMACache, key: str, user_state_dict, block_scales=None) -> bool:
+def _try_all_gather(cache: _DirectRDMACache, key: str, user_state_dict, scaled=False) -> bool:
     """Route "every rank reads every tensor in full from the ranks' own Shard(0) shards" to NCCL's
     all-gather (collectives.py).  All ranks must agree, so the local verdict is min-reduced first.
-    A pull with block-scaled destinations votes no: the all-gather moves bytes and cannot quantise."""
+    A pull with scaled fp8 destinations votes no: the all-gather moves bytes and cannot quantise."""
     from torch.distributed.tensor import DTensor
 
     from torchstore_b200.collectives import all_gather_state_dict, is_allgather_shaped
@@ -147,7 +152,7 @@ def _try_all_gather(cache: _DirectRDMACache, key: str, user_state_dict, block_sc
         return False
     rank, world = dist.get_rank(), dist.get_world_size()
     source = cache.sources.get(key)
-    ok = not block_scales and source is not None and key in cache.registered and bool(source._handles)
+    ok = not scaled and source is not None and key in cache.registered and bool(source._handles)
     shards, dests = {}, {}
     if ok:
         ok = not any(isinstance(t, DTensor) for t in user_state_dict.values())
@@ -171,7 +176,8 @@ def _try_all_gather(cache: _DirectRDMACache, key: str, user_state_dict, block_sc
     return True
 
 
-async def _get_state_dict_direct_rdma(store, key, user_state_dict, block_scales=None):
+async def _get_state_dict_direct_rdma(store, key, user_state_dict, block_scales=None, channel_scales=None,
+                                      tensor_scales=None):
     from torchstore_b200.collectives import allgather_enabled
     from torchstore_b200.direct_weight_sync import DirectWeightSyncDest
 
@@ -182,7 +188,8 @@ async def _get_state_dict_direct_rdma(store, key, user_state_dict, block_scales=
     cache.dest = cache.dests.get(key)
     if cache.dest is None:
         cache.dest = cache.dests[key] = DirectWeightSyncDest()
-    if allgather_enabled() and _try_all_gather(cache, key, user_state_dict, block_scales):
+    scaled = bool(block_scales or channel_scales or tensor_scales)
+    if allgather_enabled() and _try_all_gather(cache, key, user_state_dict, scaled):
         return
     if key not in cache.handles:
         num_ranks = await store.get(f"{key}/num_ranks")
@@ -194,4 +201,5 @@ async def _get_state_dict_direct_rdma(store, key, user_state_dict, block_scales=
             for name, handle in tables[f"{key}/rank_{r}"].items():
                 all_handles[name].append(handle)
         cache.handles[key] = all_handles
-    await cache.dests[key].pull(cache.handles[key], user_state_dict, block_scales=block_scales)
+    await cache.dests[key].pull(cache.handles[key], user_state_dict, block_scales=block_scales,
+                                channel_scales=channel_scales, tensor_scales=tensor_scales)
