@@ -26,7 +26,7 @@
 extern "C" {
 #endif
 
-#define TSB_ABI_VERSION 5
+#define TSB_ABI_VERSION 6
 #define TSB_MAX_DIMS 6
 
 enum {
@@ -282,6 +282,49 @@ int tsb_scaled_fp8_compile_host(int device, const tsb_rect_t* rects, uint64_t n,
                                 uint64_t n_targets, uint32_t flags, void* out_bands, uint64_t band_cap,
                                 uint64_t* out_n_bands, void* out_pieces, uint64_t piece_cap, uint64_t* out_n_pieces,
                                 void* out_tiles, uint64_t tile_cap, uint64_t* out_n_tiles, uint64_t* out_n_groups);
+
+/* ------------------------------------------------------------------------------------------ */
+/* dequantising pulls: block-, channel- or tensor-scaled float8_e4m3fn sources into f32, bf16   */
+/* or f16 destinations                                                                          */
+/* ------------------------------------------------------------------------------------------ */
+
+enum { TSB_SCALE_PER_BLOCK = 3 };
+
+/* One scaled fp8 source shard: `batch` contiguous [rows, cols] float8_e4m3fn matrices whose first
+ * element sits at (row0, col0) of the global tensor's last two dims.  Scales are anchored at the
+ * global origin (checkpoint semantics), and the scale tensor holds exactly the groups the shard
+ * touches:
+ *   TSB_SCALE_PER_BLOCK    float32 [batch, ceil((row0+rows)/128) - row0/128, ceil((col0+cols)/128) - col0/128]
+ *   TSB_SCALE_PER_CHANNEL  float32 [batch, rows]
+ *   TSB_SCALE_PER_TENSOR   float32 [batch]
+ * Element (b, i, j) of the shard becomes  dst = to_dst(f32(q[b, i, j]) * scale[b, g(i, j)])  with
+ * g = ((row0+i)/128 - row0/128, (col0+j)/128 - col0/128) per block, i per channel and nothing per
+ * tensor; f32(q) is exact, the multiply one correctly rounded f32 multiply (no flush to zero), and
+ * to_dst the fused cast's f32 -> bf16 / f16 narrowing (identity for f32). */
+typedef struct tsb_dq_source {
+  uint64_t src;         /* float8_e4m3fn as seen from the plan's device */
+  uint64_t scale;       /* float32, contiguous, as seen from the plan's device */
+  uint64_t batch, rows, cols;
+  uint64_t row0, col0;  /* global offset of the shard in the last two dims (the block phase) */
+  uint32_t granularity; /* TSB_SCALE_PER_BLOCK, TSB_SCALE_PER_CHANNEL or TSB_SCALE_PER_TENSOR */
+  uint32_t pad;         /* 0 */
+} tsb_dq_source_t;
+
+/* Compile a dequantising pull: `rects` are ordinary source -> destination rectangles with src_dtype
+ * == TSB_F8E4M3, dst_dtype in {TSB_F32, TSB_BF16, TSB_F16} and src inside one source (TSB_ERR_INVALID
+ * naming the rect or source otherwise).  Elements no rect reads are left alone.  The result is a plan
+ * like any other.  flags: reserved, pass 0. */
+int tsb_dequant_fp8_plan_create(int device, const tsb_rect_t* rects, uint64_t n, const tsb_dq_source_t* sources,
+                                uint64_t n_sources, uint32_t flags, tsb_plan_t* out);
+/* Host-only (no CUDA call): compile and copy the tile table out (one CTA per tile).  out_tiles: records
+ * of 56 bytes
+ *   {u64 src, u64 dst, u64 scale, i64 src_row_stride_bytes, i64 dst_row_stride_bytes, u32 rows, u32 cols,
+ *    u16 scale_step_bytes, u8 dst_dtype, u8 vector, u32 pad}
+ * (scale: the float32 scale of the tile's first row; scale_step_bytes: 4 per channel, else 0; vector:
+ * 16-byte accesses on both sides).  A NULL table only reports its count. */
+int tsb_dequant_fp8_compile_host(int device, const tsb_rect_t* rects, uint64_t n, const tsb_dq_source_t* sources,
+                                 uint64_t n_sources, uint32_t flags, void* out_tiles, uint64_t tile_cap,
+                                 uint64_t* out_n_tiles);
 
 /* ------------------------------------------------------------------------------------------ */
 /* streams and events (the await points of the reference's coroutines)                         */

@@ -16,7 +16,7 @@ import torch
 from torchstore_b200._build import LIB_PATH
 
 TSB_MAX_DIMS = 6
-TSB_ABI_VERSION = 5
+TSB_ABI_VERSION = 6
 
 TSB_OK, TSB_ERR_INVALID, TSB_ERR_CUDA, TSB_ERR_UNSUPPORTED, TSB_ERR_NOMEM, TSB_ERR_NOTFOUND = range(6)
 
@@ -113,6 +113,25 @@ class SqTarget(C.Structure):
     ]
 
 
+TSB_SCALE_PER_BLOCK = 3
+
+
+class DqSource(C.Structure):
+    """tsb_dq_source_t: one block-, channel- or tensor-scaled fp8 source shard of a dequantising pull."""
+
+    _fields_ = [
+        ("src", C.c_uint64),
+        ("scale", C.c_uint64),
+        ("batch", C.c_uint64),
+        ("rows", C.c_uint64),
+        ("cols", C.c_uint64),
+        ("row0", C.c_uint64),
+        ("col0", C.c_uint64),
+        ("granularity", C.c_uint32),
+        ("pad", C.c_uint32),
+    ]
+
+
 class ArenaStats(C.Structure):
     _fields_ = [
         ("capacity", C.c_uint64),
@@ -170,6 +189,14 @@ _SIGNATURES = {
         C.c_int,
         [C.c_int, C.POINTER(Rect), C.c_uint64, C.POINTER(SqTarget), C.c_uint64, C.c_uint32, _vp, C.c_uint64,
          C.POINTER(C.c_uint64), _vp, C.c_uint64, C.POINTER(C.c_uint64), _vp, C.c_uint64, C.POINTER(C.c_uint64),
+         C.POINTER(C.c_uint64)],
+    ),
+    "tsb_dequant_fp8_plan_create": (
+        C.c_int, [C.c_int, C.POINTER(Rect), C.c_uint64, C.POINTER(DqSource), C.c_uint64, C.c_uint32, C.POINTER(C.c_uint64)],
+    ),
+    "tsb_dequant_fp8_compile_host": (
+        C.c_int,
+        [C.c_int, C.POINTER(Rect), C.c_uint64, C.POINTER(DqSource), C.c_uint64, C.c_uint32, _vp, C.c_uint64,
          C.POINTER(C.c_uint64)],
     ),
     "tsb_stream_create": (C.c_int, [C.c_int, C.POINTER(_vp)]),
@@ -484,6 +511,34 @@ def scaled_fp8_compile_host(device: int, rects, n: int, targets, n_targets: int)
                                         C.byref(nb), pieces.ctypes.data, npc.value, C.byref(npc), tiles.ctypes.data,
                                         nt.value, C.byref(nt), C.byref(ng)))
     return bands[: nb.value], pieces[: npc.value], tiles[: nt.value], int(ng.value)
+
+
+def make_dq_source_array(n: int):
+    return (DqSource * n)()
+
+
+def dequant_fp8_plan_create(device: int, rects, n: int, sources, n_sources: int) -> int:
+    out = C.c_uint64(0)
+    check(lib().tsb_dequant_fp8_plan_create(device, rects, n, sources, n_sources, 0, C.byref(out)))
+    return int(out.value)
+
+
+# record layout of tsb_dequant_fp8_compile_host (include/tstore_b200.h)
+DQ_TILE_DTYPE = [("src", "<u8"), ("dst", "<u8"), ("scale", "<u8"), ("src_stride", "<i8"), ("dst_stride", "<i8"),
+                 ("rows", "<u4"), ("cols", "<u4"), ("scale_step", "<u2"), ("dst_dtype", "u1"), ("vec", "u1"),
+                 ("pad", "<u4")]
+
+
+def dequant_fp8_compile_host(device: int, rects, n: int, sources, n_sources: int):
+    """Host-only compilation of a dequantising pull -> its tile table as a numpy record array."""
+    import numpy as np
+
+    nt = C.c_uint64(0)
+    L = lib()
+    check(L.tsb_dequant_fp8_compile_host(device, rects, n, sources, n_sources, 0, None, 0, C.byref(nt)))
+    tiles = np.zeros(max(1, nt.value), dtype=DQ_TILE_DTYPE)
+    check(L.tsb_dequant_fp8_compile_host(device, rects, n, sources, n_sources, 0, tiles.ctypes.data, nt.value, C.byref(nt)))
+    return tiles[: nt.value]
 
 
 CUDA_STREAM_LEGACY = 0x1  # cudaStreamLegacy: an explicit handle for the default stream

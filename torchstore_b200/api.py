@@ -156,10 +156,14 @@ async def exists(key: str, store_name: str = DEFAULT_TORCHSTORE_NAME) -> bool:
 
 
 async def put_state_dict(state_dict: dict[str, Any] | None, key: str, store_name: str = DEFAULT_TORCHSTORE_NAME,
-                         direct_rdma: bool = False, transfer_dtype: "torch.dtype | None" = None) -> None:
+                         direct_rdma: bool = False, transfer_dtype: "torch.dtype | None" = None,
+                         block_scales: "dict[str, torch.Tensor] | None" = None,
+                         channel_scales: "dict[str, torch.Tensor] | None" = None,
+                         tensor_scales: "dict[str, torch.Tensor] | None" = None) -> None:
     cl = await client(store_name)
     await state_dict_utils.put_state_dict(store=cl, state_dict=state_dict, key=key, direct_rdma=direct_rdma,
-                                          transfer_dtype=transfer_dtype)
+                                          transfer_dtype=transfer_dtype, block_scales=block_scales,
+                                          channel_scales=channel_scales, tensor_scales=tensor_scales)
 
 
 async def get_state_dict(key: str, user_state_dict: dict[str, Any] | None = None, strict: bool = True,

@@ -35,39 +35,57 @@ uint32_t quant_src_bytes(uint32_t dt) {
 
 namespace {
 
+// A dim of a rect: extent, the step on the side that is not the fp8 grid (ss), the step on the grid (ds).
 struct Dim {
   int64_t e, ss, ds;
 };
 
-}  // namespace
+// What differs between mapping a rect by its destination (quantising pulls) or by its source
+// (dequantising pulls).
+struct Side {
+  bool by_src;            // the fp8 grid is the rect's source
+  const char* no_grid;    // the grid pointer lies in no grid
+  const char* not_a_box;  // its grid strides describe no box
+  int contig_code;        // the other side's columns are strided
+  const char* contig;
+  const char* unaligned;  // the other side is not aligned to its element size
+};
 
-int rect_boxes(const tsb_rect_t& in, uint64_t index, const TargetGeom* targets, uint64_t n_targets,
-               std::vector<TargetBox>* out) {
+constexpr Side kByDst{false, "dst is inside no target", "its destination strides do not describe a box of the target",
+                      TSB_ERR_UNSUPPORTED, "scaled fp8 pulls read contiguous source rows",
+                      "source not aligned to its element size"};
+constexpr Side kBySrc{true, "src is inside no source", "its source strides do not describe a box of the source",
+                      TSB_ERR_INVALID, "dequantising pulls write contiguous destination rows",
+                      "destination not aligned to its element size"};
+
+// The mapping of rect_boxes / rect_source_boxes once the dtypes are checked; `es` is the element size
+// of the side that is not the grid.
+int map_boxes(const tsb_rect_t& in, uint64_t index, const TargetGeom* targets, uint64_t n_targets, const Side& side,
+              uint32_t es, std::vector<TargetBox>* out) {
   const std::string where = "rect " + std::to_string(index) + ": ";
-  if (in.ndim < 1 || in.ndim > TSB_MAX_DIMS) return fail(TSB_ERR_INVALID, where + "ndim must be in [1, 6]");
-  const uint32_t es = quant_src_bytes(in.src_dtype);
-  if (!es) return fail(TSB_ERR_UNSUPPORTED, where + "scaled fp8 pulls read f32, bf16 or f16 sources");
-  if (in.dst_dtype != TSB_F8E4M3) return fail(TSB_ERR_UNSUPPORTED, where + "scaled fp8 destinations are float8_e4m3fn");
   std::vector<Dim> work;
   for (uint32_t i = 0; i < in.ndim; ++i) {
     if (in.extent[i] < 0) return fail(TSB_ERR_INVALID, where + "negative extent");
     if (in.extent[i] == 0) return TSB_OK;
-    if (in.extent[i] > 1) work.push_back({in.extent[i], in.src_stride[i], in.dst_stride[i]});
+    if (in.extent[i] > 1)
+      work.push_back(side.by_src ? Dim{in.extent[i], in.dst_stride[i], in.src_stride[i]}
+                                 : Dim{in.extent[i], in.src_stride[i], in.dst_stride[i]});
   }
   if (in.src == 0 || in.dst == 0) return fail(TSB_ERR_INVALID, where + "NULL src/dst");
+  const uint64_t grid_ptr = side.by_src ? in.src : in.dst, other_ptr = side.by_src ? in.dst : in.src;
   uint64_t t = 0;
-  while (t < n_targets && !(in.dst >= targets[t].dst && in.dst - targets[t].dst < targets[t].batch * targets[t].rows * targets[t].cols)) ++t;
-  if (t == n_targets) return fail(TSB_ERR_INVALID, where + "dst is inside no target");
+  while (t < n_targets && !(grid_ptr >= targets[t].dst && grid_ptr - targets[t].dst < targets[t].batch * targets[t].rows * targets[t].cols)) ++t;
+  if (t == n_targets) return fail(TSB_ERR_INVALID, where + side.no_grid);
   const int64_t R = static_cast<int64_t>(targets[t].rows), C = static_cast<int64_t>(targets[t].cols);
   const int64_t B = static_cast<int64_t>(targets[t].batch);
-  const uint64_t o = in.dst - targets[t].dst;
+  const uint64_t o = grid_ptr - targets[t].dst;
   const int64_t b0 = static_cast<int64_t>(o / (R * C)), r0 = static_cast<int64_t>(o % (R * C)) / C, c0 = static_cast<int64_t>(o % C);
-  // Classify every dim by its destination step: columns (1), rows (C) or whole matrices (multiple of
+  // Classify every dim by its grid step: columns (1), rows (C) or whole matrices (multiple of
   // R*C).  A collapsed dim that runs past the end of a row (or of a matrix) is split back.
   int64_t er = 1, ec = 1, row_ss = 0, col_ss = es;
   bool have_row = false, have_col = false;
   std::vector<Dim> batch;
-  const std::string bad = where + "its destination strides do not describe a box of the target";
+  const std::string bad = where + side.not_a_box;
   while (!work.empty()) {
     const Dim d = work.back();
     work.pop_back();
@@ -104,11 +122,10 @@ int rect_boxes(const tsb_rect_t& in, uint64_t index, const TargetGeom* targets, 
   int64_t b_last = b0;
   for (const Dim& d : batch) b_last += (d.e - 1) * d.ds;
   if (b_last >= B) return fail(TSB_ERR_INVALID, bad);
-  if (have_col && col_ss != static_cast<int64_t>(es))
-    return fail(TSB_ERR_UNSUPPORTED, where + "scaled fp8 pulls read contiguous source rows");
-  if (in.src % es || row_ss % es) return fail(TSB_ERR_INVALID, where + "source not aligned to its element size");
+  if (have_col && col_ss != static_cast<int64_t>(es)) return fail(side.contig_code, where + side.contig);
+  if (other_ptr % es || row_ss % es) return fail(TSB_ERR_INVALID, where + side.unaligned);
   for (const Dim& d : batch)
-    if (d.ss % es) return fail(TSB_ERR_INVALID, where + "source not aligned to its element size");
+    if (d.ss % es) return fail(TSB_ERR_INVALID, where + side.unaligned);
   // one box per combination of the batch dims
   std::vector<int64_t> k(batch.size(), 0);
   while (true) {
@@ -117,13 +134,36 @@ int rect_boxes(const tsb_rect_t& in, uint64_t index, const TargetGeom* targets, 
       b += k[i] * batch[i].ds;
       so += k[i] * batch[i].ss;
     }
-    out->push_back({in.src + static_cast<uint64_t>(so), row_ss, t, static_cast<uint64_t>(b), static_cast<uint64_t>(r0),
-                    static_cast<uint64_t>(c0), static_cast<uint64_t>(er), static_cast<uint64_t>(ec), in.src_dtype, in.src_device});
+    out->push_back({other_ptr + static_cast<uint64_t>(so), row_ss, t, static_cast<uint64_t>(b), static_cast<uint64_t>(r0),
+                    static_cast<uint64_t>(c0), static_cast<uint64_t>(er), static_cast<uint64_t>(ec),
+                    side.by_src ? in.dst_dtype : in.src_dtype, in.src_device});
     size_t i = batch.size();
     while (i > 0 && ++k[i - 1] == batch[i - 1].e) k[--i] = 0;
     if (i == 0) break;
   }
   return TSB_OK;
+}
+
+}  // namespace
+
+int rect_boxes(const tsb_rect_t& in, uint64_t index, const TargetGeom* targets, uint64_t n_targets,
+               std::vector<TargetBox>* out) {
+  const std::string where = "rect " + std::to_string(index) + ": ";
+  if (in.ndim < 1 || in.ndim > TSB_MAX_DIMS) return fail(TSB_ERR_INVALID, where + "ndim must be in [1, 6]");
+  const uint32_t es = quant_src_bytes(in.src_dtype);
+  if (!es) return fail(TSB_ERR_UNSUPPORTED, where + "scaled fp8 pulls read f32, bf16 or f16 sources");
+  if (in.dst_dtype != TSB_F8E4M3) return fail(TSB_ERR_UNSUPPORTED, where + "scaled fp8 destinations are float8_e4m3fn");
+  return map_boxes(in, index, targets, n_targets, kByDst, es, out);
+}
+
+int rect_source_boxes(const tsb_rect_t& in, uint64_t index, const TargetGeom* grids, uint64_t n_grids,
+                      std::vector<TargetBox>* out) {
+  const std::string where = "rect " + std::to_string(index) + ": ";
+  if (in.ndim < 1 || in.ndim > TSB_MAX_DIMS) return fail(TSB_ERR_INVALID, where + "ndim must be in [1, 6]");
+  if (in.src_dtype != TSB_F8E4M3) return fail(TSB_ERR_INVALID, where + "dequantising pulls read float8_e4m3fn sources");
+  const uint32_t es = quant_src_bytes(in.dst_dtype);
+  if (!es) return fail(TSB_ERR_INVALID, where + "dequantising pulls write f32, bf16 or f16 destinations");
+  return map_boxes(in, index, grids, n_grids, kBySrc, es, out);
 }
 
 int block_fp8_compile(int device, const tsb_rect_t* rects, uint64_t n, const tsb_bq_target_t* targets, uint64_t n_targets,

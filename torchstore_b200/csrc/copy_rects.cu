@@ -153,23 +153,11 @@ struct CastHalfV8 {
 struct F8E4M3 { unsigned char x; };
 struct F8E5M2 { unsigned char x; };
 
-// The e4m3fn / e5m2 narrowing (f32x2_to_fp8x2, fp8_fix) lives in fp8_cvt.cuh.
-// two fp8 bytes (bits 0..15) -> f16x2 (exact: every fp8 value is an f16 value)
-template <bool kE4M3>
-__device__ __forceinline__ uint32_t fp8x2_to_f16x2(uint32_t two) {
-  uint32_t r;
-  const unsigned short b = static_cast<unsigned short>(two);
-  if (kE4M3) asm("cvt.rn.f16x2.e4m3x2 %0, %1;" : "=r"(r) : "h"(b));
-  else asm("cvt.rn.f16x2.e5m2x2 %0, %1;" : "=r"(r) : "h"(b));
-  return r;
-}
+// The e4m3fn / e5m2 narrowing (f32x2_to_fp8x2, fp8_fix), the fp8 widening (fp8x2_to_f16x2) and the
+// f32 -> bf16 narrowing (float_to_bf16_bits) live in fp8_cvt.cuh.
 __device__ __forceinline__ float f16_bits_to_float(uint32_t bits16) {
   unsigned short b = static_cast<unsigned short>(bits16);
   return __half2float(*reinterpret_cast<__half*>(&b));
-}
-__device__ __forceinline__ uint32_t float_to_bf16_bits(float f) {
-  __nv_bfloat16 h = __float2bfloat16_rn(f);
-  return *reinterpret_cast<unsigned short*>(&h);
 }
 
 template <> __device__ __forceinline__ F8E4M3 convert<float, F8E4M3>(float v) { return F8E4M3{static_cast<unsigned char>(f32x2_to_fp8x2<true>(__float_as_uint(v), 0u))}; }

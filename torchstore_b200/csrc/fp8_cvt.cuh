@@ -1,7 +1,8 @@
-// f32 -> fp8 narrowing with torch's .to() semantics, shared by the copy kernel (copy_rects.cu) and the
-// block-scaled quantiser (block_fp8.cu).
+// fp8 <-> f32 conversions with torch's .to() semantics, shared by the copy kernel (copy_rects.cu), the
+// scaled quantisers (block_fp8.cu, scaled_fp8.cu) and the dequantiser (dequant_fp8.cu).
 #pragma once
 
+#include <cuda_bf16.h>
 #include <stdint.h>
 
 namespace tsb {
@@ -29,6 +30,22 @@ __device__ __forceinline__ uint32_t f32x2_to_fp8x2(uint32_t lo, uint32_t hi) {
   else
     asm("cvt.rn.satfinite.e5m2x2.f32 %0, %1, %2;" : "=h"(r) : "f"(__uint_as_float(hi)), "f"(__uint_as_float(lo)));
   return fp8_fix<kE4M3>(r & 0xffu, lo) | (fp8_fix<kE4M3>(static_cast<uint32_t>(r) >> 8, hi) << 8);
+}
+
+// two fp8 bytes (bits 0..15) -> f16x2 (exact: every fp8 value is an f16 value)
+template <bool kE4M3>
+__device__ __forceinline__ uint32_t fp8x2_to_f16x2(uint32_t two) {
+  uint32_t r;
+  const unsigned short b = static_cast<unsigned short>(two);
+  if (kE4M3) asm("cvt.rn.f16x2.e4m3x2 %0, %1;" : "=r"(r) : "h"(b));
+  else asm("cvt.rn.f16x2.e5m2x2 %0, %1;" : "=r"(r) : "h"(b));
+  return r;
+}
+
+// f32 -> bf16 bits, round to nearest even (the fused cast's narrowing, NaN bytes included)
+__device__ __forceinline__ uint32_t float_to_bf16_bits(float f) {
+  __nv_bfloat16 h = __float2bfloat16_rn(f);
+  return *reinterpret_cast<unsigned short*>(&h);
 }
 
 }  // namespace tsb

@@ -42,8 +42,9 @@ TableLayout table_layout(size_t n_rects, size_t n_tiles, size_t n_link) {
 
 // What a plan's tables drive: the copy_rects kernel, the block-scaled fp8 quantiser
 // (d_block = {BqBlock table | BqPiece table}, num_tiles = blocks), or the per-channel / per-tensor
-// scaled fp8 quantisers (d_block = {SqBand table | SqPiece table | SqTile table | amax words}).
-enum : uint32_t { PLAN_COPY = 0, PLAN_BLOCK_FP8 = 1, PLAN_SCALED_FP8 = 2 };
+// scaled fp8 quantisers (d_block = {SqBand table | SqPiece table | SqTile table | amax words}), or the
+// dequantiser of scaled fp8 sources (d_block = DqTile table, num_tiles = tiles).
+enum : uint32_t { PLAN_COPY = 0, PLAN_BLOCK_FP8 = 1, PLAN_SCALED_FP8 = 2, PLAN_DEQUANT_FP8 = 3 };
 
 struct Plan {
   int device = 0;
@@ -568,6 +569,7 @@ int run_plan(Plan* p, cudaStream_t s) {
     l.amax = reinterpret_cast<uint32_t*>(p->d_block + p->sq_off[2]);
     return launch_scaled_fp8(l, s);
   }
+  if (p->plan_kind == PLAN_DEQUANT_FP8) return launch_dequant_fp8(reinterpret_cast<const DqTile*>(p->d_block), p->num_tiles, s);
   uint32_t kind = p->kind;
   if (getenv("TSB_FORCE_GENERIC")) kind = KIND_GENERIC;
   LaunchParams lp = make_params(p->d_block, p->layout, p->num_tiles, p->num_link_tiles, kind, p->link_stage_bytes, p->link_stages);
@@ -756,6 +758,30 @@ int tsb_scaled_fp8_plan_create(int device, const tsb_rect_t* rects, uint64_t n, 
   p->sq.n_tiles = static_cast<uint32_t>(tb.tiles.size());
   p->sq.n_groups = tb.n_groups;
   p->sq.stage_bytes = tb.stage_bytes;
+  return register_plan(p, host, out);
+}
+
+int tsb_dequant_fp8_plan_create(int device, const tsb_rect_t* rects, uint64_t n, const tsb_dq_source_t* sources,
+                                uint64_t n_sources, uint32_t flags, tsb_plan_t* out) {
+  if (!out) return fail(TSB_ERR_INVALID, "tsb_dequant_fp8_plan_create: NULL argument");
+  if (flags != 0) return fail(TSB_ERR_INVALID, "tsb_dequant_fp8_plan_create: flags must be 0");
+  DqTables tb;
+  int st = dequant_fp8_compile(device, rects, n, sources, n_sources, &tb);
+  if (st) return st;
+  std::vector<char> host(std::max<size_t>(16, tb.tiles.size() * sizeof(DqTile)), 0);
+  if (!tb.tiles.empty()) memcpy(host.data(), tb.tiles.data(), tb.tiles.size() * sizeof(DqTile));
+  Plan* p = new Plan();
+  p->device = device;
+  p->plan_kind = PLAN_DEQUANT_FP8;
+  p->num_tiles = static_cast<uint32_t>(tb.tiles.size());
+  p->info.num_rects = n;
+  p->info.num_tiles = tb.tiles.size();
+  p->info.payload_bytes = tb.payload_bytes;
+  p->info.src_bytes = tb.src_bytes;
+  p->info.remote_src_bytes = tb.remote_src_bytes;
+  p->info.grid = p->num_tiles;
+  p->info.block = kDqThreads;
+  p->info.tile_bytes = kDqTileElems;
   return register_plan(p, host, out);
 }
 

@@ -176,6 +176,11 @@ uint32_t quant_src_bytes(uint32_t dtype);  // 4 / 2 for TSB_F32 / TSB_BF16, TSB_
 // Append one box per combination of the rect's batch dims to `out` (nothing for an empty rect).
 int rect_boxes(const tsb_rect_t& in, uint64_t index, const TargetGeom* targets, uint64_t n_targets,
                std::vector<TargetBox>* out);
+// The same mapping from the other side: the rect's *source* is located on the fp8 grids (its
+// TargetGeom::dst is the grid's base), and a box's `src` / `row_stride` / `dtype` describe the
+// destination side.  Destination columns must be contiguous.
+int rect_source_boxes(const tsb_rect_t& in, uint64_t index, const TargetGeom* grids, uint64_t n_grids,
+                      std::vector<TargetBox>* out);
 
 // ---- block-scaled fp8 (block_fp8.cu) ---------------------------------------------------------------
 constexpr uint32_t kBqBlock = 128;  // block edge (elements)
@@ -280,5 +285,33 @@ struct SqLaunch {
   uint32_t n_bands, n_tiles, n_groups, stage_bytes;
 };
 int launch_scaled_fp8(const SqLaunch& l, cudaStream_t stream);
+
+// ---- dequantising pulls: scaled fp8 sources -> f32 / bf16 / f16 (dequant_fp8.cu) --------------------
+constexpr uint32_t kDqThreads = 256;
+constexpr uint32_t kDqTileElems = 16384;  // most elements of one tile (one CTA; 4 16-element chunks per thread)
+constexpr uint32_t kDqTileRows = 256;     // most rows of one tile (one staged scale per row)
+
+// A rectangle of one source read under one scale (block, tensor) or one scale per row (channel).
+struct alignas(8) DqTile {
+  uint64_t src;          // fp8 element (0, 0) of the tile
+  uint64_t dst;          // its destination element
+  uint64_t scale;        // float32 scale of row 0
+  int64_t src_stride;    // bytes between source rows
+  int64_t dst_stride;    // bytes between destination rows
+  uint32_t rows, cols;
+  uint16_t scale_step;   // bytes between the scales of consecutive rows: 4 (channel) or 0
+  uint8_t dst_dtype;     // TSB_F32 / TSB_BF16 / TSB_F16
+  uint8_t vec;           // 1: source and destination rows start 16-byte aligned (16-element chunks vectorise)
+  uint32_t pad_;
+};
+static_assert(sizeof(DqTile) == 56, "DqTile is part of tsb_dequant_fp8_compile_host's output");
+
+struct DqTables {
+  std::vector<DqTile> tiles;
+  uint64_t src_bytes = 0, remote_src_bytes = 0, payload_bytes = 0;
+};
+int dequant_fp8_compile(int device, const tsb_rect_t* rects, uint64_t n, const tsb_dq_source_t* sources,
+                        uint64_t n_sources, DqTables* out);
+int launch_dequant_fp8(const DqTile* tiles, uint32_t n_tiles, cudaStream_t stream);
 
 }  // namespace tsb

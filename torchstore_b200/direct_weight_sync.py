@@ -132,6 +132,69 @@ class NvlinkBuffer:
         self._keepalive = None
 
 
+class ScaledNvlinkBuffer(NvlinkBuffer):
+    """An :class:`NvlinkBuffer` over a scaled ``float8_e4m3fn`` weight shard that also carries its
+    float32 scale (the dequantisation multiplier: ``weight_scale_inv`` per 128x128 block, ``weight_scale``
+    per channel or per tensor), the granularity, and the shard's global offset ``(row0, col0)`` in the last
+    two dims, which anchors the blocks at the global origin.  Pickles to plain data.  ``read_into`` /
+    ``write_from`` move the raw fp8 bytes; a pull into a bf16/f16/f32 destination dequantises."""
+
+    def __init__(self, tensor: torch.Tensor | None = None, scale: torch.Tensor | None = None, granularity: str = "",
+                 row0: int = 0, col0: int = 0, *, descriptor: HbmDescriptor | None = None,
+                 scale_descriptor: HbmDescriptor | None = None):
+        super().__init__(tensor, descriptor=descriptor)
+        if granularity not in GRANULARITIES:
+            raise ValueError(f"granularity must be one of {sorted(GRANULARITIES)}, not {granularity!r}")
+        self.scale_descriptor = scale_descriptor if scale_descriptor is not None else HbmDescriptor.from_tensor(scale)
+        self.granularity = granularity
+        self.row0, self.col0 = int(row0), int(col0)
+        self._scale_keepalive = scale
+
+    def __getstate__(self):
+        return {"descriptor": self.descriptor, "scale_descriptor": self.scale_descriptor,
+                "granularity": self.granularity, "row0": self.row0, "col0": self.col0}
+
+    def __setstate__(self, state):
+        super().__setstate__(state)
+        self.scale_descriptor = state["scale_descriptor"]
+        self.granularity = state["granularity"]
+        self.row0, self.col0 = state["row0"], state["col0"]
+        self._scale_keepalive = None
+
+    def scale_window(self, device: int) -> StridedMem:
+        """The scale tensor as seen from ``device``."""
+        return self.scale_descriptor.resolve(device)
+
+    async def drop(self) -> None:
+        await super().drop()
+        try:
+            self.scale_descriptor.release()
+        except Exception as e:
+            logger.warning("ScaledNvlinkBuffer.drop failed to release the scale: %s", e)
+        self._scale_keepalive = None
+
+
+# granularity of a scaled source handle: register() keyword -> (name, native code)
+_SOURCE_SCALES = {
+    "block_scales": ("block", _native.TSB_SCALE_PER_BLOCK),
+    "channel_scales": ("channel", _native.TSB_SCALE_PER_CHANNEL),
+    "tensor_scales": ("tensor", _native.TSB_SCALE_PER_TENSOR),
+}
+GRANULARITIES = {g: code for g, code in _SOURCE_SCALES.values()}
+DEQUANT_DEST_DTYPES = {torch.bfloat16, torch.float16, torch.float32}
+
+
+def source_scale_shapes(granularity: str, shape: tuple, row0: int, col0: int) -> list[tuple]:
+    """Accepted shapes of the scale of a ``shape`` fp8 shard at global offset (row0, col0) in its last
+    two dims: exactly the groups the shard touches, anchored at the global origin."""
+    lead, (n, k) = tuple(shape[:-2]), tuple(shape[-2:])
+    if granularity == "block":
+        return [lead + (-(-(row0 + n) // BLOCK) - row0 // BLOCK, -(-(col0 + k) // BLOCK) - col0 // BLOCK)]
+    if granularity == "channel":
+        return [lead + (n, 1)]
+    return [lead, lead + (1,)]
+
+
 @dataclass
 class RDMAWeightHandle:
     """Serializable handle to one weight shard (same fields as the reference)."""
@@ -139,6 +202,11 @@ class RDMAWeightHandle:
     rdma_buffer: object  # NvlinkBuffer
     tensor_slice: TensorSlice  # shard position in the global tensor
     source_rank: int
+
+
+def _last_two_offsets(tslice: TensorSlice) -> tuple[int, int]:
+    """Global (row, column) offset of a shard in its last two dims."""
+    return int(tslice.offsets[-2]), int(tslice.offsets[-1])
 
 
 def _request_to_slice(req: Request, param: torch.Tensor) -> TensorSlice:
@@ -173,11 +241,25 @@ class DirectWeightSyncSource:
 
     def register(self, state_dict: dict[str, torch.Tensor], rank: int,
                  transfer_dtype: torch.dtype | None = None,
-                 tensor_slices: dict[str, TensorSlice] | None = None) -> dict[str, RDMAWeightHandle]:
+                 tensor_slices: dict[str, TensorSlice] | None = None, *,
+                 block_scales: dict[str, torch.Tensor] | None = None,
+                 channel_scales: dict[str, torch.Tensor] | None = None,
+                 tensor_scales: dict[str, torch.Tensor] | None = None) -> dict[str, RDMAWeightHandle]:
         """Create a handle for every entry of ``state_dict`` (tensors or DTensors).
 
         ``tensor_slices`` (extension) gives the global rectangle of *plain* local shards for
-        callers that do not wrap them in DTensors."""
+        callers that do not wrap them in DTensors.
+
+        Scaled fp8 sources (extension): a ``float8_e4m3fn`` weight named in one of ``block_scales``
+        (float32 ``weight_scale_inv`` per 128x128 block), ``channel_scales`` (``weight_scale`` per row)
+        or ``tensor_scales`` (one per matrix) is published with its scale, so that a pull into a bf16, f16
+        or f32 destination dequantises it (DESIGN.md section 4).  Scales are anchored at the global
+        origin: a shard at global offset (r0, c0) of its last two dims carries exactly the groups it
+        touches (:func:`source_scale_shapes`).  Such weights are registered zero-copy.  Everything is
+        validated before anything is exported, so a failed call registers nothing."""
+        scaled = self._check_source_scales(state_dict, transfer_dtype, tensor_slices,
+                                           {"block_scales": block_scales, "channel_scales": channel_scales,
+                                            "tensor_scales": tensor_scales})
         handles: dict[str, RDMAWeightHandle] = {}
         self._refresh_plans.close()
         self._staging = {}
@@ -191,6 +273,12 @@ class DirectWeightSyncSource:
             if not local.is_cuda:
                 raise RuntimeError(f"direct weight sync registers GPU memory; '{name}' is on {local.device}")
             devices.add(local.device.index)
+            if name in scaled:
+                granularity, scale = scaled[name]
+                handles[name] = RDMAWeightHandle(
+                    rdma_buffer=ScaledNvlinkBuffer(local, scale, granularity, *_last_two_offsets(tslice)),
+                    tensor_slice=tslice, source_rank=rank)
+                continue
             if transfer_dtype is not None:
                 staging = torch.empty(local.shape, dtype=transfer_dtype, device=local.device)
                 self._staging[name] = (staging, local)
@@ -216,6 +304,53 @@ class DirectWeightSyncSource:
         logger.info("Registered %d NVLink handles (%d staged, %d direct)", len(handles), len(self._staging),
                     len(handles) - len(self._staging))
         return handles
+
+    @staticmethod
+    def _check_source_scales(state_dict, transfer_dtype, tensor_slices, scales: dict[str, dict | None]) -> dict[str, tuple]:
+        """Validate the scale dicts of :meth:`register` -> ``{name: (granularity, scale)}``.  Raises before
+        anything is exported."""
+        from torch.distributed.tensor import DTensor
+
+        seen: set[str] = set()
+        for kw, by_name in scales.items():
+            for name in by_name or {}:
+                if name not in state_dict:
+                    raise ValueError(f"{kw} names '{name}', which is not in the state dict")
+                if name in seen:
+                    raise ValueError(f"'{name}' is in more than one of block_scales, channel_scales and tensor_scales")
+                seen.add(name)
+        if seen and transfer_dtype is not None:
+            raise ValueError("scaled fp8 weights are published as they are: block_scales, channel_scales and "
+                             "tensor_scales cannot be combined with transfer_dtype")
+        out: dict[str, tuple] = {}
+        for kw, by_name in scales.items():
+            granularity = _SOURCE_SCALES[kw][0]
+            for name, scale in (by_name or {}).items():
+                req = Request.from_any(name, state_dict[name], tensor_slices.get(name) if tensor_slices else None)
+                w = req.tensor_val
+                if w.dtype != torch.float8_e4m3fn:
+                    raise TypeError(f"scaled weight '{name}' ({kw}) must be float8_e4m3fn, not {w.dtype}")
+                if w.dim() < 2 or w.numel() == 0 or not w.is_contiguous() or not w.is_cuda:
+                    raise ValueError(f"scaled weight '{name}' must be a non-empty contiguous CUDA tensor with at least "
+                                     f"2 dims; got shape {tuple(w.shape)}, strides {w.stride()} on {w.device}")
+                if isinstance(scale, DTensor):
+                    raise TypeError(
+                        f"the scale of '{name}' ({kw}) is a DTensor; pass the local scale of this shard as a plain "
+                        "tensor.  Scales are anchored at the global origin and must hold exactly the groups the "
+                        "local weight shard touches; sharding a scale tensor on its own gives local shapes that can "
+                        "match while covering the wrong groups")
+                if not isinstance(scale, torch.Tensor) or scale.dtype != torch.float32:
+                    what = type(scale).__name__ if not isinstance(scale, torch.Tensor) else str(scale.dtype)
+                    raise TypeError(f"the scale of '{name}' ({kw}) must be a plain float32 tensor, not {what}")
+                r0, c0 = _last_two_offsets(_request_to_slice(req, state_dict[name]))
+                wants = source_scale_shapes(granularity, tuple(w.shape), r0, c0)
+                if tuple(scale.shape) not in wants or not scale.is_contiguous() or scale.device != w.device:
+                    want = " or ".join(map(str, wants))
+                    raise ValueError(f"the scale of '{name}' ({kw}, shard at global offset ({r0}, {c0})) must be a "
+                                     f"contiguous {want} tensor on {w.device}; got {tuple(scale.shape)}, strides "
+                                     f"{scale.stride()} on {scale.device}")
+                out[name] = (granularity, scale)
+        return out
 
     def refresh(self) -> int:
         """Re-cast the source params into their staging buffers (no-op without transfer_dtype).
@@ -288,6 +423,7 @@ class DirectWeightSyncDest:
         self._native_plans = Plans()  # the compiled plan, one native plan per destination device
         self._block_plans = Plans()  # block-scaled fp8 names: one quantising plan per destination device
         self._scaled_plans = Plans()  # per-channel / per-tensor scaled fp8 names: likewise
+        self._dequant_plans = Plans()  # names read from scaled fp8 handles into bf16/f16/f32: one dequantising plan per device
         self._scale_keys: frozenset = frozenset()  # (name, scale keyword) pairs the cached plan quantises
         self._plan_scale_dicts: tuple | None = None  # the three scale dict objects of the last pull
         self.last_pull_ms: dict[int, float] = {}  # device -> kernel time of the last pull
@@ -417,9 +553,39 @@ class DirectWeightSyncDest:
                 out[name] = (kw, dest, scale)
         return out
 
-    def _compile(self, scaled: dict | None = None) -> None:
+    @staticmethod
+    def _check_dequant(all_handles, dest_state_dict, scaled_dests) -> set[str]:
+        """Names whose handles are scaled fp8 sources and whose destination is bf16/f16/f32: the
+        dequantising plan.  A float8_e4m3fn destination gets the plain byte move.  Raises before anything
+        is compiled or launched."""
+        out = set()
+        for name, param in dest_state_dict.items():
+            handles = all_handles.get(name) or []
+            kinds = {getattr(h.rdma_buffer, "granularity", None) for h in handles}
+            if not handles or kinds == {None}:
+                continue
+            if None in kinds:
+                raise ValueError(f"the handles of '{name}' mix scaled fp8 and unscaled sources")
+            if len(kinds) > 1:
+                raise ValueError(f"the handles of '{name}' mix scale granularities {sorted(kinds)}")
+            if name in scaled_dests:
+                continue  # a scaled destination: _check_scales refuses fp8 handles with its TypeError
+            dest = getattr(param, "_local_tensor", param)
+            if dest.dtype == torch.float8_e4m3fn:
+                continue
+            if dest.dtype not in DEQUANT_DEST_DTYPES:
+                raise TypeError(f"'{name}' has {kinds.pop()}-scaled fp8 handles: its destination must be bfloat16, "
+                                f"float16, float32 (dequantised) or float8_e4m3fn (bytes moved), not {dest.dtype}")
+            if dest.dim() < 2 or not dest.is_contiguous():
+                raise ValueError(f"dequantised destination '{name}' must be contiguous with at least 2 dims; got shape "
+                                 f"{tuple(dest.shape)}, strides {dest.stride()}")
+            out.add(name)
+        return out
+
+    def _compile(self, scaled: dict | None = None, dequant: set | None = None) -> None:
         per_device: dict[int, list] = defaultdict(list)
         quant_pairs: dict[tuple, list] = defaultdict(list)  # (device, block?) -> windows of the quantising plans
+        dq: dict[int, tuple[list, dict]] = {}  # device -> (windows, {source buffer id: (index, DqSource)})
         for op in self._plan:
             dest = op.dest_local
             if not dest.is_cuda:
@@ -435,9 +601,32 @@ class DirectWeightSyncDest:
             window = self.op_windows(op, op.rdma_buffer.window(dev))
             if scaled and op.name in scaled:
                 quant_pairs[(dev, scaled[op.name][0] == "block_scales")].append(window)
+            elif dequant and op.name in dequant:
+                pairs, sources = dq.setdefault(dev, ([], {}))
+                pairs.append(window)
+                buf = op.rdma_buffer
+                if id(buf) not in sources:
+                    w, s = buf.window(dev), buf.scale_window(dev)
+                    rows, cols = w.shape[-2:]
+                    sources[id(buf)] = (op.name, _native.DqSource(w.ptr, s.ptr, w.numel // (rows * cols), rows, cols,
+                                                                  buf.row0, buf.col0, GRANULARITIES[buf.granularity], 0))
             else:
                 per_device[dev].append(window)
         self._native_plans = Plans.build(per_device)
+        try:
+            for dev, (pairs, sources) in dq.items():
+                names = [n for n, _ in sources.values()]
+                try:
+                    self._dequant_plans.update(Plans.build_dequant_fp8({dev: (pairs, [s for _, s in sources.values()])}))
+                except _native.TsbError as e:
+                    m = re.search(r"source (\d+)", str(e))
+                    if e.code == _native.TSB_ERR_INVALID and m:
+                        raise ValueError(f"dequantising pull of '{names[int(m.group(1))]}': {e}") from e
+                    raise
+        except BaseException:
+            self._dequant_plans.close()
+            self._native_plans.close()
+            raise
         if not scaled:
             return
         try:
@@ -469,6 +658,7 @@ class DirectWeightSyncDest:
         except BaseException:
             self._block_plans.close()
             self._scaled_plans.close()
+            self._dequant_plans.close()
             self._native_plans.close()
             raise
 
@@ -496,6 +686,13 @@ class DirectWeightSyncDest:
         ``lead`` is the destination's dims before the last two (MoE stacks quantise every matrix on its
         own).  The formula is in DESIGN.md section 4.  Every element of such a destination must be
         covered by the handles.  The other names are pulled as without scales.
+
+        Scaled fp8 sources (extension): a name whose handles were registered with scales
+        (``DirectWeightSyncSource.register(block_scales= / channel_scales= / tensor_scales=)``) and whose
+        destination is bf16, f16 or f32 is dequantised during the pull, each element with the scale of
+        the handle its bytes are read from: ``(q.float() * scale).to(dst)``.  Elements the handles do not
+        cover are left alone.  A float8_e4m3fn destination not named in a scale dict gets the raw fp8
+        bytes; the caller moves the scales separately (for example as their own state-dict entries).
 
         Steady state costs one native call to launch and a poll loop: the cached plan is checked
         against the destination OBJECTS first (their ids; the plan keeps them alive), the kernel
@@ -532,9 +729,10 @@ class DirectWeightSyncDest:
             verified = True
         if self._plan is None:
             scaled = self._check_scales(all_handles, dest_state_dict, dict(zip(SCALE_KINDS, scales))) if keys else None
+            dequant = self._check_dequant(all_handles, dest_state_dict, {n for n, _ in keys})
             self._plan = self._build_plan(all_handles, dest_state_dict, dest_slices)
             try:
-                self._compile(scaled)
+                self._compile(scaled, dequant)
             except BaseException:
                 self._plan = None
                 raise
@@ -563,12 +761,14 @@ class DirectWeightSyncDest:
             self._block_plans.launch()
         if self._scaled_plans:
             self._scaled_plans.launch()
+        if self._dequant_plans:
+            self._dequant_plans.launch()
 
     async def wait(self) -> None:
         await self._native_plans.wait()
         ms = self._native_plans.elapsed_ms()
         # the plans of a device run back to back on its copy stream
-        for plans in (self._block_plans, self._scaled_plans):
+        for plans in (self._block_plans, self._scaled_plans, self._dequant_plans):
             if plans:
                 await plans.wait()
                 for dev, t in plans.elapsed_ms().items():
@@ -579,6 +779,7 @@ class DirectWeightSyncDest:
         self._native_plans.close()
         self._block_plans.close()
         self._scaled_plans.close()
+        self._dequant_plans.close()
         self._scale_keys = frozenset()
         self._plan = None
         self._plan_ids = self._plan_refs = self._plan_dict = self._plan_scale_dicts = None

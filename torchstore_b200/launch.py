@@ -124,6 +124,23 @@ class Plans(dict):
             raise
         return plans
 
+    @classmethod
+    def build_dequant_fp8(cls, per_device: dict[int, tuple[list, list]]) -> "Plans":
+        """Compile dequantising pulls of scaled fp8 sources: ``{device: ([(src, dst) StridedMem windows],
+        [DqSource])}``."""
+        plans = cls()
+        try:
+            for dev, (pairs, sources) in per_device.items():
+                rects, n = build_rects(pairs)
+                arr = _native.make_dq_source_array(max(1, len(sources)))
+                for i, s in enumerate(sources):
+                    arr[i] = s
+                plans[dev] = _native.dequant_fp8_plan_create(dev, rects, n, arr, len(sources))
+        except BaseException:
+            plans.close()
+            raise
+        return plans
+
     def launch(self, fence_out: bool = True) -> None:
         """Enqueue every plan on its device's copy stream, fenced in against the caller's current
         stream of that device.  ``fence_out=False``: the caller's stream is not made to wait for the

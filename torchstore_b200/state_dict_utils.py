@@ -56,15 +56,23 @@ def reset_direct_cache(store=None) -> None:
                 src._refresh_plans.close()
 
 
-async def put_state_dict(store, state_dict, key, direct_rdma=False, transfer_dtype=None):
+async def put_state_dict(store, state_dict, key, direct_rdma=False, transfer_dtype=None, block_scales: dict | None = None,
+                         channel_scales: dict | None = None, tensor_scales: dict | None = None):
     """Store every leaf of ``state_dict`` (one batched put), then the mapping as the commit marker.
 
     With ``direct_rdma=True`` only handles to the caller's HBM are published on the first call;
     later calls refresh dtype-cast staging (``state_dict`` may then be None).  ``transfer_dtype``
-    applies to direct mode only."""
+    applies to direct mode only.  ``block_scales`` / ``channel_scales`` / ``tensor_scales`` (direct mode
+    only, first call) publish float8_e4m3fn weights with their scales, so that pulls into bf16/f16/f32
+    destinations dequantise them (see ``DirectWeightSyncSource.register``)."""
     if direct_rdma:
-        await _put_state_dict_direct_rdma(store, state_dict, key, transfer_dtype)
+        await _put_state_dict_direct_rdma(store, state_dict, key, transfer_dtype,
+                                          dict(block_scales=block_scales, channel_scales=channel_scales,
+                                               tensor_scales=tensor_scales))
         return
+    if block_scales or channel_scales or tensor_scales:
+        raise NotImplementedError("block_scales, channel_scales and tensor_scales need direct_rdma=True: the store "
+                                  "path does not publish scaled fp8 sources")
     flat, mapping = flatten_state_dict(state_dict)
     await store.put_batch({f"{key}{DELIM}{k}": v for k, v in flat.items()})
     await store.put(f"{key}{DELIM}{MAPPING}", mapping)
@@ -118,7 +126,7 @@ def _state_dict_size(state_dict) -> int:
 # ---------------------------------------------------------------------------------------------
 # direct mode
 # ---------------------------------------------------------------------------------------------
-async def _put_state_dict_direct_rdma(store, state_dict, key, transfer_dtype=None):
+async def _put_state_dict_direct_rdma(store, state_dict, key, transfer_dtype=None, scales: dict | None = None):
     from torchstore_b200.direct_weight_sync import DirectWeightSyncSource
 
     cache = _get_rdma_cache(store)
@@ -130,7 +138,7 @@ async def _put_state_dict_direct_rdma(store, state_dict, key, transfer_dtype=Non
     if key not in cache.registered:
         assert state_dict is not None, "state_dict is required on first put_state_dict call with direct_rdma=True"
         rank, world_size = dist.get_rank(), dist.get_world_size()
-        handles = cache.source.register(state_dict, rank=rank, transfer_dtype=transfer_dtype)
+        handles = cache.source.register(state_dict, rank=rank, transfer_dtype=transfer_dtype, **(scales or {}))
         await store.put(f"{key}/rank_{rank}", handles)
         if rank == 0:
             await store.put(f"{key}/num_ranks", world_size)
