@@ -26,7 +26,7 @@
 extern "C" {
 #endif
 
-#define TSB_ABI_VERSION 6
+#define TSB_ABI_VERSION 7
 #define TSB_MAX_DIMS 6
 
 enum {
@@ -325,6 +325,47 @@ int tsb_dequant_fp8_plan_create(int device, const tsb_rect_t* rects, uint64_t n,
 int tsb_dequant_fp8_compile_host(int device, const tsb_rect_t* rects, uint64_t n, const tsb_dq_source_t* sources,
                                  uint64_t n_sources, uint32_t flags, void* out_tiles, uint64_t tile_cap,
                                  uint64_t* out_n_tiles);
+
+/* ------------------------------------------------------------------------------------------ */
+/* requantising pulls: block-, channel- or tensor-scaled float8_e4m3fn sources into block-,     */
+/* channel- or tensor-scaled float8_e4m3fn destinations                                         */
+/* ------------------------------------------------------------------------------------------ */
+
+/* Compile a requantising pull: `rects` are ordinary source -> destination rectangles with src_dtype ==
+ * dst_dtype == TSB_F8E4M3, src inside one source and dst inside one target.  `sources` are as for
+ * tsb_dequant_fp8_plan_create; `targets` as for tsb_scaled_fp8_plan_create, except that granularity may also
+ * be TSB_SCALE_PER_BLOCK (scale_inv float32 [batch, ceil(rows/128), ceil(cols/128)], 128x128 blocks anchored
+ * at (0, 0) as in tsb_block_fp8_plan_create).  Every element becomes
+ *   x = f32(q) * scale[g_src]   (what tsb_dequant_fp8_plan_create writes into an f32 destination)
+ * and is quantised with the target's formula as if x were an f32 source, so the result equals a dequantising
+ * pull into f32 followed by a quantising pull from it, byte for byte.  A rect's source rows must be rows of
+ * its source shard (TSB_ERR_INVALID naming the rect otherwise); every element of every target must be
+ * written by exactly one rect (TSB_ERR_INVALID naming the target and group otherwise).  Block targets and
+ * per-channel rows of at most 32 KiB read each source byte once; per-tensor groups and longer rows take two
+ * passes.  The result is a plan like any other.  flags: reserved, pass 0. */
+int tsb_requant_fp8_plan_create(int device, const tsb_rect_t* rects, uint64_t n, const tsb_dq_source_t* sources,
+                                uint64_t n_sources, const tsb_sq_target_t* targets, uint64_t n_targets, uint32_t flags,
+                                tsb_plan_t* out);
+/* Host-only (no CUDA call): compile and copy the kernel tables out.  A NULL table only reports its count.
+ * out_units (staged path, one CTA each: a 128x128 block, or a band of whole per-channel rows): records of 40 bytes
+ *   {u64 dst, u64 scale_inv, u32 pitch, u32 rows, u32 cols, u32 first_piece, u32 n_pieces, u32 per_row}
+ *   (scale_inv: the block's, or the band's first row's; per_row: 1 for bands, one scale per row)
+ * out_pieces: records of 56 bytes
+ *   {u64 src, i64 src_row_stride_bytes, u64 scale, u32 row0, u32 col0, u32 rows, u32 cols, u32 scale_step_bytes,
+ *    u32 vector, u32 col_phase, u32 col_blocks}
+ *   (scale: the float32 source scale of the piece's first element; scale_step_bytes: to the next row's, 0 unless
+ *   the source is per channel; col_blocks: 1 for block sources, whose scale advances 4 bytes every 128 columns
+ *   counted from col_phase; row0/col0 relative to the unit; vector: 16-byte loads)
+ * out_tiles (two-pass path, one CTA per pass each): records of 64 bytes, sorted by group
+ *   {u64 src, i64 src_row_stride_bytes, u64 scale, u64 dst, u64 scale_inv_or_0, u32 dst_pitch, u32 rows, u32 cols,
+ *    u32 group, u32 scale_step_bytes, u32 vector}
+ *   (scale_inv_or_0: non-zero in exactly one tile per group, the one that writes its scale)
+ * out_n_groups: the number of two-pass groups (amax words). */
+int tsb_requant_fp8_compile_host(int device, const tsb_rect_t* rects, uint64_t n, const tsb_dq_source_t* sources,
+                                 uint64_t n_sources, const tsb_sq_target_t* targets, uint64_t n_targets, uint32_t flags,
+                                 void* out_units, uint64_t unit_cap, uint64_t* out_n_units, void* out_pieces,
+                                 uint64_t piece_cap, uint64_t* out_n_pieces, void* out_tiles, uint64_t tile_cap,
+                                 uint64_t* out_n_tiles, uint64_t* out_n_groups);
 
 /* ------------------------------------------------------------------------------------------ */
 /* streams and events (the await points of the reference's coroutines)                         */

@@ -16,7 +16,7 @@ import torch
 from torchstore_b200._build import LIB_PATH
 
 TSB_MAX_DIMS = 6
-TSB_ABI_VERSION = 6
+TSB_ABI_VERSION = 7
 
 TSB_OK, TSB_ERR_INVALID, TSB_ERR_CUDA, TSB_ERR_UNSUPPORTED, TSB_ERR_NOMEM, TSB_ERR_NOTFOUND = range(6)
 
@@ -198,6 +198,17 @@ _SIGNATURES = {
         C.c_int,
         [C.c_int, C.POINTER(Rect), C.c_uint64, C.POINTER(DqSource), C.c_uint64, C.c_uint32, _vp, C.c_uint64,
          C.POINTER(C.c_uint64)],
+    ),
+    "tsb_requant_fp8_plan_create": (
+        C.c_int,
+        [C.c_int, C.POINTER(Rect), C.c_uint64, C.POINTER(DqSource), C.c_uint64, C.POINTER(SqTarget), C.c_uint64, C.c_uint32,
+         C.POINTER(C.c_uint64)],
+    ),
+    "tsb_requant_fp8_compile_host": (
+        C.c_int,
+        [C.c_int, C.POINTER(Rect), C.c_uint64, C.POINTER(DqSource), C.c_uint64, C.POINTER(SqTarget), C.c_uint64, C.c_uint32,
+         _vp, C.c_uint64, C.POINTER(C.c_uint64), _vp, C.c_uint64, C.POINTER(C.c_uint64), _vp, C.c_uint64,
+         C.POINTER(C.c_uint64), C.POINTER(C.c_uint64)],
     ),
     "tsb_stream_create": (C.c_int, [C.c_int, C.POINTER(_vp)]),
     "tsb_stream_destroy": (C.c_int, [_vp]),
@@ -539,6 +550,41 @@ def dequant_fp8_compile_host(device: int, rects, n: int, sources, n_sources: int
     tiles = np.zeros(max(1, nt.value), dtype=DQ_TILE_DTYPE)
     check(L.tsb_dequant_fp8_compile_host(device, rects, n, sources, n_sources, 0, tiles.ctypes.data, nt.value, C.byref(nt)))
     return tiles[: nt.value]
+
+
+def requant_fp8_plan_create(device: int, rects, n: int, sources, n_sources: int, targets, n_targets: int) -> int:
+    out = C.c_uint64(0)
+    check(lib().tsb_requant_fp8_plan_create(device, rects, n, sources, n_sources, targets, n_targets, 0, C.byref(out)))
+    return int(out.value)
+
+
+# record layouts of tsb_requant_fp8_compile_host (include/tstore_b200.h)
+RQ_UNIT_DTYPE = [("dst", "<u8"), ("scale_inv", "<u8"), ("pitch", "<u4"), ("rows", "<u4"), ("cols", "<u4"),
+                 ("piece0", "<u4"), ("n_pieces", "<u4"), ("per_row", "<u4")]
+RQ_PIECE_DTYPE = [("src", "<u8"), ("src_stride", "<i8"), ("scale", "<u8"), ("row0", "<u4"), ("col0", "<u4"),
+                  ("rows", "<u4"), ("cols", "<u4"), ("scale_step", "<u4"), ("vec", "<u4"), ("col_phase", "<u4"),
+                  ("col_blocks", "<u4")]
+RQ_TILE_DTYPE = [("src", "<u8"), ("src_stride", "<i8"), ("scale", "<u8"), ("dst", "<u8"), ("scale_inv", "<u8"),
+                 ("pitch", "<u4"), ("rows", "<u4"), ("cols", "<u4"), ("group", "<u4"), ("scale_step", "<u4"),
+                 ("vec", "<u4")]
+
+
+def requant_fp8_compile_host(device: int, rects, n: int, sources, n_sources: int, targets, n_targets: int):
+    """Host-only compilation of a requantising pull -> (units, pieces, tiles, n_groups): numpy record arrays
+    and the number of two-pass groups."""
+    import numpy as np
+
+    nu, npc, nt, ng = C.c_uint64(0), C.c_uint64(0), C.c_uint64(0), C.c_uint64(0)
+    L = lib()
+    check(L.tsb_requant_fp8_compile_host(device, rects, n, sources, n_sources, targets, n_targets, 0, None, 0,
+                                         C.byref(nu), None, 0, C.byref(npc), None, 0, C.byref(nt), C.byref(ng)))
+    units = np.zeros(max(1, nu.value), dtype=RQ_UNIT_DTYPE)
+    pieces = np.zeros(max(1, npc.value), dtype=RQ_PIECE_DTYPE)
+    tiles = np.zeros(max(1, nt.value), dtype=RQ_TILE_DTYPE)
+    check(L.tsb_requant_fp8_compile_host(device, rects, n, sources, n_sources, targets, n_targets, 0, units.ctypes.data,
+                                         nu.value, C.byref(nu), pieces.ctypes.data, npc.value, C.byref(npc),
+                                         tiles.ctypes.data, nt.value, C.byref(nt), C.byref(ng)))
+    return units[: nu.value], pieces[: npc.value], tiles[: nt.value], int(ng.value)
 
 
 CUDA_STREAM_LEGACY = 0x1  # cudaStreamLegacy: an explicit handle for the default stream

@@ -166,6 +166,15 @@ int rect_source_boxes(const tsb_rect_t& in, uint64_t index, const TargetGeom* gr
   return map_boxes(in, index, grids, n_grids, kBySrc, es, out);
 }
 
+int rect_requant_boxes(const tsb_rect_t& in, uint64_t index, const TargetGeom* targets, uint64_t n_targets,
+                       std::vector<TargetBox>* out) {
+  const std::string where = "rect " + std::to_string(index) + ": ";
+  if (in.ndim < 1 || in.ndim > TSB_MAX_DIMS) return fail(TSB_ERR_INVALID, where + "ndim must be in [1, 6]");
+  if (in.src_dtype != TSB_F8E4M3 || in.dst_dtype != TSB_F8E4M3)
+    return fail(TSB_ERR_INVALID, where + "requantising pulls read and write float8_e4m3fn");
+  return map_boxes(in, index, targets, n_targets, kByDst, 1, out);
+}
+
 int block_fp8_compile(int device, const tsb_rect_t* rects, uint64_t n, const tsb_bq_target_t* targets, uint64_t n_targets,
                       BqTables* out) {
   if ((n && !rects) || (n_targets && !targets)) return fail(TSB_ERR_INVALID, "block_fp8: NULL rects or targets");

@@ -28,10 +28,9 @@ bool aligned16(uint64_t p, int64_t stride, uint64_t rows) { return p % 16 == 0 &
 
 }  // namespace
 
-int dequant_fp8_compile(int device, const tsb_rect_t* rects, uint64_t n, const tsb_dq_source_t* sources,
-                        uint64_t n_sources, DqTables* out) {
-  if ((n && !rects) || (n_sources && !sources)) return fail(TSB_ERR_INVALID, "dequant_fp8: NULL rects or sources");
-  std::vector<TargetGeom> geom(n_sources);
+int dq_source_geoms(const tsb_dq_source_t* sources, uint64_t n_sources, std::vector<TargetGeom>* out) {
+  std::vector<TargetGeom>& geom = *out;
+  geom.resize(n_sources);
   for (uint64_t s = 0; s < n_sources; ++s) {
     const tsb_dq_source_t& S = sources[s];
     const std::string where = "source " + std::to_string(s) + ": ";
@@ -47,10 +46,18 @@ int dequant_fp8_compile(int device, const tsb_rect_t* rects, uint64_t n, const t
       return fail(TSB_ERR_INVALID, where + "source too large");
     geom[s] = {S.src, S.batch, S.rows, S.cols};
   }
+  return TSB_OK;
+}
+
+int dequant_fp8_compile(int device, const tsb_rect_t* rects, uint64_t n, const tsb_dq_source_t* sources,
+                        uint64_t n_sources, DqTables* out) {
+  if ((n && !rects) || (n_sources && !sources)) return fail(TSB_ERR_INVALID, "dequant_fp8: NULL rects or sources");
+  std::vector<TargetGeom> geom;
+  int st = dq_source_geoms(sources, n_sources, &geom);
+  if (st) return st;
   std::vector<TargetBox> boxes;
   for (uint64_t i = 0; i < n; ++i) {
-    int st = rect_source_boxes(rects[i], i, geom.data(), n_sources, &boxes);
-    if (st) return st;
+    if ((st = rect_source_boxes(rects[i], i, geom.data(), n_sources, &boxes))) return st;
   }
   for (const TargetBox& x : boxes) {
     const tsb_dq_source_t& S = sources[x.target];

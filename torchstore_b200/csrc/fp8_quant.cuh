@@ -39,6 +39,15 @@ template <> struct Src<TSB_F16> {
   static __device__ __forceinline__ uint32_t f32(uint32_t bits) { return __float_as_uint(f16_bits_to_f32(bits)); }
 };
 
+// A scaled e4m3fn source (requant_fp8.cu): two fp8 bytes (bits 0..15) -> the f32 bits of f32(q) * scale for
+// each, the value a dequantising pull into f32 writes (exact widening, one correctly rounded multiply, no
+// flush to zero).
+__device__ __forceinline__ void scaled_e4m3x2(uint32_t two, float scale, uint32_t* lo, uint32_t* hi) {
+  const uint32_t h2 = fp8x2_to_f16x2<true>(two);
+  *lo = __float_as_uint(__fmul_rn(f16_bits_to_f32(h2 & 0xffffu), scale));
+  *hi = __float_as_uint(__fmul_rn(f16_bits_to_f32(h2 >> 16), scale));
+}
+
 // |x| as an integer: finite < Inf < NaN
 __device__ __forceinline__ uint32_t abs_bits(uint32_t f32_bits) { return f32_bits & 0x7fffffffu; }
 

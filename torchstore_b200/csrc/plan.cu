@@ -43,8 +43,9 @@ TableLayout table_layout(size_t n_rects, size_t n_tiles, size_t n_link) {
 // What a plan's tables drive: the copy_rects kernel, the block-scaled fp8 quantiser
 // (d_block = {BqBlock table | BqPiece table}, num_tiles = blocks), or the per-channel / per-tensor
 // scaled fp8 quantisers (d_block = {SqBand table | SqPiece table | SqTile table | amax words}), or the
-// dequantiser of scaled fp8 sources (d_block = DqTile table, num_tiles = tiles).
-enum : uint32_t { PLAN_COPY = 0, PLAN_BLOCK_FP8 = 1, PLAN_SCALED_FP8 = 2, PLAN_DEQUANT_FP8 = 3 };
+// dequantiser of scaled fp8 sources (d_block = DqTile table, num_tiles = tiles), or the requantiser of scaled
+// fp8 sources into scaled fp8 destinations (d_block = {RqUnit table | RqPiece table | RqTile table | amax words}).
+enum : uint32_t { PLAN_COPY = 0, PLAN_BLOCK_FP8 = 1, PLAN_SCALED_FP8 = 2, PLAN_DEQUANT_FP8 = 3, PLAN_REQUANT_FP8 = 4 };
 
 struct Plan {
   int device = 0;
@@ -56,8 +57,9 @@ struct Plan {
   uint32_t kind = KIND_GENERIC;
   size_t bq_pieces_off = 0;    // PLAN_BLOCK_FP8: byte offset of the piece table in d_block
   uint32_t bq_src_bytes = 2;   // PLAN_BLOCK_FP8: largest source element size
-  size_t sq_off[3] = {};       // PLAN_SCALED_FP8: byte offsets of the piece and tile tables and the amax words
+  size_t sq_off[3] = {};       // PLAN_SCALED_FP8, PLAN_REQUANT_FP8: byte offsets of the piece and tile tables and the amax words
   SqLaunch sq{};               // PLAN_SCALED_FP8: counts (run_plan fills in the table pointers)
+  RqLaunch rq{};               // PLAN_REQUANT_FP8: likewise
   uint32_t link_stage_bytes = 0;
   uint32_t link_stages = 0;
   tsb_plan_info_t info{};
@@ -570,6 +572,14 @@ int run_plan(Plan* p, cudaStream_t s) {
     return launch_scaled_fp8(l, s);
   }
   if (p->plan_kind == PLAN_DEQUANT_FP8) return launch_dequant_fp8(reinterpret_cast<const DqTile*>(p->d_block), p->num_tiles, s);
+  if (p->plan_kind == PLAN_REQUANT_FP8) {
+    RqLaunch l = p->rq;
+    l.units = reinterpret_cast<const RqUnit*>(p->d_block);
+    l.pieces = reinterpret_cast<const RqPiece*>(p->d_block + p->sq_off[0]);
+    l.tiles = reinterpret_cast<const RqTile*>(p->d_block + p->sq_off[1]);
+    l.amax = reinterpret_cast<uint32_t*>(p->d_block + p->sq_off[2]);
+    return launch_requant_fp8(l, s);
+  }
   uint32_t kind = p->kind;
   if (getenv("TSB_FORCE_GENERIC")) kind = KIND_GENERIC;
   LaunchParams lp = make_params(p->d_block, p->layout, p->num_tiles, p->num_link_tiles, kind, p->link_stage_bytes, p->link_stages);
@@ -782,6 +792,43 @@ int tsb_dequant_fp8_plan_create(int device, const tsb_rect_t* rects, uint64_t n,
   p->info.grid = p->num_tiles;
   p->info.block = kDqThreads;
   p->info.tile_bytes = kDqTileElems;
+  return register_plan(p, host, out);
+}
+
+int tsb_requant_fp8_plan_create(int device, const tsb_rect_t* rects, uint64_t n, const tsb_dq_source_t* sources,
+                                uint64_t n_sources, const tsb_sq_target_t* targets, uint64_t n_targets, uint32_t flags,
+                                tsb_plan_t* out) {
+  if (!out) return fail(TSB_ERR_INVALID, "tsb_requant_fp8_plan_create: NULL argument");
+  if (flags != 0) return fail(TSB_ERR_INVALID, "tsb_requant_fp8_plan_create: flags must be 0");
+  RqTables tb;
+  int st = requant_fp8_compile(device, rects, n, sources, n_sources, targets, n_targets, &tb);
+  if (st) return st;
+  const size_t pieces_off = tb.units.size() * sizeof(RqUnit);
+  const size_t tiles_off = pieces_off + tb.pieces.size() * sizeof(RqPiece);
+  const size_t amax_off = tiles_off + tb.tiles.size() * sizeof(RqTile);
+  std::vector<char> host(std::max<size_t>(16, amax_off + 4ull * tb.n_groups), 0);
+  if (!tb.units.empty()) memcpy(host.data(), tb.units.data(), pieces_off);
+  if (!tb.pieces.empty()) memcpy(host.data() + pieces_off, tb.pieces.data(), tiles_off - pieces_off);
+  if (!tb.tiles.empty()) memcpy(host.data() + tiles_off, tb.tiles.data(), amax_off - tiles_off);
+  Plan* p = new Plan();
+  p->device = device;
+  p->plan_kind = PLAN_REQUANT_FP8;
+  p->num_tiles = static_cast<uint32_t>(tb.units.size() + tb.tiles.size());
+  p->info.num_rects = n;
+  p->info.num_tiles = p->num_tiles;
+  p->info.payload_bytes = tb.payload_bytes;
+  p->info.src_bytes = tb.src_bytes;
+  p->info.remote_src_bytes = tb.remote_src_bytes;
+  p->info.grid = p->num_tiles;
+  p->info.block = kRqThreads;
+  p->info.tile_bytes = tb.stage_bytes;
+  p->sq_off[0] = pieces_off;
+  p->sq_off[1] = tiles_off;
+  p->sq_off[2] = amax_off;
+  p->rq.n_units = static_cast<uint32_t>(tb.units.size());
+  p->rq.n_tiles = static_cast<uint32_t>(tb.tiles.size());
+  p->rq.n_groups = tb.n_groups;
+  p->rq.stage_bytes = tb.stage_bytes;
   return register_plan(p, host, out);
 }
 

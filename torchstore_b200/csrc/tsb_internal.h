@@ -181,6 +181,10 @@ int rect_boxes(const tsb_rect_t& in, uint64_t index, const TargetGeom* targets, 
 // destination side.  Destination columns must be contiguous.
 int rect_source_boxes(const tsb_rect_t& in, uint64_t index, const TargetGeom* grids, uint64_t n_grids,
                       std::vector<TargetBox>* out);
+// rect_boxes for requantising pulls: float8_e4m3fn on both sides; a box's `src` / `row_stride` are the
+// source's fp8 bytes.
+int rect_requant_boxes(const tsb_rect_t& in, uint64_t index, const TargetGeom* targets, uint64_t n_targets,
+                       std::vector<TargetBox>* out);
 
 // ---- block-scaled fp8 (block_fp8.cu) ---------------------------------------------------------------
 constexpr uint32_t kBqBlock = 128;  // block edge (elements)
@@ -310,8 +314,75 @@ struct DqTables {
   std::vector<DqTile> tiles;
   uint64_t src_bytes = 0, remote_src_bytes = 0, payload_bytes = 0;
 };
+// Validate scaled fp8 source shards (TSB_ERR_INVALID naming the source) -> their fp8 grids.
+int dq_source_geoms(const tsb_dq_source_t* sources, uint64_t n_sources, std::vector<TargetGeom>* out);
 int dequant_fp8_compile(int device, const tsb_rect_t* rects, uint64_t n, const tsb_dq_source_t* sources,
                         uint64_t n_sources, DqTables* out);
 int launch_dequant_fp8(const DqTile* tiles, uint32_t n_tiles, cudaStream_t stream);
+
+// ---- requantising pulls: scaled fp8 sources -> block / channel / tensor scaled fp8 (requant_fp8.cu) -----
+constexpr uint32_t kRqThreads = 256;
+
+// Staged path, one CTA each: a 128x128 block of a block-scaled target (one group), or a band of whole rows
+// of a per-channel target whose row fits kSqStageBytes (one group per row).
+struct alignas(8) RqUnit {
+  uint64_t dst;          // fp8 element (0, 0) of the unit
+  uint64_t scale_inv;    // float32 scale_inv of the block, or of the band's first row (one per row, contiguous)
+  uint32_t pitch;        // destination row pitch (bytes == elements)
+  uint32_t rows, cols;
+  uint32_t piece0, n_pieces;
+  uint32_t per_row;      // 1: one group per row (band), 0: one group (block)
+};
+static_assert(sizeof(RqUnit) == 40, "RqUnit is part of tsb_requant_fp8_compile_host's output");
+
+// A source rectangle inside one unit, read under one source scale (tensor), one per row (channel) or one per 128
+// source columns (block: the rows of a piece lie in one block row of the source).
+struct alignas(8) RqPiece {
+  uint64_t src;          // fp8 source element (row0, col0) of the piece
+  int64_t src_stride;    // bytes between source rows
+  uint64_t scale;        // float32 source scale of the piece's first element
+  uint32_t row0, col0;   // position inside the unit
+  uint32_t rows, cols;
+  uint32_t scale_step;   // bytes between the source scales of consecutive rows: 4 * row step (channel) or 0
+  uint32_t vec;          // 1: source address, stride, column offset, width and column phase allow 16-byte accesses
+  uint32_t col_phase;    // col_blocks: column of the piece's first element inside its source block
+  uint32_t col_blocks;   // 1: the scale advances 4 bytes every 128 columns from col_phase on (block sources), else 0
+};
+static_assert(sizeof(RqPiece) == 56, "RqPiece is part of tsb_requant_fp8_compile_host's output");
+
+// Two-pass path: a rectangle of one destination group (a per-tensor matrix or a long per-channel row) under
+// one source scale (or one per row), read once per pass by one CTA.
+struct alignas(8) RqTile {
+  uint64_t src;          // fp8 source element (0, 0) of the tile
+  int64_t src_stride;
+  uint64_t scale;        // float32 source scale of row 0
+  uint64_t dst;          // its fp8 destination element
+  uint64_t scale_inv;    // the group's float32 scale_inv if this tile writes it (one tile per group), else 0
+  uint32_t dst_pitch;
+  uint32_t rows, cols;
+  uint32_t group;        // index of the group's amax word
+  uint32_t scale_step;   // as RqPiece::scale_step
+  uint32_t vec;          // 1: source rows start 16-byte aligned (whole 16-element chunks vectorise)
+};
+static_assert(sizeof(RqTile) == 64, "RqTile is part of tsb_requant_fp8_compile_host's output");
+
+struct RqTables {
+  std::vector<RqUnit> units;
+  std::vector<RqPiece> pieces;
+  std::vector<RqTile> tiles;
+  uint32_t n_groups = 0;     // amax words of the two-pass path
+  uint32_t stage_bytes = 0;  // largest unit stage (dynamic shared memory of the staged kernel)
+  uint64_t src_bytes = 0, remote_src_bytes = 0, payload_bytes = 0;
+};
+int requant_fp8_compile(int device, const tsb_rect_t* rects, uint64_t n, const tsb_dq_source_t* sources, uint64_t n_sources,
+                        const tsb_sq_target_t* targets, uint64_t n_targets, RqTables* out);
+struct RqLaunch {
+  const RqUnit* units;
+  const RqPiece* pieces;
+  const RqTile* tiles;
+  uint32_t* amax;  // n_groups words, cleared by the launch
+  uint32_t n_units, n_tiles, n_groups, stage_bytes;
+};
+int launch_requant_fp8(const RqLaunch& l, cudaStream_t stream);
 
 }  // namespace tsb

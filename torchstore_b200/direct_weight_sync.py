@@ -53,6 +53,7 @@ SCALE_KINDS = {
     "tensor_scales": ("tensor scale", "tensor-scaled"),
 }
 _GRANULARITY = {"channel_scales": _native.TSB_SCALE_PER_CHANNEL, "tensor_scales": _native.TSB_SCALE_PER_TENSOR}
+_REQUANT_KEY = ("", "requantize")  # in the scale key set of a pull with requantize=True
 
 
 # ---------------------------------------------------------------------------------------------
@@ -424,7 +425,8 @@ class DirectWeightSyncDest:
         self._block_plans = Plans()  # block-scaled fp8 names: one quantising plan per destination device
         self._scaled_plans = Plans()  # per-channel / per-tensor scaled fp8 names: likewise
         self._dequant_plans = Plans()  # names read from scaled fp8 handles into bf16/f16/f32: one dequantising plan per device
-        self._scale_keys: frozenset = frozenset()  # (name, scale keyword) pairs the cached plan quantises
+        self._requant_plans = Plans()  # scaled fp8 destinations read from scaled fp8 handles: one requantising plan per device
+        self._scale_keys: frozenset = frozenset()  # (name, scale keyword) pairs the cached plan quantises (+ _REQUANT_KEY)
         self._plan_scale_dicts: tuple | None = None  # the three scale dict objects of the last pull
         self.last_pull_ms: dict[int, float] = {}  # device -> kernel time of the last pull
 
@@ -511,9 +513,12 @@ class DirectWeightSyncDest:
         return ids
 
     @staticmethod
-    def _check_scales(all_handles, dest_state_dict, scales: dict[str, dict | None]) -> dict[str, tuple]:
+    def _check_scales(all_handles, dest_state_dict, scales: dict[str, dict | None], *,
+                      requantize: bool = False) -> dict[str, tuple]:
         """Validate the scale dicts of a pull (``{keyword: {name: scale}}``, keywords of SCALE_KINDS) ->
-        ``{name: (keyword, fp8 destination, scale)}``.  Raises before anything is compiled or launched."""
+        ``{name: (keyword, fp8 destination, scale)}``.  With ``requantize``, a name whose handles are all scaled
+        fp8 sources of one granularity is accepted too (it is requantised).  Raises before anything is
+        compiled or launched."""
         out = {}
         for kw, by_name in scales.items():
             what, kind = SCALE_KINDS[kw]
@@ -546,10 +551,25 @@ class DirectWeightSyncDest:
                 handles = all_handles.get(name) or []
                 if not handles:
                     raise ValueError(f"no source handles for {kind} destination '{name}': its groups would not be covered")
+                kinds = {getattr(h.rdma_buffer, "granularity", None) for h in handles}
+                if requantize and kinds != {None}:
+                    if None in kinds:
+                        raise ValueError(f"the handles of {kind} destination '{name}' mix scaled fp8 and unscaled sources "
+                                         "(requantize=True)")
+                    if len(kinds) > 1:
+                        raise ValueError(f"the handles of {kind} destination '{name}' mix scale granularities "
+                                         f"{sorted(kinds)} (requantize=True)")
+                    out[name] = (kw, dest, scale)
+                    continue
                 dtypes = {h.rdma_buffer.dtype for h in handles}
                 if not dtypes <= BLOCK_SOURCE_DTYPES or len(dtypes) != 1:
+                    hint = ""
+                    if kinds - {None}:
+                        hint = "; scaled fp8 handles are requantised only with requantize=True"
+                    elif requantize:
+                        hint = "; requantize=True reads scaled fp8 handles (registered with a scale), not unscaled fp8"
                     raise TypeError(f"{kind} pulls of '{name}' read bf16, f16 or f32 handles of one dtype; "
-                                    f"got {sorted(map(str, dtypes))}")
+                                    f"got {sorted(map(str, dtypes))}{hint}")
                 out[name] = (kw, dest, scale)
         return out
 
@@ -582,10 +602,11 @@ class DirectWeightSyncDest:
             out.add(name)
         return out
 
-    def _compile(self, scaled: dict | None = None, dequant: set | None = None) -> None:
+    def _compile(self, scaled: dict | None = None, dequant: set | None = None, requant: set | None = None) -> None:
         per_device: dict[int, list] = defaultdict(list)
         quant_pairs: dict[tuple, list] = defaultdict(list)  # (device, block?) -> windows of the quantising plans
-        dq: dict[int, tuple[list, dict]] = {}  # device -> (windows, {source buffer id: (index, DqSource)})
+        dq: dict[int, tuple[list, dict]] = {}  # device -> (windows, {source buffer id: (name, DqSource)})
+        rq: dict[int, tuple[list, dict]] = {}  # likewise for the requantising plans
         for op in self._plan:
             dest = op.dest_local
             if not dest.is_cuda:
@@ -599,17 +620,16 @@ class DirectWeightSyncDest:
                 )
             dev = dest.device.index
             window = self.op_windows(op, op.rdma_buffer.window(dev))
-            if scaled and op.name in scaled:
+            if requant and op.name in requant:
+                pairs, sources = rq.setdefault(dev, ([], {}))
+                pairs.append(window)
+                _add_dq_source(sources, op, dev)
+            elif scaled and op.name in scaled:
                 quant_pairs[(dev, scaled[op.name][0] == "block_scales")].append(window)
             elif dequant and op.name in dequant:
                 pairs, sources = dq.setdefault(dev, ([], {}))
                 pairs.append(window)
-                buf = op.rdma_buffer
-                if id(buf) not in sources:
-                    w, s = buf.window(dev), buf.scale_window(dev)
-                    rows, cols = w.shape[-2:]
-                    sources[id(buf)] = (op.name, _native.DqSource(w.ptr, s.ptr, w.numel // (rows * cols), rows, cols,
-                                                                  buf.row0, buf.col0, GRANULARITIES[buf.granularity], 0))
+                _add_dq_source(sources, op, dev)
             else:
                 per_device[dev].append(window)
         self._native_plans = Plans.build(per_device)
@@ -630,10 +650,29 @@ class DirectWeightSyncDest:
         if not scaled:
             return
         try:
+            for dev in sorted({scaled[n][1].device.index for n in requant or ()}):
+                names = [n for n in requant if scaled[n][1].device.index == dev]
+                targets = []
+                for n in names:
+                    kw, d, s = scaled[n]
+                    rows, cols = d.shape[-2:]
+                    code = _native.TSB_SCALE_PER_BLOCK if kw == "block_scales" else _GRANULARITY[kw]
+                    targets.append(_native.SqTarget(d.data_ptr(), s.data_ptr(), d.numel() // (rows * cols), rows, cols, code, 0))
+                pairs, sources = rq.get(dev, ([], {}))
+                src_names = [n for n, _ in sources.values()]
+                try:
+                    self._requant_plans.update(Plans.build_requant_fp8({dev: (pairs, [s for _, s in sources.values()], targets)}))
+                except _native.TsbError as e:
+                    m = re.search(r"target (\d+)", str(e)) or re.search(r"source (\d+)", str(e))
+                    if e.code == _native.TSB_ERR_INVALID and m:
+                        name = (names if m.group(0).startswith("target") else src_names)[int(m.group(1))]
+                        raise ValueError(f"requantising pull of '{name}' ({scaled[name][0]}): {e}") from e
+                    raise
             for block in (True, False):
-                for dev in sorted({d.device.index for kw, d, _ in scaled.values() if (kw == "block_scales") == block}):
+                for dev in sorted({d.device.index for n, (kw, d, _) in scaled.items()
+                                   if (kw == "block_scales") == block and n not in (requant or ())}):
                     names = [n for n, (kw, d, _) in scaled.items()
-                             if d.device.index == dev and (kw == "block_scales") == block]
+                             if d.device.index == dev and (kw == "block_scales") == block and n not in (requant or ())]
                     targets = []
                     for n in names:
                         kw, d, s = scaled[n]
@@ -656,6 +695,7 @@ class DirectWeightSyncDest:
                             raise ValueError(f"{SCALE_KINDS[scaled[name][0]][1]} pull of '{name}' ({scaled[name][0]}): {e}") from e
                         raise
         except BaseException:
+            self._requant_plans.close()
             self._block_plans.close()
             self._scaled_plans.close()
             self._dequant_plans.close()
@@ -671,7 +711,7 @@ class DirectWeightSyncDest:
                    dest_slices: dict[str, TensorSlice] | None = None, *,
                    block_scales: dict[str, torch.Tensor] | None = None,
                    channel_scales: dict[str, torch.Tensor] | None = None,
-                   tensor_scales: dict[str, torch.Tensor] | None = None) -> None:
+                   tensor_scales: dict[str, torch.Tensor] | None = None, requantize: bool = False) -> None:
         """Pull every overlapping region into ``dest_state_dict`` (in place).  Returns when the
         bytes are in destination HBM (so the caller may tell the source it is done reading).
 
@@ -694,12 +734,21 @@ class DirectWeightSyncDest:
         cover are left alone.  A float8_e4m3fn destination not named in a scale dict gets the raw fp8
         bytes; the caller moves the scales separately (for example as their own state-dict entries).
 
+        Requantising (extension, ``requantize=True``): a name in one of the scale dicts may then be fed by
+        scaled fp8 handles of one granularity.  Each element is dequantised exactly as a pull into float32
+        would write it (``f32(q) * scale`` of the handle it is read from), then quantised with the
+        destination's formula: the result equals a dequantising pull into a float32 temporary followed by a
+        quantising pull from it, byte for byte.  This re-rounds, so it is refused (TypeError) by default.
+
         Steady state costs one native call to launch and a poll loop: the cached plan is checked
         against the destination OBJECTS first (their ids; the plan keeps them alive), the kernel
         is enqueued, and the data-pointer signature -- which catches ``param.data = new`` under an
         unchanged object -- is recomputed while the kernel runs."""
         scales = (block_scales, channel_scales, tensor_scales)
+        names = {n for d in scales for n in (d or ())}
         keys = frozenset((n, kw) for kw, d in zip(SCALE_KINDS, scales) for n in (d or ()))
+        if requantize:
+            keys |= {_REQUANT_KEY}
         if self._plan is not None and keys != self._scale_keys:
             logger.info("scaled names or their granularity changed; rebuilding the transfer plan")
             self.close()
@@ -728,11 +777,13 @@ class DirectWeightSyncDest:
                 self._plan_scale_dicts = scales
             verified = True
         if self._plan is None:
-            scaled = self._check_scales(all_handles, dest_state_dict, dict(zip(SCALE_KINDS, scales))) if keys else None
-            dequant = self._check_dequant(all_handles, dest_state_dict, {n for n, _ in keys})
+            scaled = self._check_scales(all_handles, dest_state_dict, dict(zip(SCALE_KINDS, scales)),
+                                        requantize=requantize) if names else None
+            dequant = self._check_dequant(all_handles, dest_state_dict, names)
+            requant = {n for n in scaled or () if getattr(all_handles[n][0].rdma_buffer, "granularity", None)}
             self._plan = self._build_plan(all_handles, dest_state_dict, dest_slices)
             try:
-                self._compile(scaled, dequant)
+                self._compile(scaled, dequant, requant)
             except BaseException:
                 self._plan = None
                 raise
@@ -749,7 +800,7 @@ class DirectWeightSyncDest:
             logger.info("destination storage changed under the same tensors; rebuilding the transfer plan")
             self.close()
             await self.pull(all_handles, dest_state_dict, dest_slices, block_scales=block_scales,
-                            channel_scales=channel_scales, tensor_scales=tensor_scales)
+                            channel_scales=channel_scales, tensor_scales=tensor_scales, requantize=requantize)
 
     def launch(self) -> None:
         """Enqueue the cached plan on each device's copy stream, fenced against the caller's current
@@ -763,12 +814,14 @@ class DirectWeightSyncDest:
             self._scaled_plans.launch()
         if self._dequant_plans:
             self._dequant_plans.launch()
+        if self._requant_plans:
+            self._requant_plans.launch()
 
     async def wait(self) -> None:
         await self._native_plans.wait()
         ms = self._native_plans.elapsed_ms()
         # the plans of a device run back to back on its copy stream
-        for plans in (self._block_plans, self._scaled_plans, self._dequant_plans):
+        for plans in (self._block_plans, self._scaled_plans, self._dequant_plans, self._requant_plans):
             if plans:
                 await plans.wait()
                 for dev, t in plans.elapsed_ms().items():
@@ -780,9 +833,20 @@ class DirectWeightSyncDest:
         self._block_plans.close()
         self._scaled_plans.close()
         self._dequant_plans.close()
+        self._requant_plans.close()
         self._scale_keys = frozenset()
         self._plan = None
         self._plan_ids = self._plan_refs = self._plan_dict = self._plan_scale_dicts = None
+
+
+def _add_dq_source(sources: dict, op: _TransferOp, dev: int) -> None:
+    """Describe the scaled fp8 shard behind ``op`` once per buffer: ``{id(buffer): (name, DqSource)}``."""
+    buf = op.rdma_buffer
+    if id(buf) not in sources:
+        w, s = buf.window(dev), buf.scale_window(dev)
+        rows, cols = w.shape[-2:]
+        sources[id(buf)] = (op.name, _native.DqSource(w.ptr, s.ptr, w.numel // (rows * cols), rows, cols,
+                                                      buf.row0, buf.col0, GRANULARITIES[buf.granularity], 0))
 
 
 def _contig(shape) -> tuple:

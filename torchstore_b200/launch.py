@@ -141,6 +141,28 @@ class Plans(dict):
             raise
         return plans
 
+    @classmethod
+    def build_requant_fp8(cls, per_device: dict[int, tuple[list, list, list]]) -> "Plans":
+        """Compile requantising pulls of scaled fp8 sources into scaled fp8 destinations: ``{device:
+        ([(src, dst) StridedMem windows], [DqSource], [SqTarget])}``."""
+        plans = cls()
+        try:
+            for dev, (pairs, sources, targets) in per_device.items():
+                rects, n = build_rects(pairs)
+                for i in range(n):  # a same-dtype fp8 window is an opaque byte move to build_rects
+                    rects[i].src_dtype = rects[i].dst_dtype = _native.TSB_F8E4M3
+                src_arr = _native.make_dq_source_array(max(1, len(sources)))
+                for i, s in enumerate(sources):
+                    src_arr[i] = s
+                arr = _native.make_sq_target_array(max(1, len(targets)))
+                for i, t in enumerate(targets):
+                    arr[i] = t
+                plans[dev] = _native.requant_fp8_plan_create(dev, rects, n, src_arr, len(sources), arr, len(targets))
+        except BaseException:
+            plans.close()
+            raise
+        return plans
+
     def launch(self, fence_out: bool = True) -> None:
         """Enqueue every plan on its device's copy stream, fenced in against the caller's current
         stream of that device.  ``fence_out=False``: the caller's stream is not made to wait for the
