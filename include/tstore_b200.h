@@ -26,7 +26,7 @@
 extern "C" {
 #endif
 
-#define TSB_ABI_VERSION 7
+#define TSB_ABI_VERSION 8
 #define TSB_MAX_DIMS 6
 
 enum {
@@ -366,6 +366,47 @@ int tsb_requant_fp8_compile_host(int device, const tsb_rect_t* rects, uint64_t n
                                  void* out_units, uint64_t unit_cap, uint64_t* out_n_units, void* out_pieces,
                                  uint64_t piece_cap, uint64_t* out_n_pieces, void* out_tiles, uint64_t tile_cap,
                                  uint64_t* out_n_tiles, uint64_t* out_n_groups);
+
+/* ------------------------------------------------------------------------------------------ */
+/* source-side quantisation: a publisher refreshes block-, channel- or tensor-scaled           */
+/* float8_e4m3fn staging from its live bf16/f16/f32 shards                                      */
+/* ------------------------------------------------------------------------------------------ */
+
+/* One shard to quantise: `batch` contiguous [rows, cols] matrices of src_dtype at src, whose first element
+ * sits at (row0, col0) of the global tensor's last two dims.  Groups are shard-local and anchored at the
+ * global origin, exactly as a tsb_dq_source_t describes them: per block the intersection of a global
+ * 128x128 block with the shard, per channel the shard's part of one row, per tensor the shard's [rows, cols]
+ * matrix.  scale_inv has the shape of tsb_dq_source_t's scale.  Per group the formula of
+ * tsb_bq_target_t / tsb_sq_target_t applies (amax_c = max(amax, 1e-4f), dst = e4m3fn(rn(x * 448 / amax_c)),
+ * scale_inv = amax_c / 448; a NaN poisons its group). */
+typedef struct tsb_source_quant_target {
+  uint64_t src;         /* TSB_F32 / TSB_BF16 / TSB_F16, contiguous [batch, rows, cols], element-aligned */
+  uint64_t dst;         /* float8_e4m3fn, contiguous [batch, rows, cols] */
+  uint64_t scale_inv;   /* float32, contiguous, one per group */
+  uint64_t batch, rows, cols;
+  uint64_t row0, col0;  /* global offset of the shard in the last two dims (the block phase) */
+  uint32_t src_dtype;   /* TSB_F32, TSB_BF16 or TSB_F16 */
+  uint32_t granularity; /* TSB_SCALE_PER_BLOCK, TSB_SCALE_PER_CHANNEL or TSB_SCALE_PER_TENSOR */
+} tsb_source_quant_target_t;
+
+/* Compile a source-side quantisation of `n` targets (TSB_ERR_INVALID naming the target otherwise).  Blocks and
+ * per-channel rows of at most 32 KiB of source bytes are quantised from registers after one read, one CTA per
+ * block or band of rows; per-tensor groups and longer rows take two passes (amax, then quantise).  The result is a plan like any other: tsb_plan_launch[_flags],
+ * _run, _poll, _wait, _elapsed_ms, _info and _destroy accept it.  flags: reserved, pass 0. */
+int tsb_source_quant_plan_create(int device, const tsb_source_quant_target_t* targets, uint64_t n, uint32_t flags,
+                                 tsb_plan_t* out);
+/* Host-only (no CUDA call): compile and copy the kernel tables out.  A NULL table only reports its count.
+ * out_units (one-read path: a block's part of the shard, or a band of whole per-channel rows; grouped by src_dtype,
+ * bf16 then f16 then f32): records of 48 bytes
+ *   {u64 src, u64 dst, u64 scale_inv, u32 src_pitch, u32 dst_pitch, u32 rows, u32 cols, u32 per_row,
+ *    u16 src_dtype, u16 vec}
+ *   (scale_inv: the block's, or the band's first row's; per_row: 1 for bands, one scale per row; pitches in
+ *   bytes; vec: 16-byte loads)
+ * out_tiles (two-pass path): the 56-byte tile records of tsb_scaled_fp8_compile_host, sorted by group
+ * out_n_groups: the number of two-pass groups (amax words). */
+int tsb_source_quant_compile_host(int device, const tsb_source_quant_target_t* targets, uint64_t n, uint32_t flags,
+                                  void* out_units, uint64_t unit_cap, uint64_t* out_n_units, void* out_tiles,
+                                  uint64_t tile_cap, uint64_t* out_n_tiles, uint64_t* out_n_groups);
 
 /* ------------------------------------------------------------------------------------------ */
 /* streams and events (the await points of the reference's coroutines)                         */

@@ -16,7 +16,7 @@ import torch
 from torchstore_b200._build import LIB_PATH
 
 TSB_MAX_DIMS = 6
-TSB_ABI_VERSION = 7
+TSB_ABI_VERSION = 8
 
 TSB_OK, TSB_ERR_INVALID, TSB_ERR_CUDA, TSB_ERR_UNSUPPORTED, TSB_ERR_NOMEM, TSB_ERR_NOTFOUND = range(6)
 
@@ -132,6 +132,23 @@ class DqSource(C.Structure):
     ]
 
 
+class SourceQuantTarget(C.Structure):
+    """tsb_source_quant_target_t: one bf16/f16/f32 shard quantised into scaled fp8 staging on its own device."""
+
+    _fields_ = [
+        ("src", C.c_uint64),
+        ("dst", C.c_uint64),
+        ("scale_inv", C.c_uint64),
+        ("batch", C.c_uint64),
+        ("rows", C.c_uint64),
+        ("cols", C.c_uint64),
+        ("row0", C.c_uint64),
+        ("col0", C.c_uint64),
+        ("src_dtype", C.c_uint32),
+        ("granularity", C.c_uint32),
+    ]
+
+
 class ArenaStats(C.Structure):
     _fields_ = [
         ("capacity", C.c_uint64),
@@ -209,6 +226,14 @@ _SIGNATURES = {
         [C.c_int, C.POINTER(Rect), C.c_uint64, C.POINTER(DqSource), C.c_uint64, C.POINTER(SqTarget), C.c_uint64, C.c_uint32,
          _vp, C.c_uint64, C.POINTER(C.c_uint64), _vp, C.c_uint64, C.POINTER(C.c_uint64), _vp, C.c_uint64,
          C.POINTER(C.c_uint64), C.POINTER(C.c_uint64)],
+    ),
+    "tsb_source_quant_plan_create": (
+        C.c_int, [C.c_int, C.POINTER(SourceQuantTarget), C.c_uint64, C.c_uint32, C.POINTER(C.c_uint64)],
+    ),
+    "tsb_source_quant_compile_host": (
+        C.c_int,
+        [C.c_int, C.POINTER(SourceQuantTarget), C.c_uint64, C.c_uint32, _vp, C.c_uint64, C.POINTER(C.c_uint64), _vp,
+         C.c_uint64, C.POINTER(C.c_uint64), C.POINTER(C.c_uint64)],
     ),
     "tsb_stream_create": (C.c_int, [C.c_int, C.POINTER(_vp)]),
     "tsb_stream_destroy": (C.c_int, [_vp]),
@@ -585,6 +610,36 @@ def requant_fp8_compile_host(device: int, rects, n: int, sources, n_sources: int
                                          nu.value, C.byref(nu), pieces.ctypes.data, npc.value, C.byref(npc),
                                          tiles.ctypes.data, nt.value, C.byref(nt), C.byref(ng)))
     return units[: nu.value], pieces[: npc.value], tiles[: nt.value], int(ng.value)
+
+
+def make_source_quant_target_array(n: int):
+    return (SourceQuantTarget * n)()
+
+
+def source_quant_plan_create(device: int, targets, n: int) -> int:
+    out = C.c_uint64(0)
+    check(lib().tsb_source_quant_plan_create(device, targets, n, 0, C.byref(out)))
+    return int(out.value)
+
+
+# record layout of the units of tsb_source_quant_compile_host (include/tstore_b200.h); its tiles are SQ_TILE_DTYPE
+SRCQ_UNIT_DTYPE = [("src", "<u8"), ("dst", "<u8"), ("scale_inv", "<u8"), ("src_pitch", "<u4"), ("dst_pitch", "<u4"),
+                   ("rows", "<u4"), ("cols", "<u4"), ("per_row", "<u4"), ("src_dtype", "<u2"), ("vec", "<u2")]
+
+
+def source_quant_compile_host(device: int, targets, n: int):
+    """Host-only compilation of a source-side quantisation -> (units, tiles, n_groups): numpy record arrays and
+    the number of two-pass groups."""
+    import numpy as np
+
+    nu, nt, ng = C.c_uint64(0), C.c_uint64(0), C.c_uint64(0)
+    L = lib()
+    check(L.tsb_source_quant_compile_host(device, targets, n, 0, None, 0, C.byref(nu), None, 0, C.byref(nt), C.byref(ng)))
+    units = np.zeros(max(1, nu.value), dtype=SRCQ_UNIT_DTYPE)
+    tiles = np.zeros(max(1, nt.value), dtype=SQ_TILE_DTYPE)
+    check(L.tsb_source_quant_compile_host(device, targets, n, 0, units.ctypes.data, nu.value, C.byref(nu),
+                                          tiles.ctypes.data, nt.value, C.byref(nt), C.byref(ng)))
+    return units[: nu.value], tiles[: nt.value], int(ng.value)
 
 
 CUDA_STREAM_LEGACY = 0x1  # cudaStreamLegacy: an explicit handle for the default stream

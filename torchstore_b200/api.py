@@ -159,11 +159,13 @@ async def put_state_dict(state_dict: dict[str, Any] | None, key: str, store_name
                          direct_rdma: bool = False, transfer_dtype: "torch.dtype | None" = None,
                          block_scales: "dict[str, torch.Tensor] | None" = None,
                          channel_scales: "dict[str, torch.Tensor] | None" = None,
-                         tensor_scales: "dict[str, torch.Tensor] | None" = None) -> None:
+                         tensor_scales: "dict[str, torch.Tensor] | None" = None,
+                         quantize: "dict[str, str] | None" = None) -> None:
     cl = await client(store_name)
     await state_dict_utils.put_state_dict(store=cl, state_dict=state_dict, key=key, direct_rdma=direct_rdma,
                                           transfer_dtype=transfer_dtype, block_scales=block_scales,
-                                          channel_scales=channel_scales, tensor_scales=tensor_scales)
+                                          channel_scales=channel_scales, tensor_scales=tensor_scales,
+                                          quantize=quantize)
 
 
 async def get_state_dict(key: str, user_state_dict: dict[str, Any] | None = None, strict: bool = True,

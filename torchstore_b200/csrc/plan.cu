@@ -44,8 +44,16 @@ TableLayout table_layout(size_t n_rects, size_t n_tiles, size_t n_link) {
 // (d_block = {BqBlock table | BqPiece table}, num_tiles = blocks), or the per-channel / per-tensor
 // scaled fp8 quantisers (d_block = {SqBand table | SqPiece table | SqTile table | amax words}), or the
 // dequantiser of scaled fp8 sources (d_block = DqTile table, num_tiles = tiles), or the requantiser of scaled
-// fp8 sources into scaled fp8 destinations (d_block = {RqUnit table | RqPiece table | RqTile table | amax words}).
-enum : uint32_t { PLAN_COPY = 0, PLAN_BLOCK_FP8 = 1, PLAN_SCALED_FP8 = 2, PLAN_DEQUANT_FP8 = 3, PLAN_REQUANT_FP8 = 4 };
+// fp8 sources into scaled fp8 destinations (d_block = {RqUnit table | RqPiece table | RqTile table | amax words}),
+// or the source-side quantiser (d_block = {SrcQUnit table | SqTile table | amax words}).
+enum : uint32_t {
+  PLAN_COPY = 0,
+  PLAN_BLOCK_FP8 = 1,
+  PLAN_SCALED_FP8 = 2,
+  PLAN_DEQUANT_FP8 = 3,
+  PLAN_REQUANT_FP8 = 4,
+  PLAN_SOURCE_QUANT = 5
+};
 
 struct Plan {
   int device = 0;
@@ -57,9 +65,10 @@ struct Plan {
   uint32_t kind = KIND_GENERIC;
   size_t bq_pieces_off = 0;    // PLAN_BLOCK_FP8: byte offset of the piece table in d_block
   uint32_t bq_src_bytes = 2;   // PLAN_BLOCK_FP8: largest source element size
-  size_t sq_off[3] = {};       // PLAN_SCALED_FP8, PLAN_REQUANT_FP8: byte offsets of the piece and tile tables and the amax words
+  size_t sq_off[3] = {};       // PLAN_SCALED_FP8, PLAN_REQUANT_FP8, PLAN_SOURCE_QUANT: byte offsets of the piece and tile tables and the amax words
   SqLaunch sq{};               // PLAN_SCALED_FP8: counts (run_plan fills in the table pointers)
   RqLaunch rq{};               // PLAN_REQUANT_FP8: likewise
+  SrcQLaunch srcq{};           // PLAN_SOURCE_QUANT: likewise
   uint32_t link_stage_bytes = 0;
   uint32_t link_stages = 0;
   tsb_plan_info_t info{};
@@ -580,6 +589,13 @@ int run_plan(Plan* p, cudaStream_t s) {
     l.amax = reinterpret_cast<uint32_t*>(p->d_block + p->sq_off[2]);
     return launch_requant_fp8(l, s);
   }
+  if (p->plan_kind == PLAN_SOURCE_QUANT) {
+    SrcQLaunch l = p->srcq;
+    l.units = reinterpret_cast<const SrcQUnit*>(p->d_block);
+    l.two_pass.tiles = reinterpret_cast<const SqTile*>(p->d_block + p->sq_off[1]);
+    l.two_pass.amax = reinterpret_cast<uint32_t*>(p->d_block + p->sq_off[2]);
+    return launch_source_quant(l, s);
+  }
   uint32_t kind = p->kind;
   if (getenv("TSB_FORCE_GENERIC")) kind = KIND_GENERIC;
   LaunchParams lp = make_params(p->d_block, p->layout, p->num_tiles, p->num_link_tiles, kind, p->link_stage_bytes, p->link_stages);
@@ -829,6 +845,37 @@ int tsb_requant_fp8_plan_create(int device, const tsb_rect_t* rects, uint64_t n,
   p->rq.n_tiles = static_cast<uint32_t>(tb.tiles.size());
   p->rq.n_groups = tb.n_groups;
   p->rq.stage_bytes = tb.stage_bytes;
+  return register_plan(p, host, out);
+}
+
+int tsb_source_quant_plan_create(int device, const tsb_source_quant_target_t* targets, uint64_t n, uint32_t flags,
+                                 tsb_plan_t* out) {
+  if (!out) return fail(TSB_ERR_INVALID, "tsb_source_quant_plan_create: NULL argument");
+  if (flags != 0) return fail(TSB_ERR_INVALID, "tsb_source_quant_plan_create: flags must be 0");
+  SrcQTables tb;
+  int st = source_quant_compile(targets, n, &tb);
+  if (st) return st;
+  const size_t tiles_off = tb.units.size() * sizeof(SrcQUnit);
+  const size_t amax_off = tiles_off + tb.tiles.size() * sizeof(SqTile);
+  std::vector<char> host(std::max<size_t>(16, amax_off + 4ull * tb.n_groups), 0);
+  if (!tb.units.empty()) memcpy(host.data(), tb.units.data(), tiles_off);
+  if (!tb.tiles.empty()) memcpy(host.data() + tiles_off, tb.tiles.data(), amax_off - tiles_off);
+  Plan* p = new Plan();
+  p->device = device;
+  p->plan_kind = PLAN_SOURCE_QUANT;
+  p->num_tiles = static_cast<uint32_t>(tb.units.size() + tb.tiles.size());
+  for (int k = 0; k < 3; ++k) p->srcq.n_units[k] = tb.n_units[k];
+  p->info.num_rects = n;
+  p->info.num_tiles = p->num_tiles;
+  p->info.payload_bytes = tb.payload_bytes;
+  p->info.src_bytes = tb.src_bytes;
+  p->info.grid = p->num_tiles;
+  p->info.block = kSrcQThreads;
+  p->info.tile_bytes = tb.unit_bytes;
+  p->sq_off[1] = tiles_off;
+  p->sq_off[2] = amax_off;
+  p->srcq.two_pass.n_tiles = static_cast<uint32_t>(tb.tiles.size());
+  p->srcq.two_pass.n_groups = tb.n_groups;
   return register_plan(p, host, out);
 }
 

@@ -1,0 +1,309 @@
+// Source-side quantisation (sm_90a, H100): a publisher's refresh of block-, channel- or tensor-scaled
+// float8_e4m3fn staging from its live bf16/f16/f32 shards, the producer half of the scaled-FP8 weight sync.
+//
+// Groups are shard-local and anchored at the global origin, the layout a scaled source handle describes
+// (tsb_dq_source_t): a block-scaled shard at global offset (row0, col0) has one group per global 128x128 block
+// it touches, cut to the shard, so an FSDP shard starting mid-block gets partial first and last block rows.
+// Per group the formula of the quantising pulls applies, from the same device helpers (fp8_quant.cuh).
+//
+// Host side: every target is cut into work in group order, with trivial addressing (a shard is one
+// contiguous tensor; there are no pieces):
+//   blocks, and per-channel rows of at most kSqStageBytes source bytes -> units (one CTA each)
+//   per-tensor matrices and longer per-channel rows                   -> two-pass tiles of at most kSqTileElems
+// Device side:
+//   source_quant_kernel<DT>  one 256-thread CTA per unit, one launch per source dtype (units are grouped by dtype,
+//                            so an f32 unit's register budget never lowers the occupancy of bf16 units).  Each
+//                            thread issues every 16-byte load of its (at most 4) 16-element chunks up front into
+//                            registers, folds |x| into its group's amax (warp redux + one shared atomicMax per warp
+//                            and group), and after the scales are known narrows the same registers and stores.  Each
+//                            source byte is read once; with 4 resident CTAs per SM (bf16/f16) one CTA's loads are in
+//                            flight while the others quantise and store.  Units whose rows are not 16-byte aligned
+//                            load element by element into the same registers.
+//   two-pass tiles           scaled_fp8.cu's amax and quantise kernels (the tile format is SqTile); the amax words
+//                            are cleared on the launch stream before pass 1, so a replayed plan starts from zero.
+
+#include <algorithm>
+#include <cstring>
+
+#include "fp8_quant.cuh"
+#include "tsb_internal.h"
+
+namespace tsb {
+
+namespace {
+
+uint32_t round16(uint64_t x) { return static_cast<uint32_t>((x + 15u) & ~uint64_t(15)); }
+
+struct Compiler {
+  SrcQTables* out;
+
+  void unit(const tsb_source_quant_target_t& T, uint32_t es, uint64_t src_elem, uint64_t scale_inv, uint64_t rows,
+            uint64_t cols, bool per_row) {
+    SrcQUnit u;
+    memset(&u, 0, sizeof(u));
+    u.src = T.src + src_elem * es;
+    u.dst = T.dst + src_elem;
+    u.scale_inv = scale_inv;
+    u.src_pitch = static_cast<uint32_t>(T.cols * es);
+    u.dst_pitch = static_cast<uint32_t>(T.cols);
+    u.rows = static_cast<uint32_t>(rows);
+    u.cols = static_cast<uint32_t>(cols);
+    u.per_row = per_row ? 1u : 0u;
+    u.src_dtype = static_cast<uint16_t>(T.src_dtype);
+    u.vec = (u.src % 16 == 0 && (rows == 1 || u.src_pitch % 16 == 0) && (cols * es) % 16 == 0) ? 1 : 0;
+    out->unit_bytes = std::max<uint32_t>(out->unit_bytes, static_cast<uint32_t>(rows * cols * es));
+    out->units.push_back(u);
+    out->src_bytes += rows * cols * es;
+  }
+
+  // `n` contiguous elements from element `first` as one two-pass group; its first tile writes `scale_inv`
+  void group(const tsb_source_quant_target_t& T, uint32_t es, uint64_t first, uint64_t n, uint64_t scale_inv) {
+    const uint32_t g = out->n_groups++;
+    for (uint64_t c = 0; c < n; c += kSqTileElems) {
+      SqTile t;
+      memset(&t, 0, sizeof(t));
+      const uint64_t cols = std::min<uint64_t>(kSqTileElems, n - c);
+      t.src = T.src + (first + c) * es;
+      t.dst = T.dst + first + c;
+      t.scale = c == 0 ? scale_inv : 0;
+      t.dst_pitch = static_cast<uint32_t>(cols);
+      t.rows = 1;
+      t.cols = static_cast<uint32_t>(cols);
+      t.group = g;
+      t.src_dtype = T.src_dtype;
+      t.vec = (t.src % 16 == 0 && (cols * es) % 16 == 0) ? 1u : 0u;
+      out->tiles.push_back(t);
+      out->src_bytes += cols * es;
+    }
+  }
+
+  void target(const tsb_source_quant_target_t& T) {
+    const uint32_t es = quant_src_bytes(T.src_dtype);
+    if (T.granularity == TSB_SCALE_PER_BLOCK) {
+      const uint64_t br0 = T.row0 / kBqBlock, br1 = (T.row0 + T.rows + kBqBlock - 1) / kBqBlock;
+      const uint64_t bc0 = T.col0 / kBqBlock, bc1 = (T.col0 + T.cols + kBqBlock - 1) / kBqBlock;
+      for (uint64_t b = 0; b < T.batch; ++b) {
+        for (uint64_t i = br0; i < br1; ++i) {
+          const uint64_t r0 = std::max(i * kBqBlock, T.row0) - T.row0, r1 = std::min((i + 1) * kBqBlock, T.row0 + T.rows) - T.row0;
+          for (uint64_t j = bc0; j < bc1; ++j) {
+            const uint64_t c0 = std::max(j * kBqBlock, T.col0) - T.col0, c1 = std::min((j + 1) * kBqBlock, T.col0 + T.cols) - T.col0;
+            const uint64_t s = ((b * (br1 - br0) + i - br0) * (bc1 - bc0) + j - bc0);
+            unit(T, es, (b * T.rows + r0) * T.cols + c0, T.scale_inv + 4 * s, r1 - r0, c1 - c0, false);
+          }
+        }
+      }
+    } else if (T.granularity == TSB_SCALE_PER_CHANNEL) {
+      const uint64_t all = T.batch * T.rows;  // per channel, the matrices of a stack are consecutive rows
+      const uint32_t spitch = round16(T.cols * es);
+      const uint64_t cpr = (T.cols + 15) / 16;  // 16-element chunks per row
+      if (spitch > kSqStageBytes || cpr > kSrcQChunks * kSrcQThreads) {
+        for (uint64_t r = 0; r < all; ++r) group(T, es, r * T.cols, T.cols, T.scale_inv + 4 * r);
+        return;
+      }
+      const uint64_t per_band =
+          std::min<uint64_t>(std::min<uint64_t>(kSqBandRows, kSqStageBytes / spitch), kSrcQChunks * kSrcQThreads / cpr);
+      for (uint64_t r = 0; r < all; r += per_band)
+        unit(T, es, r * T.cols, T.scale_inv + 4 * r, std::min(per_band, all - r), T.cols, true);
+    } else {
+      for (uint64_t b = 0; b < T.batch; ++b) group(T, es, b * T.rows * T.cols, T.rows * T.cols, T.scale_inv + 4 * b);
+    }
+  }
+};
+
+}  // namespace
+
+int source_quant_compile(const tsb_source_quant_target_t* targets, uint64_t n, SrcQTables* out) {
+  if (n && !targets) return fail(TSB_ERR_INVALID, "source_quant: NULL targets");
+  Compiler cc{out};
+  for (uint64_t t = 0; t < n; ++t) {
+    const tsb_source_quant_target_t& T = targets[t];
+    const std::string where = "target " + std::to_string(t) + ": ";
+    const uint32_t es = quant_src_bytes(T.src_dtype);
+    if (!es) return fail(TSB_ERR_INVALID, where + "src_dtype must be TSB_F32, TSB_BF16 or TSB_F16, not " + std::to_string(T.src_dtype));
+    if (!T.src || !T.dst || !T.scale_inv) return fail(TSB_ERR_INVALID, where + "NULL src, dst or scale_inv");
+    if (!T.batch || !T.rows || !T.cols) return fail(TSB_ERR_INVALID, where + "empty target");
+    if (T.src % es) return fail(TSB_ERR_INVALID, where + "src is not aligned to its element size");
+    if (T.scale_inv % 4) return fail(TSB_ERR_INVALID, where + "scale_inv is not 4-byte aligned");
+    if (T.granularity != TSB_SCALE_PER_BLOCK && T.granularity != TSB_SCALE_PER_CHANNEL && T.granularity != TSB_SCALE_PER_TENSOR)
+      return fail(TSB_ERR_INVALID, where + "granularity must be TSB_SCALE_PER_BLOCK, TSB_SCALE_PER_CHANNEL or "
+                                           "TSB_SCALE_PER_TENSOR, not " + std::to_string(T.granularity));
+    if (T.cols >= (1ull << 30) || T.rows >= (1ull << 31) || T.batch >= (1ull << 31) ||
+        T.batch * T.rows >= (1ull << 40) / T.cols || T.row0 >= (1ull << 40) || T.col0 >= (1ull << 40))
+      return fail(TSB_ERR_INVALID, where + "target too large");
+    uint64_t groups = T.batch;
+    if (T.granularity == TSB_SCALE_PER_CHANNEL) groups *= T.rows;
+    if (T.granularity == TSB_SCALE_PER_BLOCK)
+      groups *= ((T.row0 + T.rows + kBqBlock - 1) / kBqBlock - T.row0 / kBqBlock) *
+                ((T.col0 + T.cols + kBqBlock - 1) / kBqBlock - T.col0 / kBqBlock);
+    out->payload_bytes += T.batch * T.rows * T.cols + 4 * groups;
+    cc.target(T);
+    if (out->units.size() >= (1ull << 31) || out->tiles.size() >= (1ull << 31) || out->n_groups >= (1u << 31))
+      return fail(TSB_ERR_UNSUPPORTED, "source_quant: more than 2^31 units, tiles or groups");
+  }
+  // one launch per source dtype: bf16, f16, f32
+  const auto rank = [](const SrcQUnit& u) { return u.src_dtype == TSB_BF16 ? 0 : u.src_dtype == TSB_F16 ? 1 : 2; };
+  std::stable_sort(out->units.begin(), out->units.end(), [&](const SrcQUnit& a, const SrcQUnit& b) { return rank(a) < rank(b); });
+  for (const SrcQUnit& u : out->units) ++out->n_units[rank(u)];
+  return TSB_OK;
+}
+
+namespace {
+
+// Load the first `nvalid` elements of a 16-element chunk at `s` into `d` (its source words; the rest 0).
+template <uint32_t DT>
+__device__ __forceinline__ void load_chunk(const char* s, uint32_t nvalid, bool vec, uint32_t d[4 * Src<DT>::kBytes]) {
+  constexpr uint32_t es = Src<DT>::kBytes;
+#pragma unroll
+  for (uint32_t i = 0; i < 4 * es; ++i) d[i] = 0;
+  if (vec) {  // nvalid * es is a multiple of 16 here
+#pragma unroll
+    for (uint32_t i = 0; i < es; ++i) {
+      if (16 * i < nvalid * es) {
+        const uint4 v = ldg16(s + 16 * i);
+        d[4 * i] = v.x;
+        d[4 * i + 1] = v.y;
+        d[4 * i + 2] = v.z;
+        d[4 * i + 3] = v.w;
+      }
+    }
+  } else {
+#pragma unroll
+    for (uint32_t k = 0; k < 16; ++k) {
+      if (k < nvalid) {
+        if (es == 4)
+          d[k] = __ldg(reinterpret_cast<const uint32_t*>(s) + k);
+        else
+          d[k / 2] |= static_cast<uint32_t>(__ldg(reinterpret_cast<const unsigned short*>(s) + k)) << (16 * (k & 1));
+      }
+    }
+  }
+}
+
+// the f32 bits of a chunk's 16 elements from its source words
+template <uint32_t DT>
+__device__ __forceinline__ void widen_chunk(const uint32_t d[4 * Src<DT>::kBytes], uint32_t f[16]) {
+#pragma unroll
+  for (uint32_t k = 0; k < 16; ++k) {
+    if constexpr (Src<DT>::kBytes == 4)
+      f[k] = d[k];
+    else
+      f[k] = Src<DT>::f32((d[k / 2] >> (16 * (k & 1))) & 0xffffu);
+  }
+}
+
+template <uint32_t DT>
+__global__ void __launch_bounds__(kSrcQThreads) source_quant_kernel(const SrcQUnit* __restrict__ units) {
+  constexpr uint32_t es = Src<DT>::kBytes;
+  __shared__ uint32_t s_amax[kSqBandRows];
+  __shared__ float s_scale[kSqBandRows];
+  const SrcQUnit u = units[blockIdx.x];
+  const char* src = reinterpret_cast<const char*>(u.src);
+  const uint32_t cpr = (u.cols + 15u) / 16u, total = u.rows * cpr;
+  const uint32_t ng = u.per_row ? u.rows : 1u;
+  const uint32_t warp = threadIdx.x >> 5, lane = threadIdx.x & 31u;
+  for (uint32_t g = threadIdx.x; g < ng; g += kSrcQThreads) s_amax[g] = 0;
+  // every load of this thread's chunks first: chunk j is idx = threadIdx.x + j * kSrcQThreads
+  uint32_t d[kSrcQChunks][4 * es];
+#pragma unroll
+  for (uint32_t j = 0; j < kSrcQChunks; ++j) {
+    const uint32_t idx = threadIdx.x + j * kSrcQThreads;
+    const uint32_t r = idx / cpr, c = (idx - r * cpr) * 16u;
+    if (idx < total) {
+      load_chunk<DT>(src + static_cast<uint64_t>(r) * u.src_pitch + c * es, min(16u, u.cols - c), u.vec, d[j]);
+    } else {
+#pragma unroll
+      for (uint32_t i = 0; i < 4 * es; ++i) d[j][i] = 0;  // folded as zeros by the warp's other lanes
+    }
+  }
+  __syncthreads();  // the zeroed amax words are visible (the loads stay in flight)
+  uint32_t mine = 0;
+#pragma unroll
+  for (uint32_t j = 0; j < kSrcQChunks; ++j) {
+    const uint32_t base = warp * 32 + j * kSrcQThreads;  // warp-uniform
+    if (base >= total) break;
+    const uint32_t idx = base + lane;
+    uint32_t f[16], m = 0;
+    widen_chunk<DT>(d[j], f);
+#pragma unroll
+    for (uint32_t k = 0; k < 16; ++k) m = max(m, abs_bits(f[k]));  // zero words past the chunk's end or the unit's
+    if (u.per_row) {
+      const uint32_t rf = base / cpr, rl = (min(base + 32u, total) - 1u) / cpr;
+      if (rf == rl) {
+        m = __reduce_max_sync(0xffffffffu, m);
+        if (lane == 0) atomicMax(s_amax + rf, m);
+      } else if (idx < total) {
+        atomicMax(s_amax + idx / cpr, m);
+      }
+    } else {
+      mine = max(mine, m);
+    }
+  }
+  if (!u.per_row) {
+    mine = __reduce_max_sync(0xffffffffu, mine);
+    if (lane == 0) atomicMax(s_amax, mine);
+  }
+  __syncthreads();
+  for (uint32_t g = threadIdx.x; g < ng; g += kSrcQThreads) {
+    float scale, scale_inv;
+    scales_of_amax(s_amax[g], &scale, &scale_inv);
+    s_scale[g] = scale;
+    reinterpret_cast<float*>(u.scale_inv)[g] = scale_inv;
+  }
+  __syncthreads();
+#pragma unroll
+  for (uint32_t j = 0; j < kSrcQChunks; ++j) {
+    const uint32_t idx = threadIdx.x + j * kSrcQThreads;
+    if (idx < total) {
+      const uint32_t r = idx / cpr, c = (idx - r * cpr) * 16u;
+      uint32_t f[16], o[4];
+      widen_chunk<DT>(d[j], f);
+      narrow16(f, s_scale[u.per_row ? r : 0u], o);
+      store16(reinterpret_cast<char*>(u.dst) + static_cast<uint64_t>(r) * u.dst_pitch + c, min(16u, u.cols - c), o);
+    }
+  }
+}
+
+}  // namespace
+
+int launch_source_quant(const SrcQLaunch& l, cudaStream_t stream) {
+  const SrcQUnit* units = l.units;
+  for (int k = 0; k < 3; ++k) {
+    const uint32_t n = l.n_units[k];
+    if (!n) continue;
+    if (k == 0) source_quant_kernel<TSB_BF16><<<n, kSrcQThreads, 0, stream>>>(units);
+    if (k == 1) source_quant_kernel<TSB_F16><<<n, kSrcQThreads, 0, stream>>>(units);
+    if (k == 2) source_quant_kernel<TSB_F32><<<n, kSrcQThreads, 0, stream>>>(units);
+    cudaError_t e = cudaGetLastError();
+    if (e != cudaSuccess) return cuda_fail(e, "source_quant_kernel launch");
+    count_launch();
+    units += n;
+  }
+  if (l.two_pass.n_tiles) return launch_scaled_fp8(l.two_pass, stream);
+  return TSB_OK;
+}
+
+}  // namespace tsb
+
+using namespace tsb;
+
+extern "C" int tsb_source_quant_compile_host(int device, const tsb_source_quant_target_t* targets, uint64_t n, uint32_t flags,
+                                             void* out_units, uint64_t unit_cap, uint64_t* out_n_units, void* out_tiles,
+                                             uint64_t tile_cap, uint64_t* out_n_tiles, uint64_t* out_n_groups) {
+  (void)device;
+  if (flags != 0) return fail(TSB_ERR_INVALID, "tsb_source_quant_compile_host: flags must be 0");
+  SrcQTables tb;
+  int st = source_quant_compile(targets, n, &tb);
+  if (st) return st;
+  if (out_n_units) *out_n_units = tb.units.size();
+  if (out_n_tiles) *out_n_tiles = tb.tiles.size();
+  if (out_n_groups) *out_n_groups = tb.n_groups;
+  if (out_units) {
+    if (tb.units.size() > unit_cap) return fail(TSB_ERR_NOMEM, "out_units too small");
+    if (!tb.units.empty()) memcpy(out_units, tb.units.data(), tb.units.size() * sizeof(SrcQUnit));
+  }
+  if (out_tiles) {
+    if (tb.tiles.size() > tile_cap) return fail(TSB_ERR_NOMEM, "out_tiles too small");
+    if (!tb.tiles.empty()) memcpy(out_tiles, tb.tiles.data(), tb.tiles.size() * sizeof(SqTile));
+  }
+  return TSB_OK;
+}

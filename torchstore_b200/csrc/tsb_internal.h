@@ -385,4 +385,40 @@ struct RqLaunch {
 };
 int launch_requant_fp8(const RqLaunch& l, cudaStream_t stream);
 
+// ---- source-side quantisation: live bf16/f16/f32 shards -> scaled fp8 staging (source_quant.cu) ---------
+constexpr uint32_t kSrcQThreads = 256;
+constexpr uint32_t kSrcQChunks = 4;  // 16-element chunks per thread: a unit holds at most 4 * 256 of them (a 128x128 block)
+
+// One CTA's work: one group of a block-scaled shard (its part of a global 128x128 block), or a band of whole rows of
+// a per-channel shard (one group per row) of at most kSqStageBytes source bytes and kSrcQChunks * kSrcQThreads
+// 16-element chunks.  Source and destination are the shard's own contiguous rows.
+struct alignas(8) SrcQUnit {
+  uint64_t src;          // source element (0, 0) of the unit
+  uint64_t dst;          // its fp8 element
+  uint64_t scale_inv;    // float32 scale_inv of the block, or of the band's first row (one per row, contiguous)
+  uint32_t src_pitch;    // bytes between source rows
+  uint32_t dst_pitch;    // bytes between destination rows
+  uint32_t rows, cols;
+  uint32_t per_row;      // 1: one group per row (band), 0: one group (block)
+  uint16_t src_dtype;    // TSB_F32 / TSB_BF16 / TSB_F16
+  uint16_t vec;          // 1: source address, pitch and row width allow 16-byte loads
+};
+static_assert(sizeof(SrcQUnit) == 48, "SrcQUnit is part of tsb_source_quant_compile_host's output");
+
+struct SrcQTables {
+  std::vector<SrcQUnit> units;  // grouped by source dtype: bf16, then f16, then f32 (one kernel launch each)
+  std::vector<SqTile> tiles;    // two-pass path: per-tensor groups and long per-channel rows
+  uint32_t n_groups = 0;        // amax words of the two-pass path
+  uint32_t n_units[3] = {};     // units per source dtype, in the order above
+  uint32_t unit_bytes = 0;      // largest unit's source bytes
+  uint64_t src_bytes = 0, payload_bytes = 0;
+};
+int source_quant_compile(const tsb_source_quant_target_t* targets, uint64_t n, SrcQTables* out);
+struct SrcQLaunch {
+  const SrcQUnit* units;
+  uint32_t n_units[3];  // bf16, f16, f32 units, consecutive in the table
+  SqLaunch two_pass;    // tiles of the two-pass path, run by scaled_fp8.cu's amax and quantise kernels
+};
+int launch_source_quant(const SrcQLaunch& l, cudaStream_t stream);
+
 }  // namespace tsb

@@ -239,13 +239,17 @@ class DirectWeightSyncSource:
         self._refresh_plans = Plans()
         self._copied: list[tuple[torch.Tensor, torch.Tensor]] = []  # (staging, source) refreshed with copy_
         self._devices: tuple[int, ...] = ()  # devices holding registered memory (fence targets)
+        # quantize= names: name -> (fp8 staging, float32 scale, source local tensor), refreshed by _quant_plans
+        self._quantized: dict[str, tuple[torch.Tensor, torch.Tensor, torch.Tensor]] = {}
+        self._quant_plans = Plans()
 
     def register(self, state_dict: dict[str, torch.Tensor], rank: int,
                  transfer_dtype: torch.dtype | None = None,
                  tensor_slices: dict[str, TensorSlice] | None = None, *,
                  block_scales: dict[str, torch.Tensor] | None = None,
                  channel_scales: dict[str, torch.Tensor] | None = None,
-                 tensor_scales: dict[str, torch.Tensor] | None = None) -> dict[str, RDMAWeightHandle]:
+                 tensor_scales: dict[str, torch.Tensor] | None = None,
+                 quantize: dict[str, str] | None = None) -> dict[str, RDMAWeightHandle]:
         """Create a handle for every entry of ``state_dict`` (tensors or DTensors).
 
         ``tensor_slices`` (extension) gives the global rectangle of *plain* local shards for
@@ -256,16 +260,28 @@ class DirectWeightSyncSource:
         or ``tensor_scales`` (one per matrix) is published with its scale, so that a pull into a bf16, f16
         or f32 destination dequantises it (DESIGN.md section 4).  Scales are anchored at the global
         origin: a shard at global offset (r0, c0) of its last two dims carries exactly the groups it
-        touches (:func:`source_scale_shapes`).  Such weights are registered zero-copy.  Everything is
-        validated before anything is exported, so a failed call registers nothing."""
-        scaled = self._check_source_scales(state_dict, transfer_dtype, tensor_slices,
-                                           {"block_scales": block_scales, "channel_scales": channel_scales,
-                                            "tensor_scales": tensor_scales})
+        touches (:func:`source_scale_shapes`).  Such weights are registered zero-copy.
+
+        Source-side quantisation (extension): ``quantize={name: "block" | "channel" | "tensor"}`` publishes a
+        bf16, f16 or f32 weight (at least 2 dims, contiguous, on CUDA) as float8_e4m3fn staging plus a float32
+        scale, a scaled handle exactly like one registered with a scale dict, so every pull that reads scaled
+        handles reads it.  Groups are shard-local and anchored at the global origin: per block the part of a
+        global 128x128 block inside the shard, per channel the shard's part of a row, per tensor the shard's
+        [rows, cols] matrix.  Each group gets the quantising formula of DESIGN.md section 4.  ``refresh()``
+        requantises the staging from the live weights; ``transfer_dtype`` does not apply to these names.
+
+        Everything is validated before anything is exported, so a failed call registers nothing."""
+        scale_dicts = {"block_scales": block_scales, "channel_scales": channel_scales, "tensor_scales": tensor_scales}
+        quantize = self._check_quantize(state_dict, tensor_slices, quantize or {}, scale_dicts)
+        scaled = self._check_source_scales(state_dict, transfer_dtype, tensor_slices, scale_dicts)
         handles: dict[str, RDMAWeightHandle] = {}
         self._refresh_plans.close()
+        self._quant_plans.close()
         self._staging = {}
         self._copied = []
+        self._quantized = {}
         casts: dict[int, list] = defaultdict(list)  # device -> (source, staging) windows of the refresh
+        quant_targets: dict[int, list] = defaultdict(list)  # device -> SourceQuantTarget of the refresh
         devices = set()
         for name, param in state_dict.items():
             req = Request.from_any(name, param, tensor_slices.get(name) if tensor_slices else None)
@@ -274,11 +290,25 @@ class DirectWeightSyncSource:
             if not local.is_cuda:
                 raise RuntimeError(f"direct weight sync registers GPU memory; '{name}' is on {local.device}")
             devices.add(local.device.index)
-            if name in scaled:
+            if any(name in (d or {}) for d in scale_dicts.values()):
                 granularity, scale = scaled[name]
                 handles[name] = RDMAWeightHandle(
                     rdma_buffer=ScaledNvlinkBuffer(local, scale, granularity, *_last_two_offsets(tslice)),
                     tensor_slice=tslice, source_rank=rank)
+                continue
+            if name in quantize:
+                granularity = quantize[name]
+                r0, c0 = _last_two_offsets(tslice)
+                fp8 = torch.empty(local.shape, dtype=torch.float8_e4m3fn, device=local.device)
+                scale = torch.empty(source_scale_shapes(granularity, tuple(local.shape), r0, c0)[0], dtype=torch.float32,
+                                    device=local.device)
+                rows, cols = local.shape[-2:]
+                quant_targets[local.device.index].append(_native.SourceQuantTarget(
+                    local.data_ptr(), fp8.data_ptr(), scale.data_ptr(), local.numel() // (rows * cols), rows, cols, r0, c0,
+                    _native.cast_code(local.dtype), GRANULARITIES[granularity]))
+                self._quantized[name] = (fp8, scale, local)
+                handles[name] = RDMAWeightHandle(rdma_buffer=ScaledNvlinkBuffer(fp8, scale, granularity, r0, c0),
+                                                 tensor_slice=tslice, source_rank=rank)
                 continue
             if transfer_dtype is not None:
                 staging = torch.empty(local.shape, dtype=transfer_dtype, device=local.device)
@@ -294,16 +324,19 @@ class DirectWeightSyncSource:
             handles[name] = RDMAWeightHandle(rdma_buffer=NvlinkBuffer(buf), tensor_slice=tslice, source_rank=rank)
         self._handles = handles
         self._devices = tuple(sorted(devices))
-        if self._staging:
+        if self._staging or self._quantized:
             if casts:
                 self._refresh_plans = Plans.build(casts)
+            if quant_targets:
+                self._quant_plans = Plans.build_source_quant(quant_targets)
             self.refresh()
         else:
             # make sure the weights the handles point at are materialised before anyone reads them
             for dev in devices:
                 torch.cuda.current_stream(dev).synchronize()
-        logger.info("Registered %d NVLink handles (%d staged, %d direct)", len(handles), len(self._staging),
-                    len(handles) - len(self._staging))
+        staged = len(self._staging) + len(self._quantized)
+        logger.info("Registered %d NVLink handles (%d staged, %d quantised into scaled fp8, %d direct)", len(handles),
+                    staged, len(self._quantized), len(handles) - staged)
         return handles
 
     @staticmethod
@@ -353,19 +386,47 @@ class DirectWeightSyncSource:
                 out[name] = (granularity, scale)
         return out
 
+    @staticmethod
+    def _check_quantize(state_dict, tensor_slices, quantize: dict, scale_dicts: dict[str, dict | None]) -> dict[str, str]:
+        """Validate the ``quantize`` dict of :meth:`register` -> ``{name: granularity}``.  Raises before anything
+        is exported or allocated."""
+        for name, granularity in quantize.items():
+            if name not in state_dict:
+                raise ValueError(f"quantize names '{name}', which is not in the state dict")
+            if any(name in (d or {}) for d in scale_dicts.values()):
+                raise ValueError(f"'{name}' is in quantize and in one of block_scales, channel_scales and tensor_scales: "
+                                 "a weight is either published with its scale or quantised on refresh")
+            if granularity not in GRANULARITIES:
+                raise ValueError(f"quantize['{name}'] must be one of {sorted(GRANULARITIES)}, not {granularity!r}")
+            w = Request.from_any(name, state_dict[name], tensor_slices.get(name) if tensor_slices else None).tensor_val
+            if w.dtype not in BLOCK_SOURCE_DTYPES:
+                raise TypeError(f"quantised weight '{name}' must be bfloat16, float16 or float32, not {w.dtype}")
+            if w.dim() < 2:
+                raise ValueError(f"quantised weight '{name}' needs at least 2 dims; got shape {tuple(w.shape)}")
+            if w.numel() == 0:
+                raise ValueError(f"quantised weight '{name}' is empty (shape {tuple(w.shape)})")
+            if not w.is_contiguous():
+                raise ValueError(f"quantised weight '{name}' is not contiguous (shape {tuple(w.shape)}, strides {w.stride()})")
+            if not w.is_cuda:
+                raise ValueError(f"quantised weight '{name}' must live on a CUDA device, not {w.device}")
+        return dict(quantize)
+
     def refresh(self) -> int:
-        """Re-cast the source params into their staging buffers (no-op without transfer_dtype).
-        Returns the number of staging buffers refreshed.  Blocks until the cast has landed so the
-        caller may publish/notify right after, like the reference's synchronous copy loop."""
-        if not self._staging:
+        """Re-cast the source params into their staging buffers and requantise the ``quantize`` names into
+        their scaled fp8 staging (no-op without either).  Returns the number of staging buffers refreshed.
+        Blocks until everything has landed so the caller may publish/notify right after, like the
+        reference's synchronous copy loop."""
+        if not self._staging and not self._quantized:
             return 0
+        self._quant_plans.launch()
         self._refresh_plans.launch()
         for staging, local in self._copied:
             staging.copy_(local)
+        self._quant_plans.synchronize()
         self._refresh_plans.synchronize()
         for dev in {local.device.index for _, local in self._copied}:
             torch.cuda.current_stream(dev).synchronize()
-        return len(self._staging)
+        return len(self._staging) + len(self._quantized)
 
     def fence(self) -> None:
         """Make every write queued on the caller's streams (optimizer step, staging refresh) land in
@@ -380,7 +441,9 @@ class DirectWeightSyncSource:
         self._handles.clear()
         self._staging.clear()
         self._copied.clear()
+        self._quantized.clear()
         self._refresh_plans.close()
+        self._quant_plans.close()
 
 
 def fused_refresh(src_dtype: torch.dtype, transfer_dtype: torch.dtype) -> bool:

@@ -163,6 +163,21 @@ class Plans(dict):
             raise
         return plans
 
+    @classmethod
+    def build_source_quant(cls, per_device: dict[int, list]) -> "Plans":
+        """Compile source-side quantisations: ``{device: [SourceQuantTarget]}``."""
+        plans = cls()
+        try:
+            for dev, targets in per_device.items():
+                arr = _native.make_source_quant_target_array(max(1, len(targets)))
+                for i, t in enumerate(targets):
+                    arr[i] = t
+                plans[dev] = _native.source_quant_plan_create(dev, arr, len(targets))
+        except BaseException:
+            plans.close()
+            raise
+        return plans
+
     def launch(self, fence_out: bool = True) -> None:
         """Enqueue every plan on its device's copy stream, fenced in against the caller's current
         stream of that device.  ``fence_out=False``: the caller's stream is not made to wait for the

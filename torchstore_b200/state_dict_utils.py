@@ -54,22 +54,28 @@ def reset_direct_cache(store=None) -> None:
                 d.close()
             for src in cache.sources.values():
                 src._refresh_plans.close()
+                src._quant_plans.close()
 
 
 async def put_state_dict(store, state_dict, key, direct_rdma=False, transfer_dtype=None, block_scales: dict | None = None,
-                         channel_scales: dict | None = None, tensor_scales: dict | None = None):
+                         channel_scales: dict | None = None, tensor_scales: dict | None = None,
+                         quantize: dict | None = None):
     """Store every leaf of ``state_dict`` (one batched put), then the mapping as the commit marker.
 
     With ``direct_rdma=True`` only handles to the caller's HBM are published on the first call;
     later calls refresh dtype-cast staging (``state_dict`` may then be None).  ``transfer_dtype``
     applies to direct mode only.  ``block_scales`` / ``channel_scales`` / ``tensor_scales`` (direct mode
     only, first call) publish float8_e4m3fn weights with their scales, so that pulls into bf16/f16/f32
-    destinations dequantise them (see ``DirectWeightSyncSource.register``)."""
+    destinations dequantise them (see ``DirectWeightSyncSource.register``).  ``quantize`` (direct mode only,
+    first call) names bf16/f16/f32 weights published as block-, channel- or tensor-scaled fp8 staging that
+    later calls requantise from the live weights."""
     if direct_rdma:
         await _put_state_dict_direct_rdma(store, state_dict, key, transfer_dtype,
                                           dict(block_scales=block_scales, channel_scales=channel_scales,
-                                               tensor_scales=tensor_scales))
+                                               tensor_scales=tensor_scales, quantize=quantize))
         return
+    if quantize:
+        raise NotImplementedError("quantize needs direct_rdma=True: the store path does not publish scaled fp8 staging")
     if block_scales or channel_scales or tensor_scales:
         raise NotImplementedError("block_scales, channel_scales and tensor_scales need direct_rdma=True: the store "
                                   "path does not publish scaled fp8 sources")
