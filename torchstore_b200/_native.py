@@ -480,14 +480,44 @@ def plan_compile_host(device: int, rects, n: int, flags: int = 0, tile_units: in
     return rect_buf[: n_rects.value * 192], tile_buf[: n_tiles.value], info
 
 
+def _plan_create(fn, *args) -> int:
+    """One of the tsb_*_plan_create calls of the scaled fp8 plans (flags 0) -> plan id."""
+    out = C.c_uint64(0)
+    check(fn(*args, 0, C.byref(out)))
+    return int(out.value)
+
+
+def _structs(struct, items: list) -> tuple:
+    """``items`` as a C array of ``struct`` (at least one element) and their number."""
+    return (struct * max(1, len(items)))(*items), len(items)
+
+
+def _compile_host(fn, args: tuple, dtypes: list, n_groups: bool) -> list:
+    """Call a tsb_*_compile_host (flags 0) for its record counts, then for its tables -> one numpy record array per
+    table (dtypes: their layouts, in output order), then the number of two-pass groups if the call reports it."""
+    import numpy as np
+
+    counts = [C.c_uint64(0) for _ in dtypes]
+    ng = C.c_uint64(0)
+
+    def call(tables):
+        outs = []
+        for t, c in zip(tables, counts):
+            outs += [None, 0, C.byref(c)] if t is None else [t.ctypes.data, c.value, C.byref(c)]
+        check(fn(*args, 0, *outs, *([C.byref(ng)] if n_groups else [])))
+
+    call([None] * len(dtypes))
+    tables = [np.zeros(max(1, c.value), dtype=dt) for c, dt in zip(counts, dtypes)]
+    call(tables)
+    return [t[: c.value] for t, c in zip(tables, counts)] + ([int(ng.value)] if n_groups else [])
+
+
 def make_target_array(n: int):
     return (BqTarget * n)()
 
 
-def block_fp8_plan_create(device: int, rects, n: int, targets, n_targets: int) -> int:
-    out = C.c_uint64(0)
-    check(lib().tsb_block_fp8_plan_create(device, rects, n, targets, n_targets, 0, C.byref(out)))
-    return int(out.value)
+def block_fp8_plan_create(device: int, rects, n: int, targets: list) -> int:
+    return _plan_create(lib().tsb_block_fp8_plan_create, device, rects, n, *_structs(BqTarget, targets))
 
 
 # record layouts of tsb_block_fp8_compile_host (include/tstore_b200.h)
@@ -499,27 +529,16 @@ BQ_PIECE_DTYPE = [("src", "<u8"), ("src_stride", "<i8"), ("row0", "<u2"), ("col0
 
 def block_fp8_compile_host(device: int, rects, n: int, targets, n_targets: int):
     """Host-only compilation of a block-scaled fp8 pull -> (blocks, pieces) numpy record arrays."""
-    import numpy as np
-
-    nb, npc = C.c_uint64(0), C.c_uint64(0)
-    L = lib()
-    check(L.tsb_block_fp8_compile_host(device, rects, n, targets, n_targets, 0, None, 0, C.byref(nb), None, 0,
-                                       C.byref(npc)))
-    blocks = np.zeros(max(1, nb.value), dtype=BQ_BLOCK_DTYPE)
-    pieces = np.zeros(max(1, npc.value), dtype=BQ_PIECE_DTYPE)
-    check(L.tsb_block_fp8_compile_host(device, rects, n, targets, n_targets, 0, blocks.ctypes.data, nb.value,
-                                       C.byref(nb), pieces.ctypes.data, npc.value, C.byref(npc)))
-    return blocks[: nb.value], pieces[: npc.value]
+    return tuple(_compile_host(lib().tsb_block_fp8_compile_host, (device, rects, n, targets, n_targets),
+                               [BQ_BLOCK_DTYPE, BQ_PIECE_DTYPE], False))
 
 
 def make_sq_target_array(n: int):
     return (SqTarget * n)()
 
 
-def scaled_fp8_plan_create(device: int, rects, n: int, targets, n_targets: int) -> int:
-    out = C.c_uint64(0)
-    check(lib().tsb_scaled_fp8_plan_create(device, rects, n, targets, n_targets, 0, C.byref(out)))
-    return int(out.value)
+def scaled_fp8_plan_create(device: int, rects, n: int, targets: list) -> int:
+    return _plan_create(lib().tsb_scaled_fp8_plan_create, device, rects, n, *_structs(SqTarget, targets))
 
 
 # record layouts of tsb_scaled_fp8_compile_host (include/tstore_b200.h)
@@ -534,29 +553,16 @@ SQ_TILE_DTYPE = [("src", "<u8"), ("src_stride", "<i8"), ("dst", "<u8"), ("scale_
 def scaled_fp8_compile_host(device: int, rects, n: int, targets, n_targets: int):
     """Host-only compilation of a per-channel / per-tensor scaled fp8 pull -> (bands, pieces, tiles,
     n_groups): numpy record arrays and the number of two-pass groups."""
-    import numpy as np
-
-    nb, npc, nt, ng = C.c_uint64(0), C.c_uint64(0), C.c_uint64(0), C.c_uint64(0)
-    L = lib()
-    check(L.tsb_scaled_fp8_compile_host(device, rects, n, targets, n_targets, 0, None, 0, C.byref(nb), None, 0,
-                                        C.byref(npc), None, 0, C.byref(nt), C.byref(ng)))
-    bands = np.zeros(max(1, nb.value), dtype=SQ_BAND_DTYPE)
-    pieces = np.zeros(max(1, npc.value), dtype=SQ_PIECE_DTYPE)
-    tiles = np.zeros(max(1, nt.value), dtype=SQ_TILE_DTYPE)
-    check(L.tsb_scaled_fp8_compile_host(device, rects, n, targets, n_targets, 0, bands.ctypes.data, nb.value,
-                                        C.byref(nb), pieces.ctypes.data, npc.value, C.byref(npc), tiles.ctypes.data,
-                                        nt.value, C.byref(nt), C.byref(ng)))
-    return bands[: nb.value], pieces[: npc.value], tiles[: nt.value], int(ng.value)
+    return tuple(_compile_host(lib().tsb_scaled_fp8_compile_host, (device, rects, n, targets, n_targets),
+                               [SQ_BAND_DTYPE, SQ_PIECE_DTYPE, SQ_TILE_DTYPE], True))
 
 
 def make_dq_source_array(n: int):
     return (DqSource * n)()
 
 
-def dequant_fp8_plan_create(device: int, rects, n: int, sources, n_sources: int) -> int:
-    out = C.c_uint64(0)
-    check(lib().tsb_dequant_fp8_plan_create(device, rects, n, sources, n_sources, 0, C.byref(out)))
-    return int(out.value)
+def dequant_fp8_plan_create(device: int, rects, n: int, sources: list) -> int:
+    return _plan_create(lib().tsb_dequant_fp8_plan_create, device, rects, n, *_structs(DqSource, sources))
 
 
 # record layout of tsb_dequant_fp8_compile_host (include/tstore_b200.h)
@@ -567,20 +573,15 @@ DQ_TILE_DTYPE = [("src", "<u8"), ("dst", "<u8"), ("scale", "<u8"), ("src_stride"
 
 def dequant_fp8_compile_host(device: int, rects, n: int, sources, n_sources: int):
     """Host-only compilation of a dequantising pull -> its tile table as a numpy record array."""
-    import numpy as np
-
-    nt = C.c_uint64(0)
-    L = lib()
-    check(L.tsb_dequant_fp8_compile_host(device, rects, n, sources, n_sources, 0, None, 0, C.byref(nt)))
-    tiles = np.zeros(max(1, nt.value), dtype=DQ_TILE_DTYPE)
-    check(L.tsb_dequant_fp8_compile_host(device, rects, n, sources, n_sources, 0, tiles.ctypes.data, nt.value, C.byref(nt)))
-    return tiles[: nt.value]
+    return _compile_host(lib().tsb_dequant_fp8_compile_host, (device, rects, n, sources, n_sources), [DQ_TILE_DTYPE],
+                         False)[0]
 
 
-def requant_fp8_plan_create(device: int, rects, n: int, sources, n_sources: int, targets, n_targets: int) -> int:
-    out = C.c_uint64(0)
-    check(lib().tsb_requant_fp8_plan_create(device, rects, n, sources, n_sources, targets, n_targets, 0, C.byref(out)))
-    return int(out.value)
+def requant_fp8_plan_create(device: int, rects, n: int, sources: list, targets: list) -> int:
+    for i in range(n):  # a same-dtype fp8 window is an opaque byte move to build_rects
+        rects[i].src_dtype = rects[i].dst_dtype = TSB_F8E4M3
+    return _plan_create(lib().tsb_requant_fp8_plan_create, device, rects, n, *_structs(DqSource, sources),
+                        *_structs(SqTarget, targets))
 
 
 # record layouts of tsb_requant_fp8_compile_host (include/tstore_b200.h)
@@ -597,29 +598,16 @@ RQ_TILE_DTYPE = [("src", "<u8"), ("src_stride", "<i8"), ("scale", "<u8"), ("dst"
 def requant_fp8_compile_host(device: int, rects, n: int, sources, n_sources: int, targets, n_targets: int):
     """Host-only compilation of a requantising pull -> (units, pieces, tiles, n_groups): numpy record arrays
     and the number of two-pass groups."""
-    import numpy as np
-
-    nu, npc, nt, ng = C.c_uint64(0), C.c_uint64(0), C.c_uint64(0), C.c_uint64(0)
-    L = lib()
-    check(L.tsb_requant_fp8_compile_host(device, rects, n, sources, n_sources, targets, n_targets, 0, None, 0,
-                                         C.byref(nu), None, 0, C.byref(npc), None, 0, C.byref(nt), C.byref(ng)))
-    units = np.zeros(max(1, nu.value), dtype=RQ_UNIT_DTYPE)
-    pieces = np.zeros(max(1, npc.value), dtype=RQ_PIECE_DTYPE)
-    tiles = np.zeros(max(1, nt.value), dtype=RQ_TILE_DTYPE)
-    check(L.tsb_requant_fp8_compile_host(device, rects, n, sources, n_sources, targets, n_targets, 0, units.ctypes.data,
-                                         nu.value, C.byref(nu), pieces.ctypes.data, npc.value, C.byref(npc),
-                                         tiles.ctypes.data, nt.value, C.byref(nt), C.byref(ng)))
-    return units[: nu.value], pieces[: npc.value], tiles[: nt.value], int(ng.value)
+    return tuple(_compile_host(lib().tsb_requant_fp8_compile_host, (device, rects, n, sources, n_sources, targets, n_targets),
+                               [RQ_UNIT_DTYPE, RQ_PIECE_DTYPE, RQ_TILE_DTYPE], True))
 
 
 def make_source_quant_target_array(n: int):
     return (SourceQuantTarget * n)()
 
 
-def source_quant_plan_create(device: int, targets, n: int) -> int:
-    out = C.c_uint64(0)
-    check(lib().tsb_source_quant_plan_create(device, targets, n, 0, C.byref(out)))
-    return int(out.value)
+def source_quant_plan_create(device: int, targets: list) -> int:
+    return _plan_create(lib().tsb_source_quant_plan_create, device, *_structs(SourceQuantTarget, targets))
 
 
 # record layout of the units of tsb_source_quant_compile_host (include/tstore_b200.h); its tiles are SQ_TILE_DTYPE
@@ -630,16 +618,8 @@ SRCQ_UNIT_DTYPE = [("src", "<u8"), ("dst", "<u8"), ("scale_inv", "<u8"), ("src_p
 def source_quant_compile_host(device: int, targets, n: int):
     """Host-only compilation of a source-side quantisation -> (units, tiles, n_groups): numpy record arrays and
     the number of two-pass groups."""
-    import numpy as np
-
-    nu, nt, ng = C.c_uint64(0), C.c_uint64(0), C.c_uint64(0)
-    L = lib()
-    check(L.tsb_source_quant_compile_host(device, targets, n, 0, None, 0, C.byref(nu), None, 0, C.byref(nt), C.byref(ng)))
-    units = np.zeros(max(1, nu.value), dtype=SRCQ_UNIT_DTYPE)
-    tiles = np.zeros(max(1, nt.value), dtype=SQ_TILE_DTYPE)
-    check(L.tsb_source_quant_compile_host(device, targets, n, 0, units.ctypes.data, nu.value, C.byref(nu),
-                                          tiles.ctypes.data, nt.value, C.byref(nt), C.byref(ng)))
-    return units[: nu.value], tiles[: nt.value], int(ng.value)
+    return tuple(_compile_host(lib().tsb_source_quant_compile_host, (device, targets, n), [SRCQ_UNIT_DTYPE, SQ_TILE_DTYPE],
+                               True))
 
 
 CUDA_STREAM_LEGACY = 0x1  # cudaStreamLegacy: an explicit handle for the default stream

@@ -146,6 +146,30 @@ int map_boxes(const tsb_rect_t& in, uint64_t index, const TargetGeom* targets, u
 
 }  // namespace
 
+int check_grid(const GridRules& rules, uint64_t index, const Grid& g) {
+  const std::string where = std::string(rules.noun) + " " + std::to_string(index) + ": ";
+  if (g.null) return fail(TSB_ERR_INVALID, where + rules.null_msg);
+  if (!g.batch || !g.rows || !g.cols) return fail(TSB_ERR_INVALID, where + "empty " + rules.noun);
+  if (g.base % g.es) return fail(TSB_ERR_INVALID, where + rules.base_name + " is not aligned to its element size");
+  if (g.scale % 4) return fail(TSB_ERR_INVALID, where + rules.scale_name + " is not 4-byte aligned");
+  if (rules.granularities && !(g.granularity < 32 && (rules.granularities >> g.granularity) & 1)) {
+    // "must be A or B" / "must be A, B or C", in the order block, channel, tensor
+    const uint32_t codes[] = {TSB_SCALE_PER_BLOCK, TSB_SCALE_PER_CHANNEL, TSB_SCALE_PER_TENSOR};
+    const char* const code_names[] = {"TSB_SCALE_PER_BLOCK", "TSB_SCALE_PER_CHANNEL", "TSB_SCALE_PER_TENSOR"};
+    std::vector<std::string> names;
+    for (int k = 0; k < 3; ++k)
+      if ((rules.granularities >> codes[k]) & 1) names.push_back(code_names[k]);
+    std::string list = names[0];
+    for (size_t i = 1; i < names.size(); ++i) list += (i + 1 == names.size() ? " or " : ", ") + names[i];
+    return fail(TSB_ERR_INVALID, where + "granularity must be " + list + ", not " + std::to_string(g.granularity));
+  }
+  if (g.pad) return fail(TSB_ERR_INVALID, where + "pad must be 0");
+  if (g.cols >= rules.max_cols || g.rows >= (1ull << 31) || g.batch >= (1ull << 31) || g.batch * g.rows >= (1ull << 40) / g.cols ||
+      g.row0 >= (1ull << 40) || g.col0 >= (1ull << 40))
+    return fail(TSB_ERR_INVALID, where + rules.noun + " too large");
+  return TSB_OK;
+}
+
 int rect_boxes(const tsb_rect_t& in, uint64_t index, const TargetGeom* targets, uint64_t n_targets,
                std::vector<TargetBox>* out) {
   const std::string where = "rect " + std::to_string(index) + ": ";
@@ -175,6 +199,10 @@ int rect_requant_boxes(const tsb_rect_t& in, uint64_t index, const TargetGeom* t
   return map_boxes(in, index, targets, n_targets, kByDst, 1, out);
 }
 
+namespace {
+
+constexpr GridRules kTargetRules{"target", "NULL dst or scale_inv", "dst", "scale_inv", 0, 1ull << 31};
+
 int block_fp8_compile(int device, const tsb_rect_t* rects, uint64_t n, const tsb_bq_target_t* targets, uint64_t n_targets,
                       BqTables* out) {
   if ((n && !rects) || (n_targets && !targets)) return fail(TSB_ERR_INVALID, "block_fp8: NULL rects or targets");
@@ -182,13 +210,8 @@ int block_fp8_compile(int device, const tsb_rect_t* rects, uint64_t n, const tsb
   std::vector<uint64_t> base(n_targets + 1, 0);
   for (uint64_t t = 0; t < n_targets; ++t) {
     const tsb_bq_target_t& T = targets[t];
-    const std::string where = "target " + std::to_string(t) + ": ";
-    if (!T.dst || !T.scale_inv) return fail(TSB_ERR_INVALID, where + "NULL dst or scale_inv");
-    if (!T.batch || !T.rows || !T.cols) return fail(TSB_ERR_INVALID, where + "empty target");
-    if (T.scale_inv % 4) return fail(TSB_ERR_INVALID, where + "scale_inv is not 4-byte aligned");
-    if (T.cols >= (1ull << 31) || T.rows >= (1ull << 31) || T.batch >= (1ull << 31) ||
-        T.batch * T.rows >= (1ull << 40) / T.cols)
-      return fail(TSB_ERR_INVALID, where + "target too large");
+    int st = check_grid(kTargetRules, t, {T.dst, T.scale_inv, T.batch, T.rows, T.cols, 0, 0, 1, 0, 0, !T.dst || !T.scale_inv});
+    if (st) return st;
     const uint64_t nbr = (T.rows + kBqBlock - 1) / kBqBlock, nbc = (T.cols + kBqBlock - 1) / kBqBlock;
     base[t + 1] = base[t] + T.batch * nbr * nbc;
     out->payload_bytes += T.batch * T.rows * T.cols + 4 * T.batch * nbr * nbc;
@@ -223,11 +246,9 @@ int block_fp8_compile(int device, const tsb_rect_t* rects, uint64_t n, const tsb
         p.col0 = static_cast<uint16_t>(pc0 - bc * kBqBlock);
         p.rows = static_cast<uint16_t>(pr1 - pr0);
         p.cols = static_cast<uint16_t>(pc1 - pc0);
-        p.vec = (p.src % 16 == 0 && (p.rows == 1 || p.src_stride % 16 == 0) && (p.cols * es) % 16 == 0 && (p.col0 * es) % 16 == 0) ? 1u : 0u;
+        p.vec = (vec_ok(p.src, p.src_stride, p.rows, p.cols, es) && (p.col0 * es) % 16 == 0) ? 1u : 0u;
         pieces.push_back({base[x.target] + (x.b * nbr + br) * nbc + bc, x.dtype, p});
-        const uint64_t bytes = static_cast<uint64_t>(p.rows) * p.cols * es;
-        out->src_bytes += bytes;
-        if (x.src_device >= 0 && x.src_device != device) out->remote_src_bytes += bytes;
+        out->read(static_cast<uint64_t>(p.rows) * p.cols * es, x.src_device, device);
         out->max_src_bytes = std::max(out->max_src_bytes, es);
       }
     }
@@ -286,12 +307,6 @@ int block_fp8_compile(int device, const tsb_rect_t* rects, uint64_t n, const tsb
   return TSB_OK;
 }
 
-namespace {
-
-// 4 loads in flight per thread and 6 CTAs per SM (40 registers; a bf16 stage is 32 KiB): measured faster
-// on H100 than 8 loads at 4 CTAs per SM (64 registers), see DESIGN.md section 6.
-constexpr int kUnroll = 4;
-
 // Phase 1: pieces -> shared memory (source dtype, block row pitch 128 elements); returns this
 // thread's max |x| bits.
 template <uint32_t DT>
@@ -306,11 +321,11 @@ __device__ __forceinline__ uint32_t stage_block(const BqBlock& blk, const BqPiec
     if (p.vec) {
       const uint32_t upr = p.cols * es / 16;  // 16-byte units per row
       const uint32_t total = p.rows * upr;
-      for (uint32_t i = threadIdx.x; i < total; i += kBqThreads * kUnroll) {
+      for (uint32_t i = threadIdx.x; i < total; i += kQuantThreads * kUnroll) {
         uint4 v[kUnroll];
 #pragma unroll
         for (int k = 0; k < kUnroll; ++k) {
-          const uint32_t idx = i + k * kBqThreads;
+          const uint32_t idx = i + k * kQuantThreads;
           if (idx < total) {
             const uint32_t r = idx / upr, c = idx - r * upr;
             v[k] = ldg16(src + static_cast<int64_t>(r) * p.src_stride + c * 16);
@@ -318,7 +333,7 @@ __device__ __forceinline__ uint32_t stage_block(const BqBlock& blk, const BqPiec
         }
 #pragma unroll
         for (int k = 0; k < kUnroll; ++k) {
-          const uint32_t idx = i + k * kBqThreads;
+          const uint32_t idx = i + k * kQuantThreads;
           if (idx < total) {
             const uint32_t r = idx / upr, c = idx - r * upr;
             m = fold16<DT>(m, v[k]);
@@ -328,7 +343,7 @@ __device__ __forceinline__ uint32_t stage_block(const BqBlock& blk, const BqPiec
       }
     } else {
       const uint32_t total = static_cast<uint32_t>(p.rows) * p.cols;
-      for (uint32_t idx = threadIdx.x; idx < total; idx += kBqThreads) {
+      for (uint32_t idx = threadIdx.x; idx < total; idx += kQuantThreads) {
         const uint32_t r = idx / p.cols, c = idx - r * p.cols;
         const char* a = src + static_cast<int64_t>(r) * p.src_stride + c * es;
         unsigned char* s = s0 + r * spitch + c * es;
@@ -354,7 +369,7 @@ __device__ __forceinline__ void quantise_block(const BqBlock& blk, const unsigne
   constexpr uint32_t spitch = kBqBlock * es;
   const uint32_t cpr = (blk.cols + 15u) / 16u;
   const uint32_t total = blk.rows * cpr;
-  for (uint32_t idx = threadIdx.x; idx < total; idx += kBqThreads) {
+  for (uint32_t idx = threadIdx.x; idx < total; idx += kQuantThreads) {
     const uint32_t r = idx / cpr, c = (idx - r * cpr) * 16u;
     const unsigned char* s = smem + r * spitch + c * es;
     char* d = reinterpret_cast<char*>(blk.dst) + static_cast<uint64_t>(r) * blk.pitch + c;
@@ -369,26 +384,19 @@ __device__ __forceinline__ void quantise_block(const BqBlock& blk, const unsigne
 template <uint32_t DT>
 __device__ __forceinline__ void run_block(const BqBlock& blk, const BqPiece* pieces, unsigned char* smem, uint32_t* s_red,
                                           float* s_scale) {
-  uint32_t m = stage_block<DT>(blk, pieces, smem);
-  m = __reduce_max_sync(0xffffffffu, m);
-  if ((threadIdx.x & 31u) == 0) s_red[threadIdx.x >> 5] = m;
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    uint32_t a = s_red[0];
-#pragma unroll
-    for (uint32_t w = 1; w < kBqThreads / 32; ++w) a = max(a, s_red[w]);
+  cta_max(stage_block<DT>(blk, pieces, smem), s_red, [&](uint32_t a) {
     float scale, scale_inv;
     scales_of_amax(a, &scale, &scale_inv);
     *s_scale = scale;
     *reinterpret_cast<float*>(blk.scale) = scale_inv;
-  }
+  });
   __syncthreads();
   quantise_block<DT>(blk, smem, *s_scale);
 }
 
-__global__ void __launch_bounds__(kBqThreads, 6) block_fp8_kernel(const BqBlock* __restrict__ blocks, const BqPiece* __restrict__ pieces) {
+__global__ void __launch_bounds__(kQuantThreads, 6) block_fp8_kernel(const BqBlock* __restrict__ blocks, const BqPiece* __restrict__ pieces) {
   extern __shared__ __align__(16) unsigned char stage[];
-  __shared__ uint32_t s_red[kBqThreads / 32];
+  __shared__ uint32_t s_red[kQuantThreads / 32];
   __shared__ float s_scale;
   const BqBlock blk = blocks[blockIdx.x];
   switch (blk.src_dtype) {
@@ -411,40 +419,46 @@ cudaError_t prepare() {
   return e;
 }
 
-}  // namespace
-
 int launch_block_fp8(const BqBlock* blocks, const BqPiece* pieces, uint32_t n_blocks, uint32_t max_src_bytes, cudaStream_t stream) {
-  if (n_blocks == 0) return TSB_OK;
-  cudaError_t e = prepare();
-  if (e == cudaSuccess) {
-    block_fp8_kernel<<<n_blocks, kBqThreads, kBqBlock * kBqBlock * max_src_bytes, stream>>>(blocks, pieces);
-    e = cudaGetLastError();
-  }
+  const cudaError_t e = prepare();
   if (e != cudaSuccess) return cuda_fail(e, "block_fp8_kernel launch");
-  count_launch();
+  block_fp8_kernel<<<n_blocks, kQuantThreads, kBqBlock * kBqBlock * max_src_bytes, stream>>>(blocks, pieces);
+  return launched("block_fp8_kernel launch");
+}
+
+// d = {BqBlock table | BqPiece table}, one CTA per block
+int block_fp8_plan(int device, const tsb_rect_t* rects, uint64_t n, const tsb_bq_target_t* targets, uint64_t n_targets,
+                   QuantPlan* q) {
+  BqTables tb;
+  int st = block_fp8_compile(device, rects, n, targets, n_targets, &tb);
+  if (st) return st;
+  q->add(tb.blocks);
+  const size_t pieces = q->add(tb.pieces);
+  q->seal(0);
+  q->describe(n, static_cast<uint32_t>(tb.blocks.size()), kBqBlock * kBqBlock, tb);
+  q->launch = [pieces, n_blocks = static_cast<uint32_t>(tb.blocks.size()), es = tb.max_src_bytes](char* d, cudaStream_t s) {
+    return launch_block_fp8(reinterpret_cast<const BqBlock*>(d), reinterpret_cast<const BqPiece*>(d + pieces), n_blocks, es, s);
+  };
   return TSB_OK;
 }
+
+}  // namespace
 
 }  // namespace tsb
 
 using namespace tsb;
 
+extern "C" int tsb_block_fp8_plan_create(int device, const tsb_rect_t* rects, uint64_t n, const tsb_bq_target_t* targets,
+                                         uint64_t n_targets, uint32_t flags, tsb_plan_t* out) {
+  return quant_plan_create("tsb_block_fp8_plan_create", device, flags, out,
+                           [&](QuantPlan* q) { return block_fp8_plan(device, rects, n, targets, n_targets, q); });
+}
+
 extern "C" int tsb_block_fp8_compile_host(int device, const tsb_rect_t* rects, uint64_t n, const tsb_bq_target_t* targets,
                                           uint64_t n_targets, uint32_t flags, void* out_blocks, uint64_t block_cap,
                                           uint64_t* out_n_blocks, void* out_pieces, uint64_t piece_cap, uint64_t* out_n_pieces) {
-  if (flags != 0) return fail(TSB_ERR_INVALID, "tsb_block_fp8_compile_host: flags must be 0");
-  BqTables tb;
-  int st = block_fp8_compile(device, rects, n, targets, n_targets, &tb);
-  if (st) return st;
-  if (out_n_blocks) *out_n_blocks = tb.blocks.size();
-  if (out_n_pieces) *out_n_pieces = tb.pieces.size();
-  if (out_blocks) {
-    if (tb.blocks.size() > block_cap) return fail(TSB_ERR_NOMEM, "out_blocks too small");
-    if (!tb.blocks.empty()) memcpy(out_blocks, tb.blocks.data(), tb.blocks.size() * sizeof(BqBlock));
-  }
-  if (out_pieces) {
-    if (tb.pieces.size() > piece_cap) return fail(TSB_ERR_NOMEM, "out_pieces too small");
-    if (!tb.pieces.empty()) memcpy(out_pieces, tb.pieces.data(), tb.pieces.size() * sizeof(BqPiece));
-  }
-  return TSB_OK;
+  return quant_compile_host("tsb_block_fp8_compile_host", flags,
+                            [&](QuantPlan* q) { return block_fp8_plan(device, rects, n, targets, n_targets, q); },
+                            {{out_blocks, block_cap, out_n_blocks, "out_blocks"}, {out_pieces, piece_cap, out_n_pieces, "out_pieces"}},
+                            nullptr);
 }

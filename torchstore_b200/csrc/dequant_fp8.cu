@@ -22,32 +22,21 @@
 
 namespace tsb {
 
-namespace {
-
-bool aligned16(uint64_t p, int64_t stride, uint64_t rows) { return p % 16 == 0 && (rows == 1 || stride % 16 == 0); }
-
-}  // namespace
-
 int dq_source_geoms(const tsb_dq_source_t* sources, uint64_t n_sources, std::vector<TargetGeom>* out) {
+  constexpr GridRules kSourceRules{"source", "NULL src or scale", "src", "scale",
+                                   (1u << TSB_SCALE_PER_BLOCK) | (1u << TSB_SCALE_PER_CHANNEL) | (1u << TSB_SCALE_PER_TENSOR), 1ull << 31};
   std::vector<TargetGeom>& geom = *out;
   geom.resize(n_sources);
   for (uint64_t s = 0; s < n_sources; ++s) {
     const tsb_dq_source_t& S = sources[s];
-    const std::string where = "source " + std::to_string(s) + ": ";
-    if (!S.src || !S.scale) return fail(TSB_ERR_INVALID, where + "NULL src or scale");
-    if (!S.batch || !S.rows || !S.cols) return fail(TSB_ERR_INVALID, where + "empty source");
-    if (S.scale % 4) return fail(TSB_ERR_INVALID, where + "scale is not 4-byte aligned");
-    if (S.granularity != TSB_SCALE_PER_BLOCK && S.granularity != TSB_SCALE_PER_CHANNEL && S.granularity != TSB_SCALE_PER_TENSOR)
-      return fail(TSB_ERR_INVALID, where + "granularity must be TSB_SCALE_PER_BLOCK, TSB_SCALE_PER_CHANNEL or "
-                                           "TSB_SCALE_PER_TENSOR, not " + std::to_string(S.granularity));
-    if (S.pad) return fail(TSB_ERR_INVALID, where + "pad must be 0");
-    if (S.cols >= (1ull << 31) || S.rows >= (1ull << 31) || S.batch >= (1ull << 31) ||
-        S.batch * S.rows >= (1ull << 40) / S.cols || S.row0 >= (1ull << 40) || S.col0 >= (1ull << 40))
-      return fail(TSB_ERR_INVALID, where + "source too large");
+    int st = check_grid(kSourceRules, s, {S.src, S.scale, S.batch, S.rows, S.cols, S.row0, S.col0, 1, S.granularity, S.pad, !S.src || !S.scale});
+    if (st) return st;
     geom[s] = {S.src, S.batch, S.rows, S.cols};
   }
   return TSB_OK;
 }
+
+namespace {
 
 int dequant_fp8_compile(int device, const tsb_rect_t* rects, uint64_t n, const tsb_dq_source_t* sources,
                         uint64_t n_sources, DqTables* out) {
@@ -98,8 +87,7 @@ int dequant_fp8_compile(int device, const tsb_rect_t* rects, uint64_t n, const t
             t.vec = aligned16(t.src, t.src_stride, t.rows) && aligned16(t.dst, t.dst_stride, t.rows) ? 1 : 0;
             out->tiles.push_back(t);
             const uint64_t elems = static_cast<uint64_t>(t.rows) * t.cols;
-            out->src_bytes += elems;
-            if (x.src_device >= 0 && x.src_device != device) out->remote_src_bytes += elems;
+            out->read(elems, x.src_device, device);
             out->payload_bytes += elems * es;
           }
         }
@@ -111,10 +99,6 @@ int dequant_fp8_compile(int device, const tsb_rect_t* rects, uint64_t n, const t
   }
   return TSB_OK;
 }
-
-namespace {
-
-constexpr int kUnroll = 4;  // 16-element chunks in flight per thread
 
 // f32 -> destination bits: the fused cast's narrowing (copy_rects.cu), identity for f32
 template <uint32_t DT> __device__ __forceinline__ uint32_t narrow_bits(float y);
@@ -132,11 +116,11 @@ __device__ __forceinline__ void dequant_tile(const DqTile& t, const float* s_sca
   char* dst = reinterpret_cast<char*>(t.dst);
   const uint32_t cpr = (t.cols + 15u) / 16u;
   const uint32_t total = t.rows * cpr;
-  for (uint32_t base = threadIdx.x; base < total; base += kDqThreads * kUnroll) {
+  for (uint32_t base = threadIdx.x; base < total; base += kQuantThreads * kUnroll) {
     uint4 v[kUnroll];
 #pragma unroll
     for (int k = 0; k < kUnroll; ++k) {
-      const uint32_t idx = base + k * kDqThreads;
+      const uint32_t idx = base + k * kQuantThreads;
       if (idx < total) {
         const uint32_t r = idx / cpr, c = (idx - r * cpr) * 16u;
         if (t.vec && c + 16u <= t.cols) v[k] = ldg16(src + static_cast<int64_t>(r) * t.src_stride + c);
@@ -144,7 +128,7 @@ __device__ __forceinline__ void dequant_tile(const DqTile& t, const float* s_sca
     }
 #pragma unroll
     for (int k = 0; k < kUnroll; ++k) {
-      const uint32_t idx = base + k * kDqThreads;
+      const uint32_t idx = base + k * kQuantThreads;
       if (idx >= total) continue;
       const uint32_t r = idx / cpr, c = (idx - r * cpr) * 16u;
       const float scale = t.scale_step ? s_scale[r] : scale0;
@@ -183,13 +167,13 @@ __device__ __forceinline__ void dequant_tile(const DqTile& t, const float* s_sca
   }
 }
 
-__global__ void __launch_bounds__(kDqThreads) dequant_fp8_kernel(const DqTile* __restrict__ tiles) {
+__global__ void __launch_bounds__(kQuantThreads) dequant_fp8_kernel(const DqTile* __restrict__ tiles) {
   __shared__ float s_scale[kDqTileRows];
   const DqTile t = tiles[blockIdx.x];
   const float* scales = reinterpret_cast<const float*>(t.scale);
   float scale0 = 0.0f;
   if (t.scale_step) {  // per channel: one scale per row, fetched once
-    for (uint32_t r = threadIdx.x; r < t.rows; r += kDqThreads) s_scale[r] = __ldg(scales + r);
+    for (uint32_t r = threadIdx.x; r < t.rows; r += kQuantThreads) s_scale[r] = __ldg(scales + r);
     __syncthreads();
   } else {
     scale0 = __ldg(scales);
@@ -201,32 +185,39 @@ __global__ void __launch_bounds__(kDqThreads) dequant_fp8_kernel(const DqTile* _
   }
 }
 
-}  // namespace
-
-int launch_dequant_fp8(const DqTile* tiles, uint32_t n_tiles, cudaStream_t stream) {
-  if (!n_tiles) return TSB_OK;
-  dequant_fp8_kernel<<<n_tiles, kDqThreads, 0, stream>>>(tiles);
-  cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) return cuda_fail(e, "dequant_fp8_kernel launch");
-  count_launch();
+// d = DqTile table, one CTA per tile
+int dequant_fp8_plan(int device, const tsb_rect_t* rects, uint64_t n, const tsb_dq_source_t* sources, uint64_t n_sources,
+                     QuantPlan* q) {
+  DqTables tb;
+  int st = dequant_fp8_compile(device, rects, n, sources, n_sources, &tb);
+  if (st) return st;
+  q->add(tb.tiles);
+  q->seal(0);
+  const uint32_t n_tiles = static_cast<uint32_t>(tb.tiles.size());
+  q->describe(n, n_tiles, kDqTileElems, tb);
+  q->launch = [n_tiles](char* d, cudaStream_t s) {
+    dequant_fp8_kernel<<<n_tiles, kQuantThreads, 0, s>>>(reinterpret_cast<const DqTile*>(d));
+    return launched("dequant_fp8_kernel launch");
+  };
   return TSB_OK;
 }
+
+}  // namespace
 
 }  // namespace tsb
 
 using namespace tsb;
 
+extern "C" int tsb_dequant_fp8_plan_create(int device, const tsb_rect_t* rects, uint64_t n, const tsb_dq_source_t* sources,
+                                           uint64_t n_sources, uint32_t flags, tsb_plan_t* out) {
+  return quant_plan_create("tsb_dequant_fp8_plan_create", device, flags, out,
+                           [&](QuantPlan* q) { return dequant_fp8_plan(device, rects, n, sources, n_sources, q); });
+}
+
 extern "C" int tsb_dequant_fp8_compile_host(int device, const tsb_rect_t* rects, uint64_t n, const tsb_dq_source_t* sources,
                                             uint64_t n_sources, uint32_t flags, void* out_tiles, uint64_t tile_cap,
                                             uint64_t* out_n_tiles) {
-  if (flags != 0) return fail(TSB_ERR_INVALID, "tsb_dequant_fp8_compile_host: flags must be 0");
-  DqTables tb;
-  int st = dequant_fp8_compile(device, rects, n, sources, n_sources, &tb);
-  if (st) return st;
-  if (out_n_tiles) *out_n_tiles = tb.tiles.size();
-  if (out_tiles) {
-    if (tb.tiles.size() > tile_cap) return fail(TSB_ERR_NOMEM, "out_tiles too small");
-    if (!tb.tiles.empty()) memcpy(out_tiles, tb.tiles.data(), tb.tiles.size() * sizeof(DqTile));
-  }
-  return TSB_OK;
+  return quant_compile_host("tsb_dequant_fp8_compile_host", flags,
+                            [&](QuantPlan* q) { return dequant_fp8_plan(device, rects, n, sources, n_sources, q); },
+                            {{out_tiles, tile_cap, out_n_tiles, "out_tiles"}}, nullptr);
 }

@@ -1,6 +1,6 @@
-// Device helpers of the scaled fp8 quantisers (block_fp8.cu: 128x128 blocks; scaled_fp8.cu: per-channel
-// and per-tensor scales): exact widening of bf16/f16/f32 source bits to f32, |x| as an ordered integer,
-// the folding 16-byte loads, and the 16-element narrowing x * scale -> e4m3fn with its stores.
+// Device helpers of the scaled fp8 kernels (block_fp8.cu, scaled_fp8.cu, dequant_fp8.cu, requant_fp8.cu,
+// source_quant.cu): exact widening of bf16/f16/f32 source bits to f32, |x| as an ordered integer, the folding
+// 16-byte loads, the CTA max, and the 16-element narrowing x * scale -> e4m3fn with its stores.
 #pragma once
 
 #include <cuda_fp16.h>
@@ -10,6 +10,39 @@
 #include "tsb_internal.h"
 
 namespace tsb {
+
+// 16-byte loads (16-element chunks) in flight per thread.  4 at 6 CTAs per SM (block_fp8_kernel: 40 registers,
+// a bf16 stage is 32 KiB) measured faster on H100 than 8 at 4 CTAs per SM (64 registers), see DESIGN.md section 6.
+constexpr int kUnroll = 4;
+
+// The CTA's max of every thread's `m` (s_red: one word per warp), handed to thread0(max) in thread 0.
+template <class F>
+__device__ __forceinline__ void cta_max(uint32_t m, uint32_t* s_red, F&& thread0) {
+  m = __reduce_max_sync(0xffffffffu, m);
+  if ((threadIdx.x & 31u) == 0) s_red[threadIdx.x >> 5] = m;
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    uint32_t a = s_red[0];
+#pragma unroll
+    for (uint32_t w = 1; w < kQuantThreads / 32; ++w) a = max(a, s_red[w]);
+    thread0(a);
+  }
+}
+
+// The two passes over a plan's tiles (scaled_fp8.cu, requant_fp8.cu): clear the n_groups amax words on the
+// stream, then the amax kernel and the quantise kernel, one CTA per tile.  `name` prefixes the error messages.
+template <class Tile>
+int launch_two_pass(void (*amax_kernel)(const Tile*, uint32_t*), void (*quant_kernel)(const Tile*, const uint32_t*),
+                    const char* name, const Tile* tiles, uint32_t n_tiles, uint32_t* amax, uint32_t n_groups,
+                    cudaStream_t stream) {
+  const std::string what(name);
+  const cudaError_t e = cudaMemsetAsync(amax, 0, 4ull * n_groups, stream);
+  if (e != cudaSuccess) return cuda_fail(e, (what + " amax clear").c_str());
+  amax_kernel<<<n_tiles, kQuantThreads, 0, stream>>>(tiles, amax);
+  if (int st = launched((what + "_amax_kernel launch").c_str())) return st;
+  quant_kernel<<<n_tiles, kQuantThreads, 0, stream>>>(tiles, amax);
+  return launched((what + "_quant_kernel launch").c_str());
+}
 
 __device__ __forceinline__ uint4 ldg16(const char* p) {
   uint4 v;

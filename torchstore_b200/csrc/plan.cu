@@ -10,6 +10,7 @@
 #include <algorithm>
 #include <cstdlib>
 #include <cstring>
+#include <functional>
 #include <map>
 #include <mutex>
 #include <set>
@@ -40,35 +41,16 @@ TableLayout table_layout(size_t n_rects, size_t n_tiles, size_t n_link) {
   return l;
 }
 
-// What a plan's tables drive: the copy_rects kernel, the block-scaled fp8 quantiser
-// (d_block = {BqBlock table | BqPiece table}, num_tiles = blocks), or the per-channel / per-tensor
-// scaled fp8 quantisers (d_block = {SqBand table | SqPiece table | SqTile table | amax words}), or the
-// dequantiser of scaled fp8 sources (d_block = DqTile table, num_tiles = tiles), or the requantiser of scaled
-// fp8 sources into scaled fp8 destinations (d_block = {RqUnit table | RqPiece table | RqTile table | amax words}),
-// or the source-side quantiser (d_block = {SrcQUnit table | SqTile table | amax words}).
-enum : uint32_t {
-  PLAN_COPY = 0,
-  PLAN_BLOCK_FP8 = 1,
-  PLAN_SCALED_FP8 = 2,
-  PLAN_DEQUANT_FP8 = 3,
-  PLAN_REQUANT_FP8 = 4,
-  PLAN_SOURCE_QUANT = 5
-};
-
 struct Plan {
   int device = 0;
-  uint32_t plan_kind = PLAN_COPY;
   char* d_block = nullptr;
   TableLayout layout;
   uint32_t num_tiles = 0;
   uint32_t num_link_tiles = 0;
   uint32_t kind = KIND_GENERIC;
-  size_t bq_pieces_off = 0;    // PLAN_BLOCK_FP8: byte offset of the piece table in d_block
-  uint32_t bq_src_bytes = 2;   // PLAN_BLOCK_FP8: largest source element size
-  size_t sq_off[3] = {};       // PLAN_SCALED_FP8, PLAN_REQUANT_FP8, PLAN_SOURCE_QUANT: byte offsets of the piece and tile tables and the amax words
-  SqLaunch sq{};               // PLAN_SCALED_FP8: counts (run_plan fills in the table pointers)
-  RqLaunch rq{};               // PLAN_REQUANT_FP8: likewise
-  SrcQLaunch srcq{};           // PLAN_SOURCE_QUANT: likewise
+  // scaled fp8 plans: runs them from d_block (QuantPlan::launch); empty for copy plans, which d_block's
+  // {sched | rects | copy tiles | link tiles} drive through the copy_rects kernel
+  std::function<int(char*, cudaStream_t)> quant;
   uint32_t link_stage_bytes = 0;
   uint32_t link_stages = 0;
   tsb_plan_info_t info{};
@@ -569,33 +551,7 @@ int find_plan(tsb_plan_t plan, Plan** out) {
 }
 
 int run_plan(Plan* p, cudaStream_t s) {
-  if (p->plan_kind == PLAN_BLOCK_FP8)
-    return launch_block_fp8(reinterpret_cast<const BqBlock*>(p->d_block), reinterpret_cast<const BqPiece*>(p->d_block + p->bq_pieces_off),
-                            p->num_tiles, p->bq_src_bytes, s);
-  if (p->plan_kind == PLAN_SCALED_FP8) {
-    SqLaunch l = p->sq;
-    l.bands = reinterpret_cast<const SqBand*>(p->d_block);
-    l.pieces = reinterpret_cast<const SqPiece*>(p->d_block + p->sq_off[0]);
-    l.tiles = reinterpret_cast<const SqTile*>(p->d_block + p->sq_off[1]);
-    l.amax = reinterpret_cast<uint32_t*>(p->d_block + p->sq_off[2]);
-    return launch_scaled_fp8(l, s);
-  }
-  if (p->plan_kind == PLAN_DEQUANT_FP8) return launch_dequant_fp8(reinterpret_cast<const DqTile*>(p->d_block), p->num_tiles, s);
-  if (p->plan_kind == PLAN_REQUANT_FP8) {
-    RqLaunch l = p->rq;
-    l.units = reinterpret_cast<const RqUnit*>(p->d_block);
-    l.pieces = reinterpret_cast<const RqPiece*>(p->d_block + p->sq_off[0]);
-    l.tiles = reinterpret_cast<const RqTile*>(p->d_block + p->sq_off[1]);
-    l.amax = reinterpret_cast<uint32_t*>(p->d_block + p->sq_off[2]);
-    return launch_requant_fp8(l, s);
-  }
-  if (p->plan_kind == PLAN_SOURCE_QUANT) {
-    SrcQLaunch l = p->srcq;
-    l.units = reinterpret_cast<const SrcQUnit*>(p->d_block);
-    l.two_pass.tiles = reinterpret_cast<const SqTile*>(p->d_block + p->sq_off[1]);
-    l.two_pass.amax = reinterpret_cast<uint32_t*>(p->d_block + p->sq_off[2]);
-    return launch_source_quant(l, s);
-  }
+  if (p->quant) return p->quant(p->d_block, s);
   uint32_t kind = p->kind;
   if (getenv("TSB_FORCE_GENERIC")) kind = KIND_GENERIC;
   LaunchParams lp = make_params(p->d_block, p->layout, p->num_tiles, p->num_link_tiles, kind, p->link_stage_bytes, p->link_stages);
@@ -639,6 +595,42 @@ int register_plan(Plan* p, const std::vector<char>& host, tsb_plan_t* out) {
 }
 
 }  // namespace
+
+int quant_plan_create(const char* fn, int device, uint32_t flags, tsb_plan_t* out, const QuantCompile& compile) {
+  if (!out) return fail(TSB_ERR_INVALID, std::string(fn) + ": NULL argument");
+  if (flags != 0) return fail(TSB_ERR_INVALID, std::string(fn) + ": flags must be 0");
+  QuantPlan q;
+  int st = compile(&q);
+  if (st) return st;
+  Plan* p = new Plan();
+  p->device = device;
+  p->num_tiles = static_cast<uint32_t>(q.info.num_tiles);
+  p->info = q.info;
+  p->quant = std::move(q.launch);
+  return register_plan(p, q.tables, out);
+}
+
+int quant_compile_host(const char* fn, uint32_t flags, const QuantCompile& compile, std::initializer_list<TableOut> outs,
+                       uint64_t* out_n_groups) {
+  if (flags != 0) return fail(TSB_ERR_INVALID, std::string(fn) + ": flags must be 0");
+  QuantPlan q;
+  int st = compile(&q);
+  if (st) return st;
+  size_t k = 0;
+  for (const TableOut& o : outs) {
+    if (o.n) *o.n = q.sections[k].count;
+    ++k;
+  }
+  if (out_n_groups) *out_n_groups = q.n_groups;
+  k = 0;
+  for (const TableOut& o : outs) {
+    const QuantPlan::Section& t = q.sections[k++];
+    if (!o.out) continue;
+    if (t.count > o.cap) return fail(TSB_ERR_NOMEM, std::string(o.name) + " too small");
+    if (t.count) memcpy(o.out, q.tables.data() + t.off, t.bytes);
+  }
+  return TSB_OK;
+}
 
 int plans_shutdown() {
   PlanRegistry& reg = R();
@@ -721,161 +713,6 @@ int tsb_plan_create(int device, const tsb_rect_t* rects, uint64_t n, uint32_t fl
   p->layout = table_layout(cp.c.rects.size(), cp.tiles.size(), cp.link_tiles.size());
   std::vector<char> host(p->layout.total);
   fill_block(host.data(), p->layout, cp);
-  return register_plan(p, host, out);
-}
-
-int tsb_block_fp8_plan_create(int device, const tsb_rect_t* rects, uint64_t n, const tsb_bq_target_t* targets,
-                              uint64_t n_targets, uint32_t flags, tsb_plan_t* out) {
-  if (!out) return fail(TSB_ERR_INVALID, "tsb_block_fp8_plan_create: NULL argument");
-  if (flags != 0) return fail(TSB_ERR_INVALID, "tsb_block_fp8_plan_create: flags must be 0");
-  BqTables tb;
-  int st = block_fp8_compile(device, rects, n, targets, n_targets, &tb);
-  if (st) return st;
-  Plan* p = new Plan();
-  p->device = device;
-  p->plan_kind = PLAN_BLOCK_FP8;
-  p->num_tiles = static_cast<uint32_t>(tb.blocks.size());
-  p->bq_src_bytes = tb.max_src_bytes;
-  p->bq_pieces_off = tb.blocks.size() * sizeof(BqBlock);
-  p->info.num_rects = n;
-  p->info.num_tiles = tb.blocks.size();
-  p->info.payload_bytes = tb.payload_bytes;
-  p->info.src_bytes = tb.src_bytes;
-  p->info.remote_src_bytes = tb.remote_src_bytes;
-  p->info.grid = static_cast<uint32_t>(tb.blocks.size());
-  p->info.block = kBqThreads;
-  p->info.tile_bytes = kBqBlock * kBqBlock;
-  std::vector<char> host(std::max<size_t>(16, p->bq_pieces_off + tb.pieces.size() * sizeof(BqPiece)));
-  if (!tb.blocks.empty()) memcpy(host.data(), tb.blocks.data(), p->bq_pieces_off);
-  if (!tb.pieces.empty()) memcpy(host.data() + p->bq_pieces_off, tb.pieces.data(), tb.pieces.size() * sizeof(BqPiece));
-  return register_plan(p, host, out);
-}
-
-int tsb_scaled_fp8_plan_create(int device, const tsb_rect_t* rects, uint64_t n, const tsb_sq_target_t* targets,
-                               uint64_t n_targets, uint32_t flags, tsb_plan_t* out) {
-  if (!out) return fail(TSB_ERR_INVALID, "tsb_scaled_fp8_plan_create: NULL argument");
-  if (flags != 0) return fail(TSB_ERR_INVALID, "tsb_scaled_fp8_plan_create: flags must be 0");
-  SqTables tb;
-  int st = scaled_fp8_compile(device, rects, n, targets, n_targets, &tb);
-  if (st) return st;
-  const size_t pieces_off = tb.bands.size() * sizeof(SqBand);
-  const size_t tiles_off = pieces_off + tb.pieces.size() * sizeof(SqPiece);
-  const size_t amax_off = tiles_off + tb.tiles.size() * sizeof(SqTile);
-  std::vector<char> host(std::max<size_t>(16, amax_off + 4ull * tb.n_groups), 0);
-  if (!tb.bands.empty()) memcpy(host.data(), tb.bands.data(), pieces_off);
-  if (!tb.pieces.empty()) memcpy(host.data() + pieces_off, tb.pieces.data(), tiles_off - pieces_off);
-  if (!tb.tiles.empty()) memcpy(host.data() + tiles_off, tb.tiles.data(), amax_off - tiles_off);
-  Plan* p = new Plan();
-  p->device = device;
-  p->plan_kind = PLAN_SCALED_FP8;
-  p->num_tiles = static_cast<uint32_t>(tb.bands.size() + tb.tiles.size());
-  p->info.num_rects = n;
-  p->info.num_tiles = p->num_tiles;
-  p->info.payload_bytes = tb.payload_bytes;
-  p->info.src_bytes = tb.src_bytes;
-  p->info.remote_src_bytes = tb.remote_src_bytes;
-  p->info.grid = p->num_tiles;
-  p->info.block = kSqThreads;
-  p->info.tile_bytes = kSqStageBytes;
-  p->sq_off[0] = pieces_off;
-  p->sq_off[1] = tiles_off;
-  p->sq_off[2] = amax_off;
-  p->sq.n_bands = static_cast<uint32_t>(tb.bands.size());
-  p->sq.n_tiles = static_cast<uint32_t>(tb.tiles.size());
-  p->sq.n_groups = tb.n_groups;
-  p->sq.stage_bytes = tb.stage_bytes;
-  return register_plan(p, host, out);
-}
-
-int tsb_dequant_fp8_plan_create(int device, const tsb_rect_t* rects, uint64_t n, const tsb_dq_source_t* sources,
-                                uint64_t n_sources, uint32_t flags, tsb_plan_t* out) {
-  if (!out) return fail(TSB_ERR_INVALID, "tsb_dequant_fp8_plan_create: NULL argument");
-  if (flags != 0) return fail(TSB_ERR_INVALID, "tsb_dequant_fp8_plan_create: flags must be 0");
-  DqTables tb;
-  int st = dequant_fp8_compile(device, rects, n, sources, n_sources, &tb);
-  if (st) return st;
-  std::vector<char> host(std::max<size_t>(16, tb.tiles.size() * sizeof(DqTile)), 0);
-  if (!tb.tiles.empty()) memcpy(host.data(), tb.tiles.data(), tb.tiles.size() * sizeof(DqTile));
-  Plan* p = new Plan();
-  p->device = device;
-  p->plan_kind = PLAN_DEQUANT_FP8;
-  p->num_tiles = static_cast<uint32_t>(tb.tiles.size());
-  p->info.num_rects = n;
-  p->info.num_tiles = tb.tiles.size();
-  p->info.payload_bytes = tb.payload_bytes;
-  p->info.src_bytes = tb.src_bytes;
-  p->info.remote_src_bytes = tb.remote_src_bytes;
-  p->info.grid = p->num_tiles;
-  p->info.block = kDqThreads;
-  p->info.tile_bytes = kDqTileElems;
-  return register_plan(p, host, out);
-}
-
-int tsb_requant_fp8_plan_create(int device, const tsb_rect_t* rects, uint64_t n, const tsb_dq_source_t* sources,
-                                uint64_t n_sources, const tsb_sq_target_t* targets, uint64_t n_targets, uint32_t flags,
-                                tsb_plan_t* out) {
-  if (!out) return fail(TSB_ERR_INVALID, "tsb_requant_fp8_plan_create: NULL argument");
-  if (flags != 0) return fail(TSB_ERR_INVALID, "tsb_requant_fp8_plan_create: flags must be 0");
-  RqTables tb;
-  int st = requant_fp8_compile(device, rects, n, sources, n_sources, targets, n_targets, &tb);
-  if (st) return st;
-  const size_t pieces_off = tb.units.size() * sizeof(RqUnit);
-  const size_t tiles_off = pieces_off + tb.pieces.size() * sizeof(RqPiece);
-  const size_t amax_off = tiles_off + tb.tiles.size() * sizeof(RqTile);
-  std::vector<char> host(std::max<size_t>(16, amax_off + 4ull * tb.n_groups), 0);
-  if (!tb.units.empty()) memcpy(host.data(), tb.units.data(), pieces_off);
-  if (!tb.pieces.empty()) memcpy(host.data() + pieces_off, tb.pieces.data(), tiles_off - pieces_off);
-  if (!tb.tiles.empty()) memcpy(host.data() + tiles_off, tb.tiles.data(), amax_off - tiles_off);
-  Plan* p = new Plan();
-  p->device = device;
-  p->plan_kind = PLAN_REQUANT_FP8;
-  p->num_tiles = static_cast<uint32_t>(tb.units.size() + tb.tiles.size());
-  p->info.num_rects = n;
-  p->info.num_tiles = p->num_tiles;
-  p->info.payload_bytes = tb.payload_bytes;
-  p->info.src_bytes = tb.src_bytes;
-  p->info.remote_src_bytes = tb.remote_src_bytes;
-  p->info.grid = p->num_tiles;
-  p->info.block = kRqThreads;
-  p->info.tile_bytes = tb.stage_bytes;
-  p->sq_off[0] = pieces_off;
-  p->sq_off[1] = tiles_off;
-  p->sq_off[2] = amax_off;
-  p->rq.n_units = static_cast<uint32_t>(tb.units.size());
-  p->rq.n_tiles = static_cast<uint32_t>(tb.tiles.size());
-  p->rq.n_groups = tb.n_groups;
-  p->rq.stage_bytes = tb.stage_bytes;
-  return register_plan(p, host, out);
-}
-
-int tsb_source_quant_plan_create(int device, const tsb_source_quant_target_t* targets, uint64_t n, uint32_t flags,
-                                 tsb_plan_t* out) {
-  if (!out) return fail(TSB_ERR_INVALID, "tsb_source_quant_plan_create: NULL argument");
-  if (flags != 0) return fail(TSB_ERR_INVALID, "tsb_source_quant_plan_create: flags must be 0");
-  SrcQTables tb;
-  int st = source_quant_compile(targets, n, &tb);
-  if (st) return st;
-  const size_t tiles_off = tb.units.size() * sizeof(SrcQUnit);
-  const size_t amax_off = tiles_off + tb.tiles.size() * sizeof(SqTile);
-  std::vector<char> host(std::max<size_t>(16, amax_off + 4ull * tb.n_groups), 0);
-  if (!tb.units.empty()) memcpy(host.data(), tb.units.data(), tiles_off);
-  if (!tb.tiles.empty()) memcpy(host.data() + tiles_off, tb.tiles.data(), amax_off - tiles_off);
-  Plan* p = new Plan();
-  p->device = device;
-  p->plan_kind = PLAN_SOURCE_QUANT;
-  p->num_tiles = static_cast<uint32_t>(tb.units.size() + tb.tiles.size());
-  for (int k = 0; k < 3; ++k) p->srcq.n_units[k] = tb.n_units[k];
-  p->info.num_rects = n;
-  p->info.num_tiles = p->num_tiles;
-  p->info.payload_bytes = tb.payload_bytes;
-  p->info.src_bytes = tb.src_bytes;
-  p->info.grid = p->num_tiles;
-  p->info.block = kSrcQThreads;
-  p->info.tile_bytes = tb.unit_bytes;
-  p->sq_off[1] = tiles_off;
-  p->sq_off[2] = amax_off;
-  p->srcq.two_pass.n_tiles = static_cast<uint32_t>(tb.tiles.size());
-  p->srcq.two_pass.n_groups = tb.n_groups;
   return register_plan(p, host, out);
 }
 

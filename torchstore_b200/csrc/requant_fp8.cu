@@ -35,8 +35,6 @@ namespace tsb {
 
 namespace {
 
-uint32_t round16(uint32_t x) { return (x + 15u) & ~15u; }
-
 // A box of a destination matrix read from one source under one scale, or one per row.
 struct Seg {
   uint64_t t, b, r0, c0, er, ec;  // target, matrix, first row and column, extent
@@ -98,10 +96,7 @@ struct Compiler {
   const tsb_sq_target_t* targets;
   RqTables* out;
 
-  void count(uint64_t elems, const Seg& x) {
-    out->src_bytes += elems;
-    if (x.src_device >= 0 && x.src_device != device) out->remote_src_bytes += elems;
-  }
+  void count(uint64_t elems, const Seg& x) { out->read(elems, x.src_device, device); }
 
   // rows [y0, y0 + h) and columns [c0, c0 + w) of segment x as a piece at (row0, col0) of a unit
   void piece(const Seg& x, uint64_t y0, uint64_t h, uint64_t c0, uint64_t w, uint64_t row0, uint64_t col0) {
@@ -118,8 +113,7 @@ struct Compiler {
     p.col0 = static_cast<uint32_t>(col0);
     p.rows = static_cast<uint32_t>(h);
     p.cols = static_cast<uint32_t>(w);
-    p.vec = (p.src % 16 == 0 && (h == 1 || p.src_stride % 16 == 0) && w % 16 == 0 && col0 % 16 == 0 && p.col_phase % 16 == 0)
-                ? 1u : 0u;
+    p.vec = (vec_ok(p.src, p.src_stride, h, w, 1) && col0 % 16 == 0 && p.col_phase % 16 == 0) ? 1u : 0u;
     out->pieces.push_back(p);
     count(h * w, x);
   }
@@ -161,7 +155,7 @@ struct Compiler {
         t.rows = static_cast<uint32_t>(rows);
         t.cols = static_cast<uint32_t>(cols);
         t.group = g;
-        t.vec = (t.src % 16 == 0 && (rows == 1 || t.src_stride % 16 == 0)) ? 1u : 0u;
+        t.vec = aligned16(t.src, t.src_stride, rows) ? 1u : 0u;
         t.scale_inv = first_row && r == 0 && x.c0 + c == 0 ? scale_inv : 0;
         out->tiles.push_back(t);
         count(rows * cols, x);
@@ -170,40 +164,20 @@ struct Compiler {
     }
   }
 
-  // Exact coverage of matrix b of target t by its segments (sorted by first row): a sweep between
-  // consecutive segment row boundaries, in time proportional to the segments.
+  // Exact coverage of matrix b of target t by its segments (sorted by first row).
   int check_cover(uint64_t t, uint64_t b, const Seg* const* segs, size_t ns) {
     const tsb_sq_target_t& T = targets[t];
-    std::vector<const Seg*> act;
-    size_t i = 0;
-    for (uint64_t y = 0; y < T.rows;) {
-      while (i < ns && segs[i]->r0 == y) act.push_back(segs[i++]);
-      act.erase(std::remove_if(act.begin(), act.end(), [y](const Seg* x) { return x->r0 + x->er <= y; }), act.end());
-      uint64_t y1 = i < ns ? segs[i]->r0 : T.rows;
-      for (const Seg* x : act) y1 = std::min(y1, x->r0 + x->er);
-      std::sort(act.begin(), act.end(), [](const Seg* a, const Seg* c) { return a->c0 < c->c0; });
-      uint64_t c = 0;
-      bool ok = true;
-      for (const Seg* x : act) {
-        if (x->c0 != c) {
-          ok = false;
-          c = std::min(c, x->c0);
-          break;
-        }
-        c += x->ec;
-      }
-      if (!ok || c != T.cols) {
-        std::string grp = "target " + std::to_string(t) + " group (" + std::to_string(b);
-        if (T.granularity == TSB_SCALE_PER_BLOCK)
-          grp += ", " + std::to_string(y / kBqBlock) + ", " + std::to_string(std::min(c, T.cols - 1) / kBqBlock);
-        else if (T.granularity == TSB_SCALE_PER_CHANNEL)
-          grp += ", " + std::to_string(y);
-        return fail(TSB_ERR_INVALID, grp + "): its elements are not all written exactly once (at row " + std::to_string(y) +
-                                         ", column " + std::to_string(std::min(c, T.cols - 1)) + ")");
-      }
-      y = y1;
-    }
-    return TSB_OK;
+    return sweep_cover(
+        T.rows, T.cols, segs, ns, [](uint64_t, uint64_t, const std::vector<const Seg*>&) { return 0; },
+        [&](uint64_t y, uint64_t c) {
+          std::string grp = "target " + std::to_string(t) + " group (" + std::to_string(b);
+          if (T.granularity == TSB_SCALE_PER_BLOCK)
+            grp += ", " + std::to_string(y / kBqBlock) + ", " + std::to_string(c / kBqBlock);
+          else if (T.granularity == TSB_SCALE_PER_CHANNEL)
+            grp += ", " + std::to_string(y);
+          return fail(TSB_ERR_INVALID, grp + "): its elements are not all written exactly once (at row " + std::to_string(y) +
+                                           ", column " + std::to_string(c) + ")");
+        });
   }
 
   // Emit the work of matrix b of target t.
@@ -264,7 +238,8 @@ struct Compiler {
   }
 };
 
-}  // namespace
+constexpr GridRules kTargetRules{"target", "NULL dst or scale_inv", "dst", "scale_inv",
+                                 (1u << TSB_SCALE_PER_BLOCK) | (1u << TSB_SCALE_PER_CHANNEL) | (1u << TSB_SCALE_PER_TENSOR), 1ull << 31};
 
 int requant_fp8_compile(int device, const tsb_rect_t* rects, uint64_t n, const tsb_dq_source_t* sources, uint64_t n_sources,
                         const tsb_sq_target_t* targets, uint64_t n_targets, RqTables* out) {
@@ -277,17 +252,9 @@ int requant_fp8_compile(int device, const tsb_rect_t* rects, uint64_t n, const t
   std::vector<uint64_t> base(n_targets + 1, 0);  // matrix index of every target's first matrix
   for (uint64_t t = 0; t < n_targets; ++t) {
     const tsb_sq_target_t& T = targets[t];
-    const std::string where = "target " + std::to_string(t) + ": ";
-    if (!T.dst || !T.scale_inv) return fail(TSB_ERR_INVALID, where + "NULL dst or scale_inv");
-    if (!T.batch || !T.rows || !T.cols) return fail(TSB_ERR_INVALID, where + "empty target");
-    if (T.scale_inv % 4) return fail(TSB_ERR_INVALID, where + "scale_inv is not 4-byte aligned");
-    if (T.granularity != TSB_SCALE_PER_BLOCK && T.granularity != TSB_SCALE_PER_CHANNEL && T.granularity != TSB_SCALE_PER_TENSOR)
-      return fail(TSB_ERR_INVALID, where + "granularity must be TSB_SCALE_PER_BLOCK, TSB_SCALE_PER_CHANNEL or "
-                                           "TSB_SCALE_PER_TENSOR, not " + std::to_string(T.granularity));
-    if (T.pad) return fail(TSB_ERR_INVALID, where + "pad must be 0");
-    if (T.cols >= (1ull << 31) || T.rows >= (1ull << 31) || T.batch >= (1ull << 31) ||
-        T.batch * T.rows >= (1ull << 40) / T.cols)
-      return fail(TSB_ERR_INVALID, where + "target too large");
+    if ((st = check_grid(kTargetRules, t, {T.dst, T.scale_inv, T.batch, T.rows, T.cols, 0, 0, 1, T.granularity, T.pad,
+                                           !T.dst || !T.scale_inv})))
+      return st;
     geom[t] = {T.dst, T.batch, T.rows, T.cols};
     base[t + 1] = base[t] + T.batch;
     const uint64_t groups = T.granularity == TSB_SCALE_PER_BLOCK ? ((T.rows + kBqBlock - 1) / kBqBlock) * ((T.cols + kBqBlock - 1) / kBqBlock)
@@ -324,10 +291,6 @@ int requant_fp8_compile(int device, const tsb_rect_t* rects, uint64_t n, const t
   }
   return TSB_OK;
 }
-
-namespace {
-
-constexpr int kUnroll = 4;  // 16-byte loads in flight per thread
 
 // max abs_bits of the 16 scaled elements of v
 __device__ __forceinline__ uint32_t fold_scaled16(uint32_t m, const uint4& v, float scale) {
@@ -382,7 +345,7 @@ __device__ __forceinline__ uint32_t stage_unit(const RqUnit& u, const RqPiece* _
       // each warp takes 32 * kUnroll consecutive 16-byte units per step (coalesced 512-byte loads)
       const uint32_t upr = p.cols / 16;
       const uint32_t total = p.rows * upr;
-      for (uint32_t base = warp * 32 * kUnroll; base < total; base += kRqThreads * kUnroll) {
+      for (uint32_t base = warp * 32 * kUnroll; base < total; base += kQuantThreads * kUnroll) {
         uint4 v[kUnroll];
 #pragma unroll
         for (int k = 0; k < kUnroll; ++k) {
@@ -418,7 +381,7 @@ __device__ __forceinline__ uint32_t stage_unit(const RqUnit& u, const RqPiece* _
       }
     } else {
       const uint32_t total = p.rows * p.cols;
-      for (uint32_t base = warp * 32; base < total; base += kRqThreads) {
+      for (uint32_t base = warp * 32; base < total; base += kQuantThreads) {
         const uint32_t idx = base + lane;
         const uint32_t rf = base / p.cols, rl = (min(base + 32, total) - 1) / p.cols;
         uint32_t m = 0;
@@ -451,7 +414,7 @@ __device__ __forceinline__ void quantise_unit(const RqUnit& u, const RqPiece* __
     const RqPiece p = pieces[u.piece0 + q];
     const uint32_t cpr = (p.cols + 15u) / 16u;
     const uint32_t total = p.rows * cpr;
-    for (uint32_t idx = threadIdx.x; idx < total; idx += kRqThreads) {
+    for (uint32_t idx = threadIdx.x; idx < total; idx += kQuantThreads) {
       const uint32_t r = idx / cpr, c = (idx - r * cpr) * 16u;
       const uint32_t nvalid = min(16u, p.cols - c);
       const uint32_t row = p.row0 + r, col = p.col0 + c;
@@ -475,42 +438,36 @@ __device__ __forceinline__ void run_unit(const RqUnit& u, const RqPiece* pieces,
                                          float* s_scale, uint32_t* s_red) {
   const uint32_t spitch = (u.cols + 15u) & ~15u;
   if (kPerRow) {
-    for (uint32_t r = threadIdx.x; r < u.rows; r += kRqThreads) s_amax[r] = 0;
+    for (uint32_t r = threadIdx.x; r < u.rows; r += kQuantThreads) s_amax[r] = 0;
     __syncthreads();
   }
   uint32_t m = stage_unit<kPerRow>(u, pieces, smem, spitch, s_amax);
   if (kPerRow) {
     __syncthreads();
-    for (uint32_t r = threadIdx.x; r < u.rows; r += kRqThreads) {
+    for (uint32_t r = threadIdx.x; r < u.rows; r += kQuantThreads) {
       float scale, scale_inv;
       scales_of_amax(s_amax[r], &scale, &scale_inv);
       s_scale[r] = scale;
       reinterpret_cast<float*>(u.scale_inv)[r] = scale_inv;
     }
   } else {
-    m = __reduce_max_sync(0xffffffffu, m);
-    if ((threadIdx.x & 31u) == 0) s_red[threadIdx.x >> 5] = m;
-    __syncthreads();
-    if (threadIdx.x == 0) {
-      uint32_t a = s_red[0];
-#pragma unroll
-      for (uint32_t w = 1; w < kRqThreads / 32; ++w) a = max(a, s_red[w]);
+    cta_max(m, s_red, [&](uint32_t a) {
       float scale, scale_inv;
       scales_of_amax(a, &scale, &scale_inv);
       s_scale[0] = scale;
       *reinterpret_cast<float*>(u.scale_inv) = scale_inv;
-    }
+    });
   }
   __syncthreads();
   quantise_unit<kPerRow>(u, pieces, smem, spitch, s_scale);
 }
 
-__global__ void __launch_bounds__(kRqThreads) requant_fp8_staged_kernel(const RqUnit* __restrict__ units,
+__global__ void __launch_bounds__(kQuantThreads) requant_fp8_staged_kernel(const RqUnit* __restrict__ units,
                                                                         const RqPiece* __restrict__ pieces) {
   extern __shared__ __align__(16) unsigned char stage[];
   __shared__ uint32_t s_amax[kSqBandRows];
   __shared__ float s_scale[kSqBandRows];
-  __shared__ uint32_t s_red[kRqThreads / 32];
+  __shared__ uint32_t s_red[kQuantThreads / 32];
   const RqUnit u = units[blockIdx.x];
   if (u.per_row)
     run_unit<true>(u, pieces, stage, s_amax, s_scale, s_red);
@@ -518,19 +475,19 @@ __global__ void __launch_bounds__(kRqThreads) requant_fp8_staged_kernel(const Rq
     run_unit<false>(u, pieces, stage, s_amax, s_scale, s_red);
 }
 
-__global__ void __launch_bounds__(kRqThreads) requant_fp8_amax_kernel(const RqTile* __restrict__ tiles, uint32_t* amax) {
-  __shared__ uint32_t s_red[kRqThreads / 32];
+__global__ void __launch_bounds__(kQuantThreads) requant_fp8_amax_kernel(const RqTile* __restrict__ tiles, uint32_t* amax) {
+  __shared__ uint32_t s_red[kQuantThreads / 32];
   const RqTile t = tiles[blockIdx.x];
   const char* src = reinterpret_cast<const char*>(t.src);
   const float scale0 = __ldg(reinterpret_cast<const float*>(t.scale));
   const uint32_t cpr = (t.cols + 15u) / 16u;
   const uint32_t total = t.rows * cpr;
   uint32_t m = 0;
-  for (uint32_t base = threadIdx.x; base < total; base += kRqThreads * kUnroll) {
+  for (uint32_t base = threadIdx.x; base < total; base += kQuantThreads * kUnroll) {
     uint4 v[kUnroll];
 #pragma unroll
     for (int k = 0; k < kUnroll; ++k) {
-      const uint32_t idx = base + k * kRqThreads;
+      const uint32_t idx = base + k * kQuantThreads;
       if (idx < total) {
         const uint32_t r = idx / cpr, c = (idx - r * cpr) * 16u;
         if (t.vec && c + 16u <= t.cols) v[k] = ldg16(src + static_cast<int64_t>(r) * t.src_stride + c);
@@ -538,7 +495,7 @@ __global__ void __launch_bounds__(kRqThreads) requant_fp8_amax_kernel(const RqTi
     }
 #pragma unroll
     for (int k = 0; k < kUnroll; ++k) {
-      const uint32_t idx = base + k * kRqThreads;
+      const uint32_t idx = base + k * kQuantThreads;
       if (idx >= total) continue;
       const uint32_t r = idx / cpr, c = (idx - r * cpr) * 16u;
       const float scale = row_scale(t.scale, t.scale_step, r, scale0);
@@ -551,18 +508,12 @@ __global__ void __launch_bounds__(kRqThreads) requant_fp8_amax_kernel(const RqTi
       }
     }
   }
-  m = __reduce_max_sync(0xffffffffu, m);
-  if ((threadIdx.x & 31u) == 0) s_red[threadIdx.x >> 5] = m;
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    uint32_t a = s_red[0];
-#pragma unroll
-    for (uint32_t w = 1; w < kRqThreads / 32; ++w) a = max(a, s_red[w]);
+  cta_max(m, s_red, [&](uint32_t a) {
     if (a) atomicMax(amax + t.group, a);
-  }
+  });
 }
 
-__global__ void __launch_bounds__(kRqThreads) requant_fp8_quant_kernel(const RqTile* __restrict__ tiles,
+__global__ void __launch_bounds__(kQuantThreads) requant_fp8_quant_kernel(const RqTile* __restrict__ tiles,
                                                                        const uint32_t* __restrict__ amax) {
   const RqTile t = tiles[blockIdx.x];
   float dscale, scale_inv;
@@ -572,7 +523,7 @@ __global__ void __launch_bounds__(kRqThreads) requant_fp8_quant_kernel(const RqT
   const float scale0 = __ldg(reinterpret_cast<const float*>(t.scale));
   const uint32_t cpr = (t.cols + 15u) / 16u;
   const uint32_t total = t.rows * cpr;
-  for (uint32_t idx = threadIdx.x; idx < total; idx += kRqThreads) {
+  for (uint32_t idx = threadIdx.x; idx < total; idx += kQuantThreads) {
     const uint32_t r = idx / cpr, c = (idx - r * cpr) * 16u;
     const uint32_t nvalid = min(16u, t.cols - c);
     const char* s = src + static_cast<int64_t>(r) * t.src_stride + c;
@@ -589,55 +540,52 @@ __global__ void __launch_bounds__(kRqThreads) requant_fp8_quant_kernel(const RqT
   }
 }
 
-}  // namespace
-
-int launch_requant_fp8(const RqLaunch& l, cudaStream_t stream) {
-  cudaError_t e = cudaSuccess;
-  if (l.n_units) {
-    requant_fp8_staged_kernel<<<l.n_units, kRqThreads, l.stage_bytes, stream>>>(l.units, l.pieces);
-    if ((e = cudaGetLastError()) != cudaSuccess) return cuda_fail(e, "requant_fp8_staged_kernel launch");
-    count_launch();
-  }
-  if (l.n_tiles) {
-    if ((e = cudaMemsetAsync(l.amax, 0, 4ull * l.n_groups, stream)) != cudaSuccess) return cuda_fail(e, "requant_fp8 amax clear");
-    requant_fp8_amax_kernel<<<l.n_tiles, kRqThreads, 0, stream>>>(l.tiles, l.amax);
-    if ((e = cudaGetLastError()) != cudaSuccess) return cuda_fail(e, "requant_fp8_amax_kernel launch");
-    count_launch();
-    requant_fp8_quant_kernel<<<l.n_tiles, kRqThreads, 0, stream>>>(l.tiles, l.amax);
-    if ((e = cudaGetLastError()) != cudaSuccess) return cuda_fail(e, "requant_fp8_quant_kernel launch");
-    count_launch();
-  }
+// d = {RqUnit table | RqPiece table | RqTile table | amax words}, one CTA per unit and per tile (and pass)
+int requant_fp8_plan(int device, const tsb_rect_t* rects, uint64_t n, const tsb_dq_source_t* sources, uint64_t n_sources,
+                     const tsb_sq_target_t* targets, uint64_t n_targets, QuantPlan* q) {
+  RqTables tb;
+  int st = requant_fp8_compile(device, rects, n, sources, n_sources, targets, n_targets, &tb);
+  if (st) return st;
+  q->add(tb.units);
+  const size_t pieces = q->add(tb.pieces), tiles = q->add(tb.tiles), amax = q->seal(tb.n_groups);
+  q->describe(n, static_cast<uint32_t>(tb.units.size() + tb.tiles.size()), tb.stage_bytes, tb);
+  q->launch = [pieces, tiles, amax, n_units = static_cast<uint32_t>(tb.units.size()), n_tiles = static_cast<uint32_t>(tb.tiles.size()),
+               n_groups = tb.n_groups, stage_bytes = tb.stage_bytes](char* d, cudaStream_t s) -> int {
+    if (n_units) {
+      requant_fp8_staged_kernel<<<n_units, kQuantThreads, stage_bytes, s>>>(reinterpret_cast<const RqUnit*>(d),
+                                                                         reinterpret_cast<const RqPiece*>(d + pieces));
+      if (int st = launched("requant_fp8_staged_kernel launch")) return st;
+    }
+    if (!n_tiles) return TSB_OK;
+    return launch_two_pass(requant_fp8_amax_kernel, requant_fp8_quant_kernel, "requant_fp8", reinterpret_cast<const RqTile*>(d + tiles),
+                           n_tiles, reinterpret_cast<uint32_t*>(d + amax), n_groups, s);
+  };
   return TSB_OK;
 }
+
+}  // namespace
 
 }  // namespace tsb
 
 using namespace tsb;
+
+extern "C" int tsb_requant_fp8_plan_create(int device, const tsb_rect_t* rects, uint64_t n, const tsb_dq_source_t* sources,
+                                           uint64_t n_sources, const tsb_sq_target_t* targets, uint64_t n_targets, uint32_t flags,
+                                           tsb_plan_t* out) {
+  return quant_plan_create("tsb_requant_fp8_plan_create", device, flags, out, [&](QuantPlan* q) {
+    return requant_fp8_plan(device, rects, n, sources, n_sources, targets, n_targets, q);
+  });
+}
 
 extern "C" int tsb_requant_fp8_compile_host(int device, const tsb_rect_t* rects, uint64_t n, const tsb_dq_source_t* sources,
                                             uint64_t n_sources, const tsb_sq_target_t* targets, uint64_t n_targets,
                                             uint32_t flags, void* out_units, uint64_t unit_cap, uint64_t* out_n_units,
                                             void* out_pieces, uint64_t piece_cap, uint64_t* out_n_pieces, void* out_tiles,
                                             uint64_t tile_cap, uint64_t* out_n_tiles, uint64_t* out_n_groups) {
-  if (flags != 0) return fail(TSB_ERR_INVALID, "tsb_requant_fp8_compile_host: flags must be 0");
-  RqTables tb;
-  int st = requant_fp8_compile(device, rects, n, sources, n_sources, targets, n_targets, &tb);
-  if (st) return st;
-  if (out_n_units) *out_n_units = tb.units.size();
-  if (out_n_pieces) *out_n_pieces = tb.pieces.size();
-  if (out_n_tiles) *out_n_tiles = tb.tiles.size();
-  if (out_n_groups) *out_n_groups = tb.n_groups;
-  if (out_units) {
-    if (tb.units.size() > unit_cap) return fail(TSB_ERR_NOMEM, "out_units too small");
-    if (!tb.units.empty()) memcpy(out_units, tb.units.data(), tb.units.size() * sizeof(RqUnit));
-  }
-  if (out_pieces) {
-    if (tb.pieces.size() > piece_cap) return fail(TSB_ERR_NOMEM, "out_pieces too small");
-    if (!tb.pieces.empty()) memcpy(out_pieces, tb.pieces.data(), tb.pieces.size() * sizeof(RqPiece));
-  }
-  if (out_tiles) {
-    if (tb.tiles.size() > tile_cap) return fail(TSB_ERR_NOMEM, "out_tiles too small");
-    if (!tb.tiles.empty()) memcpy(out_tiles, tb.tiles.data(), tb.tiles.size() * sizeof(RqTile));
-  }
-  return TSB_OK;
+  return quant_compile_host(
+      "tsb_requant_fp8_compile_host", flags,
+      [&](QuantPlan* q) { return requant_fp8_plan(device, rects, n, sources, n_sources, targets, n_targets, q); },
+      {{out_units, unit_cap, out_n_units, "out_units"}, {out_pieces, piece_cap, out_n_pieces, "out_pieces"},
+       {out_tiles, tile_cap, out_n_tiles, "out_tiles"}},
+      out_n_groups);
 }

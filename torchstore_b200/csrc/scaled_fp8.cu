@@ -32,21 +32,12 @@ namespace tsb {
 
 namespace {
 
-uint32_t round16(uint32_t x) { return (x + 15u) & ~15u; }
-
-bool vec_ok(uint64_t src, int64_t stride, uint64_t rows, uint64_t cols, uint32_t es) {
-  return src % 16 == 0 && (rows == 1 || stride % 16 == 0) && (cols * es) % 16 == 0;
-}
-
 struct Compiler {
   int device;
   const tsb_sq_target_t* targets;
   SqTables* out;
 
-  void count(uint64_t bytes, const TargetBox& x) {
-    out->src_bytes += bytes;
-    if (x.src_device >= 0 && x.src_device != device) out->remote_src_bytes += bytes;
-  }
+  void count(uint64_t bytes, const TargetBox& x) { out->read(bytes, x.src_device, device); }
 
   // rows [y0, y1) of box x as two-pass tiles of group g; the tile holding the group's element (0, 0)
   // writes `scale`
@@ -124,46 +115,33 @@ struct Compiler {
   int matrix(uint64_t t, uint64_t b, const TargetBox* const* boxes, size_t nb) {
     const tsb_sq_target_t& T = targets[t];
     const bool tensor = T.granularity == TSB_SCALE_PER_TENSOR;
-    const std::string where = "target " + std::to_string(t) + " group (" + std::to_string(b);  // + ")" or ", row)"
-    std::vector<const TargetBox*> act, sorted;
+    const auto group = [&](uint64_t y) {
+      return "target " + std::to_string(t) + " group (" + std::to_string(b) + (tensor ? std::string(")") : ", " + std::to_string(y) + ")");
+    };
     uint32_t g = 0;
     uint32_t dtype = nb ? boxes[0]->dtype : 0;
-    size_t i = 0;
-    for (uint64_t y = 0; y < T.rows;) {
-      while (i < nb && boxes[i]->r0 == y) act.push_back(boxes[i++]);
-      act.erase(std::remove_if(act.begin(), act.end(), [y](const TargetBox* x) { return x->r0 + x->er <= y; }), act.end());
-      const std::string grp = where + (tensor ? std::string(")") : ", " + std::to_string(y) + ")");
-      uint64_t y1 = i < nb ? boxes[i]->r0 : T.rows;
-      for (const TargetBox* x : act) y1 = std::min(y1, x->r0 + x->er);
-      sorted = act;
-      std::sort(sorted.begin(), sorted.end(), [](const TargetBox* a, const TargetBox* c) { return a->c0 < c->c0; });
-      uint64_t c = 0;
-      bool tiled = !sorted.empty();
-      for (const TargetBox* x : sorted) {
-        if (x->c0 != c) {
-          tiled = false;
-          break;
-        }
-        c += x->ec;
-      }
-      if (!tiled || c != T.cols)
-        return fail(TSB_ERR_INVALID, grp + ": its elements are not all written exactly once (at row " + std::to_string(y) + ")");
-      if (!tensor) dtype = sorted[0]->dtype;
-      for (const TargetBox* x : sorted)
-        if (x->dtype != dtype) return fail(TSB_ERR_INVALID, grp + ": sources of different dtypes");
-      if (tensor) {
-        if (y == 0) g = out->n_groups++;
-        for (const TargetBox* x : sorted) tiles(*x, y, y1, g, T.scale_inv + 4 * b);
-      } else {
-        channel_rows(sorted, y, y1);
-      }
-      y = y1;
-    }
-    return TSB_OK;
+    return sweep_cover(
+        T.rows, T.cols, boxes, nb,
+        [&](uint64_t y, uint64_t y1, const std::vector<const TargetBox*>& sorted) -> int {
+          if (!tensor) dtype = sorted[0]->dtype;
+          for (const TargetBox* x : sorted)
+            if (x->dtype != dtype) return fail(TSB_ERR_INVALID, group(y) + ": sources of different dtypes");
+          if (tensor) {
+            if (y == 0) g = out->n_groups++;
+            for (const TargetBox* x : sorted) tiles(*x, y, y1, g, T.scale_inv + 4 * b);
+          } else {
+            channel_rows(sorted, y, y1);
+          }
+          return TSB_OK;
+        },
+        [&](uint64_t y, uint64_t) {
+          return fail(TSB_ERR_INVALID, group(y) + ": its elements are not all written exactly once (at row " + std::to_string(y) + ")");
+        });
   }
 };
 
-}  // namespace
+constexpr GridRules kTargetRules{"target", "NULL dst or scale_inv", "dst", "scale_inv",
+                                 (1u << TSB_SCALE_PER_CHANNEL) | (1u << TSB_SCALE_PER_TENSOR), 1ull << 31};
 
 int scaled_fp8_compile(int device, const tsb_rect_t* rects, uint64_t n, const tsb_sq_target_t* targets,
                        uint64_t n_targets, SqTables* out) {
@@ -172,17 +150,8 @@ int scaled_fp8_compile(int device, const tsb_rect_t* rects, uint64_t n, const ts
   std::vector<uint64_t> base(n_targets + 1, 0);  // matrix index of every target's first matrix
   for (uint64_t t = 0; t < n_targets; ++t) {
     const tsb_sq_target_t& T = targets[t];
-    const std::string where = "target " + std::to_string(t) + ": ";
-    if (!T.dst || !T.scale_inv) return fail(TSB_ERR_INVALID, where + "NULL dst or scale_inv");
-    if (!T.batch || !T.rows || !T.cols) return fail(TSB_ERR_INVALID, where + "empty target");
-    if (T.scale_inv % 4) return fail(TSB_ERR_INVALID, where + "scale_inv is not 4-byte aligned");
-    if (T.granularity != TSB_SCALE_PER_CHANNEL && T.granularity != TSB_SCALE_PER_TENSOR)
-      return fail(TSB_ERR_INVALID, where + "granularity must be TSB_SCALE_PER_CHANNEL or TSB_SCALE_PER_TENSOR, not " +
-                                       std::to_string(T.granularity));
-    if (T.pad) return fail(TSB_ERR_INVALID, where + "pad must be 0");
-    if (T.cols >= (1ull << 31) || T.rows >= (1ull << 31) || T.batch >= (1ull << 31) ||
-        T.batch * T.rows >= (1ull << 40) / T.cols)
-      return fail(TSB_ERR_INVALID, where + "target too large");
+    int st = check_grid(kTargetRules, t, {T.dst, T.scale_inv, T.batch, T.rows, T.cols, 0, 0, 1, T.granularity, T.pad, !T.dst || !T.scale_inv});
+    if (st) return st;
     geom[t] = {T.dst, T.batch, T.rows, T.cols};
     base[t + 1] = base[t] + T.batch;
     out->payload_bytes += T.batch * T.rows * T.cols + 4 * T.batch * (T.granularity == TSB_SCALE_PER_CHANNEL ? T.rows : 1);
@@ -214,10 +183,6 @@ int scaled_fp8_compile(int device, const tsb_rect_t* rects, uint64_t n, const ts
   return TSB_OK;
 }
 
-namespace {
-
-constexpr int kUnroll = 4;  // 16-byte loads in flight per thread
-
 // max abs_bits of `a` (one word per lane, 0 for lanes without data) into s_amax[row] when the whole warp
 // holds one row (warp-uniform `one_row`), else per lane
 __device__ __forceinline__ void fold_rows(bool one_row, uint32_t row, uint32_t m, uint32_t* s_amax) {
@@ -242,7 +207,7 @@ __device__ __forceinline__ void stage_band(const SqBand& band, const SqPiece* __
       // each warp takes 32 * kUnroll consecutive 16-byte units per step (coalesced 512-byte loads)
       const uint32_t upr = p.cols * es / 16;
       const uint32_t total = p.rows * upr;
-      for (uint32_t base = warp * 32 * kUnroll; base < total; base += kSqThreads * kUnroll) {
+      for (uint32_t base = warp * 32 * kUnroll; base < total; base += kQuantThreads * kUnroll) {
         uint4 v[kUnroll];
 #pragma unroll
         for (int k = 0; k < kUnroll; ++k) {
@@ -270,7 +235,7 @@ __device__ __forceinline__ void stage_band(const SqBand& band, const SqPiece* __
       }
     } else {
       const uint32_t total = p.rows * p.cols;
-      for (uint32_t base = warp * 32; base < total; base += kSqThreads) {
+      for (uint32_t base = warp * 32; base < total; base += kQuantThreads) {
         const uint32_t idx = base + lane;
         const uint32_t rf = base / p.cols, rl = (min(base + 32, total) - 1) / p.cols;
         uint32_t m = 0;
@@ -301,11 +266,11 @@ __device__ __forceinline__ void run_band(const SqBand& band, const SqPiece* piec
                                          float* s_scale) {
   constexpr uint32_t es = Src<DT>::kBytes;
   const uint32_t spitch = (band.cols * es + 15u) & ~15u;
-  for (uint32_t r = threadIdx.x; r < band.rows; r += kSqThreads) s_amax[r] = 0;
+  for (uint32_t r = threadIdx.x; r < band.rows; r += kQuantThreads) s_amax[r] = 0;
   __syncthreads();
   stage_band<DT>(band, pieces, smem, spitch, s_amax);
   __syncthreads();
-  for (uint32_t r = threadIdx.x; r < band.rows; r += kSqThreads) {
+  for (uint32_t r = threadIdx.x; r < band.rows; r += kQuantThreads) {
     float scale, scale_inv;
     scales_of_amax(s_amax[r], &scale, &scale_inv);
     s_scale[r] = scale;
@@ -314,7 +279,7 @@ __device__ __forceinline__ void run_band(const SqBand& band, const SqPiece* piec
   __syncthreads();
   const uint32_t cpr = (band.cols + 15u) / 16u;
   const uint32_t total = band.rows * cpr;
-  for (uint32_t idx = threadIdx.x; idx < total; idx += kSqThreads) {
+  for (uint32_t idx = threadIdx.x; idx < total; idx += kQuantThreads) {
     const uint32_t r = idx / cpr, c = (idx - r * cpr) * 16u;
     const uint32_t nvalid = min(16u, band.cols - c);
     uint32_t f[16], o[4];
@@ -324,7 +289,7 @@ __device__ __forceinline__ void run_band(const SqBand& band, const SqPiece* piec
   }
 }
 
-__global__ void __launch_bounds__(kSqThreads, 5) scaled_fp8_rows_kernel(const SqBand* __restrict__ bands,
+__global__ void __launch_bounds__(kQuantThreads, 5) scaled_fp8_rows_kernel(const SqBand* __restrict__ bands,
                                                                        const SqPiece* __restrict__ pieces) {
   extern __shared__ __align__(16) unsigned char stage[];
   __shared__ uint32_t s_amax[kSqBandRows];
@@ -346,11 +311,11 @@ __device__ __forceinline__ uint32_t tile_amax(const SqTile& t) {
   if (t.vec) {
     const uint32_t upr = t.cols * es / 16;
     const uint32_t total = t.rows * upr;
-    for (uint32_t i = threadIdx.x; i < total; i += kSqThreads * kUnroll) {
+    for (uint32_t i = threadIdx.x; i < total; i += kQuantThreads * kUnroll) {
       uint4 v[kUnroll];
 #pragma unroll
       for (int k = 0; k < kUnroll; ++k) {
-        const uint32_t idx = i + k * kSqThreads;
+        const uint32_t idx = i + k * kQuantThreads;
         if (idx < total) {
           const uint32_t r = idx / upr, c = idx - r * upr;
           v[k] = ldg16(src + static_cast<int64_t>(r) * t.src_stride + c * 16);
@@ -358,11 +323,11 @@ __device__ __forceinline__ uint32_t tile_amax(const SqTile& t) {
       }
 #pragma unroll
       for (int k = 0; k < kUnroll; ++k)
-        if (i + k * kSqThreads < total) m = fold16<DT>(m, v[k]);
+        if (i + k * kQuantThreads < total) m = fold16<DT>(m, v[k]);
     }
   } else {
     const uint32_t total = t.rows * t.cols;
-    for (uint32_t idx = threadIdx.x; idx < total; idx += kSqThreads) {
+    for (uint32_t idx = threadIdx.x; idx < total; idx += kQuantThreads) {
       const uint32_t r = idx / t.cols, c = idx - r * t.cols;
       m = max(m, abs_bits(elem<DT>(reinterpret_cast<const unsigned char*>(src + static_cast<int64_t>(r) * t.src_stride), c)));
     }
@@ -370,8 +335,8 @@ __device__ __forceinline__ uint32_t tile_amax(const SqTile& t) {
   return m;
 }
 
-__global__ void __launch_bounds__(kSqThreads) scaled_fp8_amax_kernel(const SqTile* __restrict__ tiles, uint32_t* amax) {
-  __shared__ uint32_t s_red[kSqThreads / 32];
+__global__ void __launch_bounds__(kQuantThreads) scaled_fp8_amax_kernel(const SqTile* __restrict__ tiles, uint32_t* amax) {
+  __shared__ uint32_t s_red[kQuantThreads / 32];
   const SqTile t = tiles[blockIdx.x];
   uint32_t m;
   switch (t.src_dtype) {
@@ -379,15 +344,9 @@ __global__ void __launch_bounds__(kSqThreads) scaled_fp8_amax_kernel(const SqTil
     case TSB_F16: m = tile_amax<TSB_F16>(t); break;
     default: m = tile_amax<TSB_F32>(t); break;
   }
-  m = __reduce_max_sync(0xffffffffu, m);
-  if ((threadIdx.x & 31u) == 0) s_red[threadIdx.x >> 5] = m;
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    uint32_t a = s_red[0];
-#pragma unroll
-    for (uint32_t w = 1; w < kSqThreads / 32; ++w) a = max(a, s_red[w]);
+  cta_max(m, s_red, [&](uint32_t a) {
     if (a) atomicMax(amax + t.group, a);
-  }
+  });
 }
 
 template <uint32_t DT>
@@ -395,7 +354,7 @@ __device__ __forceinline__ void quantise_tile(const SqTile& t, float scale) {
   constexpr uint32_t es = Src<DT>::kBytes;
   const uint32_t cpr = (t.cols + 15u) / 16u;
   const uint32_t total = t.rows * cpr;
-  for (uint32_t idx = threadIdx.x; idx < total; idx += kSqThreads) {
+  for (uint32_t idx = threadIdx.x; idx < total; idx += kQuantThreads) {
     const uint32_t r = idx / cpr, c = (idx - r * cpr) * 16u;
     const uint32_t nvalid = min(16u, t.cols - c);
     const char* s = reinterpret_cast<const char*>(t.src) + static_cast<int64_t>(r) * t.src_stride + c * es;
@@ -414,7 +373,7 @@ __device__ __forceinline__ void quantise_tile(const SqTile& t, float scale) {
   }
 }
 
-__global__ void __launch_bounds__(kSqThreads) scaled_fp8_quant_kernel(const SqTile* __restrict__ tiles,
+__global__ void __launch_bounds__(kQuantThreads) scaled_fp8_quant_kernel(const SqTile* __restrict__ tiles,
                                                                     const uint32_t* __restrict__ amax) {
   const SqTile t = tiles[blockIdx.x];
   float scale, scale_inv;
@@ -430,51 +389,58 @@ __global__ void __launch_bounds__(kSqThreads) scaled_fp8_quant_kernel(const SqTi
 }  // namespace
 
 int launch_scaled_fp8(const SqLaunch& l, cudaStream_t stream) {
-  cudaError_t e = cudaSuccess;
   if (l.n_bands) {
-    scaled_fp8_rows_kernel<<<l.n_bands, kSqThreads, l.stage_bytes, stream>>>(l.bands, l.pieces);
-    if ((e = cudaGetLastError()) != cudaSuccess) return cuda_fail(e, "scaled_fp8_rows_kernel launch");
-    count_launch();
+    scaled_fp8_rows_kernel<<<l.n_bands, kQuantThreads, l.stage_bytes, stream>>>(l.bands, l.pieces);
+    if (int st = launched("scaled_fp8_rows_kernel launch")) return st;
   }
-  if (l.n_tiles) {
-    if ((e = cudaMemsetAsync(l.amax, 0, 4ull * l.n_groups, stream)) != cudaSuccess) return cuda_fail(e, "scaled_fp8 amax clear");
-    scaled_fp8_amax_kernel<<<l.n_tiles, kSqThreads, 0, stream>>>(l.tiles, l.amax);
-    if ((e = cudaGetLastError()) != cudaSuccess) return cuda_fail(e, "scaled_fp8_amax_kernel launch");
-    count_launch();
-    scaled_fp8_quant_kernel<<<l.n_tiles, kSqThreads, 0, stream>>>(l.tiles, l.amax);
-    if ((e = cudaGetLastError()) != cudaSuccess) return cuda_fail(e, "scaled_fp8_quant_kernel launch");
-    count_launch();
-  }
+  if (!l.n_tiles) return TSB_OK;
+  return launch_two_pass(scaled_fp8_amax_kernel, scaled_fp8_quant_kernel, "scaled_fp8", l.tiles, l.n_tiles, l.amax, l.n_groups,
+                         stream);
+}
+
+namespace {
+
+// d = {SqBand table | SqPiece table | SqTile table | amax words}, one CTA per band and per tile (and pass)
+int scaled_fp8_plan(int device, const tsb_rect_t* rects, uint64_t n, const tsb_sq_target_t* targets, uint64_t n_targets,
+                    QuantPlan* q) {
+  SqTables tb;
+  int st = scaled_fp8_compile(device, rects, n, targets, n_targets, &tb);
+  if (st) return st;
+  q->add(tb.bands);
+  const size_t pieces = q->add(tb.pieces), tiles = q->add(tb.tiles), amax = q->seal(tb.n_groups);
+  q->describe(n, static_cast<uint32_t>(tb.bands.size() + tb.tiles.size()), kSqStageBytes, tb);
+  const SqLaunch l{nullptr, nullptr, nullptr, nullptr, static_cast<uint32_t>(tb.bands.size()), static_cast<uint32_t>(tb.tiles.size()),
+                   tb.n_groups, tb.stage_bytes};
+  q->launch = [l, pieces, tiles, amax](char* d, cudaStream_t s) {
+    SqLaunch x = l;
+    x.bands = reinterpret_cast<const SqBand*>(d);
+    x.pieces = reinterpret_cast<const SqPiece*>(d + pieces);
+    x.tiles = reinterpret_cast<const SqTile*>(d + tiles);
+    x.amax = reinterpret_cast<uint32_t*>(d + amax);
+    return launch_scaled_fp8(x, s);
+  };
   return TSB_OK;
 }
+
+}  // namespace
 
 }  // namespace tsb
 
 using namespace tsb;
 
+extern "C" int tsb_scaled_fp8_plan_create(int device, const tsb_rect_t* rects, uint64_t n, const tsb_sq_target_t* targets,
+                                          uint64_t n_targets, uint32_t flags, tsb_plan_t* out) {
+  return quant_plan_create("tsb_scaled_fp8_plan_create", device, flags, out,
+                           [&](QuantPlan* q) { return scaled_fp8_plan(device, rects, n, targets, n_targets, q); });
+}
+
 extern "C" int tsb_scaled_fp8_compile_host(int device, const tsb_rect_t* rects, uint64_t n, const tsb_sq_target_t* targets,
                                            uint64_t n_targets, uint32_t flags, void* out_bands, uint64_t band_cap,
                                            uint64_t* out_n_bands, void* out_pieces, uint64_t piece_cap, uint64_t* out_n_pieces,
                                            void* out_tiles, uint64_t tile_cap, uint64_t* out_n_tiles, uint64_t* out_n_groups) {
-  if (flags != 0) return fail(TSB_ERR_INVALID, "tsb_scaled_fp8_compile_host: flags must be 0");
-  SqTables tb;
-  int st = scaled_fp8_compile(device, rects, n, targets, n_targets, &tb);
-  if (st) return st;
-  if (out_n_bands) *out_n_bands = tb.bands.size();
-  if (out_n_pieces) *out_n_pieces = tb.pieces.size();
-  if (out_n_tiles) *out_n_tiles = tb.tiles.size();
-  if (out_n_groups) *out_n_groups = tb.n_groups;
-  if (out_bands) {
-    if (tb.bands.size() > band_cap) return fail(TSB_ERR_NOMEM, "out_bands too small");
-    if (!tb.bands.empty()) memcpy(out_bands, tb.bands.data(), tb.bands.size() * sizeof(SqBand));
-  }
-  if (out_pieces) {
-    if (tb.pieces.size() > piece_cap) return fail(TSB_ERR_NOMEM, "out_pieces too small");
-    if (!tb.pieces.empty()) memcpy(out_pieces, tb.pieces.data(), tb.pieces.size() * sizeof(SqPiece));
-  }
-  if (out_tiles) {
-    if (tb.tiles.size() > tile_cap) return fail(TSB_ERR_NOMEM, "out_tiles too small");
-    if (!tb.tiles.empty()) memcpy(out_tiles, tb.tiles.data(), tb.tiles.size() * sizeof(SqTile));
-  }
-  return TSB_OK;
+  return quant_compile_host("tsb_scaled_fp8_compile_host", flags,
+                            [&](QuantPlan* q) { return scaled_fp8_plan(device, rects, n, targets, n_targets, q); },
+                            {{out_bands, band_cap, out_n_bands, "out_bands"}, {out_pieces, piece_cap, out_n_pieces, "out_pieces"},
+                             {out_tiles, tile_cap, out_n_tiles, "out_tiles"}},
+                            out_n_groups);
 }

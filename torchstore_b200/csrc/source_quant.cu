@@ -23,6 +23,7 @@
 //                            are cleared on the launch stream before pass 1, so a replayed plan starts from zero.
 
 #include <algorithm>
+#include <array>
 #include <cstring>
 
 #include "fp8_quant.cuh"
@@ -31,8 +32,6 @@
 namespace tsb {
 
 namespace {
-
-uint32_t round16(uint64_t x) { return static_cast<uint32_t>((x + 15u) & ~uint64_t(15)); }
 
 struct Compiler {
   SrcQTables* out;
@@ -50,7 +49,7 @@ struct Compiler {
     u.cols = static_cast<uint32_t>(cols);
     u.per_row = per_row ? 1u : 0u;
     u.src_dtype = static_cast<uint16_t>(T.src_dtype);
-    u.vec = (u.src % 16 == 0 && (rows == 1 || u.src_pitch % 16 == 0) && (cols * es) % 16 == 0) ? 1 : 0;
+    u.vec = vec_ok(u.src, u.src_pitch, rows, cols, es) ? 1 : 0;
     out->unit_bytes = std::max<uint32_t>(out->unit_bytes, static_cast<uint32_t>(rows * cols * es));
     out->units.push_back(u);
     out->src_bytes += rows * cols * es;
@@ -71,7 +70,7 @@ struct Compiler {
       t.cols = static_cast<uint32_t>(cols);
       t.group = g;
       t.src_dtype = T.src_dtype;
-      t.vec = (t.src % 16 == 0 && (cols * es) % 16 == 0) ? 1u : 0u;
+      t.vec = vec_ok(t.src, 0, 1, cols, es) ? 1u : 0u;
       out->tiles.push_back(t);
       out->src_bytes += cols * es;
     }
@@ -96,12 +95,12 @@ struct Compiler {
       const uint64_t all = T.batch * T.rows;  // per channel, the matrices of a stack are consecutive rows
       const uint32_t spitch = round16(T.cols * es);
       const uint64_t cpr = (T.cols + 15) / 16;  // 16-element chunks per row
-      if (spitch > kSqStageBytes || cpr > kSrcQChunks * kSrcQThreads) {
+      if (spitch > kSqStageBytes || cpr > kSrcQChunks * kQuantThreads) {
         for (uint64_t r = 0; r < all; ++r) group(T, es, r * T.cols, T.cols, T.scale_inv + 4 * r);
         return;
       }
       const uint64_t per_band =
-          std::min<uint64_t>(std::min<uint64_t>(kSqBandRows, kSqStageBytes / spitch), kSrcQChunks * kSrcQThreads / cpr);
+          std::min<uint64_t>(std::min<uint64_t>(kSqBandRows, kSqStageBytes / spitch), kSrcQChunks * kQuantThreads / cpr);
       for (uint64_t r = 0; r < all; r += per_band)
         unit(T, es, r * T.cols, T.scale_inv + 4 * r, std::min(per_band, all - r), T.cols, true);
     } else {
@@ -110,26 +109,21 @@ struct Compiler {
   }
 };
 
-}  // namespace
+constexpr GridRules kTargetRules{"target", "NULL src, dst or scale_inv", "src", "scale_inv",
+                                 (1u << TSB_SCALE_PER_BLOCK) | (1u << TSB_SCALE_PER_CHANNEL) | (1u << TSB_SCALE_PER_TENSOR), 1ull << 30};
 
 int source_quant_compile(const tsb_source_quant_target_t* targets, uint64_t n, SrcQTables* out) {
   if (n && !targets) return fail(TSB_ERR_INVALID, "source_quant: NULL targets");
   Compiler cc{out};
   for (uint64_t t = 0; t < n; ++t) {
     const tsb_source_quant_target_t& T = targets[t];
-    const std::string where = "target " + std::to_string(t) + ": ";
     const uint32_t es = quant_src_bytes(T.src_dtype);
-    if (!es) return fail(TSB_ERR_INVALID, where + "src_dtype must be TSB_F32, TSB_BF16 or TSB_F16, not " + std::to_string(T.src_dtype));
-    if (!T.src || !T.dst || !T.scale_inv) return fail(TSB_ERR_INVALID, where + "NULL src, dst or scale_inv");
-    if (!T.batch || !T.rows || !T.cols) return fail(TSB_ERR_INVALID, where + "empty target");
-    if (T.src % es) return fail(TSB_ERR_INVALID, where + "src is not aligned to its element size");
-    if (T.scale_inv % 4) return fail(TSB_ERR_INVALID, where + "scale_inv is not 4-byte aligned");
-    if (T.granularity != TSB_SCALE_PER_BLOCK && T.granularity != TSB_SCALE_PER_CHANNEL && T.granularity != TSB_SCALE_PER_TENSOR)
-      return fail(TSB_ERR_INVALID, where + "granularity must be TSB_SCALE_PER_BLOCK, TSB_SCALE_PER_CHANNEL or "
-                                           "TSB_SCALE_PER_TENSOR, not " + std::to_string(T.granularity));
-    if (T.cols >= (1ull << 30) || T.rows >= (1ull << 31) || T.batch >= (1ull << 31) ||
-        T.batch * T.rows >= (1ull << 40) / T.cols || T.row0 >= (1ull << 40) || T.col0 >= (1ull << 40))
-      return fail(TSB_ERR_INVALID, where + "target too large");
+    if (!es)
+      return fail(TSB_ERR_INVALID, "target " + std::to_string(t) + ": src_dtype must be TSB_F32, TSB_BF16 or TSB_F16, not " +
+                                       std::to_string(T.src_dtype));
+    int st = check_grid(kTargetRules, t, {T.src, T.scale_inv, T.batch, T.rows, T.cols, T.row0, T.col0, es, T.granularity, 0,
+                                          !T.src || !T.dst || !T.scale_inv});
+    if (st) return st;
     uint64_t groups = T.batch;
     if (T.granularity == TSB_SCALE_PER_CHANNEL) groups *= T.rows;
     if (T.granularity == TSB_SCALE_PER_BLOCK)
@@ -146,8 +140,6 @@ int source_quant_compile(const tsb_source_quant_target_t* targets, uint64_t n, S
   for (const SrcQUnit& u : out->units) ++out->n_units[rank(u)];
   return TSB_OK;
 }
-
-namespace {
 
 // Load the first `nvalid` elements of a 16-element chunk at `s` into `d` (its source words; the rest 0).
 template <uint32_t DT>
@@ -192,7 +184,7 @@ __device__ __forceinline__ void widen_chunk(const uint32_t d[4 * Src<DT>::kBytes
 }
 
 template <uint32_t DT>
-__global__ void __launch_bounds__(kSrcQThreads) source_quant_kernel(const SrcQUnit* __restrict__ units) {
+__global__ void __launch_bounds__(kQuantThreads) source_quant_kernel(const SrcQUnit* __restrict__ units) {
   constexpr uint32_t es = Src<DT>::kBytes;
   __shared__ uint32_t s_amax[kSqBandRows];
   __shared__ float s_scale[kSqBandRows];
@@ -201,12 +193,12 @@ __global__ void __launch_bounds__(kSrcQThreads) source_quant_kernel(const SrcQUn
   const uint32_t cpr = (u.cols + 15u) / 16u, total = u.rows * cpr;
   const uint32_t ng = u.per_row ? u.rows : 1u;
   const uint32_t warp = threadIdx.x >> 5, lane = threadIdx.x & 31u;
-  for (uint32_t g = threadIdx.x; g < ng; g += kSrcQThreads) s_amax[g] = 0;
-  // every load of this thread's chunks first: chunk j is idx = threadIdx.x + j * kSrcQThreads
+  for (uint32_t g = threadIdx.x; g < ng; g += kQuantThreads) s_amax[g] = 0;
+  // every load of this thread's chunks first: chunk j is idx = threadIdx.x + j * kQuantThreads
   uint32_t d[kSrcQChunks][4 * es];
 #pragma unroll
   for (uint32_t j = 0; j < kSrcQChunks; ++j) {
-    const uint32_t idx = threadIdx.x + j * kSrcQThreads;
+    const uint32_t idx = threadIdx.x + j * kQuantThreads;
     const uint32_t r = idx / cpr, c = (idx - r * cpr) * 16u;
     if (idx < total) {
       load_chunk<DT>(src + static_cast<uint64_t>(r) * u.src_pitch + c * es, min(16u, u.cols - c), u.vec, d[j]);
@@ -219,7 +211,7 @@ __global__ void __launch_bounds__(kSrcQThreads) source_quant_kernel(const SrcQUn
   uint32_t mine = 0;
 #pragma unroll
   for (uint32_t j = 0; j < kSrcQChunks; ++j) {
-    const uint32_t base = warp * 32 + j * kSrcQThreads;  // warp-uniform
+    const uint32_t base = warp * 32 + j * kQuantThreads;  // warp-uniform
     if (base >= total) break;
     const uint32_t idx = base + lane;
     uint32_t f[16], m = 0;
@@ -243,7 +235,7 @@ __global__ void __launch_bounds__(kSrcQThreads) source_quant_kernel(const SrcQUn
     if (lane == 0) atomicMax(s_amax, mine);
   }
   __syncthreads();
-  for (uint32_t g = threadIdx.x; g < ng; g += kSrcQThreads) {
+  for (uint32_t g = threadIdx.x; g < ng; g += kQuantThreads) {
     float scale, scale_inv;
     scales_of_amax(s_amax[g], &scale, &scale_inv);
     s_scale[g] = scale;
@@ -252,7 +244,7 @@ __global__ void __launch_bounds__(kSrcQThreads) source_quant_kernel(const SrcQUn
   __syncthreads();
 #pragma unroll
   for (uint32_t j = 0; j < kSrcQChunks; ++j) {
-    const uint32_t idx = threadIdx.x + j * kSrcQThreads;
+    const uint32_t idx = threadIdx.x + j * kQuantThreads;
     if (idx < total) {
       const uint32_t r = idx / cpr, c = (idx - r * cpr) * 16u;
       uint32_t f[16], o[4];
@@ -263,47 +255,53 @@ __global__ void __launch_bounds__(kSrcQThreads) source_quant_kernel(const SrcQUn
   }
 }
 
-}  // namespace
-
-int launch_source_quant(const SrcQLaunch& l, cudaStream_t stream) {
-  const SrcQUnit* units = l.units;
-  for (int k = 0; k < 3; ++k) {
-    const uint32_t n = l.n_units[k];
-    if (!n) continue;
-    if (k == 0) source_quant_kernel<TSB_BF16><<<n, kSrcQThreads, 0, stream>>>(units);
-    if (k == 1) source_quant_kernel<TSB_F16><<<n, kSrcQThreads, 0, stream>>>(units);
-    if (k == 2) source_quant_kernel<TSB_F32><<<n, kSrcQThreads, 0, stream>>>(units);
-    cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) return cuda_fail(e, "source_quant_kernel launch");
-    count_launch();
-    units += n;
-  }
-  if (l.two_pass.n_tiles) return launch_scaled_fp8(l.two_pass, stream);
+// d = {SrcQUnit table | SqTile table | amax words}: one launch per source dtype over its units, one CTA each, then
+// scaled_fp8.cu's two passes over the tiles
+int source_quant_plan(const tsb_source_quant_target_t* targets, uint64_t n, QuantPlan* q) {
+  SrcQTables tb;
+  int st = source_quant_compile(targets, n, &tb);
+  if (st) return st;
+  q->add(tb.units);
+  const size_t tiles = q->add(tb.tiles), amax = q->seal(tb.n_groups);
+  q->describe(n, static_cast<uint32_t>(tb.units.size() + tb.tiles.size()), tb.unit_bytes, tb);
+  const SqLaunch two_pass{nullptr, nullptr, nullptr, nullptr, 0, static_cast<uint32_t>(tb.tiles.size()), tb.n_groups, 0};
+  q->launch = [two_pass, tiles, amax, n_units = std::array<uint32_t, 3>{tb.n_units[0], tb.n_units[1], tb.n_units[2]}](char* d, cudaStream_t s) -> int {
+    const SrcQUnit* units = reinterpret_cast<const SrcQUnit*>(d);
+    for (int k = 0; k < 3; ++k) {
+      const uint32_t n = n_units[k];
+      if (!n) continue;
+      if (k == 0) source_quant_kernel<TSB_BF16><<<n, kQuantThreads, 0, s>>>(units);
+      if (k == 1) source_quant_kernel<TSB_F16><<<n, kQuantThreads, 0, s>>>(units);
+      if (k == 2) source_quant_kernel<TSB_F32><<<n, kQuantThreads, 0, s>>>(units);
+      if (int st = launched("source_quant_kernel launch")) return st;
+      units += n;
+    }
+    if (!two_pass.n_tiles) return TSB_OK;
+    SqLaunch l = two_pass;
+    l.tiles = reinterpret_cast<const SqTile*>(d + tiles);
+    l.amax = reinterpret_cast<uint32_t*>(d + amax);
+    return launch_scaled_fp8(l, s);
+  };
   return TSB_OK;
 }
+
+}  // namespace
 
 }  // namespace tsb
 
 using namespace tsb;
 
+extern "C" int tsb_source_quant_plan_create(int device, const tsb_source_quant_target_t* targets, uint64_t n, uint32_t flags,
+                                            tsb_plan_t* out) {
+  return quant_plan_create("tsb_source_quant_plan_create", device, flags, out,
+                           [&](QuantPlan* q) { return source_quant_plan(targets, n, q); });
+}
+
 extern "C" int tsb_source_quant_compile_host(int device, const tsb_source_quant_target_t* targets, uint64_t n, uint32_t flags,
                                              void* out_units, uint64_t unit_cap, uint64_t* out_n_units, void* out_tiles,
                                              uint64_t tile_cap, uint64_t* out_n_tiles, uint64_t* out_n_groups) {
   (void)device;
-  if (flags != 0) return fail(TSB_ERR_INVALID, "tsb_source_quant_compile_host: flags must be 0");
-  SrcQTables tb;
-  int st = source_quant_compile(targets, n, &tb);
-  if (st) return st;
-  if (out_n_units) *out_n_units = tb.units.size();
-  if (out_n_tiles) *out_n_tiles = tb.tiles.size();
-  if (out_n_groups) *out_n_groups = tb.n_groups;
-  if (out_units) {
-    if (tb.units.size() > unit_cap) return fail(TSB_ERR_NOMEM, "out_units too small");
-    if (!tb.units.empty()) memcpy(out_units, tb.units.data(), tb.units.size() * sizeof(SrcQUnit));
-  }
-  if (out_tiles) {
-    if (tb.tiles.size() > tile_cap) return fail(TSB_ERR_NOMEM, "out_tiles too small");
-    if (!tb.tiles.empty()) memcpy(out_tiles, tb.tiles.data(), tb.tiles.size() * sizeof(SqTile));
-  }
-  return TSB_OK;
+  return quant_compile_host("tsb_source_quant_compile_host", flags, [&](QuantPlan* q) { return source_quant_plan(targets, n, q); },
+                            {{out_units, unit_cap, out_n_units, "out_units"}, {out_tiles, tile_cap, out_n_tiles, "out_tiles"}},
+                            out_n_groups);
 }

@@ -4,6 +4,10 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include <algorithm>
+#include <cstring>
+#include <functional>
+#include <initializer_list>
 #include <string>
 #include <vector>
 
@@ -159,6 +163,143 @@ int launch_copy_rects(const LaunchParams& p, uint32_t grid, cudaStream_t stream)
 void count_launch();
 int max_ctas_per_sm(uint32_t kind, bool with_link, uint32_t link_smem_bytes, int* out);
 
+// ---- scaled fp8 plans: what every kind shares ---------------------------------------------------------
+constexpr uint32_t kQuantThreads = 256;  // CTA size of every scaled fp8 kernel
+
+inline uint32_t round16(uint64_t x) { return static_cast<uint32_t>((x + 15u) & ~uint64_t(15)); }
+
+// rows from p, `stride` bytes apart, all start 16-byte aligned
+inline bool aligned16(uint64_t p, int64_t stride, uint64_t rows) { return p % 16 == 0 && (rows == 1 || stride % 16 == 0); }
+
+// ... and rows of `cols` elements of `es` bytes are whole 16-byte units: 16-byte accesses cover them
+inline bool vec_ok(uint64_t p, int64_t stride, uint64_t rows, uint64_t cols, uint32_t es) {
+  return aligned16(p, stride, rows) && (cols * es) % 16 == 0;
+}
+
+// The byte counts of tsb_plan_info_t a scaled fp8 compiler accumulates.
+struct PlanBytes {
+  uint64_t src_bytes = 0, remote_src_bytes = 0, payload_bytes = 0;
+  // `bytes` read by a plan of `device` from a source on `src_device` (< 0: not a GPU)
+  void read(uint64_t bytes, int32_t src_device, int device) {
+    src_bytes += bytes;
+    if (src_device >= 0 && src_device != device) remote_src_bytes += bytes;
+  }
+};
+
+// A scaled fp8 grid as the compilers validate it: `batch` [rows, cols] matrices of `es`-byte elements at `base`
+// and global offset (row0, col0), with their float32 scales at `scale`.  `null`: one of its pointers is NULL.
+struct Grid {
+  uint64_t base, scale, batch, rows, cols, row0, col0;
+  uint32_t es, granularity, pad;
+  bool null;
+};
+// What differs between the compilers' checks of their grids.
+struct GridRules {
+  const char* noun;          // "target" / "source": messages start "<noun> N: "
+  const char* null_msg;      // the message for `null`
+  const char* base_name;     // names the base in the element-alignment message
+  const char* scale_name;    // names the scale in the 4-byte-alignment message
+  uint32_t granularities;    // the accepted TSB_SCALE_* as bits 1 << g; 0: the grid has no granularity
+  uint64_t max_cols;         // cols must stay below this
+};
+// TSB_ERR_INVALID naming grid `index` unless it passes `rules` (block_fp8.cu).
+int check_grid(const GridRules& rules, uint64_t index, const Grid& g);
+
+// Exact coverage of one [rows, cols] matrix by `boxes` (anything with r0, er, c0, ec; sorted by r0): between two
+// consecutive box row boundaries y and y1 the boxes spanning those rows, sorted by column, must cut [0, cols) into
+// contiguous, disjoint runs.  Checks in time proportional to the boxes, not the elements.  Calls band(y, y1, sorted)
+// for each band of rows that passes, and returns gap(y, c) at the first that does not, c being the first column not
+// covered exactly once (clamped to cols - 1); a non-zero status of either ends the sweep.
+template <class Box, class Band, class Gap>
+int sweep_cover(uint64_t rows, uint64_t cols, const Box* const* boxes, size_t nb, Band&& band, Gap&& gap) {
+  std::vector<const Box*> act, sorted;
+  size_t i = 0;
+  for (uint64_t y = 0; y < rows;) {
+    while (i < nb && boxes[i]->r0 == y) act.push_back(boxes[i++]);
+    act.erase(std::remove_if(act.begin(), act.end(), [y](const Box* x) { return x->r0 + x->er <= y; }), act.end());
+    uint64_t y1 = i < nb ? boxes[i]->r0 : rows;
+    for (const Box* x : act) y1 = std::min(y1, x->r0 + x->er);
+    sorted = act;
+    std::sort(sorted.begin(), sorted.end(), [](const Box* a, const Box* b) { return a->c0 < b->c0; });
+    uint64_t c = 0;
+    bool ok = true;
+    for (const Box* x : sorted) {
+      if (x->c0 != c) {
+        ok = false;
+        c = std::min(c, x->c0);
+        break;
+      }
+      c += x->ec;
+    }
+    if (!ok || c != cols) return gap(y, std::min(c, cols - 1));
+    if (int st = band(y, y1, sorted)) return st;
+    y = y1;
+  }
+  return TSB_OK;
+}
+
+// One sealed scaled fp8 plan, as its kind's .cu file describes it to plan.cu: only that file knows the tables'
+// layout and how to launch from them.
+struct QuantPlan {
+  struct Section {
+    size_t off;      // byte offset in `tables`
+    uint64_t count;  // records
+    size_t bytes;    // count * record size
+  };
+  std::vector<char> tables;       // every table back to back, then the zeroed amax words
+  std::vector<Section> sections;  // the tables, in the order of the kind's tsb_*_compile_host outputs
+  uint32_t n_groups = 0;          // amax words
+  tsb_plan_info_t info{};
+  std::function<int(char* d, cudaStream_t)> launch;  // runs the plan from its tables' device copy at d
+
+  // Append a table; returns its byte offset.
+  template <class T>
+  size_t add(const std::vector<T>& v) {
+    const size_t off = tables.size();
+    tables.resize(off + v.size() * sizeof(T));
+    if (!v.empty()) memcpy(tables.data() + off, v.data(), v.size() * sizeof(T));
+    sections.push_back({off, v.size(), v.size() * sizeof(T)});
+    return off;
+  }
+  // After the last table: `groups` zeroed amax words (at the returned offset), at least 16 bytes in all.
+  size_t seal(uint32_t groups) {
+    const size_t off = tables.size();
+    n_groups = groups;
+    tables.resize(std::max<size_t>(16, off + 4ull * groups), 0);
+    return off;
+  }
+  // tsb_plan_info_t: `inputs` rects (or targets), one kQuantThreads CTA per each of `ctas` records
+  void describe(uint64_t inputs, uint32_t ctas, uint32_t tile_bytes, const PlanBytes& b) {
+    info.num_rects = inputs;
+    info.num_tiles = ctas;
+    info.grid = ctas;
+    info.block = kQuantThreads;
+    info.tile_bytes = tile_bytes;
+    info.payload_bytes = b.payload_bytes;
+    info.src_bytes = b.src_bytes;
+    info.remote_src_bytes = b.remote_src_bytes;
+  }
+};
+using QuantCompile = std::function<int(QuantPlan*)>;
+// The bodies of tsb_*_plan_create and tsb_*_compile_host (plan.cu): `fn` names the entry in its argument errors.
+int quant_plan_create(const char* fn, int device, uint32_t flags, tsb_plan_t* out, const QuantCompile& compile);
+struct TableOut {
+  void* out;          // NULL: not wanted
+  uint64_t cap;       // records out can take
+  uint64_t* n;        // the table's record count (if not NULL)
+  const char* name;   // the argument, for TSB_ERR_NOMEM
+};
+int quant_compile_host(const char* fn, uint32_t flags, const QuantCompile& compile, std::initializer_list<TableOut> outs,
+                       uint64_t* out_n_groups);
+
+// After a kernel launch: its launch error, or count it.
+inline int launched(const char* what) {
+  const cudaError_t e = cudaGetLastError();
+  if (e != cudaSuccess) return cuda_fail(e, what);
+  count_launch();
+  return TSB_OK;
+}
+
 // ---- scaled fp8 destinations: the rect -> [batch, rows, cols] mapping (block_fp8.cu) ----------------
 // Where a quantised destination lives: `batch` contiguous [rows, cols] float8_e4m3fn matrices at dst.
 struct TargetGeom {
@@ -188,7 +329,6 @@ int rect_requant_boxes(const tsb_rect_t& in, uint64_t index, const TargetGeom* t
 
 // ---- block-scaled fp8 (block_fp8.cu) ---------------------------------------------------------------
 constexpr uint32_t kBqBlock = 128;  // block edge (elements)
-constexpr uint32_t kBqThreads = 256;
 
 // One 128x128 (or partial edge) block of a target: CTA-sized unit of work.
 struct alignas(16) BqBlock {
@@ -213,19 +353,13 @@ struct alignas(16) BqPiece {
 };
 static_assert(sizeof(BqPiece) == 32, "BqPiece is part of tsb_block_fp8_compile_host's output");
 
-struct BqTables {
+struct BqTables : PlanBytes {
   std::vector<BqBlock> blocks;
   std::vector<BqPiece> pieces;
   uint32_t max_src_bytes = 2;  // largest source element size: sizes the shared-memory stage
-  uint64_t src_bytes = 0, remote_src_bytes = 0, payload_bytes = 0;
 };
-int block_fp8_compile(int device, const tsb_rect_t* rects, uint64_t n, const tsb_bq_target_t* targets, uint64_t n_targets,
-                      BqTables* out);
-int launch_block_fp8(const BqBlock* blocks, const BqPiece* pieces, uint32_t n_blocks, uint32_t max_src_bytes,
-                     cudaStream_t stream);
 
 // ---- per-channel / per-tensor scaled fp8 (scaled_fp8.cu) -------------------------------------------
-constexpr uint32_t kSqThreads = 256;
 // Shared-memory stage of the row-staged kernel: a per-channel row whose source bytes (rounded up to 16)
 // fit takes the one-read path.  32 KiB admits a bf16 row of K = 14336 (28 KiB) and four of K = 4096,
 // stays under the 48 KiB default (no opt-in), and leaves room for 6 CTAs of 256 threads per SM.
@@ -271,16 +405,13 @@ struct alignas(8) SqTile {
 };
 static_assert(sizeof(SqTile) == 56, "SqTile is part of tsb_scaled_fp8_compile_host's output");
 
-struct SqTables {
+struct SqTables : PlanBytes {
   std::vector<SqBand> bands;
   std::vector<SqPiece> pieces;
   std::vector<SqTile> tiles;
   uint32_t n_groups = 0;        // amax words of the two-pass path
   uint32_t stage_bytes = 0;     // largest band stage (dynamic shared memory of the row-staged kernel)
-  uint64_t src_bytes = 0, remote_src_bytes = 0, payload_bytes = 0;
 };
-int scaled_fp8_compile(int device, const tsb_rect_t* rects, uint64_t n, const tsb_sq_target_t* targets,
-                       uint64_t n_targets, SqTables* out);
 struct SqLaunch {
   const SqBand* bands;
   const SqPiece* pieces;
@@ -291,7 +422,6 @@ struct SqLaunch {
 int launch_scaled_fp8(const SqLaunch& l, cudaStream_t stream);
 
 // ---- dequantising pulls: scaled fp8 sources -> f32 / bf16 / f16 (dequant_fp8.cu) --------------------
-constexpr uint32_t kDqThreads = 256;
 constexpr uint32_t kDqTileElems = 16384;  // most elements of one tile (one CTA; 4 16-element chunks per thread)
 constexpr uint32_t kDqTileRows = 256;     // most rows of one tile (one staged scale per row)
 
@@ -310,18 +440,13 @@ struct alignas(8) DqTile {
 };
 static_assert(sizeof(DqTile) == 56, "DqTile is part of tsb_dequant_fp8_compile_host's output");
 
-struct DqTables {
+struct DqTables : PlanBytes {
   std::vector<DqTile> tiles;
-  uint64_t src_bytes = 0, remote_src_bytes = 0, payload_bytes = 0;
 };
 // Validate scaled fp8 source shards (TSB_ERR_INVALID naming the source) -> their fp8 grids.
 int dq_source_geoms(const tsb_dq_source_t* sources, uint64_t n_sources, std::vector<TargetGeom>* out);
-int dequant_fp8_compile(int device, const tsb_rect_t* rects, uint64_t n, const tsb_dq_source_t* sources,
-                        uint64_t n_sources, DqTables* out);
-int launch_dequant_fp8(const DqTile* tiles, uint32_t n_tiles, cudaStream_t stream);
 
 // ---- requantising pulls: scaled fp8 sources -> block / channel / tensor scaled fp8 (requant_fp8.cu) -----
-constexpr uint32_t kRqThreads = 256;
 
 // Staged path, one CTA each: a 128x128 block of a block-scaled target (one group), or a band of whole rows
 // of a per-channel target whose row fits kSqStageBytes (one group per row).
@@ -366,31 +491,19 @@ struct alignas(8) RqTile {
 };
 static_assert(sizeof(RqTile) == 64, "RqTile is part of tsb_requant_fp8_compile_host's output");
 
-struct RqTables {
+struct RqTables : PlanBytes {
   std::vector<RqUnit> units;
   std::vector<RqPiece> pieces;
   std::vector<RqTile> tiles;
   uint32_t n_groups = 0;     // amax words of the two-pass path
   uint32_t stage_bytes = 0;  // largest unit stage (dynamic shared memory of the staged kernel)
-  uint64_t src_bytes = 0, remote_src_bytes = 0, payload_bytes = 0;
 };
-int requant_fp8_compile(int device, const tsb_rect_t* rects, uint64_t n, const tsb_dq_source_t* sources, uint64_t n_sources,
-                        const tsb_sq_target_t* targets, uint64_t n_targets, RqTables* out);
-struct RqLaunch {
-  const RqUnit* units;
-  const RqPiece* pieces;
-  const RqTile* tiles;
-  uint32_t* amax;  // n_groups words, cleared by the launch
-  uint32_t n_units, n_tiles, n_groups, stage_bytes;
-};
-int launch_requant_fp8(const RqLaunch& l, cudaStream_t stream);
 
 // ---- source-side quantisation: live bf16/f16/f32 shards -> scaled fp8 staging (source_quant.cu) ---------
-constexpr uint32_t kSrcQThreads = 256;
 constexpr uint32_t kSrcQChunks = 4;  // 16-element chunks per thread: a unit holds at most 4 * 256 of them (a 128x128 block)
 
 // One CTA's work: one group of a block-scaled shard (its part of a global 128x128 block), or a band of whole rows of
-// a per-channel shard (one group per row) of at most kSqStageBytes source bytes and kSrcQChunks * kSrcQThreads
+// a per-channel shard (one group per row) of at most kSqStageBytes source bytes and kSrcQChunks * kQuantThreads
 // 16-element chunks.  Source and destination are the shard's own contiguous rows.
 struct alignas(8) SrcQUnit {
   uint64_t src;          // source element (0, 0) of the unit
@@ -405,20 +518,12 @@ struct alignas(8) SrcQUnit {
 };
 static_assert(sizeof(SrcQUnit) == 48, "SrcQUnit is part of tsb_source_quant_compile_host's output");
 
-struct SrcQTables {
+struct SrcQTables : PlanBytes {
   std::vector<SrcQUnit> units;  // grouped by source dtype: bf16, then f16, then f32 (one kernel launch each)
   std::vector<SqTile> tiles;    // two-pass path: per-tensor groups and long per-channel rows
   uint32_t n_groups = 0;        // amax words of the two-pass path
   uint32_t n_units[3] = {};     // units per source dtype, in the order above
   uint32_t unit_bytes = 0;      // largest unit's source bytes
-  uint64_t src_bytes = 0, payload_bytes = 0;
 };
-int source_quant_compile(const tsb_source_quant_target_t* targets, uint64_t n, SrcQTables* out);
-struct SrcQLaunch {
-  const SrcQUnit* units;
-  uint32_t n_units[3];  // bf16, f16, f32 units, consecutive in the table
-  SqLaunch two_pass;    // tiles of the two-pass path, run by scaled_fp8.cu's amax and quantise kernels
-};
-int launch_source_quant(const SrcQLaunch& l, cudaStream_t stream);
 
 }  // namespace tsb

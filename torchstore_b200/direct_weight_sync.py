@@ -699,20 +699,11 @@ class DirectWeightSyncDest:
         try:
             for dev, (pairs, sources) in dq.items():
                 names = [n for n, _ in sources.values()]
-                try:
-                    self._dequant_plans.update(Plans.build_dequant_fp8({dev: (pairs, [s for _, s in sources.values()])}))
-                except _native.TsbError as e:
-                    m = re.search(r"source (\d+)", str(e))
-                    if e.code == _native.TSB_ERR_INVALID and m:
-                        raise ValueError(f"dequantising pull of '{names[int(m.group(1))]}': {e}") from e
-                    raise
-        except BaseException:
-            self._dequant_plans.close()
-            self._native_plans.close()
-            raise
-        if not scaled:
-            return
-        try:
+                _build_named(self._dequant_plans, Plans.build_dequant_fp8,
+                             {dev: (pairs, [s for _, s in sources.values()])}, {"source": names},
+                             lambda n: f"dequantising pull of '{n}'")
+            if not scaled:
+                return
             for dev in sorted({scaled[n][1].device.index for n in requant or ()}):
                 names = [n for n in requant if scaled[n][1].device.index == dev]
                 targets = []
@@ -722,15 +713,10 @@ class DirectWeightSyncDest:
                     code = _native.TSB_SCALE_PER_BLOCK if kw == "block_scales" else _GRANULARITY[kw]
                     targets.append(_native.SqTarget(d.data_ptr(), s.data_ptr(), d.numel() // (rows * cols), rows, cols, code, 0))
                 pairs, sources = rq.get(dev, ([], {}))
-                src_names = [n for n, _ in sources.values()]
-                try:
-                    self._requant_plans.update(Plans.build_requant_fp8({dev: (pairs, [s for _, s in sources.values()], targets)}))
-                except _native.TsbError as e:
-                    m = re.search(r"target (\d+)", str(e)) or re.search(r"source (\d+)", str(e))
-                    if e.code == _native.TSB_ERR_INVALID and m:
-                        name = (names if m.group(0).startswith("target") else src_names)[int(m.group(1))]
-                        raise ValueError(f"requantising pull of '{name}' ({scaled[name][0]}): {e}") from e
-                    raise
+                _build_named(self._requant_plans, Plans.build_requant_fp8,
+                             {dev: (pairs, [s for _, s in sources.values()], targets)},
+                             {"target": names, "source": [n for n, _ in sources.values()]},
+                             lambda n: f"requantising pull of '{n}' ({scaled[n][0]})")
             for block in (True, False):
                 for dev in sorted({d.device.index for n, (kw, d, _) in scaled.items()
                                    if (kw == "block_scales") == block and n not in (requant or ())}):
@@ -745,25 +731,20 @@ class DirectWeightSyncDest:
                         else:
                             targets.append(_native.SqTarget(d.data_ptr(), s.data_ptr(), d.numel() // (rows * cols), rows, cols,
                                                             _GRANULARITY[kw], 0))
-                    pairs = quant_pairs.get((dev, block), [])
-                    try:
-                        if block:
-                            self._block_plans.update(Plans.build_block_fp8({dev: (pairs, targets)}))
-                        else:
-                            self._scaled_plans.update(Plans.build_scaled_fp8({dev: (pairs, targets)}))
-                    except _native.TsbError as e:
-                        m = re.search(r"target (\d+)", str(e))
-                        if e.code == _native.TSB_ERR_INVALID and m:
-                            name = names[int(m.group(1))]
-                            raise ValueError(f"{SCALE_KINDS[scaled[name][0]][1]} pull of '{name}' ({scaled[name][0]}): {e}") from e
-                        raise
+                    plans, build = (self._block_plans, Plans.build_block_fp8) if block else \
+                        (self._scaled_plans, Plans.build_scaled_fp8)
+                    _build_named(plans, build, {dev: (quant_pairs.get((dev, block), []), targets)}, {"target": names},
+                                 lambda n: f"{SCALE_KINDS[scaled[n][0]][1]} pull of '{n}' ({scaled[n][0]})")
         except BaseException:
-            self._requant_plans.close()
-            self._block_plans.close()
-            self._scaled_plans.close()
-            self._dequant_plans.close()
+            for plans in self._fp8_plans:
+                plans.close()
             self._native_plans.close()
             raise
+
+    @property
+    def _fp8_plans(self) -> tuple:
+        """The scaled fp8 plans in launch order (after the copy plan on each device's copy stream)."""
+        return self._block_plans, self._scaled_plans, self._dequant_plans, self._requant_plans
 
     def plan_info(self) -> dict[int, dict]:
         return self._native_plans.info()
@@ -871,20 +852,15 @@ class DirectWeightSyncDest:
         if self._plan is None:
             raise RuntimeError("pull() must build the plan first")
         self._native_plans.launch()
-        if self._block_plans:
-            self._block_plans.launch()
-        if self._scaled_plans:
-            self._scaled_plans.launch()
-        if self._dequant_plans:
-            self._dequant_plans.launch()
-        if self._requant_plans:
-            self._requant_plans.launch()
+        for plans in self._fp8_plans:
+            if plans:
+                plans.launch()
 
     async def wait(self) -> None:
         await self._native_plans.wait()
         ms = self._native_plans.elapsed_ms()
         # the plans of a device run back to back on its copy stream
-        for plans in (self._block_plans, self._scaled_plans, self._dequant_plans, self._requant_plans):
+        for plans in self._fp8_plans:
             if plans:
                 await plans.wait()
                 for dev, t in plans.elapsed_ms().items():
@@ -893,13 +869,25 @@ class DirectWeightSyncDest:
 
     def close(self) -> None:
         self._native_plans.close()
-        self._block_plans.close()
-        self._scaled_plans.close()
-        self._dequant_plans.close()
-        self._requant_plans.close()
+        for plans in self._fp8_plans:
+            plans.close()
         self._scale_keys = frozenset()
         self._plan = None
         self._plan_ids = self._plan_refs = self._plan_dict = self._plan_scale_dicts = None
+
+
+def _build_named(plans: Plans, build, per_device: dict, names: dict[str, list[str]], pull_of) -> None:
+    """Add ``build(per_device)`` (a ``Plans.build_*`` call) to ``plans``.  A TSB_ERR_INVALID naming "target N" (or else
+    "source N") becomes a ValueError naming the weight ``names[noun][N]``, whose pull ``pull_of(name)`` describes."""
+    try:
+        plans.update(build(per_device))
+    except _native.TsbError as e:
+        if e.code == _native.TSB_ERR_INVALID:
+            for noun, by_index in names.items():
+                m = re.search(noun + r" (\d+)", str(e))
+                if m:
+                    raise ValueError(f"{pull_of(by_index[int(m.group(1))])}: {e}") from e
+        raise
 
 
 def _add_dq_source(sources: dict, op: _TransferOp, dev: int) -> None:

@@ -92,91 +92,50 @@ class Plans(dict):
         return plans
 
     @classmethod
-    def build_block_fp8(cls, per_device: dict[int, tuple[list, list]]) -> "Plans":
-        """Compile block-scaled fp8 pulls: ``{device: ([(src, dst) StridedMem windows], [BqTarget])}``."""
+    def build_fp8(cls, create, per_device: dict[int, tuple]) -> "Plans":
+        """Compile scaled fp8 plans: ``create(device, *args)`` for each ``{device: args}``, ``create`` being one of
+        the ``_native.*_plan_create`` calls."""
         plans = cls()
         try:
-            for dev, (pairs, targets) in per_device.items():
-                rects, n = build_rects(pairs)
-                arr = _native.make_target_array(max(1, len(targets)))
-                for i, t in enumerate(targets):
-                    arr[i] = t
-                plans[dev] = _native.block_fp8_plan_create(dev, rects, n, arr, len(targets))
+            for dev, args in per_device.items():
+                plans[dev] = create(dev, *args)
         except BaseException:
             plans.close()
             raise
         return plans
+
+    @classmethod
+    def _build_pulls(cls, create, per_device: dict[int, tuple]) -> "Plans":
+        """build_fp8 of pulls: ``{device: ([(src, dst) StridedMem windows], *tables)}``, the windows as rects."""
+        return cls.build_fp8(create, {dev: (*build_rects(pairs), *tables) for dev, (pairs, *tables) in per_device.items()})
+
+    @classmethod
+    def build_block_fp8(cls, per_device: dict[int, tuple[list, list]]) -> "Plans":
+        """Compile block-scaled fp8 pulls: ``{device: ([(src, dst) StridedMem windows], [BqTarget])}``."""
+        return cls._build_pulls(_native.block_fp8_plan_create, per_device)
 
     @classmethod
     def build_scaled_fp8(cls, per_device: dict[int, tuple[list, list]]) -> "Plans":
         """Compile per-channel / per-tensor scaled fp8 pulls: ``{device: ([(src, dst) StridedMem windows],
         [SqTarget])}``."""
-        plans = cls()
-        try:
-            for dev, (pairs, targets) in per_device.items():
-                rects, n = build_rects(pairs)
-                arr = _native.make_sq_target_array(max(1, len(targets)))
-                for i, t in enumerate(targets):
-                    arr[i] = t
-                plans[dev] = _native.scaled_fp8_plan_create(dev, rects, n, arr, len(targets))
-        except BaseException:
-            plans.close()
-            raise
-        return plans
+        return cls._build_pulls(_native.scaled_fp8_plan_create, per_device)
 
     @classmethod
     def build_dequant_fp8(cls, per_device: dict[int, tuple[list, list]]) -> "Plans":
         """Compile dequantising pulls of scaled fp8 sources: ``{device: ([(src, dst) StridedMem windows],
         [DqSource])}``."""
-        plans = cls()
-        try:
-            for dev, (pairs, sources) in per_device.items():
-                rects, n = build_rects(pairs)
-                arr = _native.make_dq_source_array(max(1, len(sources)))
-                for i, s in enumerate(sources):
-                    arr[i] = s
-                plans[dev] = _native.dequant_fp8_plan_create(dev, rects, n, arr, len(sources))
-        except BaseException:
-            plans.close()
-            raise
-        return plans
+        return cls._build_pulls(_native.dequant_fp8_plan_create, per_device)
 
     @classmethod
     def build_requant_fp8(cls, per_device: dict[int, tuple[list, list, list]]) -> "Plans":
         """Compile requantising pulls of scaled fp8 sources into scaled fp8 destinations: ``{device:
         ([(src, dst) StridedMem windows], [DqSource], [SqTarget])}``."""
-        plans = cls()
-        try:
-            for dev, (pairs, sources, targets) in per_device.items():
-                rects, n = build_rects(pairs)
-                for i in range(n):  # a same-dtype fp8 window is an opaque byte move to build_rects
-                    rects[i].src_dtype = rects[i].dst_dtype = _native.TSB_F8E4M3
-                src_arr = _native.make_dq_source_array(max(1, len(sources)))
-                for i, s in enumerate(sources):
-                    src_arr[i] = s
-                arr = _native.make_sq_target_array(max(1, len(targets)))
-                for i, t in enumerate(targets):
-                    arr[i] = t
-                plans[dev] = _native.requant_fp8_plan_create(dev, rects, n, src_arr, len(sources), arr, len(targets))
-        except BaseException:
-            plans.close()
-            raise
-        return plans
+        return cls._build_pulls(_native.requant_fp8_plan_create, per_device)
 
     @classmethod
     def build_source_quant(cls, per_device: dict[int, list]) -> "Plans":
         """Compile source-side quantisations: ``{device: [SourceQuantTarget]}``."""
-        plans = cls()
-        try:
-            for dev, targets in per_device.items():
-                arr = _native.make_source_quant_target_array(max(1, len(targets)))
-                for i, t in enumerate(targets):
-                    arr[i] = t
-                plans[dev] = _native.source_quant_plan_create(dev, arr, len(targets))
-        except BaseException:
-            plans.close()
-            raise
-        return plans
+        return cls.build_fp8(_native.source_quant_plan_create, {dev: (targets,) for dev, targets in per_device.items()})
 
     def launch(self, fence_out: bool = True) -> None:
         """Enqueue every plan on its device's copy stream, fenced in against the caller's current
