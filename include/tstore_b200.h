@@ -26,8 +26,17 @@
 extern "C" {
 #endif
 
-#define TSB_ABI_VERSION 8
+#define TSB_ABI_VERSION 9
 #define TSB_MAX_DIMS 6
+
+/* `flags` bit of the quantising plan calls (tsb_block_fp8_*, tsb_scaled_fp8_*, tsb_requant_fp8_*,
+ * tsb_source_quant_*): power-of-two (UE8M0) scales.  Per group, with t = amax_c / 448 correctly rounded,
+ *   scale_inv = t                                      if t's mantissa bits are 0 (a power of two, or Inf)
+ *               (bits(t) & 0x7f800000) + 0x00800000    otherwise (the next power of two up)
+ *   dst = e4m3fn(rn(x * (1 / scale_inv)))              (1 / scale_inv is exact; 0 for Inf)
+ * still stored as float32.  The flag selects the kernels only: *_compile_host returns the same tables with and
+ * without it.  The dequantising calls refuse it (TSB_ERR_INVALID), as they refuse every other bit. */
+#define TSB_QUANT_UE8M0 1u
 
 enum {
   TSB_OK = 0,
@@ -226,7 +235,7 @@ typedef struct tsb_bq_target {
  * src_dtype in {TSB_F32, TSB_BF16, TSB_F16}, dst_dtype == TSB_F8E4M3 and dst inside one target.
  * Every element of every target must be written by exactly one rect (TSB_ERR_INVALID otherwise: a
  * block's scale needs all of it).  The result is a plan like any other: tsb_plan_launch[_flags],
- * _run, _poll, _wait, _elapsed_ms, _info and _destroy accept it.  flags: reserved, pass 0. */
+ * _run, _poll, _wait, _elapsed_ms, _info and _destroy accept it.  flags: 0 or TSB_QUANT_UE8M0. */
 int tsb_block_fp8_plan_create(int device, const tsb_rect_t* rects, uint64_t n, const tsb_bq_target_t* targets,
                               uint64_t n_targets, uint32_t flags, tsb_plan_t* out);
 /* Host-only (no CUDA call): compile and copy the kernel tables out.  out_blocks: records of 32 bytes
@@ -264,7 +273,7 @@ typedef struct tsb_sq_target {
  * naming the target and group otherwise).  A per-channel row of at most 32 KiB of source bytes is
  * quantised from shared memory after one read; per-tensor groups and longer rows take two passes
  * (amax, then quantise), reading the source twice.  The result is a plan like any other.
- * flags: reserved, pass 0. */
+ * flags: 0 or TSB_QUANT_UE8M0. */
 int tsb_scaled_fp8_plan_create(int device, const tsb_rect_t* rects, uint64_t n, const tsb_sq_target_t* targets,
                                uint64_t n_targets, uint32_t flags, tsb_plan_t* out);
 /* Host-only (no CUDA call): compile and copy the kernel tables out.  A NULL table only reports its count.
@@ -313,7 +322,8 @@ typedef struct tsb_dq_source {
 /* Compile a dequantising pull: `rects` are ordinary source -> destination rectangles with src_dtype
  * == TSB_F8E4M3, dst_dtype in {TSB_F32, TSB_BF16, TSB_F16} and src inside one source (TSB_ERR_INVALID
  * naming the rect or source otherwise).  Elements no rect reads are left alone.  The result is a plan
- * like any other.  flags: reserved, pass 0. */
+ * like any other.  flags: reserved, pass 0 (TSB_QUANT_UE8M0 is refused: a float32 scale dequantises the
+ * same whatever its format). */
 int tsb_dequant_fp8_plan_create(int device, const tsb_rect_t* rects, uint64_t n, const tsb_dq_source_t* sources,
                                 uint64_t n_sources, uint32_t flags, tsb_plan_t* out);
 /* Host-only (no CUDA call): compile and copy the tile table out (one CTA per tile).  out_tiles: records
@@ -342,7 +352,8 @@ int tsb_dequant_fp8_compile_host(int device, const tsb_rect_t* rects, uint64_t n
  * its source shard (TSB_ERR_INVALID naming the rect otherwise); every element of every target must be
  * written by exactly one rect (TSB_ERR_INVALID naming the target and group otherwise).  Block targets and
  * per-channel rows of at most 32 KiB read each source byte once; per-tensor groups and longer rows take two
- * passes.  The result is a plan like any other.  flags: reserved, pass 0. */
+ * passes.  The result is a plan like any other.  flags: 0 or TSB_QUANT_UE8M0 (the target's formula with
+ * power-of-two scales). */
 int tsb_requant_fp8_plan_create(int device, const tsb_rect_t* rects, uint64_t n, const tsb_dq_source_t* sources,
                                 uint64_t n_sources, const tsb_sq_target_t* targets, uint64_t n_targets, uint32_t flags,
                                 tsb_plan_t* out);
@@ -392,7 +403,7 @@ typedef struct tsb_source_quant_target {
 /* Compile a source-side quantisation of `n` targets (TSB_ERR_INVALID naming the target otherwise).  Blocks and
  * per-channel rows of at most 32 KiB of source bytes are quantised from registers after one read, one CTA per
  * block or band of rows; per-tensor groups and longer rows take two passes (amax, then quantise).  The result is a plan like any other: tsb_plan_launch[_flags],
- * _run, _poll, _wait, _elapsed_ms, _info and _destroy accept it.  flags: reserved, pass 0. */
+ * _run, _poll, _wait, _elapsed_ms, _info and _destroy accept it.  flags: 0 or TSB_QUANT_UE8M0. */
 int tsb_source_quant_plan_create(int device, const tsb_source_quant_target_t* targets, uint64_t n, uint32_t flags,
                                  tsb_plan_t* out);
 /* Host-only (no CUDA call): compile and copy the kernel tables out.  A NULL table only reports its count.

@@ -16,13 +16,14 @@ import torch
 from torchstore_b200._build import LIB_PATH
 
 TSB_MAX_DIMS = 6
-TSB_ABI_VERSION = 8
+TSB_ABI_VERSION = 9
 
 TSB_OK, TSB_ERR_INVALID, TSB_ERR_CUDA, TSB_ERR_UNSUPPORTED, TSB_ERR_NOMEM, TSB_ERR_NOTFOUND = range(6)
 
 TSB_U8, TSB_U16, TSB_U32, TSB_U64, TSB_F16, TSB_BF16, TSB_F32, TSB_F64, TSB_F8E4M3, TSB_F8E5M2 = range(10)
 TSB_H2D, TSB_D2H, TSB_D2D = 1, 2, 3
 TSB_PLAN_DEFAULT, TSB_PLAN_NO_INTERLEAVE = 0, 1
+TSB_QUANT_UE8M0 = 1  # flags of the quantising plan calls: power-of-two scales
 
 
 class TsbError(RuntimeError):
@@ -480,10 +481,10 @@ def plan_compile_host(device: int, rects, n: int, flags: int = 0, tile_units: in
     return rect_buf[: n_rects.value * 192], tile_buf[: n_tiles.value], info
 
 
-def _plan_create(fn, *args) -> int:
-    """One of the tsb_*_plan_create calls of the scaled fp8 plans (flags 0) -> plan id."""
+def _plan_create(fn, *args, flags: int = 0) -> int:
+    """One of the tsb_*_plan_create calls of the scaled fp8 plans -> plan id."""
     out = C.c_uint64(0)
-    check(fn(*args, 0, C.byref(out)))
+    check(fn(*args, flags, C.byref(out)))
     return int(out.value)
 
 
@@ -492,8 +493,8 @@ def _structs(struct, items: list) -> tuple:
     return (struct * max(1, len(items)))(*items), len(items)
 
 
-def _compile_host(fn, args: tuple, dtypes: list, n_groups: bool) -> list:
-    """Call a tsb_*_compile_host (flags 0) for its record counts, then for its tables -> one numpy record array per
+def _compile_host(fn, args: tuple, dtypes: list, n_groups: bool, flags: int = 0) -> list:
+    """Call a tsb_*_compile_host for its record counts, then for its tables -> one numpy record array per
     table (dtypes: their layouts, in output order), then the number of two-pass groups if the call reports it."""
     import numpy as np
 
@@ -504,7 +505,7 @@ def _compile_host(fn, args: tuple, dtypes: list, n_groups: bool) -> list:
         outs = []
         for t, c in zip(tables, counts):
             outs += [None, 0, C.byref(c)] if t is None else [t.ctypes.data, c.value, C.byref(c)]
-        check(fn(*args, 0, *outs, *([C.byref(ng)] if n_groups else [])))
+        check(fn(*args, flags, *outs, *([C.byref(ng)] if n_groups else [])))
 
     call([None] * len(dtypes))
     tables = [np.zeros(max(1, c.value), dtype=dt) for c, dt in zip(counts, dtypes)]
@@ -516,8 +517,8 @@ def make_target_array(n: int):
     return (BqTarget * n)()
 
 
-def block_fp8_plan_create(device: int, rects, n: int, targets: list) -> int:
-    return _plan_create(lib().tsb_block_fp8_plan_create, device, rects, n, *_structs(BqTarget, targets))
+def block_fp8_plan_create(device: int, rects, n: int, targets: list, flags: int = 0) -> int:
+    return _plan_create(lib().tsb_block_fp8_plan_create, device, rects, n, *_structs(BqTarget, targets), flags=flags)
 
 
 # record layouts of tsb_block_fp8_compile_host (include/tstore_b200.h)
@@ -527,18 +528,18 @@ BQ_PIECE_DTYPE = [("src", "<u8"), ("src_stride", "<i8"), ("row0", "<u2"), ("col0
                   ("cols", "<u2"), ("vec", "<u4"), ("pad", "<u4")]
 
 
-def block_fp8_compile_host(device: int, rects, n: int, targets, n_targets: int):
+def block_fp8_compile_host(device: int, rects, n: int, targets, n_targets: int, flags: int = 0):
     """Host-only compilation of a block-scaled fp8 pull -> (blocks, pieces) numpy record arrays."""
     return tuple(_compile_host(lib().tsb_block_fp8_compile_host, (device, rects, n, targets, n_targets),
-                               [BQ_BLOCK_DTYPE, BQ_PIECE_DTYPE], False))
+                               [BQ_BLOCK_DTYPE, BQ_PIECE_DTYPE], False, flags))
 
 
 def make_sq_target_array(n: int):
     return (SqTarget * n)()
 
 
-def scaled_fp8_plan_create(device: int, rects, n: int, targets: list) -> int:
-    return _plan_create(lib().tsb_scaled_fp8_plan_create, device, rects, n, *_structs(SqTarget, targets))
+def scaled_fp8_plan_create(device: int, rects, n: int, targets: list, flags: int = 0) -> int:
+    return _plan_create(lib().tsb_scaled_fp8_plan_create, device, rects, n, *_structs(SqTarget, targets), flags=flags)
 
 
 # record layouts of tsb_scaled_fp8_compile_host (include/tstore_b200.h)
@@ -550,19 +551,19 @@ SQ_TILE_DTYPE = [("src", "<u8"), ("src_stride", "<i8"), ("dst", "<u8"), ("scale_
                  ("rows", "<u4"), ("cols", "<u4"), ("group", "<u4"), ("src_dtype", "<u4"), ("vec", "<u4")]
 
 
-def scaled_fp8_compile_host(device: int, rects, n: int, targets, n_targets: int):
+def scaled_fp8_compile_host(device: int, rects, n: int, targets, n_targets: int, flags: int = 0):
     """Host-only compilation of a per-channel / per-tensor scaled fp8 pull -> (bands, pieces, tiles,
     n_groups): numpy record arrays and the number of two-pass groups."""
     return tuple(_compile_host(lib().tsb_scaled_fp8_compile_host, (device, rects, n, targets, n_targets),
-                               [SQ_BAND_DTYPE, SQ_PIECE_DTYPE, SQ_TILE_DTYPE], True))
+                               [SQ_BAND_DTYPE, SQ_PIECE_DTYPE, SQ_TILE_DTYPE], True, flags))
 
 
 def make_dq_source_array(n: int):
     return (DqSource * n)()
 
 
-def dequant_fp8_plan_create(device: int, rects, n: int, sources: list) -> int:
-    return _plan_create(lib().tsb_dequant_fp8_plan_create, device, rects, n, *_structs(DqSource, sources))
+def dequant_fp8_plan_create(device: int, rects, n: int, sources: list, flags: int = 0) -> int:
+    return _plan_create(lib().tsb_dequant_fp8_plan_create, device, rects, n, *_structs(DqSource, sources), flags=flags)
 
 
 # record layout of tsb_dequant_fp8_compile_host (include/tstore_b200.h)
@@ -571,17 +572,17 @@ DQ_TILE_DTYPE = [("src", "<u8"), ("dst", "<u8"), ("scale", "<u8"), ("src_stride"
                  ("pad", "<u4")]
 
 
-def dequant_fp8_compile_host(device: int, rects, n: int, sources, n_sources: int):
+def dequant_fp8_compile_host(device: int, rects, n: int, sources, n_sources: int, flags: int = 0):
     """Host-only compilation of a dequantising pull -> its tile table as a numpy record array."""
     return _compile_host(lib().tsb_dequant_fp8_compile_host, (device, rects, n, sources, n_sources), [DQ_TILE_DTYPE],
-                         False)[0]
+                         False, flags)[0]
 
 
-def requant_fp8_plan_create(device: int, rects, n: int, sources: list, targets: list) -> int:
+def requant_fp8_plan_create(device: int, rects, n: int, sources: list, targets: list, flags: int = 0) -> int:
     for i in range(n):  # a same-dtype fp8 window is an opaque byte move to build_rects
         rects[i].src_dtype = rects[i].dst_dtype = TSB_F8E4M3
     return _plan_create(lib().tsb_requant_fp8_plan_create, device, rects, n, *_structs(DqSource, sources),
-                        *_structs(SqTarget, targets))
+                        *_structs(SqTarget, targets), flags=flags)
 
 
 # record layouts of tsb_requant_fp8_compile_host (include/tstore_b200.h)
@@ -595,19 +596,20 @@ RQ_TILE_DTYPE = [("src", "<u8"), ("src_stride", "<i8"), ("scale", "<u8"), ("dst"
                  ("vec", "<u4")]
 
 
-def requant_fp8_compile_host(device: int, rects, n: int, sources, n_sources: int, targets, n_targets: int):
+def requant_fp8_compile_host(device: int, rects, n: int, sources, n_sources: int, targets, n_targets: int,
+                             flags: int = 0):
     """Host-only compilation of a requantising pull -> (units, pieces, tiles, n_groups): numpy record arrays
     and the number of two-pass groups."""
     return tuple(_compile_host(lib().tsb_requant_fp8_compile_host, (device, rects, n, sources, n_sources, targets, n_targets),
-                               [RQ_UNIT_DTYPE, RQ_PIECE_DTYPE, RQ_TILE_DTYPE], True))
+                               [RQ_UNIT_DTYPE, RQ_PIECE_DTYPE, RQ_TILE_DTYPE], True, flags))
 
 
 def make_source_quant_target_array(n: int):
     return (SourceQuantTarget * n)()
 
 
-def source_quant_plan_create(device: int, targets: list) -> int:
-    return _plan_create(lib().tsb_source_quant_plan_create, device, *_structs(SourceQuantTarget, targets))
+def source_quant_plan_create(device: int, targets: list, flags: int = 0) -> int:
+    return _plan_create(lib().tsb_source_quant_plan_create, device, *_structs(SourceQuantTarget, targets), flags=flags)
 
 
 # record layout of the units of tsb_source_quant_compile_host (include/tstore_b200.h); its tiles are SQ_TILE_DTYPE
@@ -615,11 +617,11 @@ SRCQ_UNIT_DTYPE = [("src", "<u8"), ("dst", "<u8"), ("scale_inv", "<u8"), ("src_p
                    ("rows", "<u4"), ("cols", "<u4"), ("per_row", "<u4"), ("src_dtype", "<u2"), ("vec", "<u2")]
 
 
-def source_quant_compile_host(device: int, targets, n: int):
+def source_quant_compile_host(device: int, targets, n: int, flags: int = 0):
     """Host-only compilation of a source-side quantisation -> (units, tiles, n_groups): numpy record arrays and
     the number of two-pass groups."""
     return tuple(_compile_host(lib().tsb_source_quant_compile_host, (device, targets, n), [SRCQ_UNIT_DTYPE, SQ_TILE_DTYPE],
-                               True))
+                               True, flags))
 
 
 CUDA_STREAM_LEGACY = 0x1  # cudaStreamLegacy: an explicit handle for the default stream

@@ -160,12 +160,12 @@ async def put_state_dict(state_dict: dict[str, Any] | None, key: str, store_name
                          block_scales: "dict[str, torch.Tensor] | None" = None,
                          channel_scales: "dict[str, torch.Tensor] | None" = None,
                          tensor_scales: "dict[str, torch.Tensor] | None" = None,
-                         quantize: "dict[str, str] | None" = None) -> None:
+                         quantize: "dict[str, str] | None" = None, scale_fmt: "str | None" = None) -> None:
     cl = await client(store_name)
     await state_dict_utils.put_state_dict(store=cl, state_dict=state_dict, key=key, direct_rdma=direct_rdma,
                                           transfer_dtype=transfer_dtype, block_scales=block_scales,
                                           channel_scales=channel_scales, tensor_scales=tensor_scales,
-                                          quantize=quantize)
+                                          quantize=quantize, scale_fmt=scale_fmt)
 
 
 async def get_state_dict(key: str, user_state_dict: dict[str, Any] | None = None, strict: bool = True,
@@ -173,8 +173,9 @@ async def get_state_dict(key: str, user_state_dict: dict[str, Any] | None = None
                          block_scales: "dict[str, torch.Tensor] | None" = None,
                          channel_scales: "dict[str, torch.Tensor] | None" = None,
                          tensor_scales: "dict[str, torch.Tensor] | None" = None,
-                         requantize: bool = False) -> dict[str, Any]:
+                         requantize: bool = False, scale_fmt: "str | None" = None) -> dict[str, Any]:
     cl = await client(store_name)
     return await state_dict_utils.get_state_dict(cl, key, user_state_dict, strict, direct_rdma=direct_rdma,
                                                  block_scales=block_scales, channel_scales=channel_scales,
-                                                 tensor_scales=tensor_scales, requantize=requantize)
+                                                 tensor_scales=tensor_scales, requantize=requantize,
+                                                 scale_fmt=scale_fmt)

@@ -12,7 +12,8 @@
 //            bit cleared): for non-negative floats that orders finite < Inf < NaN, so a NaN anywhere
 //            makes the block's amax NaN (fmaxf would drop it).
 //   reduce   warp max, then one thread: amax_c = max(amax, 1e-4f), scale = 448 / amax_c and
-//            scale_inv = amax_c / 448, both correctly rounded (__fdiv_rn).
+//            scale_inv = amax_c / 448, both correctly rounded (__fdiv_rn); with TSB_QUANT_UE8M0 scale_inv is
+//            rounded up to a power of two and scale = 1 / scale_inv (fp8_quant.cuh).
 //   phase 2  shared -> e4m3fn: x * scale (__fmul_rn), torch-exact narrowing (fp8_cvt.cuh), 16
 //            destination bytes per thread and step (one STG.128 when aligned, byte stores at ragged edges).
 
@@ -381,12 +382,12 @@ __device__ __forceinline__ void quantise_block(const BqBlock& blk, const unsigne
   }
 }
 
-template <uint32_t DT>
+template <uint32_t DT, bool kUe8m0>
 __device__ __forceinline__ void run_block(const BqBlock& blk, const BqPiece* pieces, unsigned char* smem, uint32_t* s_red,
                                           float* s_scale) {
   cta_max(stage_block<DT>(blk, pieces, smem), s_red, [&](uint32_t a) {
     float scale, scale_inv;
-    scales_of_amax(a, &scale, &scale_inv);
+    group_scales<kUe8m0>(a, &scale, &scale_inv);
     *s_scale = scale;
     *reinterpret_cast<float*>(blk.scale) = scale_inv;
   });
@@ -394,15 +395,17 @@ __device__ __forceinline__ void run_block(const BqBlock& blk, const BqPiece* pie
   quantise_block<DT>(blk, smem, *s_scale);
 }
 
+// kUe8m0: power-of-two scales (TSB_QUANT_UE8M0)
+template <bool kUe8m0>
 __global__ void __launch_bounds__(kQuantThreads, 6) block_fp8_kernel(const BqBlock* __restrict__ blocks, const BqPiece* __restrict__ pieces) {
   extern __shared__ __align__(16) unsigned char stage[];
   __shared__ uint32_t s_red[kQuantThreads / 32];
   __shared__ float s_scale;
   const BqBlock blk = blocks[blockIdx.x];
   switch (blk.src_dtype) {
-    case TSB_BF16: run_block<TSB_BF16>(blk, pieces, stage, s_red, &s_scale); break;
-    case TSB_F16: run_block<TSB_F16>(blk, pieces, stage, s_red, &s_scale); break;
-    default: run_block<TSB_F32>(blk, pieces, stage, s_red, &s_scale); break;
+    case TSB_BF16: run_block<TSB_BF16, kUe8m0>(blk, pieces, stage, s_red, &s_scale); break;
+    case TSB_F16: run_block<TSB_F16, kUe8m0>(blk, pieces, stage, s_red, &s_scale); break;
+    default: run_block<TSB_F32, kUe8m0>(blk, pieces, stage, s_red, &s_scale); break;
   }
 }
 
@@ -414,15 +417,20 @@ cudaError_t prepare() {
   if (e != cudaSuccess) return e;
   const uint64_t bit = 1ull << (dev & 63);
   if (prepared.load(std::memory_order_acquire) & bit) return cudaSuccess;
-  e = cudaFuncSetAttribute(block_fp8_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(kBqBlock * kBqBlock * 4));
-  if (e == cudaSuccess) prepared.fetch_or(bit, std::memory_order_release);
+  for (auto kernel : {block_fp8_kernel<false>, block_fp8_kernel<true>}) {
+    e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(kBqBlock * kBqBlock * 4));
+    if (e != cudaSuccess) return e;
+  }
+  prepared.fetch_or(bit, std::memory_order_release);
   return e;
 }
 
-int launch_block_fp8(const BqBlock* blocks, const BqPiece* pieces, uint32_t n_blocks, uint32_t max_src_bytes, cudaStream_t stream) {
+int launch_block_fp8(const BqBlock* blocks, const BqPiece* pieces, uint32_t n_blocks, uint32_t max_src_bytes, bool ue8m0,
+                     cudaStream_t stream) {
   const cudaError_t e = prepare();
   if (e != cudaSuccess) return cuda_fail(e, "block_fp8_kernel launch");
-  block_fp8_kernel<<<n_blocks, kQuantThreads, kBqBlock * kBqBlock * max_src_bytes, stream>>>(blocks, pieces);
+  const auto kernel = ue8m0 ? block_fp8_kernel<true> : block_fp8_kernel<false>;
+  kernel<<<n_blocks, kQuantThreads, kBqBlock * kBqBlock * max_src_bytes, stream>>>(blocks, pieces);
   return launched("block_fp8_kernel launch");
 }
 
@@ -436,8 +444,10 @@ int block_fp8_plan(int device, const tsb_rect_t* rects, uint64_t n, const tsb_bq
   const size_t pieces = q->add(tb.pieces);
   q->seal(0);
   q->describe(n, static_cast<uint32_t>(tb.blocks.size()), kBqBlock * kBqBlock, tb);
-  q->launch = [pieces, n_blocks = static_cast<uint32_t>(tb.blocks.size()), es = tb.max_src_bytes](char* d, cudaStream_t s) {
-    return launch_block_fp8(reinterpret_cast<const BqBlock*>(d), reinterpret_cast<const BqPiece*>(d + pieces), n_blocks, es, s);
+  q->launch = [pieces, n_blocks = static_cast<uint32_t>(tb.blocks.size()), es = tb.max_src_bytes, ue8m0 = q->ue8m0](char* d,
+                                                                                                               cudaStream_t s) {
+    return launch_block_fp8(reinterpret_cast<const BqBlock*>(d), reinterpret_cast<const BqPiece*>(d + pieces), n_blocks, es, ue8m0,
+                            s);
   };
   return TSB_OK;
 }
@@ -450,14 +460,14 @@ using namespace tsb;
 
 extern "C" int tsb_block_fp8_plan_create(int device, const tsb_rect_t* rects, uint64_t n, const tsb_bq_target_t* targets,
                                          uint64_t n_targets, uint32_t flags, tsb_plan_t* out) {
-  return quant_plan_create("tsb_block_fp8_plan_create", device, flags, out,
+  return quant_plan_create("tsb_block_fp8_plan_create", device, flags, TSB_QUANT_UE8M0, out,
                            [&](QuantPlan* q) { return block_fp8_plan(device, rects, n, targets, n_targets, q); });
 }
 
 extern "C" int tsb_block_fp8_compile_host(int device, const tsb_rect_t* rects, uint64_t n, const tsb_bq_target_t* targets,
                                           uint64_t n_targets, uint32_t flags, void* out_blocks, uint64_t block_cap,
                                           uint64_t* out_n_blocks, void* out_pieces, uint64_t piece_cap, uint64_t* out_n_pieces) {
-  return quant_compile_host("tsb_block_fp8_compile_host", flags,
+  return quant_compile_host("tsb_block_fp8_compile_host", flags, TSB_QUANT_UE8M0,
                             [&](QuantPlan* q) { return block_fp8_plan(device, rects, n, targets, n_targets, q); },
                             {{out_blocks, block_cap, out_n_blocks, "out_blocks"}, {out_pieces, piece_cap, out_n_pieces, "out_pieces"}},
                             nullptr);

@@ -210,14 +210,14 @@ using namespace tsb;
 
 extern "C" int tsb_dequant_fp8_plan_create(int device, const tsb_rect_t* rects, uint64_t n, const tsb_dq_source_t* sources,
                                            uint64_t n_sources, uint32_t flags, tsb_plan_t* out) {
-  return quant_plan_create("tsb_dequant_fp8_plan_create", device, flags, out,
+  return quant_plan_create("tsb_dequant_fp8_plan_create", device, flags, 0, out,
                            [&](QuantPlan* q) { return dequant_fp8_plan(device, rects, n, sources, n_sources, q); });
 }
 
 extern "C" int tsb_dequant_fp8_compile_host(int device, const tsb_rect_t* rects, uint64_t n, const tsb_dq_source_t* sources,
                                             uint64_t n_sources, uint32_t flags, void* out_tiles, uint64_t tile_cap,
                                             uint64_t* out_n_tiles) {
-  return quant_compile_host("tsb_dequant_fp8_compile_host", flags,
+  return quant_compile_host("tsb_dequant_fp8_compile_host", flags, 0,
                             [&](QuantPlan* q) { return dequant_fp8_plan(device, rects, n, sources, n_sources, q); },
                             {{out_tiles, tile_cap, out_n_tiles, "out_tiles"}}, nullptr);
 }

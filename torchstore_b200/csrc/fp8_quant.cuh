@@ -170,4 +170,28 @@ __device__ __forceinline__ void scales_of_amax(uint32_t a, float* scale, float* 
   }
 }
 
+// The UE8M0 variant (TSB_QUANT_UE8M0): scale_inv is t = amax_c / 448 (correctly rounded) when t is a power of two
+// (or Inf), else the next power of two up, found on t's bits; scale = 1 / scale_inv is exact (0 for Inf).  t is
+// always a normal float here (2.2e-7 <= t <= FLT_MAX / 448), so the exponent step has no subnormal or overflow
+// case.  A NaN amax gives NaN for both.
+__device__ __forceinline__ void ue8m0_scales_of_amax(uint32_t a, float* scale, float* scale_inv) {
+  if (a > 0x7f800000u) {
+    *scale = __uint_as_float(0x7fffffffu);
+    *scale_inv = *scale;
+  } else {
+    const uint32_t t = __float_as_uint(__fdiv_rn(fmaxf(__uint_as_float(a), 1e-4f), 448.0f));
+    *scale_inv = __uint_as_float((t & 0x007fffffu) ? (t & 0x7f800000u) + 0x00800000u : t);
+    *scale = __fdiv_rn(1.0f, *scale_inv);
+  }
+}
+
+// A group's (scale, scale_inv) from its amax bits, by the plan's scale format
+template <bool kUe8m0>
+__device__ __forceinline__ void group_scales(uint32_t a, float* scale, float* scale_inv) {
+  if constexpr (kUe8m0)
+    ue8m0_scales_of_amax(a, scale, scale_inv);
+  else
+    scales_of_amax(a, scale, scale_inv);
+}
+
 }  // namespace tsb

@@ -596,10 +596,21 @@ int register_plan(Plan* p, const std::vector<char>& host, tsb_plan_t* out) {
 
 }  // namespace
 
-int quant_plan_create(const char* fn, int device, uint32_t flags, tsb_plan_t* out, const QuantCompile& compile) {
+namespace {
+
+int check_quant_flags(const char* fn, uint32_t flags, uint32_t accepted) {
+  if (flags & ~accepted)
+    return fail(TSB_ERR_INVALID, std::string(fn) + (accepted ? ": flags must be 0 or TSB_QUANT_UE8M0" : ": flags must be 0"));
+  return TSB_OK;
+}
+
+}  // namespace
+
+int quant_plan_create(const char* fn, int device, uint32_t flags, uint32_t accepted, tsb_plan_t* out, const QuantCompile& compile) {
   if (!out) return fail(TSB_ERR_INVALID, std::string(fn) + ": NULL argument");
-  if (flags != 0) return fail(TSB_ERR_INVALID, std::string(fn) + ": flags must be 0");
+  if (int st = check_quant_flags(fn, flags, accepted)) return st;
   QuantPlan q;
+  q.ue8m0 = (flags & TSB_QUANT_UE8M0) != 0;
   int st = compile(&q);
   if (st) return st;
   Plan* p = new Plan();
@@ -610,10 +621,11 @@ int quant_plan_create(const char* fn, int device, uint32_t flags, tsb_plan_t* ou
   return register_plan(p, q.tables, out);
 }
 
-int quant_compile_host(const char* fn, uint32_t flags, const QuantCompile& compile, std::initializer_list<TableOut> outs,
-                       uint64_t* out_n_groups) {
-  if (flags != 0) return fail(TSB_ERR_INVALID, std::string(fn) + ": flags must be 0");
+int quant_compile_host(const char* fn, uint32_t flags, uint32_t accepted, const QuantCompile& compile,
+                       std::initializer_list<TableOut> outs, uint64_t* out_n_groups) {
+  if (int st = check_quant_flags(fn, flags, accepted)) return st;
   QuantPlan q;
+  q.ue8m0 = (flags & TSB_QUANT_UE8M0) != 0;
   int st = compile(&q);
   if (st) return st;
   size_t k = 0;

@@ -433,7 +433,7 @@ __device__ __forceinline__ void quantise_unit(const RqUnit& u, const RqPiece* __
   }
 }
 
-template <bool kPerRow>
+template <bool kPerRow, bool kUe8m0>
 __device__ __forceinline__ void run_unit(const RqUnit& u, const RqPiece* pieces, unsigned char* smem, uint32_t* s_amax,
                                          float* s_scale, uint32_t* s_red) {
   const uint32_t spitch = (u.cols + 15u) & ~15u;
@@ -446,14 +446,14 @@ __device__ __forceinline__ void run_unit(const RqUnit& u, const RqPiece* pieces,
     __syncthreads();
     for (uint32_t r = threadIdx.x; r < u.rows; r += kQuantThreads) {
       float scale, scale_inv;
-      scales_of_amax(s_amax[r], &scale, &scale_inv);
+      group_scales<kUe8m0>(s_amax[r], &scale, &scale_inv);
       s_scale[r] = scale;
       reinterpret_cast<float*>(u.scale_inv)[r] = scale_inv;
     }
   } else {
     cta_max(m, s_red, [&](uint32_t a) {
       float scale, scale_inv;
-      scales_of_amax(a, &scale, &scale_inv);
+      group_scales<kUe8m0>(a, &scale, &scale_inv);
       s_scale[0] = scale;
       *reinterpret_cast<float*>(u.scale_inv) = scale_inv;
     });
@@ -462,6 +462,8 @@ __device__ __forceinline__ void run_unit(const RqUnit& u, const RqPiece* pieces,
   quantise_unit<kPerRow>(u, pieces, smem, spitch, s_scale);
 }
 
+// kUe8m0 (here and in requant_fp8_quant_kernel): power-of-two scales (TSB_QUANT_UE8M0)
+template <bool kUe8m0>
 __global__ void __launch_bounds__(kQuantThreads) requant_fp8_staged_kernel(const RqUnit* __restrict__ units,
                                                                         const RqPiece* __restrict__ pieces) {
   extern __shared__ __align__(16) unsigned char stage[];
@@ -470,9 +472,9 @@ __global__ void __launch_bounds__(kQuantThreads) requant_fp8_staged_kernel(const
   __shared__ uint32_t s_red[kQuantThreads / 32];
   const RqUnit u = units[blockIdx.x];
   if (u.per_row)
-    run_unit<true>(u, pieces, stage, s_amax, s_scale, s_red);
+    run_unit<true, kUe8m0>(u, pieces, stage, s_amax, s_scale, s_red);
   else
-    run_unit<false>(u, pieces, stage, s_amax, s_scale, s_red);
+    run_unit<false, kUe8m0>(u, pieces, stage, s_amax, s_scale, s_red);
 }
 
 __global__ void __launch_bounds__(kQuantThreads) requant_fp8_amax_kernel(const RqTile* __restrict__ tiles, uint32_t* amax) {
@@ -513,11 +515,12 @@ __global__ void __launch_bounds__(kQuantThreads) requant_fp8_amax_kernel(const R
   });
 }
 
+template <bool kUe8m0>
 __global__ void __launch_bounds__(kQuantThreads) requant_fp8_quant_kernel(const RqTile* __restrict__ tiles,
                                                                        const uint32_t* __restrict__ amax) {
   const RqTile t = tiles[blockIdx.x];
   float dscale, scale_inv;
-  scales_of_amax(amax[t.group], &dscale, &scale_inv);
+  group_scales<kUe8m0>(amax[t.group], &dscale, &scale_inv);
   if (t.scale_inv && threadIdx.x == 0) *reinterpret_cast<float*>(t.scale_inv) = scale_inv;
   const char* src = reinterpret_cast<const char*>(t.src);
   const float scale0 = __ldg(reinterpret_cast<const float*>(t.scale));
@@ -550,15 +553,16 @@ int requant_fp8_plan(int device, const tsb_rect_t* rects, uint64_t n, const tsb_
   const size_t pieces = q->add(tb.pieces), tiles = q->add(tb.tiles), amax = q->seal(tb.n_groups);
   q->describe(n, static_cast<uint32_t>(tb.units.size() + tb.tiles.size()), tb.stage_bytes, tb);
   q->launch = [pieces, tiles, amax, n_units = static_cast<uint32_t>(tb.units.size()), n_tiles = static_cast<uint32_t>(tb.tiles.size()),
-               n_groups = tb.n_groups, stage_bytes = tb.stage_bytes](char* d, cudaStream_t s) -> int {
+               n_groups = tb.n_groups, stage_bytes = tb.stage_bytes, ue8m0 = q->ue8m0](char* d, cudaStream_t s) -> int {
     if (n_units) {
-      requant_fp8_staged_kernel<<<n_units, kQuantThreads, stage_bytes, s>>>(reinterpret_cast<const RqUnit*>(d),
-                                                                         reinterpret_cast<const RqPiece*>(d + pieces));
+      const auto staged = ue8m0 ? requant_fp8_staged_kernel<true> : requant_fp8_staged_kernel<false>;
+      staged<<<n_units, kQuantThreads, stage_bytes, s>>>(reinterpret_cast<const RqUnit*>(d), reinterpret_cast<const RqPiece*>(d + pieces));
       if (int st = launched("requant_fp8_staged_kernel launch")) return st;
     }
     if (!n_tiles) return TSB_OK;
-    return launch_two_pass(requant_fp8_amax_kernel, requant_fp8_quant_kernel, "requant_fp8", reinterpret_cast<const RqTile*>(d + tiles),
-                           n_tiles, reinterpret_cast<uint32_t*>(d + amax), n_groups, s);
+    return launch_two_pass(requant_fp8_amax_kernel, ue8m0 ? requant_fp8_quant_kernel<true> : requant_fp8_quant_kernel<false>,
+                           "requant_fp8", reinterpret_cast<const RqTile*>(d + tiles), n_tiles, reinterpret_cast<uint32_t*>(d + amax),
+                           n_groups, s);
   };
   return TSB_OK;
 }
@@ -572,7 +576,7 @@ using namespace tsb;
 extern "C" int tsb_requant_fp8_plan_create(int device, const tsb_rect_t* rects, uint64_t n, const tsb_dq_source_t* sources,
                                            uint64_t n_sources, const tsb_sq_target_t* targets, uint64_t n_targets, uint32_t flags,
                                            tsb_plan_t* out) {
-  return quant_plan_create("tsb_requant_fp8_plan_create", device, flags, out, [&](QuantPlan* q) {
+  return quant_plan_create("tsb_requant_fp8_plan_create", device, flags, TSB_QUANT_UE8M0, out, [&](QuantPlan* q) {
     return requant_fp8_plan(device, rects, n, sources, n_sources, targets, n_targets, q);
   });
 }
@@ -583,7 +587,7 @@ extern "C" int tsb_requant_fp8_compile_host(int device, const tsb_rect_t* rects,
                                             void* out_pieces, uint64_t piece_cap, uint64_t* out_n_pieces, void* out_tiles,
                                             uint64_t tile_cap, uint64_t* out_n_tiles, uint64_t* out_n_groups) {
   return quant_compile_host(
-      "tsb_requant_fp8_compile_host", flags,
+      "tsb_requant_fp8_compile_host", flags, TSB_QUANT_UE8M0,
       [&](QuantPlan* q) { return requant_fp8_plan(device, rects, n, sources, n_sources, targets, n_targets, q); },
       {{out_units, unit_cap, out_n_units, "out_units"}, {out_pieces, piece_cap, out_n_pieces, "out_pieces"},
        {out_tiles, tile_cap, out_n_tiles, "out_tiles"}},

@@ -261,7 +261,7 @@ __device__ __forceinline__ void stage_band(const SqBand& band, const SqPiece* __
   }
 }
 
-template <uint32_t DT>
+template <uint32_t DT, bool kUe8m0>
 __device__ __forceinline__ void run_band(const SqBand& band, const SqPiece* pieces, unsigned char* smem, uint32_t* s_amax,
                                          float* s_scale) {
   constexpr uint32_t es = Src<DT>::kBytes;
@@ -272,7 +272,7 @@ __device__ __forceinline__ void run_band(const SqBand& band, const SqPiece* piec
   __syncthreads();
   for (uint32_t r = threadIdx.x; r < band.rows; r += kQuantThreads) {
     float scale, scale_inv;
-    scales_of_amax(s_amax[r], &scale, &scale_inv);
+    group_scales<kUe8m0>(s_amax[r], &scale, &scale_inv);
     s_scale[r] = scale;
     reinterpret_cast<float*>(band.scale)[r] = scale_inv;
   }
@@ -289,6 +289,8 @@ __device__ __forceinline__ void run_band(const SqBand& band, const SqPiece* piec
   }
 }
 
+// kUe8m0 (here and in scaled_fp8_quant_kernel): power-of-two scales (TSB_QUANT_UE8M0)
+template <bool kUe8m0>
 __global__ void __launch_bounds__(kQuantThreads, 5) scaled_fp8_rows_kernel(const SqBand* __restrict__ bands,
                                                                        const SqPiece* __restrict__ pieces) {
   extern __shared__ __align__(16) unsigned char stage[];
@@ -296,9 +298,9 @@ __global__ void __launch_bounds__(kQuantThreads, 5) scaled_fp8_rows_kernel(const
   __shared__ float s_scale[kSqBandRows];
   const SqBand band = bands[blockIdx.x];
   switch (band.src_dtype) {
-    case TSB_BF16: run_band<TSB_BF16>(band, pieces, stage, s_amax, s_scale); break;
-    case TSB_F16: run_band<TSB_F16>(band, pieces, stage, s_amax, s_scale); break;
-    default: run_band<TSB_F32>(band, pieces, stage, s_amax, s_scale); break;
+    case TSB_BF16: run_band<TSB_BF16, kUe8m0>(band, pieces, stage, s_amax, s_scale); break;
+    case TSB_F16: run_band<TSB_F16, kUe8m0>(band, pieces, stage, s_amax, s_scale); break;
+    default: run_band<TSB_F32, kUe8m0>(band, pieces, stage, s_amax, s_scale); break;
   }
 }
 
@@ -373,11 +375,12 @@ __device__ __forceinline__ void quantise_tile(const SqTile& t, float scale) {
   }
 }
 
+template <bool kUe8m0>
 __global__ void __launch_bounds__(kQuantThreads) scaled_fp8_quant_kernel(const SqTile* __restrict__ tiles,
                                                                     const uint32_t* __restrict__ amax) {
   const SqTile t = tiles[blockIdx.x];
   float scale, scale_inv;
-  scales_of_amax(amax[t.group], &scale, &scale_inv);
+  group_scales<kUe8m0>(amax[t.group], &scale, &scale_inv);
   if (t.scale && threadIdx.x == 0) *reinterpret_cast<float*>(t.scale) = scale_inv;
   switch (t.src_dtype) {
     case TSB_BF16: quantise_tile<TSB_BF16>(t, scale); break;
@@ -390,12 +393,13 @@ __global__ void __launch_bounds__(kQuantThreads) scaled_fp8_quant_kernel(const S
 
 int launch_scaled_fp8(const SqLaunch& l, cudaStream_t stream) {
   if (l.n_bands) {
-    scaled_fp8_rows_kernel<<<l.n_bands, kQuantThreads, l.stage_bytes, stream>>>(l.bands, l.pieces);
+    const auto rows_kernel = l.ue8m0 ? scaled_fp8_rows_kernel<true> : scaled_fp8_rows_kernel<false>;
+    rows_kernel<<<l.n_bands, kQuantThreads, l.stage_bytes, stream>>>(l.bands, l.pieces);
     if (int st = launched("scaled_fp8_rows_kernel launch")) return st;
   }
   if (!l.n_tiles) return TSB_OK;
-  return launch_two_pass(scaled_fp8_amax_kernel, scaled_fp8_quant_kernel, "scaled_fp8", l.tiles, l.n_tiles, l.amax, l.n_groups,
-                         stream);
+  return launch_two_pass(scaled_fp8_amax_kernel, l.ue8m0 ? scaled_fp8_quant_kernel<true> : scaled_fp8_quant_kernel<false>,
+                         "scaled_fp8", l.tiles, l.n_tiles, l.amax, l.n_groups, stream);
 }
 
 namespace {
@@ -410,7 +414,7 @@ int scaled_fp8_plan(int device, const tsb_rect_t* rects, uint64_t n, const tsb_s
   const size_t pieces = q->add(tb.pieces), tiles = q->add(tb.tiles), amax = q->seal(tb.n_groups);
   q->describe(n, static_cast<uint32_t>(tb.bands.size() + tb.tiles.size()), kSqStageBytes, tb);
   const SqLaunch l{nullptr, nullptr, nullptr, nullptr, static_cast<uint32_t>(tb.bands.size()), static_cast<uint32_t>(tb.tiles.size()),
-                   tb.n_groups, tb.stage_bytes};
+                   tb.n_groups, tb.stage_bytes, q->ue8m0};
   q->launch = [l, pieces, tiles, amax](char* d, cudaStream_t s) {
     SqLaunch x = l;
     x.bands = reinterpret_cast<const SqBand*>(d);
@@ -430,7 +434,7 @@ using namespace tsb;
 
 extern "C" int tsb_scaled_fp8_plan_create(int device, const tsb_rect_t* rects, uint64_t n, const tsb_sq_target_t* targets,
                                           uint64_t n_targets, uint32_t flags, tsb_plan_t* out) {
-  return quant_plan_create("tsb_scaled_fp8_plan_create", device, flags, out,
+  return quant_plan_create("tsb_scaled_fp8_plan_create", device, flags, TSB_QUANT_UE8M0, out,
                            [&](QuantPlan* q) { return scaled_fp8_plan(device, rects, n, targets, n_targets, q); });
 }
 
@@ -438,7 +442,7 @@ extern "C" int tsb_scaled_fp8_compile_host(int device, const tsb_rect_t* rects, 
                                            uint64_t n_targets, uint32_t flags, void* out_bands, uint64_t band_cap,
                                            uint64_t* out_n_bands, void* out_pieces, uint64_t piece_cap, uint64_t* out_n_pieces,
                                            void* out_tiles, uint64_t tile_cap, uint64_t* out_n_tiles, uint64_t* out_n_groups) {
-  return quant_compile_host("tsb_scaled_fp8_compile_host", flags,
+  return quant_compile_host("tsb_scaled_fp8_compile_host", flags, TSB_QUANT_UE8M0,
                             [&](QuantPlan* q) { return scaled_fp8_plan(device, rects, n, targets, n_targets, q); },
                             {{out_bands, band_cap, out_n_bands, "out_bands"}, {out_pieces, piece_cap, out_n_pieces, "out_pieces"},
                              {out_tiles, tile_cap, out_n_tiles, "out_tiles"}},

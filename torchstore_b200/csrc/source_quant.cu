@@ -183,7 +183,8 @@ __device__ __forceinline__ void widen_chunk(const uint32_t d[4 * Src<DT>::kBytes
   }
 }
 
-template <uint32_t DT>
+// kUe8m0: power-of-two scales (TSB_QUANT_UE8M0)
+template <uint32_t DT, bool kUe8m0>
 __global__ void __launch_bounds__(kQuantThreads) source_quant_kernel(const SrcQUnit* __restrict__ units) {
   constexpr uint32_t es = Src<DT>::kBytes;
   __shared__ uint32_t s_amax[kSqBandRows];
@@ -237,7 +238,7 @@ __global__ void __launch_bounds__(kQuantThreads) source_quant_kernel(const SrcQU
   __syncthreads();
   for (uint32_t g = threadIdx.x; g < ng; g += kQuantThreads) {
     float scale, scale_inv;
-    scales_of_amax(s_amax[g], &scale, &scale_inv);
+    group_scales<kUe8m0>(s_amax[g], &scale, &scale_inv);
     s_scale[g] = scale;
     reinterpret_cast<float*>(u.scale_inv)[g] = scale_inv;
   }
@@ -264,15 +265,19 @@ int source_quant_plan(const tsb_source_quant_target_t* targets, uint64_t n, Quan
   q->add(tb.units);
   const size_t tiles = q->add(tb.tiles), amax = q->seal(tb.n_groups);
   q->describe(n, static_cast<uint32_t>(tb.units.size() + tb.tiles.size()), tb.unit_bytes, tb);
-  const SqLaunch two_pass{nullptr, nullptr, nullptr, nullptr, 0, static_cast<uint32_t>(tb.tiles.size()), tb.n_groups, 0};
-  q->launch = [two_pass, tiles, amax, n_units = std::array<uint32_t, 3>{tb.n_units[0], tb.n_units[1], tb.n_units[2]}](char* d, cudaStream_t s) -> int {
+  const SqLaunch two_pass{nullptr, nullptr, nullptr, nullptr, 0, static_cast<uint32_t>(tb.tiles.size()), tb.n_groups, 0, q->ue8m0};
+  // the unit kernels by rank (bf16, f16, f32) and scale format
+  using Kernel = void (*)(const SrcQUnit*);
+  const std::array<Kernel, 3> kernels =
+      q->ue8m0 ? std::array<Kernel, 3>{source_quant_kernel<TSB_BF16, true>, source_quant_kernel<TSB_F16, true>, source_quant_kernel<TSB_F32, true>}
+               : std::array<Kernel, 3>{source_quant_kernel<TSB_BF16, false>, source_quant_kernel<TSB_F16, false>,
+                                       source_quant_kernel<TSB_F32, false>};
+  q->launch = [two_pass, tiles, amax, kernels, n_units = std::array<uint32_t, 3>{tb.n_units[0], tb.n_units[1], tb.n_units[2]}](char* d, cudaStream_t s) -> int {
     const SrcQUnit* units = reinterpret_cast<const SrcQUnit*>(d);
     for (int k = 0; k < 3; ++k) {
       const uint32_t n = n_units[k];
       if (!n) continue;
-      if (k == 0) source_quant_kernel<TSB_BF16><<<n, kQuantThreads, 0, s>>>(units);
-      if (k == 1) source_quant_kernel<TSB_F16><<<n, kQuantThreads, 0, s>>>(units);
-      if (k == 2) source_quant_kernel<TSB_F32><<<n, kQuantThreads, 0, s>>>(units);
+      kernels[k]<<<n, kQuantThreads, 0, s>>>(units);
       if (int st = launched("source_quant_kernel launch")) return st;
       units += n;
     }
@@ -293,7 +298,7 @@ using namespace tsb;
 
 extern "C" int tsb_source_quant_plan_create(int device, const tsb_source_quant_target_t* targets, uint64_t n, uint32_t flags,
                                             tsb_plan_t* out) {
-  return quant_plan_create("tsb_source_quant_plan_create", device, flags, out,
+  return quant_plan_create("tsb_source_quant_plan_create", device, flags, TSB_QUANT_UE8M0, out,
                            [&](QuantPlan* q) { return source_quant_plan(targets, n, q); });
 }
 
@@ -301,7 +306,7 @@ extern "C" int tsb_source_quant_compile_host(int device, const tsb_source_quant_
                                              void* out_units, uint64_t unit_cap, uint64_t* out_n_units, void* out_tiles,
                                              uint64_t tile_cap, uint64_t* out_n_tiles, uint64_t* out_n_groups) {
   (void)device;
-  return quant_compile_host("tsb_source_quant_compile_host", flags, [&](QuantPlan* q) { return source_quant_plan(targets, n, q); },
+  return quant_compile_host("tsb_source_quant_compile_host", flags, TSB_QUANT_UE8M0, [&](QuantPlan* q) { return source_quant_plan(targets, n, q); },
                             {{out_units, unit_cap, out_n_units, "out_units"}, {out_tiles, tile_cap, out_n_tiles, "out_tiles"}},
                             out_n_groups);
 }

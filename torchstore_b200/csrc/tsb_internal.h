@@ -249,6 +249,7 @@ struct QuantPlan {
   std::vector<char> tables;       // every table back to back, then the zeroed amax words
   std::vector<Section> sections;  // the tables, in the order of the kind's tsb_*_compile_host outputs
   uint32_t n_groups = 0;          // amax words
+  bool ue8m0 = false;             // TSB_QUANT_UE8M0: the launch runs the power-of-two scale kernels (tables unchanged)
   tsb_plan_info_t info{};
   std::function<int(char* d, cudaStream_t)> launch;  // runs the plan from its tables' device copy at d
 
@@ -281,16 +282,18 @@ struct QuantPlan {
   }
 };
 using QuantCompile = std::function<int(QuantPlan*)>;
-// The bodies of tsb_*_plan_create and tsb_*_compile_host (plan.cu): `fn` names the entry in its argument errors.
-int quant_plan_create(const char* fn, int device, uint32_t flags, tsb_plan_t* out, const QuantCompile& compile);
+// The bodies of tsb_*_plan_create and tsb_*_compile_host (plan.cu): `fn` names the entry in its argument errors,
+// `accepted` the TSB_QUANT_* bits the kind takes in `flags` (any other bit is TSB_ERR_INVALID); compile() sees
+// them in QuantPlan::ue8m0.
+int quant_plan_create(const char* fn, int device, uint32_t flags, uint32_t accepted, tsb_plan_t* out, const QuantCompile& compile);
 struct TableOut {
   void* out;          // NULL: not wanted
   uint64_t cap;       // records out can take
   uint64_t* n;        // the table's record count (if not NULL)
   const char* name;   // the argument, for TSB_ERR_NOMEM
 };
-int quant_compile_host(const char* fn, uint32_t flags, const QuantCompile& compile, std::initializer_list<TableOut> outs,
-                       uint64_t* out_n_groups);
+int quant_compile_host(const char* fn, uint32_t flags, uint32_t accepted, const QuantCompile& compile,
+                       std::initializer_list<TableOut> outs, uint64_t* out_n_groups);
 
 // After a kernel launch: its launch error, or count it.
 inline int launched(const char* what) {
@@ -418,6 +421,7 @@ struct SqLaunch {
   const SqTile* tiles;
   uint32_t* amax;  // n_groups words, cleared by the launch
   uint32_t n_bands, n_tiles, n_groups, stage_bytes;
+  bool ue8m0;      // power-of-two scales (QuantPlan::ue8m0)
 };
 int launch_scaled_fp8(const SqLaunch& l, cudaStream_t stream);
 

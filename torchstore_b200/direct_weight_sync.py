@@ -54,6 +54,14 @@ SCALE_KINDS = {
 }
 _GRANULARITY = {"channel_scales": _native.TSB_SCALE_PER_CHANNEL, "tensor_scales": _native.TSB_SCALE_PER_TENSOR}
 _REQUANT_KEY = ("", "requantize")  # in the scale key set of a pull with requantize=True
+SCALE_FORMATS = (None, "ue8m0")  # scale_fmt of the quantising routes: float32 amax / 448, or its power of two up
+
+
+def scale_fmt_flags(scale_fmt: str | None) -> int:
+    """The native quantising plans' ``flags`` for ``scale_fmt`` (ValueError for an unknown format)."""
+    if scale_fmt is not None and (not isinstance(scale_fmt, str) or scale_fmt not in SCALE_FORMATS):
+        raise ValueError(f"scale_fmt must be None or 'ue8m0', not {scale_fmt!r}")
+    return _native.TSB_QUANT_UE8M0 if scale_fmt == "ue8m0" else 0
 
 
 # ---------------------------------------------------------------------------------------------
@@ -249,7 +257,8 @@ class DirectWeightSyncSource:
                  block_scales: dict[str, torch.Tensor] | None = None,
                  channel_scales: dict[str, torch.Tensor] | None = None,
                  tensor_scales: dict[str, torch.Tensor] | None = None,
-                 quantize: dict[str, str] | None = None) -> dict[str, RDMAWeightHandle]:
+                 quantize: dict[str, str] | None = None,
+                 scale_fmt: str | None = None) -> dict[str, RDMAWeightHandle]:
         """Create a handle for every entry of ``state_dict`` (tensors or DTensors).
 
         ``tensor_slices`` (extension) gives the global rectangle of *plain* local shards for
@@ -269,9 +278,14 @@ class DirectWeightSyncSource:
         global 128x128 block inside the shard, per channel the shard's part of a row, per tensor the shard's
         [rows, cols] matrix.  Each group gets the quantising formula of DESIGN.md section 4.  ``refresh()``
         requantises the staging from the live weights; ``transfer_dtype`` does not apply to these names.
+        ``scale_fmt="ue8m0"`` rounds every such scale up to a power of two (DESIGN.md section 4, "UE8M0 scales");
+        the scales stay float32, so every consumer of scaled handles reads them unchanged.
 
         Everything is validated before anything is exported, so a failed call registers nothing."""
         scale_dicts = {"block_scales": block_scales, "channel_scales": channel_scales, "tensor_scales": tensor_scales}
+        quant_flags = scale_fmt_flags(scale_fmt)
+        if scale_fmt is not None and not quantize:
+            raise ValueError("scale_fmt applies to source-side quantisation: it needs quantize")
         quantize = self._check_quantize(state_dict, tensor_slices, quantize or {}, scale_dicts)
         scaled = self._check_source_scales(state_dict, transfer_dtype, tensor_slices, scale_dicts)
         handles: dict[str, RDMAWeightHandle] = {}
@@ -328,7 +342,7 @@ class DirectWeightSyncSource:
             if casts:
                 self._refresh_plans = Plans.build(casts)
             if quant_targets:
-                self._quant_plans = Plans.build_source_quant(quant_targets)
+                self._quant_plans = Plans.build_source_quant(quant_targets, quant_flags)
             self.refresh()
         else:
             # make sure the weights the handles point at are materialised before anyone reads them
@@ -665,7 +679,9 @@ class DirectWeightSyncDest:
             out.add(name)
         return out
 
-    def _compile(self, scaled: dict | None = None, dequant: set | None = None, requant: set | None = None) -> None:
+    def _compile(self, scaled: dict | None = None, dequant: set | None = None, requant: set | None = None,
+                 flags: int = 0) -> None:
+        """Compile the cached transfer plan; ``flags`` go to the quantising and requantising plans."""
         per_device: dict[int, list] = defaultdict(list)
         quant_pairs: dict[tuple, list] = defaultdict(list)  # (device, block?) -> windows of the quantising plans
         dq: dict[int, tuple[list, dict]] = {}  # device -> (windows, {source buffer id: (name, DqSource)})
@@ -713,7 +729,7 @@ class DirectWeightSyncDest:
                     code = _native.TSB_SCALE_PER_BLOCK if kw == "block_scales" else _GRANULARITY[kw]
                     targets.append(_native.SqTarget(d.data_ptr(), s.data_ptr(), d.numel() // (rows * cols), rows, cols, code, 0))
                 pairs, sources = rq.get(dev, ([], {}))
-                _build_named(self._requant_plans, Plans.build_requant_fp8,
+                _build_named(self._requant_plans, lambda per_device: Plans.build_requant_fp8(per_device, flags),
                              {dev: (pairs, [s for _, s in sources.values()], targets)},
                              {"target": names, "source": [n for n, _ in sources.values()]},
                              lambda n: f"requantising pull of '{n}' ({scaled[n][0]})")
@@ -733,7 +749,8 @@ class DirectWeightSyncDest:
                                                             _GRANULARITY[kw], 0))
                     plans, build = (self._block_plans, Plans.build_block_fp8) if block else \
                         (self._scaled_plans, Plans.build_scaled_fp8)
-                    _build_named(plans, build, {dev: (quant_pairs.get((dev, block), []), targets)}, {"target": names},
+                    _build_named(plans, lambda per_device, build=build: build(per_device, flags),
+                                 {dev: (quant_pairs.get((dev, block), []), targets)}, {"target": names},
                                  lambda n: f"{SCALE_KINDS[scaled[n][0]][1]} pull of '{n}' ({scaled[n][0]})")
         except BaseException:
             for plans in self._fp8_plans:
@@ -755,7 +772,8 @@ class DirectWeightSyncDest:
                    dest_slices: dict[str, TensorSlice] | None = None, *,
                    block_scales: dict[str, torch.Tensor] | None = None,
                    channel_scales: dict[str, torch.Tensor] | None = None,
-                   tensor_scales: dict[str, torch.Tensor] | None = None, requantize: bool = False) -> None:
+                   tensor_scales: dict[str, torch.Tensor] | None = None, requantize: bool = False,
+                   scale_fmt: str | None = None) -> None:
         """Pull every overlapping region into ``dest_state_dict`` (in place).  Returns when the
         bytes are in destination HBM (so the caller may tell the source it is done reading).
 
@@ -784,15 +802,27 @@ class DirectWeightSyncDest:
         destination's formula: the result equals a dequantising pull into a float32 temporary followed by a
         quantising pull from it, byte for byte.  This re-rounds, so it is refused (TypeError) by default.
 
+        Power-of-two scales (extension, ``scale_fmt="ue8m0"``): every name of the three scale dicts, quantised or
+        requantised, gets its float32 ``amax_c / 448`` rounded up to a power of two (DESIGN.md section 4, "UE8M0
+        scales"), the scales of DeepSeek-V3.1 checkpoints (``"scale_fmt": "ue8m0"``) and of FP8 recipes that round
+        scales to powers of two.  ``None`` keeps the plain float32 formula.  ValueError for another value, or for a
+        ``scale_fmt`` without a name in the scale dicts.  Changing it rebuilds the plan.
+
         Steady state costs one native call to launch and a poll loop: the cached plan is checked
         against the destination OBJECTS first (their ids; the plan keeps them alive), the kernel
         is enqueued, and the data-pointer signature -- which catches ``param.data = new`` under an
         unchanged object -- is recomputed while the kernel runs."""
         scales = (block_scales, channel_scales, tensor_scales)
         names = {n for d in scales for n in (d or ())}
+        flags = scale_fmt_flags(scale_fmt)
+        if scale_fmt is not None and not names:
+            raise ValueError("scale_fmt applies to quantised and requantised names: block_scales, channel_scales or "
+                             "tensor_scales must name at least one")
         keys = frozenset((n, kw) for kw, d in zip(SCALE_KINDS, scales) for n in (d or ()))
         if requantize:
             keys |= {_REQUANT_KEY}
+        if scale_fmt is not None:
+            keys |= {("", f"scale_fmt={scale_fmt}")}
         if self._plan is not None and keys != self._scale_keys:
             logger.info("scaled names or their granularity changed; rebuilding the transfer plan")
             self.close()
@@ -827,7 +857,7 @@ class DirectWeightSyncDest:
             requant = {n for n in scaled or () if getattr(all_handles[n][0].rdma_buffer, "granularity", None)}
             self._plan = self._build_plan(all_handles, dest_state_dict, dest_slices)
             try:
-                self._compile(scaled, dequant, requant)
+                self._compile(scaled, dequant, requant, flags)
             except BaseException:
                 self._plan = None
                 raise
@@ -844,7 +874,8 @@ class DirectWeightSyncDest:
             logger.info("destination storage changed under the same tensors; rebuilding the transfer plan")
             self.close()
             await self.pull(all_handles, dest_state_dict, dest_slices, block_scales=block_scales,
-                            channel_scales=channel_scales, tensor_scales=tensor_scales, requantize=requantize)
+                            channel_scales=channel_scales, tensor_scales=tensor_scales, requantize=requantize,
+                            scale_fmt=scale_fmt)
 
     def launch(self) -> None:
         """Enqueue the cached plan on each device's copy stream, fenced against the caller's current

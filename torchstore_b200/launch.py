@@ -92,33 +92,35 @@ class Plans(dict):
         return plans
 
     @classmethod
-    def build_fp8(cls, create, per_device: dict[int, tuple]) -> "Plans":
-        """Compile scaled fp8 plans: ``create(device, *args)`` for each ``{device: args}``, ``create`` being one of
-        the ``_native.*_plan_create`` calls."""
+    def build_fp8(cls, create, per_device: dict[int, tuple], flags: int = 0) -> "Plans":
+        """Compile scaled fp8 plans: ``create(device, *args, flags=flags)`` for each ``{device: args}``, ``create``
+        being one of the ``_native.*_plan_create`` calls (``flags``: ``_native.TSB_QUANT_UE8M0`` or 0)."""
         plans = cls()
         try:
             for dev, args in per_device.items():
-                plans[dev] = create(dev, *args)
+                plans[dev] = create(dev, *args, flags=flags)
         except BaseException:
             plans.close()
             raise
         return plans
 
     @classmethod
-    def _build_pulls(cls, create, per_device: dict[int, tuple]) -> "Plans":
+    def _build_pulls(cls, create, per_device: dict[int, tuple], flags: int = 0) -> "Plans":
         """build_fp8 of pulls: ``{device: ([(src, dst) StridedMem windows], *tables)}``, the windows as rects."""
-        return cls.build_fp8(create, {dev: (*build_rects(pairs), *tables) for dev, (pairs, *tables) in per_device.items()})
+        return cls.build_fp8(create, {dev: (*build_rects(pairs), *tables) for dev, (pairs, *tables) in per_device.items()},
+                             flags)
 
     @classmethod
-    def build_block_fp8(cls, per_device: dict[int, tuple[list, list]]) -> "Plans":
-        """Compile block-scaled fp8 pulls: ``{device: ([(src, dst) StridedMem windows], [BqTarget])}``."""
-        return cls._build_pulls(_native.block_fp8_plan_create, per_device)
+    def build_block_fp8(cls, per_device: dict[int, tuple[list, list]], flags: int = 0) -> "Plans":
+        """Compile block-scaled fp8 pulls: ``{device: ([(src, dst) StridedMem windows], [BqTarget])}``; ``flags``:
+        ``_native.TSB_QUANT_UE8M0`` for power-of-two scales, here and in the other quantising builders."""
+        return cls._build_pulls(_native.block_fp8_plan_create, per_device, flags)
 
     @classmethod
-    def build_scaled_fp8(cls, per_device: dict[int, tuple[list, list]]) -> "Plans":
+    def build_scaled_fp8(cls, per_device: dict[int, tuple[list, list]], flags: int = 0) -> "Plans":
         """Compile per-channel / per-tensor scaled fp8 pulls: ``{device: ([(src, dst) StridedMem windows],
         [SqTarget])}``."""
-        return cls._build_pulls(_native.scaled_fp8_plan_create, per_device)
+        return cls._build_pulls(_native.scaled_fp8_plan_create, per_device, flags)
 
     @classmethod
     def build_dequant_fp8(cls, per_device: dict[int, tuple[list, list]]) -> "Plans":
@@ -127,15 +129,16 @@ class Plans(dict):
         return cls._build_pulls(_native.dequant_fp8_plan_create, per_device)
 
     @classmethod
-    def build_requant_fp8(cls, per_device: dict[int, tuple[list, list, list]]) -> "Plans":
+    def build_requant_fp8(cls, per_device: dict[int, tuple[list, list, list]], flags: int = 0) -> "Plans":
         """Compile requantising pulls of scaled fp8 sources into scaled fp8 destinations: ``{device:
         ([(src, dst) StridedMem windows], [DqSource], [SqTarget])}``."""
-        return cls._build_pulls(_native.requant_fp8_plan_create, per_device)
+        return cls._build_pulls(_native.requant_fp8_plan_create, per_device, flags)
 
     @classmethod
-    def build_source_quant(cls, per_device: dict[int, list]) -> "Plans":
+    def build_source_quant(cls, per_device: dict[int, list], flags: int = 0) -> "Plans":
         """Compile source-side quantisations: ``{device: [SourceQuantTarget]}``."""
-        return cls.build_fp8(_native.source_quant_plan_create, {dev: (targets,) for dev, targets in per_device.items()})
+        return cls.build_fp8(_native.source_quant_plan_create, {dev: (targets,) for dev, targets in per_device.items()},
+                             flags)
 
     def launch(self, fence_out: bool = True) -> None:
         """Enqueue every plan on its device's copy stream, fenced in against the caller's current

@@ -59,7 +59,7 @@ def reset_direct_cache(store=None) -> None:
 
 async def put_state_dict(store, state_dict, key, direct_rdma=False, transfer_dtype=None, block_scales: dict | None = None,
                          channel_scales: dict | None = None, tensor_scales: dict | None = None,
-                         quantize: dict | None = None):
+                         quantize: dict | None = None, scale_fmt: str | None = None):
     """Store every leaf of ``state_dict`` (one batched put), then the mapping as the commit marker.
 
     With ``direct_rdma=True`` only handles to the caller's HBM are published on the first call;
@@ -68,12 +68,14 @@ async def put_state_dict(store, state_dict, key, direct_rdma=False, transfer_dty
     only, first call) publish float8_e4m3fn weights with their scales, so that pulls into bf16/f16/f32
     destinations dequantise them (see ``DirectWeightSyncSource.register``).  ``quantize`` (direct mode only,
     first call) names bf16/f16/f32 weights published as block-, channel- or tensor-scaled fp8 staging that
-    later calls requantise from the live weights."""
+    later calls requantise from the live weights; ``scale_fmt="ue8m0"`` gives that staging power-of-two scales."""
     if direct_rdma:
         await _put_state_dict_direct_rdma(store, state_dict, key, transfer_dtype,
                                           dict(block_scales=block_scales, channel_scales=channel_scales,
-                                               tensor_scales=tensor_scales, quantize=quantize))
+                                               tensor_scales=tensor_scales, quantize=quantize, scale_fmt=scale_fmt))
         return
+    if scale_fmt is not None:
+        raise NotImplementedError("scale_fmt needs direct_rdma=True: the store path does not quantise")
     if quantize:
         raise NotImplementedError("quantize needs direct_rdma=True: the store path does not publish scaled fp8 staging")
     if block_scales or channel_scales or tensor_scales:
@@ -86,19 +88,21 @@ async def put_state_dict(store, state_dict, key, direct_rdma=False, transfer_dty
 
 async def get_state_dict(store, key, user_state_dict: dict | None = None, strict=True, direct_rdma=False,
                          block_scales: dict | None = None, channel_scales: dict | None = None,
-                         tensor_scales: dict | None = None, requantize: bool = False):
+                         tensor_scales: dict | None = None, requantize: bool = False, scale_fmt: str | None = None):
     """Fetch a state dict.  ``user_state_dict`` tensors are filled in place (and required in direct
     mode).  A missing mapping means no matching push finished: RuntimeError.  ``block_scales``
     (direct mode only) names float8_e4m3fn destinations quantised into the 128x128 block-scaled
     layout during the pull; ``channel_scales`` / ``tensor_scales`` likewise name destinations with one
     float32 scale per row / per matrix (see ``DirectWeightSyncDest.pull``).  ``requantize=True`` (direct
     mode only) lets such destinations be fed by scaled fp8 handles, re-rounding them into the destination's
-    layout."""
+    layout.  ``scale_fmt="ue8m0"`` (direct mode only) gives every such destination power-of-two scales."""
     if direct_rdma:
         assert user_state_dict is not None, "user_state_dict is required for direct_rdma mode"
         await _get_state_dict_direct_rdma(store, key, user_state_dict, block_scales, channel_scales, tensor_scales,
-                                          requantize)
+                                          requantize, scale_fmt)
         return user_state_dict
+    if scale_fmt is not None:
+        raise NotImplementedError("scale_fmt needs direct_rdma=True: the store path does not quantise")
     if requantize:
         raise NotImplementedError("requantize needs direct_rdma=True: the store path does not requantise scaled fp8")
     if block_scales:
@@ -196,7 +200,7 @@ def _try_all_gather(cache: _DirectRDMACache, key: str, user_state_dict, scaled=F
 
 
 async def _get_state_dict_direct_rdma(store, key, user_state_dict, block_scales=None, channel_scales=None,
-                                      tensor_scales=None, requantize=False):
+                                      tensor_scales=None, requantize=False, scale_fmt=None):
     from torchstore_b200.collectives import allgather_enabled
     from torchstore_b200.direct_weight_sync import DirectWeightSyncDest
 
@@ -221,4 +225,5 @@ async def _get_state_dict_direct_rdma(store, key, user_state_dict, block_scales=
                 all_handles[name].append(handle)
         cache.handles[key] = all_handles
     await cache.dests[key].pull(cache.handles[key], user_state_dict, block_scales=block_scales,
-                                channel_scales=channel_scales, tensor_scales=tensor_scales, requantize=requantize)
+                                channel_scales=channel_scales, tensor_scales=tensor_scales, requantize=requantize,
+                                scale_fmt=scale_fmt)
