@@ -293,3 +293,124 @@ def replay_requant(units: np.ndarray, pieces: np.ndarray, tiles: np.ndarray, n_g
     values = [x_of(int(t["src"]), int(t["src_stride"]), int(t["scale"]), int(t["scale_step"]), int(t["rows"]), int(t["cols"]))
               for t in tiles]
     _replay_tiles(tiles, values, n_groups, scale_fmt)
+
+
+# ---- inputs on the step's edges, power-of-two source scales and checks -----------------------------------------
+BRANCHES = ("keep", "up", "clamp")
+
+
+def branch_of_amax(amax: np.ndarray) -> np.ndarray:
+    """The branch of the step each finite amax takes: "clamp" below 1e-4 (zero and subnormal groups included),
+    "keep" where t = amax / 448 is a power of two, "up" elsewhere."""
+    amax = np.asarray(amax, dtype=np.float32)
+    with np.errstate(all="ignore"):
+        t = (np.maximum(amax, _CLAMP) / _FMAX).astype(np.float32)
+    keep = (t.view(np.uint32) & np.uint32(0x007FFFFF)) == 0
+    return np.where(amax < _CLAMP, "clamp", np.where(keep, "keep", "up"))
+
+
+def group_amax(x: np.ndarray, gid: np.ndarray, n_groups: int) -> np.ndarray:
+    """max |x| per group id (x float32, gid an int array of x's shape)."""
+    out = np.zeros(n_groups, dtype=np.float32)
+    np.maximum.at(out, gid.reshape(-1), np.abs(np.asarray(x, np.float32)).reshape(-1))
+    return out
+
+
+def group_ids(granularity: str, shape, row0: int = 0, col0: int = 0) -> tuple[np.ndarray, int]:
+    """(group id of every element of a ``shape`` shard at (row0, col0), number of groups): blocks anchored at the
+    global origin, rows, or matrices, numbered in row-major order."""
+    *lead, n, k = shape
+    m = int(np.prod(lead, dtype=np.int64))
+    mat = np.arange(m).reshape(tuple(lead) + (1, 1)) if lead else np.zeros((1, 1), dtype=np.int64)
+    if granularity == "tensor":
+        return np.broadcast_to(mat, tuple(shape)).copy(), m
+    if granularity == "channel":
+        return (mat * n + np.arange(n)[:, None] + 0 * np.arange(k)[None, :]).astype(np.int64), m * n
+    rows = (row0 + np.arange(n)) // 128 - row0 // 128
+    cols = (col0 + np.arange(k)) // 128 - col0 // 128
+    nr, nc = int(rows[-1]) + 1, int(cols[-1]) + 1
+    return (mat * nr * nc + rows[:, None] * nc + cols[None, :]).astype(np.int64), m * nr * nc
+
+
+def edge_amaxes_for(dtype: torch.dtype) -> np.ndarray:
+    """edge_amaxes() restricted to the finite values ``dtype`` holds exactly, plus that dtype's own neighbours of
+    448 * 2^k (one of its ulps above, and its largest value below 448 * 2^(k+1)) and its largest finite value."""
+    if dtype == torch.float32:
+        return edge_amaxes()
+    top = float(torch.finfo(dtype).max)
+    vals = [float(v) for v in edge_amaxes() if np.isfinite(v) and v <= top and float(torch.tensor(float(v)).to(dtype)) == float(v)]
+    for k in (-20, -8, -1, 0, 1, 7, 40, 100):
+        base = torch.tensor(448.0 * 2.0 ** k, dtype=dtype)
+        if not torch.isfinite(base) or float(base) != 448.0 * 2.0 ** k:
+            continue
+        up = torch.nextafter(base, torch.tensor(float("inf"), dtype=dtype))
+        down = torch.nextafter(2 * base, torch.tensor(0.0, dtype=dtype))
+        vals += [float(v) for v in (up, down) if torch.isfinite(v)]
+    vals.append(top)
+    return np.unique(np.array(vals, dtype=np.float32))
+
+
+def plant_edges(shape, dtype: torch.dtype, granularity: str, row0: int = 0, col0: int = 0, seed: int = 0):
+    """A ``dtype`` shard whose groups (as ``group_ids``) take the amaxes edge_amaxes_for(dtype) in turn, then one
+    all-zero (+-0) group and one all-subnormal group; later groups keep random finite data.  Each edge group holds
+    its amax once (+-) among values of at most half of it.  -> (x, branch of every group)."""
+    gid, n = group_ids(granularity, shape, row0, col0)
+    vals = list(edge_amaxes_for(dtype))
+    assert n >= len(vals) + 2, f"{n} groups for {len(vals) + 2} planted ones"
+    u = synth_f32(tuple(shape), seed, spread=0).numpy()
+    x = u * np.float32(4.0)
+    tiny = np.float32(torch.finfo(dtype).tiny)
+    first = {}
+    for i, g in enumerate(gid.reshape(-1)):
+        first.setdefault(int(g), i)
+    flat, uf, gf = x.reshape(-1), u.reshape(-1), gid.reshape(-1)
+    for j, v in enumerate(vals):
+        sel = gf == j
+        flat[sel] = uf[sel] * np.float32(0.5) * np.float32(v)
+        flat[first[j]] = -v if j % 2 else v
+    zero, sub = len(vals), len(vals) + 1
+    flat[gf == zero] = np.where(uf[gf == zero] < 0, np.float32(-0.0), np.float32(0.0))
+    flat[gf == sub] = uf[gf == sub] * tiny * np.float32(0.5)
+    out = torch.from_numpy(x).to(dtype)
+    amax = group_amax(widen(bits_of(out), str(dtype)[6:]), gid, n)
+    return out, branch_of_amax(amax)
+
+
+def plant_edge_sources(n_groups: int, group_shape, seed: int = 0) -> tuple[np.ndarray, np.ndarray]:
+    """fp8 source groups whose dequantised amax takes every value of edge_amaxes() in turn (the byte 1.0 once under
+    the scale v, the other bytes below 1.0), then an all-zero group and an all-subnormal one (scale 2^-140); later
+    groups are random under scale 2^-3.  -> (q uint8 [n_groups, *group_shape], scale float32 [n_groups])."""
+    vals = edge_amaxes()
+    assert n_groups >= vals.size + 2
+    rng = np.random.default_rng(seed)
+    q = rng.integers(0, 0x38, size=(n_groups,) + tuple(group_shape), dtype=np.uint8) | \
+        (rng.integers(0, 2, size=(n_groups,) + tuple(group_shape), dtype=np.uint8) << 7)
+    s = np.full(n_groups, 2.0 ** -3, dtype=np.float32)
+    first = (0,) * len(group_shape)
+    for j, v in enumerate(vals):
+        s[j] = v
+        q[(j,) + first] = 0xB8 if j % 2 else 0x38  # -+1.0
+    q[vals.size] = 0
+    s[vals.size] = 1.0
+    s[vals.size + 1] = np.float32(2.0 ** -140)
+    return q, s
+
+
+def pow2_scales(shape, seed: int, lo: int = -22, hi: int = 119) -> np.ndarray:
+    """float32 powers of two 2^k, k uniform in [lo, hi] (both ends present when there are two entries or more)."""
+    rng = np.random.default_rng(seed)
+    k = rng.integers(lo, hi + 1, size=int(np.prod(shape, dtype=np.int64)))
+    if k.size >= 2:
+        k[0], k[-1] = lo, hi
+    return np.ldexp(np.float32(1.0), k).astype(np.float32).reshape(shape)
+
+
+def assert_pow2_over(s: torch.Tensor, s_f32: torch.Tensor) -> None:
+    """Every finite UE8M0 scale_inv is a power of two, at least the float32 formula's scale_inv of the same group
+    and below twice it; the non-finite ones sit where the float32 formula's do."""
+    s, f = s.reshape(-1).float(), s_f32.reshape(-1).float()
+    fin = torch.isfinite(s)
+    assert torch.equal(fin, torch.isfinite(f)) and torch.equal(torch.isnan(s), torch.isnan(f))
+    assert ((s[fin].view(torch.int32) & 0x7FFFFF) == 0).all()
+    sd, fd = s[fin].double(), f[fin].double()
+    assert (sd >= fd).all() and (sd < 2 * fd).all()

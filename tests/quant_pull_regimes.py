@@ -213,11 +213,12 @@ class Geometry:
         return s.pull, tuple(int(o + i) for o, i in zip(s.off, local))
 
 
-def compile_tables(pulls, ops, handles, window_of, dests, scales) -> tuple[Tables, Geometry]:
+def compile_tables(pulls, ops, handles, window_of, dests, scales, flags: int = 0) -> tuple[Tables, Geometry]:
     """Compile on the host the quantising plans a pull of `pulls` (names w0, w1, ...) builds: the windows of
     `ops` (the planner's ops of the pull, the quantised names' ones used) with `window_of(buffer)` mapping a
     source buffer, and the targets of the fp8 destinations `dests` and their `scales`, in the order the pull
-    orders them (block, channel, tensor names).  -> (Tables, Geometry); keep `dests`, `scales` alive."""
+    orders them (block, channel, tensor names), with the plan `flags` (0 or _native.TSB_QUANT_UE8M0).  -> (Tables,
+    Geometry); keep `dests`, `scales` alive."""
     grans = {f"w{i}": p.g for i, p in enumerate(pulls)}
     order = sorted(grans, key=lambda n: GRANULARITIES.index(grans[n]))
     pairs = {True: [], False: []}
@@ -238,9 +239,9 @@ def compile_tables(pulls, ops, handles, window_of, dests, scales) -> tuple[Table
             arr[i] = _native.BqTarget(*args) if block else \
                 _native.SqTarget(*args, _native.TSB_SCALE_PER_CHANNEL if grans[n] == "channel" else _native.TSB_SCALE_PER_TENSOR, 0)
         if block:
-            tables.block = _native.block_fp8_compile_host(0, rects, nr, arr, len(names))
+            tables.block = _native.block_fp8_compile_host(0, rects, nr, arr, len(names), flags)
         else:
-            tables.scaled = _native.scaled_fp8_compile_host(0, rects, nr, arr, len(names))
+            tables.scaled = _native.scaled_fp8_compile_host(0, rects, nr, arr, len(names), flags)
     dgeom = []
     for n in order:
         d = dests[n]

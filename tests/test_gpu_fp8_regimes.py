@@ -120,21 +120,29 @@ def inputs(w: Workload, variant: str):
     return q, s
 
 
-@pytest.mark.parametrize("variant", ["finite", "poisoned_scale", "zero_group"])
+VARIANTS = ("finite", "poisoned_scale", "zero_group")
+
+
+@pytest.mark.parametrize("variant", VARIANTS)
 @pytest.mark.parametrize("regime", sorted(REGIMES))
 def test_regime_on_the_h100(regime, variant):
+    run_regime(regime, variant)
+
+
+def run_regime(regime, variant, scale_fmt=None):
+    """Pull the regime's workload in `variant` (requantising ones with the scale format `scale_fmt`) and check it."""
     r = REGIMES[regime]
     w = WORKLOADS[r.workload]
     q, s = inputs(w, variant)
     sources, handles = register(q, s, w.sg, list(w.src))
-    where = f"{regime} ({r.doc}), {variant}: {w.describe()}"
+    where = f"{regime} ({r.doc}), {variant}, scale_fmt={scale_fmt}: {w.describe()}"
     if w.kind == "requant":
-        sync, y, ys, bases = rq_gpu.pull_into(handles, w.shape, w.dst, w.out)
+        sync, y, ys, bases = rq_gpu.pull_into(handles, w.shape, w.dst, w.out, scale_fmt=scale_fmt)
         tables, geom = live_tables(sync, y, ys, w.out)
         assert r.holds(tables, geom), f"not reached: {where}"
         with named(where):
-            rq_gpu.assert_oracle(y, ys, q, s, w.sg, w.dst, w.out)
-            rq_gpu.assert_torch_cuda(y, ys, q, s, w.sg, w.dst, w.out)
+            rq_gpu.assert_oracle(y, ys, q, s, w.sg, w.dst, w.out, scale_fmt)
+            rq_gpu.assert_torch_cuda(y, ys, q, s, w.sg, w.dst, w.out, scale_fmt)
     else:
         sync, y, base = dq_gpu.pull_into(handles, w.shape, w.dst, DST[w.out])
         tables, geom = live_tables(sync, y)

@@ -22,7 +22,7 @@ import numpy as np
 import pytest
 import torch
 
-from oracle import block_fp8_oracle, scaled_fp8_oracle
+from oracle import block_fp8_oracle, scaled_fp8_oracle, ue8m0_oracle
 from oracle.block_fp8_oracle import synth_f32
 from tests import test_gpu_block_fp8 as bq_gpu
 from tests.fp8_regimes import split, whole
@@ -138,10 +138,11 @@ def inputs(name: str, variant: str):
 # ---- one pull of several names ----------------------------------------------------------------------
 class Pulled:
     """The names w0, w1, ... of `pulls` registered shard by shard (one source each), pulled into guarded fp8
-    destinations and scales by one DirectWeightSyncDest; `extra` handles and destinations join the pull."""
+    destinations and scales by one DirectWeightSyncDest with the scale format `scale_fmt`; `extra` handles and
+    destinations join the pull."""
 
-    def __init__(self, pulls, xs, extra_handles=None, extra_dests=None):
-        self.pulls, self.sources, self.shards = tuple(pulls), [], {}
+    def __init__(self, pulls, xs, extra_handles=None, extra_dests=None, scale_fmt=None):
+        self.pulls, self.sources, self.shards, self.scale_fmt = tuple(pulls), [], {}, scale_fmt
         self.handles, self.dests, self.scales, self.slices, self.bases = {}, {}, {}, {}, []
         try:
             for i, (p, x) in enumerate(zip(pulls, xs)):
@@ -169,7 +170,7 @@ class Pulled:
         self.sync = DirectWeightSyncDest()
 
     def pull(self):
-        run(self.sync.pull(self.all_handles, self.all_dests, self.slices, **self.by_kw))
+        run(self.sync.pull(self.all_handles, self.all_dests, self.slices, **self.by_kw, scale_fmt=self.scale_fmt))
 
     def plans(self):
         return dict(self.sync._block_plans), dict(self.sync._scaled_plans)
@@ -191,7 +192,7 @@ class Pulled:
         for i, (p, x) in enumerate(zip(self.pulls, xs)):
             n = f"w{i}"
             with named(f"w{i}: {p.describe()}"):
-                assert_quantised(self.dests[n], self.scales[n], region(x, *p.dst), p.g)
+                assert_quantised(self.dests[n], self.scales[n], region(x, *p.dst), p.g, self.scale_fmt)
         assert all(guards_intact(b) for b in self.bases)
 
     def update(self, xs):
@@ -209,16 +210,29 @@ class Pulled:
             run(src.cleanup())
 
 
-def assert_quantised(y, ys, x, g):
+def assert_quantised(y, ys, x, g, scale_fmt=None):
     """The fp8 weight y and its scale_inv ys against the numpy oracle of the source region x (bit-exact in
-    finite groups, NaN-agnostic in the others) and the torch CUDA composition (bit-exact, NaN bytes included)."""
-    want_q, want_s = oracle_quantize(x.float().numpy(), g)
+    finite groups, NaN-agnostic in the others) and the torch CUDA composition (bit-exact, NaN bytes included),
+    both in the scale format `scale_fmt`."""
+    if scale_fmt is None:
+        want_q, want_s = oracle_quantize(x.float().numpy(), g)
+    else:
+        want_q, want_s = ue8m0_oracle.quantize(x.float().numpy(), g, scale_fmt=scale_fmt)
     q, s = y.view(torch.uint8).cpu().numpy(), ys.cpu().numpy()
     if g == "block":
         assert_block_fp8_equal(q, s, want_q, want_s)
-        bq_gpu.assert_torch_cuda(y, ys, x)
     else:
         assert_scaled_fp8_equal(q, s, want_q, np.asarray(want_s, np.float32), g)
+    if scale_fmt is not None:
+        want_q, want_s = ue8m0_oracle.torch_quantize(x.to(DEV), g, scale_fmt=scale_fmt)
+        want_s = want_s.reshape(ys.shape)
+        assert torch.equal(y.view(torch.uint8), want_q.view(torch.uint8))  # NaN bytes included
+        nan = torch.isnan(want_s)
+        assert torch.equal(torch.isnan(ys), nan) and torch.equal(ys.view(torch.int32)[~nan], want_s.view(torch.int32)[~nan])
+        ue8m0_oracle.assert_pow2_over(ys, ue8m0_oracle.torch_quantize(x.to(DEV), g)[1])
+    elif g == "block":
+        bq_gpu.assert_torch_cuda(y, ys, x)
+    else:
         sq_gpu.assert_torch_cuda(y, ys, x, g)
 
 
@@ -229,11 +243,16 @@ VARIANTS = ("finite", "special", "near_top", "update")
 @pytest.mark.parametrize("variant", VARIANTS)
 @pytest.mark.parametrize("regime", sorted(REGIMES))
 def test_regime_on_the_h100(regime, variant):
+    run_regime(regime, variant)
+
+
+def run_regime(regime, variant, scale_fmt=None):
+    """Pull the regime's workload in `variant` with the scale format `scale_fmt`, and check it (module doc)."""
     r = REGIMES[regime]
     w = WORKLOADS[r.workload]
     xs = inputs(r.workload, variant)
-    where = f"{regime} ({r.doc}), {variant}: {w.describe()}"
-    pulled = Pulled(w.pulls, xs)
+    where = f"{regime} ({r.doc}), {variant}, scale_fmt={scale_fmt}: {w.describe()}"
+    pulled = Pulled(w.pulls, xs, scale_fmt=scale_fmt)
     try:
         pulled.pull()
         tables, geom = pulled.live_tables()

@@ -12,6 +12,7 @@ import pytest
 import torch
 
 import torchstore_b200 as ts
+from oracle import ue8m0_oracle
 from oracle.dequant_fp8_oracle import GRANULARITIES, SCALE_SET, scale_shape, torch_dequantize
 from oracle.requant_fp8_oracle import PAIRS, quantize, requantize, torch_requantize
 from tests.test_gpu_dequant_fp8 import KW, cleanup, guarded, guards_intact, register
@@ -35,31 +36,35 @@ def run(coro):
     return asyncio.run(coro)
 
 
-def pull_into(handles, full_shape, box, dg, sync=None, device=DEV):
-    """Requantising pull of `handles` into a guarded `dg`-scaled fp8 window `box` -> (sync, q, scale, guards)."""
+def pull_into(handles, full_shape, box, dg, sync=None, device=DEV, scale_fmt=None):
+    """Requantising pull of `handles` into a guarded `dg`-scaled fp8 window `box` in the scale format `scale_fmt`
+    -> (sync, q, scale, guards)."""
     off, loc = box
     qbase, q = guarded(loc, E4M3, device)
     sbase, s = guarded(dest_scale_shape(dg, loc), torch.float32, device)
     sync = sync or DirectWeightSyncDest()
     run(sync.pull({"w": handles}, {"w": q}, {"w": TensorSlice(off, (0,), tuple(full_shape), loc, (1,))},
-                  **{KW[dg]: {"w": s}}, requantize=True))
+                  **{KW[dg]: {"w": s}}, requantize=True, scale_fmt=scale_fmt))
     return sync, q, s, (qbase, sbase)
 
 
-def assert_torch_cuda(q, s, q_full, full_scale, sg, box, dg):
+def assert_torch_cuda(q, s, q_full, full_scale, sg, box, dg, scale_fmt=None):
     """Bit-exact, NaN bytes included, against the torch CUDA composition of the same window."""
-    want_q, want_s = torch_requantize(region(q_full, *box).to(DEV), local_scale(full_scale, sg, *box).to(DEV), sg,
-                                      box[0][-2], box[0][-1], dg)
+    args = (region(q_full, *box).to(DEV), local_scale(full_scale, sg, *box).to(DEV), sg, box[0][-2], box[0][-1], dg)
+    want_q, want_s = ue8m0_oracle.torch_requantize(*args, scale_fmt=scale_fmt) if scale_fmt else torch_requantize(*args)
+    if scale_fmt:
+        ue8m0_oracle.assert_pow2_over(s, torch_requantize(*args)[1])
     assert torch.equal(q.view(torch.uint8), want_q.view(torch.uint8))
     got_s, want_s = s.reshape(-1), want_s.reshape(-1)
     nan = torch.isnan(want_s)  # a NaN scale_inv's bits are torch's choice
     assert torch.equal(torch.isnan(got_s), nan) and torch.equal(got_s[~nan].view(torch.int32), want_s[~nan].view(torch.int32))
 
 
-def assert_oracle(q, s, q_full, full_scale, sg, box, dg):
+def assert_oracle(q, s, q_full, full_scale, sg, box, dg, scale_fmt=None):
     """Bit-exact against the numpy composition wherever it is not NaN."""
-    want_q, want_s = requantize(region(q_full, *box).view(torch.uint8).numpy(), local_scale(full_scale, sg, *box).numpy(),
-                                sg, box[0][-2], box[0][-1], dg)
+    args = (region(q_full, *box).view(torch.uint8).numpy(), local_scale(full_scale, sg, *box).numpy(), sg, box[0][-2],
+            box[0][-1], dg)
+    want_q, want_s = ue8m0_oracle.requantize(*args, scale_fmt=scale_fmt) if scale_fmt else requantize(*args)
     got_q = q.view(torch.uint8).cpu().numpy()
     nan = (want_q & 0x7F) == 0x7F
     assert np.array_equal(got_q[~nan], want_q[~nan])

@@ -10,7 +10,7 @@ import pytest
 import torch
 
 import torchstore_b200 as ts
-from oracle import block_fp8_oracle
+from oracle import block_fp8_oracle, ue8m0_oracle
 from oracle.source_quant_oracle import GRANULARITIES, bits_of, element_scales, quantize, synth_f32, torch_quantize, widen
 from tests.test_source_quant_cpu import CODE, DT
 from torchstore_b200 import _native
@@ -60,12 +60,17 @@ def staging(src: DirectWeightSyncSource, name="w"):
     return q, s
 
 
-def assert_exact(q: torch.Tensor, s: torch.Tensor, x: torch.Tensor, g: str, r0: int, c0: int):
-    """Bit-exact against torch CUDA everywhere (NaN bytes included) and against the numpy oracle on finite groups."""
-    tq, tsc = torch_quantize(x.to(q.device), g, r0, c0)
+def assert_exact(q: torch.Tensor, s: torch.Tensor, x: torch.Tensor, g: str, r0: int, c0: int, scale_fmt=None):
+    """Bit-exact against torch CUDA everywhere (NaN bytes included) and against the numpy oracle on finite groups,
+    both in the scale format `scale_fmt`."""
+    tq, tsc = ue8m0_oracle.torch_quantize(x.to(q.device), g, r0, c0, scale_fmt=scale_fmt)
     assert torch.equal(q.view(torch.uint8), tq.view(torch.uint8))
-    assert torch.equal(s.view(torch.int32), tsc.view(torch.int32))
-    want_q, want_s = quantize(widen(bits_of(x.cpu()), str(x.dtype)[6:]), g, r0, c0)
+    assert torch.equal(s.view(torch.int32), tsc.reshape(s.shape).view(torch.int32))
+    xf = widen(bits_of(x.cpu()), str(x.dtype)[6:])
+    want_q, want_s = ue8m0_oracle.quantize(xf, g, r0, c0, scale_fmt=scale_fmt) if scale_fmt else quantize(xf, g, r0, c0)
+    want_s = np.asarray(want_s, np.float32).reshape(tuple(s.shape))
+    if scale_fmt:
+        ue8m0_oracle.assert_pow2_over(s, torch_quantize(x.to(q.device), g, r0, c0)[1])
     got_q, got_s = q.view(torch.uint8).cpu().numpy(), s.cpu().numpy()
     fin = np.isfinite(element_scales(want_s, g, want_q.shape, r0, c0))
     assert np.array_equal(got_q[fin], want_q[fin])

@@ -103,8 +103,9 @@ def plant(x: torch.Tensor, t: Target, kind: str, seed: int) -> torch.Tensor:
     return x.to(getattr(torch, t.dtype))
 
 
-def register_workload(name, xs):
-    """One register() of every target of workload `name` (values `xs`) -> (source, handles, device shards)."""
+def register_workload(name, xs, scale_fmt=None):
+    """One register() of every target of workload `name` (values `xs`), in the scale format `scale_fmt` ->
+    (source, handles, device shards)."""
     w = WORKLOADS[name]
     src = DirectWeightSyncSource()
     sd, slices, quant = {}, {}, {}
@@ -112,7 +113,7 @@ def register_workload(name, xs):
         sd[f"t{i}"] = on_device(x, t.misalign)
         slices[f"t{i}"] = local_slice(t.shape, t.row0, t.col0)
         quant[f"t{i}"] = t.granularity
-    handles = src.register(sd, rank=0, tensor_slices=slices, quantize=quant)
+    handles = src.register(sd, rank=0, tensor_slices=slices, quantize=quant, scale_fmt=scale_fmt)
     return src, handles, sd
 
 
@@ -132,11 +133,11 @@ def live_tables(src, handles, w):
     return tables, targets
 
 
-def check_staging(src, w, xs):
+def check_staging(src, w, xs, scale_fmt=None):
     for i, (t, x) in enumerate(zip(w.targets, xs)):
         q, s, _ = src._quantized[f"t{i}"]
         with named(t.describe()):
-            assert_exact(q, s, x, t.granularity, t.row0, t.col0)
+            assert_exact(q, s, x, t.granularity, t.row0, t.col0, scale_fmt)
 
 
 VARIANTS = ("finite", "inf", "nan", "zero", "subnormal", "refresh")
@@ -145,24 +146,29 @@ VARIANTS = ("finite", "inf", "nan", "zero", "subnormal", "refresh")
 @pytest.mark.parametrize("variant", VARIANTS)
 @pytest.mark.parametrize("regime", sorted(REGIMES))
 def test_regime_on_the_h100(regime, variant):
+    run_regime(regime, variant)
+
+
+def run_regime(regime, variant, scale_fmt=None):
+    """Register the regime's workload in `variant` with the scale format `scale_fmt`, and check it (module doc)."""
     r = REGIMES[regime]
     w = WORKLOADS[r.workload]
     xs = workload_inputs(r.workload)
     if variant not in ("finite", "refresh"):
         xs = [plant(x, t, variant, w.seed + i) for i, (t, x) in enumerate(zip(w.targets, xs))]
-    src, handles, sd = register_workload(r.workload, xs)
-    where = f"{regime} ({r.doc}), {variant}: {w.describe()}"
+    src, handles, sd = register_workload(r.workload, xs, scale_fmt)
+    where = f"{regime} ({r.doc}), {variant}, scale_fmt={scale_fmt}: {w.describe()}"
     try:
         tables, targets = live_tables(src, handles, w)
         assert r.holds(tables, targets), f"not reached: {where}"
         with named(where):
-            check_staging(src, w, xs)
+            check_staging(src, w, xs, scale_fmt)
             if variant == "refresh":
                 xs = [synth_f32(t.shape, w.seed + 50 + i).to(x.dtype) * 0.25 for i, (t, x) in enumerate(zip(w.targets, xs))]
                 for i, x in enumerate(xs):
                     sd[f"t{i}"].copy_(x.to(DEV))
                 assert src.refresh() == len(w.targets)
-                check_staging(src, w, xs)
+                check_staging(src, w, xs, scale_fmt)
     finally:
         run(src.cleanup())
 
@@ -170,6 +176,10 @@ def test_regime_on_the_h100(regime, variant):
 @pytest.mark.parametrize("name", sorted(WORKLOADS))
 def test_workload_writes_nothing_outside_its_outputs(name):
     """The workload's plan driven directly on guarded fp8 and scale buffers, launched twice."""
+    run_guarded(name)
+
+
+def run_guarded(name, scale_fmt=None):
     w = WORKLOADS[name]
     xs = workload_inputs(name)
     targets, outs = [], []
@@ -182,7 +192,7 @@ def test_workload_writes_nothing_outside_its_outputs(name):
         targets.append(_native.SourceQuantTarget(sv.data_ptr(), q.data_ptr(), s.data_ptr(), x.numel() // (rows * cols), rows, cols,
                                                  t.row0, t.col0, CODE[t.dtype], GCODE[t.granularity]))
         outs.append((sv, q, s, qbase, sbase))
-    plans = Plans.build_source_quant({0: targets})
+    plans = Plans.build_source_quant({0: targets}, _native.TSB_QUANT_UE8M0 if scale_fmt else 0)
     try:
         for _ in range(2):
             plans.launch()
@@ -191,7 +201,7 @@ def test_workload_writes_nothing_outside_its_outputs(name):
         plans.close()
     for t, x, (_, q, s, qbase, sbase) in zip(w.targets, xs, outs):
         with named(f"{name}: {t.describe()}"):
-            assert_exact(q, s, x, t.granularity, t.row0, t.col0)
+            assert_exact(q, s, x, t.granularity, t.row0, t.col0, scale_fmt)
             assert guards_intact(qbase) and guards_intact(sbase)
 
 

@@ -63,9 +63,9 @@ def oracle_quantize(x, g):
 
 
 @functools.lru_cache(maxsize=None)
-def compiled(name):
-    """Plan workload `name` on host memory -> (tables, geometry, xs, dests, scales, keepalive).  The
-    destinations are zero; the addresses stay valid while the result is cached."""
+def compiled(name, flags=0):
+    """Plan workload `name` on host memory with the plan `flags` -> (tables, geometry, xs, dests, scales,
+    keepalive).  The destinations are zero; the addresses stay valid while the result is cached."""
     w = WORKLOADS[name]
     xs = workload_inputs(name)
     handles, dests, scales, slices = {}, {}, {}, {}
@@ -79,7 +79,7 @@ def compiled(name):
         scales[n] = torch.zeros(scale_shape(p.g, loc), dtype=torch.float32)
         slices[n] = TensorSlice(off, (0,), p.shape, loc, (1,))
     ops = DirectWeightSyncDest()._build_plan(handles, dests, slices)
-    tables, geom = compile_tables(w.pulls, ops, handles, StridedMem.from_tensor, dests, scales)
+    tables, geom = compile_tables(w.pulls, ops, handles, StridedMem.from_tensor, dests, scales, flags)
     return tables, geom, xs, dests, scales, handles
 
 

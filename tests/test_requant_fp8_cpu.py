@@ -105,9 +105,9 @@ class FakeScaledBuffer:
         self.dtype = shard.dtype
 
 
-def compile_pull(q_full, full_scale, sg, src_boxes, dst_box, dg):
-    """Plan a requantising pull of `q_full`'s `sg`-scaled shards into a `dg`-scaled fp8 window `dst_box`;
-    returns (dest, dest_scale, tables, keepalive)."""
+def compile_pull(q_full, full_scale, sg, src_boxes, dst_box, dg, flags=0):
+    """Plan a requantising pull of `q_full`'s `sg`-scaled shards into a `dg`-scaled fp8 window `dst_box` with the
+    plan `flags`; returns (dest, dest_scale, tables, keepalive)."""
     gshape = tuple(q_full.shape)
     handles, keep = [], []
     for r, (off, loc) in enumerate(src_boxes):
@@ -141,7 +141,7 @@ def compile_pull(q_full, full_scale, sg, src_boxes, dst_box, dg):
     n, k = loc[-2:]
     tgt = _native.make_sq_target_array(1)
     tgt[0] = _native.SqTarget(dest.data_ptr(), dest_scale.data_ptr(), dest.numel() // (n * k), n, k, CODE[dg], 0)
-    tables = _native.requant_fp8_compile_host(0, rects, nr, arr, len(sources), tgt, 1)
+    tables = _native.requant_fp8_compile_host(0, rects, nr, arr, len(sources), tgt, 1, flags)
     return dest, dest_scale, tables, (keep, rects, arr, tgt, handles)
 
 

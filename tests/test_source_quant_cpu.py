@@ -112,11 +112,11 @@ def host_shard(x: torch.Tensor, g: str, r0: int, c0: int, misalign: int = 0):
     return backing, q, s, t
 
 
-def compile_host(targets):
+def compile_host(targets, flags=0):
     arr = _native.make_source_quant_target_array(max(1, len(targets)))
     for i, t in enumerate(targets):
         arr[i] = t
-    return _native.source_quant_compile_host(0, arr, len(targets))
+    return _native.source_quant_compile_host(0, arr, len(targets), flags)
 
 
 def coverage(units, tiles, t, es):
