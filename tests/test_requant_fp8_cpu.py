@@ -356,7 +356,7 @@ def test_plan_cache_key_includes_the_flag():
     for built, flag in ((False, True), (True, False)):
         d = DirectWeightSyncDest()
         d._plan = []
-        d._scale_keys = frozenset({("w", "block_scales")} | ({("", "requantize")} if built else set()))
+        d._plan_key = (frozenset({("w", "block_scales")}), built, None)
         d.close = lambda: (_ for _ in ()).throw(Boom("rebuilt"))
         with pytest.raises(Boom):
             asyncio.run(d.pull({}, {}, block_scales={"w": torch.zeros(1, 1)}, requantize=flag))

@@ -371,7 +371,7 @@ def test_plan_cache_key_includes_the_scale_format():
     for built, fmt in ((None, "ue8m0"), ("ue8m0", None)):
         d = DirectWeightSyncDest()
         d._plan = []
-        d._scale_keys = frozenset({("w", "block_scales")} | ({("", f"scale_fmt={built}")} if built else set()))
+        d._plan_key = (frozenset({("w", "block_scales")}), False, built)
         d.close = lambda: (_ for _ in ()).throw(Boom("rebuilt"))
         with pytest.raises(Boom):
             asyncio.run(d.pull({}, {}, block_scales={"w": torch.zeros(1, 1)}, scale_fmt=fmt))

@@ -45,15 +45,10 @@ logger = logging.getLogger(__name__)
 
 RDMA_KEY_PREFIX = "policy_rdma"
 BLOCK = 128  # edge of a block-scaled fp8 block (elements)
-BLOCK_SOURCE_DTYPES = {torch.bfloat16, torch.float16, torch.float32}
-# the scale granularities of pull(): keyword -> (what its validation messages call the scale, the destination)
-SCALE_KINDS = {
-    "block_scales": ("block scale", "block-scaled"),
-    "channel_scales": ("channel scale", "channel-scaled"),
-    "tensor_scales": ("tensor scale", "tensor-scaled"),
-}
-_GRANULARITY = {"channel_scales": _native.TSB_SCALE_PER_CHANNEL, "tensor_scales": _native.TSB_SCALE_PER_TENSOR}
-_REQUANT_KEY = ("", "requantize")  # in the scale key set of a pull with requantize=True
+# scale granularity -> native code; register() and pull() take one f"{granularity}_scales" dict for each
+GRANULARITIES = {"block": _native.TSB_SCALE_PER_BLOCK, "channel": _native.TSB_SCALE_PER_CHANNEL,
+                 "tensor": _native.TSB_SCALE_PER_TENSOR}
+UNQUANTISED_DTYPES = {torch.bfloat16, torch.float16, torch.float32}  # what quantising routes read and dequantising writes
 SCALE_FORMATS = (None, "ue8m0")  # scale_fmt of the quantising routes: float32 amax / 448, or its power of two up
 
 
@@ -181,16 +176,6 @@ class ScaledNvlinkBuffer(NvlinkBuffer):
         except Exception as e:
             logger.warning("ScaledNvlinkBuffer.drop failed to release the scale: %s", e)
         self._scale_keepalive = None
-
-
-# granularity of a scaled source handle: register() keyword -> (name, native code)
-_SOURCE_SCALES = {
-    "block_scales": ("block", _native.TSB_SCALE_PER_BLOCK),
-    "channel_scales": ("channel", _native.TSB_SCALE_PER_CHANNEL),
-    "tensor_scales": ("tensor", _native.TSB_SCALE_PER_TENSOR),
-}
-GRANULARITIES = {g: code for g, code in _SOURCE_SCALES.values()}
-DEQUANT_DEST_DTYPES = {torch.bfloat16, torch.float16, torch.float32}
 
 
 def source_scale_shapes(granularity: str, shape: tuple, row0: int, col0: int) -> list[tuple]:
@@ -372,7 +357,7 @@ class DirectWeightSyncSource:
                              "tensor_scales cannot be combined with transfer_dtype")
         out: dict[str, tuple] = {}
         for kw, by_name in scales.items():
-            granularity = _SOURCE_SCALES[kw][0]
+            granularity = kw.removesuffix("_scales")
             for name, scale in (by_name or {}).items():
                 req = Request.from_any(name, state_dict[name], tensor_slices.get(name) if tensor_slices else None)
                 w = req.tensor_val
@@ -413,7 +398,7 @@ class DirectWeightSyncSource:
             if granularity not in GRANULARITIES:
                 raise ValueError(f"quantize['{name}'] must be one of {sorted(GRANULARITIES)}, not {granularity!r}")
             w = Request.from_any(name, state_dict[name], tensor_slices.get(name) if tensor_slices else None).tensor_val
-            if w.dtype not in BLOCK_SOURCE_DTYPES:
+            if w.dtype not in UNQUANTISED_DTYPES:
                 raise TypeError(f"quantised weight '{name}' must be bfloat16, float16 or float32, not {w.dtype}")
             if w.dim() < 2:
                 raise ValueError(f"quantised weight '{name}' needs at least 2 dims; got shape {tuple(w.shape)}")
@@ -503,7 +488,7 @@ class DirectWeightSyncDest:
         self._scaled_plans = Plans()  # per-channel / per-tensor scaled fp8 names: likewise
         self._dequant_plans = Plans()  # names read from scaled fp8 handles into bf16/f16/f32: one dequantising plan per device
         self._requant_plans = Plans()  # scaled fp8 destinations read from scaled fp8 handles: one requantising plan per device
-        self._scale_keys: frozenset = frozenset()  # (name, scale keyword) pairs the cached plan quantises (+ _REQUANT_KEY)
+        self._plan_key: tuple | None = None  # ({(name, scale keyword)}, requantize, scale_fmt) of the cached plan's pull
         self._plan_scale_dicts: tuple | None = None  # the three scale dict objects of the last pull
         self.last_pull_ms: dict[int, float] = {}  # device -> kernel time of the last pull
 
@@ -592,13 +577,14 @@ class DirectWeightSyncDest:
     @staticmethod
     def _check_scales(all_handles, dest_state_dict, scales: dict[str, dict | None], *,
                       requantize: bool = False) -> dict[str, tuple]:
-        """Validate the scale dicts of a pull (``{keyword: {name: scale}}``, keywords of SCALE_KINDS) ->
-        ``{name: (keyword, fp8 destination, scale)}``.  With ``requantize``, a name whose handles are all scaled
-        fp8 sources of one granularity is accepted too (it is requantised).  Raises before anything is
-        compiled or launched."""
+        """Validate the scale dicts of a pull (``{keyword: {name: scale}}``, keyword ``f"{granularity}_scales"``) ->
+        ``{name: (keyword, fp8 destination, scale, requantised)}``.  With ``requantize``, a name whose handles are all
+        scaled fp8 sources of one granularity is accepted too, and requantised.  Raises before anything is compiled or
+        launched."""
         out = {}
         for kw, by_name in scales.items():
-            what, kind = SCALE_KINDS[kw]
+            granularity = kw.removesuffix("_scales")
+            what, kind = f"{granularity} scale", f"{granularity}-scaled"
             for name, scale in (by_name or {}).items():
                 if name not in dest_state_dict:
                     raise ValueError(f"{kw} names '{name}', which is not in the destination state dict")
@@ -612,15 +598,9 @@ class DirectWeightSyncDest:
                 if dest.dim() < 2 or dest.numel() == 0 or not dest.is_contiguous() or not dest.is_cuda:
                     raise ValueError(f"{kind} destination '{name}' must be a non-empty contiguous CUDA tensor with at "
                                      f"least 2 dims; got shape {tuple(dest.shape)}, strides {dest.stride()} on {dest.device}")
-                lead, (rows, cols) = tuple(dest.shape[:-2]), dest.shape[-2:]
-                if kw == "block_scales":
-                    wants = [lead + (-(-rows // BLOCK), -(-cols // BLOCK))]
-                elif kw == "channel_scales":
-                    wants = [lead + (rows, 1)]
-                else:
-                    wants = [lead, lead + (1,)]
                 if scale.dtype != torch.float32:
                     raise TypeError(f"{what} of '{name}' must be float32, not {scale.dtype}")
+                wants = source_scale_shapes(granularity, tuple(dest.shape), 0, 0)
                 if tuple(scale.shape) not in wants or not scale.is_contiguous() or scale.device != dest.device:
                     want = " or ".join(map(str, wants))
                     raise ValueError(f"{what} of '{name}' must be a contiguous {want} tensor on {dest.device}; got "
@@ -629,25 +609,25 @@ class DirectWeightSyncDest:
                 if not handles:
                     raise ValueError(f"no source handles for {kind} destination '{name}': its groups would not be covered")
                 kinds = {getattr(h.rdma_buffer, "granularity", None) for h in handles}
-                if requantize and kinds != {None}:
+                requant = requantize and kinds != {None}
+                if requant:
                     if None in kinds:
                         raise ValueError(f"the handles of {kind} destination '{name}' mix scaled fp8 and unscaled sources "
                                          "(requantize=True)")
                     if len(kinds) > 1:
                         raise ValueError(f"the handles of {kind} destination '{name}' mix scale granularities "
                                          f"{sorted(kinds)} (requantize=True)")
-                    out[name] = (kw, dest, scale)
-                    continue
-                dtypes = {h.rdma_buffer.dtype for h in handles}
-                if not dtypes <= BLOCK_SOURCE_DTYPES or len(dtypes) != 1:
-                    hint = ""
-                    if kinds - {None}:
-                        hint = "; scaled fp8 handles are requantised only with requantize=True"
-                    elif requantize:
-                        hint = "; requantize=True reads scaled fp8 handles (registered with a scale), not unscaled fp8"
-                    raise TypeError(f"{kind} pulls of '{name}' read bf16, f16 or f32 handles of one dtype; "
-                                    f"got {sorted(map(str, dtypes))}{hint}")
-                out[name] = (kw, dest, scale)
+                else:
+                    dtypes = {h.rdma_buffer.dtype for h in handles}
+                    if not dtypes <= UNQUANTISED_DTYPES or len(dtypes) != 1:
+                        hint = ""
+                        if kinds - {None}:
+                            hint = "; scaled fp8 handles are requantised only with requantize=True"
+                        elif requantize:
+                            hint = "; requantize=True reads scaled fp8 handles (registered with a scale), not unscaled fp8"
+                        raise TypeError(f"{kind} pulls of '{name}' read bf16, f16 or f32 handles of one dtype; "
+                                        f"got {sorted(map(str, dtypes))}{hint}")
+                out[name] = (kw, dest, scale, requant)
         return out
 
     @staticmethod
@@ -670,7 +650,7 @@ class DirectWeightSyncDest:
             dest = getattr(param, "_local_tensor", param)
             if dest.dtype == torch.float8_e4m3fn:
                 continue
-            if dest.dtype not in DEQUANT_DEST_DTYPES:
+            if dest.dtype not in UNQUANTISED_DTYPES:
                 raise TypeError(f"'{name}' has {kinds.pop()}-scaled fp8 handles: its destination must be bfloat16, "
                                 f"float16, float32 (dequantised) or float8_e4m3fn (bytes moved), not {dest.dtype}")
             if dest.dim() < 2 or not dest.is_contiguous():
@@ -681,11 +661,16 @@ class DirectWeightSyncDest:
 
     def _compile(self, scaled: dict | None = None, dequant: set | None = None, requant: set | None = None,
                  flags: int = 0) -> None:
-        """Compile the cached transfer plan; ``flags`` go to the quantising and requantising plans."""
+        """Compile the cached transfer plan along the routes :meth:`_check_scales` chose: ``scaled`` is its
+        ``{name: (keyword, fp8 destination, scale, ...)}`` and ``requant`` the names it requantises; ``dequant`` is
+        what :meth:`_check_dequant` returned.  ``flags`` go to the quantising and requantising plans."""
+        scaled, requant = scaled or {}, requant or set()
+        # the plan kind of each scaled name, in build order: 0 requantises, 1 quantises into blocks, 2 into channels
+        # or tensors
+        kind = {n: 0 if n in requant else 1 if kw == "block_scales" else 2 for n, (kw, *_) in scaled.items()}
         per_device: dict[int, list] = defaultdict(list)
-        quant_pairs: dict[tuple, list] = defaultdict(list)  # (device, block?) -> windows of the quantising plans
         dq: dict[int, tuple[list, dict]] = {}  # device -> (windows, {source buffer id: (name, DqSource)})
-        rq: dict[int, tuple[list, dict]] = {}  # likewise for the requantising plans
+        quant: dict[tuple, tuple] = defaultdict(lambda: ([], {}, [], []))  # (kind, device) -> the same, names, targets
         for op in self._plan:
             dest = op.dest_local
             if not dest.is_cuda:
@@ -699,12 +684,11 @@ class DirectWeightSyncDest:
                 )
             dev = dest.device.index
             window = self.op_windows(op, op.rdma_buffer.window(dev))
-            if requant and op.name in requant:
-                pairs, sources = rq.setdefault(dev, ([], {}))
+            if op.name in kind:
+                pairs, sources, _, _ = quant[(kind[op.name], dev)]
                 pairs.append(window)
-                _add_dq_source(sources, op, dev)
-            elif scaled and op.name in scaled:
-                quant_pairs[(dev, scaled[op.name][0] == "block_scales")].append(window)
+                if kind[op.name] == 0:
+                    _add_dq_source(sources, op, dev)
             elif dequant and op.name in dequant:
                 pairs, sources = dq.setdefault(dev, ([], {}))
                 pairs.append(window)
@@ -718,40 +702,26 @@ class DirectWeightSyncDest:
                 _build_named(self._dequant_plans, Plans.build_dequant_fp8,
                              {dev: (pairs, [s for _, s in sources.values()])}, {"source": names},
                              lambda n: f"dequantising pull of '{n}'")
-            if not scaled:
-                return
-            for dev in sorted({scaled[n][1].device.index for n in requant or ()}):
-                names = [n for n in requant if scaled[n][1].device.index == dev]
-                targets = []
-                for n in names:
-                    kw, d, s = scaled[n]
-                    rows, cols = d.shape[-2:]
-                    code = _native.TSB_SCALE_PER_BLOCK if kw == "block_scales" else _GRANULARITY[kw]
-                    targets.append(_native.SqTarget(d.data_ptr(), s.data_ptr(), d.numel() // (rows * cols), rows, cols, code, 0))
-                pairs, sources = rq.get(dev, ([], {}))
-                _build_named(self._requant_plans, lambda per_device: Plans.build_requant_fp8(per_device, flags),
-                             {dev: (pairs, [s for _, s in sources.values()], targets)},
-                             {"target": names, "source": [n for n, _ in sources.values()]},
-                             lambda n: f"requantising pull of '{n}' ({scaled[n][0]})")
-            for block in (True, False):
-                for dev in sorted({d.device.index for n, (kw, d, _) in scaled.items()
-                                   if (kw == "block_scales") == block and n not in (requant or ())}):
-                    names = [n for n, (kw, d, _) in scaled.items()
-                             if d.device.index == dev and (kw == "block_scales") == block and n not in (requant or ())]
-                    targets = []
-                    for n in names:
-                        kw, d, s = scaled[n]
-                        rows, cols = d.shape[-2:]
-                        if block:
-                            targets.append(_native.BqTarget(d.data_ptr(), s.data_ptr(), d.numel() // (rows * cols), rows, cols))
-                        else:
-                            targets.append(_native.SqTarget(d.data_ptr(), s.data_ptr(), d.numel() // (rows * cols), rows, cols,
-                                                            _GRANULARITY[kw], 0))
-                    plans, build = (self._block_plans, Plans.build_block_fp8) if block else \
-                        (self._scaled_plans, Plans.build_scaled_fp8)
-                    _build_named(plans, lambda per_device, build=build: build(per_device, flags),
-                                 {dev: (quant_pairs.get((dev, block), []), targets)}, {"target": names},
-                                 lambda n: f"{SCALE_KINDS[scaled[n][0]][1]} pull of '{n}' ({scaled[n][0]})")
+            for n, (kw, d, s, *_) in scaled.items():
+                _, _, names, targets = quant[(kind[n], d.device.index)]
+                names.append(n)
+                targets.append(_quant_target(kw.removesuffix("_scales"), d, s, n in requant))
+
+            def pull_of(n):
+                kw = scaled[n][0]
+                what = "requantising" if n in requant else f"{kw.removesuffix('_scales')}-scaled"
+                return f"{what} pull of '{n}' ({kw})"
+
+            builds = ((self._requant_plans, Plans.build_requant_fp8), (self._block_plans, Plans.build_block_fp8),
+                      (self._scaled_plans, Plans.build_scaled_fp8))
+            for (k, dev), (pairs, sources, names, targets) in sorted(quant.items()):
+                plans, build = builds[k]
+                args, by_index = (pairs, targets), {"target": names}
+                if k == 0:
+                    args = (pairs, [s for _, s in sources.values()], targets)
+                    by_index["source"] = [n for n, _ in sources.values()]
+                _build_named(plans, lambda per_device, build=build: build(per_device, flags), {dev: args}, by_index,
+                             pull_of)
         except BaseException:
             for plans in self._fp8_plans:
                 plans.close()
@@ -813,17 +783,14 @@ class DirectWeightSyncDest:
         is enqueued, and the data-pointer signature -- which catches ``param.data = new`` under an
         unchanged object -- is recomputed while the kernel runs."""
         scales = (block_scales, channel_scales, tensor_scales)
-        names = {n for d in scales for n in (d or ())}
+        scale_dicts = {f"{g}_scales": d for g, d in zip(GRANULARITIES, scales)}
+        scaled_names = frozenset((n, kw) for kw, d in scale_dicts.items() for n in (d or ()))
         flags = scale_fmt_flags(scale_fmt)
-        if scale_fmt is not None and not names:
+        if scale_fmt is not None and not scaled_names:
             raise ValueError("scale_fmt applies to quantised and requantised names: block_scales, channel_scales or "
                              "tensor_scales must name at least one")
-        keys = frozenset((n, kw) for kw, d in zip(SCALE_KINDS, scales) for n in (d or ()))
-        if requantize:
-            keys |= {_REQUANT_KEY}
-        if scale_fmt is not None:
-            keys |= {("", f"scale_fmt={scale_fmt}")}
-        if self._plan is not None and keys != self._scale_keys:
+        key = (scaled_names, bool(requantize), scale_fmt)
+        if self._plan is not None and key != self._plan_key:
             logger.info("scaled names or their granularity changed; rebuilding the transfer plan")
             self.close()
         if self._plan is not None and dest_state_dict is self._plan_dict and \
@@ -851,17 +818,16 @@ class DirectWeightSyncDest:
                 self._plan_scale_dicts = scales
             verified = True
         if self._plan is None:
-            scaled = self._check_scales(all_handles, dest_state_dict, dict(zip(SCALE_KINDS, scales)),
-                                        requantize=requantize) if names else None
-            dequant = self._check_dequant(all_handles, dest_state_dict, names)
-            requant = {n for n in scaled or () if getattr(all_handles[n][0].rdma_buffer, "granularity", None)}
+            scaled = self._check_scales(all_handles, dest_state_dict, scale_dicts, requantize=requantize)
+            dequant = self._check_dequant(all_handles, dest_state_dict, scaled)
+            requant = {n for n, (*_, requantised) in scaled.items() if requantised}
             self._plan = self._build_plan(all_handles, dest_state_dict, dest_slices)
             try:
                 self._compile(scaled, dequant, requant, flags)
             except BaseException:
                 self._plan = None
                 raise
-            self._scale_keys = keys
+            self._plan_key = key
             self._plan_signature = self._signature(dest_state_dict, scales)
             self._plan_ids, self._plan_refs, self._plan_dict = ids, refs, dest_state_dict
             self._plan_scale_dicts = scales
@@ -902,9 +868,8 @@ class DirectWeightSyncDest:
         self._native_plans.close()
         for plans in self._fp8_plans:
             plans.close()
-        self._scale_keys = frozenset()
         self._plan = None
-        self._plan_ids = self._plan_refs = self._plan_dict = self._plan_scale_dicts = None
+        self._plan_key = self._plan_ids = self._plan_refs = self._plan_dict = self._plan_scale_dicts = None
 
 
 def _build_named(plans: Plans, build, per_device: dict, names: dict[str, list[str]], pull_of) -> None:
@@ -929,6 +894,16 @@ def _add_dq_source(sources: dict, op: _TransferOp, dev: int) -> None:
         rows, cols = w.shape[-2:]
         sources[id(buf)] = (op.name, _native.DqSource(w.ptr, s.ptr, w.numel // (rows * cols), rows, cols,
                                                       buf.row0, buf.col0, GRANULARITIES[buf.granularity], 0))
+
+
+def _quant_target(granularity: str, dest: torch.Tensor, scale: torch.Tensor, requant: bool):
+    """The native target of a scaled fp8 destination: a BqTarget for a block-quantising pull, else an SqTarget (the
+    requantising plan takes SqTargets of every granularity)."""
+    rows, cols = dest.shape[-2:]
+    args = (dest.data_ptr(), scale.data_ptr(), dest.numel() // (rows * cols), rows, cols)
+    if granularity == "block" and not requant:
+        return _native.BqTarget(*args)
+    return _native.SqTarget(*args, GRANULARITIES[granularity], 0)
 
 
 def _contig(shape) -> tuple:
