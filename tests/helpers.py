@@ -156,10 +156,27 @@ def edge_case(rng: random.Random, tile_units: int, kind: str, uniform: str | Non
         sdt = ddt = rng.choice(SAME_DTYPES)
         aligned, vec_cast = kind == "aligned" or rng.random() < 0.5, False
     cast = sdt != ddt
-    big = T >= 4096  # keep the largest tile sizes to a few tens of MiB per workload
     # elements per unit: 8 for a vector cast, 16 bytes for an aligned byte move, one element otherwise
     epu = 8 if vec_cast else (16 // sdt.itemsize if aligned and not cast else 1)
+    units, rows, n_outer = edge_geometry(rng, T, kind)
+    outer = _edge_outer(rng, rows, n_outer) if n_outer else []
+    if not outer and rows > 1:
+        outer = [rows]
+    shape = outer + [units * epu]
+    pad_outer = kind in ("wide_nd", "deep_nd") or rng.random() < 0.7
+    sbase, sidx = _edge_window(rng, shape, sdt.itemsize, aligned, pad_outer)
+    dbase, didx = _edge_window(rng, shape, ddt.itemsize, aligned, pad_outer)
+    if not aligned and cast and rng.random() < 0.5:
+        # misalign only one side: still no vector mode, but the other side is a clean pitch
+        dbase, didx = _edge_window(rng, shape, ddt.itemsize, True, pad_outer)
+    return RectCase(sbase, dbase, sdt, ddt, lambda b, i=sidx: b[i], lambda b, i=didx: b[i])
 
+
+def edge_geometry(rng: random.Random, tile_units: int, kind: str):
+    """(units per row, rows, outer dims) of a window of `kind` (see EDGE_KINDS) for copy tiles of
+    `tile_units` units."""
+    T = tile_units
+    big = T >= 4096  # keep the largest tile sizes to a few tens of MiB per workload
     n_outer = 0
     if kind in ("wide_exact", "wide_minus", "wide_plus"):
         k = rng.choice([1, 2])
@@ -188,18 +205,7 @@ def edge_case(rng: random.Random, tile_units: int, kind: str, uniform: str | Non
         n_outer = rng.choice([0, 1, 2, 3])
         units = rng.choice([1, 2, 5, 31, T // 2, T, T + 3])
         rows = max(1, rng.choice([1, 3, 8, 17]) * max(1, n_outer))
-    units = max(1, units)
-    outer = _edge_outer(rng, rows, n_outer) if n_outer else []
-    if not outer and rows > 1:
-        outer = [rows]
-    shape = outer + [units * epu]
-    pad_outer = kind in ("wide_nd", "deep_nd") or rng.random() < 0.7
-    sbase, sidx = _edge_window(rng, shape, sdt.itemsize, aligned, pad_outer)
-    dbase, didx = _edge_window(rng, shape, ddt.itemsize, aligned, pad_outer)
-    if not aligned and cast and rng.random() < 0.5:
-        # misalign only one side: still no vector mode, but the other side is a clean pitch
-        dbase, didx = _edge_window(rng, shape, ddt.itemsize, True, pad_outer)
-    return RectCase(sbase, dbase, sdt, ddt, lambda b, i=sidx: b[i], lambda b, i=didx: b[i])
+    return max(1, units), rows, n_outer
 
 
 def edge_workload(rng: random.Random, tile_units: int, uniform: str | None = None, cast: bool | None = None,
@@ -229,9 +235,9 @@ DEV_RECT = np.dtype([
     ("pad_", "<u4", (3,)),
 ])
 assert DEV_RECT.itemsize == 192
-MODE_B16, MODE_F32_BF16_V8 = 4, 8
+MODE_B16, MODE_F32_BF16_V8, MODE_BF16_E4M3_V16 = 4, 8, 26
 VECTOR_CAST_MODES = (8, 10, 12, 14, 16, 18)
-KIND_GENERIC, KIND_B16, KIND_F32_BF16 = 0, 1, 2
+KIND_GENERIC, KIND_B16, KIND_F32_BF16, KIND_BF16_E4M3 = 0, 1, 2, 3
 
 
 def rect_fields(table: np.ndarray) -> np.ndarray:
@@ -245,6 +251,8 @@ def plan_kind(fields: np.ndarray) -> int:
         return KIND_B16
     if len(fields) and (fields["mode"] == MODE_F32_BF16_V8).all():
         return KIND_F32_BF16
+    if len(fields) and (fields["mode"] == MODE_BF16_E4M3_V16).all():
+        return KIND_BF16_E4M3
     return KIND_GENERIC
 
 
