@@ -29,6 +29,7 @@ Typical usage is unchanged::
 from __future__ import annotations
 
 import logging
+import math
 import re
 from collections import defaultdict
 from dataclasses import dataclass
@@ -187,6 +188,91 @@ def source_scale_shapes(granularity: str, shape: tuple, row0: int, col0: int) ->
     if granularity == "channel":
         return [lead + (n, 1)]
     return [lead, lead + (1,)]
+
+
+def scale_grid(granularity: str, shape: tuple, row0: int, col0: int) -> tuple:
+    """The scale of a ``shape`` fp8 shard at global offset (row0, col0) viewed as ``lead + (group rows, group
+    cols)``: one of :func:`source_scale_shapes`, with ``lead + (1, 1)`` per tensor."""
+    if granularity == "tensor":
+        return tuple(shape[:-2]) + (1, 1)
+    return source_scale_shapes(granularity, shape, row0, col0)[0]
+
+
+def verbatim_scale_rects(granularity: str, shape: tuple, offset: tuple, ops: list) -> tuple[list, tuple | None]:
+    """Map the scales of a verbatim pull: fp8 bytes and scales of same-granularity sources moved as they are.
+
+    ``shape`` and ``offset`` are the destination's local shape and global offset (all dims); each op is
+    ``(source shard shape, source shard global offset, (global offset, extent) of the op's rectangle)``.
+    Destination groups are anchored at the destination's local origin (128x128 blocks, rows, or the matrix
+    per leading index); source groups at the global origin, cut by the source shard.
+
+    Returns ``(rects, None)`` when every destination group lies inside one source group of one op:
+    ``rects[i] = (op index, source index, destination index)``, unit-step slices into the :func:`scale_grid`
+    views of the op's source scale and of the destination scale, together writing every destination scale
+    once.  Otherwise ``([], group)``: the first (lexicographically smallest) offending destination group as
+    ``lead + (group row, group col)``.  ValueError when a destination element lies in no op's rectangle or in
+    two."""
+    nd = len(shape)
+    lead = nd - 2
+    rows, cols = shape[-2:]
+    # per dim: destination group size and source group size (None: the whole dim, as far as the shard reaches)
+    size, src_size = [1] * lead, [1] * lead
+    if granularity == "block":
+        size, src_size = size + [BLOCK, BLOCK], src_size + [BLOCK, BLOCK]
+    elif granularity == "channel":
+        size, src_size = size + [1, cols], src_size + [1, None]
+    else:
+        size, src_size = size + [rows, cols], src_size + [None, None]
+    local = []  # op rectangles in destination-local coordinates: [(start, stop) per dim]
+    volume = 0
+    for src_shape, src_off, (g_off, ext) in ops:
+        box = [(g - o, g - o + e) for g, o, e in zip(g_off, offset, ext)]
+        if any(s < 0 or t > n or s >= t for (s, t), n in zip(box, shape)) or \
+                any(g < so or g + e > so + n for g, e, so, n in zip(g_off, ext, src_off, src_shape)):
+            raise ValueError(f"op rectangle at {tuple(g_off)} extent {tuple(ext)} is empty or leaves its source shard "
+                             "or the destination")
+        local.append(box)
+        volume += math.prod(ext)
+    for i, a in enumerate(local):
+        for b in local[:i]:
+            if all(max(sa, sb) < min(ta, tb) for (sa, ta), (sb, tb) in zip(a, b)):
+                first = tuple(o + max(sa, sb) for o, (sa, _), (sb, _) in zip(offset, a, b))
+                raise ValueError(f"global element {first} is covered by two handles")
+    if volume != math.prod(shape):
+        raise ValueError(f"{math.prod(shape) - volume} of its {math.prod(shape)} elements are covered by no handle")
+
+    def groups(d, s, t):  # destination groups [first, last + 1) meeting local [s, t) in dim d
+        return s // size[d], (t - 1) // size[d] + 1
+
+    bad = []  # low corners of boxes of offending groups
+    for box in local:
+        low = [groups(d, s, t)[0] for d, (s, t) in enumerate(box)]
+        for d, (s, t) in enumerate(box):  # an op edge inside a group: the group straddles two handles
+            if s % size[d]:
+                bad.append(tuple(low))
+            if t % size[d] and t != shape[d]:
+                bad.append(tuple(low[:d] + [(t - 1) // size[d]] + low[d + 1:]))
+    for d in range(lead, nd):  # a group across a source group edge (only 128-blocks have such edges)
+        if src_size[d] is None:
+            continue
+        for j in range(-(-shape[d] // size[d])):
+            s, t = offset[d] + j * size[d], offset[d] + min((j + 1) * size[d], shape[d])
+            if s // src_size[d] != (t - 1) // src_size[d]:
+                bad.append(tuple(j if e == d else 0 for e in range(nd)))
+                break
+    if bad:
+        return [], min(bad)
+    rects = []
+    for i, (box, (_, src_off, _)) in enumerate(zip(local, ops)):
+        src_idx, dst_idx = [], []
+        for d, (s, t) in enumerate(box):
+            j0, j1 = groups(d, s, t)
+            g0 = offset[d] + j0 * size[d]  # global start of the first group
+            k0 = 0 if src_size[d] is None else g0 // src_size[d] - src_off[d] // src_size[d]
+            src_idx.append(slice(k0, k0 + j1 - j0))
+            dst_idx.append(slice(j0, j1))
+        rects.append((i, tuple(src_idx), tuple(dst_idx)))
+    return rects, None
 
 
 @dataclass
@@ -468,6 +554,8 @@ class _TransferOp:
     # planner metadata
     name: str = ""
     dest_local: torch.Tensor | None = None
+    dest_offsets: tuple = ()  # global offsets of the destination shard and of the source shard
+    src_offsets: tuple = ()
 
 
 class DirectWeightSyncDest:
@@ -488,7 +576,7 @@ class DirectWeightSyncDest:
         self._scaled_plans = Plans()  # per-channel / per-tensor scaled fp8 names: likewise
         self._dequant_plans = Plans()  # names read from scaled fp8 handles into bf16/f16/f32: one dequantising plan per device
         self._requant_plans = Plans()  # scaled fp8 destinations read from scaled fp8 handles: one requantising plan per device
-        self._plan_key: tuple | None = None  # ({(name, scale keyword)}, requantize, scale_fmt) of the cached plan's pull
+        self._plan_key: tuple | None = None  # ({(name, scale keyword)}, requantize, scale_fmt, verbatim) of its pull
         self._plan_scale_dicts: tuple | None = None  # the three scale dict objects of the last pull
         self.last_pull_ms: dict[int, float] = {}  # device -> kernel time of the last pull
 
@@ -526,7 +614,8 @@ class DirectWeightSyncDest:
                         f"Expected contiguous dest tensor for key={name}, strides={dest_tensor.stride()}"
                     )
                     ops.append(_TransferOp(rdma_buffer=handle.rdma_buffer, dest_byte_view=to_byte_view(dest_tensor),
-                                           name=name, dest_local=dest_tensor))
+                                           name=name, dest_local=dest_tensor, dest_offsets=tuple(dest_slice.offsets),
+                                           src_offsets=tuple(src_slice.offsets)))
                 else:
                     ndim = len(inter.offsets)
                     src_idx = tuple(
@@ -540,7 +629,8 @@ class DirectWeightSyncDest:
                         for d in range(ndim)
                     )
                     ops.append(_TransferOp(rdma_buffer=handle.rdma_buffer, dest_byte_view=None, dest_tensor=dest_tensor,
-                                           src_slices=src_idx, dest_slices=dst_idx, name=name, dest_local=dest_tensor))
+                                           src_slices=src_idx, dest_slices=dst_idx, name=name, dest_local=dest_tensor,
+                                           dest_offsets=tuple(dest_slice.offsets), src_offsets=tuple(src_slice.offsets)))
         logger.info("Built transfer plan with %d NVLink ops", len(ops))
         return ops
 
@@ -576,11 +666,16 @@ class DirectWeightSyncDest:
 
     @staticmethod
     def _check_scales(all_handles, dest_state_dict, scales: dict[str, dict | None], *,
-                      requantize: bool = False) -> dict[str, tuple]:
+                      requantize: bool = False, verbatim: bool = False) -> dict[str, tuple]:
         """Validate the scale dicts of a pull (``{keyword: {name: scale}}``, keyword ``f"{granularity}_scales"``) ->
-        ``{name: (keyword, fp8 destination, scale, requantised)}``.  With ``requantize``, a name whose handles are all
-        scaled fp8 sources of one granularity is accepted too, and requantised.  Raises before anything is compiled or
-        launched."""
+        ``{name: (keyword, fp8 destination, scale, route)}``, route ``"quantise"``, ``"requantise"`` or
+        ``"verbatim"``.  With ``requantize``, a name whose handles are all scaled fp8 sources of one granularity is
+        accepted too, and requantised; with ``verbatim``, such a name of the destination's granularity is moved as
+        it is.  Raises before anything is compiled or launched."""
+        if requantize and verbatim:
+            raise ValueError("requantize=True and verbatim=True are exclusive: verbatim=True moves scaled fp8 bytes and "
+                             "scales as they are (same granularity, groups that line up), requantize=True re-rounds "
+                             "them into any destination layout")
         out = {}
         for kw, by_name in scales.items():
             granularity = kw.removesuffix("_scales")
@@ -609,25 +704,72 @@ class DirectWeightSyncDest:
                 if not handles:
                     raise ValueError(f"no source handles for {kind} destination '{name}': its groups would not be covered")
                 kinds = {getattr(h.rdma_buffer, "granularity", None) for h in handles}
-                requant = requantize and kinds != {None}
-                if requant:
+                route = "quantise"
+                if requantize and kinds != {None}:
+                    route = "requantise"
                     if None in kinds:
                         raise ValueError(f"the handles of {kind} destination '{name}' mix scaled fp8 and unscaled sources "
                                          "(requantize=True)")
                     if len(kinds) > 1:
                         raise ValueError(f"the handles of {kind} destination '{name}' mix scale granularities "
                                          f"{sorted(kinds)} (requantize=True)")
+                elif verbatim and kinds != {None}:
+                    route = "verbatim"
+                    if None in kinds:
+                        raise TypeError(f"the handles of {kind} destination '{name}' mix scaled fp8 and unscaled sources "
+                                        "(verbatim=True)")
+                    if kinds != {granularity}:
+                        raise ValueError(f"{kind} destination '{name}' has {'/'.join(sorted(kinds))}-scaled handles: a "
+                                         "verbatim pull moves scales of the destination's granularity only; use "
+                                         "requantize=True to convert them")
                 else:
                     dtypes = {h.rdma_buffer.dtype for h in handles}
                     if not dtypes <= UNQUANTISED_DTYPES or len(dtypes) != 1:
                         hint = ""
                         if kinds - {None}:
                             hint = "; scaled fp8 handles are requantised only with requantize=True"
-                        elif requantize:
-                            hint = "; requantize=True reads scaled fp8 handles (registered with a scale), not unscaled fp8"
+                        elif requantize or verbatim:
+                            flag = "requantize" if requantize else "verbatim"
+                            hint = f"; {flag}=True reads scaled fp8 handles (registered with a scale), not unscaled fp8"
                         raise TypeError(f"{kind} pulls of '{name}' read bf16, f16 or f32 handles of one dtype; "
                                         f"got {sorted(map(str, dtypes))}{hint}")
-                out[name] = (kw, dest, scale, requant)
+                out[name] = (kw, dest, scale, route)
+        return out
+
+    @staticmethod
+    def _verbatim_rects(plan: list[_TransferOp], scaled: dict) -> dict[str, list]:
+        """The scale rectangles of every verbatim name of ``scaled`` (:meth:`_check_scales`' verdict) ->
+        ``{name: [(op, source scale index, destination scale index)]}`` (:func:`verbatim_scale_rects`).  Raises
+        ValueError naming the weight before anything is compiled or launched."""
+        ops: dict[str, list] = {n: [] for n, (*_, route) in scaled.items() if route == "verbatim"}
+        for op in plan:
+            if op.name in ops:
+                ops[op.name].append(op)
+        out = {}
+        for name, mine in ops.items():
+            kw, dest, _, _ = scaled[name]
+            granularity = kw.removesuffix("_scales")
+            if not mine:
+                raise ValueError(f"verbatim pull of '{name}' ({kw}): no handle covers its destination")
+            shape, offset = tuple(dest.shape), mine[0].dest_offsets
+            rects = []
+            for op in mine:
+                start = [0] * len(shape) if op.dest_slices is None else [s.start for s in op.dest_slices]
+                ext = shape if op.dest_slices is None else [s.stop - s.start for s in op.dest_slices]
+                rects.append((tuple(op.rdma_buffer.shape), op.src_offsets,
+                              (tuple(o + s for o, s in zip(offset, start)), tuple(ext))))
+            try:
+                mapped, group = verbatim_scale_rects(granularity, shape, offset, rects)
+            except ValueError as e:
+                raise ValueError(f"verbatim pull of '{name}' ({kw}): {e}") from None
+            if group is not None:
+                what, idx, legend = {"block": ("block", group, "leading indices, block row, block column"),
+                                     "channel": ("row", group[:-1], "leading indices, row"),
+                                     "tensor": ("matrix", group[:-2], "leading indices")}[granularity]
+                raise ValueError(f"verbatim pull of '{name}' ({kw}): destination {what} {idx} ({legend}) does not lie "
+                                 "inside one source group of one handle; requantize=True pulls it into these groups (the "
+                                 "usual cause is a TP shard whose global column offset is not a multiple of 128)")
+            out[name] = [(mine[i], src, dst) for i, src, dst in mapped]
         return out
 
     @staticmethod
@@ -660,15 +802,27 @@ class DirectWeightSyncDest:
         return out
 
     def _compile(self, scaled: dict | None = None, dequant: set | None = None, requant: set | None = None,
-                 flags: int = 0) -> None:
+                 flags: int = 0, verbatim: dict | None = None) -> None:
         """Compile the cached transfer plan along the routes :meth:`_check_scales` chose: ``scaled`` is its
-        ``{name: (keyword, fp8 destination, scale, ...)}`` and ``requant`` the names it requantises; ``dequant`` is
-        what :meth:`_check_dequant` returned.  ``flags`` go to the quantising and requantising plans."""
-        scaled, requant = scaled or {}, requant or set()
-        # the plan kind of each scaled name, in build order: 0 requantises, 1 quantises into blocks, 2 into channels
-        # or tensors
-        kind = {n: 0 if n in requant else 1 if kw == "block_scales" else 2 for n, (kw, *_) in scaled.items()}
+        ``{name: (keyword, fp8 destination, scale, ...)}``, ``requant`` the names it requantises and ``verbatim``
+        :meth:`_verbatim_rects` of the names it moves as they are; ``dequant`` is what :meth:`_check_dequant`
+        returned.  ``flags`` go to the quantising and requantising plans."""
+        scaled, requant, verbatim = scaled or {}, requant or set(), verbatim or {}
+        # the plan kind of each quantised or requantised name, in build order: 0 requantises, 1 quantises into blocks,
+        # 2 into channels or tensors
+        kind = {n: 0 if n in requant else 1 if kw == "block_scales" else 2 for n, (kw, *_) in scaled.items()
+                if n not in verbatim}
         per_device: dict[int, list] = defaultdict(list)
+        # verbatim names: their fp8 bytes go with the plain copies below, their scales as float32 rectangles
+        for n, rects in verbatim.items():
+            kw, dest_q, dest_s, *_ = scaled[n]
+            dev, granularity = dest_q.device.index, kw.removesuffix("_scales")
+            dst = StridedMem.from_tensor(dest_s)
+            dst = _as_grid(dst, scale_grid(granularity, tuple(dest_q.shape), 0, 0))
+            for op, src_idx, dst_idx in rects:
+                buf = op.rdma_buffer
+                src = _as_grid(buf.scale_window(dev), scale_grid(granularity, tuple(buf.shape), buf.row0, buf.col0))
+                per_device[dev].append((src.sub(src_idx), dst.sub(dst_idx)))
         dq: dict[int, tuple[list, dict]] = {}  # device -> (windows, {source buffer id: (name, DqSource)})
         quant: dict[tuple, tuple] = defaultdict(lambda: ([], {}, [], []))  # (kind, device) -> the same, names, targets
         for op in self._plan:
@@ -703,6 +857,8 @@ class DirectWeightSyncDest:
                              {dev: (pairs, [s for _, s in sources.values()])}, {"source": names},
                              lambda n: f"dequantising pull of '{n}'")
             for n, (kw, d, s, *_) in scaled.items():
+                if n not in kind:
+                    continue
                 _, _, names, targets = quant[(kind[n], d.device.index)]
                 names.append(n)
                 targets.append(_quant_target(kw.removesuffix("_scales"), d, s, n in requant))
@@ -743,7 +899,7 @@ class DirectWeightSyncDest:
                    block_scales: dict[str, torch.Tensor] | None = None,
                    channel_scales: dict[str, torch.Tensor] | None = None,
                    tensor_scales: dict[str, torch.Tensor] | None = None, requantize: bool = False,
-                   scale_fmt: str | None = None) -> None:
+                   scale_fmt: str | None = None, verbatim: bool = False) -> None:
         """Pull every overlapping region into ``dest_state_dict`` (in place).  Returns when the
         bytes are in destination HBM (so the caller may tell the source it is done reading).
 
@@ -778,6 +934,15 @@ class DirectWeightSyncDest:
         scales to powers of two.  ``None`` keeps the plain float32 formula.  ValueError for another value, or for a
         ``scale_fmt`` without a name in the scale dicts.  Changing it rebuilds the plan.
 
+        Verbatim (extension, ``verbatim=True``): a name in one of the scale dicts whose handles are all scaled fp8
+        sources of the destination's granularity is moved as it is: its fp8 bytes and the float32 scales of the
+        source groups holding its groups go into the copy plan, with no arithmetic, so ``f32(q) * scale`` is the
+        source's bit for bit (NaN and Inf groups, UE8M0 and any checkpoint scale included).  Every destination group
+        must lie inside one source group of one handle (:func:`verbatim_scale_rects`); ValueError naming the first
+        group that does not, for handles of another granularity, for an element covered by no handle or by two,
+        with ``requantize=True``, and for a ``scale_fmt`` when every scaled name is verbatim.  Names fed by
+        bf16/f16/f32 handles are still quantised.  Changing it rebuilds the plan.
+
         Steady state costs one native call to launch and a poll loop: the cached plan is checked
         against the destination OBJECTS first (their ids; the plan keeps them alive), the kernel
         is enqueued, and the data-pointer signature -- which catches ``param.data = new`` under an
@@ -789,7 +954,7 @@ class DirectWeightSyncDest:
         if scale_fmt is not None and not scaled_names:
             raise ValueError("scale_fmt applies to quantised and requantised names: block_scales, channel_scales or "
                              "tensor_scales must name at least one")
-        key = (scaled_names, bool(requantize), scale_fmt)
+        key = (scaled_names, bool(requantize), scale_fmt, bool(verbatim))
         if self._plan is not None and key != self._plan_key:
             logger.info("scaled names or their granularity changed; rebuilding the transfer plan")
             self.close()
@@ -818,12 +983,17 @@ class DirectWeightSyncDest:
                 self._plan_scale_dicts = scales
             verified = True
         if self._plan is None:
-            scaled = self._check_scales(all_handles, dest_state_dict, scale_dicts, requantize=requantize)
+            scaled = self._check_scales(all_handles, dest_state_dict, scale_dicts, requantize=requantize,
+                                        verbatim=verbatim)
+            if scale_fmt is not None and all(route == "verbatim" for *_, route in scaled.values()):
+                raise ValueError("scale_fmt does nothing here: every name of block_scales, channel_scales and "
+                                 "tensor_scales is moved verbatim and keeps its source's scales")
             dequant = self._check_dequant(all_handles, dest_state_dict, scaled)
-            requant = {n for n, (*_, requantised) in scaled.items() if requantised}
+            requant = {n for n, (*_, route) in scaled.items() if route == "requantise"}
             self._plan = self._build_plan(all_handles, dest_state_dict, dest_slices)
             try:
-                self._compile(scaled, dequant, requant, flags)
+                verbatim_rects = self._verbatim_rects(self._plan, scaled)
+                self._compile(scaled, dequant, requant, flags, verbatim_rects)
             except BaseException:
                 self._plan = None
                 raise
@@ -841,7 +1011,7 @@ class DirectWeightSyncDest:
             self.close()
             await self.pull(all_handles, dest_state_dict, dest_slices, block_scales=block_scales,
                             channel_scales=channel_scales, tensor_scales=tensor_scales, requantize=requantize,
-                            scale_fmt=scale_fmt)
+                            scale_fmt=scale_fmt, verbatim=verbatim)
 
     def launch(self) -> None:
         """Enqueue the cached plan on each device's copy stream, fenced against the caller's current
@@ -904,6 +1074,11 @@ def _quant_target(granularity: str, dest: torch.Tensor, scale: torch.Tensor, req
     if granularity == "block" and not requant:
         return _native.BqTarget(*args)
     return _native.SqTarget(*args, GRANULARITIES[granularity], 0)
+
+
+def _as_grid(scale: StridedMem, grid: tuple) -> StridedMem:
+    """A contiguous scale window viewed with the shape of its :func:`scale_grid`."""
+    return StridedMem(scale.ptr, grid, _contig(grid), scale.dtype, scale.device)
 
 
 def _contig(shape) -> tuple:

@@ -88,23 +88,28 @@ async def put_state_dict(store, state_dict, key, direct_rdma=False, transfer_dty
 
 async def get_state_dict(store, key, user_state_dict: dict | None = None, strict=True, direct_rdma=False,
                          block_scales: dict | None = None, channel_scales: dict | None = None,
-                         tensor_scales: dict | None = None, requantize: bool = False, scale_fmt: str | None = None):
+                         tensor_scales: dict | None = None, requantize: bool = False, scale_fmt: str | None = None,
+                         verbatim: bool = False):
     """Fetch a state dict.  ``user_state_dict`` tensors are filled in place (and required in direct
     mode).  A missing mapping means no matching push finished: RuntimeError.  ``block_scales``
     (direct mode only) names float8_e4m3fn destinations quantised into the 128x128 block-scaled
     layout during the pull; ``channel_scales`` / ``tensor_scales`` likewise name destinations with one
     float32 scale per row / per matrix (see ``DirectWeightSyncDest.pull``).  ``requantize=True`` (direct
     mode only) lets such destinations be fed by scaled fp8 handles, re-rounding them into the destination's
-    layout.  ``scale_fmt="ue8m0"`` (direct mode only) gives every such destination power-of-two scales."""
+    layout.  ``scale_fmt="ue8m0"`` (direct mode only) gives every such destination power-of-two scales.
+    ``verbatim=True`` (direct mode only) moves the fp8 bytes and scales of such destinations fed by scaled fp8
+    handles of their own granularity as they are, without re-rounding."""
     if direct_rdma:
         assert user_state_dict is not None, "user_state_dict is required for direct_rdma mode"
         await _get_state_dict_direct_rdma(store, key, user_state_dict, block_scales, channel_scales, tensor_scales,
-                                          requantize, scale_fmt)
+                                          requantize, scale_fmt, verbatim)
         return user_state_dict
     if scale_fmt is not None:
         raise NotImplementedError("scale_fmt needs direct_rdma=True: the store path does not quantise")
     if requantize:
         raise NotImplementedError("requantize needs direct_rdma=True: the store path does not requantise scaled fp8")
+    if verbatim:
+        raise NotImplementedError("verbatim needs direct_rdma=True: the store path does not move scaled fp8 sources")
     if block_scales:
         raise NotImplementedError("block_scales needs direct_rdma=True: the store path does not quantise into block-scaled fp8")
     if channel_scales or tensor_scales:
@@ -200,7 +205,7 @@ def _try_all_gather(cache: _DirectRDMACache, key: str, user_state_dict, scaled=F
 
 
 async def _get_state_dict_direct_rdma(store, key, user_state_dict, block_scales=None, channel_scales=None,
-                                      tensor_scales=None, requantize=False, scale_fmt=None):
+                                      tensor_scales=None, requantize=False, scale_fmt=None, verbatim=False):
     from torchstore_b200.collectives import allgather_enabled
     from torchstore_b200.direct_weight_sync import DirectWeightSyncDest
 
@@ -226,4 +231,4 @@ async def _get_state_dict_direct_rdma(store, key, user_state_dict, block_scales=
         cache.handles[key] = all_handles
     await cache.dests[key].pull(cache.handles[key], user_state_dict, block_scales=block_scales,
                                 channel_scales=channel_scales, tensor_scales=tensor_scales, requantize=requantize,
-                                scale_fmt=scale_fmt)
+                                scale_fmt=scale_fmt, verbatim=verbatim)
