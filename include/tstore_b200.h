@@ -60,6 +60,14 @@ enum {
   TSB_F64 = 7,
   TSB_F8E4M3 = 8, /* float8_e4m3fn: one side of a cast (a same-dtype fp8 move is TSB_U8) */
   TSB_F8E5M2 = 9, /* float8_e5m2: likewise */
+  TSB_I8 = 10,    /* int8, valid ONLY as the dst_dtype of the rects of tsb_block_fp8_* and tsb_scaled_fp8_*: the
+                   * destination is quantised to symmetric int8 (see tsb_bq_target_t).  Every rect of one such plan
+                   * writes one dtype, TSB_F8E4M3 or TSB_I8 (a mix is TSB_ERR_INVALID); TSB_I8 with TSB_QUANT_UE8M0
+                   * is TSB_ERR_INVALID.  The copy plan, the fused casts (tsb_cast_supported), the dequantising,
+                   * requantising and source-side calls refuse it; a plain int8 move is TSB_U8.  *_compile_host
+                   * returns the same tables for TSB_I8 rects as for TSB_F8E4M3 rects: the dtype selects the
+                   * kernels only.  Libraries that predate it refuse TSB_I8 rects with TSB_ERR_UNSUPPORTED, so
+                   * callers can detect it without an ABI version change. */
 };
 
 /* ------------------------------------------------------------------------------------------ */
@@ -224,18 +232,23 @@ int tsb_pool_stats(uint64_t* out_blocks, uint64_t* out_allocs, uint64_t* out_reu
  *   amax = max |x| over the block (NaN if any x is NaN); amax_c = max(amax, 1e-4f) (NaN stays NaN)
  *   dst[i, j] = e4m3fn(rn(x[i, j] * (448 / amax_c)))  with torch's .to(float8_e4m3fn) rounding
  *   scale_inv[i / 128, j / 128] = amax_c / 448
- * with correctly rounded f32 divisions and multiply, x widened exactly to f32. */
+ * with correctly rounded f32 divisions and multiply, x widened exactly to f32.  With TSB_I8 rects dst is int8:
+ *   scale = 127 / amax_c;  scale_inv = amax_c / 127
+ *   dst[i, j] = int8(sat[-128, 127](rne_int(rn(x[i, j] * scale))))  with NaN -> 0
+ * (a NaN group: scale_inv NaN, dst 0; an Inf group: scale 0, scale_inv Inf, dst 0).  The same holds for the
+ * groups of tsb_sq_target_t. */
 typedef struct tsb_bq_target {
-  uint64_t dst;       /* float8_e4m3fn, contiguous [batch, rows, cols] */
+  uint64_t dst;       /* float8_e4m3fn (or int8 for TSB_I8 rects), contiguous [batch, rows, cols] */
   uint64_t scale_inv; /* float32, contiguous [batch, ceil(rows/128), ceil(cols/128)] */
   uint64_t batch, rows, cols;
 } tsb_bq_target_t;
 
 /* Compile a block-scaled pull: `rects` are ordinary source -> destination rectangles with
- * src_dtype in {TSB_F32, TSB_BF16, TSB_F16}, dst_dtype == TSB_F8E4M3 and dst inside one target.
+ * src_dtype in {TSB_F32, TSB_BF16, TSB_F16}, dst_dtype == TSB_F8E4M3 (or TSB_I8 for every rect) and dst inside
+ * one target.
  * Every element of every target must be written by exactly one rect (TSB_ERR_INVALID otherwise: a
  * block's scale needs all of it).  The result is a plan like any other: tsb_plan_launch[_flags],
- * _run, _poll, _wait, _elapsed_ms, _info and _destroy accept it.  flags: 0 or TSB_QUANT_UE8M0. */
+ * _run, _poll, _wait, _elapsed_ms, _info and _destroy accept it.  flags: 0 or TSB_QUANT_UE8M0 (not with TSB_I8). */
 int tsb_block_fp8_plan_create(int device, const tsb_rect_t* rects, uint64_t n, const tsb_bq_target_t* targets,
                               uint64_t n_targets, uint32_t flags, tsb_plan_t* out);
 /* Host-only (no CUDA call): compile and copy the kernel tables out.  out_blocks: records of 32 bytes
@@ -259,9 +272,10 @@ enum { TSB_SCALE_PER_CHANNEL = 1, TSB_SCALE_PER_TENSOR = 2 };
  * (TSB_SCALE_PER_TENSOR; scale_inv is float32 [batch]).  Per group:
  *   amax = max |x| over the group (NaN if any x is NaN); amax_c = max(amax, 1e-4f) (NaN stays NaN)
  *   dst = e4m3fn(rn(x * (448 / amax_c)))  with torch's .to(float8_e4m3fn) rounding;  scale_inv = amax_c / 448
- * with correctly rounded f32 divisions and multiply, x widened exactly to f32. */
+ * with correctly rounded f32 divisions and multiply, x widened exactly to f32.  TSB_I8 rects quantise into int8 with
+ * the formula of tsb_bq_target_t. */
 typedef struct tsb_sq_target {
-  uint64_t dst;       /* float8_e4m3fn, contiguous [batch, rows, cols] */
+  uint64_t dst;       /* float8_e4m3fn (or int8 for TSB_I8 rects), contiguous [batch, rows, cols] */
   uint64_t scale_inv; /* float32, contiguous, one per group */
   uint64_t batch, rows, cols;
   uint32_t granularity; /* TSB_SCALE_PER_CHANNEL or TSB_SCALE_PER_TENSOR */
@@ -273,7 +287,7 @@ typedef struct tsb_sq_target {
  * naming the target and group otherwise).  A per-channel row of at most 32 KiB of source bytes is
  * quantised from shared memory after one read; per-tensor groups and longer rows take two passes
  * (amax, then quantise), reading the source twice.  The result is a plan like any other.
- * flags: 0 or TSB_QUANT_UE8M0. */
+ * flags: 0 or TSB_QUANT_UE8M0 (not with TSB_I8). */
 int tsb_scaled_fp8_plan_create(int device, const tsb_rect_t* rects, uint64_t n, const tsb_sq_target_t* targets,
                                uint64_t n_targets, uint32_t flags, tsb_plan_t* out);
 /* Host-only (no CUDA call): compile and copy the kernel tables out.  A NULL table only reports its count.

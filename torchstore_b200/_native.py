@@ -24,6 +24,7 @@ TSB_U8, TSB_U16, TSB_U32, TSB_U64, TSB_F16, TSB_BF16, TSB_F32, TSB_F64, TSB_F8E4
 TSB_H2D, TSB_D2H, TSB_D2D = 1, 2, 3
 TSB_PLAN_DEFAULT, TSB_PLAN_NO_INTERLEAVE = 0, 1
 TSB_QUANT_UE8M0 = 1  # flags of the quantising plan calls: power-of-two scales
+TSB_I8 = 10  # int8, only as the dst_dtype of a quantising pull's rects (tsb_block_fp8_*, tsb_scaled_fp8_*)
 
 
 class TsbError(RuntimeError):

@@ -16,6 +16,8 @@
 //            rounded up to a power of two and scale = 1 / scale_inv (fp8_quant.cuh).
 //   phase 2  shared -> e4m3fn: x * scale (__fmul_rn), torch-exact narrowing (fp8_cvt.cuh), 16
 //            destination bytes per thread and step (one STG.128 when aligned, byte stores at ragged edges).
+// int8 destinations (TSB_I8 rects) run the same kernel with the int8 format of fp8_quant.cuh: scale step 127
+// instead of 448, and a round-to-nearest-even saturating int8 narrowing (NaN -> 0).  The tables are the same.
 
 #include <algorithm>
 #include <atomic>
@@ -177,8 +179,19 @@ int rect_boxes(const tsb_rect_t& in, uint64_t index, const TargetGeom* targets, 
   if (in.ndim < 1 || in.ndim > TSB_MAX_DIMS) return fail(TSB_ERR_INVALID, where + "ndim must be in [1, 6]");
   const uint32_t es = quant_src_bytes(in.src_dtype);
   if (!es) return fail(TSB_ERR_UNSUPPORTED, where + "scaled fp8 pulls read f32, bf16 or f16 sources");
-  if (in.dst_dtype != TSB_F8E4M3) return fail(TSB_ERR_UNSUPPORTED, where + "scaled fp8 destinations are float8_e4m3fn");
+  if (in.dst_dtype != TSB_F8E4M3 && in.dst_dtype != TSB_I8)
+    return fail(TSB_ERR_UNSUPPORTED, where + "scaled destinations are float8_e4m3fn or int8");
   return map_boxes(in, index, targets, n_targets, kByDst, es, out);
+}
+
+int quant_dst_int8(const tsb_rect_t* rects, uint64_t n, bool ue8m0, bool* int8) {
+  *int8 = n && rects[0].dst_dtype == TSB_I8;
+  for (uint64_t i = 1; i < n; ++i)
+    if ((rects[i].dst_dtype == TSB_I8) != *int8)
+      return fail(TSB_ERR_INVALID, "rect " + std::to_string(i) + ": the rects of one plan write one destination dtype, "
+                                   "float8_e4m3fn or int8");
+  if (*int8 && ue8m0) return fail(TSB_ERR_INVALID, "int8 destinations take float32 scales: TSB_QUANT_UE8M0 is refused");
+  return TSB_OK;
 }
 
 int rect_source_boxes(const tsb_rect_t& in, uint64_t index, const TargetGeom* grids, uint64_t n_grids,
@@ -363,8 +376,8 @@ __device__ __forceinline__ uint32_t stage_block(const BqBlock& blk, const BqPiec
   return m;
 }
 
-// Phase 2: shared memory -> e4m3fn, 16 destination bytes per thread and step.
-template <uint32_t DT>
+// Phase 2: shared memory -> the destination format, 16 destination bytes per thread and step.
+template <uint32_t DT, class Out>
 __device__ __forceinline__ void quantise_block(const BqBlock& blk, const unsigned char* smem, float scale) {
   constexpr uint32_t es = Src<DT>::kBytes;
   constexpr uint32_t spitch = kBqBlock * es;
@@ -377,22 +390,34 @@ __device__ __forceinline__ void quantise_block(const BqBlock& blk, const unsigne
     const uint32_t nvalid = min(16u, static_cast<uint32_t>(blk.cols) - c);
     uint32_t f[16], o[4];
     load16_shared<DT>(s, nvalid, f);
-    narrow16(f, scale, o);
+    Out::narrow(f, scale, o);
     store16(d, nvalid, o);
   }
 }
 
-template <uint32_t DT, bool kUe8m0>
+template <uint32_t DT, class Out>
 __device__ __forceinline__ void run_block(const BqBlock& blk, const BqPiece* pieces, unsigned char* smem, uint32_t* s_red,
                                           float* s_scale) {
   cta_max(stage_block<DT>(blk, pieces, smem), s_red, [&](uint32_t a) {
     float scale, scale_inv;
-    group_scales<kUe8m0>(a, &scale, &scale_inv);
+    Out::scales(a, &scale, &scale_inv);
     *s_scale = scale;
     *reinterpret_cast<float*>(blk.scale) = scale_inv;
   });
   __syncthreads();
-  quantise_block<DT>(blk, smem, *s_scale);
+  quantise_block<DT, Out>(blk, smem, *s_scale);
+}
+
+// The CTA's block in destination format Out (fp8_quant.cuh), the body of the kernels below
+template <class Out>
+__device__ __forceinline__ void quantise_blocks(const BqBlock* __restrict__ blocks, const BqPiece* __restrict__ pieces,
+                                                unsigned char* stage, uint32_t* s_red, float* s_scale) {
+  const BqBlock blk = blocks[blockIdx.x];
+  switch (blk.src_dtype) {
+    case TSB_BF16: run_block<TSB_BF16, Out>(blk, pieces, stage, s_red, s_scale); break;
+    case TSB_F16: run_block<TSB_F16, Out>(blk, pieces, stage, s_red, s_scale); break;
+    default: run_block<TSB_F32, Out>(blk, pieces, stage, s_red, s_scale); break;
+  }
 }
 
 // kUe8m0: power-of-two scales (TSB_QUANT_UE8M0)
@@ -401,12 +426,15 @@ __global__ void __launch_bounds__(kQuantThreads, 6) block_fp8_kernel(const BqBlo
   extern __shared__ __align__(16) unsigned char stage[];
   __shared__ uint32_t s_red[kQuantThreads / 32];
   __shared__ float s_scale;
-  const BqBlock blk = blocks[blockIdx.x];
-  switch (blk.src_dtype) {
-    case TSB_BF16: run_block<TSB_BF16, kUe8m0>(blk, pieces, stage, s_red, &s_scale); break;
-    case TSB_F16: run_block<TSB_F16, kUe8m0>(blk, pieces, stage, s_red, &s_scale); break;
-    default: run_block<TSB_F32, kUe8m0>(blk, pieces, stage, s_red, &s_scale); break;
-  }
+  quantise_blocks<E4m3Out<kUe8m0>>(blocks, pieces, stage, s_red, &s_scale);
+}
+
+// int8 destinations (TSB_I8)
+__global__ void __launch_bounds__(kQuantThreads, 6) block_int8_kernel(const BqBlock* __restrict__ blocks, const BqPiece* __restrict__ pieces) {
+  extern __shared__ __align__(16) unsigned char stage[];
+  __shared__ uint32_t s_red[kQuantThreads / 32];
+  __shared__ float s_scale;
+  quantise_blocks<I8Out>(blocks, pieces, stage, s_red, &s_scale);
 }
 
 cudaError_t prepare() {
@@ -417,7 +445,7 @@ cudaError_t prepare() {
   if (e != cudaSuccess) return e;
   const uint64_t bit = 1ull << (dev & 63);
   if (prepared.load(std::memory_order_acquire) & bit) return cudaSuccess;
-  for (auto kernel : {block_fp8_kernel<false>, block_fp8_kernel<true>}) {
+  for (auto kernel : {block_fp8_kernel<false>, block_fp8_kernel<true>, block_int8_kernel}) {
     e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(kBqBlock * kBqBlock * 4));
     if (e != cudaSuccess) return e;
   }
@@ -426,12 +454,12 @@ cudaError_t prepare() {
 }
 
 int launch_block_fp8(const BqBlock* blocks, const BqPiece* pieces, uint32_t n_blocks, uint32_t max_src_bytes, bool ue8m0,
-                     cudaStream_t stream) {
+                     bool int8, cudaStream_t stream) {
   const cudaError_t e = prepare();
   if (e != cudaSuccess) return cuda_fail(e, "block_fp8_kernel launch");
-  const auto kernel = ue8m0 ? block_fp8_kernel<true> : block_fp8_kernel<false>;
+  const auto kernel = int8 ? block_int8_kernel : ue8m0 ? block_fp8_kernel<true> : block_fp8_kernel<false>;
   kernel<<<n_blocks, kQuantThreads, kBqBlock * kBqBlock * max_src_bytes, stream>>>(blocks, pieces);
-  return launched("block_fp8_kernel launch");
+  return launched(int8 ? "block_int8_kernel launch" : "block_fp8_kernel launch");
 }
 
 // d = {BqBlock table | BqPiece table}, one CTA per block
@@ -439,15 +467,15 @@ int block_fp8_plan(int device, const tsb_rect_t* rects, uint64_t n, const tsb_bq
                    QuantPlan* q) {
   BqTables tb;
   int st = block_fp8_compile(device, rects, n, targets, n_targets, &tb);
-  if (st) return st;
+  if (st || (st = quant_dst_int8(rects, n, q->ue8m0, &q->int8))) return st;
   q->add(tb.blocks);
   const size_t pieces = q->add(tb.pieces);
   q->seal(0);
   q->describe(n, static_cast<uint32_t>(tb.blocks.size()), kBqBlock * kBqBlock, tb);
-  q->launch = [pieces, n_blocks = static_cast<uint32_t>(tb.blocks.size()), es = tb.max_src_bytes, ue8m0 = q->ue8m0](char* d,
-                                                                                                               cudaStream_t s) {
+  q->launch = [pieces, n_blocks = static_cast<uint32_t>(tb.blocks.size()), es = tb.max_src_bytes, ue8m0 = q->ue8m0,
+               int8 = q->int8](char* d, cudaStream_t s) {
     return launch_block_fp8(reinterpret_cast<const BqBlock*>(d), reinterpret_cast<const BqPiece*>(d + pieces), n_blocks, es, ue8m0,
-                            s);
+                            int8, s);
   };
   return TSB_OK;
 }

@@ -1,6 +1,6 @@
 // Device helpers of the scaled fp8 kernels (block_fp8.cu, scaled_fp8.cu, dequant_fp8.cu, requant_fp8.cu,
 // source_quant.cu): exact widening of bf16/f16/f32 source bits to f32, |x| as an ordered integer, the folding
-// 16-byte loads, the CTA max, and the 16-element narrowing x * scale -> e4m3fn with its stores.
+// 16-byte loads, the CTA max, and the 16-element narrowing x * scale -> e4m3fn (or int8) with its stores.
 #pragma once
 
 #include <cuda_fp16.h>
@@ -146,6 +146,27 @@ __device__ __forceinline__ void narrow16(const uint32_t f[16], float scale, uint
   }
 }
 
+// x * scale (correctly rounded) -> int8: round to nearest even, saturated to [-128, 127], NaN -> 0, 4 bytes per
+// word.  `scale` is I8Out's: a NaN product arises exactly in the groups whose scale is not positive (a NaN group's
+// scale is NaN; an Inf group's is 0, and Inf * 0 is NaN while its finite elements give +-0), so the NaN rule is
+// applied per group here, not left to what the cvt does with NaN.  In a finite group scale is positive and finite
+// and |x * scale| stays below 128.
+__device__ __forceinline__ void narrow16_i8(const uint32_t f[16], float scale, uint32_t o[4]) {
+  const bool finite_group = scale > 0.0f;
+#pragma unroll
+  for (uint32_t q = 0; q < 4; ++q) {
+    int32_t i[4];
+#pragma unroll
+    for (uint32_t j = 0; j < 4; ++j) i[j] = __float2int_rn(__fmul_rn(__uint_as_float(f[4 * q + j]), scale));
+    // saturate pairs to s8 and pack: bytes 2, 3 first, then 0, 1 below them
+    uint32_t hi;
+    asm("cvt.pack.sat.s8.s32.b32 %0, %1, %2, 0;" : "=r"(hi) : "r"(i[3]), "r"(i[2]));
+    uint32_t w;
+    asm("cvt.pack.sat.s8.s32.b32 %0, %1, %2, %3;" : "=r"(w) : "r"(i[1]), "r"(i[0]), "r"(hi));
+    o[q] = finite_group ? w : 0u;
+  }
+}
+
 // the first nvalid of 16 fp8 bytes to global memory: one STG.128 when whole and aligned, else bytes
 __device__ __forceinline__ void store16(char* d, uint32_t nvalid, const uint32_t o[4]) {
   if (nvalid == 16 && (reinterpret_cast<uintptr_t>(d) & 15u) == 0) {
@@ -157,16 +178,17 @@ __device__ __forceinline__ void store16(char* d, uint32_t nvalid, const uint32_t
   }
 }
 
-// amax bits -> (scale, scale_inv): amax_c = max(amax, 1e-4f), scale = 448 / amax_c, scale_inv = amax_c / 448,
-// both correctly rounded; a NaN amax gives NaN for both
-__device__ __forceinline__ void scales_of_amax(uint32_t a, float* scale, float* scale_inv) {
+// amax bits -> (scale, scale_inv) of a format whose largest magnitude is qmax (448 for e4m3fn, 127 for int8):
+// amax_c = max(amax, 1e-4f), scale = qmax / amax_c, scale_inv = amax_c / qmax, both correctly rounded; a NaN amax
+// gives NaN for both
+__device__ __forceinline__ void scales_of_amax(uint32_t a, float* scale, float* scale_inv, float qmax = 448.0f) {
   if (a > 0x7f800000u) {
     *scale = __uint_as_float(0x7fffffffu);
     *scale_inv = *scale;
   } else {
     const float amax_c = fmaxf(__uint_as_float(a), 1e-4f);
-    *scale = __fdiv_rn(448.0f, amax_c);
-    *scale_inv = __fdiv_rn(amax_c, 448.0f);
+    *scale = __fdiv_rn(qmax, amax_c);
+    *scale_inv = __fdiv_rn(amax_c, qmax);
   }
 }
 
@@ -193,5 +215,21 @@ __device__ __forceinline__ void group_scales(uint32_t a, float* scale, float* sc
   else
     scales_of_amax(a, scale, scale_inv);
 }
+
+// The destination formats of the quantising pulls (block_fp8.cu, scaled_fp8.cu): a group's (scale, scale_inv)
+// from its amax bits, and the 16-element narrowing.  Their kernels are templates on one of these.
+template <bool kUe8m0>
+struct E4m3Out {  // float8_e4m3fn (TSB_F8E4M3), float32 or power-of-two scales
+  static __device__ __forceinline__ void scales(uint32_t a, float* scale, float* scale_inv) {
+    group_scales<kUe8m0>(a, scale, scale_inv);
+  }
+  static __device__ __forceinline__ void narrow(const uint32_t f[16], float scale, uint32_t o[4]) { narrow16(f, scale, o); }
+};
+struct I8Out {  // int8 (TSB_I8), symmetric, scale step 127
+  static __device__ __forceinline__ void scales(uint32_t a, float* scale, float* scale_inv) {
+    scales_of_amax(a, scale, scale_inv, 127.0f);
+  }
+  static __device__ __forceinline__ void narrow(const uint32_t f[16], float scale, uint32_t o[4]) { narrow16_i8(f, scale, o); }
+};
 
 }  // namespace tsb

@@ -19,6 +19,9 @@
 //                            amax word (|x| as an integer: finite < Inf < NaN, so a NaN poisons the group).
 //   scaled_fp8_quant_kernel  pass 2, one CTA per tile: the group's scale from its amax, the tile re-read and
 //                            quantised straight to HBM; the group's one designated tile writes scale_inv.
+// int8 destinations (TSB_I8 rects) run scaled_int8_rows_kernel and scaled_int8_quant_kernel, the same kernels in
+// the int8 format of fp8_quant.cuh (scale step 127, round-to-nearest-even saturating narrowing, NaN -> 0), after
+// the same amax pass, from the same tables.
 // The amax words live in the plan's device allocation and are cleared on the launch stream before pass 1,
 // so a replayed plan starts from zero.
 
@@ -261,7 +264,7 @@ __device__ __forceinline__ void stage_band(const SqBand& band, const SqPiece* __
   }
 }
 
-template <uint32_t DT, bool kUe8m0>
+template <uint32_t DT, class Out>
 __device__ __forceinline__ void run_band(const SqBand& band, const SqPiece* pieces, unsigned char* smem, uint32_t* s_amax,
                                          float* s_scale) {
   constexpr uint32_t es = Src<DT>::kBytes;
@@ -272,7 +275,7 @@ __device__ __forceinline__ void run_band(const SqBand& band, const SqPiece* piec
   __syncthreads();
   for (uint32_t r = threadIdx.x; r < band.rows; r += kQuantThreads) {
     float scale, scale_inv;
-    group_scales<kUe8m0>(s_amax[r], &scale, &scale_inv);
+    Out::scales(s_amax[r], &scale, &scale_inv);
     s_scale[r] = scale;
     reinterpret_cast<float*>(band.scale)[r] = scale_inv;
   }
@@ -284,8 +287,20 @@ __device__ __forceinline__ void run_band(const SqBand& band, const SqPiece* piec
     const uint32_t nvalid = min(16u, band.cols - c);
     uint32_t f[16], o[4];
     load16_shared<DT>(smem + r * spitch + c * es, nvalid, f);
-    narrow16(f, s_scale[r], o);
+    Out::narrow(f, s_scale[r], o);
     store16(reinterpret_cast<char*>(band.dst) + static_cast<uint64_t>(r) * band.cols + c, nvalid, o);
+  }
+}
+
+// The CTA's band in destination format Out (fp8_quant.cuh), the body of the row-staged kernels below
+template <class Out>
+__device__ __forceinline__ void quantise_bands(const SqBand* __restrict__ bands, const SqPiece* __restrict__ pieces,
+                                               unsigned char* stage, uint32_t* s_amax, float* s_scale) {
+  const SqBand band = bands[blockIdx.x];
+  switch (band.src_dtype) {
+    case TSB_BF16: run_band<TSB_BF16, Out>(band, pieces, stage, s_amax, s_scale); break;
+    case TSB_F16: run_band<TSB_F16, Out>(band, pieces, stage, s_amax, s_scale); break;
+    default: run_band<TSB_F32, Out>(band, pieces, stage, s_amax, s_scale); break;
   }
 }
 
@@ -296,12 +311,16 @@ __global__ void __launch_bounds__(kQuantThreads, 5) scaled_fp8_rows_kernel(const
   extern __shared__ __align__(16) unsigned char stage[];
   __shared__ uint32_t s_amax[kSqBandRows];
   __shared__ float s_scale[kSqBandRows];
-  const SqBand band = bands[blockIdx.x];
-  switch (band.src_dtype) {
-    case TSB_BF16: run_band<TSB_BF16, kUe8m0>(band, pieces, stage, s_amax, s_scale); break;
-    case TSB_F16: run_band<TSB_F16, kUe8m0>(band, pieces, stage, s_amax, s_scale); break;
-    default: run_band<TSB_F32, kUe8m0>(band, pieces, stage, s_amax, s_scale); break;
-  }
+  quantise_bands<E4m3Out<kUe8m0>>(bands, pieces, stage, s_amax, s_scale);
+}
+
+// int8 destinations (TSB_I8), here and in scaled_int8_quant_kernel
+__global__ void __launch_bounds__(kQuantThreads, 5) scaled_int8_rows_kernel(const SqBand* __restrict__ bands,
+                                                                        const SqPiece* __restrict__ pieces) {
+  extern __shared__ __align__(16) unsigned char stage[];
+  __shared__ uint32_t s_amax[kSqBandRows];
+  __shared__ float s_scale[kSqBandRows];
+  quantise_bands<I8Out>(bands, pieces, stage, s_amax, s_scale);
 }
 
 // this thread's max abs_bits over the tile
@@ -351,7 +370,7 @@ __global__ void __launch_bounds__(kQuantThreads) scaled_fp8_amax_kernel(const Sq
   });
 }
 
-template <uint32_t DT>
+template <uint32_t DT, class Out>
 __device__ __forceinline__ void quantise_tile(const SqTile& t, float scale) {
   constexpr uint32_t es = Src<DT>::kBytes;
   const uint32_t cpr = (t.cols + 15u) / 16u;
@@ -370,36 +389,48 @@ __device__ __forceinline__ void quantise_tile(const SqTile& t, float scale) {
 #pragma unroll
       for (uint32_t j = 0; j < 16; ++j) f[j] = j < nvalid ? elem<DT>(reinterpret_cast<const unsigned char*>(s), j) : 0u;
     }
-    narrow16(f, scale, o);
+    Out::narrow(f, scale, o);
     store16(reinterpret_cast<char*>(t.dst) + static_cast<uint64_t>(r) * t.dst_pitch + c, nvalid, o);
+  }
+}
+
+// Pass 2 of the CTA's tile in destination format Out, the body of the quantise kernels below
+template <class Out>
+__device__ __forceinline__ void quantise_tiles(const SqTile* __restrict__ tiles, const uint32_t* __restrict__ amax) {
+  const SqTile t = tiles[blockIdx.x];
+  float scale, scale_inv;
+  Out::scales(amax[t.group], &scale, &scale_inv);
+  if (t.scale && threadIdx.x == 0) *reinterpret_cast<float*>(t.scale) = scale_inv;
+  switch (t.src_dtype) {
+    case TSB_BF16: quantise_tile<TSB_BF16, Out>(t, scale); break;
+    case TSB_F16: quantise_tile<TSB_F16, Out>(t, scale); break;
+    default: quantise_tile<TSB_F32, Out>(t, scale); break;
   }
 }
 
 template <bool kUe8m0>
 __global__ void __launch_bounds__(kQuantThreads) scaled_fp8_quant_kernel(const SqTile* __restrict__ tiles,
                                                                     const uint32_t* __restrict__ amax) {
-  const SqTile t = tiles[blockIdx.x];
-  float scale, scale_inv;
-  group_scales<kUe8m0>(amax[t.group], &scale, &scale_inv);
-  if (t.scale && threadIdx.x == 0) *reinterpret_cast<float*>(t.scale) = scale_inv;
-  switch (t.src_dtype) {
-    case TSB_BF16: quantise_tile<TSB_BF16>(t, scale); break;
-    case TSB_F16: quantise_tile<TSB_F16>(t, scale); break;
-    default: quantise_tile<TSB_F32>(t, scale); break;
-  }
+  quantise_tiles<E4m3Out<kUe8m0>>(tiles, amax);
+}
+
+__global__ void __launch_bounds__(kQuantThreads) scaled_int8_quant_kernel(const SqTile* __restrict__ tiles,
+                                                                     const uint32_t* __restrict__ amax) {
+  quantise_tiles<I8Out>(tiles, amax);
 }
 
 }  // namespace
 
 int launch_scaled_fp8(const SqLaunch& l, cudaStream_t stream) {
   if (l.n_bands) {
-    const auto rows_kernel = l.ue8m0 ? scaled_fp8_rows_kernel<true> : scaled_fp8_rows_kernel<false>;
+    const auto rows_kernel = l.int8 ? scaled_int8_rows_kernel : l.ue8m0 ? scaled_fp8_rows_kernel<true> : scaled_fp8_rows_kernel<false>;
     rows_kernel<<<l.n_bands, kQuantThreads, l.stage_bytes, stream>>>(l.bands, l.pieces);
-    if (int st = launched("scaled_fp8_rows_kernel launch")) return st;
+    if (int st = launched(l.int8 ? "scaled_int8_rows_kernel launch" : "scaled_fp8_rows_kernel launch")) return st;
   }
   if (!l.n_tiles) return TSB_OK;
-  return launch_two_pass(scaled_fp8_amax_kernel, l.ue8m0 ? scaled_fp8_quant_kernel<true> : scaled_fp8_quant_kernel<false>,
-                         "scaled_fp8", l.tiles, l.n_tiles, l.amax, l.n_groups, stream);
+  const auto quant_kernel = l.int8 ? scaled_int8_quant_kernel : l.ue8m0 ? scaled_fp8_quant_kernel<true> : scaled_fp8_quant_kernel<false>;
+  return launch_two_pass(scaled_fp8_amax_kernel, quant_kernel, l.int8 ? "scaled_int8" : "scaled_fp8", l.tiles, l.n_tiles, l.amax,
+                         l.n_groups, stream);
 }
 
 namespace {
@@ -409,12 +440,12 @@ int scaled_fp8_plan(int device, const tsb_rect_t* rects, uint64_t n, const tsb_s
                     QuantPlan* q) {
   SqTables tb;
   int st = scaled_fp8_compile(device, rects, n, targets, n_targets, &tb);
-  if (st) return st;
+  if (st || (st = quant_dst_int8(rects, n, q->ue8m0, &q->int8))) return st;
   q->add(tb.bands);
   const size_t pieces = q->add(tb.pieces), tiles = q->add(tb.tiles), amax = q->seal(tb.n_groups);
   q->describe(n, static_cast<uint32_t>(tb.bands.size() + tb.tiles.size()), kSqStageBytes, tb);
   const SqLaunch l{nullptr, nullptr, nullptr, nullptr, static_cast<uint32_t>(tb.bands.size()), static_cast<uint32_t>(tb.tiles.size()),
-                   tb.n_groups, tb.stage_bytes, q->ue8m0};
+                   tb.n_groups, tb.stage_bytes, q->ue8m0, q->int8};
   q->launch = [l, pieces, tiles, amax](char* d, cudaStream_t s) {
     SqLaunch x = l;
     x.bands = reinterpret_cast<const SqBand*>(d);

@@ -250,6 +250,7 @@ struct QuantPlan {
   std::vector<Section> sections;  // the tables, in the order of the kind's tsb_*_compile_host outputs
   uint32_t n_groups = 0;          // amax words
   bool ue8m0 = false;             // TSB_QUANT_UE8M0: the launch runs the power-of-two scale kernels (tables unchanged)
+  bool int8 = false;              // TSB_I8 destinations: the launch runs the int8 kernels (tables unchanged)
   tsb_plan_info_t info{};
   std::function<int(char* d, cudaStream_t)> launch;  // runs the plan from its tables' device copy at d
 
@@ -325,6 +326,9 @@ int rect_boxes(const tsb_rect_t& in, uint64_t index, const TargetGeom* targets, 
 // destination side.  Destination columns must be contiguous.
 int rect_source_boxes(const tsb_rect_t& in, uint64_t index, const TargetGeom* grids, uint64_t n_grids,
                       std::vector<TargetBox>* out);
+// Whether the rects of a quantising pull (each already checked by rect_boxes) write int8 (TSB_I8) rather than
+// float8_e4m3fn: TSB_ERR_INVALID when they mix the two, or for int8 with TSB_QUANT_UE8M0 (`ue8m0`).
+int quant_dst_int8(const tsb_rect_t* rects, uint64_t n, bool ue8m0, bool* int8);
 // rect_boxes for requantising pulls: float8_e4m3fn on both sides; a box's `src` / `row_stride` are the
 // source's fp8 bytes.
 int rect_requant_boxes(const tsb_rect_t& in, uint64_t index, const TargetGeom* targets, uint64_t n_targets,
@@ -422,6 +426,7 @@ struct SqLaunch {
   uint32_t* amax;  // n_groups words, cleared by the launch
   uint32_t n_bands, n_tiles, n_groups, stage_bytes;
   bool ue8m0;      // power-of-two scales (QuantPlan::ue8m0)
+  bool int8;       // int8 destinations (QuantPlan::int8)
 };
 int launch_scaled_fp8(const SqLaunch& l, cudaStream_t stream);
 

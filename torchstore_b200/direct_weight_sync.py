@@ -576,7 +576,9 @@ class DirectWeightSyncDest:
         self._scaled_plans = Plans()  # per-channel / per-tensor scaled fp8 names: likewise
         self._dequant_plans = Plans()  # names read from scaled fp8 handles into bf16/f16/f32: one dequantising plan per device
         self._requant_plans = Plans()  # scaled fp8 destinations read from scaled fp8 handles: one requantising plan per device
-        self._plan_key: tuple | None = None  # ({(name, scale keyword)}, requantize, scale_fmt, verbatim) of its pull
+        self._int8_block_plans = Plans()  # block-scaled int8 names: one quantising plan per destination device
+        self._int8_scaled_plans = Plans()  # per-channel / per-tensor scaled int8 names: likewise
+        self._plan_key: tuple | None = None  # ({(name, scale keyword)}, requantize, scale_fmt, verbatim, {int8 names})
         self._plan_scale_dicts: tuple | None = None  # the three scale dict objects of the last pull
         self.last_pull_ms: dict[int, float] = {}  # device -> kernel time of the last pull
 
@@ -668,10 +670,11 @@ class DirectWeightSyncDest:
     def _check_scales(all_handles, dest_state_dict, scales: dict[str, dict | None], *,
                       requantize: bool = False, verbatim: bool = False) -> dict[str, tuple]:
         """Validate the scale dicts of a pull (``{keyword: {name: scale}}``, keyword ``f"{granularity}_scales"``) ->
-        ``{name: (keyword, fp8 destination, scale, route)}``, route ``"quantise"``, ``"requantise"`` or
+        ``{name: (keyword, destination, scale, route)}``, route ``"quantise"``, ``"requantise"`` or
         ``"verbatim"``.  With ``requantize``, a name whose handles are all scaled fp8 sources of one granularity is
         accepted too, and requantised; with ``verbatim``, such a name of the destination's granularity is moved as
-        it is.  Raises before anything is compiled or launched."""
+        it is.  A float8_e4m3fn destination takes every route; an int8 destination only ``"quantise"``, from
+        bf16/f16/f32 handles.  Raises before anything is compiled or launched."""
         if requantize and verbatim:
             raise ValueError("requantize=True and verbatim=True are exclusive: verbatim=True moves scaled fp8 bytes and "
                              "scales as they are (same granularity, groups that line up), requantize=True re-rounds "
@@ -688,8 +691,8 @@ class DirectWeightSyncDest:
                 dest = getattr(dest_state_dict[name], "_local_tensor", dest_state_dict[name])
                 if not isinstance(scale, torch.Tensor):
                     raise TypeError(f"{what} of '{name}' is a {type(scale).__name__}, not a tensor")
-                if dest.dtype != torch.float8_e4m3fn:
-                    raise TypeError(f"{kind} destination '{name}' must be float8_e4m3fn, not {dest.dtype}")
+                if dest.dtype not in (torch.float8_e4m3fn, torch.int8):
+                    raise TypeError(f"{kind} destination '{name}' must be float8_e4m3fn or int8, not {dest.dtype}")
                 if dest.dim() < 2 or dest.numel() == 0 or not dest.is_contiguous() or not dest.is_cuda:
                     raise ValueError(f"{kind} destination '{name}' must be a non-empty contiguous CUDA tensor with at "
                                      f"least 2 dims; got shape {tuple(dest.shape)}, strides {dest.stride()} on {dest.device}")
@@ -704,8 +707,13 @@ class DirectWeightSyncDest:
                 if not handles:
                     raise ValueError(f"no source handles for {kind} destination '{name}': its groups would not be covered")
                 kinds = {getattr(h.rdma_buffer, "granularity", None) for h in handles}
+                int8 = dest.dtype == torch.int8
                 route = "quantise"
-                if requantize and kinds != {None}:
+                if int8 and kinds != {None}:
+                    raise TypeError(f"{kind} int8 destination '{name}' has scaled fp8 handles: int8 destinations are "
+                                    "quantised from bf16, f16 or f32 handles (scaled fp8 handles are neither "
+                                    "requantised nor moved verbatim into int8)")
+                if requantize and kinds != {None} and not int8:
                     route = "requantise"
                     if None in kinds:
                         raise ValueError(f"the handles of {kind} destination '{name}' mix scaled fp8 and unscaled sources "
@@ -713,7 +721,7 @@ class DirectWeightSyncDest:
                     if len(kinds) > 1:
                         raise ValueError(f"the handles of {kind} destination '{name}' mix scale granularities "
                                          f"{sorted(kinds)} (requantize=True)")
-                elif verbatim and kinds != {None}:
+                elif verbatim and kinds != {None} and not int8:
                     route = "verbatim"
                     if None in kinds:
                         raise TypeError(f"the handles of {kind} destination '{name}' mix scaled fp8 and unscaled sources "
@@ -728,7 +736,7 @@ class DirectWeightSyncDest:
                         hint = ""
                         if kinds - {None}:
                             hint = "; scaled fp8 handles are requantised only with requantize=True"
-                        elif requantize or verbatim:
+                        elif (requantize or verbatim) and not int8:
                             flag = "requantize" if requantize else "verbatim"
                             hint = f"; {flag}=True reads scaled fp8 handles (registered with a scale), not unscaled fp8"
                         raise TypeError(f"{kind} pulls of '{name}' read bf16, f16 or f32 handles of one dtype; "
@@ -804,14 +812,14 @@ class DirectWeightSyncDest:
     def _compile(self, scaled: dict | None = None, dequant: set | None = None, requant: set | None = None,
                  flags: int = 0, verbatim: dict | None = None) -> None:
         """Compile the cached transfer plan along the routes :meth:`_check_scales` chose: ``scaled`` is its
-        ``{name: (keyword, fp8 destination, scale, ...)}``, ``requant`` the names it requantises and ``verbatim``
+        ``{name: (keyword, destination, scale, ...)}``, ``requant`` the names it requantises and ``verbatim``
         :meth:`_verbatim_rects` of the names it moves as they are; ``dequant`` is what :meth:`_check_dequant`
         returned.  ``flags`` go to the quantising and requantising plans."""
         scaled, requant, verbatim = scaled or {}, requant or set(), verbatim or {}
-        # the plan kind of each quantised or requantised name, in build order: 0 requantises, 1 quantises into blocks,
-        # 2 into channels or tensors
-        kind = {n: 0 if n in requant else 1 if kw == "block_scales" else 2 for n, (kw, *_) in scaled.items()
-                if n not in verbatim}
+        # the plan kind of each quantised or requantised name, in build order: 0 requantises, 1 quantises into fp8
+        # blocks, 2 into fp8 channels or tensors, 3 and 4 the same into int8 (a plan writes one destination dtype)
+        kind = {n: 0 if n in requant else (1 if kw == "block_scales" else 2) + (2 if _is_int8(d) else 0)
+                for n, (kw, d, *_) in scaled.items() if n not in verbatim}
         per_device: dict[int, list] = defaultdict(list)
         # verbatim names: their fp8 bytes go with the plain copies below, their scales as float32 rectangles
         for n, rects in verbatim.items():
@@ -864,12 +872,13 @@ class DirectWeightSyncDest:
                 targets.append(_quant_target(kw.removesuffix("_scales"), d, s, n in requant))
 
             def pull_of(n):
-                kw = scaled[n][0]
+                kw, d = scaled[n][:2]
                 what = "requantising" if n in requant else f"{kw.removesuffix('_scales')}-scaled"
-                return f"{what} pull of '{n}' ({kw})"
+                return f"{what}{' int8' if _is_int8(d) else ''} pull of '{n}' ({kw})"
 
             builds = ((self._requant_plans, Plans.build_requant_fp8), (self._block_plans, Plans.build_block_fp8),
-                      (self._scaled_plans, Plans.build_scaled_fp8))
+                      (self._scaled_plans, Plans.build_scaled_fp8), (self._int8_block_plans, Plans.build_block_fp8),
+                      (self._int8_scaled_plans, Plans.build_scaled_fp8))
             for (k, dev), (pairs, sources, names, targets) in sorted(quant.items()):
                 plans, build = builds[k]
                 args, by_index = (pairs, targets), {"target": names}
@@ -886,8 +895,9 @@ class DirectWeightSyncDest:
 
     @property
     def _fp8_plans(self) -> tuple:
-        """The scaled fp8 plans in launch order (after the copy plan on each device's copy stream)."""
-        return self._block_plans, self._scaled_plans, self._dequant_plans, self._requant_plans
+        """The scaled fp8 and int8 plans in launch order (after the copy plan on each device's copy stream)."""
+        return (self._block_plans, self._scaled_plans, self._dequant_plans, self._requant_plans, self._int8_block_plans,
+                self._int8_scaled_plans)
 
     def plan_info(self) -> dict[int, dict]:
         return self._native_plans.info()
@@ -914,6 +924,14 @@ class DirectWeightSyncDest:
         ``lead`` is the destination's dims before the last two (MoE stacks quantise every matrix on its
         own).  The formula is in DESIGN.md section 4.  Every element of such a destination must be
         covered by the handles.  The other names are pulled as without scales.
+
+        Scaled int8 destinations (extension): a name of the three scale dicts whose destination is ``torch.int8``
+        is quantised the same way into symmetric int8 (W8A8-INT8 ``weight_scale`` per channel, one scale per
+        tensor, block-INT8 ``weight_scale_inv`` per 128x128 block): ``scale_inv = max(amax, 1e-4) / 127`` and
+        ``q = round_half_even(x * (127 / max(amax, 1e-4)))`` saturated to [-128, 127], NaN -> 0 (DESIGN.md
+        section 4, "INT8 destinations").  Only bf16/f16/f32 handles feed it: scaled fp8 handles raise TypeError
+        (with or without ``requantize`` / ``verbatim``), and ``scale_fmt`` raises ValueError.  An int8
+        destination outside the scale dicts is still moved as bytes.
 
         Scaled fp8 sources (extension): a name whose handles were registered with scales
         (``DirectWeightSyncSource.register(block_scales= / channel_scales= / tensor_scales=)``) and whose
@@ -954,7 +972,10 @@ class DirectWeightSyncDest:
         if scale_fmt is not None and not scaled_names:
             raise ValueError("scale_fmt applies to quantised and requantised names: block_scales, channel_scales or "
                              "tensor_scales must name at least one")
-        key = (scaled_names, bool(requantize), scale_fmt, bool(verbatim))
+        # a name whose destination turns from float8_e4m3fn into int8 (or back) at the same address needs other kernels
+        int8_names = frozenset(n for n, _ in scaled_names
+                               if _is_int8(getattr(dest_state_dict.get(n), "_local_tensor", dest_state_dict.get(n))))
+        key = (scaled_names, bool(requantize), scale_fmt, bool(verbatim), int8_names)
         if self._plan is not None and key != self._plan_key:
             logger.info("scaled names or their granularity changed; rebuilding the transfer plan")
             self.close()
@@ -985,6 +1006,9 @@ class DirectWeightSyncDest:
         if self._plan is None:
             scaled = self._check_scales(all_handles, dest_state_dict, scale_dicts, requantize=requantize,
                                         verbatim=verbatim)
+            if scale_fmt is not None and any(_is_int8(d) for _, d, *_ in scaled.values()):
+                raise ValueError("scale_fmt='ue8m0' does not apply to int8 destinations: their scales are float32 "
+                                 "amax / 127 (power-of-two int8 scales are not offered)")
             if scale_fmt is not None and all(route == "verbatim" for *_, route in scaled.values()):
                 raise ValueError("scale_fmt does nothing here: every name of block_scales, channel_scales and "
                                  "tensor_scales is moved verbatim and keeps its source's scales")
@@ -1054,6 +1078,11 @@ def _build_named(plans: Plans, build, per_device: dict, names: dict[str, list[st
                 if m:
                     raise ValueError(f"{pull_of(by_index[int(m.group(1))])}: {e}") from e
         raise
+
+
+def _is_int8(dest) -> bool:
+    """Whether a scaled destination (or None for a name the dict lacks) is quantised into int8."""
+    return getattr(dest, "dtype", None) == torch.int8
 
 
 def _add_dq_source(sources: dict, op: _TransferOp, dev: int) -> None:

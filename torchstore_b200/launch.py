@@ -105,22 +105,25 @@ class Plans(dict):
         return plans
 
     @classmethod
-    def _build_pulls(cls, create, per_device: dict[int, tuple], flags: int = 0) -> "Plans":
-        """build_fp8 of pulls: ``{device: ([(src, dst) StridedMem windows], *tables)}``, the windows as rects."""
-        return cls.build_fp8(create, {dev: (*build_rects(pairs), *tables) for dev, (pairs, *tables) in per_device.items()},
-                             flags)
+    def _build_pulls(cls, create, per_device: dict[int, tuple], flags: int = 0, quantise: bool = False) -> "Plans":
+        """build_fp8 of pulls: ``{device: ([(src, dst) StridedMem windows], *tables)}``, the windows as rects
+        (``quantise``: an int8 destination window is quantised, see :func:`build_rects`)."""
+        return cls.build_fp8(create, {dev: (*build_rects(pairs, quantise), *tables) for dev, (pairs, *tables) in
+                                      per_device.items()}, flags)
 
     @classmethod
     def build_block_fp8(cls, per_device: dict[int, tuple[list, list]], flags: int = 0) -> "Plans":
         """Compile block-scaled fp8 pulls: ``{device: ([(src, dst) StridedMem windows], [BqTarget])}``; ``flags``:
-        ``_native.TSB_QUANT_UE8M0`` for power-of-two scales, here and in the other quantising builders."""
-        return cls._build_pulls(_native.block_fp8_plan_create, per_device, flags)
+        ``_native.TSB_QUANT_UE8M0`` for power-of-two scales, here and in the other quantising builders.  Windows
+        into int8 destinations quantise into int8 (one plan writes one destination dtype), here and in
+        :meth:`build_scaled_fp8`."""
+        return cls._build_pulls(_native.block_fp8_plan_create, per_device, flags, quantise=True)
 
     @classmethod
     def build_scaled_fp8(cls, per_device: dict[int, tuple[list, list]], flags: int = 0) -> "Plans":
         """Compile per-channel / per-tensor scaled fp8 pulls: ``{device: ([(src, dst) StridedMem windows],
         [SqTarget])}``."""
-        return cls._build_pulls(_native.scaled_fp8_plan_create, per_device, flags)
+        return cls._build_pulls(_native.scaled_fp8_plan_create, per_device, flags, quantise=True)
 
     @classmethod
     def build_dequant_fp8(cls, per_device: dict[int, tuple[list, list]]) -> "Plans":

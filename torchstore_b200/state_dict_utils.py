@@ -92,7 +92,7 @@ async def get_state_dict(store, key, user_state_dict: dict | None = None, strict
                          verbatim: bool = False):
     """Fetch a state dict.  ``user_state_dict`` tensors are filled in place (and required in direct
     mode).  A missing mapping means no matching push finished: RuntimeError.  ``block_scales``
-    (direct mode only) names float8_e4m3fn destinations quantised into the 128x128 block-scaled
+    (direct mode only) names float8_e4m3fn (or int8) destinations quantised into the 128x128 block-scaled
     layout during the pull; ``channel_scales`` / ``tensor_scales`` likewise name destinations with one
     float32 scale per row / per matrix (see ``DirectWeightSyncDest.pull``).  ``requantize=True`` (direct
     mode only) lets such destinations be fed by scaled fp8 handles, re-rounding them into the destination's
