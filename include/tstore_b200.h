@@ -63,11 +63,13 @@ enum {
   TSB_I8 = 10,    /* int8, valid ONLY as the dst_dtype of the rects of tsb_block_fp8_* and tsb_scaled_fp8_*: the
                    * destination is quantised to symmetric int8 (see tsb_bq_target_t).  Every rect of one such plan
                    * writes one dtype, TSB_F8E4M3 or TSB_I8 (a mix is TSB_ERR_INVALID); TSB_I8 with TSB_QUANT_UE8M0
-                   * is TSB_ERR_INVALID.  The copy plan, the fused casts (tsb_cast_supported), the dequantising,
-                   * requantising and source-side calls refuse it; a plain int8 move is TSB_U8.  *_compile_host
-                   * returns the same tables for TSB_I8 rects as for TSB_F8E4M3 rects: the dtype selects the
-                   * kernels only.  Libraries that predate it refuse TSB_I8 rects with TSB_ERR_UNSUPPORTED, so
-                   * callers can detect it without an ABI version change. */
+                   * is TSB_ERR_INVALID.  Also valid as the src_dtype of the rects of tsb_dequant_fp8_* (an int8
+                   * source dequantised; one plan reads one source dtype) and as the dst_dtype of
+                   * tsb_source_quant_*_as (int8 staging).  The copy plan, the fused casts (tsb_cast_supported),
+                   * the requantising calls and the other sides refuse it; a plain int8 move is TSB_U8.
+                   * *_compile_host returns the same tables for TSB_I8 as for TSB_F8E4M3: the dtype selects the
+                   * kernels only.  Libraries that predate it refuse TSB_I8 rects with TSB_ERR_UNSUPPORTED (or
+                   * TSB_ERR_INVALID), so callers can detect it without an ABI version change. */
 };
 
 /* ------------------------------------------------------------------------------------------ */
@@ -307,13 +309,13 @@ int tsb_scaled_fp8_compile_host(int device, const tsb_rect_t* rects, uint64_t n,
                                 void* out_tiles, uint64_t tile_cap, uint64_t* out_n_tiles, uint64_t* out_n_groups);
 
 /* ------------------------------------------------------------------------------------------ */
-/* dequantising pulls: block-, channel- or tensor-scaled float8_e4m3fn sources into f32, bf16   */
-/* or f16 destinations                                                                          */
+/* dequantising pulls: block-, channel- or tensor-scaled float8_e4m3fn (or int8) sources into   */
+/* f32, bf16 or f16 destinations                                                                */
 /* ------------------------------------------------------------------------------------------ */
 
 enum { TSB_SCALE_PER_BLOCK = 3 };
 
-/* One scaled fp8 source shard: `batch` contiguous [rows, cols] float8_e4m3fn matrices whose first
+/* One scaled source shard: `batch` contiguous [rows, cols] float8_e4m3fn (or int8) matrices whose first
  * element sits at (row0, col0) of the global tensor's last two dims.  Scales are anchored at the
  * global origin (checkpoint semantics), and the scale tensor holds exactly the groups the shard
  * touches:
@@ -325,7 +327,7 @@ enum { TSB_SCALE_PER_BLOCK = 3 };
  * tensor; f32(q) is exact, the multiply one correctly rounded f32 multiply (no flush to zero), and
  * to_dst the fused cast's f32 -> bf16 / f16 narrowing (identity for f32). */
 typedef struct tsb_dq_source {
-  uint64_t src;         /* float8_e4m3fn as seen from the plan's device */
+  uint64_t src;         /* float8_e4m3fn or int8 (the rects' src_dtype) as seen from the plan's device */
   uint64_t scale;       /* float32, contiguous, as seen from the plan's device */
   uint64_t batch, rows, cols;
   uint64_t row0, col0;  /* global offset of the shard in the last two dims (the block phase) */
@@ -334,8 +336,9 @@ typedef struct tsb_dq_source {
 } tsb_dq_source_t;
 
 /* Compile a dequantising pull: `rects` are ordinary source -> destination rectangles with src_dtype
- * == TSB_F8E4M3, dst_dtype in {TSB_F32, TSB_BF16, TSB_F16} and src inside one source (TSB_ERR_INVALID
- * naming the rect or source otherwise).  Elements no rect reads are left alone.  The result is a plan
+ * == TSB_F8E4M3 or TSB_I8, dst_dtype in {TSB_F32, TSB_BF16, TSB_F16} and src inside one source (TSB_ERR_INVALID
+ * naming the rect or source otherwise).  Every rect of one plan reads one source dtype (a mix of TSB_F8E4M3 and
+ * TSB_I8 is TSB_ERR_INVALID); for TSB_I8, f32(q) is (float)(int8_t)q.  The tile table is the same for either.  Elements no rect reads are left alone.  The result is a plan
  * like any other.  flags: reserved, pass 0 (TSB_QUANT_UE8M0 is refused: a float32 scale dequantises the
  * same whatever its format). */
 int tsb_dequant_fp8_plan_create(int device, const tsb_rect_t* rects, uint64_t n, const tsb_dq_source_t* sources,
@@ -394,7 +397,7 @@ int tsb_requant_fp8_compile_host(int device, const tsb_rect_t* rects, uint64_t n
 
 /* ------------------------------------------------------------------------------------------ */
 /* source-side quantisation: a publisher refreshes block-, channel- or tensor-scaled           */
-/* float8_e4m3fn staging from its live bf16/f16/f32 shards                                      */
+/* float8_e4m3fn (or int8) staging from its live bf16/f16/f32 shards                            */
 /* ------------------------------------------------------------------------------------------ */
 
 /* One shard to quantise: `batch` contiguous [rows, cols] matrices of src_dtype at src, whose first element
@@ -406,7 +409,7 @@ int tsb_requant_fp8_compile_host(int device, const tsb_rect_t* rects, uint64_t n
  * scale_inv = amax_c / 448; a NaN poisons its group). */
 typedef struct tsb_source_quant_target {
   uint64_t src;         /* TSB_F32 / TSB_BF16 / TSB_F16, contiguous [batch, rows, cols], element-aligned */
-  uint64_t dst;         /* float8_e4m3fn, contiguous [batch, rows, cols] */
+  uint64_t dst;         /* float8_e4m3fn (int8 with tsb_source_quant_*_as(TSB_I8)), contiguous [batch, rows, cols] */
   uint64_t scale_inv;   /* float32, contiguous, one per group */
   uint64_t batch, rows, cols;
   uint64_t row0, col0;  /* global offset of the shard in the last two dims (the block phase) */
@@ -432,6 +435,17 @@ int tsb_source_quant_plan_create(int device, const tsb_source_quant_target_t* ta
 int tsb_source_quant_compile_host(int device, const tsb_source_quant_target_t* targets, uint64_t n, uint32_t flags,
                                   void* out_units, uint64_t unit_cap, uint64_t* out_n_units, void* out_tiles,
                                   uint64_t tile_cap, uint64_t* out_n_tiles, uint64_t* out_n_groups);
+/* The same two calls with the staging format named: dst_dtype TSB_F8E4M3 (exactly the calls above) or TSB_I8,
+ * symmetric int8 with the formula of tsb_bq_target_t's TSB_I8 rects (amax_c = max(amax, 1e-4f), scale_inv =
+ * amax_c / 127, dst = sat_s8(rne(rn(x * 127 / amax_c))), NaN -> 0; a NaN group gets a NaN scale, an Inf group an
+ * Inf scale, both all zeros).  Any other dst_dtype, and TSB_I8 with TSB_QUANT_UE8M0, is TSB_ERR_INVALID.  The
+ * tables do not depend on dst_dtype. */
+int tsb_source_quant_plan_create_as(int device, const tsb_source_quant_target_t* targets, uint64_t n, uint32_t dst_dtype,
+                                    uint32_t flags, tsb_plan_t* out);
+int tsb_source_quant_compile_host_as(int device, const tsb_source_quant_target_t* targets, uint64_t n,
+                                     uint32_t dst_dtype, uint32_t flags, void* out_units, uint64_t unit_cap,
+                                     uint64_t* out_n_units, void* out_tiles, uint64_t tile_cap, uint64_t* out_n_tiles,
+                                     uint64_t* out_n_groups);
 
 /* ------------------------------------------------------------------------------------------ */
 /* streams and events (the await points of the reference's coroutines)                         */

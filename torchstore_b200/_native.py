@@ -24,7 +24,8 @@ TSB_U8, TSB_U16, TSB_U32, TSB_U64, TSB_F16, TSB_BF16, TSB_F32, TSB_F64, TSB_F8E4
 TSB_H2D, TSB_D2H, TSB_D2D = 1, 2, 3
 TSB_PLAN_DEFAULT, TSB_PLAN_NO_INTERLEAVE = 0, 1
 TSB_QUANT_UE8M0 = 1  # flags of the quantising plan calls: power-of-two scales
-TSB_I8 = 10  # int8, only as the dst_dtype of a quantising pull's rects (tsb_block_fp8_*, tsb_scaled_fp8_*)
+TSB_I8 = 10  # int8: dst_dtype of a quantising pull's rects (tsb_block_fp8_*, tsb_scaled_fp8_*), src_dtype of a
+# dequantising pull's (tsb_dequant_fp8_*), dst_dtype of tsb_source_quant_*_as
 
 
 class TsbError(RuntimeError):
@@ -236,6 +237,14 @@ _SIGNATURES = {
         C.c_int,
         [C.c_int, C.POINTER(SourceQuantTarget), C.c_uint64, C.c_uint32, _vp, C.c_uint64, C.POINTER(C.c_uint64), _vp,
          C.c_uint64, C.POINTER(C.c_uint64), C.POINTER(C.c_uint64)],
+    ),
+    "tsb_source_quant_plan_create_as": (
+        C.c_int, [C.c_int, C.POINTER(SourceQuantTarget), C.c_uint64, C.c_uint32, C.c_uint32, C.POINTER(C.c_uint64)],
+    ),
+    "tsb_source_quant_compile_host_as": (
+        C.c_int,
+        [C.c_int, C.POINTER(SourceQuantTarget), C.c_uint64, C.c_uint32, C.c_uint32, _vp, C.c_uint64, C.POINTER(C.c_uint64),
+         _vp, C.c_uint64, C.POINTER(C.c_uint64), C.POINTER(C.c_uint64)],
     ),
     "tsb_stream_create": (C.c_int, [C.c_int, C.POINTER(_vp)]),
     "tsb_stream_destroy": (C.c_int, [_vp]),
@@ -609,8 +618,10 @@ def make_source_quant_target_array(n: int):
     return (SourceQuantTarget * n)()
 
 
-def source_quant_plan_create(device: int, targets: list, flags: int = 0) -> int:
-    return _plan_create(lib().tsb_source_quant_plan_create, device, *_structs(SourceQuantTarget, targets), flags=flags)
+def source_quant_plan_create(device: int, targets: list, flags: int = 0, dst_dtype: int = TSB_F8E4M3) -> int:
+    """``dst_dtype``: the staging format, TSB_F8E4M3 or TSB_I8 (tsb_source_quant_plan_create_as)."""
+    return _plan_create(lib().tsb_source_quant_plan_create_as, device, *_structs(SourceQuantTarget, targets), dst_dtype,
+                        flags=flags)
 
 
 # record layout of the units of tsb_source_quant_compile_host (include/tstore_b200.h); its tiles are SQ_TILE_DTYPE
@@ -618,11 +629,15 @@ SRCQ_UNIT_DTYPE = [("src", "<u8"), ("dst", "<u8"), ("scale_inv", "<u8"), ("src_p
                    ("rows", "<u4"), ("cols", "<u4"), ("per_row", "<u4"), ("src_dtype", "<u2"), ("vec", "<u2")]
 
 
-def source_quant_compile_host(device: int, targets, n: int, flags: int = 0):
+def source_quant_compile_host(device: int, targets, n: int, flags: int = 0, dst_dtype: int | None = None):
     """Host-only compilation of a source-side quantisation -> (units, tiles, n_groups): numpy record arrays and
-    the number of two-pass groups."""
-    return tuple(_compile_host(lib().tsb_source_quant_compile_host, (device, targets, n), [SRCQ_UNIT_DTYPE, SQ_TILE_DTYPE],
-                               True, flags))
+    the number of two-pass groups.  ``dst_dtype`` (TSB_F8E4M3 or TSB_I8) goes to tsb_source_quant_compile_host_as;
+    None calls tsb_source_quant_compile_host."""
+    if dst_dtype is None:
+        fn, args = lib().tsb_source_quant_compile_host, (device, targets, n)
+    else:
+        fn, args = lib().tsb_source_quant_compile_host_as, (device, targets, n, dst_dtype)
+    return tuple(_compile_host(fn, args, [SRCQ_UNIT_DTYPE, SQ_TILE_DTYPE], True, flags))
 
 
 CUDA_STREAM_LEGACY = 0x1  # cudaStreamLegacy: an explicit handle for the default stream

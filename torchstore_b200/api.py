@@ -160,12 +160,13 @@ async def put_state_dict(state_dict: dict[str, Any] | None, key: str, store_name
                          block_scales: "dict[str, torch.Tensor] | None" = None,
                          channel_scales: "dict[str, torch.Tensor] | None" = None,
                          tensor_scales: "dict[str, torch.Tensor] | None" = None,
-                         quantize: "dict[str, str] | None" = None, scale_fmt: "str | None" = None) -> None:
+                         quantize: "dict[str, str] | None" = None, scale_fmt: "str | None" = None, *,
+                         quant_dtype: "torch.dtype | None" = None) -> None:
     cl = await client(store_name)
     await state_dict_utils.put_state_dict(store=cl, state_dict=state_dict, key=key, direct_rdma=direct_rdma,
                                           transfer_dtype=transfer_dtype, block_scales=block_scales,
                                           channel_scales=channel_scales, tensor_scales=tensor_scales,
-                                          quantize=quantize, scale_fmt=scale_fmt)
+                                          quantize=quantize, scale_fmt=scale_fmt, quant_dtype=quant_dtype)
 
 
 async def get_state_dict(key: str, user_state_dict: dict[str, Any] | None = None, strict: bool = True,

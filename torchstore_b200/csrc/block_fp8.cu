@@ -198,7 +198,8 @@ int rect_source_boxes(const tsb_rect_t& in, uint64_t index, const TargetGeom* gr
                       std::vector<TargetBox>* out) {
   const std::string where = "rect " + std::to_string(index) + ": ";
   if (in.ndim < 1 || in.ndim > TSB_MAX_DIMS) return fail(TSB_ERR_INVALID, where + "ndim must be in [1, 6]");
-  if (in.src_dtype != TSB_F8E4M3) return fail(TSB_ERR_INVALID, where + "dequantising pulls read float8_e4m3fn sources");
+  if (in.src_dtype != TSB_F8E4M3 && in.src_dtype != TSB_I8)
+    return fail(TSB_ERR_INVALID, where + "dequantising pulls read float8_e4m3fn or int8 sources");
   const uint32_t es = quant_src_bytes(in.dst_dtype);
   if (!es) return fail(TSB_ERR_INVALID, where + "dequantising pulls write f32, bf16 or f16 destinations");
   return map_boxes(in, index, grids, n_grids, kBySrc, es, out);

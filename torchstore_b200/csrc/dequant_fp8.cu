@@ -1,6 +1,7 @@
-// Dequantising pulls (sm_90a, H100): gather block-, channel- or tensor-scaled float8_e4m3fn source
+// Dequantising pulls (sm_90a, H100): gather block-, channel- or tensor-scaled float8_e4m3fn or int8 source
 // rectangles into f32 / bf16 / f16 destinations, y = to_dst(f32(q) * scale), the torch rendering
-// (q.float() * s_expanded).to(dst) of DeepSeek's weight_dequant.
+// (q.float() * s_expanded).to(dst) of DeepSeek's weight_dequant.  One plan reads one source format; its
+// launch picks the kernel instantiation (E4m3In / I8In), the tables are the same for both.
 //
 // Host side: the plan compiler maps every rect's *source* onto its source shard's [batch, rows, cols]
 // grid (rect_source_boxes, block_fp8.cu), cuts the boxes at the scale groups (128x128 blocks anchored at
@@ -8,7 +9,7 @@
 // a tile carries the scale of its first row and the step to the next row's) and splits them into tiles of
 // at most kDqTileElems elements and kDqTileRows rows, so that a big shard spreads over every SM.
 // Device side: one 256-thread CTA per tile, streaming, no reduction and no shared-memory staging of data.
-// Each thread takes 16 fp8 elements per step, kUnroll steps in flight: one 16-byte load when the tile is
+// Each thread takes 16 fp8 (or int8) elements per step, kUnroll steps in flight: one 16-byte load when the tile is
 // aligned, widening (exact), one f32 multiply per element (__fmul_rn: round to nearest even, no flush to
 // zero), the fused cast's narrowing, then 32 B (bf16/f16) or 64 B (f32) of 16-byte stores.  A channel
 // tile's scales are staged in shared memory once per row; block and tensor tiles load their one scale.
@@ -106,10 +107,22 @@ template <> __device__ __forceinline__ uint32_t narrow_bits<TSB_F32>(float y) { 
 template <> __device__ __forceinline__ uint32_t narrow_bits<TSB_BF16>(float y) { return float_to_bf16_bits(y); }
 template <> __device__ __forceinline__ uint32_t narrow_bits<TSB_F16>(float y) { return __half_as_ushort(__float2half_rn(y)); }
 
-// one e4m3fn byte -> f32 (exact; NaN stays NaN)
-__device__ __forceinline__ float widen1(uint32_t byte) { return f16_bits_to_f32(fp8x2_to_f16x2<true>(byte) & 0xffffu); }
+// The source formats: the exact widening to f32 of one byte (widen1), and of the two bytes in bits 0..15 (pair,
+// then lo and hi of its result)
+struct E4m3In {  // float8_e4m3fn (TSB_F8E4M3): through f16, NaN stays NaN
+  static __device__ __forceinline__ uint32_t pair(uint32_t two) { return fp8x2_to_f16x2<true>(two); }
+  static __device__ __forceinline__ float lo(uint32_t p) { return f16_bits_to_f32(p & 0xffffu); }
+  static __device__ __forceinline__ float hi(uint32_t p) { return f16_bits_to_f32(p >> 16); }
+  static __device__ __forceinline__ float widen1(uint32_t byte) { return lo(pair(byte)); }
+};
+struct I8In {  // int8 (TSB_I8): (float)(int8_t)b
+  static __device__ __forceinline__ uint32_t pair(uint32_t two) { return two; }
+  static __device__ __forceinline__ float lo(uint32_t p) { return static_cast<float>(static_cast<int8_t>(p & 0xffu)); }
+  static __device__ __forceinline__ float hi(uint32_t p) { return static_cast<float>(static_cast<int8_t>((p >> 8) & 0xffu)); }
+  static __device__ __forceinline__ float widen1(uint32_t byte) { return lo(byte); }
+};
 
-template <uint32_t DT>
+template <uint32_t DT, class In>
 __device__ __forceinline__ void dequant_tile(const DqTile& t, const float* s_scale, float scale0) {
   constexpr uint32_t es = Src<DT>::kBytes;
   const char* src = reinterpret_cast<const char*>(t.src);
@@ -138,9 +151,9 @@ __device__ __forceinline__ void dequant_tile(const DqTile& t, const float* s_sca
         uint32_t o[4 * es];
 #pragma unroll
         for (uint32_t j = 0; j < 8; ++j) {  // element pairs (2j, 2j+1)
-          const uint32_t h2 = fp8x2_to_f16x2<true>(words[j >> 1] >> (16 * (j & 1)));
-          const uint32_t lo = narrow_bits<DT>(__fmul_rn(f16_bits_to_f32(h2 & 0xffffu), scale));
-          const uint32_t hi = narrow_bits<DT>(__fmul_rn(f16_bits_to_f32(h2 >> 16), scale));
+          const uint32_t h2 = In::pair(words[j >> 1] >> (16 * (j & 1)));
+          const uint32_t lo = narrow_bits<DT>(__fmul_rn(In::lo(h2), scale));
+          const uint32_t hi = narrow_bits<DT>(__fmul_rn(In::hi(h2), scale));
           if constexpr (es == 4) {
             o[2 * j] = lo;
             o[2 * j + 1] = hi;
@@ -156,7 +169,7 @@ __device__ __forceinline__ void dequant_tile(const DqTile& t, const float* s_sca
         const unsigned char* s = reinterpret_cast<const unsigned char*>(src + static_cast<int64_t>(r) * t.src_stride + c);
         const uint32_t nvalid = min(16u, t.cols - c);
         for (uint32_t j = 0; j < nvalid; ++j) {
-          const uint32_t y = narrow_bits<DT>(__fmul_rn(widen1(__ldg(s + j)), scale));
+          const uint32_t y = narrow_bits<DT>(__fmul_rn(In::widen1(__ldg(s + j)), scale));
           if constexpr (es == 4)
             *reinterpret_cast<uint32_t*>(d + 4 * j) = y;
           else
@@ -167,6 +180,8 @@ __device__ __forceinline__ void dequant_tile(const DqTile& t, const float* s_sca
   }
 }
 
+// In: the source format, E4m3In or I8In (one per plan)
+template <class In>
 __global__ void __launch_bounds__(kQuantThreads) dequant_fp8_kernel(const DqTile* __restrict__ tiles) {
   __shared__ float s_scale[kDqTileRows];
   const DqTile t = tiles[blockIdx.x];
@@ -179,10 +194,21 @@ __global__ void __launch_bounds__(kQuantThreads) dequant_fp8_kernel(const DqTile
     scale0 = __ldg(scales);
   }
   switch (t.dst_dtype) {
-    case TSB_BF16: dequant_tile<TSB_BF16>(t, s_scale, scale0); break;
-    case TSB_F16: dequant_tile<TSB_F16>(t, s_scale, scale0); break;
-    default: dequant_tile<TSB_F32>(t, s_scale, scale0); break;
+    case TSB_BF16: dequant_tile<TSB_BF16, In>(t, s_scale, scale0); break;
+    case TSB_F16: dequant_tile<TSB_F16, In>(t, s_scale, scale0); break;
+    default: dequant_tile<TSB_F32, In>(t, s_scale, scale0); break;
   }
+}
+
+// Whether the rects of a dequantising pull (each already checked by rect_source_boxes) read int8 (TSB_I8) rather
+// than float8_e4m3fn: TSB_ERR_INVALID when they mix the two.
+int dq_src_int8(const tsb_rect_t* rects, uint64_t n, bool* int8) {
+  *int8 = n && rects[0].src_dtype == TSB_I8;
+  for (uint64_t i = 1; i < n; ++i)
+    if ((rects[i].src_dtype == TSB_I8) != *int8)
+      return fail(TSB_ERR_INVALID, "rect " + std::to_string(i) + ": the rects of one plan read one source dtype, "
+                                   "float8_e4m3fn or int8");
+  return TSB_OK;
 }
 
 // d = DqTile table, one CTA per tile
@@ -190,13 +216,14 @@ int dequant_fp8_plan(int device, const tsb_rect_t* rects, uint64_t n, const tsb_
                      QuantPlan* q) {
   DqTables tb;
   int st = dequant_fp8_compile(device, rects, n, sources, n_sources, &tb);
-  if (st) return st;
+  if (st || (st = dq_src_int8(rects, n, &q->int8))) return st;
   q->add(tb.tiles);
   q->seal(0);
   const uint32_t n_tiles = static_cast<uint32_t>(tb.tiles.size());
   q->describe(n, n_tiles, kDqTileElems, tb);
-  q->launch = [n_tiles](char* d, cudaStream_t s) {
-    dequant_fp8_kernel<<<n_tiles, kQuantThreads, 0, s>>>(reinterpret_cast<const DqTile*>(d));
+  const auto kernel = q->int8 ? dequant_fp8_kernel<I8In> : dequant_fp8_kernel<E4m3In>;
+  q->launch = [n_tiles, kernel](char* d, cudaStream_t s) {
+    kernel<<<n_tiles, kQuantThreads, 0, s>>>(reinterpret_cast<const DqTile*>(d));
     return launched("dequant_fp8_kernel launch");
   };
   return TSB_OK;

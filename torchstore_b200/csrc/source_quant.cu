@@ -1,10 +1,11 @@
 // Source-side quantisation (sm_90a, H100): a publisher's refresh of block-, channel- or tensor-scaled
-// float8_e4m3fn staging from its live bf16/f16/f32 shards, the producer half of the scaled-FP8 weight sync.
+// float8_e4m3fn (or int8) staging from its live bf16/f16/f32 shards, the producer half of the scaled weight sync.
 //
 // Groups are shard-local and anchored at the global origin, the layout a scaled source handle describes
 // (tsb_dq_source_t): a block-scaled shard at global offset (row0, col0) has one group per global 128x128 block
 // it touches, cut to the shard, so an FSDP shard starting mid-block gets partial first and last block rows.
-// Per group the formula of the quantising pulls applies, from the same device helpers (fp8_quant.cuh).
+// Per group the formula of the quantising pulls applies, from the same device helpers (fp8_quant.cuh): the staging
+// format (E4m3Out / I8Out) picks the unit kernel (source_quant_kernel / source_int8_kernel) and the two-pass kernels.
 //
 // Host side: every target is cut into work in group order, with trivial addressing (a shard is one
 // contiguous tensor; there are no pieces):
@@ -183,12 +184,10 @@ __device__ __forceinline__ void widen_chunk(const uint32_t d[4 * Src<DT>::kBytes
   }
 }
 
-// kUe8m0: power-of-two scales (TSB_QUANT_UE8M0)
-template <uint32_t DT, bool kUe8m0>
-__global__ void __launch_bounds__(kQuantThreads) source_quant_kernel(const SrcQUnit* __restrict__ units) {
+// The CTA's unit in staging format Out (fp8_quant.cuh), the body of the unit kernels below
+template <uint32_t DT, class Out>
+__device__ __forceinline__ void quantise_unit(const SrcQUnit* __restrict__ units, uint32_t* s_amax, float* s_scale) {
   constexpr uint32_t es = Src<DT>::kBytes;
-  __shared__ uint32_t s_amax[kSqBandRows];
-  __shared__ float s_scale[kSqBandRows];
   const SrcQUnit u = units[blockIdx.x];
   const char* src = reinterpret_cast<const char*>(u.src);
   const uint32_t cpr = (u.cols + 15u) / 16u, total = u.rows * cpr;
@@ -238,7 +237,7 @@ __global__ void __launch_bounds__(kQuantThreads) source_quant_kernel(const SrcQU
   __syncthreads();
   for (uint32_t g = threadIdx.x; g < ng; g += kQuantThreads) {
     float scale, scale_inv;
-    group_scales<kUe8m0>(s_amax[g], &scale, &scale_inv);
+    Out::scales(s_amax[g], &scale, &scale_inv);
     s_scale[g] = scale;
     reinterpret_cast<float*>(u.scale_inv)[g] = scale_inv;
   }
@@ -250,35 +249,65 @@ __global__ void __launch_bounds__(kQuantThreads) source_quant_kernel(const SrcQU
       const uint32_t r = idx / cpr, c = (idx - r * cpr) * 16u;
       uint32_t f[16], o[4];
       widen_chunk<DT>(d[j], f);
-      narrow16(f, s_scale[u.per_row ? r : 0u], o);
+      Out::narrow(f, s_scale[u.per_row ? r : 0u], o);
       store16(reinterpret_cast<char*>(u.dst) + static_cast<uint64_t>(r) * u.dst_pitch + c, min(16u, u.cols - c), o);
     }
   }
 }
 
+// float8_e4m3fn staging; kUe8m0: power-of-two scales (TSB_QUANT_UE8M0)
+template <uint32_t DT, bool kUe8m0>
+__global__ void __launch_bounds__(kQuantThreads) source_quant_kernel(const SrcQUnit* __restrict__ units) {
+  __shared__ uint32_t s_amax[kSqBandRows];
+  __shared__ float s_scale[kSqBandRows];
+  quantise_unit<DT, E4m3Out<kUe8m0>>(units, s_amax, s_scale);
+}
+
+// int8 staging (TSB_I8).  Capped at the registers of its float8_e4m3fn twin: left alone, the int8 narrowing takes
+// 64 on 2-byte sources against the twin's 62, with no spill either way.
+template <uint32_t DT>
+__global__ void __maxnreg__(Src<DT>::kBytes == 4 ? 95 : 62) source_int8_kernel(const SrcQUnit* __restrict__ units) {
+  __shared__ uint32_t s_amax[kSqBandRows];
+  __shared__ float s_scale[kSqBandRows];
+  quantise_unit<DT, I8Out>(units, s_amax, s_scale);
+}
+
+// The staging format of `dst_dtype` in q->int8: TSB_ERR_INVALID unless TSB_F8E4M3 or TSB_I8, and for TSB_I8 with
+// TSB_QUANT_UE8M0 (q->ue8m0)
+int source_quant_dst(uint32_t dst_dtype, QuantPlan* q) {
+  if (dst_dtype != TSB_F8E4M3 && dst_dtype != TSB_I8)
+    return fail(TSB_ERR_INVALID, "source_quant: dst_dtype must be TSB_F8E4M3 or TSB_I8, not " + std::to_string(dst_dtype));
+  q->int8 = dst_dtype == TSB_I8;
+  if (q->int8 && q->ue8m0) return fail(TSB_ERR_INVALID, "source_quant: int8 staging takes float32 scales: TSB_QUANT_UE8M0 is refused");
+  return TSB_OK;
+}
+
 // d = {SrcQUnit table | SqTile table | amax words}: one launch per source dtype over its units, one CTA each, then
-// scaled_fp8.cu's two passes over the tiles
-int source_quant_plan(const tsb_source_quant_target_t* targets, uint64_t n, QuantPlan* q) {
+// scaled_fp8.cu's two passes over the tiles.  The tables do not depend on dst_dtype.
+int source_quant_plan(const tsb_source_quant_target_t* targets, uint64_t n, uint32_t dst_dtype, QuantPlan* q) {
   SrcQTables tb;
-  int st = source_quant_compile(targets, n, &tb);
-  if (st) return st;
+  int st = source_quant_dst(dst_dtype, q);
+  if (st || (st = source_quant_compile(targets, n, &tb))) return st;
   q->add(tb.units);
   const size_t tiles = q->add(tb.tiles), amax = q->seal(tb.n_groups);
   q->describe(n, static_cast<uint32_t>(tb.units.size() + tb.tiles.size()), tb.unit_bytes, tb);
-  const SqLaunch two_pass{nullptr, nullptr, nullptr, nullptr, 0, static_cast<uint32_t>(tb.tiles.size()), tb.n_groups, 0, q->ue8m0};
-  // the unit kernels by rank (bf16, f16, f32) and scale format
+  const SqLaunch two_pass{nullptr, nullptr, nullptr, nullptr, 0, static_cast<uint32_t>(tb.tiles.size()), tb.n_groups, 0, q->ue8m0,
+                          q->int8};
+  // the unit kernels by rank (bf16, f16, f32) and staging format
   using Kernel = void (*)(const SrcQUnit*);
   const std::array<Kernel, 3> kernels =
-      q->ue8m0 ? std::array<Kernel, 3>{source_quant_kernel<TSB_BF16, true>, source_quant_kernel<TSB_F16, true>, source_quant_kernel<TSB_F32, true>}
-               : std::array<Kernel, 3>{source_quant_kernel<TSB_BF16, false>, source_quant_kernel<TSB_F16, false>,
-                                       source_quant_kernel<TSB_F32, false>};
-  q->launch = [two_pass, tiles, amax, kernels, n_units = std::array<uint32_t, 3>{tb.n_units[0], tb.n_units[1], tb.n_units[2]}](char* d, cudaStream_t s) -> int {
+      q->int8    ? std::array<Kernel, 3>{source_int8_kernel<TSB_BF16>, source_int8_kernel<TSB_F16>, source_int8_kernel<TSB_F32>}
+      : q->ue8m0 ? std::array<Kernel, 3>{source_quant_kernel<TSB_BF16, true>, source_quant_kernel<TSB_F16, true>,
+                                         source_quant_kernel<TSB_F32, true>}
+                 : std::array<Kernel, 3>{source_quant_kernel<TSB_BF16, false>, source_quant_kernel<TSB_F16, false>,
+                                         source_quant_kernel<TSB_F32, false>};
+  q->launch = [two_pass, tiles, amax, kernels, int8 = q->int8, n_units = std::array<uint32_t, 3>{tb.n_units[0], tb.n_units[1], tb.n_units[2]}](char* d, cudaStream_t s) -> int {
     const SrcQUnit* units = reinterpret_cast<const SrcQUnit*>(d);
     for (int k = 0; k < 3; ++k) {
       const uint32_t n = n_units[k];
       if (!n) continue;
       kernels[k]<<<n, kQuantThreads, 0, s>>>(units);
-      if (int st = launched("source_quant_kernel launch")) return st;
+      if (int st = launched(int8 ? "source_int8_kernel launch" : "source_quant_kernel launch")) return st;
       units += n;
     }
     if (!two_pass.n_tiles) return TSB_OK;
@@ -296,17 +325,31 @@ int source_quant_plan(const tsb_source_quant_target_t* targets, uint64_t n, Quan
 
 using namespace tsb;
 
+extern "C" int tsb_source_quant_plan_create_as(int device, const tsb_source_quant_target_t* targets, uint64_t n,
+                                               uint32_t dst_dtype, uint32_t flags, tsb_plan_t* out) {
+  return quant_plan_create("tsb_source_quant_plan_create", device, flags, TSB_QUANT_UE8M0, out,
+                           [&](QuantPlan* q) { return source_quant_plan(targets, n, dst_dtype, q); });
+}
+
+extern "C" int tsb_source_quant_compile_host_as(int device, const tsb_source_quant_target_t* targets, uint64_t n,
+                                                uint32_t dst_dtype, uint32_t flags, void* out_units, uint64_t unit_cap,
+                                                uint64_t* out_n_units, void* out_tiles, uint64_t tile_cap,
+                                                uint64_t* out_n_tiles, uint64_t* out_n_groups) {
+  (void)device;
+  return quant_compile_host("tsb_source_quant_compile_host", flags, TSB_QUANT_UE8M0,
+                            [&](QuantPlan* q) { return source_quant_plan(targets, n, dst_dtype, q); },
+                            {{out_units, unit_cap, out_n_units, "out_units"}, {out_tiles, tile_cap, out_n_tiles, "out_tiles"}},
+                            out_n_groups);
+}
+
 extern "C" int tsb_source_quant_plan_create(int device, const tsb_source_quant_target_t* targets, uint64_t n, uint32_t flags,
                                             tsb_plan_t* out) {
-  return quant_plan_create("tsb_source_quant_plan_create", device, flags, TSB_QUANT_UE8M0, out,
-                           [&](QuantPlan* q) { return source_quant_plan(targets, n, q); });
+  return tsb_source_quant_plan_create_as(device, targets, n, TSB_F8E4M3, flags, out);
 }
 
 extern "C" int tsb_source_quant_compile_host(int device, const tsb_source_quant_target_t* targets, uint64_t n, uint32_t flags,
                                              void* out_units, uint64_t unit_cap, uint64_t* out_n_units, void* out_tiles,
                                              uint64_t tile_cap, uint64_t* out_n_tiles, uint64_t* out_n_groups) {
-  (void)device;
-  return quant_compile_host("tsb_source_quant_compile_host", flags, TSB_QUANT_UE8M0, [&](QuantPlan* q) { return source_quant_plan(targets, n, q); },
-                            {{out_units, unit_cap, out_n_units, "out_units"}, {out_tiles, tile_cap, out_n_tiles, "out_tiles"}},
-                            out_n_groups);
+  return tsb_source_quant_compile_host_as(device, targets, n, TSB_F8E4M3, flags, out_units, unit_cap, out_n_units, out_tiles,
+                                          tile_cap, out_n_tiles, out_n_groups);
 }

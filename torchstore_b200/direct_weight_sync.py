@@ -51,6 +51,7 @@ GRANULARITIES = {"block": _native.TSB_SCALE_PER_BLOCK, "channel": _native.TSB_SC
                  "tensor": _native.TSB_SCALE_PER_TENSOR}
 UNQUANTISED_DTYPES = {torch.bfloat16, torch.float16, torch.float32}  # what quantising routes read and dequantising writes
 SCALE_FORMATS = (None, "ue8m0")  # scale_fmt of the quantising routes: float32 amax / 448, or its power of two up
+SCALED_DTYPES = (torch.float8_e4m3fn, torch.int8)  # what a scaled handle holds, and quant_dtype's choices
 
 
 def scale_fmt_flags(scale_fmt: str | None) -> int:
@@ -138,11 +139,11 @@ class NvlinkBuffer:
 
 
 class ScaledNvlinkBuffer(NvlinkBuffer):
-    """An :class:`NvlinkBuffer` over a scaled ``float8_e4m3fn`` weight shard that also carries its
-    float32 scale (the dequantisation multiplier: ``weight_scale_inv`` per 128x128 block, ``weight_scale``
-    per channel or per tensor), the granularity, and the shard's global offset ``(row0, col0)`` in the last
+    """An :class:`NvlinkBuffer` over a scaled ``float8_e4m3fn`` or ``int8`` weight shard (its descriptor's dtype
+    says which) that also carries its float32 scale (the dequantisation multiplier: ``weight_scale_inv`` per
+    128x128 block, ``weight_scale`` per channel or per tensor), the granularity, and the shard's global offset ``(row0, col0)`` in the last
     two dims, which anchors the blocks at the global origin.  Pickles to plain data.  ``read_into`` /
-    ``write_from`` move the raw fp8 bytes; a pull into a bf16/f16/f32 destination dequantises."""
+    ``write_from`` move the raw fp8 (or int8) bytes; a pull into a bf16/f16/f32 destination dequantises."""
 
     def __init__(self, tensor: torch.Tensor | None = None, scale: torch.Tensor | None = None, granularity: str = "",
                  row0: int = 0, col0: int = 0, *, descriptor: HbmDescriptor | None = None,
@@ -318,7 +319,7 @@ class DirectWeightSyncSource:
         self._refresh_plans = Plans()
         self._copied: list[tuple[torch.Tensor, torch.Tensor]] = []  # (staging, source) refreshed with copy_
         self._devices: tuple[int, ...] = ()  # devices holding registered memory (fence targets)
-        # quantize= names: name -> (fp8 staging, float32 scale, source local tensor), refreshed by _quant_plans
+        # quantize= names: name -> (fp8 or int8 staging, float32 scale, source local tensor), refreshed by _quant_plans
         self._quantized: dict[str, tuple[torch.Tensor, torch.Tensor, torch.Tensor]] = {}
         self._quant_plans = Plans()
 
@@ -329,7 +330,8 @@ class DirectWeightSyncSource:
                  channel_scales: dict[str, torch.Tensor] | None = None,
                  tensor_scales: dict[str, torch.Tensor] | None = None,
                  quantize: dict[str, str] | None = None,
-                 scale_fmt: str | None = None) -> dict[str, RDMAWeightHandle]:
+                 scale_fmt: str | None = None,
+                 quant_dtype: torch.dtype | None = None) -> dict[str, RDMAWeightHandle]:
         """Create a handle for every entry of ``state_dict`` (tensors or DTensors).
 
         ``tensor_slices`` (extension) gives the global rectangle of *plain* local shards for
@@ -340,7 +342,10 @@ class DirectWeightSyncSource:
         or ``tensor_scales`` (one per matrix) is published with its scale, so that a pull into a bf16, f16
         or f32 destination dequantises it (DESIGN.md section 4).  Scales are anchored at the global
         origin: a shard at global offset (r0, c0) of its last two dims carries exactly the groups it
-        touches (:func:`source_scale_shapes`).  Such weights are registered zero-copy.
+        touches (:func:`source_scale_shapes`).  Such weights are registered zero-copy.  An ``int8`` weight
+        (W8A8-INT8 ``weight_scale`` per channel or per tensor, block-INT8 ``weight_scale_inv``) is published the
+        same way: a pull dequantises it into bf16/f16/f32 as ``(q.float() * scale).to(dst)``, moves it verbatim
+        into a scaled int8 destination, or moves its bytes into an unscaled int8 one.
 
         Source-side quantisation (extension): ``quantize={name: "block" | "channel" | "tensor"}`` publishes a
         bf16, f16 or f32 weight (at least 2 dims, contiguous, on CUDA) as float8_e4m3fn staging plus a float32
@@ -351,12 +356,25 @@ class DirectWeightSyncSource:
         requantises the staging from the live weights; ``transfer_dtype`` does not apply to these names.
         ``scale_fmt="ue8m0"`` rounds every such scale up to a power of two (DESIGN.md section 4, "UE8M0 scales");
         the scales stay float32, so every consumer of scaled handles reads them unchanged.
+        ``quant_dtype=torch.int8`` publishes int8 staging instead (``None`` or ``torch.float8_e4m3fn``: fp8): per
+        group ``scale_inv = max(amax, 1e-4) / 127`` and ``q = round_half_even(x * (127 / max(amax, 1e-4)))``
+        saturated to [-128, 127], NaN -> 0 (DESIGN.md section 4, "INT8 sources").  ValueError without
+        ``quantize``, for another dtype, and together with ``scale_fmt``.
 
         Everything is validated before anything is exported, so a failed call registers nothing."""
         scale_dicts = {"block_scales": block_scales, "channel_scales": channel_scales, "tensor_scales": tensor_scales}
         quant_flags = scale_fmt_flags(scale_fmt)
         if scale_fmt is not None and not quantize:
             raise ValueError("scale_fmt applies to source-side quantisation: it needs quantize")
+        if quant_dtype is not None:
+            if not quantize:
+                raise ValueError("quant_dtype applies to source-side quantisation: it needs quantize")
+            if not isinstance(quant_dtype, torch.dtype) or quant_dtype not in SCALED_DTYPES:
+                raise ValueError(f"quant_dtype must be None, torch.float8_e4m3fn or torch.int8, not {quant_dtype!r}")
+            if quant_dtype == torch.int8 and scale_fmt is not None:
+                raise ValueError("scale_fmt='ue8m0' does not apply to int8 staging: its scales are float32 amax / 127 "
+                                 "(power-of-two int8 scales are not offered)")
+        staging_dtype = quant_dtype or torch.float8_e4m3fn
         quantize = self._check_quantize(state_dict, tensor_slices, quantize or {}, scale_dicts)
         scaled = self._check_source_scales(state_dict, transfer_dtype, tensor_slices, scale_dicts)
         handles: dict[str, RDMAWeightHandle] = {}
@@ -384,15 +402,15 @@ class DirectWeightSyncSource:
             if name in quantize:
                 granularity = quantize[name]
                 r0, c0 = _last_two_offsets(tslice)
-                fp8 = torch.empty(local.shape, dtype=torch.float8_e4m3fn, device=local.device)
+                qbuf = torch.empty(local.shape, dtype=staging_dtype, device=local.device)
                 scale = torch.empty(source_scale_shapes(granularity, tuple(local.shape), r0, c0)[0], dtype=torch.float32,
                                     device=local.device)
                 rows, cols = local.shape[-2:]
                 quant_targets[local.device.index].append(_native.SourceQuantTarget(
-                    local.data_ptr(), fp8.data_ptr(), scale.data_ptr(), local.numel() // (rows * cols), rows, cols, r0, c0,
+                    local.data_ptr(), qbuf.data_ptr(), scale.data_ptr(), local.numel() // (rows * cols), rows, cols, r0, c0,
                     _native.cast_code(local.dtype), GRANULARITIES[granularity]))
-                self._quantized[name] = (fp8, scale, local)
-                handles[name] = RDMAWeightHandle(rdma_buffer=ScaledNvlinkBuffer(fp8, scale, granularity, r0, c0),
+                self._quantized[name] = (qbuf, scale, local)
+                handles[name] = RDMAWeightHandle(rdma_buffer=ScaledNvlinkBuffer(qbuf, scale, granularity, r0, c0),
                                                  tensor_slice=tslice, source_rank=rank)
                 continue
             if transfer_dtype is not None:
@@ -413,15 +431,16 @@ class DirectWeightSyncSource:
             if casts:
                 self._refresh_plans = Plans.build(casts)
             if quant_targets:
-                self._quant_plans = Plans.build_source_quant(quant_targets, quant_flags)
+                self._quant_plans = Plans.build_source_quant(
+                    quant_targets, quant_flags, _native.TSB_I8 if staging_dtype == torch.int8 else _native.TSB_F8E4M3)
             self.refresh()
         else:
             # make sure the weights the handles point at are materialised before anyone reads them
             for dev in devices:
                 torch.cuda.current_stream(dev).synchronize()
         staged = len(self._staging) + len(self._quantized)
-        logger.info("Registered %d NVLink handles (%d staged, %d quantised into scaled fp8, %d direct)", len(handles),
-                    staged, len(self._quantized), len(handles) - staged)
+        logger.info("Registered %d NVLink handles (%d staged, %d quantised into scaled %s, %d direct)", len(handles),
+                    staged, len(self._quantized), "int8" if staging_dtype == torch.int8 else "fp8", len(handles) - staged)
         return handles
 
     @staticmethod
@@ -447,8 +466,8 @@ class DirectWeightSyncSource:
             for name, scale in (by_name or {}).items():
                 req = Request.from_any(name, state_dict[name], tensor_slices.get(name) if tensor_slices else None)
                 w = req.tensor_val
-                if w.dtype != torch.float8_e4m3fn:
-                    raise TypeError(f"scaled weight '{name}' ({kw}) must be float8_e4m3fn, not {w.dtype}")
+                if w.dtype not in SCALED_DTYPES:
+                    raise TypeError(f"scaled weight '{name}' ({kw}) must be float8_e4m3fn or int8, not {w.dtype}")
                 if w.dim() < 2 or w.numel() == 0 or not w.is_contiguous() or not w.is_cuda:
                     raise ValueError(f"scaled weight '{name}' must be a non-empty contiguous CUDA tensor with at least "
                                      f"2 dims; got shape {tuple(w.shape)}, strides {w.stride()} on {w.device}")
@@ -498,7 +517,7 @@ class DirectWeightSyncSource:
 
     def refresh(self) -> int:
         """Re-cast the source params into their staging buffers and requantise the ``quantize`` names into
-        their scaled fp8 staging (no-op without either).  Returns the number of staging buffers refreshed.
+        their scaled fp8 (or int8) staging (no-op without either).  Returns the number of staging buffers refreshed.
         Blocks until everything has landed so the caller may publish/notify right after, like the
         reference's synchronous copy loop."""
         if not self._staging and not self._quantized:
@@ -578,6 +597,7 @@ class DirectWeightSyncDest:
         self._requant_plans = Plans()  # scaled fp8 destinations read from scaled fp8 handles: one requantising plan per device
         self._int8_block_plans = Plans()  # block-scaled int8 names: one quantising plan per destination device
         self._int8_scaled_plans = Plans()  # per-channel / per-tensor scaled int8 names: likewise
+        self._int8_dequant_plans = Plans()  # names read from scaled int8 handles into bf16/f16/f32: one plan per device
         self._plan_key: tuple | None = None  # ({(name, scale keyword)}, requantize, scale_fmt, verbatim, {int8 names})
         self._plan_scale_dicts: tuple | None = None  # the three scale dict objects of the last pull
         self.last_pull_ms: dict[int, float] = {}  # device -> kernel time of the last pull
@@ -673,8 +693,9 @@ class DirectWeightSyncDest:
         ``{name: (keyword, destination, scale, route)}``, route ``"quantise"``, ``"requantise"`` or
         ``"verbatim"``.  With ``requantize``, a name whose handles are all scaled fp8 sources of one granularity is
         accepted too, and requantised; with ``verbatim``, such a name of the destination's granularity is moved as
-        it is.  A float8_e4m3fn destination takes every route; an int8 destination only ``"quantise"``, from
-        bf16/f16/f32 handles.  Raises before anything is compiled or launched."""
+        it is.  A float8_e4m3fn destination takes every route; an int8 destination ``"quantise"`` from bf16/f16/f32
+        handles, and ``"verbatim"`` (``verbatim=True`` only) from scaled int8 handles, which no other route reads.
+        Raises before anything is compiled or launched."""
         if requantize and verbatim:
             raise ValueError("requantize=True and verbatim=True are exclusive: verbatim=True moves scaled fp8 bytes and "
                              "scales as they are (same granularity, groups that line up), requantize=True re-rounds "
@@ -708,6 +729,10 @@ class DirectWeightSyncDest:
                     raise ValueError(f"no source handles for {kind} destination '{name}': its groups would not be covered")
                 kinds = {getattr(h.rdma_buffer, "granularity", None) for h in handles}
                 int8 = dest.dtype == torch.int8
+                if torch.int8 in _scaled_dtypes(handles):
+                    out[name] = (kw, dest, scale, _int8_source_route(name, kind, granularity, dest, handles, kinds,
+                                                                     requantize, verbatim))
+                    continue
                 route = "quantise"
                 if int8 and kinds != {None}:
                     raise TypeError(f"{kind} int8 destination '{name}' has scaled fp8 handles: int8 destinations are "
@@ -782,23 +807,34 @@ class DirectWeightSyncDest:
 
     @staticmethod
     def _check_dequant(all_handles, dest_state_dict, scaled_dests) -> set[str]:
-        """Names whose handles are scaled fp8 sources and whose destination is bf16/f16/f32: the
-        dequantising plan.  A float8_e4m3fn destination gets the plain byte move.  Raises before anything
-        is compiled or launched."""
+        """Names whose handles are scaled fp8 (or scaled int8) sources and whose destination is bf16/f16/f32: the
+        dequantising plans.  A float8_e4m3fn destination of fp8 handles, or an int8 destination of int8 handles,
+        gets the plain byte move.  Raises before anything is compiled or launched."""
         out = set()
         for name, param in dest_state_dict.items():
             handles = all_handles.get(name) or []
             kinds = {getattr(h.rdma_buffer, "granularity", None) for h in handles}
             if not handles or kinds == {None}:
                 continue
+            dtypes = _scaled_dtypes(handles)
+            if len(dtypes) > 1:
+                raise ValueError(f"the handles of '{name}' mix scaled int8 and scaled fp8 sources")
+            fmt = "int8" if torch.int8 in dtypes else "fp8"
             if None in kinds:
-                raise ValueError(f"the handles of '{name}' mix scaled fp8 and unscaled sources")
+                raise ValueError(f"the handles of '{name}' mix scaled {fmt} and unscaled sources")
             if len(kinds) > 1:
                 raise ValueError(f"the handles of '{name}' mix scale granularities {sorted(kinds)}")
             if name in scaled_dests:
                 continue  # a scaled destination: _check_scales refuses fp8 handles with its TypeError
             dest = getattr(param, "_local_tensor", param)
-            if dest.dtype == torch.float8_e4m3fn:
+            if fmt == "int8":
+                if dest.dtype == torch.int8:
+                    continue
+                if dest.dtype not in UNQUANTISED_DTYPES:
+                    raise TypeError(f"'{name}' has {kinds.pop()}-scaled int8 handles: its destination must be bfloat16, "
+                                    f"float16, float32 (dequantised) or int8 (bytes moved), not {dest.dtype}; int8 is not "
+                                    "converted to fp8")
+            elif dest.dtype == torch.float8_e4m3fn:
                 continue
             if dest.dtype not in UNQUANTISED_DTYPES:
                 raise TypeError(f"'{name}' has {kinds.pop()}-scaled fp8 handles: its destination must be bfloat16, "
@@ -831,7 +867,8 @@ class DirectWeightSyncDest:
                 buf = op.rdma_buffer
                 src = _as_grid(buf.scale_window(dev), scale_grid(granularity, tuple(buf.shape), buf.row0, buf.col0))
                 per_device[dev].append((src.sub(src_idx), dst.sub(dst_idx)))
-        dq: dict[int, tuple[list, dict]] = {}  # device -> (windows, {source buffer id: (name, DqSource)})
+        # (int8 sources, device) -> (windows, {source buffer id: (name, DqSource)}): a plan reads one source format
+        dq: dict[tuple, tuple[list, dict]] = {}
         quant: dict[tuple, tuple] = defaultdict(lambda: ([], {}, [], []))  # (kind, device) -> the same, names, targets
         for op in self._plan:
             dest = op.dest_local
@@ -852,16 +889,16 @@ class DirectWeightSyncDest:
                 if kind[op.name] == 0:
                     _add_dq_source(sources, op, dev)
             elif dequant and op.name in dequant:
-                pairs, sources = dq.setdefault(dev, ([], {}))
+                pairs, sources = dq.setdefault((op.rdma_buffer.dtype == torch.int8, dev), ([], {}))
                 pairs.append(window)
                 _add_dq_source(sources, op, dev)
             else:
                 per_device[dev].append(window)
         self._native_plans = Plans.build(per_device)
         try:
-            for dev, (pairs, sources) in dq.items():
+            for (int8_src, dev), (pairs, sources) in sorted(dq.items()):
                 names = [n for n, _ in sources.values()]
-                _build_named(self._dequant_plans, Plans.build_dequant_fp8,
+                _build_named(self._int8_dequant_plans if int8_src else self._dequant_plans, Plans.build_dequant_fp8,
                              {dev: (pairs, [s for _, s in sources.values()])}, {"source": names},
                              lambda n: f"dequantising pull of '{n}'")
             for n, (kw, d, s, *_) in scaled.items():
@@ -897,7 +934,7 @@ class DirectWeightSyncDest:
     def _fp8_plans(self) -> tuple:
         """The scaled fp8 and int8 plans in launch order (after the copy plan on each device's copy stream)."""
         return (self._block_plans, self._scaled_plans, self._dequant_plans, self._requant_plans, self._int8_block_plans,
-                self._int8_scaled_plans)
+                self._int8_scaled_plans, self._int8_dequant_plans)
 
     def plan_info(self) -> dict[int, dict]:
         return self._native_plans.info()
@@ -960,6 +997,15 @@ class DirectWeightSyncDest:
         group that does not, for handles of another granularity, for an element covered by no handle or by two,
         with ``requantize=True``, and for a ``scale_fmt`` when every scaled name is verbatim.  Names fed by
         bf16/f16/f32 handles are still quantised.  Changing it rebuilds the plan.
+
+        Scaled int8 sources (extension): handles registered as int8 with a scale (``register(block_scales= /
+        channel_scales= / tensor_scales=)`` of an int8 weight, or ``quantize=`` with ``quant_dtype=torch.int8``)
+        are dequantised into a bf16/f16/f32 destination, ``(q.float() * scale).to(dst)``, and moved as raw bytes
+        into an int8 destination outside the scale dicts.  An int8 destination in a scale dict takes them only with
+        ``verbatim=True`` (the verbatim rule above, bytes and scales as they are); without it, with
+        ``requantize=True`` (int8 handles are not requantised), and into any float8_e4m3fn destination they raise
+        TypeError.  A name whose handles mix scaled int8 and scaled fp8 sources raises ValueError (DESIGN.md section
+        4, "INT8 sources").
 
         Steady state costs one native call to launch and a poll loop: the cached plan is checked
         against the destination OBJECTS first (their ids; the plan keeps them alive), the kernel
@@ -1078,6 +1124,34 @@ def _build_named(plans: Plans, build, per_device: dict, names: dict[str, list[st
                 if m:
                     raise ValueError(f"{pull_of(by_index[int(m.group(1))])}: {e}") from e
         raise
+
+
+def _scaled_dtypes(handles) -> set:
+    """The dtypes of the scaled handles (:class:`ScaledNvlinkBuffer`) among ``handles``."""
+    return {h.rdma_buffer.dtype for h in handles if getattr(h.rdma_buffer, "granularity", None) is not None}
+
+
+def _int8_source_route(name: str, kind: str, granularity: str, dest, handles, kinds: set, requantize: bool,
+                       verbatim: bool) -> str:
+    """:meth:`DirectWeightSyncDest._check_scales`' verdict on a scaled destination fed by scaled int8 handles: only
+    ``"verbatim"`` into int8 of the destination's granularity; every other case raises."""
+    if len(_scaled_dtypes(handles)) > 1:
+        raise ValueError(f"the handles of {kind} destination '{name}' mix scaled int8 and scaled fp8 sources")
+    if None in kinds:
+        raise ValueError(f"the handles of {kind} destination '{name}' mix scaled int8 and unscaled sources")
+    if dest.dtype != torch.int8:
+        raise TypeError(f"{kind} {dest.dtype} destination '{name}' has scaled int8 handles: int8 is not converted to "
+                        "fp8 (int8 handles are dequantised into bf16, f16 or f32, or moved into int8)")
+    if requantize:
+        raise TypeError(f"{kind} int8 destination '{name}' has scaled int8 handles: int8 handles are not requantised; "
+                        "verbatim=True moves their bytes and scales as they are")
+    if not verbatim:
+        raise TypeError(f"{kind} int8 destination '{name}' has scaled int8 handles: pass verbatim=True to move their "
+                        "bytes and scales as they are (int8 destinations are quantised from bf16, f16 or f32 handles)")
+    if kinds != {granularity}:
+        raise ValueError(f"{kind} destination '{name}' has {'/'.join(sorted(kinds))}-scaled int8 handles: a verbatim "
+                         "pull moves scales of the destination's granularity only")
+    return "verbatim"
 
 
 def _is_int8(dest) -> bool:

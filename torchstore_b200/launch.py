@@ -105,10 +105,12 @@ class Plans(dict):
         return plans
 
     @classmethod
-    def _build_pulls(cls, create, per_device: dict[int, tuple], flags: int = 0, quantise: bool = False) -> "Plans":
+    def _build_pulls(cls, create, per_device: dict[int, tuple], flags: int = 0, quantise: bool = False,
+                     dequantise: bool = False) -> "Plans":
         """build_fp8 of pulls: ``{device: ([(src, dst) StridedMem windows], *tables)}``, the windows as rects
-        (``quantise``: an int8 destination window is quantised, see :func:`build_rects`)."""
-        return cls.build_fp8(create, {dev: (*build_rects(pairs, quantise), *tables) for dev, (pairs, *tables) in
+        (``quantise``: an int8 destination window is quantised; ``dequantise``: an int8 source window is
+        dequantised; see :func:`build_rects`)."""
+        return cls.build_fp8(create, {dev: (*build_rects(pairs, quantise, dequantise), *tables) for dev, (pairs, *tables) in
                                       per_device.items()}, flags)
 
     @classmethod
@@ -127,9 +129,9 @@ class Plans(dict):
 
     @classmethod
     def build_dequant_fp8(cls, per_device: dict[int, tuple[list, list]]) -> "Plans":
-        """Compile dequantising pulls of scaled fp8 sources: ``{device: ([(src, dst) StridedMem windows],
-        [DqSource])}``."""
-        return cls._build_pulls(_native.dequant_fp8_plan_create, per_device)
+        """Compile dequantising pulls of scaled fp8 (or int8) sources: ``{device: ([(src, dst) StridedMem windows],
+        [DqSource])}``; one plan reads one source format."""
+        return cls._build_pulls(_native.dequant_fp8_plan_create, per_device, dequantise=True)
 
     @classmethod
     def build_requant_fp8(cls, per_device: dict[int, tuple[list, list, list]], flags: int = 0) -> "Plans":
@@ -138,10 +140,14 @@ class Plans(dict):
         return cls._build_pulls(_native.requant_fp8_plan_create, per_device, flags)
 
     @classmethod
-    def build_source_quant(cls, per_device: dict[int, list], flags: int = 0) -> "Plans":
-        """Compile source-side quantisations: ``{device: [SourceQuantTarget]}``."""
-        return cls.build_fp8(_native.source_quant_plan_create, {dev: (targets,) for dev, targets in per_device.items()},
-                             flags)
+    def build_source_quant(cls, per_device: dict[int, list], flags: int = 0,
+                           dst_dtype: int = _native.TSB_F8E4M3) -> "Plans":
+        """Compile source-side quantisations: ``{device: [SourceQuantTarget]}`` into ``dst_dtype`` staging
+        (``_native.TSB_F8E4M3`` or ``_native.TSB_I8``)."""
+        def create(dev, targets, flags):
+            return _native.source_quant_plan_create(dev, targets, flags, dst_dtype)
+
+        return cls.build_fp8(create, {dev: (targets,) for dev, targets in per_device.items()}, flags)
 
     def launch(self, fence_out: bool = True) -> None:
         """Enqueue every plan on its device's copy stream, fenced in against the caller's current

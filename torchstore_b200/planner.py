@@ -96,14 +96,21 @@ def _collapse(shape, sstride, dstride):
     return out
 
 
-def fill_rect(rect: "_native.Rect", src: StridedMem, dst: StridedMem, quantise: bool = False) -> bool:
+_FLOATS = (torch.bfloat16, torch.float16, torch.float32)
+
+
+def fill_rect(rect: "_native.Rect", src: StridedMem, dst: StridedMem, quantise: bool = False,
+              dequantise: bool = False) -> bool:
     """Fill a tsb_rect_t moving window ``src`` onto window ``dst`` (same shape; dtypes may differ
     when the pair is a supported cast).  Returns False for an empty window (nothing to move).
-    ``quantise``: the window feeds a quantising plan, where a bf16/f16/f32 -> int8 window is TSB_I8."""
+    ``quantise``: the window feeds a quantising plan, where a bf16/f16/f32 -> int8 window is TSB_I8 on its
+    destination side; ``dequantise``: a dequantising plan, where an int8 -> bf16/f16/f32 window is TSB_I8 on
+    its source side."""
     if tuple(src.shape) != tuple(dst.shape):
         raise ValueError(f"source window {src.shape} and destination window {dst.shape} differ")
-    int8 = quantise and dst.dtype == torch.int8 and src.dtype in (torch.bfloat16, torch.float16, torch.float32)
-    if src.dtype != dst.dtype and not int8 and not _native.cast_supported(src.dtype, dst.dtype):
+    int8 = quantise and dst.dtype == torch.int8 and src.dtype in _FLOATS
+    int8_src = dequantise and src.dtype == torch.int8 and dst.dtype in _FLOATS
+    if src.dtype != dst.dtype and not int8 and not int8_src and not _native.cast_supported(src.dtype, dst.dtype):
         raise NotImplementedError(f"no fused cast kernel for {src.dtype} -> {dst.dtype}")
     if any(e == 0 for e in src.shape):
         return False
@@ -130,19 +137,19 @@ def fill_rect(rect: "_native.Rect", src: StridedMem, dst: StridedMem, quantise: 
             raise NotImplementedError("16-byte elements are not supported")
         rect.src_dtype = rect.dst_dtype = code
     else:
-        rect.src_dtype = _native.cast_code(src.dtype)
+        rect.src_dtype = _native.TSB_I8 if int8_src else _native.cast_code(src.dtype)
         rect.dst_dtype = _native.TSB_I8 if int8 else _native.cast_code(dst.dtype)
     rect.src_device = src.device
     return True
 
 
-def build_rects(pairs: Sequence[tuple[StridedMem, StridedMem]], quantise: bool = False):
-    """(src, dst) windows -> (ctypes array of tsb_rect_t, count).  Empty windows are skipped.  ``quantise``: as
-    for :func:`fill_rect`."""
+def build_rects(pairs: Sequence[tuple[StridedMem, StridedMem]], quantise: bool = False, dequantise: bool = False):
+    """(src, dst) windows -> (ctypes array of tsb_rect_t, count).  Empty windows are skipped.  ``quantise``,
+    ``dequantise``: as for :func:`fill_rect`."""
     arr = _native.make_rect_array(max(1, len(pairs)))
     n = 0
     for src, dst in pairs:
-        if fill_rect(arr[n], src, dst, quantise):
+        if fill_rect(arr[n], src, dst, quantise, dequantise):
             n += 1
     return arr, n
 

@@ -59,21 +59,25 @@ def reset_direct_cache(store=None) -> None:
 
 async def put_state_dict(store, state_dict, key, direct_rdma=False, transfer_dtype=None, block_scales: dict | None = None,
                          channel_scales: dict | None = None, tensor_scales: dict | None = None,
-                         quantize: dict | None = None, scale_fmt: str | None = None):
+                         quantize: dict | None = None, scale_fmt: str | None = None, *, quant_dtype=None):
     """Store every leaf of ``state_dict`` (one batched put), then the mapping as the commit marker.
 
     With ``direct_rdma=True`` only handles to the caller's HBM are published on the first call;
     later calls refresh dtype-cast staging (``state_dict`` may then be None).  ``transfer_dtype``
     applies to direct mode only.  ``block_scales`` / ``channel_scales`` / ``tensor_scales`` (direct mode
-    only, first call) publish float8_e4m3fn weights with their scales, so that pulls into bf16/f16/f32
+    only, first call) publish float8_e4m3fn or int8 weights with their scales, so that pulls into bf16/f16/f32
     destinations dequantise them (see ``DirectWeightSyncSource.register``).  ``quantize`` (direct mode only,
     first call) names bf16/f16/f32 weights published as block-, channel- or tensor-scaled fp8 staging that
-    later calls requantise from the live weights; ``scale_fmt="ue8m0"`` gives that staging power-of-two scales."""
+    later calls requantise from the live weights; ``scale_fmt="ue8m0"`` gives that staging power-of-two scales,
+    ``quant_dtype=torch.int8`` makes it int8 staging."""
     if direct_rdma:
         await _put_state_dict_direct_rdma(store, state_dict, key, transfer_dtype,
                                           dict(block_scales=block_scales, channel_scales=channel_scales,
-                                               tensor_scales=tensor_scales, quantize=quantize, scale_fmt=scale_fmt))
+                                               tensor_scales=tensor_scales, quantize=quantize, scale_fmt=scale_fmt,
+                                               quant_dtype=quant_dtype))
         return
+    if quant_dtype is not None:
+        raise NotImplementedError("quant_dtype needs direct_rdma=True: the store path does not quantise")
     if scale_fmt is not None:
         raise NotImplementedError("scale_fmt needs direct_rdma=True: the store path does not quantise")
     if quantize:
