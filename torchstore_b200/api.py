@@ -175,9 +175,9 @@ async def get_state_dict(key: str, user_state_dict: dict[str, Any] | None = None
                          channel_scales: "dict[str, torch.Tensor] | None" = None,
                          tensor_scales: "dict[str, torch.Tensor] | None" = None,
                          requantize: bool = False, scale_fmt: "str | None" = None,
-                         verbatim: bool = False) -> dict[str, Any]:
+                         verbatim: bool = False, *, packed: "dict[str, tuple] | None" = None) -> dict[str, Any]:
     cl = await client(store_name)
     return await state_dict_utils.get_state_dict(cl, key, user_state_dict, strict, direct_rdma=direct_rdma,
                                                  block_scales=block_scales, channel_scales=channel_scales,
                                                  tensor_scales=tensor_scales, requantize=requantize,
-                                                 scale_fmt=scale_fmt, verbatim=verbatim)
+                                                 scale_fmt=scale_fmt, verbatim=verbatim, packed=packed)

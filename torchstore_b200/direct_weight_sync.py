@@ -28,6 +28,7 @@ Typical usage is unchanged::
 
 from __future__ import annotations
 
+import itertools
 import logging
 import math
 import re
@@ -199,13 +200,16 @@ def scale_grid(granularity: str, shape: tuple, row0: int, col0: int) -> tuple:
     return source_scale_shapes(granularity, shape, row0, col0)[0]
 
 
-def verbatim_scale_rects(granularity: str, shape: tuple, offset: tuple, ops: list) -> tuple[list, tuple | None]:
+def verbatim_scale_rects(granularity: str, shape: tuple, offset: tuple, ops: list, *,
+                         src_starts: list | None = None) -> tuple[list, tuple | None]:
     """Map the scales of a verbatim pull: fp8 bytes and scales of same-granularity sources moved as they are.
 
     ``shape`` and ``offset`` are the destination's local shape and global offset (all dims); each op is
     ``(source shard shape, source shard global offset, (global offset, extent) of the op's rectangle)``.
     Destination groups are anchored at the destination's local origin (128x128 blocks, rows, or the matrix
-    per leading index); source groups at the global origin, cut by the source shard.
+    per leading index); source groups at the global origin, cut by the source shard.  ``src_starts`` (packed
+    destinations) gives, per op, the source's global coordinates of the rectangle's first element, where they
+    differ from the destination's; without it the two coordinate systems are the same.
 
     Returns ``(rects, None)`` when every destination group lies inside one source group of one op:
     ``rects[i] = (op index, source index, destination index)``, unit-step slices into the :func:`scale_grid`
@@ -224,12 +228,13 @@ def verbatim_scale_rects(granularity: str, shape: tuple, offset: tuple, ops: lis
         size, src_size = size + [1, cols], src_size + [1, None]
     else:
         size, src_size = size + [rows, cols], src_size + [None, None]
+    starts = src_starts if src_starts is not None else [g_off for _, _, (g_off, _) in ops]
     local = []  # op rectangles in destination-local coordinates: [(start, stop) per dim]
     volume = 0
-    for src_shape, src_off, (g_off, ext) in ops:
+    for (src_shape, src_off, (g_off, ext)), sg in zip(ops, starts):
         box = [(g - o, g - o + e) for g, o, e in zip(g_off, offset, ext)]
         if any(s < 0 or t > n or s >= t for (s, t), n in zip(box, shape)) or \
-                any(g < so or g + e > so + n for g, e, so, n in zip(g_off, ext, src_off, src_shape)):
+                any(g < so or g + e > so + n for g, e, so, n in zip(sg, ext, src_off, src_shape)):
             raise ValueError(f"op rectangle at {tuple(g_off)} extent {tuple(ext)} is empty or leaves its source shard "
                              "or the destination")
         local.append(box)
@@ -256,24 +261,49 @@ def verbatim_scale_rects(granularity: str, shape: tuple, offset: tuple, ops: lis
     for d in range(lead, nd):  # a group across a source group edge (only 128-blocks have such edges)
         if src_size[d] is None:
             continue
-        for j in range(-(-shape[d] // size[d])):
-            s, t = offset[d] + j * size[d], offset[d] + min((j + 1) * size[d], shape[d])
-            if s // src_size[d] != (t - 1) // src_size[d]:
-                bad.append(tuple(j if e == d else 0 for e in range(nd)))
-                break
+        if src_starts is None:
+            for j in range(-(-shape[d] // size[d])):
+                s, t = offset[d] + j * size[d], offset[d] + min((j + 1) * size[d], shape[d])
+                if s // src_size[d] != (t - 1) // src_size[d]:
+                    bad.append(tuple(j if e == d else 0 for e in range(nd)))
+                    break
+            continue
+        for box, sg in zip(local, starts):  # packed: each op's own shift between the two coordinate systems
+            s0, t0 = box[d]
+            for j in range(*groups(d, s0, t0)):
+                s, t = sg[d] + max(s0, j * size[d]) - s0, sg[d] + min(t0, (j + 1) * size[d]) - s0
+                if s // src_size[d] != (t - 1) // src_size[d]:
+                    bad.append(tuple(j if e == d else groups(e, *box[e])[0] for e in range(nd)))
+                    break
     if bad:
         return [], min(bad)
     rects = []
-    for i, (box, (_, src_off, _)) in enumerate(zip(local, ops)):
+    for i, (box, (_, src_off, _), sg) in enumerate(zip(local, ops, starts)):
         src_idx, dst_idx = [], []
         for d, (s, t) in enumerate(box):
             j0, j1 = groups(d, s, t)
-            g0 = offset[d] + j0 * size[d]  # global start of the first group
+            g0 = sg[d] - s + j0 * size[d]  # global start of the first group, in the source's coordinates
             k0 = 0 if src_size[d] is None else g0 // src_size[d] - src_off[d] // src_size[d]
             src_idx.append(slice(k0, k0 + j1 - j0))
             dst_idx.append(slice(j0, j1))
         rects.append((i, tuple(src_idx), tuple(dst_idx)))
     return rects, None
+
+
+@dataclass(frozen=True)
+class PackedPart:
+    """One part of a packed (fused) destination, such as vLLM's ``qkv_proj`` or an expert of ``w13_weight``.
+
+    ``dest_index`` is a tuple of ints and unit-step slices into the destination's *local* tensor, one entry per
+    dim; the box it selects is what the part fills, and an int entry drops its dim.  The box is read from the
+    handles named ``source``, starting at global offsets ``source_offsets`` of the source tensor (one per source
+    dim: the box's rank after the int entries are dropped).  Each element at local index ``i`` of the box takes
+    the source's value at ``source_offsets + (i - box start)``, through the route the destination's dtype and
+    scale dicts select (DESIGN.md section 4, "Packed destinations")."""
+
+    source: str
+    dest_index: tuple
+    source_offsets: tuple
 
 
 @dataclass
@@ -575,6 +605,10 @@ class _TransferOp:
     dest_local: torch.Tensor | None = None
     dest_offsets: tuple = ()  # global offsets of the destination shard and of the source shard
     src_offsets: tuple = ()
+    # packed parts: the source's global coordinates of the op's first element (None: the destination's global
+    # coordinates are the source's), and the destination dims an int index dropped (unit slices in dest_slices)
+    src_start: tuple | None = None
+    dest_dropped: tuple = ()
 
 
 class DirectWeightSyncDest:
@@ -598,21 +632,33 @@ class DirectWeightSyncDest:
         self._int8_block_plans = Plans()  # block-scaled int8 names: one quantising plan per destination device
         self._int8_scaled_plans = Plans()  # per-channel / per-tensor scaled int8 names: likewise
         self._int8_dequant_plans = Plans()  # names read from scaled int8 handles into bf16/f16/f32: one plan per device
-        self._plan_key: tuple | None = None  # ({(name, scale keyword)}, requantize, scale_fmt, verbatim, {int8 names})
+        # ({(name, scale keyword)}, requantize, scale_fmt, verbatim, {int8 names}, packed spec)
+        self._plan_key: tuple | None = None
+        self._packed_last: tuple | None = None  # (packed dict, its items, its key) of the last pull (_packed_spec)
         self._plan_scale_dicts: tuple | None = None  # the three scale dict objects of the last pull
         self.last_pull_ms: dict[int, float] = {}  # device -> kernel time of the last pull
 
     # -- planning (host, metadata only) ----------------------------------------------------------
     def _build_plan(self, all_handles: dict[str, list[RDMAWeightHandle]],
                     dest_state_dict: dict[str, torch.Tensor],
-                    dest_slices: dict[str, TensorSlice] | None = None) -> list[_TransferOp]:
+                    dest_slices: dict[str, TensorSlice] | None = None, *,
+                    packed: dict[str, tuple[PackedPart, ...]] | None = None) -> list[_TransferOp]:
         """Per destination param x per source handle: intersect, dedup replicated regions, classify
         exact / partial (same rules and op order as the reference, :221-317).
 
         ``dest_slices`` (extension) names the rectangle a *plain* local tensor holds, for callers
-        that keep raw shards instead of DTensors (e.g. torchrun ranks)."""
+        that keep raw shards instead of DTensors (e.g. torchrun ranks).  ``packed`` (extension) fills the
+        named destinations part by part (:meth:`_check_packed`): per part x per handle of its source, the
+        intersection with the part's source box becomes one partial op in the destination's local
+        coordinates."""
+        parts = self._check_packed(all_handles, dest_state_dict, packed)
         ops: list[_TransferOp] = []
         for name, param in dest_state_dict.items():
+            if name in parts:
+                dest_req = Request.from_any(name, param, dest_slices.get(name) if dest_slices else None)
+                ops += _packed_ops(name, dest_req.tensor_val, tuple(_request_to_slice(dest_req, param).offsets),
+                                   parts[name])
+                continue
             handles = all_handles.get(name)
             if not handles:
                 continue
@@ -666,7 +712,52 @@ class DirectWeightSyncDest:
             if tuple(src.shape) != tuple(dst_full.shape):
                 src = StridedMem(src.ptr, dst_full.shape, _contig(dst_full.shape), src.dtype, src.device)
             return src, dst_full
-        return src_window.sub(op.src_slices), dst_full.sub(op.dest_slices)
+        src, dst = src_window.sub(op.src_slices), dst_full.sub(op.dest_slices)
+        if op.dest_dropped:  # a packed part whose int index dropped destination dims: unit dims on the source side
+            src = StridedMem(src.ptr, dst.shape, _lift(src.stride, op.dest_dropped, 0), src.dtype, src.device)
+        return src, dst
+
+    @staticmethod
+    def _check_packed(all_handles, dest_state_dict, packed: dict | None) -> dict[str, list]:
+        """Validate the ``packed`` spec of a pull -> ``{name: [(part index, part, box, dropped dims, handles)]}``,
+        ``box`` the part's ``(start, stop)`` in every destination-local dim (``(i, i + 1)`` where an int index
+        drops the dim).  Raises ValueError naming the destination and the part before anything is compiled."""
+        out: dict[str, list] = {}
+        for name, spec in (packed or {}).items():
+            if name not in dest_state_dict:
+                raise ValueError(f"packed names '{name}', which is not in the destination state dict")
+            if all_handles.get(name):
+                raise ValueError(f"packed destination '{name}' also has handles of its own name: a packed destination "
+                                 "is filled from its parts only")
+            dest = getattr(dest_state_dict[name], "_local_tensor", dest_state_dict[name])
+            entries = []
+            for k, part in enumerate(spec):
+                what = f"packed destination '{name}' part {k} (source '{part.source}')"
+                handles = all_handles.get(part.source) or []
+                if not handles:
+                    raise ValueError(f"{what}: the source has no handles")
+                box, dropped = _index_box(what, part.dest_index, tuple(dest.shape))
+                ext = [t - s for d, (s, t) in enumerate(box) if d not in dropped]
+                gshape = tuple(handles[0].tensor_slice.global_shape)
+                offs = tuple(part.source_offsets)
+                if len(ext) != len(gshape) or len(offs) != len(gshape):
+                    raise ValueError(f"{what}: a {len(ext)}-dim box with {len(offs)} source offsets does not match "
+                                     f"the source's {len(gshape)}-dim global shape {gshape}")
+                if not all(isinstance(o, int) and not isinstance(o, bool) for o in offs):
+                    raise ValueError(f"{what}: source_offsets {offs} must be ints")
+                if any(o < 0 or o + e > g for o, e, g in zip(offs, ext, gshape)):
+                    raise ValueError(f"{what}: the source box at {offs} with extent {tuple(ext)} leaves the source's "
+                                     f"global shape {gshape}")
+                for j, _, other, _, _ in entries:
+                    if all(max(s, a) < min(t, b) for (s, t), (a, b) in zip(box, other)):
+                        raise ValueError(f"{what}: its box overlaps part {j}'s")
+                hole = _first_uncovered(offs, ext, [(tuple(h.tensor_slice.offsets), tuple(h.tensor_slice.local_shape))
+                                                    for h in handles])
+                if hole is not None:
+                    raise ValueError(f"{what}: no handle covers global element {hole} of the source")
+                entries.append((k, part, box, dropped, handles))
+            out[name] = entries
+        return out
 
     @staticmethod
     def _signature(dest_state_dict, scales: tuple = ()) -> tuple:
@@ -785,14 +876,20 @@ class DirectWeightSyncDest:
             if not mine:
                 raise ValueError(f"verbatim pull of '{name}' ({kw}): no handle covers its destination")
             shape, offset = tuple(dest.shape), mine[0].dest_offsets
-            rects = []
+            rects, starts = [], []
             for op in mine:
                 start = [0] * len(shape) if op.dest_slices is None else [s.start for s in op.dest_slices]
                 ext = shape if op.dest_slices is None else [s.stop - s.start for s in op.dest_slices]
-                rects.append((tuple(op.rdma_buffer.shape), op.src_offsets,
-                              (tuple(o + s for o, s in zip(offset, start)), tuple(ext))))
+                src_shape, src_off = tuple(op.rdma_buffer.shape), op.src_offsets
+                if op.src_start is not None:  # a packed part: the source in the destination's rank
+                    if any(d >= len(shape) - 2 for d in op.dest_dropped):
+                        raise ValueError(f"verbatim pull of '{name}' ({kw}): a packed part whose int index drops one "
+                                         "of the destination's last two dims cannot keep its source's scale groups")
+                    src_shape, src_off = _lift(src_shape, op.dest_dropped, 1), _lift(src_off, op.dest_dropped, 0)
+                    starts.append(_lift(op.src_start, op.dest_dropped, 0))
+                rects.append((src_shape, src_off, (tuple(o + s for o, s in zip(offset, start)), tuple(ext))))
             try:
-                mapped, group = verbatim_scale_rects(granularity, shape, offset, rects)
+                mapped, group = verbatim_scale_rects(granularity, shape, offset, rects, src_starts=starts or None)
             except ValueError as e:
                 raise ValueError(f"verbatim pull of '{name}' ({kw}): {e}") from None
             if group is not None:
@@ -865,7 +962,8 @@ class DirectWeightSyncDest:
             dst = _as_grid(dst, scale_grid(granularity, tuple(dest_q.shape), 0, 0))
             for op, src_idx, dst_idx in rects:
                 buf = op.rdma_buffer
-                src = _as_grid(buf.scale_window(dev), scale_grid(granularity, tuple(buf.shape), buf.row0, buf.col0))
+                grid = _lift(scale_grid(granularity, tuple(buf.shape), buf.row0, buf.col0), op.dest_dropped, 1)
+                src = _as_grid(buf.scale_window(dev), grid)
                 per_device[dev].append((src.sub(src_idx), dst.sub(dst_idx)))
         # (int8 sources, device) -> (windows, {source buffer id: (name, DqSource)}): a plan reads one source format
         dq: dict[tuple, tuple[list, dict]] = {}
@@ -946,9 +1044,21 @@ class DirectWeightSyncDest:
                    block_scales: dict[str, torch.Tensor] | None = None,
                    channel_scales: dict[str, torch.Tensor] | None = None,
                    tensor_scales: dict[str, torch.Tensor] | None = None, requantize: bool = False,
-                   scale_fmt: str | None = None, verbatim: bool = False) -> None:
+                   scale_fmt: str | None = None, verbatim: bool = False,
+                   packed: dict[str, tuple[PackedPart, ...]] | None = None) -> None:
         """Pull every overlapping region into ``dest_state_dict`` (in place).  Returns when the
         bytes are in destination HBM (so the caller may tell the source it is done reading).
+
+        Packed destinations (extension): ``packed={name: (PackedPart, ...)}`` fills a fused generator parameter
+        (``qkv_proj``, ``gate_up_proj``, a stacked MoE ``w13_weight``) from handles of other names, part by part
+        (:class:`PackedPart`); values must be tuples (TypeError otherwise).  A packed name takes no handles of its
+        own name.  Every route below applies unchanged: element-wise routes per element, with the scale of the
+        handle each byte is read from; grouped routes (quantising, requantising, verbatim) over the destination's
+        local groups whichever part an element came from, and their route checks over the union of the parts'
+        handles.  ValueError naming the destination and part, before anything is compiled, for an unknown name,
+        a source without handles, a name with handles of its own, a bad index, a source box outside the source,
+        overlapping parts and a part the handles do not cover (DESIGN.md section 4, "Packed destinations").
+        Elements outside every part are left alone.  Changing the spec rebuilds the plan.
 
         Scaled fp8 destinations (extension): float8_e4m3fn weights quantised during the pull from
         bf16/f16/f32 handles, each name in at most one of
@@ -1021,7 +1131,7 @@ class DirectWeightSyncDest:
         # a name whose destination turns from float8_e4m3fn into int8 (or back) at the same address needs other kernels
         int8_names = frozenset(n for n, _ in scaled_names
                                if _is_int8(getattr(dest_state_dict.get(n), "_local_tensor", dest_state_dict.get(n))))
-        key = (scaled_names, bool(requantize), scale_fmt, bool(verbatim), int8_names)
+        key = (scaled_names, bool(requantize), scale_fmt, bool(verbatim), int8_names, self._packed_spec(packed))
         if self._plan is not None and key != self._plan_key:
             logger.info("scaled names or their granularity changed; rebuilding the transfer plan")
             self.close()
@@ -1050,7 +1160,8 @@ class DirectWeightSyncDest:
                 self._plan_scale_dicts = scales
             verified = True
         if self._plan is None:
-            scaled = self._check_scales(all_handles, dest_state_dict, scale_dicts, requantize=requantize,
+            route_handles = _route_handles(all_handles, self._check_packed(all_handles, dest_state_dict, packed))
+            scaled = self._check_scales(route_handles, dest_state_dict, scale_dicts, requantize=requantize,
                                         verbatim=verbatim)
             if scale_fmt is not None and any(_is_int8(d) for _, d, *_ in scaled.values()):
                 raise ValueError("scale_fmt='ue8m0' does not apply to int8 destinations: their scales are float32 "
@@ -1058,9 +1169,9 @@ class DirectWeightSyncDest:
             if scale_fmt is not None and all(route == "verbatim" for *_, route in scaled.values()):
                 raise ValueError("scale_fmt does nothing here: every name of block_scales, channel_scales and "
                                  "tensor_scales is moved verbatim and keeps its source's scales")
-            dequant = self._check_dequant(all_handles, dest_state_dict, scaled)
+            dequant = self._check_dequant(route_handles, dest_state_dict, scaled)
             requant = {n for n, (*_, route) in scaled.items() if route == "requantise"}
-            self._plan = self._build_plan(all_handles, dest_state_dict, dest_slices)
+            self._plan = self._build_plan(all_handles, dest_state_dict, dest_slices, packed=packed)
             try:
                 verbatim_rects = self._verbatim_rects(self._plan, scaled)
                 self._compile(scaled, dequant, requant, flags, verbatim_rects)
@@ -1081,7 +1192,19 @@ class DirectWeightSyncDest:
             self.close()
             await self.pull(all_handles, dest_state_dict, dest_slices, block_scales=block_scales,
                             channel_scales=channel_scales, tensor_scales=tensor_scales, requantize=requantize,
-                            scale_fmt=scale_fmt, verbatim=verbatim)
+                            scale_fmt=scale_fmt, verbatim=verbatim, packed=packed)
+
+    def _packed_spec(self, packed: dict | None) -> frozenset | None:
+        """The plan-key entry of ``packed`` (:func:`_packed_key`).  The dict object of the previous pull, with the same
+        names mapped to the very same tuples, reuses its key without looking at a single part (the tuples are kept
+        alive, so their ids cannot be recycled)."""
+        last = self._packed_last
+        if packed and last is not None and packed is last[0] and len(packed) == len(last[1]) and \
+                all(n == m and v is w for (n, v), (m, w) in zip(packed.items(), last[1])):
+            return last[2]
+        key = _packed_key(packed)
+        self._packed_last = (packed, tuple(packed.items()), key) if packed else None
+        return key
 
     def launch(self) -> None:
         """Enqueue the cached plan on each device's copy stream, fenced against the caller's current
@@ -1177,6 +1300,109 @@ def _quant_target(granularity: str, dest: torch.Tensor, scale: torch.Tensor, req
     if granularity == "block" and not requant:
         return _native.BqTarget(*args)
     return _native.SqTarget(*args, GRANULARITIES[granularity], 0)
+
+
+def _packed_key(packed: dict | None) -> frozenset | None:
+    """The content of a ``packed`` spec as a plan-key entry (None without packed names).  TypeError unless every
+    value is a tuple of :class:`PackedPart` whose index and offsets are tuples: immutable values are what lets a
+    later pull with the same dict trust the ids of its values."""
+    if not packed:
+        return None
+    if not isinstance(packed, dict):
+        raise TypeError(f"packed must be a dict of name -> tuple of PackedPart, not {type(packed).__name__}")
+    out = []
+    for name, parts in packed.items():
+        if not isinstance(parts, tuple) or not all(isinstance(p, PackedPart) for p in parts):
+            raise TypeError(f"packed['{name}'] must be a tuple of PackedPart, not {type(parts).__name__}: the cached "
+                            "plan recognises an unchanged spec by the identity of these (immutable) tuples")
+        for p in parts:
+            if not isinstance(p.dest_index, tuple) or not isinstance(p.source_offsets, tuple):
+                raise TypeError(f"packed['{name}']: dest_index and source_offsets of a PackedPart must be tuples")
+        out.append((name, tuple((p.source, tuple((e.start, e.stop, e.step) if isinstance(e, slice) else e
+                                                 for e in p.dest_index), p.source_offsets) for p in parts)))
+    return frozenset(out)
+
+
+def _index_box(what: str, index: tuple, shape: tuple) -> tuple[list, tuple]:
+    """``(box, dropped dims)`` of a packed part's ``dest_index`` into a destination of local ``shape``."""
+    if len(index) != len(shape):
+        raise ValueError(f"{what}: dest_index has {len(index)} entries for a {len(shape)}-dim destination")
+    box, dropped = [], []
+    for d, (e, n) in enumerate(zip(index, shape)):
+        if isinstance(e, int) and not isinstance(e, bool):
+            if not 0 <= e < n:
+                raise ValueError(f"{what}: dest_index entry {d} ({e}) is out of range for extent {n}")
+            box.append((e, e + 1))
+            dropped.append(d)
+        elif isinstance(e, slice):
+            if e.step not in (None, 1):
+                raise ValueError(f"{what}: dest_index entry {d} ({e}) has a non-unit step")
+            s, t = 0 if e.start is None else e.start, n if e.stop is None else e.stop
+            if not (isinstance(s, int) and isinstance(t, int) and 0 <= s < t <= n):
+                raise ValueError(f"{what}: dest_index entry {d} ({e}) is out of range (or empty) for extent {n}")
+            box.append((s, t))
+        else:
+            raise ValueError(f"{what}: dest_index entry {d} is a {type(e).__name__}, not an int or a slice")
+    return box, tuple(dropped)
+
+
+def _first_uncovered(lo: tuple, ext: list, boxes: list) -> tuple | None:
+    """The lexicographically first global element of the box ``lo + [0, ext)`` outside every ``(offsets, shape)``
+    box, or None.  The boxes' edges cut it into cells that are covered or not as a whole, so that element is the
+    low corner of the first uncovered cell."""
+    hi = [a + e for a, e in zip(lo, ext)]
+    cuts = [sorted({a, b} | {min(max(v, a), b) for bo, bs in boxes for v in (bo[d], bo[d] + bs[d])})
+            for d, (a, b) in enumerate(zip(lo, hi))]
+    for corner in itertools.product(*(c[:-1] for c in cuts)):
+        if not any(all(o <= c < o + s for c, o, s in zip(corner, bo, bs)) for bo, bs in boxes):
+            return tuple(corner)
+    return None
+
+
+def _packed_ops(name: str, dest: torch.Tensor, dest_offsets: tuple, entries: list) -> list[_TransferOp]:
+    """The ops of one packed destination (:meth:`DirectWeightSyncDest._check_packed` ``entries``): per part, per
+    handle of its source (replicated regions read once), the intersection of the handle with the part's source
+    box, placed in the destination's local coordinates."""
+    ops = []
+    nd = dest.dim()
+    for _, part, box, dropped, handles in entries:
+        kept = [d for d in range(nd) if d not in dropped]
+        so = part.source_offsets
+        seen: set[tuple] = set()
+        for h in handles:
+            ho, hs = h.tensor_slice.offsets, h.tensor_slice.local_shape
+            lo = tuple(max(a, b) for a, b in zip(ho, so))
+            hi = tuple(min(a + x, b + t - s) for a, x, b, (s, t) in zip(ho, hs, so, (box[d] for d in kept)))
+            if any(t <= s for s, t in zip(lo, hi)) or (lo, hi) in seen:
+                continue
+            seen.add((lo, hi))
+            dst_idx = [slice(s, t) for s, t in box]
+            for i, d in enumerate(kept):
+                dst_idx[d] = slice(box[d][0] + lo[i] - so[i], box[d][0] + hi[i] - so[i])
+            ops.append(_TransferOp(rdma_buffer=h.rdma_buffer, dest_byte_view=None, dest_tensor=dest,
+                                   src_slices=tuple(slice(s - o, t - o) for s, t, o in zip(lo, hi, ho)),
+                                   dest_slices=tuple(dst_idx), name=name, dest_local=dest, dest_offsets=dest_offsets,
+                                   src_offsets=tuple(ho), src_start=lo, dest_dropped=dropped))
+    return ops
+
+
+def _route_handles(all_handles: dict, parts: dict) -> dict:
+    """``all_handles`` with every packed name mapped to the handles of all its parts: the route checks
+    (:meth:`DirectWeightSyncDest._check_scales`, :meth:`~DirectWeightSyncDest._check_dequant`) apply to them."""
+    if not parts:
+        return all_handles
+    out = dict(all_handles)
+    for name, entries in parts.items():
+        out[name] = list({id(h): h for *_, handles in entries for h in handles}.values())
+    return out
+
+
+def _lift(values: tuple, dims: tuple, fill) -> tuple:
+    """``values`` (one per source dim) with ``fill`` inserted at each destination dim of ``dims`` (ascending)."""
+    out = list(values)
+    for d in dims:
+        out.insert(d, fill)
+    return tuple(out)
 
 
 def _as_grid(scale: StridedMem, grid: tuple) -> StridedMem:

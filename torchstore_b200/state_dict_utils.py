@@ -93,7 +93,7 @@ async def put_state_dict(store, state_dict, key, direct_rdma=False, transfer_dty
 async def get_state_dict(store, key, user_state_dict: dict | None = None, strict=True, direct_rdma=False,
                          block_scales: dict | None = None, channel_scales: dict | None = None,
                          tensor_scales: dict | None = None, requantize: bool = False, scale_fmt: str | None = None,
-                         verbatim: bool = False):
+                         verbatim: bool = False, *, packed: dict | None = None):
     """Fetch a state dict.  ``user_state_dict`` tensors are filled in place (and required in direct
     mode).  A missing mapping means no matching push finished: RuntimeError.  ``block_scales``
     (direct mode only) names float8_e4m3fn (or int8) destinations quantised into the 128x128 block-scaled
@@ -102,12 +102,17 @@ async def get_state_dict(store, key, user_state_dict: dict | None = None, strict
     mode only) lets such destinations be fed by scaled fp8 handles, re-rounding them into the destination's
     layout.  ``scale_fmt="ue8m0"`` (direct mode only) gives every such destination power-of-two scales.
     ``verbatim=True`` (direct mode only) moves the fp8 bytes and scales of such destinations fed by scaled fp8
-    handles of their own granularity as they are, without re-rounding."""
+    handles of their own granularity as they are, without re-rounding.  ``packed`` (direct mode only) fills fused
+    destinations such as ``qkv_proj`` from handles of other names, part by part (``PackedPart``; see
+    ``DirectWeightSyncDest.pull``)."""
     if direct_rdma:
         assert user_state_dict is not None, "user_state_dict is required for direct_rdma mode"
         await _get_state_dict_direct_rdma(store, key, user_state_dict, block_scales, channel_scales, tensor_scales,
-                                          requantize, scale_fmt, verbatim)
+                                          requantize, scale_fmt, verbatim, packed)
         return user_state_dict
+    if packed:
+        raise NotImplementedError("packed needs direct_rdma=True: the store path fills destinations of their own "
+                                  "names only")
     if scale_fmt is not None:
         raise NotImplementedError("scale_fmt needs direct_rdma=True: the store path does not quantise")
     if requantize:
@@ -172,10 +177,11 @@ async def _put_state_dict_direct_rdma(store, state_dict, key, transfer_dtype=Non
         cache.source.fence()
 
 
-def _try_all_gather(cache: _DirectRDMACache, key: str, user_state_dict, scaled=False) -> bool:
+def _try_all_gather(cache: _DirectRDMACache, key: str, user_state_dict, scaled=False, *, packed=False) -> bool:
     """Route "every rank reads every tensor in full from the ranks' own Shard(0) shards" to NCCL's
     all-gather (collectives.py).  All ranks must agree, so the local verdict is min-reduced first.
-    A pull with scaled fp8 destinations votes no: the all-gather moves bytes and cannot quantise."""
+    A pull with scaled fp8 destinations votes no: the all-gather moves bytes and cannot quantise.  So does a
+    pull with packed destinations: the all-gather fills each tensor from the shards of its own name."""
     from torch.distributed.tensor import DTensor
 
     from torchstore_b200.collectives import all_gather_state_dict, is_allgather_shaped
@@ -184,7 +190,7 @@ def _try_all_gather(cache: _DirectRDMACache, key: str, user_state_dict, scaled=F
         return False
     rank, world = dist.get_rank(), dist.get_world_size()
     source = cache.sources.get(key)
-    ok = not scaled and source is not None and key in cache.registered and bool(source._handles)
+    ok = not scaled and not packed and source is not None and key in cache.registered and bool(source._handles)
     shards, dests = {}, {}
     if ok:
         ok = not any(isinstance(t, DTensor) for t in user_state_dict.values())
@@ -209,7 +215,8 @@ def _try_all_gather(cache: _DirectRDMACache, key: str, user_state_dict, scaled=F
 
 
 async def _get_state_dict_direct_rdma(store, key, user_state_dict, block_scales=None, channel_scales=None,
-                                      tensor_scales=None, requantize=False, scale_fmt=None, verbatim=False):
+                                      tensor_scales=None, requantize=False, scale_fmt=None, verbatim=False,
+                                      packed=None):
     from torchstore_b200.collectives import allgather_enabled
     from torchstore_b200.direct_weight_sync import DirectWeightSyncDest
 
@@ -221,7 +228,7 @@ async def _get_state_dict_direct_rdma(store, key, user_state_dict, block_scales=
     if cache.dest is None:
         cache.dest = cache.dests[key] = DirectWeightSyncDest()
     scaled = bool(block_scales or channel_scales or tensor_scales)
-    if allgather_enabled() and _try_all_gather(cache, key, user_state_dict, scaled):
+    if allgather_enabled() and _try_all_gather(cache, key, user_state_dict, scaled, packed=bool(packed)):
         return
     if key not in cache.handles:
         num_ranks = await store.get(f"{key}/num_ranks")
@@ -235,4 +242,4 @@ async def _get_state_dict_direct_rdma(store, key, user_state_dict, block_scales=
         cache.handles[key] = all_handles
     await cache.dests[key].pull(cache.handles[key], user_state_dict, block_scales=block_scales,
                                 channel_scales=channel_scales, tensor_scales=tensor_scales, requantize=requantize,
-                                scale_fmt=scale_fmt, verbatim=verbatim)
+                                scale_fmt=scale_fmt, verbatim=verbatim, packed=packed)

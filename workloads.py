@@ -1,6 +1,8 @@
 """Synthetic weight-sync workloads shared by bench.py, tools/ and the tests: Llama-3 state-dict
-layouts (shapes + the torchtitan TP plan of SURVEY.md section 8) and their FSDP/TP rectangles.
-Metadata only -- no tensors are created here."""
+layouts (shapes + the torchtitan TP plan of SURVEY.md section 8) and their FSDP/TP rectangles, the
+same model under its Hugging Face names, a small Qwen3-MoE-style model, and the vLLM tensor-parallel
+layout a generator holds for either (fused qkv_proj / gate_up_proj, stacked experts) as packed parts
+of the Hugging Face tensors.  Metadata only -- no tensors are created here."""
 
 from __future__ import annotations
 
@@ -8,6 +10,9 @@ import math
 
 LLAMA3_8B = dict(name="llama3-8b", dim=4096, n_layers=32, n_heads=32, n_kv_heads=8, vocab=128256, ffn=14336)
 LLAMA3_70B = dict(name="llama3-70b", dim=8192, n_layers=80, n_heads=64, n_kv_heads=8, vocab=128256, ffn=28672)
+# Qwen3-30B-A3B's shapes (head_dim 128, so the q rows are 32 * 128 = 4096 against a hidden size of 2048)
+QWEN3_MOE = dict(name="qwen3-moe", dim=2048, n_layers=48, n_heads=32, n_kv_heads=4, head_dim=128, vocab=151936,
+                 n_experts=128, moe_ffn=768)
 
 
 def llama_layout(cfg=LLAMA3_8B, n_layers: int | None = None, scale: int = 1, with_embeddings: bool = True):
@@ -81,4 +86,134 @@ def fsdp_to_tp_rects(layout, n: int, dest_rank: int, itemsize: int = 2):
             src_idx = tuple((l - o, h - o) for l, h, o in zip(lo, hi, s_off))
             dst_idx = tuple((l - o, h - o) for l, h, o in zip(lo, hi, d_off))
             out.append((name, s, src_idx, dst_idx, exact))
+    return out
+
+
+_HF_LLAMA = {"attention.wq": "self_attn.q_proj", "attention.wk": "self_attn.k_proj", "attention.wv": "self_attn.v_proj",
+             "attention.wo": "self_attn.o_proj", "feed_forward.w1": "mlp.gate_proj", "feed_forward.w2": "mlp.down_proj",
+             "feed_forward.w3": "mlp.up_proj", "attention_norm": "input_layernorm", "ffn_norm": "post_attention_layernorm"}
+
+
+def hf_llama_layout(cfg=LLAMA3_8B, n_layers: int | None = None, scale: int = 1, with_embeddings: bool = True):
+    """:func:`llama_layout` under the Hugging Face names a trainer of an HF-layout model publishes
+    (``model.layers.{i}.self_attn.q_proj.weight``, ``mlp.gate_proj``, ``model.embed_tokens``, ``lm_head``, ...):
+    the same shapes and placements, in the same order."""
+    out = {}
+    for name, entry in llama_layout(cfg, n_layers, scale, with_embeddings).items():
+        if name.startswith("layers."):
+            _, i, rest = name.split(".", 2)
+            mod = rest.removesuffix(".weight")
+            name = f"model.layers.{i}.{_HF_LLAMA[mod]}.weight"
+        else:
+            name = {"tok_embeddings.weight": "model.embed_tokens.weight", "norm.weight": "model.norm.weight",
+                    "output.weight": "lm_head.weight"}[name]
+        out[name] = entry
+    return out
+
+
+def qwen3_moe_layout(cfg=QWEN3_MOE, n_layers: int | None = None, scale: int = 1, with_embeddings: bool = True,
+                     n_experts: int | None = None):
+    """A Qwen3-MoE model under its Hugging Face names: name -> (global shape, placement), as :func:`llama_layout`
+    (the placements are those of an FSDP-style trainer's view and do not matter for packed pulls).  Per layer: q/k/v/o
+    projections with q_norm / k_norm, the router ``mlp.gate``, and one gate/up/down projection per expert.
+    ``scale`` divides hidden size, head_dim, expert width and vocabulary; ``n_experts`` overrides the expert count."""
+    d, hd = cfg["dim"] // scale, cfg["head_dim"] // scale
+    q, kv, ffn = cfg["n_heads"] * hd, cfg["n_kv_heads"] * hd, cfg["moe_ffn"] // scale
+    experts = cfg["n_experts"] if n_experts is None else n_experts
+    layers = cfg["n_layers"] if n_layers is None else n_layers
+    out = {}
+    if with_embeddings:
+        out["model.embed_tokens.weight"] = ((cfg["vocab"] // scale, d), ("S", 0))
+    for i in range(layers):
+        p = f"model.layers.{i}."
+        out[p + "self_attn.q_proj.weight"] = ((q, d), ("S", 0))
+        out[p + "self_attn.k_proj.weight"] = ((kv, d), ("S", 0))
+        out[p + "self_attn.v_proj.weight"] = ((kv, d), ("S", 0))
+        out[p + "self_attn.o_proj.weight"] = ((d, q), ("S", 1))
+        out[p + "self_attn.q_norm.weight"] = ((hd,), ("R",))
+        out[p + "self_attn.k_norm.weight"] = ((hd,), ("R",))
+        out[p + "mlp.gate.weight"] = ((experts, d), ("R",))
+        for e in range(experts):
+            out[p + f"mlp.experts.{e}.gate_proj.weight"] = ((ffn, d), ("S", 0))
+            out[p + f"mlp.experts.{e}.up_proj.weight"] = ((ffn, d), ("S", 0))
+            out[p + f"mlp.experts.{e}.down_proj.weight"] = ((d, ffn), ("S", 1))
+        out[p + "input_layernorm.weight"] = ((d,), ("R",))
+        out[p + "post_attention_layernorm.weight"] = ((d,), ("R",))
+    if with_embeddings:
+        out["model.norm.weight"] = ((d,), ("R",))
+        out["lm_head.weight"] = ((cfg["vocab"] // scale, d), ("S", 0))
+    return out
+
+
+def vllm_tp_layout(hf_layout, cfg, tp: int, rank: int, ep: bool = False):
+    """What vLLM tensor-parallel rank ``rank`` of ``tp`` holds for ``hf_layout`` (:func:`hf_llama_layout` or
+    :func:`qwen3_moe_layout` of ``cfg``): vLLM name -> (local shape, parts, box).
+
+    * Fused parameters have ``parts``, a tuple of ``PackedPart`` reading the HF tensors, and ``box`` None:
+      ``qkv_proj`` = ``[q_r; k_r; v_r]`` (rank r's query heads, then its kv head(s): when tp exceeds the kv heads,
+      kv head ``r // (tp / n_kv)``, as vLLM replicates them), ``gate_up_proj`` = ``[gate_r; up_r]``, and for MoE
+      ``mlp.experts.w13_weight [E, 2I/tp, H]`` / ``w2_weight [E, H, I/tp]`` with every expert stacked on dim 0.
+      With ``ep`` the experts are split over the ranks instead (``E/tp`` whole experts each).
+    * Every other parameter keeps its HF name: ``parts`` None and ``box`` = (global offsets, global shape) of the
+      rank's shard of that tensor: ``o_proj`` / ``down_proj`` column shards, vocab-parallel ``embed_tokens`` /
+      ``lm_head`` row shards, replicated norms and router."""
+    from torchstore_b200.direct_weight_sync import PackedPart
+
+    n_heads, n_kv = cfg["n_heads"], cfg["n_kv_heads"]
+    if n_heads % tp or (n_kv % tp and tp % n_kv):
+        raise ValueError(f"tp={tp} must divide {n_heads} query heads and divide or be a multiple of {n_kv} kv heads")
+    out = {}
+    for name, (shape, _) in hf_layout.items():
+        mod = name.removesuffix(".weight")
+        if mod.endswith("self_attn.q_proj"):
+            base = mod.removesuffix("q_proj")
+            qs, h = shape
+            kvs = hf_layout[base + "k_proj.weight"][0][0]
+            hd = qs // n_heads
+            q_r = qs // tp
+            if tp <= n_kv:
+                kv_r, kv0 = kvs // tp, rank * (kvs // tp)
+            else:
+                kv_r, kv0 = hd, rank // (tp // n_kv) * hd
+            parts = (PackedPart(name, (slice(0, q_r), slice(0, h)), (rank * q_r, 0)),
+                     PackedPart(base + "k_proj.weight", (slice(q_r, q_r + kv_r), slice(0, h)), (kv0, 0)),
+                     PackedPart(base + "v_proj.weight", (slice(q_r + kv_r, q_r + 2 * kv_r), slice(0, h)), (kv0, 0)))
+            out[base + "qkv_proj.weight"] = ((q_r + 2 * kv_r, h), parts, None)
+        elif mod.endswith(("self_attn.k_proj", "self_attn.v_proj", "mlp.up_proj")) or ".experts." in mod:
+            continue  # read by the fused parameters
+        elif mod.endswith("mlp.gate_proj"):
+            base = mod.removesuffix("gate_proj")
+            ffn, h = shape
+            f_r = ffn // tp
+            parts = (PackedPart(name, (slice(0, f_r), slice(0, h)), (rank * f_r, 0)),
+                     PackedPart(base + "up_proj.weight", (slice(f_r, 2 * f_r), slice(0, h)), (rank * f_r, 0)))
+            out[base + "gate_up_proj.weight"] = ((2 * f_r, h), parts, None)
+        elif mod.endswith("mlp.gate") and "n_experts" in cfg:
+            out[name] = (tuple(shape), None, ((0,) * len(shape), tuple(shape)))  # the router, replicated
+            base = mod.removesuffix("gate")
+            n_exp = shape[0]
+            ffn, h = hf_layout[base + "experts.0.gate_proj.weight"][0]
+            if ep:
+                if n_exp % tp:
+                    raise ValueError(f"ep over tp={tp} ranks needs the {n_exp} experts to split evenly")
+                mine, f_r, f0 = range(rank * n_exp // tp, (rank + 1) * n_exp // tp), ffn, 0
+            else:
+                mine, f_r, f0 = range(n_exp), ffn // tp, rank * (ffn // tp)
+            w13, w2 = [], []
+            for j, e in enumerate(mine):
+                ex = f"{base}experts.{e}."
+                w13 += [PackedPart(ex + "gate_proj.weight", (j, slice(0, f_r), slice(0, h)), (f0, 0)),
+                        PackedPart(ex + "up_proj.weight", (j, slice(f_r, 2 * f_r), slice(0, h)), (f0, 0))]
+                w2.append(PackedPart(ex + "down_proj.weight", (j, slice(0, h), slice(0, f_r)), (0, f0)))
+            out[base + "experts.w13_weight"] = ((len(mine), 2 * f_r, h), tuple(w13), None)
+            out[base + "experts.w2_weight"] = ((len(mine), h, f_r), tuple(w2), None)
+        else:
+            if mod.endswith(("o_proj", "down_proj")):
+                placement = ("S", 1)
+            elif mod.endswith(("embed_tokens", "lm_head")):
+                placement = ("S", 0)
+            else:
+                placement = ("R",)
+            off, loc = shard_box(shape, tp, rank, placement) if tp > 1 else ((0,) * len(shape), tuple(shape))
+            out[name] = (tuple(loc), None, (tuple(off), tuple(shape)))
     return out
