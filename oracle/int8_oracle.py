@@ -12,6 +12,7 @@ A NaN group gets scale_inv NaN and q = 0; an Inf group scale 0, scale_inv Inf an
 
 from __future__ import annotations
 
+import functools
 from collections import defaultdict
 
 import numpy as np
@@ -216,6 +217,183 @@ def special_stack(dtype: torch.dtype, shape=(130, 260)) -> torch.Tensor:
             m[m.abs() >= tiny] = 0
         out.append(m.to(dtype))
     return torch.stack(out)
+
+
+# ---- edge values of the scale step: inputs that tell the formula from plausible wrong renderings of it ----------
+# Each rendering maps (float32 x, the group's float32 scale and scale_inv) to the integer before the NaN rule and the
+# saturation; RENDERINGS[0] is the formula, the others are slips a kernel could make.
+RENDERINGS = ("formula", "div_scale_inv", "mul_rcp_scale_inv", "unrounded_product", "half_away_from_zero", "truncation")
+WRONG = RENDERINGS[1:]
+
+
+def render(name: str, x: np.ndarray, scale, scale_inv) -> np.ndarray:
+    """x (float32) -> int8 by rendering ``name``, with the NaN rule and saturation of ``narrow``:
+    formula              rint(rn_f32(x * scale))
+    div_scale_inv        rint(rn_f32(x / scale_inv))
+    mul_rcp_scale_inv    rint(rn_f32(x * rn_f32(1 / scale_inv)))
+    unrounded_product    rint(x * scale in float64)
+    half_away_from_zero  rn_f32(x * scale) rounded half away from zero
+    truncation           rn_f32(x * scale) truncated toward zero"""
+    x = np.asarray(x, dtype=np.float32)
+    scale, scale_inv = np.float32(scale), np.float32(scale_inv)
+    with np.errstate(all="ignore"):
+        prod = (x * scale).astype(np.float32)
+        if name == "formula":
+            r = np.rint(prod)
+        elif name == "div_scale_inv":
+            r = np.rint((x / scale_inv).astype(np.float32))
+        elif name == "mul_rcp_scale_inv":
+            r = np.rint((x * (np.float32(1) / scale_inv).astype(np.float32)).astype(np.float32))
+        elif name == "unrounded_product":
+            r = np.rint(x.astype(np.float64) * np.float64(scale))
+        elif name == "half_away_from_zero":
+            p = prod.astype(np.float64)
+            r = np.sign(p) * np.floor(np.abs(p) + 0.5)
+        elif name == "truncation":
+            r = np.trunc(prod)
+        else:
+            raise ValueError(f"rendering must be one of {RENDERINGS}, not {name!r}")
+    r = np.where(np.isnan(r), 0, r)
+    return np.clip(r, -128, 127).astype(np.int8)
+
+
+def discriminated(x: np.ndarray, amax) -> dict[str, np.ndarray]:
+    """{wrong rendering: mask of the elements of x where it gives another byte than the formula}, for a group of
+    max |x| ``amax`` (broadcast: one amax per element is fine)."""
+    x = np.asarray(x, dtype=np.float32)
+    amax = np.broadcast_to(np.asarray(amax, dtype=np.float32), x.shape)
+    out = {n: np.zeros(x.shape, dtype=bool) for n in WRONG}
+    for a in np.unique(amax):
+        sel = amax == a
+        scale, scale_inv = scales_of_amax(a)
+        want = render("formula", x[sel], scale, scale_inv)
+        for n in WRONG:
+            out[n][sel] = render(n, x[sel], scale, scale_inv) != want
+    return out
+
+
+def tie_kinds(x: np.ndarray, amax) -> set:
+    """{(k parity "even"/"odd", sign +1/-1)} of the elements whose rounded product x * scale is exactly k + 1/2."""
+    x = np.asarray(x, dtype=np.float32)
+    scale, _ = scales_of_amax(np.broadcast_to(np.asarray(amax, dtype=np.float32), x.shape))
+    with np.errstate(all="ignore"):
+        p = (x * scale).astype(np.float32).astype(np.float64)
+    tie = np.isfinite(p) & (np.abs(p) - np.floor(np.abs(p)) == 0.5)
+    k = np.floor(np.abs(p[tie])).astype(np.int64)
+    return {("even" if kk % 2 == 0 else "odd", 1 if s > 0 else -1) for kk, s in zip(k, p[tie])}
+
+
+_TOP_BITS = {"bfloat16": 0x7F80, "float16": 0x7C00}  # the first non-finite bit pattern
+
+
+@functools.lru_cache(maxsize=None)
+def _positive_values(dtype: str) -> np.ndarray:
+    """Every positive finite value of a 2-byte float dtype, widened to float32, ascending."""
+    return widen(np.arange(1, _TOP_BITS[dtype], dtype=np.uint16), dtype)
+
+
+def edge_values(dtype: str, amax) -> np.ndarray:
+    """The positive values of ``dtype`` up to ``amax`` (itself a ``dtype`` value) at which some wrong rendering
+    differs from the formula, for a group of that amax: every finite bf16 / f16 value is tried; for float32, 8 ulps
+    either side of each (k + 1/2) / scale."""
+    a = np.float32(amax)
+    scale, scale_inv = scales_of_amax(a)
+    if dtype == "float32":
+        centre = ((np.arange(128) + 0.5) / np.float64(scale)).astype(np.float32)
+        cand = [centre]
+        up, down = centre.copy(), centre.copy()
+        for _ in range(8):
+            up, down = np.nextafter(up, np.float32(np.inf)), np.nextafter(down, np.float32(0))
+            cand += [up, down]
+        cand = np.unique(np.concatenate(cand))
+    else:
+        cand = _positive_values(dtype)
+    cand = cand[(cand > 0) & (cand <= a)]
+    told = discriminated(cand, a)
+    hard = np.any([told[n] for n in HARD], axis=0)
+    # the values that tell a HARD rendering apart first, then the ties k + 1/2, then the rest
+    p = (cand * scale).astype(np.float32).astype(np.float64)
+    rank = np.where(hard, 0, np.where(p - np.floor(p) == 0.5, 1, 2))
+    hit = np.any(list(told.values()), axis=0)
+    return cand[hit][np.argsort(rank[hit], kind="stable")]
+
+
+HARD = ("div_scale_inv", "mul_rcp_scale_inv", "unrounded_product")  # the renderings few values tell apart
+
+
+def clamp_amaxes(dtype: str) -> np.ndarray:
+    """Three amaxes at the 1e-4 floor in ``dtype``: for float32 the values just below, at and just above 1e-4f; for
+    bf16 / f16 (which do not hold 1e-4f) its two largest values below 1e-4f and its smallest one above."""
+    if dtype == "float32":
+        return np.array([np.nextafter(_CLAMP, np.float32(0)), _CLAMP, np.nextafter(_CLAMP, np.float32(1))], dtype=np.float32)
+    v = _positive_values(dtype)
+    i = int(np.searchsorted(v, _CLAMP))  # v[i - 1] < 1e-4f <= v[i]; neither dtype holds 1e-4f exactly
+    assert v[i] > _CLAMP
+    return np.array([v[i - 2], v[i - 1], v[i]], dtype=np.float32)
+
+
+@functools.lru_cache(maxsize=None)
+def edge_groups(dtype: str, n: int = 12) -> tuple:
+    """(amax, edge values) of the groups an edge input plants in ``dtype``: the three clamp_amaxes, 127 (scale exactly
+    1: the ties k + 1/2), then ``n`` amaxes searched from a log-uniform sequence over [2^-6, 2^8], picked so that each
+    rendering of HARD is told apart in at least two of them."""
+    out = [(a, edge_values(dtype, a)) for a in clamp_amaxes(dtype)] + [(np.float32(127), edge_values(dtype, np.float32(127)))]
+    rng = np.random.default_rng({"bfloat16": 1, "float16": 2, "float32": 3}[dtype])
+    need = {h: 2 for h in HARD}
+    spare = []
+    for _ in range(4000):
+        if len(out) == n + 4:
+            break
+        a = np.float32(2.0 ** rng.uniform(-6, 8))
+        a = widen(bits_of(torch.tensor(float(a)).to(getattr(torch, dtype))), dtype)[()]
+        vals = edge_values(dtype, a)
+        if not len(vals):
+            continue
+        told = {h for h, m in discriminated(vals, a).items() if h in HARD and m.any()}
+        if any(need[h] > 0 for h in told):
+            for h in told:
+                need[h] -= 1
+            out.append((a, vals))
+        elif len(spare) < n:
+            spare.append((a, vals))
+    out += spare[: n + 4 - len(out)]
+    assert len(out) == n + 4 and all(v <= 0 for v in need.values()), (dtype, need)
+    return tuple(out)
+
+
+def plant_rounding_edges(shape, dtype: torch.dtype, granularity: str, row0: int = 0, col0: int = 0):
+    """A ``dtype`` shard whose groups (anchored as the granularity's, at (row0, col0)) take edge_groups(dtype) in
+    turn: the amax, negated in odd groups, at the group's first element, then the group's edge values in turn as
+    +v, -v.  Groups past the last edge group repeat them from the first.  -> (x, number of groups)."""
+    from oracle.ue8m0_oracle import group_ids
+
+    name = str(dtype)[6:]
+    groups = edge_groups(name)
+    gid, n = group_ids(granularity, shape, row0, col0)
+    flat_gid = gid.reshape(-1)
+    x = np.zeros(flat_gid.shape, dtype=np.float32)
+    order = np.argsort(flat_gid, kind="stable")
+    starts = np.searchsorted(flat_gid[order], np.arange(n + 1))
+    for g in range(n):
+        idx = order[starts[g]: starts[g + 1]]
+        a, vals = groups[g % len(groups)]
+        seq = np.stack([vals, -vals], axis=1).reshape(-1)
+        fill = np.resize(seq, max(0, idx.size - 1)) if seq.size else np.zeros(max(0, idx.size - 1), np.float32)
+        x[idx[1:]] = fill
+        x[idx[0]] = -a if g % 2 else a
+    return torch.from_numpy(x.reshape(tuple(shape))).to(dtype), n
+
+
+def told_apart(x: torch.Tensor, granularity: str, row0: int = 0, col0: int = 0) -> tuple[set, set]:
+    """From a shard's values alone: (the wrong renderings that give another byte than the formula somewhere in it,
+    the tie kinds of tie_kinds over it), each element with its own group's amax."""
+    from oracle.ue8m0_oracle import group_amax, group_ids
+
+    xf = widen(bits_of(x), str(x.dtype)[6:])
+    gid, n = group_ids(granularity, tuple(x.shape), row0, col0)
+    amax = group_amax(xf, gid, n)[gid]
+    told = {name for name, m in discriminated(xf, amax).items() if m.any()}
+    return told, tie_kinds(xf, amax)
 
 
 def fixture_inputs() -> list[tuple[str, torch.Tensor, str]]:

@@ -68,6 +68,40 @@ def torch_dequantize(q: torch.Tensor, scale: torch.Tensor, granularity: str, r0:
     return _torch_dequantize(q, scale, granularity, r0, c0, dst)
 
 
+def assert_invariants(q: np.ndarray, xf: np.ndarray, granularity: str, row0: int = 0, col0: int = 0) -> None:
+    """What the formula guarantees in every group of a shard at (row0, col0), whatever its values: no byte is -128,
+    a non-finite group is all zeros, and a finite group with amax >= 1e-4 holds +-127 at each of its amax elements."""
+    from oracle.ue8m0_oracle import group_amax, group_ids
+
+    gid, n = group_ids(granularity, xf.shape, row0, col0)
+    amax = group_amax(xf, gid, n)  # NaN propagates
+    finite = np.isfinite(amax)
+    assert (q != -128).all(), "a byte is -128"
+    assert (q[~finite[gid]] == 0).all(), "a non-finite group holds a non-zero byte"
+    big = finite & (amax >= np.float32(1e-4))
+    with np.errstate(invalid="ignore"):
+        at = big[gid] & (np.abs(xf) == amax[gid])
+    assert (np.abs(q[at].astype(np.int16)) == 127).all(), "an amax element is not +-127"
+    assert np.array_equal(np.unique(gid[at]), np.flatnonzero(big)), "a finite group lacks its amax element"
+
+
+def assert_exact(q: torch.Tensor, s: torch.Tensor, x: torch.Tensor, granularity: str, row0: int = 0, col0: int = 0) -> None:
+    """int8 q and float32 scale_inv s of a bf16/f16/f32 shard x at (row0, col0): bit for bit the torch rendering on
+    q's device and the numpy oracle (bytes exact everywhere, non-finite groups included; scale bits exact,
+    NaN-agnostic only where the scale is NaN), and the formula's invariants (``assert_invariants``)."""
+    assert q.dtype == torch.int8
+    tq, ts = torch_quantize(x.to(q.device), granularity, row0, col0)
+    assert torch.equal(q, tq), "int8 bytes differ from the torch rendering"
+    got_s = s.cpu().numpy().reshape(-1)
+    assert int8_oracle.same_scales(got_s, ts.cpu().numpy().reshape(-1)), "scale_inv differs from the torch rendering"
+    xf = widen(bits_of(x.cpu()), str(x.dtype)[6:])
+    want_q, want_s = quantize(xf, granularity, row0, col0)
+    got_q = q.cpu().numpy()
+    assert np.array_equal(got_q, want_q), "int8 bytes differ from the numpy oracle"
+    assert int8_oracle.same_scales(got_s, want_s.reshape(-1)), "scale_inv differs from the numpy oracle"
+    assert_invariants(got_q, xf, granularity, row0, col0)
+
+
 def replay_source(units: np.ndarray, tiles: np.ndarray, n_groups: int) -> None:
     """Execute tsb_source_quant_compile_host_as(TSB_I8) tables on host memory: a unit is one group (a block) or
     one group per row (a band); the tiles are the two-pass path, interpreted by int8_oracle.replay_scaled."""

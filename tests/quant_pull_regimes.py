@@ -216,7 +216,7 @@ class Geometry:
 def compile_tables(pulls, ops, handles, window_of, dests, scales, flags: int = 0) -> tuple[Tables, Geometry]:
     """Compile on the host the quantising plans a pull of `pulls` (names w0, w1, ...) builds: the windows of
     `ops` (the planner's ops of the pull, the quantised names' ones used) with `window_of(buffer)` mapping a
-    source buffer, and the targets of the fp8 destinations `dests` and their `scales`, in the order the pull
+    source buffer, and the targets of the fp8 (or int8) destinations `dests` and their `scales`, in the order the pull
     orders them (block, channel, tensor names), with the plan `flags` (0 or _native.TSB_QUANT_UE8M0).  -> (Tables,
     Geometry); keep `dests`, `scales` alive."""
     grans = {f"w{i}": p.g for i, p in enumerate(pulls)}
@@ -230,7 +230,7 @@ def compile_tables(pulls, ops, handles, window_of, dests, scales, flags: int = 0
         names = [n for n in order if (grans[n] == "block") == block]
         if not names:
             continue
-        rects, nr = build_rects(pairs[block])
+        rects, nr = build_rects(pairs[block], quantise=True)  # TSB_I8 rects for int8 destinations
         arr = _native.make_target_array(len(names)) if block else _native.make_sq_target_array(len(names))
         for i, n in enumerate(names):
             d, s = dests[n], scales[n]

@@ -151,7 +151,7 @@ def compile_pull(q_full, full_scale, g, src_boxes, dst_box, dst_dtype):
             n, k = buf.shard.shape[-2:]
             sources.append(_native.DqSource(buf.shard.data_ptr(), buf.scale.data_ptr(), buf.shard.numel() // (n * k), n, k,
                                             buf.row0, buf.col0, CODE[g], 0))
-    rects, nr = build_rects(pairs)
+    rects, nr = build_rects(pairs, dequantise=True)  # TSB_I8 rects for int8 sources
     arr = _native.make_dq_source_array(max(1, len(sources)))
     for i, s in enumerate(sources):
         arr[i] = s

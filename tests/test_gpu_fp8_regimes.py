@@ -5,7 +5,8 @@ allocations, and across random layouts of all four scaled plan kinds.
   source scale (Inf, NaN, 0 and a negative scale) and with an all-zero destination group; the regime asserted
   again from the tables of the live plan's inputs (and their size against plan_info); bit-exact against the
   numpy oracle wherever it is not NaN, against the torch CUDA composition with NaN bytes included; guard bytes
-  around the weight and the scale tensor.
+  around the weight and the scale tensor.  The dequantising regimes also run from int8 handles (``src_dtype``: the
+  bytes of ``int8_of``, checked against oracle/int8_source_oracle.py and its torch rendering).
 * Past 32 bits: a requantising and a dequantising pull of a fp8 MoE stack whose source shard and destination
   both extend past byte 2^32.
 * Random layouts: seeded draws of a global shape, a source layout (FSDP rows starting mid-block, column
@@ -21,14 +22,14 @@ import numpy as np
 import pytest
 import torch
 
-from oracle import block_fp8_oracle, scaled_fp8_oracle
+from oracle import block_fp8_oracle, int8_source_oracle, scaled_fp8_oracle
 from oracle.dequant_fp8_oracle import DST, GRANULARITIES, torch_dequantize
 from oracle.requant_fp8_oracle import SCALE_POISON, torch_requantize
 from tests import test_gpu_dequant_fp8 as dq_gpu
 from tests import test_gpu_requant_fp8 as rq_gpu
 from tests.fp8_regimes import REGIMES, WORKLOADS, Workload, geometry, split, whole
 from tests.test_gpu_dequant_fp8 import KW, cleanup, guarded, guards_intact, register
-from tests.test_requant_fp8_cpu import CODE, dest_scale_shape, fp8_full, global_scale, region, shard_box
+from tests.test_requant_fp8_cpu import CODE, dest_scale_shape, fp8_full, global_scale, local_scale, region, shard_box
 from torchstore_b200 import _native
 from torchstore_b200.direct_weight_sync import DirectWeightSyncDest, DirectWeightSyncSource, _add_dq_source
 from torchstore_b200.planner import build_rects
@@ -60,10 +61,10 @@ def named(what):
 
 
 # ---- the live plan's tables -------------------------------------------------------------------------
-def live_tables(sync, dest, dest_scale=None, dg=None):
+def live_tables(sync, dest, dest_scale=None, dg=None, int8_src=False):
     """Compile on the host the tables of the plan `sync` built for its one name: the same windows, sources and
-    target it compiled from, with the live device addresses.  Checks their size against plan_info and returns
-    (tables, Geometry)."""
+    target it compiled from, with the live device addresses (`int8_src`: a dequantising plan of int8 handles, TSB_I8
+    rects).  Checks their size against plan_info and returns (tables, Geometry)."""
     dev = dest.device.index
     pairs, sources = [], {}
     for op in sync._plan:
@@ -72,11 +73,13 @@ def live_tables(sync, dest, dest_scale=None, dg=None):
     arr = _native.make_dq_source_array(max(1, len(sources)))
     for i, (_, s) in enumerate(sources.values()):
         arr[i] = s
-    rects, n = build_rects(pairs)
+    rects, n = build_rects(pairs, dequantise=int8_src)
     *lead, rows, cols = dest.shape
     if dg is None:
         tables = _native.dequant_fp8_compile_host(dev, rects, n, arr, len(sources))
-        info = _native.plan_info(sync._dequant_plans[dev])
+        mine, other = (sync._int8_dequant_plans, sync._dequant_plans) if int8_src else (sync._dequant_plans, sync._int8_dequant_plans)
+        assert not other, "dequantising plans of the other source format"
+        info = _native.plan_info(mine[dev])
         count, read = len(tables), int((tables["rows"].astype(np.int64) * tables["cols"]).sum())
     else:
         for i in range(n):
@@ -111,8 +114,10 @@ def zero_first_group(q, w: Workload):
     return q
 
 
-def inputs(w: Workload, variant: str):
-    q, s = fp8_full(w.shape, w.seed), global_scale(w.sg, w.shape, w.seed)
+def inputs(w: Workload, variant: str, src_dtype=E4M3):
+    """The source weight (fp8 bytes, or int8 ones from int8_of) and its global scale of workload `w` in `variant`."""
+    q = int8_source_oracle.int8_of(w.shape, w.seed) if src_dtype == torch.int8 else fp8_full(w.shape, w.seed)
+    s = global_scale(w.sg, w.shape, w.seed)
     if variant == "poisoned_scale":
         s = poison(s, w.seed)
     elif variant == "zero_group":
@@ -129,13 +134,16 @@ def test_regime_on_the_h100(regime, variant):
     run_regime(regime, variant)
 
 
-def run_regime(regime, variant, scale_fmt=None):
-    """Pull the regime's workload in `variant` (requantising ones with the scale format `scale_fmt`) and check it."""
+def run_regime(regime, variant, scale_fmt=None, src_dtype=E4M3):
+    """Pull the regime's workload in `variant` (requantising ones with the scale format `scale_fmt`; dequantising
+    ones from handles of `src_dtype`, float8_e4m3fn or int8) and check it."""
     r = REGIMES[regime]
     w = WORKLOADS[r.workload]
-    q, s = inputs(w, variant)
+    int8 = src_dtype == torch.int8
+    assert not (int8 and w.kind == "requant"), "int8 handles are not requantised"
+    q, s = inputs(w, variant, src_dtype)
     sources, handles = register(q, s, w.sg, list(w.src))
-    where = f"{regime} ({r.doc}), {variant}, scale_fmt={scale_fmt}: {w.describe()}"
+    where = f"{regime} ({r.doc}), {variant}, scale_fmt={scale_fmt}, {src_dtype}: {w.describe()}"
     if w.kind == "requant":
         sync, y, ys, bases = rq_gpu.pull_into(handles, w.shape, w.dst, w.out, scale_fmt=scale_fmt)
         tables, geom = live_tables(sync, y, ys, w.out)
@@ -145,15 +153,28 @@ def run_regime(regime, variant, scale_fmt=None):
             rq_gpu.assert_torch_cuda(y, ys, q, s, w.sg, w.dst, w.out, scale_fmt)
     else:
         sync, y, base = dq_gpu.pull_into(handles, w.shape, w.dst, DST[w.out])
-        tables, geom = live_tables(sync, y)
+        tables, geom = live_tables(sync, y, int8_src=int8)
         assert r.holds(tables, geom), f"not reached: {where}"
         with named(where):
-            dq_gpu.assert_oracle(y, dq_gpu.want_bits(q, s, w.sg, w.dst, DST[w.out]))
-            dq_gpu.assert_torch_cuda(y, q, s, w.sg, w.dst)
+            if int8:
+                assert_int8_dequantised(y, q, s, w.sg, w.dst)
+            else:
+                dq_gpu.assert_oracle(y, dq_gpu.want_bits(q, s, w.sg, w.dst, DST[w.out]))
+                dq_gpu.assert_torch_cuda(y, q, s, w.sg, w.dst)
         bases = (base,)
     assert all(guards_intact(b) for b in bases), where
     sync.close()
     cleanup(sources)
+
+
+def assert_int8_dequantised(y, q, s, g, box):
+    """A destination y dequantised from the `box` of int8 handles (q, global scale s): bit for bit the numpy oracle
+    (NaN-agnostic) and the torch CUDA rendering (NaN bytes included)."""
+    off, loc = box
+    qr, sr = region(q, off, loc), local_scale(s, g, off, loc)
+    dq_gpu.assert_oracle(y, int8_source_oracle.dequantize(qr.numpy(), sr.numpy(), g, off[-2], off[-1], str(y.dtype)[6:]))
+    want = int8_source_oracle.torch_dequantize(qr.to(DEV), sr.to(DEV), g, off[-2], off[-1], y.dtype)
+    assert torch.equal(y.view(torch.uint8), want.view(torch.uint8))
 
 
 # ---- past byte 2^32 ---------------------------------------------------------------------------------

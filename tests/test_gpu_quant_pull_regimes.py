@@ -13,7 +13,10 @@ byte 2^32 of their allocations, and across random layouts with special values.
   replayed over overwritten destinations.
 * Past 32 bits: a bf16 MoE stack whose source runs past byte 2^32 and whose fp8 destination does too.
 * Random layouts: seeded draws of a global shape, source shards and a destination window with NaN, Inf,
-  zero and subnormal groups planted at shard, block and row boundaries."""
+  zero and subnormal groups planted at shard, block and row boundaries.
+
+The regime and random-layout runners take the destination dtype (``dst_dtype``, float8_e4m3fn by default; int8
+destinations are checked against oracle/int8_oracle.py and its torch rendering)."""
 
 import asyncio
 import random
@@ -22,7 +25,7 @@ import numpy as np
 import pytest
 import torch
 
-from oracle import block_fp8_oracle, scaled_fp8_oracle, ue8m0_oracle
+from oracle import block_fp8_oracle, int8_source_oracle, scaled_fp8_oracle, ue8m0_oracle
 from oracle.block_fp8_oracle import synth_f32
 from tests import test_gpu_block_fp8 as bq_gpu
 from tests.fp8_regimes import split, whole
@@ -137,12 +140,13 @@ def inputs(name: str, variant: str):
 
 # ---- one pull of several names ----------------------------------------------------------------------
 class Pulled:
-    """The names w0, w1, ... of `pulls` registered shard by shard (one source each), pulled into guarded fp8
-    destinations and scales by one DirectWeightSyncDest with the scale format `scale_fmt`; `extra` handles and
-    destinations join the pull."""
+    """The names w0, w1, ... of `pulls` registered shard by shard (one source each), pulled into guarded
+    destinations of `dst_dtype` (float8_e4m3fn or int8) and scales by one DirectWeightSyncDest with the scale format
+    `scale_fmt`; `extra` handles and destinations join the pull."""
 
-    def __init__(self, pulls, xs, extra_handles=None, extra_dests=None, scale_fmt=None):
+    def __init__(self, pulls, xs, extra_handles=None, extra_dests=None, scale_fmt=None, dst_dtype=E4M3):
         self.pulls, self.sources, self.shards, self.scale_fmt = tuple(pulls), [], {}, scale_fmt
+        self.dst_dtype = dst_dtype
         self.handles, self.dests, self.scales, self.slices, self.bases = {}, {}, {}, {}, []
         try:
             for i, (p, x) in enumerate(zip(pulls, xs)):
@@ -155,7 +159,7 @@ class Pulled:
                     sl = TensorSlice(off, (r,), p.shape, loc, (len(p.src),))
                     self.handles[n].append(src.register({n: shard}, rank=r, tensor_slices={n: sl})[n])
                     self.shards[n].append(shard)
-                qb, self.dests[n] = guarded(p.dst[1], E4M3)
+                qb, self.dests[n] = guarded(p.dst[1], dst_dtype)
                 sb, self.scales[n] = guarded(scale_shape(p.g, p.dst[1]), torch.float32)
                 self.bases += [qb, sb]
                 self.slices[n] = TensorSlice(p.dst[0], (0,), p.shape, p.dst[1], (1,))
@@ -172,15 +176,22 @@ class Pulled:
     def pull(self):
         run(self.sync.pull(self.all_handles, self.all_dests, self.slices, **self.by_kw, scale_fmt=self.scale_fmt))
 
+    def plan_dicts(self):
+        """The (block, per-channel / per-tensor) plans of the destination format; the other format's stay empty."""
+        fp8, int8 = (self.sync._block_plans, self.sync._scaled_plans), (self.sync._int8_block_plans, self.sync._int8_scaled_plans)
+        mine, other = (int8, fp8) if self.dst_dtype == torch.int8 else (fp8, int8)
+        assert not any(other), "plans of the other destination format"
+        return mine
+
     def plans(self):
-        return dict(self.sync._block_plans), dict(self.sync._scaled_plans)
+        return tuple(dict(p) for p in self.plan_dicts())
 
     def live_tables(self):
         """The tables of the plans the pull built, compiled on the host from the same windows and targets with
         the live device addresses; their size checked against plan_info."""
         tables, geom = compile_tables(self.pulls, self.sync._plan, self.handles, lambda b: b.window(0), self.dests, self.scales)
         want = plan_bytes(tables)
-        for kind, plans in (("block", self.sync._block_plans), ("scaled", self.sync._scaled_plans)):
+        for kind, plans in zip(("block", "scaled"), self.plan_dicts()):
             if kind in want:
                 info = _native.plan_info(plans[0])
                 assert (info.num_tiles, info.src_bytes) == want[kind], kind
@@ -192,7 +203,7 @@ class Pulled:
         for i, (p, x) in enumerate(zip(self.pulls, xs)):
             n = f"w{i}"
             with named(f"w{i}: {p.describe()}"):
-                assert_quantised(self.dests[n], self.scales[n], region(x, *p.dst), p.g, self.scale_fmt)
+                assert_quantised(self.dests[n], self.scales[n], region(x, *p.dst), p.g, self.scale_fmt, self.dst_dtype)
         assert all(guards_intact(b) for b in self.bases)
 
     def update(self, xs):
@@ -210,10 +221,13 @@ class Pulled:
             run(src.cleanup())
 
 
-def assert_quantised(y, ys, x, g, scale_fmt=None):
+def assert_quantised(y, ys, x, g, scale_fmt=None, dst_dtype=E4M3):
     """The fp8 weight y and its scale_inv ys against the numpy oracle of the source region x (bit-exact in
     finite groups, NaN-agnostic in the others) and the torch CUDA composition (bit-exact, NaN bytes included),
-    both in the scale format `scale_fmt`."""
+    both in the scale format `scale_fmt`.  An int8 y: int8_source_oracle.assert_exact."""
+    if dst_dtype == torch.int8:
+        int8_source_oracle.assert_exact(y, ys, x, g)
+        return
     if scale_fmt is None:
         want_q, want_s = oracle_quantize(x.float().numpy(), g)
     else:
@@ -246,13 +260,14 @@ def test_regime_on_the_h100(regime, variant):
     run_regime(regime, variant)
 
 
-def run_regime(regime, variant, scale_fmt=None):
-    """Pull the regime's workload in `variant` with the scale format `scale_fmt`, and check it (module doc)."""
+def run_regime(regime, variant, scale_fmt=None, dst_dtype=E4M3):
+    """Pull the regime's workload in `variant` with the scale format `scale_fmt` into `dst_dtype` destinations,
+    and check it (module doc)."""
     r = REGIMES[regime]
     w = WORKLOADS[r.workload]
     xs = inputs(r.workload, variant)
-    where = f"{regime} ({r.doc}), {variant}, scale_fmt={scale_fmt}: {w.describe()}"
-    pulled = Pulled(w.pulls, xs, scale_fmt=scale_fmt)
+    where = f"{regime} ({r.doc}), {variant}, scale_fmt={scale_fmt}, {dst_dtype}: {w.describe()}"
+    pulled = Pulled(w.pulls, xs, scale_fmt=scale_fmt, dst_dtype=dst_dtype)
     try:
         pulled.pull()
         tables, geom = pulled.live_tables()
@@ -384,11 +399,16 @@ def plant_random(x, p: Pull, rng: random.Random, seed: int):
 
 @pytest.mark.parametrize("seed", range(24))
 def test_random_layouts_with_special_values(seed):
+    run_random_layout(seed)
+
+
+def run_random_layout(seed, dst_dtype=E4M3):
+    """Pull the layout drawn from `seed`, with special values, into a `dst_dtype` destination and check it."""
     rng = random.Random(19000 + seed)
     w = draw(rng, "quant", seed)
     p = Pull(("bfloat16", "float16", "float32")[seed % 3], w.shape, w.src, w.dst, w.out)
     x = plant_random(torch.randn(w.shape, generator=torch.Generator().manual_seed(seed)) * 0.05, p, rng, seed)
-    pulled = Pulled((p,), [x])
+    pulled = Pulled((p,), [x], dst_dtype=dst_dtype)
     try:
         with named(f"seed {seed}: {p.describe()}"):
             pulled.pull()

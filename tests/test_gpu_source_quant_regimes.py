@@ -7,7 +7,8 @@ carry their own scales.
   target, and after an in-place update and ``refresh()``; the regime asserted again from the tables of the
   live addresses (and their size against plan_info); bit-exact against torch CUDA (NaN bytes included) and the
   numpy oracle on finite groups.  Each workload is also driven through Plans.build_source_quant on guarded
-  buffers.
+  buffers.  The regime runners take the staging dtype (``quant_dtype``, float8_e4m3fn by default; int8 staging is
+  checked against oracle/int8_source_oracle.py and its torch rendering).
 * The torch CPU fixture (tests/golden/source_quant_vectors.npz) on the device, at its recorded offsets.
 * Consumers: dequantising, requantising and raw fp8 pulls of source-quantised shards that hold different scales
   for the groups they share (column shards, 2-D meshes, EP x FSDP x TP, replicas), against per-shard references.
@@ -21,6 +22,7 @@ import numpy as np
 import pytest
 import torch
 
+from oracle import int8_source_oracle
 from oracle.source_quant_oracle import GRANULARITIES, fixture_inputs, synth_f32, torch_quantize
 from tests import test_gpu_dequant_fp8 as dq_gpu
 from tests import test_gpu_requant_fp8 as rq_gpu
@@ -103,9 +105,9 @@ def plant(x: torch.Tensor, t: Target, kind: str, seed: int) -> torch.Tensor:
     return x.to(getattr(torch, t.dtype))
 
 
-def register_workload(name, xs, scale_fmt=None):
-    """One register() of every target of workload `name` (values `xs`), in the scale format `scale_fmt` ->
-    (source, handles, device shards)."""
+def register_workload(name, xs, scale_fmt=None, quant_dtype=None):
+    """One register() of every target of workload `name` (values `xs`), in the scale format `scale_fmt` and the
+    staging dtype `quant_dtype` -> (source, handles, device shards)."""
     w = WORKLOADS[name]
     src = DirectWeightSyncSource()
     sd, slices, quant = {}, {}, {}
@@ -113,13 +115,13 @@ def register_workload(name, xs, scale_fmt=None):
         sd[f"t{i}"] = on_device(x, t.misalign)
         slices[f"t{i}"] = local_slice(t.shape, t.row0, t.col0)
         quant[f"t{i}"] = t.granularity
-    handles = src.register(sd, rank=0, tensor_slices=slices, quantize=quant, scale_fmt=scale_fmt)
+    handles = src.register(sd, rank=0, tensor_slices=slices, quantize=quant, scale_fmt=scale_fmt, quant_dtype=quant_dtype)
     return src, handles, sd
 
 
-def live_tables(src, handles, w):
+def live_tables(src, handles, w, quant_dtype=None):
     """Compile on the host the targets register() built, from the staging it allocated and the handles'
-    offsets; check their size against plan_info -> (tables, targets)."""
+    offsets (for int8 staging with TSB_I8); check their size against plan_info -> (tables, targets)."""
     targets = []
     for i, t in enumerate(w.targets):
         fp8, scale, local = src._quantized[f"t{i}"]
@@ -127,17 +129,26 @@ def live_tables(src, handles, w):
         rows, cols = local.shape[-2:]
         targets.append(_native.SourceQuantTarget(local.data_ptr(), fp8.data_ptr(), scale.data_ptr(), local.numel() // (rows * cols),
                                                  rows, cols, buf.row0, buf.col0, CODE[t.dtype], GCODE[t.granularity]))
-    tables = compile_host(targets)
+    if quant_dtype == torch.int8:
+        arr = _native.make_source_quant_target_array(len(targets))
+        for i, t in enumerate(targets):
+            arr[i] = t
+        tables = _native.source_quant_compile_host(0, arr, len(targets), dst_dtype=_native.TSB_I8)
+    else:
+        tables = compile_host(targets)
     info = _native.plan_info(src._quant_plans[0])
     assert (info.num_tiles, info.src_bytes) == plan_bytes(tables)
     return tables, targets
 
 
-def check_staging(src, w, xs, scale_fmt=None):
+def check_staging(src, w, xs, scale_fmt=None, quant_dtype=None):
     for i, (t, x) in enumerate(zip(w.targets, xs)):
         q, s, _ = src._quantized[f"t{i}"]
         with named(t.describe()):
-            assert_exact(q, s, x, t.granularity, t.row0, t.col0, scale_fmt)
+            if quant_dtype == torch.int8:
+                int8_source_oracle.assert_exact(q, s, x, t.granularity, t.row0, t.col0)
+            else:
+                assert_exact(q, s, x, t.granularity, t.row0, t.col0, scale_fmt)
 
 
 VARIANTS = ("finite", "inf", "nan", "zero", "subnormal", "refresh")
@@ -149,26 +160,27 @@ def test_regime_on_the_h100(regime, variant):
     run_regime(regime, variant)
 
 
-def run_regime(regime, variant, scale_fmt=None):
-    """Register the regime's workload in `variant` with the scale format `scale_fmt`, and check it (module doc)."""
+def run_regime(regime, variant, scale_fmt=None, quant_dtype=None):
+    """Register the regime's workload in `variant` with the scale format `scale_fmt` and the staging dtype
+    `quant_dtype`, and check it (module doc)."""
     r = REGIMES[regime]
     w = WORKLOADS[r.workload]
     xs = workload_inputs(r.workload)
     if variant not in ("finite", "refresh"):
         xs = [plant(x, t, variant, w.seed + i) for i, (t, x) in enumerate(zip(w.targets, xs))]
-    src, handles, sd = register_workload(r.workload, xs, scale_fmt)
-    where = f"{regime} ({r.doc}), {variant}, scale_fmt={scale_fmt}: {w.describe()}"
+    src, handles, sd = register_workload(r.workload, xs, scale_fmt, quant_dtype)
+    where = f"{regime} ({r.doc}), {variant}, scale_fmt={scale_fmt}, quant_dtype={quant_dtype}: {w.describe()}"
     try:
-        tables, targets = live_tables(src, handles, w)
+        tables, targets = live_tables(src, handles, w, quant_dtype)
         assert r.holds(tables, targets), f"not reached: {where}"
         with named(where):
-            check_staging(src, w, xs, scale_fmt)
+            check_staging(src, w, xs, scale_fmt, quant_dtype)
             if variant == "refresh":
                 xs = [synth_f32(t.shape, w.seed + 50 + i).to(x.dtype) * 0.25 for i, (t, x) in enumerate(zip(w.targets, xs))]
                 for i, x in enumerate(xs):
                     sd[f"t{i}"].copy_(x.to(DEV))
                 assert src.refresh() == len(w.targets)
-                check_staging(src, w, xs, scale_fmt)
+                check_staging(src, w, xs, scale_fmt, quant_dtype)
     finally:
         run(src.cleanup())
 
@@ -179,20 +191,21 @@ def test_workload_writes_nothing_outside_its_outputs(name):
     run_guarded(name)
 
 
-def run_guarded(name, scale_fmt=None):
+def run_guarded(name, scale_fmt=None, quant_dtype=None):
     w = WORKLOADS[name]
     xs = workload_inputs(name)
     targets, outs = [], []
     for t, x in zip(w.targets, xs):
         sv = on_device(x, t.misalign)
         sshape = source_scale_shapes(t.granularity, t.shape, t.row0, t.col0)[0]
-        qbase, q = guarded(t.shape, E4M3)
+        qbase, q = guarded(t.shape, quant_dtype or E4M3)
         sbase, s = guarded(sshape, torch.float32)
         rows, cols = t.shape[-2:]
         targets.append(_native.SourceQuantTarget(sv.data_ptr(), q.data_ptr(), s.data_ptr(), x.numel() // (rows * cols), rows, cols,
                                                  t.row0, t.col0, CODE[t.dtype], GCODE[t.granularity]))
         outs.append((sv, q, s, qbase, sbase))
-    plans = Plans.build_source_quant({0: targets}, _native.TSB_QUANT_UE8M0 if scale_fmt else 0)
+    plans = Plans.build_source_quant({0: targets}, _native.TSB_QUANT_UE8M0 if scale_fmt else 0,
+                                     _native.TSB_I8 if quant_dtype == torch.int8 else _native.TSB_F8E4M3)
     try:
         for _ in range(2):
             plans.launch()
@@ -201,7 +214,10 @@ def run_guarded(name, scale_fmt=None):
         plans.close()
     for t, x, (_, q, s, qbase, sbase) in zip(w.targets, xs, outs):
         with named(f"{name}: {t.describe()}"):
-            assert_exact(q, s, x, t.granularity, t.row0, t.col0, scale_fmt)
+            if quant_dtype == torch.int8:
+                int8_source_oracle.assert_exact(q, s, x, t.granularity, t.row0, t.col0)
+            else:
+                assert_exact(q, s, x, t.granularity, t.row0, t.col0, scale_fmt)
             assert guards_intact(qbase) and guards_intact(sbase)
 
 
