@@ -942,6 +942,24 @@ class DirectWeightSyncDest:
             out.add(name)
         return out
 
+    @staticmethod
+    def _check_packed_rows(parts: dict, dequant: set, requant: set) -> None:
+        """Refuse a packed part whose int index drops the destination's last dim on a route that reads scaled handles
+        (``dequant`` and ``requant`` names): those kernels move whole rows of a scaled source shard into whole
+        destination rows, and such a part gives each destination row one element of a source row.  ValueError naming the
+        destination and the part, before anything is compiled (verbatim parts are refused by :meth:`_verbatim_rects`;
+        quantising and element-wise routes take such parts)."""
+        for name, entries in parts.items():
+            if name not in dequant and name not in requant:
+                continue
+            for k, part, box, dropped, _ in entries:
+                if dropped and dropped[-1] == len(box) - 1:
+                    what = "dequantising" if name in dequant else "requantising"
+                    raise ValueError(f"packed destination '{name}' part {k} (source '{part.source}'): its int index drops "
+                                     f"the destination's last dim, which a {what} pull cannot fill (it moves whole rows of "
+                                     "its scaled handles into whole destination rows); quantising and element-wise pulls "
+                                     "take such parts")
+
     def _compile(self, scaled: dict | None = None, dequant: set | None = None, requant: set | None = None,
                  flags: int = 0, verbatim: dict | None = None) -> None:
         """Compile the cached transfer plan along the routes :meth:`_check_scales` chose: ``scaled`` is its
@@ -1057,7 +1075,8 @@ class DirectWeightSyncDest:
         local groups whichever part an element came from, and their route checks over the union of the parts'
         handles.  ValueError naming the destination and part, before anything is compiled, for an unknown name,
         a source without handles, a name with handles of its own, a bad index, a source box outside the source,
-        overlapping parts and a part the handles do not cover (DESIGN.md section 4, "Packed destinations").
+        overlapping parts, a part the handles do not cover, and a part whose int index drops the destination's last
+        dim on a dequantising or requantising route (DESIGN.md section 4, "Packed destinations").
         Elements outside every part are left alone.  Changing the spec rebuilds the plan.
 
         Scaled fp8 destinations (extension): float8_e4m3fn weights quantised during the pull from
@@ -1160,7 +1179,8 @@ class DirectWeightSyncDest:
                 self._plan_scale_dicts = scales
             verified = True
         if self._plan is None:
-            route_handles = _route_handles(all_handles, self._check_packed(all_handles, dest_state_dict, packed))
+            parts = self._check_packed(all_handles, dest_state_dict, packed)
+            route_handles = _route_handles(all_handles, parts)
             scaled = self._check_scales(route_handles, dest_state_dict, scale_dicts, requantize=requantize,
                                         verbatim=verbatim)
             if scale_fmt is not None and any(_is_int8(d) for _, d, *_ in scaled.values()):
@@ -1171,6 +1191,7 @@ class DirectWeightSyncDest:
                                  "tensor_scales is moved verbatim and keeps its source's scales")
             dequant = self._check_dequant(route_handles, dest_state_dict, scaled)
             requant = {n for n, (*_, route) in scaled.items() if route == "requantise"}
+            self._check_packed_rows(parts, dequant, requant)
             self._plan = self._build_plan(all_handles, dest_state_dict, dest_slices, packed=packed)
             try:
                 verbatim_rects = self._verbatim_rects(self._plan, scaled)
