@@ -85,7 +85,7 @@ int map_boxes(const tsb_rect_t& in, uint64_t index, const TargetGeom* targets, u
   const int64_t b0 = static_cast<int64_t>(o / (R * C)), r0 = static_cast<int64_t>(o % (R * C)) / C, c0 = static_cast<int64_t>(o % C);
   // Classify every dim by its grid step: columns (1), rows (C) or whole matrices (multiple of
   // R*C).  A collapsed dim that runs past the end of a row (or of a matrix) is split back.
-  int64_t er = 1, ec = 1, row_ss = 0, col_ss = es;
+  int64_t er = 1, ec = 1, row_ss = 0, col_ss = es, rstep = 1;
   bool have_row = false, have_col = false;
   std::vector<Dim> batch;
   const std::string bad = where + side.not_a_box;
@@ -116,6 +116,12 @@ int map_boxes(const tsb_rect_t& in, uint64_t index, const TargetGeom* targets, u
       } else {
         return fail(TSB_ERR_INVALID, bad);
       }
+    } else if (side.by_src && d.ds == 2 * C && r0 + 2 * (d.e - 1) < R) {  // a rotary head half: every other row
+      if (have_row) return fail(TSB_ERR_INVALID, bad);
+      have_row = true;
+      er = d.e;
+      row_ss = d.ss;
+      rstep = 2;
     } else if (d.ds > 0 && d.ds % (R * C) == 0) {
       batch.push_back({d.e, d.ss, d.ds / (R * C)});
     } else {
@@ -139,7 +145,7 @@ int map_boxes(const tsb_rect_t& in, uint64_t index, const TargetGeom* targets, u
     }
     out->push_back({other_ptr + static_cast<uint64_t>(so), row_ss, t, static_cast<uint64_t>(b), static_cast<uint64_t>(r0),
                     static_cast<uint64_t>(c0), static_cast<uint64_t>(er), static_cast<uint64_t>(ec),
-                    side.by_src ? in.dst_dtype : in.src_dtype, in.src_device});
+                    side.by_src ? in.dst_dtype : in.src_dtype, in.src_device, static_cast<uint32_t>(rstep)});
     size_t i = batch.size();
     while (i > 0 && ++k[i - 1] == batch[i - 1].e) k[--i] = 0;
     if (i == 0) break;

@@ -57,18 +57,22 @@ int dequant_fp8_compile(int device, const tsb_rect_t* rects, uint64_t n, const t
     // block grid of the shard's scale tensor: blocks anchored at the global origin
     const uint64_t br0 = S.row0 / kBqBlock, bc0 = S.col0 / kBqBlock;
     const uint64_t nbr = (S.row0 + S.rows + kBqBlock - 1) / kBqBlock - br0, nbc = (S.col0 + S.cols + kBqBlock - 1) / kBqBlock - bc0;
-    for (uint64_t y0 = x.r0; y0 < x.r0 + x.er;) {
-      const uint64_t y1 = block ? std::min(x.r0 + x.er, ((S.row0 + y0) / g + 1) * g - S.row0) : x.r0 + x.er;
+    // box row y reads source row x.r0 + rs * y (rs 2: a rotary head half); a block cut falls where that row
+    // crosses a block edge
+    const uint64_t rs = x.rstep;
+    for (uint64_t y0 = 0; y0 < x.er;) {
+      const uint64_t sy = x.r0 + rs * y0;
+      const uint64_t y1 = block ? std::min(x.er, y0 + (((S.row0 + sy) / g + 1) * g - S.row0 - sy + rs - 1) / rs) : x.er;
       for (uint64_t c0 = x.c0; c0 < x.c0 + x.ec;) {
         const uint64_t c1 = block ? std::min(x.c0 + x.ec, ((S.col0 + c0) / g + 1) * g - S.col0) : x.c0 + x.ec;
         uint64_t scale;
         if (block)
-          scale = S.scale + 4 * ((x.b * nbr + (S.row0 + y0) / kBqBlock - br0) * nbc + (S.col0 + c0) / kBqBlock - bc0);
+          scale = S.scale + 4 * ((x.b * nbr + (S.row0 + sy) / kBqBlock - br0) * nbc + (S.col0 + c0) / kBqBlock - bc0);
         else if (S.granularity == TSB_SCALE_PER_CHANNEL)
-          scale = S.scale + 4 * (x.b * S.rows + y0);
+          scale = S.scale + 4 * (x.b * S.rows + sy);
         else
           scale = S.scale + 4 * x.b;
-        const uint16_t step = S.granularity == TSB_SCALE_PER_CHANNEL ? 4 : 0;
+        const uint16_t step = S.granularity == TSB_SCALE_PER_CHANNEL ? static_cast<uint16_t>(4 * rs) : 0;
         const uint64_t h = y1 - y0, w = c1 - c0;
         const uint64_t tr = std::min<uint64_t>(kDqTileRows, std::max<uint64_t>(1, kDqTileElems / w));
         const uint64_t tc = std::min<uint64_t>(w, kDqTileElems);
@@ -78,9 +82,9 @@ int dequant_fp8_compile(int device, const tsb_rect_t* rects, uint64_t n, const t
             memset(&t, 0, sizeof(t));
             t.rows = static_cast<uint32_t>(std::min(tr, h - r));
             t.cols = static_cast<uint32_t>(std::min(tc, w - c));
-            t.src = S.src + (x.b * S.rows + y0 + r) * S.cols + c0 + c;
-            t.src_stride = static_cast<int64_t>(S.cols);
-            t.dst = x.src + (y0 + r - x.r0) * x.row_stride + (c0 + c - x.c0) * es;
+            t.src = S.src + (x.b * S.rows + sy + rs * r) * S.cols + c0 + c;
+            t.src_stride = static_cast<int64_t>(rs * S.cols);
+            t.dst = x.src + (y0 + r) * x.row_stride + (c0 + c - x.c0) * es;
             t.dst_stride = x.row_stride;
             t.scale = scale + step * r;
             t.scale_step = step;
@@ -180,15 +184,17 @@ __device__ __forceinline__ void dequant_tile(const DqTile& t, const float* s_sca
   }
 }
 
-// In: the source format, E4m3In or I8In (one per plan)
-template <class In>
+// In: the source format, E4m3In or I8In (one per plan).  kStepped: channel tiles may read every other source row
+// (a rotary head half), so a row's scale is scale_step bytes after the previous one; otherwise 4 bytes.
+template <class In, bool kStepped = false>
 __global__ void __launch_bounds__(kQuantThreads) dequant_fp8_kernel(const DqTile* __restrict__ tiles) {
   __shared__ float s_scale[kDqTileRows];
   const DqTile t = tiles[blockIdx.x];
   const float* scales = reinterpret_cast<const float*>(t.scale);
   float scale0 = 0.0f;
   if (t.scale_step) {  // per channel: one scale per row, fetched once
-    for (uint32_t r = threadIdx.x; r < t.rows; r += kQuantThreads) s_scale[r] = __ldg(scales + r);
+    for (uint32_t r = threadIdx.x; r < t.rows; r += kQuantThreads)
+      s_scale[r] = __ldg(kStepped ? scales + r * (t.scale_step / 4u) : scales + r);
     __syncthreads();
   } else {
     scale0 = __ldg(scales);
@@ -221,7 +227,10 @@ int dequant_fp8_plan(int device, const tsb_rect_t* rects, uint64_t n, const tsb_
   q->seal(0);
   const uint32_t n_tiles = static_cast<uint32_t>(tb.tiles.size());
   q->describe(n, n_tiles, kDqTileElems, tb);
-  const auto kernel = q->int8 ? dequant_fp8_kernel<I8In> : dequant_fp8_kernel<E4m3In>;
+  // plans with rotary channel tiles (scale step 8) take the stepped instantiations, every other plan the plain ones
+  const bool stepped = std::any_of(tb.tiles.begin(), tb.tiles.end(), [](const DqTile& t) { return t.scale_step > 4; });
+  const auto kernel = stepped ? (q->int8 ? dequant_fp8_kernel<I8In, true> : dequant_fp8_kernel<E4m3In, true>)
+                              : (q->int8 ? dequant_fp8_kernel<I8In> : dequant_fp8_kernel<E4m3In>);
   q->launch = [n_tiles, kernel](char* d, cudaStream_t s) {
     kernel<<<n_tiles, kQuantThreads, 0, s>>>(reinterpret_cast<const DqTile*>(d));
     return launched("dequant_fp8_kernel launch");

@@ -316,6 +316,7 @@ struct TargetBox {
   uint64_t target, b, r0, c0, er, ec;
   uint32_t dtype;
   int32_t src_device;
+  uint32_t rstep = 1;  // grid rows between the box's rows: 2 for a rotary head half mapped by its source, else 1
 };
 uint32_t quant_src_bytes(uint32_t dtype);  // 4 / 2 for TSB_F32 / TSB_BF16, TSB_F16; 0 otherwise
 // Append one box per combination of the rect's batch dims to `out` (nothing for an empty rect).
@@ -323,7 +324,8 @@ int rect_boxes(const tsb_rect_t& in, uint64_t index, const TargetGeom* targets, 
                std::vector<TargetBox>* out);
 // The same mapping from the other side: the rect's *source* is located on the fp8 grids (its
 // TargetGeom::dst is the grid's base), and a box's `src` / `row_stride` / `dtype` describe the
-// destination side.  Destination columns must be contiguous.
+// destination side.  Destination columns must be contiguous.  A row dim that steps two grid rows (a rotary
+// head half, read in interleaved order) gives a box of rows r0, r0 + 2, ... (TargetBox::rstep 2).
 int rect_source_boxes(const tsb_rect_t& in, uint64_t index, const TargetGeom* grids, uint64_t n_grids,
                       std::vector<TargetBox>* out);
 // Whether the rects of a quantising pull (each already checked by rect_boxes) write int8 (TSB_I8) rather than
@@ -442,7 +444,7 @@ struct alignas(8) DqTile {
   int64_t src_stride;    // bytes between source rows
   int64_t dst_stride;    // bytes between destination rows
   uint32_t rows, cols;
-  uint16_t scale_step;   // bytes between the scales of consecutive rows: 4 (channel) or 0
+  uint16_t scale_step;   // bytes between the scales of consecutive rows: 4 * source row step (channel) or 0
   uint8_t dst_dtype;     // TSB_F32 / TSB_BF16 / TSB_F16
   uint8_t vec;           // 1: source and destination rows start 16-byte aligned (16-element chunks vectorise)
   uint32_t pad_;

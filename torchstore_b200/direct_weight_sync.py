@@ -201,7 +201,7 @@ def scale_grid(granularity: str, shape: tuple, row0: int, col0: int) -> tuple:
 
 
 def verbatim_scale_rects(granularity: str, shape: tuple, offset: tuple, ops: list, *,
-                         src_starts: list | None = None) -> tuple[list, tuple | None]:
+                         src_starts: list | None = None, src_rows: list | None = None) -> tuple[list, tuple | None]:
     """Map the scales of a verbatim pull: fp8 bytes and scales of same-granularity sources moved as they are.
 
     ``shape`` and ``offset`` are the destination's local shape and global offset (all dims); each op is
@@ -209,7 +209,9 @@ def verbatim_scale_rects(granularity: str, shape: tuple, offset: tuple, ops: lis
     Destination groups are anchored at the destination's local origin (128x128 blocks, rows, or the matrix
     per leading index); source groups at the global origin, cut by the source shard.  ``src_starts`` (packed
     destinations) gives, per op, the source's global coordinates of the rectangle's first element, where they
-    differ from the destination's; without it the two coordinate systems are the same.
+    differ from the destination's; without it the two coordinate systems are the same.  ``src_rows`` (rotary packed
+    parts, with ``src_starts``) gives, per op, None or ``(hd, heads, halves, rows)``: the op's rows in the destination's
+    dim -2 are (heads, halves, rows) whose source rows step by (hd, 1, 2) from its first (:class:`PackedPart`).
 
     Returns ``(rects, None)`` when every destination group lies inside one source group of one op:
     ``rects[i] = (op index, source index, destination index)``, unit-step slices into the :func:`scale_grid`
@@ -229,12 +231,16 @@ def verbatim_scale_rects(granularity: str, shape: tuple, offset: tuple, ops: lis
     else:
         size, src_size = size + [rows, cols], src_size + [None, None]
     starts = src_starts if src_starts is not None else [g_off for _, _, (g_off, _) in ops]
+    row_maps = src_rows if src_rows is not None else [None] * len(ops)
     local = []  # op rectangles in destination-local coordinates: [(start, stop) per dim]
     volume = 0
-    for (src_shape, src_off, (g_off, ext)), sg in zip(ops, starts):
+    for (src_shape, src_off, (g_off, ext)), sg, rm in zip(ops, starts, row_maps):
         box = [(g - o, g - o + e) for g, o, e in zip(g_off, offset, ext)]
+        sext = list(ext)
+        if rm is not None:  # the source rows the op reads: whole heads, or one head half of step 2
+            sext[-2] = rm[1] * rm[0] if rm[2] == 2 else 2 * rm[3] - 1
         if any(s < 0 or t > n or s >= t for (s, t), n in zip(box, shape)) or \
-                any(g < so or g + e > so + n for g, e, so, n in zip(sg, ext, src_off, src_shape)):
+                any(g < so or g + e > so + n for g, e, so, n in zip(sg, sext, src_off, src_shape)):
             raise ValueError(f"op rectangle at {tuple(g_off)} extent {tuple(ext)} is empty or leaves its source shard "
                              "or the destination")
         local.append(box)
@@ -268,17 +274,20 @@ def verbatim_scale_rects(granularity: str, shape: tuple, offset: tuple, ops: lis
                     bad.append(tuple(j if e == d else 0 for e in range(nd)))
                     break
             continue
-        for box, sg in zip(local, starts):  # packed: each op's own shift between the two coordinate systems
+        for box, sg, rm in zip(local, starts, row_maps):  # packed: each op's own shift between the two coordinate systems
             s0, t0 = box[d]
             for j in range(*groups(d, s0, t0)):
-                s, t = sg[d] + max(s0, j * size[d]) - s0, sg[d] + min(t0, (j + 1) * size[d]) - s0
+                lo, hi = max(s0, j * size[d]) - s0, min(t0, (j + 1) * size[d]) - s0
+                if rm is not None and d == nd - 2:  # the rows' image under the rotary order: its first and last
+                    lo, hi = _rotary_image(rm, lo, hi)
+                s, t = sg[d] + lo, sg[d] + hi
                 if s // src_size[d] != (t - 1) // src_size[d]:
                     bad.append(tuple(j if e == d else groups(e, *box[e])[0] for e in range(nd)))
                     break
     if bad:
         return [], min(bad)
     rects = []
-    for i, (box, (_, src_off, _), sg) in enumerate(zip(local, ops, starts)):
+    for i, (box, (_, src_off, _), sg, rm) in enumerate(zip(local, ops, starts, row_maps)):
         src_idx, dst_idx = [], []
         for d, (s, t) in enumerate(box):
             j0, j1 = groups(d, s, t)
@@ -286,8 +295,46 @@ def verbatim_scale_rects(granularity: str, shape: tuple, offset: tuple, ops: lis
             k0 = 0 if src_size[d] is None else g0 // src_size[d] - src_off[d] // src_size[d]
             src_idx.append(slice(k0, k0 + j1 - j0))
             dst_idx.append(slice(j0, j1))
-        rects.append((i, tuple(src_idx), tuple(dst_idx)))
+        if rm is None or src_size[nd - 2] is None:
+            rects.append((i, tuple(src_idx), tuple(dst_idx)))
+            continue
+        # rotary rows: per destination row group, the source group holding its image (one source row per channel)
+        s, t = box[nd - 2]
+        pieces = []  # (source start, step, destination start, count) along the rows
+        if granularity == "channel":
+            hd, heads, halves, rows = rm
+            for a in range(heads):
+                for b in range(halves):
+                    pieces.append((sg[nd - 2] - src_off[nd - 2] + a * hd + b, 2, s + (a * halves + b) * rows, rows))
+        else:
+            for j in range(*groups(nd - 2, s, t)):
+                lo, _ = _rotary_image(rm, max(s, j * BLOCK) - s, min(t, (j + 1) * BLOCK) - s)
+                k = (sg[nd - 2] + lo) // BLOCK - src_off[nd - 2] // BLOCK
+                if pieces and pieces[-1][0] + pieces[-1][3] == k and pieces[-1][2] + pieces[-1][3] == j:
+                    pieces[-1] = pieces[-1][:3] + (pieces[-1][3] + 1,)
+                else:
+                    pieces.append((k, 1, j, 1))
+        for k, step, j, n in pieces:
+            src_idx[nd - 2], dst_idx[nd - 2] = slice(k, k + step * (n - 1) + 1, step), slice(j, j + n)
+            rects.append((i, tuple(src_idx), tuple(dst_idx)))
     return rects, None
+
+
+def _rotary_image(rm: tuple, lo: int, hi: int) -> tuple[int, int]:
+    """``(first, last + 1)`` of the source rows (relative to the op's first) that the op's destination rows
+    ``[lo, hi)`` read, for the rotary row map ``rm = (hd, heads, halves, rows)`` (:func:`verbatim_scale_rects`)."""
+    hd, _, halves, rows = rm
+    def src(i):
+        a, r = divmod(i, halves * rows)
+        b, c = divmod(r, rows)
+        return a * hd + b + 2 * c
+    first = last = src(lo)
+    i = lo
+    while i < hi:  # per head half, the rows of [lo, hi) are one progression of step 2
+        end = min(hi, (i // rows + 1) * rows)
+        first, last = min(first, src(i)), max(last, src(end - 1))
+        i = end
+    return first, last + 1
 
 
 @dataclass(frozen=True)
@@ -299,11 +346,19 @@ class PackedPart:
     handles named ``source``, starting at global offsets ``source_offsets`` of the source tensor (one per source
     dim: the box's rank after the int entries are dropped).  Each element at local index ``i`` of the box takes
     the source's value at ``source_offsets + (i - box start)``, through the route the destination's dtype and
-    scale dicts select (DESIGN.md section 4, "Packed destinations")."""
+    scale dicts select (DESIGN.md section 4, "Packed destinations").
+
+    ``rotary_head_dim = hd`` reorders the rows of every head, as a torchtitan (Meta) Llama's ``wq`` / ``wk`` need
+    on their way into a Hugging Face / vLLM ``qkv_proj``: the source holds each head's ``hd`` rows (its dim -2) in
+    interleaved rotary order, pairs ``(2j, 2j + 1)``, and the destination receives them in half-split order, pairs
+    ``(j, j + hd / 2)``.  A box element whose component along the source's dim -2 is ``h * hd + t * hd / 2 + j``
+    (``t`` in {0, 1}) reads source row ``source_offsets[-2] + h * hd + 2 * j + t``; every other dim is as above.
+    ``None`` keeps the rows in order."""
 
     source: str
     dest_index: tuple
     source_offsets: tuple
+    rotary_head_dim: int | None = None
 
 
 @dataclass
@@ -609,6 +664,10 @@ class _TransferOp:
     # coordinates are the source's), and the destination dims an int index dropped (unit slices in dest_slices)
     src_start: tuple | None = None
     dest_dropped: tuple = ()
+    # rotary parts: (destination dim of the source's rows, head dim hd, heads, halves, rows per half).  The op's rows
+    # are (heads, halves, rows) with source row steps (hd, 1, 2) and destination row steps (hd, hd / 2, 1) from its
+    # first row; src_slices then bound the source rows it reads
+    rotary: tuple | None = None
 
 
 class DirectWeightSyncDest:
@@ -715,6 +774,10 @@ class DirectWeightSyncDest:
         src, dst = src_window.sub(op.src_slices), dst_full.sub(op.dest_slices)
         if op.dest_dropped:  # a packed part whose int index dropped destination dims: unit dims on the source side
             src = StridedMem(src.ptr, dst.shape, _lift(src.stride, op.dest_dropped, 0), src.dtype, src.device)
+        if getattr(op, "rotary", None) is not None:
+            k, hd, heads, halves, rows = op.rotary
+            src = _split_rows(src, k, (heads, halves, rows), (hd, 1, 2))
+            dst = _split_rows(dst, k, (heads, halves, rows), (hd, hd // 2, 1))
         return src, dst
 
     @staticmethod
@@ -748,6 +811,19 @@ class DirectWeightSyncDest:
                 if any(o < 0 or o + e > g for o, e, g in zip(offs, ext, gshape)):
                     raise ValueError(f"{what}: the source box at {offs} with extent {tuple(ext)} leaves the source's "
                                      f"global shape {gshape}")
+                hd = part.rotary_head_dim
+                if hd is not None:
+                    if not isinstance(hd, int) or isinstance(hd, bool) or hd <= 0 or hd % 2:
+                        raise ValueError(f"{what}: rotary_head_dim must be None or a positive even int, not {hd!r}")
+                    if len(gshape) < 2:
+                        raise ValueError(f"{what}: rotary_head_dim reorders the rows (dim -2) of each head, and the "
+                                         f"source has {len(gshape)} dim")
+                    if ext[-2] % hd:
+                        raise ValueError(f"{what}: its extent {ext[-2]} along the source's dim -2 is not a multiple of "
+                                         f"rotary_head_dim {hd}")
+                    if offs[-2] % hd:
+                        raise ValueError(f"{what}: source_offsets[-2] ({offs[-2]}) is not a multiple of rotary_head_dim "
+                                         f"{hd} (heads start at source row 0)")
                 for j, _, other, _, _ in entries:
                     if all(max(s, a) < min(t, b) for (s, t), (a, b) in zip(box, other)):
                         raise ValueError(f"{what}: its box overlaps part {j}'s")
@@ -877,6 +953,7 @@ class DirectWeightSyncDest:
                 raise ValueError(f"verbatim pull of '{name}' ({kw}): no handle covers its destination")
             shape, offset = tuple(dest.shape), mine[0].dest_offsets
             rects, starts = [], []
+            rows = [op.rotary[1:] if getattr(op, "rotary", None) is not None else None for op in mine]
             for op in mine:
                 start = [0] * len(shape) if op.dest_slices is None else [s.start for s in op.dest_slices]
                 ext = shape if op.dest_slices is None else [s.stop - s.start for s in op.dest_slices]
@@ -889,7 +966,8 @@ class DirectWeightSyncDest:
                     starts.append(_lift(op.src_start, op.dest_dropped, 0))
                 rects.append((src_shape, src_off, (tuple(o + s for o, s in zip(offset, start)), tuple(ext))))
             try:
-                mapped, group = verbatim_scale_rects(granularity, shape, offset, rects, src_starts=starts or None)
+                mapped, group = verbatim_scale_rects(granularity, shape, offset, rects, src_starts=starts or None,
+                                                     src_rows=rows if any(rows) else None)
             except ValueError as e:
                 raise ValueError(f"verbatim pull of '{name}' ({kw}): {e}") from None
             if group is not None:
@@ -982,7 +1060,7 @@ class DirectWeightSyncDest:
                 buf = op.rdma_buffer
                 grid = _lift(scale_grid(granularity, tuple(buf.shape), buf.row0, buf.col0), op.dest_dropped, 1)
                 src = _as_grid(buf.scale_window(dev), grid)
-                per_device[dev].append((src.sub(src_idx), dst.sub(dst_idx)))
+                per_device[dev].append((_stepped_sub(src, src_idx), dst.sub(dst_idx)))
         # (int8 sources, device) -> (windows, {source buffer id: (name, DqSource)}): a plan reads one source format
         dq: dict[tuple, tuple[list, dict]] = {}
         quant: dict[tuple, tuple] = defaultdict(lambda: ([], {}, [], []))  # (kind, device) -> the same, names, targets
@@ -999,14 +1077,17 @@ class DirectWeightSyncDest:
                 )
             dev = dest.device.index
             window = self.op_windows(op, op.rdma_buffer.window(dev))
+            rotary = getattr(op, "rotary", None)  # plan ops built by hand (tests) may lack it
+            grid = op.name in kind or (dequant and op.name in dequant)
+            windows = _head_halves(window, rotary) if grid and rotary is not None else [window]
             if op.name in kind:
                 pairs, sources, _, _ = quant[(kind[op.name], dev)]
-                pairs.append(window)
+                pairs += windows
                 if kind[op.name] == 0:
                     _add_dq_source(sources, op, dev)
             elif dequant and op.name in dequant:
                 pairs, sources = dq.setdefault((op.rdma_buffer.dtype == torch.int8, dev), ([], {}))
-                pairs.append(window)
+                pairs += windows
                 _add_dq_source(sources, op, dev)
             else:
                 per_device[dev].append(window)
@@ -1340,7 +1421,8 @@ def _packed_key(packed: dict | None) -> frozenset | None:
             if not isinstance(p.dest_index, tuple) or not isinstance(p.source_offsets, tuple):
                 raise TypeError(f"packed['{name}']: dest_index and source_offsets of a PackedPart must be tuples")
         out.append((name, tuple((p.source, tuple((e.start, e.stop, e.step) if isinstance(e, slice) else e
-                                                 for e in p.dest_index), p.source_offsets) for p in parts)))
+                                                 for e in p.dest_index), p.source_offsets, p.rotary_head_dim)
+                                for p in parts)))
     return frozenset(out)
 
 
@@ -1397,14 +1479,84 @@ def _packed_ops(name: str, dest: torch.Tensor, dest_offsets: tuple, entries: lis
             if any(t <= s for s, t in zip(lo, hi)) or (lo, hi) in seen:
                 continue
             seen.add((lo, hi))
-            dst_idx = [slice(s, t) for s, t in box]
-            for i, d in enumerate(kept):
-                dst_idx[d] = slice(box[d][0] + lo[i] - so[i], box[d][0] + hi[i] - so[i])
-            ops.append(_TransferOp(rdma_buffer=h.rdma_buffer, dest_byte_view=None, dest_tensor=dest,
-                                   src_slices=tuple(slice(s - o, t - o) for s, t, o in zip(lo, hi, ho)),
-                                   dest_slices=tuple(dst_idx), name=name, dest_local=dest, dest_offsets=dest_offsets,
-                                   src_offsets=tuple(ho), src_start=lo, dest_dropped=dropped))
+            # rotary parts: (first source row, first destination row of the box, row spans) of the handle's rows
+            pieces = [(None, None, None)] if part.rotary_head_dim is None else \
+                _rotary_pieces(so[-2], part.rotary_head_dim, lo[-2], hi[-2])
+            for srow, drow, rotary in pieces:
+                slo, shi, dlo, dhi = list(lo), list(hi), [a - b for a, b in zip(lo, so)], [a - b for a, b in zip(hi, so)]
+                if rotary is not None:
+                    heads, halves, rows = rotary
+                    n_dst = heads * halves * rows
+                    n_src = heads * part.rotary_head_dim if halves == 2 else 2 * rows - 1
+                    slo[-2], shi[-2], dlo[-2], dhi[-2] = srow, srow + n_src, drow, drow + n_dst
+                    rotary = (kept[-2], part.rotary_head_dim) + rotary
+                dst_idx = [slice(s, t) for s, t in box]
+                for i, d in enumerate(kept):
+                    dst_idx[d] = slice(box[d][0] + dlo[i], box[d][0] + dhi[i])
+                ops.append(_TransferOp(rdma_buffer=h.rdma_buffer, dest_byte_view=None, dest_tensor=dest,
+                                       src_slices=tuple(slice(s - o, t - o) for s, t, o in zip(slo, shi, ho)),
+                                       dest_slices=tuple(dst_idx), name=name, dest_local=dest, dest_offsets=dest_offsets,
+                                       src_offsets=tuple(ho), src_start=tuple(slo), dest_dropped=dropped, rotary=rotary))
     return ops
+
+
+def _rotary_pieces(r0: int, hd: int, a: int, b: int) -> list[tuple]:
+    """The source rows ``[a, b)`` of a rotary part whose heads start at source row ``r0`` (a multiple of ``hd``
+    rows before ``a``), as ``(first source row, its row in the part's box, (heads, halves, rows))`` pieces: one
+    piece for the whole heads, and one per head half that the handle's edges cut (one arithmetic progression of
+    step 2 each)."""
+    h2 = hd // 2
+    first, last = -(-(a - r0) // hd), (b - r0) // hd  # whole heads [first, last)
+    if first >= last:
+        return [p for h in range((a - r0) // hd, -(-(b - r0) // hd)) for p in _half_pieces(r0, hd, h, a, b)]
+    lead = [p for h in range((a - r0) // hd, first) for p in _half_pieces(r0, hd, h, a, b)]
+    tail = _half_pieces(r0, hd, last, a, b) if last * hd + r0 < b else []
+    return lead + [(r0 + first * hd, first * hd, (last - first, 2, h2))] + tail
+
+
+def _half_pieces(r0: int, hd: int, h: int, a: int, b: int) -> list[tuple]:
+    """The pieces of head ``h`` inside source rows ``[a, b)``: per half ``t``, rows ``r0 + h * hd + t + 2j``."""
+    h2, out = hd // 2, []
+    for t in (0, 1):
+        base = r0 + h * hd + t
+        j0, j1 = max(0, -(-(a - base) // 2)), min(h2, -(-(b - base) // 2))
+        if j0 < j1:
+            out.append((base + 2 * j0, h * hd + t * h2 + j0, (1, 1, j1 - j0)))
+    return out
+
+
+def _split_rows(win: StridedMem, k: int, shape: tuple, steps: tuple) -> StridedMem:
+    """``win`` with its dim ``k`` replaced by dims of extents ``shape`` and strides ``steps`` times its row stride."""
+    st = win.stride[k]
+    return StridedMem(win.ptr, win.shape[:k] + shape + win.shape[k + 1:],
+                      win.stride[:k] + tuple(s * st for s in steps) + win.stride[k + 1:], win.dtype, win.device)
+
+
+def _head_halves(window: tuple, rotary: tuple) -> list[tuple]:
+    """The (source, destination) windows of a rotary op (:meth:`DirectWeightSyncDest.op_windows`) cut into one pair per
+    head half, each a plain box of destination rows whose source rows step by 2: the kernels that map a rect onto a
+    scale grid take one row dim."""
+    k = rotary[0]
+    src, dst = window
+    heads, halves, rows = src.shape[k:k + 3]
+    out = []
+    for h in range(heads):
+        for t in range(halves):
+            pair = []
+            for w in (src, dst):
+                off = (h * w.stride[k] + t * w.stride[k + 1]) * w.itemsize
+                pair.append(StridedMem(w.ptr + off, w.shape[:k] + (rows,) + w.shape[k + 3:],
+                                       w.stride[:k] + (w.stride[k + 2],) + w.stride[k + 3:], w.dtype, w.device))
+            out.append(tuple(pair))
+    return out
+
+
+def _stepped_sub(win: StridedMem, index: tuple) -> StridedMem:
+    """``win[index]`` for slices of positive step (:meth:`StridedMem.sub` takes unit steps only)."""
+    base = win.sub(tuple(slice(s.start, s.stop) for s in index))
+    shape = tuple(len(range(s.start, s.stop, s.step or 1)) for s in index)
+    stride = tuple(st * (s.step or 1) for st, s in zip(win.stride, index))
+    return StridedMem(base.ptr, shape, stride, win.dtype, win.device)
 
 
 def _route_handles(all_handles: dict, parts: dict) -> dict:

@@ -94,21 +94,20 @@ _HF_LLAMA = {"attention.wq": "self_attn.q_proj", "attention.wk": "self_attn.k_pr
              "feed_forward.w3": "mlp.up_proj", "attention_norm": "input_layernorm", "ffn_norm": "post_attention_layernorm"}
 
 
+def hf_name(name: str) -> str:
+    """The Hugging Face name of a :func:`llama_layout` (torchtitan) name."""
+    if name.startswith("layers."):
+        _, i, rest = name.split(".", 2)
+        return f"model.layers.{i}.{_HF_LLAMA[rest.removesuffix('.weight')]}.weight"
+    return {"tok_embeddings.weight": "model.embed_tokens.weight", "norm.weight": "model.norm.weight",
+            "output.weight": "lm_head.weight"}[name]
+
+
 def hf_llama_layout(cfg=LLAMA3_8B, n_layers: int | None = None, scale: int = 1, with_embeddings: bool = True):
     """:func:`llama_layout` under the Hugging Face names a trainer of an HF-layout model publishes
     (``model.layers.{i}.self_attn.q_proj.weight``, ``mlp.gate_proj``, ``model.embed_tokens``, ``lm_head``, ...):
     the same shapes and placements, in the same order."""
-    out = {}
-    for name, entry in llama_layout(cfg, n_layers, scale, with_embeddings).items():
-        if name.startswith("layers."):
-            _, i, rest = name.split(".", 2)
-            mod = rest.removesuffix(".weight")
-            name = f"model.layers.{i}.{_HF_LLAMA[mod]}.weight"
-        else:
-            name = {"tok_embeddings.weight": "model.embed_tokens.weight", "norm.weight": "model.norm.weight",
-                    "output.weight": "lm_head.weight"}[name]
-        out[name] = entry
-    return out
+    return {hf_name(name): entry for name, entry in llama_layout(cfg, n_layers, scale, with_embeddings).items()}
 
 
 def qwen3_moe_layout(cfg=QWEN3_MOE, n_layers: int | None = None, scale: int = 1, with_embeddings: bool = True,
@@ -145,9 +144,15 @@ def qwen3_moe_layout(cfg=QWEN3_MOE, n_layers: int | None = None, scale: int = 1,
     return out
 
 
-def vllm_tp_layout(hf_layout, cfg, tp: int, rank: int, ep: bool = False):
+def vllm_tp_layout(hf_layout, cfg, tp: int, rank: int, ep: bool = False, source: str = "hf"):
     """What vLLM tensor-parallel rank ``rank`` of ``tp`` holds for ``hf_layout`` (:func:`hf_llama_layout` or
     :func:`qwen3_moe_layout` of ``cfg``): vLLM name -> (local shape, parts, box).
+
+    ``source="torchtitan"`` reads a torchtitan trainer instead: ``hf_layout`` is then a :func:`llama_layout`
+    (``layers.{i}.attention.wq.weight``, ...), and every vLLM parameter is a packed destination whose parts read the
+    torchtitan names (wq / wk / wv into ``qkv_proj``, w1 / w3 into ``gate_up_proj``, and one part per renamed tensor:
+    wo, w2, tok_embeddings, output and the norms).  The q and k parts carry ``rotary_head_dim = dim / n_heads``:
+    torchtitan keeps Meta's interleaved rotary rows, vLLM (like Hugging Face) the half-split ones.
 
     * Fused parameters have ``parts``, a tuple of ``PackedPart`` reading the HF tensors, and ``box`` None:
       ``qkv_proj`` = ``[q_r; k_r; v_r]`` (rank r's query heads, then its kv head(s): when tp exceeds the kv heads,
@@ -159,6 +164,10 @@ def vllm_tp_layout(hf_layout, cfg, tp: int, rank: int, ep: bool = False):
       ``lm_head`` row shards, replicated norms and router."""
     from torchstore_b200.direct_weight_sync import PackedPart
 
+    if source == "torchtitan":
+        return _from_torchtitan(hf_layout, cfg, tp, rank, ep)
+    if source != "hf":
+        raise ValueError(f"source must be 'hf' or 'torchtitan', not {source!r}")
     n_heads, n_kv = cfg["n_heads"], cfg["n_kv_heads"]
     if n_heads % tp or (n_kv % tp and tp % n_kv):
         raise ValueError(f"tp={tp} must divide {n_heads} query heads and divide or be a multiple of {n_kv} kv heads")
@@ -216,4 +225,26 @@ def vllm_tp_layout(hf_layout, cfg, tp: int, rank: int, ep: bool = False):
                 placement = ("R",)
             off, loc = shard_box(shape, tp, rank, placement) if tp > 1 else ((0,) * len(shape), tuple(shape))
             out[name] = (tuple(loc), None, (tuple(off), tuple(shape)))
+    return out
+
+
+def _from_torchtitan(titan_layout, cfg, tp: int, rank: int, ep: bool):
+    """:func:`vllm_tp_layout` with ``source="torchtitan"``: the HF layout's parts renamed back to the torchtitan
+    tensors, the q and k parts rotary, and every unpacked parameter one part of its renamed tensor."""
+    import dataclasses
+
+    from torchstore_b200.direct_weight_sync import PackedPart
+
+    back = {hf_name(n): n for n in titan_layout}
+    hf = {hf_name(n): e for n, e in titan_layout.items()}
+    out = {}
+    for name, (shape, parts, box) in vllm_tp_layout(hf, cfg, tp, rank, ep).items():
+        if parts is None:
+            parts = (PackedPart(back[name], tuple(slice(0, e) for e in shape), tuple(box[0])),)
+        else:
+            hd = hf[parts[0].source][0][0] // cfg["n_heads"] if name.endswith("qkv_proj.weight") else None
+            parts = tuple(dataclasses.replace(p, source=back[p.source],
+                                              rotary_head_dim=hd if p.source.endswith(("q_proj.weight", "k_proj.weight"))
+                                              else None) for p in parts)
+        out[name] = (tuple(shape), parts, None)
     return out
