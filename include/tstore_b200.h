@@ -448,6 +448,31 @@ int tsb_source_quant_compile_host_as(int device, const tsb_source_quant_target_t
                                      uint64_t* out_n_groups);
 
 /* ------------------------------------------------------------------------------------------ */
+/* transposing pulls: input-major sources into output-major destinations                       */
+/* ------------------------------------------------------------------------------------------ */
+
+/* Compile a transposing pull: `rects` are ordinary tsb_rect_t with 2 <= ndim <= TSB_MAX_DIMS whose destination is
+ * contiguous along dim ndim-1 (dst_stride == its element size) and whose source is contiguous along dim ndim-2
+ * (src_stride == its element size); a dim of extent 1 is exempt from its rule.  The outer dims take any strides, and
+ * src may be local or peer-mapped.  Element (o, i, j) becomes dst[o, i, j] = to_dst(src[o, i, j]) as for the copy
+ * plan, but the mover reads 16-byte sectors along the source's dim ndim-2 and writes them along the destination's
+ * dim ndim-1 (a 2-D transpose through shared memory).  Same-dtype moves of 1-, 2-, 4- and 8-byte elements and every
+ * pair of tsb_cast_supported are accepted; any other pair is TSB_ERR_UNSUPPORTED, any other rect TSB_ERR_INVALID,
+ * both naming "rect N".  The result is a plan like any other: tsb_plan_launch[_flags], _run, _poll, _wait,
+ * _elapsed_ms, _info and _destroy accept it.  flags: reserved, pass 0. */
+int tsb_transpose_plan_create(int device, const tsb_rect_t* rects, uint64_t n, uint32_t flags, tsb_plan_t* out);
+/* Host-only (no CUDA call): compile and copy the tile table out (grouped by dtype pair, rect order inside a group).
+ * out_tiles: records of 48 bytes
+ *   {u64 src, u64 dst, i64 src_stride_bytes, i64 dst_stride_bytes, u32 rows, u32 cols, u8 src_dtype, u8 dst_dtype,
+ *    u8 vector, u8 pad, u32 pad}
+ * (tile element (i, j), i < rows, j < cols, moves from src + i * src_elem + j * src_stride_bytes to
+ * dst + i * dst_stride_bytes + j * dst_elem; tiles are at most 64 x 64 elements for 1- and 2-byte sources, 32 x 32
+ * otherwise; vector bit 0: 16-byte source loads, bit 1: 16-byte destination stores, each set only where that side's
+ * address and stride are 16-byte aligned).  A NULL table only reports its count. */
+int tsb_transpose_compile_host(int device, const tsb_rect_t* rects, uint64_t n, uint32_t flags, void* out_tiles,
+                               uint64_t tile_cap, uint64_t* out_n_tiles);
+
+/* ------------------------------------------------------------------------------------------ */
 /* streams and events (the await points of the reference's coroutines)                         */
 /* ------------------------------------------------------------------------------------------ */
 

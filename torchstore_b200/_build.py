@@ -13,8 +13,8 @@ CSRC = os.path.join(PKG_DIR, "csrc")
 LIB_DIR = os.path.join(PKG_DIR, "lib")
 LIB_PATH = os.path.join(LIB_DIR, "libtstore_b200.so")
 SOURCES = ["copy_rects.cu", "plan.cu", "runtime.cu", "host_tier.cu", "block_fp8.cu", "scaled_fp8.cu", "dequant_fp8.cu",
-           "requant_fp8.cu", "source_quant.cu"]
-HEADERS = [os.path.join(CSRC, "tsb_internal.h"), os.path.join(CSRC, "fp8_cvt.cuh"), os.path.join(CSRC, "fp8_quant.cuh"),
+           "requant_fp8.cu", "source_quant.cu", "transpose_rects.cu"]
+HEADERS = [os.path.join(CSRC, "tsb_internal.h"), os.path.join(CSRC, "fp8_cvt.cuh"), os.path.join(CSRC, "cast_cvt.cuh"), os.path.join(CSRC, "fp8_quant.cuh"),
            os.path.join(REPO_ROOT, "include", "tstore_b200.h")]
 
 NVCC_FLAGS = [

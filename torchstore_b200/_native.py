@@ -246,6 +246,10 @@ _SIGNATURES = {
         [C.c_int, C.POINTER(SourceQuantTarget), C.c_uint64, C.c_uint32, C.c_uint32, _vp, C.c_uint64, C.POINTER(C.c_uint64),
          _vp, C.c_uint64, C.POINTER(C.c_uint64), C.POINTER(C.c_uint64)],
     ),
+    "tsb_transpose_plan_create": (C.c_int, [C.c_int, C.POINTER(Rect), C.c_uint64, C.c_uint32, C.POINTER(C.c_uint64)]),
+    "tsb_transpose_compile_host": (
+        C.c_int, [C.c_int, C.POINTER(Rect), C.c_uint64, C.c_uint32, _vp, C.c_uint64, C.POINTER(C.c_uint64)],
+    ),
     "tsb_stream_create": (C.c_int, [C.c_int, C.POINTER(_vp)]),
     "tsb_stream_destroy": (C.c_int, [_vp]),
     "tsb_stream_sync": (C.c_int, [C.c_int, _vp]),
@@ -638,6 +642,20 @@ def source_quant_compile_host(device: int, targets, n: int, flags: int = 0, dst_
     else:
         fn, args = lib().tsb_source_quant_compile_host_as, (device, targets, n, dst_dtype)
     return tuple(_compile_host(fn, args, [SRCQ_UNIT_DTYPE, SQ_TILE_DTYPE], True, flags))
+
+
+def transpose_plan_create(device: int, rects, n: int, flags: int = 0) -> int:
+    return _plan_create(lib().tsb_transpose_plan_create, device, rects, n, flags=flags)
+
+
+# record layout of tsb_transpose_compile_host (include/tstore_b200.h)
+TR_TILE_DTYPE = [("src", "<u8"), ("dst", "<u8"), ("src_stride", "<i8"), ("dst_stride", "<i8"), ("rows", "<u4"),
+                 ("cols", "<u4"), ("src_dtype", "u1"), ("dst_dtype", "u1"), ("vec", "u1"), ("pad0", "u1"), ("pad1", "<u4")]
+
+
+def transpose_compile_host(device: int, rects, n: int, flags: int = 0):
+    """Host-only compilation of a transposing pull -> its tile table as a numpy record array."""
+    return _compile_host(lib().tsb_transpose_compile_host, (device, rects, n), [TR_TILE_DTYPE], False, flags)[0]
 
 
 CUDA_STREAM_LEGACY = 0x1  # cudaStreamLegacy: an explicit handle for the default stream

@@ -353,12 +353,23 @@ class PackedPart:
     interleaved rotary order, pairs ``(2j, 2j + 1)``, and the destination receives them in half-split order, pairs
     ``(j, j + hd / 2)``.  A box element whose component along the source's dim -2 is ``h * hd + t * hd / 2 + j``
     (``t`` in {0, 1}) reads source row ``source_offsets[-2] + h * hd + 2 * j + t``; every other dim is as above.
-    ``None`` keeps the rows in order."""
+    ``None`` keeps the rows in order.
+
+    ``transpose = True`` reads an input-major source into an output-major destination, as a grouped-GEMM trainer's
+    MoE experts (``w1`` / ``w3`` ``[E, dim, hidden]``, ``w2`` ``[E, hidden, dim]``) need on their way into vLLM's
+    ``w13_weight`` / ``w2_weight``: the box, after its int dims are dropped, has shape ``(..., a, b)`` and reads the
+    source box of shape ``(..., b, a)`` at ``source_offsets`` (in the source's own coordinates), its last two dims
+    swapped.  A box element at ``(..., i, j)`` reads source index ``source_offsets + (..., j, i)``.  The swapped dims
+    must be the destination's last two (no int index on them), the source needs at least 2 dims, and it does not
+    combine with ``rotary_head_dim``.  Transposed parts take the element-wise routes only (byte copies, fused casts,
+    ``transfer_dtype`` staging): a quantised destination (a scale dict names it) and scaled source handles are
+    refused (DESIGN.md section 4, "Transposed packed parts")."""
 
     source: str
     dest_index: tuple
     source_offsets: tuple
     rotary_head_dim: int | None = None
+    transpose: bool = False
 
 
 @dataclass
@@ -668,6 +679,8 @@ class _TransferOp:
     # are (heads, halves, rows) with source row steps (hd, 1, 2) and destination row steps (hd, hd / 2, 1) from its
     # first row; src_slices then bound the source rows it reads
     rotary: tuple | None = None
+    # transposed parts: src_slices index the source in its own order; op_windows swaps its last two dims
+    transpose: bool = False
 
 
 class DirectWeightSyncDest:
@@ -691,6 +704,7 @@ class DirectWeightSyncDest:
         self._int8_block_plans = Plans()  # block-scaled int8 names: one quantising plan per destination device
         self._int8_scaled_plans = Plans()  # per-channel / per-tensor scaled int8 names: likewise
         self._int8_dequant_plans = Plans()  # names read from scaled int8 handles into bf16/f16/f32: one plan per device
+        self._transpose_plans = Plans()  # transposed packed parts: one transposing plan per destination device
         # ({(name, scale keyword)}, requantize, scale_fmt, verbatim, {int8 names}, packed spec)
         self._plan_key: tuple | None = None
         self._packed_last: tuple | None = None  # (packed dict, its items, its key) of the last pull (_packed_spec)
@@ -772,6 +786,8 @@ class DirectWeightSyncDest:
                 src = StridedMem(src.ptr, dst_full.shape, _contig(dst_full.shape), src.dtype, src.device)
             return src, dst_full
         src, dst = src_window.sub(op.src_slices), dst_full.sub(op.dest_slices)
+        if getattr(op, "transpose", False):  # the source box in the destination's order: its last two dims swapped
+            src = StridedMem(src.ptr, _swap_last(src.shape), _swap_last(src.stride), src.dtype, src.device)
         if op.dest_dropped:  # a packed part whose int index dropped destination dims: unit dims on the source side
             src = StridedMem(src.ptr, dst.shape, _lift(src.stride, op.dest_dropped, 0), src.dtype, src.device)
         if getattr(op, "rotary", None) is not None:
@@ -808,6 +824,18 @@ class DirectWeightSyncDest:
                                      f"the source's {len(gshape)}-dim global shape {gshape}")
                 if not all(isinstance(o, int) and not isinstance(o, bool) for o in offs):
                     raise ValueError(f"{what}: source_offsets {offs} must be ints")
+                if not isinstance(part.transpose, bool):
+                    raise ValueError(f"{what}: transpose must be a bool, not {part.transpose!r}")
+                if part.transpose:
+                    if len(gshape) < 2:
+                        raise ValueError(f"{what}: transpose swaps the source's last two dims, and the source has "
+                                         f"{len(gshape)} dim")
+                    if part.rotary_head_dim is not None:
+                        raise ValueError(f"{what}: transpose and rotary_head_dim do not combine")
+                    if any(d >= len(box) - 2 for d in dropped):
+                        raise ValueError(f"{what}: its int index drops one of the destination's last two dims, which "
+                                         "transpose swaps (they must be slices)")
+                    ext = _swap_last(ext)  # the source box's extents, in the source's order
                 if any(o < 0 or o + e > g for o, e, g in zip(offs, ext, gshape)):
                     raise ValueError(f"{what}: the source box at {offs} with extent {tuple(ext)} leaves the source's "
                                      f"global shape {gshape}")
@@ -1038,6 +1066,24 @@ class DirectWeightSyncDest:
                                      "its scaled handles into whole destination rows); quantising and element-wise pulls "
                                      "take such parts")
 
+    @staticmethod
+    def _check_transposed_routes(parts: dict, scaled: dict) -> None:
+        """Refuse a transposed packed part on any route but the element-wise ones: its destination in a scale dict
+        (quantised, requantised or verbatim), or scaled handles feeding it (dequantised, or fp8 bytes moved with
+        their scales elsewhere).  ValueError naming the destination and the part, before anything is compiled."""
+        for name, entries in parts.items():
+            for k, part, _, _, handles in entries:
+                if not part.transpose:
+                    continue
+                what = f"packed destination '{name}' part {k} (source '{part.source}')"
+                if name in scaled:
+                    raise ValueError(f"{what}: a transposed part takes element-wise routes only (copies and fused casts), "
+                                     f"and '{name}' is in {scaled[name][0]}: quantising transposed sources is not "
+                                     "supported")
+                if any(getattr(h.rdma_buffer, "granularity", None) is not None for h in handles):
+                    raise ValueError(f"{what}: a transposed part takes element-wise routes only (copies and fused casts), "
+                                     "and its source handles are scaled: dequantising transposed sources is not supported")
+
     def _compile(self, scaled: dict | None = None, dequant: set | None = None, requant: set | None = None,
                  flags: int = 0, verbatim: dict | None = None) -> None:
         """Compile the cached transfer plan along the routes :meth:`_check_scales` chose: ``scaled`` is its
@@ -1064,6 +1110,7 @@ class DirectWeightSyncDest:
         # (int8 sources, device) -> (windows, {source buffer id: (name, DqSource)}): a plan reads one source format
         dq: dict[tuple, tuple[list, dict]] = {}
         quant: dict[tuple, tuple] = defaultdict(lambda: ([], {}, [], []))  # (kind, device) -> the same, names, targets
+        transposed: dict[int, tuple] = defaultdict(lambda: ([], []))  # device -> (windows, the name of each)
         for op in self._plan:
             dest = op.dest_local
             if not dest.is_cuda:
@@ -1077,6 +1124,11 @@ class DirectWeightSyncDest:
                 )
             dev = dest.device.index
             window = self.op_windows(op, op.rdma_buffer.window(dev))
+            if getattr(op, "transpose", False):
+                pairs, names = transposed[dev]
+                pairs.append(window)
+                names.append(op.name)
+                continue
             rotary = getattr(op, "rotary", None)  # plan ops built by hand (tests) may lack it
             grid = op.name in kind or (dequant and op.name in dequant)
             windows = _head_halves(window, rotary) if grid and rotary is not None else [window]
@@ -1093,6 +1145,9 @@ class DirectWeightSyncDest:
                 per_device[dev].append(window)
         self._native_plans = Plans.build(per_device)
         try:
+            for dev, (pairs, names) in sorted(transposed.items()):
+                _build_named(self._transpose_plans, Plans.build_transpose, {dev: pairs}, {"rect": names},
+                             lambda n: f"transposed pull of '{n}'", (_native.TSB_ERR_INVALID, _native.TSB_ERR_UNSUPPORTED))
             for (int8_src, dev), (pairs, sources) in sorted(dq.items()):
                 names = [n for n, _ in sources.values()]
                 _build_named(self._int8_dequant_plans if int8_src else self._dequant_plans, Plans.build_dequant_fp8,
@@ -1129,8 +1184,9 @@ class DirectWeightSyncDest:
 
     @property
     def _fp8_plans(self) -> tuple:
-        """The scaled fp8 and int8 plans in launch order (after the copy plan on each device's copy stream)."""
-        return (self._block_plans, self._scaled_plans, self._dequant_plans, self._requant_plans, self._int8_block_plans,
+        """The plans launched after the copy plan on each device's copy stream, in launch order: the transposing plans,
+        then the scaled fp8 and int8 plans."""
+        return (self._transpose_plans, self._block_plans, self._scaled_plans, self._dequant_plans, self._requant_plans, self._int8_block_plans,
                 self._int8_scaled_plans, self._int8_dequant_plans)
 
     def plan_info(self) -> dict[int, dict]:
@@ -1158,7 +1214,10 @@ class DirectWeightSyncDest:
         a source without handles, a name with handles of its own, a bad index, a source box outside the source,
         overlapping parts, a part the handles do not cover, and a part whose int index drops the destination's last
         dim on a dequantising or requantising route (DESIGN.md section 4, "Packed destinations").
-        Elements outside every part are left alone.  Changing the spec rebuilds the plan.
+        Elements outside every part are left alone.  Changing the spec rebuilds the plan.  A transposed part
+        (``PackedPart(transpose=True)``) is moved by its own transposing plan after the copy plan; it takes the byte
+        copy and fused casts only, and a ValueError naming the destination and the part refuses it for a name in the
+        scale dicts or fed by scaled handles (DESIGN.md section 4, "Transposed packed parts").
 
         Scaled fp8 destinations (extension): float8_e4m3fn weights quantised during the pull from
         bf16/f16/f32 handles, each name in at most one of
@@ -1273,6 +1332,7 @@ class DirectWeightSyncDest:
             dequant = self._check_dequant(route_handles, dest_state_dict, scaled)
             requant = {n for n, (*_, route) in scaled.items() if route == "requantise"}
             self._check_packed_rows(parts, dequant, requant)
+            self._check_transposed_routes(parts, scaled)
             self._plan = self._build_plan(all_handles, dest_state_dict, dest_slices, packed=packed)
             try:
                 verbatim_rects = self._verbatim_rects(self._plan, scaled)
@@ -1337,13 +1397,15 @@ class DirectWeightSyncDest:
         self._plan_key = self._plan_ids = self._plan_refs = self._plan_dict = self._plan_scale_dicts = None
 
 
-def _build_named(plans: Plans, build, per_device: dict, names: dict[str, list[str]], pull_of) -> None:
-    """Add ``build(per_device)`` (a ``Plans.build_*`` call) to ``plans``.  A TSB_ERR_INVALID naming "target N" (or else
-    "source N") becomes a ValueError naming the weight ``names[noun][N]``, whose pull ``pull_of(name)`` describes."""
+def _build_named(plans: Plans, build, per_device: dict, names: dict[str, list[str]], pull_of,
+                 codes: tuple = (_native.TSB_ERR_INVALID,)) -> None:
+    """Add ``build(per_device)`` (a ``Plans.build_*`` call) to ``plans``.  A TsbError of one of ``codes`` naming
+    "target N" (or else "source N", or "rect N") becomes a ValueError naming the weight ``names[noun][N]``, whose pull
+    ``pull_of(name)`` describes."""
     try:
         plans.update(build(per_device))
     except _native.TsbError as e:
-        if e.code == _native.TSB_ERR_INVALID:
+        if e.code in codes:
             for noun, by_index in names.items():
                 m = re.search(noun + r" (\d+)", str(e))
                 if m:
@@ -1421,7 +1483,8 @@ def _packed_key(packed: dict | None) -> frozenset | None:
             if not isinstance(p.dest_index, tuple) or not isinstance(p.source_offsets, tuple):
                 raise TypeError(f"packed['{name}']: dest_index and source_offsets of a PackedPart must be tuples")
         out.append((name, tuple((p.source, tuple((e.start, e.stop, e.step) if isinstance(e, slice) else e
-                                                 for e in p.dest_index), p.source_offsets, p.rotary_head_dim)
+                                                 for e in p.dest_index), p.source_offsets, p.rotary_head_dim,
+                                    p.transpose)
                                 for p in parts)))
     return frozenset(out)
 
@@ -1471,11 +1534,13 @@ def _packed_ops(name: str, dest: torch.Tensor, dest_offsets: tuple, entries: lis
     for _, part, box, dropped, handles in entries:
         kept = [d for d in range(nd) if d not in dropped]
         so = part.source_offsets
+        flip = _swap_last if part.transpose else tuple  # destination order <-> source order of the kept dims
+        ext = flip([box[d][1] - box[d][0] for d in kept])
         seen: set[tuple] = set()
         for h in handles:
             ho, hs = h.tensor_slice.offsets, h.tensor_slice.local_shape
             lo = tuple(max(a, b) for a, b in zip(ho, so))
-            hi = tuple(min(a + x, b + t - s) for a, x, b, (s, t) in zip(ho, hs, so, (box[d] for d in kept)))
+            hi = tuple(min(a + x, b + e) for a, x, b, e in zip(ho, hs, so, ext))
             if any(t <= s for s, t in zip(lo, hi)) or (lo, hi) in seen:
                 continue
             seen.add((lo, hi))
@@ -1490,13 +1555,15 @@ def _packed_ops(name: str, dest: torch.Tensor, dest_offsets: tuple, entries: lis
                     n_src = heads * part.rotary_head_dim if halves == 2 else 2 * rows - 1
                     slo[-2], shi[-2], dlo[-2], dhi[-2] = srow, srow + n_src, drow, drow + n_dst
                     rotary = (kept[-2], part.rotary_head_dim) + rotary
+                dlo, dhi = flip(dlo), flip(dhi)
                 dst_idx = [slice(s, t) for s, t in box]
                 for i, d in enumerate(kept):
                     dst_idx[d] = slice(box[d][0] + dlo[i], box[d][0] + dhi[i])
                 ops.append(_TransferOp(rdma_buffer=h.rdma_buffer, dest_byte_view=None, dest_tensor=dest,
                                        src_slices=tuple(slice(s - o, t - o) for s, t, o in zip(slo, shi, ho)),
                                        dest_slices=tuple(dst_idx), name=name, dest_local=dest, dest_offsets=dest_offsets,
-                                       src_offsets=tuple(ho), src_start=tuple(slo), dest_dropped=dropped, rotary=rotary))
+                                       src_offsets=tuple(ho), src_start=tuple(slo), dest_dropped=dropped, rotary=rotary,
+                                       transpose=part.transpose))
     return ops
 
 
@@ -1523,6 +1590,12 @@ def _half_pieces(r0: int, hd: int, h: int, a: int, b: int) -> list[tuple]:
         if j0 < j1:
             out.append((base + 2 * j0, h * hd + t * h2 + j0, (1, 1, j1 - j0)))
     return out
+
+
+def _swap_last(values) -> tuple:
+    """``values`` with its last two entries swapped (a transposed part's box between destination and source order)."""
+    v = tuple(values)
+    return v[:-2] + (v[-1], v[-2])
 
 
 def _split_rows(win: StridedMem, k: int, shape: tuple, steps: tuple) -> StridedMem:

@@ -11,7 +11,7 @@ import logging
 import threading
 
 from torchstore_b200 import _native
-from torchstore_b200.planner import build_rects
+from torchstore_b200.planner import build_rects, build_transpose_rects
 
 logger = logging.getLogger(__name__)
 
@@ -138,6 +138,13 @@ class Plans(dict):
         """Compile requantising pulls of scaled fp8 sources into scaled fp8 destinations: ``{device:
         ([(src, dst) StridedMem windows], [DqSource], [SqTarget])}``."""
         return cls._build_pulls(_native.requant_fp8_plan_create, per_device, flags)
+
+    @classmethod
+    def build_transpose(cls, per_device: dict[int, list]) -> "Plans":
+        """Compile transposing pulls: ``{device: [(src, dst) StridedMem windows]}``, each window's destination
+        contiguous along its dim -1 and its source along dim -2 (:func:`build_transpose_rects`)."""
+        return cls.build_fp8(lambda dev, rects, n, flags: _native.transpose_plan_create(dev, rects, n, flags),
+                             {dev: build_transpose_rects(pairs) for dev, pairs in per_device.items()})
 
     @classmethod
     def build_source_quant(cls, per_device: dict[int, list], flags: int = 0,

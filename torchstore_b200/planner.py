@@ -154,6 +154,38 @@ def build_rects(pairs: Sequence[tuple[StridedMem, StridedMem]], quantise: bool =
     return arr, n
 
 
+def build_transpose_rects(pairs: Sequence[tuple[StridedMem, StridedMem]]):
+    """(src, dst) windows of transposed packed parts -> (ctypes array of tsb_rect_t, count), for
+    tsb_transpose_plan_create.  Unlike :func:`build_rects` the last two dims stay as they are, unit extents included:
+    they are the transposed pair (destination contiguous along dim -1, source along dim -2).  The outer dims lose
+    their unit extents.  Empty windows are skipped."""
+    arr = _native.make_rect_array(max(1, len(pairs)))
+    n = 0
+    for src, dst in pairs:
+        if tuple(src.shape) != tuple(dst.shape):
+            raise ValueError(f"source window {src.shape} and destination window {dst.shape} differ")
+        if src.dtype != dst.dtype and not _native.cast_supported(src.dtype, dst.dtype):
+            raise NotImplementedError(f"no fused cast kernel for {src.dtype} -> {dst.dtype}")
+        if len(src.shape) < 2 or any(e == 0 for e in src.shape):
+            continue
+        sb, db = src.itemsize, dst.itemsize
+        outer = [(e, ss * sb, ds * db) for e, ss, ds in zip(src.shape[:-2], src.stride[:-2], dst.stride[:-2]) if e != 1]
+        dims = outer + [(e, ss * sb, ds * db) for e, ss, ds in zip(src.shape[-2:], src.stride[-2:], dst.stride[-2:])]
+        if len(dims) > MAX_DIMS:
+            raise NotImplementedError(f"rectangle has {len(dims)} dims (> {MAX_DIMS})")
+        rect = arr[n]
+        rect.src, rect.dst, rect.ndim = src.ptr, dst.ptr, len(dims)
+        for i in range(MAX_DIMS):
+            rect.extent[i], rect.src_stride[i], rect.dst_stride[i] = dims[i] if i < len(dims) else (1, 0, 0)
+        if src.dtype == dst.dtype:
+            rect.src_dtype = rect.dst_dtype = _native.dtype_code(src.dtype)
+        else:
+            rect.src_dtype, rect.dst_dtype = _native.cast_code(src.dtype), _native.cast_code(dst.dtype)
+        rect.src_device = src.device
+        n += 1
+    return arr, n
+
+
 # ------------------------------------------------------------------------------------------------
 # picklable handle
 # ------------------------------------------------------------------------------------------------

@@ -111,11 +111,14 @@ def hf_llama_layout(cfg=LLAMA3_8B, n_layers: int | None = None, scale: int = 1, 
 
 
 def qwen3_moe_layout(cfg=QWEN3_MOE, n_layers: int | None = None, scale: int = 1, with_embeddings: bool = True,
-                     n_experts: int | None = None):
+                     n_experts: int | None = None, grouped_experts: bool = False):
     """A Qwen3-MoE model under its Hugging Face names: name -> (global shape, placement), as :func:`llama_layout`
     (the placements are those of an FSDP-style trainer's view and do not matter for packed pulls).  Per layer: q/k/v/o
     projections with q_norm / k_norm, the router ``mlp.gate``, and one gate/up/down projection per expert.
-    ``scale`` divides hidden size, head_dim, expert width and vocabulary; ``n_experts`` overrides the expert count."""
+    ``scale`` divides hidden size, head_dim, expert width and vocabulary; ``n_experts`` overrides the expert count.
+    ``grouped_experts`` replaces each layer's per-expert tensors by the input-major stacks of a grouped-GEMM trainer
+    (the layout ``torch._grouped_mm(x, w)`` takes without a transpose), placement Shard(0):
+    ``mlp.experts.w1`` / ``mlp.experts.w3`` ``[E, dim, moe_ffn]`` and ``mlp.experts.w2`` ``[E, moe_ffn, dim]``."""
     d, hd = cfg["dim"] // scale, cfg["head_dim"] // scale
     q, kv, ffn = cfg["n_heads"] * hd, cfg["n_kv_heads"] * hd, cfg["moe_ffn"] // scale
     experts = cfg["n_experts"] if n_experts is None else n_experts
@@ -132,7 +135,11 @@ def qwen3_moe_layout(cfg=QWEN3_MOE, n_layers: int | None = None, scale: int = 1,
         out[p + "self_attn.q_norm.weight"] = ((hd,), ("R",))
         out[p + "self_attn.k_norm.weight"] = ((hd,), ("R",))
         out[p + "mlp.gate.weight"] = ((experts, d), ("R",))
-        for e in range(experts):
+        if grouped_experts:
+            out[p + "mlp.experts.w1"] = ((experts, d, ffn), ("S", 0))
+            out[p + "mlp.experts.w3"] = ((experts, d, ffn), ("S", 0))
+            out[p + "mlp.experts.w2"] = ((experts, ffn, d), ("S", 0))
+        for e in range(0 if grouped_experts else experts):
             out[p + f"mlp.experts.{e}.gate_proj.weight"] = ((ffn, d), ("S", 0))
             out[p + f"mlp.experts.{e}.up_proj.weight"] = ((ffn, d), ("S", 0))
             out[p + f"mlp.experts.{e}.down_proj.weight"] = ((d, ffn), ("S", 1))
@@ -158,7 +165,9 @@ def vllm_tp_layout(hf_layout, cfg, tp: int, rank: int, ep: bool = False, source:
       ``qkv_proj`` = ``[q_r; k_r; v_r]`` (rank r's query heads, then its kv head(s): when tp exceeds the kv heads,
       kv head ``r // (tp / n_kv)``, as vLLM replicates them), ``gate_up_proj`` = ``[gate_r; up_r]``, and for MoE
       ``mlp.experts.w13_weight [E, 2I/tp, H]`` / ``w2_weight [E, H, I/tp]`` with every expert stacked on dim 0.
-      With ``ep`` the experts are split over the ranks instead (``E/tp`` whole experts each).
+      With ``ep`` the experts are split over the ranks instead (``E/tp`` whole experts each).  From a
+      ``qwen3_moe_layout(grouped_experts=True)`` both are filled by transposed parts (``PackedPart(transpose=True)``)
+      of the input-major stacks: ``w13_weight`` from ``w1`` and ``w3``, ``w2_weight`` from ``w2``, one part each.
     * Every other parameter keeps its HF name: ``parts`` None and ``box`` = (global offsets, global shape) of the
       rank's shard of that tensor: ``o_proj`` / ``down_proj`` column shards, vocab-parallel ``embed_tokens`` /
       ``lm_head`` row shards, replicated norms and router."""
@@ -201,6 +210,9 @@ def vllm_tp_layout(hf_layout, cfg, tp: int, rank: int, ep: bool = False, source:
             out[name] = (tuple(shape), None, ((0,) * len(shape), tuple(shape)))  # the router, replicated
             base = mod.removesuffix("gate")
             n_exp = shape[0]
+            if base + "experts.w1" in hf_layout:
+                out.update(_grouped_experts(base, hf_layout[base + "experts.w1"][0], tp, rank, ep))
+                continue
             ffn, h = hf_layout[base + "experts.0.gate_proj.weight"][0]
             if ep:
                 if n_exp % tp:
@@ -226,6 +238,25 @@ def vllm_tp_layout(hf_layout, cfg, tp: int, rank: int, ep: bool = False, source:
             off, loc = shard_box(shape, tp, rank, placement) if tp > 1 else ((0,) * len(shape), tuple(shape))
             out[name] = (tuple(loc), None, (tuple(off), tuple(shape)))
     return out
+
+
+def _grouped_experts(base: str, w1_shape, tp: int, rank: int, ep: bool):
+    """:func:`vllm_tp_layout`'s ``w13_weight`` / ``w2_weight`` of rank ``rank`` from grouped-GEMM stacks ``w1`` / ``w3``
+    ``[E, H, I]`` and ``w2`` ``[E, I, H]`` (``w1_shape``): transposed parts, TP slicing the ffn dim or EP the experts."""
+    from torchstore_b200.direct_weight_sync import PackedPart
+
+    n_exp, h, ffn = w1_shape
+    if ep:
+        if n_exp % tp:
+            raise ValueError(f"ep over tp={tp} ranks needs the {n_exp} experts to split evenly")
+        e_r, e0, f_r, f0 = n_exp // tp, rank * (n_exp // tp), ffn, 0
+    else:
+        e_r, e0, f_r, f0 = n_exp, 0, ffn // tp, rank * (ffn // tp)
+    ex = base + "experts."
+    w13 = (PackedPart(ex + "w1", (slice(0, e_r), slice(0, f_r), slice(0, h)), (e0, 0, f0), transpose=True),
+           PackedPart(ex + "w3", (slice(0, e_r), slice(f_r, 2 * f_r), slice(0, h)), (e0, 0, f0), transpose=True))
+    w2 = (PackedPart(ex + "w2", (slice(0, e_r), slice(0, h), slice(0, f_r)), (e0, f0, 0), transpose=True),)
+    return {ex + "w13_weight": ((e_r, 2 * f_r, h), w13, None), ex + "w2_weight": ((e_r, h, f_r), w2, None)}
 
 
 def _from_torchtitan(titan_layout, cfg, tp: int, rank: int, ep: bool):
