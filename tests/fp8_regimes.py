@@ -27,7 +27,7 @@ from typing import Callable
 
 import numpy as np
 
-from tests.test_requant_fp8_cpu import shard_box
+from tests.helpers import shard_box
 from torchstore_b200 import _native
 
 STAGE_BYTES, TILE_ELEMS, BAND_ROWS, DQ_TILE_ROWS = 32768, 16384, 256, 256

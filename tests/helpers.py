@@ -1,15 +1,22 @@
 """Shared helpers for the test-suite: seeded random rectangle workloads that can be materialised on
-the CPU (for the C oracle) and on CUDA (for the product), plus Llama-3 layouts."""
+the CPU (for the C oracle) and on CUDA (for the product), Llama-3 layouts, and the host-memory stand-ins,
+shards, handles and plans of the pull suites that run without a GPU."""
 
 from __future__ import annotations
 
+import hashlib
 import random
+import types
 
 import numpy as np
+import pytest
 import torch
 
+import workloads
 from torchstore_b200 import _native
+from torchstore_b200.direct_weight_sync import DirectWeightSyncDest, RDMAWeightHandle
 from torchstore_b200.planner import StridedMem, build_rects
+from torchstore_b200.transport.types import TensorSlice
 
 SAME_DTYPES = [torch.uint8, torch.int16, torch.bfloat16, torch.float16, torch.int32, torch.float32, torch.int64, torch.float64]
 CAST_PAIRS = [
@@ -347,3 +354,170 @@ def llama_layout(cfg=LLAMA3_8B, n_layers: int | None = None, scale: int = 1):
     out["norm.weight"] = ((d,), ("R",))
     out["output.weight"] = ((vocab, d), ("S", 0))
     return out
+
+
+# ---- host-side pulls: shards, handles and plans on host memory -----------------------------------------
+def shard_box(shape, n, r, dim):
+    """(offsets, local shape) of rank r of n torch.chunk-style Shard(dim) shards of `shape` (empty past the end)."""
+    return workloads.shard_box(shape, n, r, ("S", dim))
+
+
+def region(t, off, loc):
+    """The box of `t` at offsets `off` with extent `loc`."""
+    return t[tuple(slice(o, o + s) for o, s in zip(off, loc))]
+
+
+def rand_full(shape, dtype, seed):
+    """Seeded normal values scaled by powers of two from 2^-6 to 2^5, in `dtype`."""
+    g = torch.Generator().manual_seed(seed)
+    return (torch.randn(shape, generator=g) * 2.0 ** torch.randint(-6, 6, shape, generator=g).float()).to(dtype)
+
+
+def sha256_of(t: torch.Tensor) -> str:
+    return hashlib.sha256(t.detach().cpu().contiguous().view(torch.uint8).numpy().tobytes()).hexdigest()
+
+
+class HostBuffer:
+    """Host-memory stand-in for NvlinkBuffer: the planner reads ``shape`` and ``dtype`` only; ``shard`` is what
+    the tests move (None for metadata-only plans)."""
+
+    def __init__(self, shard, shape, dtype):
+        self.shard, self.shape, self.dtype = shard, tuple(shape), dtype
+
+
+def shard_handles(full, src_boxes, make_buffer):
+    """Handles over the `src_boxes` shards of `full`, rank r holding box r (an empty box gets no handle);
+    ``make_buffer(shard, offsets, local shape)`` wraps each contiguous shard -> (handles, keepalive)."""
+    gshape = tuple(full.shape)
+    handles, keep = [], []
+    for r, (off, loc) in enumerate(src_boxes):
+        if 0 in loc:
+            continue
+        shard = region(full, off, loc).contiguous()
+        keep.append(shard)
+        handles.append(RDMAWeightHandle(rdma_buffer=make_buffer(shard, off, loc),
+                                        tensor_slice=TensorSlice(off, (r,), gshape, loc, (len(src_boxes),)), source_rank=r))
+    return handles, keep
+
+
+def plan_windows(handles, dest, dst_box):
+    """The product's plan of a pull of one tensor's `handles` into `dest`, the tensor's box `dst_box`
+    -> (ops, their (source, destination) windows over each buffer's ``shard``)."""
+    off, loc = dst_box
+    gshape = tuple(handles[0].tensor_slice.global_shape)
+    ops = DirectWeightSyncDest()._build_plan({"w": handles}, {"w": dest}, {"w": TensorSlice(off, (0,), gshape, loc, (1,))})
+    return ops, [DirectWeightSyncDest.op_windows(op, StridedMem.from_tensor(op.rdma_buffer.shard)) for op in ops]
+
+
+def fsdp_handles(layout, n: int, make_buffer, names=None) -> dict[str, list]:
+    """Every tensor of ``layout`` cut into ``n`` Shard(0) shards: name -> handles in rank order.
+    ``make_buffer(name, offsets, local shape)`` creates each handle's buffer."""
+    out = {}
+    for name, (shape, _) in layout.items():
+        if names is not None and name not in names:
+            continue
+        hs = []
+        for r in range(n):
+            off, loc = workloads.shard_box(shape, n, r, ("S", 0)) if n > 1 else ((0,) * len(shape), tuple(shape))
+            hs.append(RDMAWeightHandle(make_buffer(name, off, loc), TensorSlice(off, (r,), tuple(shape), loc, (n,)), r))
+        out[name] = hs
+    return out
+
+
+def handles_of(shape, n=1, dtype=torch.bfloat16, dim=0, sources=None):
+    """FSDP(n) handles of one ``shape`` tensor cut along ``dim`` (torch.chunk-style, uneven when n does not divide
+    it), over the shards of ``sources``, or metadata-only buffers without."""
+    out = []
+    for r in range(n):
+        off, loc = workloads.shard_box(shape, n, r, ("S", dim)) if n > 1 else ((0,) * len(shape), tuple(shape))
+        shard = None if sources is None else region(sources, off, loc).contiguous()
+        out.append(RDMAWeightHandle(HostBuffer(shard, loc, dtype), TensorSlice(off, (r,), tuple(shape), loc, (n,)), r))
+    return out
+
+
+def pull_args(vlayout, tp: int, rank: int, make_dest):
+    """-> (destination dict, dest_slices, packed) of a vLLM layout; ``make_dest(name, local shape)``."""
+    dests, slices, packed = {}, {}, {}
+    for name, (shape, parts, box) in vlayout.items():
+        dests[name] = make_dest(name, shape)
+        if parts is None:
+            slices[name] = TensorSlice(box[0], (rank,), box[1], tuple(shape), (tp,))
+        else:
+            packed[name] = parts
+    return dests, slices, packed
+
+
+def unfused_args(vlayout, hf_layout, tp: int, rank: int, make_dest):
+    """The same bytes pulled without packing: one HF-named destination per part (its box, at the part's source
+    offsets) plus the unpacked names -> (destination dict, dest_slices, {fused name: [(part, unfused name)]})."""
+    dests, slices, where = {}, {}, {}
+    for name, (shape, parts, box) in vlayout.items():
+        if parts is None:
+            dests[name] = make_dest(name, shape)
+            slices[name] = TensorSlice(box[0], (rank,), box[1], tuple(shape), (tp,))
+            continue
+        for k, p in enumerate(parts):
+            ext = tuple(torch.empty(shape, device="meta")[p.dest_index].shape)
+            uname = p.source if p.source not in dests else f"{p.source}#{k}"
+            assert uname == p.source, "one unfused destination per source"
+            dests[uname] = make_dest(uname, ext)
+            slices[uname] = TensorSlice(tuple(p.source_offsets), (rank,), tuple(hf_layout[p.source][0]), ext, (tp,))
+            where.setdefault(name, []).append((p, uname))
+    return dests, slices, where
+
+
+# ---- validation before anything is exported or compiled ------------------------------------------------
+def expect_invalid(fn, needle=None):
+    """``fn()`` raises TsbError with TSB_ERR_INVALID (and a message matching ``needle``) -> the message."""
+    with pytest.raises(_native.TsbError, match=needle) as e:
+        fn()
+    assert e.value.code == _native.TSB_ERR_INVALID, e.value
+    return str(e.value)
+
+
+def cuda_like(t):
+    """A CPU tensor's metadata that claims to be on CUDA (validation reads nothing else)."""
+    return types.SimpleNamespace(dtype=t.dtype, shape=t.shape, dim=t.dim, numel=t.numel, is_contiguous=t.is_contiguous,
+                                 stride=t.stride, is_cuda=True, device=t.device)
+
+
+def fake_dest(dtype, shape=(256, 256)):
+    """A contiguous 'CUDA' destination stand-in for _check_scales (it reads dtype, shape, contiguity and device)."""
+    return types.SimpleNamespace(dtype=dtype, shape=torch.Size(shape), dim=lambda: len(shape), numel=lambda: 256 * 256,
+                                 is_contiguous=lambda: True, is_cuda=True, device=torch.device("cpu"), data_ptr=lambda: 0)
+
+
+def scaled_handle(dtype, granularity=None):
+    """A handle whose buffer has ``dtype`` and, when given, a scale ``granularity``: all the route checks read."""
+    buf = types.SimpleNamespace(dtype=dtype)
+    if granularity:
+        buf.granularity = granularity
+    return types.SimpleNamespace(rdma_buffer=buf)
+
+
+class Boom(Exception):
+    pass
+
+
+def _boom(*a, **k):
+    raise Boom("exported, allocated or compiled before validation finished")
+
+
+def no_compile(monkeypatch):
+    """Any plan compile during the test raises Boom.  A module binds it as a fixture with
+    ``no_compile = pytest.fixture(no_compile)``."""
+    import torchstore_b200.direct_weight_sync as dws
+
+    for name in ("build", "build_source_quant", "build_dequant_fp8", "build_requant_fp8", "build_block_fp8",
+                 "build_scaled_fp8"):
+        monkeypatch.setattr(dws.Plans, name, classmethod(_boom))
+
+
+def no_export(monkeypatch):
+    """Any export, allocation (torch.empty) or plan compile during the test raises Boom.  A module binds it as a
+    fixture with ``no_export = pytest.fixture(no_export)``."""
+    import torchstore_b200.direct_weight_sync as dws
+
+    monkeypatch.setattr(dws.HbmDescriptor, "from_tensor", staticmethod(_boom))
+    monkeypatch.setattr(torch, "empty", _boom)
+    no_compile(monkeypatch)

@@ -20,7 +20,6 @@ from __future__ import annotations
 
 import itertools
 import random
-import types
 from dataclasses import dataclass, field
 
 import numpy as np
@@ -36,8 +35,8 @@ from torchstore_b200.direct_weight_sync import (DirectWeightSyncDest, PackedPart
 from torchstore_b200.planner import StridedMem, build_rects
 from torchstore_b200.transport.types import TensorSlice
 
-from tests import packed_harness
-from tests.helpers import rect_fields
+from tests import helpers
+from tests.helpers import cuda_like, rect_fields, region
 
 BLOCK = 128
 E4M3, E5M2 = torch.float8_e4m3fn, torch.float8_e5m2
@@ -678,8 +677,8 @@ def assert_pull(spec: Spec, got: dict, want: dict, what: str) -> None:
 
 
 # ---- host tier -------------------------------------------------------------------------------------------------------
-class HostBuffer(packed_harness.HostBuffer):
-    """packed_harness.HostBuffer that also stands in for ScaledNvlinkBuffer and maps its memory, as the compile reads
+class HostBuffer(helpers.HostBuffer):
+    """helpers.HostBuffer that also stands in for ScaledNvlinkBuffer and maps its memory, as the compile reads
     it (``window``, ``scale_window``)."""
 
     def __init__(self, shard: torch.Tensor, scale=None, granularity=None, row0: int = 0, col0: int = 0):
@@ -693,17 +692,13 @@ class HostBuffer(packed_harness.HostBuffer):
         return StridedMem.from_tensor(self.scale)
 
 
-def _region(t, off, loc):
-    return t[tuple(slice(o, o + e) for o, e in zip(off, loc))]
-
-
 def handles_of(spec: Spec, data: Data, make) -> dict:
     """{source: [RDMAWeightHandle]} with ``make(shard, scale or None, granularity, row0, col0)`` buffers."""
     out = {}
     for name, src in spec.sources.items():
         hs = []
         for k, (off, loc) in enumerate(src.boxes):
-            shard_ = _region(data.full[name], off, loc).contiguous().clone()
+            shard_ = region(data.full[name], off, loc).contiguous().clone()
             scale = data.scales[name][k].clone() if src.g is not None else None
             buf = make(shard_, scale, src.g, off[-2], off[-1])
             hs.append(RDMAWeightHandle(buf, TensorSlice(tuple(off), (k,), tuple(src.shape), tuple(loc), (len(src.boxes),)), k))
@@ -715,7 +710,7 @@ def refill(spec: Spec, handles: dict, data: Data, shard_of, scale_of) -> None:
     """Write ``data`` into the existing handles' memory (``shard_of(buffer)``, ``scale_of(buffer)`` tensors)."""
     for name, src in spec.sources.items():
         for k, (h, (off, loc)) in enumerate(zip(handles[name], src.boxes)):
-            shard_of(h.rdma_buffer).copy_(_region(data.full[name], off, loc))
+            shard_of(h.rdma_buffer).copy_(region(data.full[name], off, loc))
             if src.g is not None:
                 scale_of(h.rdma_buffer).copy_(data.scales[name][k])
 
@@ -733,12 +728,6 @@ def dests_of(spec: Spec, device="cpu") -> tuple[dict, dict, dict]:
             src = spec.sources[name]
             slices[name] = TensorSlice(tuple(d.window), (0,), tuple(src.shape), tuple(d.shape), (1,))
     return dests, scales, slices
-
-
-def cuda_like(t):
-    """A CPU tensor's metadata that claims to be on CUDA (the route checks read nothing else)."""
-    return types.SimpleNamespace(dtype=t.dtype, shape=t.shape, dim=t.dim, numel=t.numel, is_contiguous=t.is_contiguous,
-                                 stride=t.stride, is_cuda=True, device=t.device)
 
 
 @dataclass

@@ -14,6 +14,7 @@ import torch
 
 from oracle.dequant_fp8_oracle import (DST, GRANULARITIES, SCALE_SET, decode_e4m3, dequantize, digest, fixture_inputs,
                                        replay, scale_shape, torch_dequantize)
+from tests.helpers import cuda_like, expect_invalid, no_export, plan_windows, region, shard_box, shard_handles
 from torchstore_b200 import _native
 from torchstore_b200.direct_weight_sync import (DirectWeightSyncDest, DirectWeightSyncSource, RDMAWeightHandle,
                                                 source_scale_shapes)
@@ -88,18 +89,6 @@ def test_torch_rendering_matches_the_oracle():
 
 
 # ---- the plan compiler, replayed on host memory ----------------------------------------------------
-def shard_box(shape, n, r, dim):
-    off, loc = [0] * len(shape), list(shape)
-    chunk = -(-shape[dim] // n)
-    start, stop = min(shape[dim], chunk * r), min(shape[dim], chunk * (r + 1))
-    off[dim], loc[dim] = start, max(0, stop - start)
-    return tuple(off), tuple(loc)
-
-
-def region(t, off, loc):
-    return t[tuple(slice(o, o + s) for o, s in zip(off, loc))]
-
-
 def global_scale(g, shape, seed):
     """A global scale tensor of the full tensor (anchored at the origin)."""
     gen = torch.Generator().manual_seed(seed)
@@ -128,24 +117,13 @@ class FakeScaledBuffer:
 def compile_pull(q_full, full_scale, g, src_boxes, dst_box, dst_dtype):
     """Plan a pull of `q_full`'s shards (each with its own slice of the global scale) into a `dst_dtype`
     window `dst_box`; returns (dest, tiles, keepalive)."""
-    gshape = tuple(q_full.shape)
-    handles, keep = [], []
-    for r, (off, loc) in enumerate(src_boxes):
-        if 0 in loc:
-            continue
-        shard = region(q_full, off, loc).contiguous()
-        scale = local_scale(full_scale, g, off, loc)
-        keep += [shard, scale]
-        buf = FakeScaledBuffer(shard, scale, g, off[-2], off[-1])
-        handles.append(RDMAWeightHandle(rdma_buffer=buf, tensor_slice=TensorSlice(off, (r,), gshape, loc, (len(src_boxes),)),
-                                        source_rank=r))
-    off, loc = dst_box
-    dest = torch.zeros(loc, dtype=dst_dtype)
-    ops = DirectWeightSyncDest()._build_plan({"w": handles}, {"w": dest}, {"w": TensorSlice(off, (0,), gshape, loc, (1,))})
-    pairs, sources, index = [], [], {}
+    handles, keep = shard_handles(q_full, src_boxes, lambda shard, off, loc: FakeScaledBuffer(
+        shard, local_scale(full_scale, g, off, loc), g, off[-2], off[-1]))
+    dest = torch.zeros(dst_box[1], dtype=dst_dtype)
+    ops, pairs = plan_windows(handles, dest, dst_box)
+    sources, index = [], {}
     for op in ops:
         buf = op.rdma_buffer
-        pairs.append(DirectWeightSyncDest.op_windows(op, StridedMem.from_tensor(buf.shard)))
         if id(buf) not in index:
             index[id(buf)] = len(sources)
             n, k = buf.shard.shape[-2:]
@@ -265,13 +243,6 @@ def test_full_size_llama3_8b_compile(g):
 
 
 # ---- compiler errors ------------------------------------------------------------------------------
-def expect_invalid(fn):
-    with pytest.raises(_native.TsbError) as e:
-        fn()
-    assert e.value.code == _native.TSB_ERR_INVALID, e.value
-    return str(e.value)
-
-
 def test_compile_errors_name_the_rect_or_source():
     q = torch.zeros(64, 64, dtype=E4M3)
     s = torch.zeros(64, 1)
@@ -309,27 +280,7 @@ def test_compile_errors_name_the_rect_or_source():
 
 
 # ---- register / pull validation (before anything is exported or launched) ---------------------------
-class Boom(Exception):
-    pass
-
-
-@pytest.fixture
-def no_export(monkeypatch):
-    """Any export or plan compile during the test fails loudly."""
-    import torchstore_b200.direct_weight_sync as dws
-
-    def boom(*a, **k):
-        raise Boom("exported or compiled")
-
-    monkeypatch.setattr(dws.HbmDescriptor, "from_tensor", classmethod(lambda cls, t: boom()))
-    monkeypatch.setattr(dws.Plans, "build", classmethod(lambda cls, *a: boom()))
-    monkeypatch.setattr(dws.Plans, "build_dequant_fp8", classmethod(lambda cls, *a: boom()))
-
-
-def cuda_like(t):
-    """A CPU tensor's metadata that claims to be on CUDA (validation reads nothing else)."""
-    return types.SimpleNamespace(dtype=t.dtype, shape=t.shape, dim=t.dim, numel=t.numel, is_contiguous=t.is_contiguous,
-                                 stride=t.stride, is_cuda=True, device=t.device)
+no_export = pytest.fixture(no_export)
 
 
 def test_register_errors_raise_before_export(no_export):

@@ -12,6 +12,7 @@ from oracle import dequant_fp8_oracle, requant_fp8_oracle
 from tests import test_dequant_fp8_cpu as dq_cpu
 from tests import test_requant_fp8_cpu as rq_cpu
 from tests.fp8_regimes import ES, REGIMES, WORKLOADS, geometry
+from tests.helpers import region
 
 # Every regime the catalogue names.  A regime added there without a workload that reaches it, or dropped
 # from it, fails test_catalogue_is_complete until this list says so too.
@@ -51,7 +52,7 @@ def replayed(name):
         dest, dest_scale, tables, (_, _, arr, _, _) = rq_cpu.compile_pull(q, s, w.sg, list(w.src), w.dst, w.out)
         geom = geometry(dest.data_ptr(), loc, 1, arr, len(arr))
         requant_fp8_oracle.replay(*tables)
-        want_q, want_s = requant_fp8_oracle.requantize(rq_cpu.region(q, off, loc).view(torch.uint8).numpy(),
+        want_q, want_s = requant_fp8_oracle.requantize(region(q, off, loc).view(torch.uint8).numpy(),
                                                        rq_cpu.local_scale(s, w.sg, off, loc).numpy(), w.sg, off[-2], off[-1], w.out)
         assert np.array_equal(dest.view(torch.uint8).numpy(), want_q), w.describe()
         assert rq_cpu.same_scale(dest_scale.numpy(), want_s), w.describe()
@@ -59,7 +60,7 @@ def replayed(name):
         dest, tables, (_, _, arr, _) = dq_cpu.compile_pull(q, s, w.sg, list(w.src), w.dst, dequant_fp8_oracle.DST[w.out])
         geom = geometry(dest.data_ptr(), loc, ES[w.out], arr, len(arr))
         dequant_fp8_oracle.replay(tables)
-        want = dequant_fp8_oracle.dequantize(rq_cpu.region(q, off, loc).view(torch.uint8).numpy(),
+        want = dequant_fp8_oracle.dequantize(region(q, off, loc).view(torch.uint8).numpy(),
                                              dq_cpu.local_scale(s, w.sg, off, loc).numpy(), w.sg, off[-2], off[-1], w.out)
         assert np.array_equal(dq_cpu.torch_bits(dest), want), w.describe()
     return tables, geom

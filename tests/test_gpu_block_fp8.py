@@ -12,7 +12,8 @@ import torch
 
 import torchstore_b200 as ts
 from oracle.block_fp8_oracle import quantize, torch_quantize
-from tests.test_block_fp8_cpu import fixture_cases, rand_full, region, shard_box
+from tests.helpers import rand_full, region, shard_box
+from tests.test_block_fp8_cpu import fixture_cases
 from torchstore_b200 import _native
 from torchstore_b200.direct_weight_sync import DirectWeightSyncDest, DirectWeightSyncSource
 from torchstore_b200.transport.types import TensorSlice

@@ -12,7 +12,8 @@ import torch
 import torchstore_b200 as ts
 from oracle.block_fp8_oracle import quantize as block_quantize
 from oracle.dequant_fp8_oracle import GRANULARITIES, SCALE_SET, dequantize, scale_shape, torch_dequantize
-from tests.test_dequant_fp8_cpu import fp8_full, global_scale, local_scale, region, shard_box, torch_bits
+from tests.helpers import region, shard_box
+from tests.test_dequant_fp8_cpu import fp8_full, global_scale, local_scale, torch_bits
 from torchstore_b200 import _native
 from torchstore_b200.direct_weight_sync import DirectWeightSyncDest, DirectWeightSyncSource, ScaledNvlinkBuffer
 from torchstore_b200.transport.types import TensorSlice

@@ -4,7 +4,6 @@ the second replays the golden plans recorded from the reference; the third check
 Llama-3 FSDP->TP sync against the numpy oracle."""
 
 import asyncio
-import hashlib
 import itertools
 import json
 import os
@@ -14,7 +13,7 @@ import pytest
 import torch
 
 from oracle import reshard_oracle as ro
-from tests.helpers import llama_layout
+from tests.helpers import llama_layout, sha256_of
 from torchstore_b200.direct_weight_sync import (DirectWeightSyncDest, DirectWeightSyncSource, NvlinkBuffer,
                                                 RDMAWeightHandle)
 from torchstore_b200.transport.types import TensorSlice
@@ -209,10 +208,6 @@ def test_cpu_destination_fails_loudly():
 # ---------------------------------------------------------------------------------------------
 # golden plans from the reference
 # ---------------------------------------------------------------------------------------------
-def _sha(t):
-    return hashlib.sha256(t.detach().cpu().contiguous().view(torch.uint8).numpy().tobytes()).hexdigest()
-
-
 def test_golden_reference_plans_and_results():
     cases = json.load(open(os.path.join(GOLDEN, "direct_plan.json")))["cases"]
     for case in cases:
@@ -252,7 +247,7 @@ def test_golden_reference_plans_and_results():
             })
         assert got_ops == case["ops"], case["label"]
         for name, digest in case["dest_sha256"].items():
-            assert _sha(dest_sd[name]) == digest, (case["label"], name)
+            assert sha256_of(dest_sd[name]) == digest, (case["label"], name)
         sync.close()
 
 

@@ -4,7 +4,6 @@ multi-rect fp8 workloads against the C oracle, direct weight sync with fp8 stagi
 destinations, and the store path's fused fp8 gets."""
 
 import asyncio
-import hashlib
 import json
 import os
 import random
@@ -13,8 +12,9 @@ import pytest
 import torch
 
 import torchstore_b200 as ts
+import workloads
 from oracle import fp8_oracle
-from tests.helpers import assert_equal_modulo_nan, rect_fields
+from tests.helpers import assert_equal_modulo_nan, rect_fields, sha256_of
 from tests.test_fp8_cast_cpu import SHORT as SHORT_NAMES
 from tests.test_fp8_cast_cpu import VECTOR_MODE, fp8_case, host_bases
 from torchstore_b200 import _native
@@ -213,19 +213,8 @@ def direct_fp8_full(gshape, src_dtype, seed):
     return full.to(getattr(torch, src_dtype))
 
 
-def shard_box(shape, n, r, placement):
-    off, loc = [0] * len(shape), list(shape)
-    if placement[0] == "S":
-        d = placement[1]
-        chunk = -(-shape[d] // n)
-        start, stop = min(shape[d], chunk * r), min(shape[d], chunk * (r + 1))
-        off[d] = start if stop > start else shape[d]
-        loc[d] = max(0, stop - start)
-    return tuple(off), tuple(loc)
-
-
 def tslice(shape, n, r, placement):
-    off, loc = shard_box(shape, n, r, placement)
+    off, loc = workloads.shard_box(shape, n, r, placement)
     return TensorSlice(off, (r,), tuple(shape), loc, (n,))
 
 
@@ -246,10 +235,6 @@ def register_fsdp(full, n_src, **kw):
     return sources, handles
 
 
-def sha(t):
-    return hashlib.sha256(u8(t.detach().cpu()).numpy().tobytes()).hexdigest()
-
-
 def test_register_fp8_transfer_dtype_and_pull_matches_torch_and_the_reference():
     with open(GOLDEN) as f:
         cases = json.load(f)["cases"]
@@ -265,7 +250,7 @@ def test_register_fp8_transfer_dtype_and_pull_matches_torch_and_the_reference():
             sync = DirectWeightSyncDest()
             run(sync.pull({"w": handles}, {"w": dest}, {"w": dsl}))
             assert torch.equal(u8(dest), u8(box(want_full, dsl))), (c, drank)
-            assert sha(dest) == rec["sha256"], (c, drank)
+            assert sha256_of(dest) == rec["sha256"], (c, drank)
             sync.close()
         for src, _ in sources:
             run(src.cleanup())

@@ -28,8 +28,9 @@ from oracle.requant_fp8_oracle import SCALE_POISON, torch_requantize
 from tests import test_gpu_dequant_fp8 as dq_gpu
 from tests import test_gpu_requant_fp8 as rq_gpu
 from tests.fp8_regimes import REGIMES, WORKLOADS, Workload, geometry, split, whole
+from tests.helpers import region, shard_box
 from tests.test_gpu_dequant_fp8 import KW, cleanup, guarded, guards_intact, register
-from tests.test_requant_fp8_cpu import CODE, dest_scale_shape, fp8_full, global_scale, local_scale, region, shard_box
+from tests.test_requant_fp8_cpu import CODE, dest_scale_shape, fp8_full, global_scale, local_scale
 from torchstore_b200 import _native
 from torchstore_b200.direct_weight_sync import DirectWeightSyncDest, DirectWeightSyncSource, _add_dq_source
 from torchstore_b200.planner import build_rects

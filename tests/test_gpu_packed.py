@@ -11,7 +11,7 @@ import torch
 
 import workloads
 from oracle import packed_oracle as po
-from tests.packed_harness import fsdp_handles, pull_args, unfused_args, window
+from tests.helpers import fsdp_handles, pull_args, region, unfused_args
 from torchstore_b200.direct_weight_sync import (DirectWeightSyncDest, DirectWeightSyncSource, NvlinkBuffer, PackedPart,
                                                 RDMAWeightHandle, source_scale_shapes)
 from torchstore_b200.transport.types import TensorSlice
@@ -34,7 +34,7 @@ def masters(layout, seed, device=DEV):
 
 
 def nv_handles(layout, n, full):
-    return fsdp_handles(layout, n, lambda name, off, loc: NvlinkBuffer(window(full[name], off, loc).contiguous()))
+    return fsdp_handles(layout, n, lambda name, off, loc: NvlinkBuffer(region(full[name], off, loc).contiguous()))
 
 
 def as_np(t):
@@ -93,7 +93,7 @@ def test_llama_into_fp8_destinations(staged):
             sd, sl = {}, {}
             for name, (shape, _) in hf.items():
                 off, loc = workloads.shard_box(shape, 8, r, ("S", 0))
-                sd[name], sl[name] = window(full[name], off, loc).contiguous(), TensorSlice(off, (r,), shape, loc, (8,))
+                sd[name], sl[name] = region(full[name], off, loc).contiguous(), TensorSlice(off, (r,), shape, loc, (8,))
             src = DirectWeightSyncSource()
             for name, h in src.register(sd, rank=r, transfer_dtype=E4M3, tensor_slices=sl).items():
                 handles.setdefault(name, []).append(h)
@@ -194,7 +194,7 @@ def scaled_sources(g, qdtype, seed):
         sd, sl = {}, {}
         for name, (shape, _) in layout.items():
             off, loc = workloads.shard_box(shape, 2, r, ("S", 0))
-            sd[name], sl[name] = window(full[name], off, loc).contiguous(), TensorSlice(off, (r,), shape, loc, (2,))
+            sd[name], sl[name] = region(full[name], off, loc).contiguous(), TensorSlice(off, (r,), shape, loc, (2,))
         src = DirectWeightSyncSource()
         for name, h in src.register(sd, rank=r, tensor_slices=sl, quantize={n: g for n in sd},
                                     quant_dtype=qdtype).items():

@@ -29,10 +29,11 @@ from oracle import block_fp8_oracle, int8_source_oracle, scaled_fp8_oracle, ue8m
 from oracle.block_fp8_oracle import synth_f32
 from tests import test_gpu_block_fp8 as bq_gpu
 from tests.fp8_regimes import split, whole
+from tests.helpers import rand_full, region
 from tests import test_gpu_scaled_fp8 as sq_gpu
 from tests.quant_pull_regimes import (BLOCK, ES, GRANULARITIES, KW, REGIMES, WORKLOADS, Pull, compile_tables, plan_bytes,
                                       scale_shape, spots)
-from tests.test_block_fp8_cpu import assert_block_fp8_equal, rand_full, region
+from tests.test_block_fp8_cpu import assert_block_fp8_equal
 from tests.test_gpu_dequant_fp8 import guarded, guards_intact
 from tests.test_gpu_fp8_regimes import draw, named, skip_unless_free
 from tests.test_gpu_source_quant_regimes import on_device

@@ -15,8 +15,9 @@ import torchstore_b200 as ts
 from oracle import ue8m0_oracle
 from oracle.dequant_fp8_oracle import GRANULARITIES, SCALE_SET, scale_shape, torch_dequantize
 from oracle.requant_fp8_oracle import PAIRS, quantize, requantize, torch_requantize
+from tests.helpers import region, shard_box
 from tests.test_gpu_dequant_fp8 import KW, cleanup, guarded, guards_intact, register
-from tests.test_requant_fp8_cpu import dest_scale_shape, fp8_full, global_scale, local_scale, region, shard_box
+from tests.test_requant_fp8_cpu import dest_scale_shape, fp8_full, global_scale, local_scale
 from torchstore_b200 import _native
 from torchstore_b200.direct_weight_sync import DirectWeightSyncDest, DirectWeightSyncSource
 from torchstore_b200.transport.types import TensorSlice

@@ -11,7 +11,7 @@ import torch
 import workloads
 from oracle import packed_oracle as po
 from oracle import rotary_oracle as ro
-from tests.packed_harness import pull_args, window
+from tests.helpers import pull_args, region
 from tests.test_gpu_packed import as_np, masters, nv_handles, pull, run, whole_handle
 from torchstore_b200.direct_weight_sync import (DirectWeightSyncDest, DirectWeightSyncSource, PackedPart,
                                                 RDMAWeightHandle, source_scale_shapes)
@@ -68,7 +68,7 @@ def test_llama_into_fp8_destinations(staged):
             sd, sl = {}, {}
             for name, (shape, _) in layout.items():
                 off, loc = workloads.shard_box(shape, 8, r, ("S", 0))
-                sd[name], sl[name] = window(full[name], off, loc).contiguous(), TensorSlice(off, (r,), shape, loc, (8,))
+                sd[name], sl[name] = region(full[name], off, loc).contiguous(), TensorSlice(off, (r,), shape, loc, (8,))
             src = DirectWeightSyncSource()
             for name, h in src.register(sd, rank=r, transfer_dtype=E4M3, tensor_slices=sl).items():
                 handles.setdefault(name, []).append(h)
@@ -143,7 +143,7 @@ def scaled_attention(g, qdtype, seed, n=2):
         sd, sl = {}, {}
         for name, t in full.items():
             off, loc = workloads.shard_box(tuple(t.shape), n, r, ("S", 0))
-            sd[name], sl[name] = window(t, off, loc).contiguous(), TensorSlice(off, (r,), tuple(t.shape), loc, (n,))
+            sd[name], sl[name] = region(t, off, loc).contiguous(), TensorSlice(off, (r,), tuple(t.shape), loc, (n,))
         src = DirectWeightSyncSource()
         for name, h in src.register(sd, rank=r, tensor_slices=sl, quantize={k: g for k in sd}, quant_dtype=qdtype).items():
             handles.setdefault(name, []).append(h)

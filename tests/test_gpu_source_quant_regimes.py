@@ -27,11 +27,11 @@ from oracle.source_quant_oracle import GRANULARITIES, fixture_inputs, synth_f32,
 from tests import test_gpu_dequant_fp8 as dq_gpu
 from tests import test_gpu_requant_fp8 as rq_gpu
 from tests.fp8_regimes import split, whole
+from tests.helpers import region, shard_box
 from tests.source_quant_regimes import CODE, REGIMES, WORKLOADS, Target, plan_bytes
 from tests.test_gpu_dequant_fp8 import guarded, guards_intact
 from tests.test_gpu_fp8_regimes import named, skip_unless_free
 from tests.test_gpu_source_quant import assert_exact
-from tests.test_requant_fp8_cpu import region, shard_box
 from tests.test_source_quant_cpu import CODE as GCODE
 from tests.test_source_quant_cpu import assert_source_quant_equal, compile_host, fixture_cases
 from tests.test_source_quant_regimes_cpu import (CONSUMERS, SHARD_LAYOUTS, assert_shared_groups_differ, layout_shards,

@@ -3,7 +3,6 @@ fixtures recorded from the reference's LocalClient + SharedMemory transport, plu
 reference's integration tests pin (tests/test_store.py, test_tensor_slice.py, test_state_dict.py)."""
 
 import asyncio
-import hashlib
 import itertools
 import json
 import os
@@ -15,6 +14,7 @@ import torch
 import torchstore_b200 as ts
 from torchstore_b200 import _native
 from oracle import reshard_oracle as ro
+from tests.helpers import sha256_of
 from torchstore_b200.transport import create_transport_buffer
 from torchstore_b200.transport.types import Request, TensorSlice
 
@@ -25,10 +25,6 @@ DEV = "cuda:0"
 
 def run(coro):
     return asyncio.run(coro)
-
-
-def _sha(t):
-    return hashlib.sha256(t.detach().cpu().contiguous().view(torch.uint8).numpy().tobytes()).hexdigest()
 
 
 @pytest.fixture(autouse=True)
@@ -111,10 +107,10 @@ def test_tensor_slice_gets():
             await ts.put("t", t)
             spec = TensorSlice(tuple(ts_gold["offsets"]), (), tuple(ts_gold["global_shape"]), tuple(ts_gold["local_shape"]), ())
             got = await ts.get("t", tensor_slice_spec=spec)
-            assert _sha(got) == ts_gold["sha256"]
+            assert sha256_of(got) == ts_gold["sha256"]
             buf = torch.zeros(5, 10, device=DEV)
             out = await ts.get("t", buf, spec)
-            assert out is buf and _sha(buf) == ts_gold["sha256"]
+            assert out is buf and sha256_of(buf) == ts_gold["sha256"]
             with pytest.raises(ValueError, match="does not match"):
                 await ts.get("t", torch.zeros(3, 3, device=DEV), spec)
         finally:
@@ -155,9 +151,9 @@ def test_reshard_matrix_matches_reference(monkeypatch):
                     got = await ts.get("test_key", dest, TensorSlice(dsl.offsets, dsl.coordinates, dsl.global_shape,
                                                                      dsl.local_shape, dsl.mesh_shape))
                     assert got is dest
-                    assert _sha(dest) == r["sha256"], (case["src_mesh"], case["dst_mesh"], r["rank"])
+                    assert sha256_of(dest) == r["sha256"], (case["src_mesh"], case["dst_mesh"], r["rank"])
                 whole = await ts.get("test_key")
-                assert _sha(whole) == case["full_get_sha256"]
+                assert sha256_of(whole) == case["full_get_sha256"]
             finally:
                 await ts.shutdown()
 

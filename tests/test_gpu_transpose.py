@@ -9,7 +9,7 @@ import torch
 
 import workloads
 from oracle import transpose_oracle as to
-from tests.packed_harness import fsdp_handles, pull_args, window
+from tests.helpers import fsdp_handles, pull_args, region
 from tests.test_gpu_packed import as_np, masters, nv_handles, pull, run, whole_handle
 from torchstore_b200.direct_weight_sync import DirectWeightSyncDest, NvlinkBuffer, PackedPart, RDMAWeightHandle
 from torchstore_b200.transport.types import TensorSlice
@@ -79,12 +79,12 @@ def test_qwen3_30b_a3b_full_size_layer(tp, rank, ep):
 # -- element sizes, casts, alignment -----------------------------------------------------------------------------------
 def one_part(src, dest, index, offsets, n=1, dim=0):
     shape = tuple(src.shape)
-    handles = fsdp_handles({"s": (shape, None)}, n, lambda _, off, loc: NvlinkBuffer(window(src, off, loc).contiguous()))
+    handles = fsdp_handles({"s": (shape, None)}, n, lambda _, off, loc: NvlinkBuffer(region(src, off, loc).contiguous()))
     if dim:  # shards cut along another dim
         handles = {"s": []}
         for r in range(n):
             off, loc = workloads.shard_box(shape, n, r, ("S", dim))
-            handles["s"].append(RDMAWeightHandle(NvlinkBuffer(window(src, off, loc).contiguous()),
+            handles["s"].append(RDMAWeightHandle(NvlinkBuffer(region(src, off, loc).contiguous()),
                                                  TensorSlice(off, (r,), shape, loc, (n,)), r))
     part = PackedPart("s", index, offsets, transpose=True)
     return pull(handles, {"d": dest}, packed={"d": (part,)}), part

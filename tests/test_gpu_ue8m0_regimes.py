@@ -30,11 +30,11 @@ from tests import test_gpu_fp8_regimes as fp8_gpu
 from tests import test_gpu_quant_pull_regimes as qp_gpu
 from tests import test_gpu_requant_fp8 as rq_gpu
 from tests import test_gpu_source_quant_regimes as sq_gpu
+from tests.helpers import region
 from tests.quant_pull_regimes import Pull
 from tests.test_gpu_dequant_fp8 import cleanup, guarded, guards_intact, register
 from tests.test_gpu_fp8_regimes import named
 from tests.test_gpu_source_quant import assert_exact
-from tests.test_requant_fp8_cpu import region
 from tests.test_ue8m0_cpu import fixture_cases, is_pow2, u32
 from tests.test_ue8m0_regimes_cpu import LOSSLESS, RQ_REGIMES, assert_lossless
 from torchstore_b200 import _native

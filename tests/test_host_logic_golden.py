@@ -3,7 +3,6 @@ planner) against the fixtures recorded from the reference.  CPU only: plans are 
 tensors and checked as metadata; bytes are moved by the ORACLE's C routine from the product's
 rectangle descriptors, which validates planner + descriptor builder end to end without a GPU."""
 
-import hashlib
 import itertools
 import json
 import os
@@ -14,6 +13,7 @@ import torch
 
 from oracle import c_oracle
 from oracle import reshard_oracle as ro
+from tests.helpers import HostBuffer, sha256_of
 from torchstore_b200.direct_weight_sync import DirectWeightSyncDest, RDMAWeightHandle
 from torchstore_b200.planner import StridedMem, build_rects
 from torchstore_b200.transport.types import Request, TensorSlice
@@ -83,19 +83,6 @@ def test_to_byte_view():
     assert to_byte_view(t).shape == (12,) and to_byte_view(t).data_ptr() == t.data_ptr()
 
 
-class HostBuffer:
-    """Stands in for NvlinkBuffer in CPU planning tests: only identity and metadata are used."""
-
-    def __init__(self, tensor):
-        self.tensor = tensor
-        self.dtype = tensor.dtype
-        self.shape = tuple(tensor.shape)
-
-
-def _sha(t):
-    return hashlib.sha256(t.contiguous().view(torch.uint8).numpy().tobytes()).hexdigest()
-
-
 def test_direct_plan_golden_ops_and_bytes_via_oracle_executor():
     cases = load("direct_plan.json")["cases"]
     for case in cases:
@@ -110,7 +97,7 @@ def test_direct_plan_golden_ops_and_bytes_via_oracle_executor():
                 sl = ro.make_slice(shape, smesh, coord, spl)
                 shard = full[tuple(slice(o, o + s) for o, s in zip(sl.offsets, sl.local_shape))].contiguous()
                 ts = TensorSlice(sl.offsets, sl.coordinates, sl.global_shape, sl.local_shape, sl.mesh_shape)
-                hl.append(RDMAWeightHandle(HostBuffer(shard), ts, rank))
+                hl.append(RDMAWeightHandle(HostBuffer(shard, shard.shape, shard.dtype), ts, rank))
             all_handles[name] = hl
             if p["dst_mesh"] is None:
                 dest_sd[name] = torch.zeros(shape)
@@ -132,11 +119,11 @@ def test_direct_plan_golden_ops_and_bytes_via_oracle_executor():
                         "dest_index": None if op.dest_slices is None else [[s.start, s.stop] for s in op.dest_slices]})
         assert got == case["ops"], case["label"]
         # descriptors built by the product, bytes moved by the oracle
-        pairs = [sync.op_windows(op, StridedMem.from_tensor(op.rdma_buffer.tensor)) for op in plan]
+        pairs = [sync.op_windows(op, StridedMem.from_tensor(op.rdma_buffer.shard)) for op in plan]
         rects, n = build_rects(pairs)
         c_oracle.copy_rects(rects, n)
         for name, digest in case["dest_sha256"].items():
-            assert _sha(dest_sd[name]) == digest, (case["label"], name)
+            assert sha256_of(dest_sd[name]) == digest, (case["label"], name)
 
 
 def test_request_from_dtensor_on_fake_process_group():

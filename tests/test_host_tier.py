@@ -259,21 +259,17 @@ def test_put_batch_wait_false_on_the_host_tier_completes_inline():
 
 
 # ---- the reference's own results as the oracle for the host tiers ---------------------------------------
-import hashlib
 import itertools
 import json
 
 import numpy as np
 
 from oracle import reshard_oracle as ro
+from tests.helpers import sha256_of
 from torchstore_b200.transport import create_transport_buffer
 from torchstore_b200.transport.types import Request
 
 GOLDEN = os.path.join(os.path.dirname(__file__), "golden")
-
-
-def _sha(t):
-    return hashlib.sha256(t.detach().cpu().contiguous().view(torch.uint8).numpy().tobytes()).hexdigest()
 
 
 @pytest.mark.parametrize("transport", ["SharedMemory", "MonarchRPC"])
@@ -320,8 +316,8 @@ def test_reshard_matrix_matches_the_reference_results_on_the_host_tiers(transpor
                     got = await ts.get("test_key", dest, TensorSlice(dsl.offsets, dsl.coordinates, dsl.global_shape,
                                                                      dsl.local_shape, dsl.mesh_shape))
                     assert got is dest
-                    assert _sha(dest) == r["sha256"], (transport, case["src_mesh"], case["dst_mesh"], r["rank"])
-                assert _sha(await ts.get("test_key")) == case["full_get_sha256"]
+                    assert sha256_of(dest) == r["sha256"], (transport, case["src_mesh"], case["dst_mesh"], r["rank"])
+                assert sha256_of(await ts.get("test_key")) == case["full_get_sha256"]
             finally:
                 await ts.shutdown()
 

@@ -13,6 +13,7 @@ import torch
 
 from oracle.int8_oracle import (GRANULARITIES, SPECIALS, bits_of, digest, fixture_inputs, quantize, replay_block,
                                 replay_scaled, same_scales, scales_of_amax, synth_f32, torch_quantize, widen)
+from tests.helpers import Boom, fake_dest, no_export, scaled_handle
 from torchstore_b200 import _native
 from torchstore_b200.direct_weight_sync import DirectWeightSyncDest
 from torchstore_b200.planner import StridedMem, build_rects
@@ -242,33 +243,7 @@ def test_tsb_i8_stays_out_of_the_copy_plan_and_the_other_kinds():
 
 
 # ---- Python routing and refusals, before any device work ---------------------------------------------------------
-class Boom(Exception):
-    pass
-
-
-@pytest.fixture
-def nothing_compiled(monkeypatch):
-    from torchstore_b200 import direct_weight_sync as dws
-
-    def boom(*a, **k):
-        raise Boom("exported or compiled before validation finished")
-
-    monkeypatch.setattr(dws.HbmDescriptor, "from_tensor", staticmethod(boom))
-    for name in ("build", "build_source_quant", "build_dequant_fp8", "build_requant_fp8", "build_block_fp8", "build_scaled_fp8"):
-        monkeypatch.setattr(dws.Plans, name, classmethod(boom))
-
-
-def fake_dest(dtype, shape=(256, 256)):
-    """A contiguous 'CUDA' destination stand-in for _check_scales (it reads dtype, shape, contiguity and device)."""
-    return types.SimpleNamespace(dtype=dtype, shape=torch.Size(shape), dim=lambda: len(shape), numel=lambda: 256 * 256,
-                                 is_contiguous=lambda: True, is_cuda=True, device=torch.device("cpu"), data_ptr=lambda: 0)
-
-
-def handle(dtype, granularity=None):
-    buf = types.SimpleNamespace(dtype=dtype)
-    if granularity:
-        buf.granularity = granularity
-    return types.SimpleNamespace(rdma_buffer=buf)
+no_export = pytest.fixture(no_export)
 
 
 def scale_for(g):
@@ -279,7 +254,7 @@ def scale_for(g):
 def test_int8_destinations_take_the_quantise_route(g):
     for dtype in (torch.bfloat16, torch.float16, torch.float32):
         d = fake_dest(torch.int8)
-        out = DirectWeightSyncDest._check_scales({"w": [handle(dtype)] * 2}, {"w": d}, {KW[g]: {"w": scale_for(g)}})
+        out = DirectWeightSyncDest._check_scales({"w": [scaled_handle(dtype)] * 2}, {"w": d}, {KW[g]: {"w": scale_for(g)}})
         assert out["w"][0] == KW[g] and out["w"][1] is d and out["w"][3] == "quantise"
 
 
@@ -287,12 +262,13 @@ def test_int8_destinations_take_the_quantise_route(g):
 def test_scaled_fp8_handles_into_int8_are_refused(g):
     for kw in ({}, {"requantize": True}, {"verbatim": True}):
         with pytest.raises(TypeError, match="int8 destinations are quantised from bf16, f16 or f32 handles"):
-            DirectWeightSyncDest._check_scales({"w": [handle(E4M3, g)]}, {"w": fake_dest(torch.int8)},
+            DirectWeightSyncDest._check_scales({"w": [scaled_handle(E4M3, g)]}, {"w": fake_dest(torch.int8)},
                                                {KW[g]: {"w": scale_for(g)}}, **kw)
 
 
 def test_int8_handles_need_one_float_dtype():
-    for handles in ([handle(torch.int8)], [handle(E4M3)], [handle(torch.bfloat16), handle(torch.float32)]):
+    for handles in ([scaled_handle(torch.int8)], [scaled_handle(E4M3)],
+                    [scaled_handle(torch.bfloat16), scaled_handle(torch.float32)]):
         with pytest.raises(TypeError, match="read bf16, f16 or f32 handles of one dtype"):
             DirectWeightSyncDest._check_scales({"w": handles}, {"w": fake_dest(torch.int8)},
                                                {"channel_scales": {"w": scale_for("channel")}}, requantize=True)
@@ -301,16 +277,16 @@ def test_int8_handles_need_one_float_dtype():
 def test_other_destination_dtypes_are_still_refused():
     for dtype in (torch.uint8, torch.float8_e5m2, torch.bfloat16, torch.int16):
         with pytest.raises(TypeError, match="must be float8_e4m3fn or int8"):
-            DirectWeightSyncDest._check_scales({"w": [handle(torch.bfloat16)]}, {"w": fake_dest(dtype)},
+            DirectWeightSyncDest._check_scales({"w": [scaled_handle(torch.bfloat16)]}, {"w": fake_dest(dtype)},
                                                {"block_scales": {"w": scale_for("block")}})
 
 
-def test_scale_fmt_with_an_int8_destination_is_refused(nothing_compiled, monkeypatch):
+def test_scale_fmt_with_an_int8_destination_is_refused(no_export, monkeypatch):
     d = DirectWeightSyncDest()
     monkeypatch.setattr(DirectWeightSyncDest, "_build_plan", lambda *a, **k: (_ for _ in ()).throw(Boom("planned")))
     dest = fake_dest(torch.int8)
     with pytest.raises(ValueError, match="does not apply to int8 destinations"):
-        asyncio.run(d.pull({"w": [handle(torch.bfloat16)]}, {"w": dest}, channel_scales={"w": scale_for("channel")},
+        asyncio.run(d.pull({"w": [scaled_handle(torch.bfloat16)]}, {"w": dest}, channel_scales={"w": scale_for("channel")},
                            scale_fmt="ue8m0"))
     assert d._plan is None
 
@@ -370,7 +346,7 @@ def test_plan_rebuilds_on_a_dtype_flip(monkeypatch, built, now):
     monkeypatch.setattr(DirectWeightSyncDest, "_build_plan", lambda self, *a, **k: plans_built.append(1) or [])
     monkeypatch.setattr(dws.Plans, "build", classmethod(lambda cls, per_device: dws.Plans()))
     monkeypatch.setattr(dws.Plans, "build_scaled_fp8", classmethod(lambda cls, per_device, flags=0: dws.Plans()))
-    handles = {"w": [handle(torch.bfloat16)]}
+    handles = {"w": [scaled_handle(torch.bfloat16)]}
     scales = {"w": scale_for("channel")}
     d = DirectWeightSyncDest()
     asyncio.run(d.pull(handles, {"w": fake_dest(built)}, channel_scales=scales))

@@ -22,7 +22,7 @@ from oracle.ue8m0_oracle import group_amax, group_ids
 from tests import fp8_regimes, quant_pull_regimes, source_quant_regimes
 from tests import test_dequant_fp8_cpu as dq_cpu
 from tests import test_requant_fp8_cpu as rq_cpu
-from tests.test_block_fp8_cpu import region
+from tests.helpers import region
 from tests.test_quant_pull_regimes_cpu import host_shard, workload_inputs
 from tests.test_source_quant_cpu import host_shard as source_shard
 from tests.test_source_quant_regimes_cpu import workload_inputs as source_inputs
@@ -180,7 +180,7 @@ def test_dequant_workload_replays_to_the_int8_oracle(name):
     w = fp8_regimes.WORKLOADS[name]
     q, s, dest, _, _ = dequant(name)
     off, loc = w.dst
-    qr, sr = rq_cpu.region(q, off, loc), dq_cpu.local_scale(s, w.sg, off, loc)
+    qr, sr = region(q, off, loc), dq_cpu.local_scale(s, w.sg, off, loc)
     want = i8s.dequantize(qr.numpy(), sr.numpy(), w.sg, off[-2], off[-1], w.out)
     assert np.array_equal(i8s.bits_of(dest), want), w.describe()
     torch_want = i8s.torch_dequantize(qr, sr, w.sg, off[-2], off[-1], getattr(torch, w.out))

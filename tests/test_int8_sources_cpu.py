@@ -14,6 +14,7 @@ import torch
 from oracle.int8_source_oracle import (DSTS, GRANULARITIES, bits_of, dequant_inputs, dequantize, digest, int8_of,
                                        quant_inputs, quantize, replay_dequant, replay_source, scale_of, scale_shape,
                                        synth_f32, torch_dequantize, torch_quantize, widen)
+from tests.helpers import Boom, fake_dest, no_export, scaled_handle
 from torchstore_b200 import _native
 from torchstore_b200.direct_weight_sync import DirectWeightSyncDest, DirectWeightSyncSource
 from torchstore_b200.planner import StridedMem, build_rects
@@ -244,18 +245,6 @@ def test_tsb_i8_stays_out_of_the_casts_the_copy_plan_and_requantising():
 
 
 # ---- the route table -----------------------------------------------------------------------------------------------
-def fake_dest(dtype, shape=(256, 256)):
-    return types.SimpleNamespace(dtype=dtype, shape=torch.Size(shape), dim=lambda: len(shape), numel=lambda: 256 * 256,
-                                 is_contiguous=lambda: True, is_cuda=True, device=torch.device("cpu"), data_ptr=lambda: 0)
-
-
-def handle(dtype, granularity=None):
-    buf = types.SimpleNamespace(dtype=dtype)
-    if granularity:
-        buf.granularity = granularity
-    return types.SimpleNamespace(rdma_buffer=buf)
-
-
 def scale_for(g):
     return torch.zeros({"block": (2, 2), "channel": (256, 1), "tensor": ()}[g])
 
@@ -274,12 +263,12 @@ FLAGS = ({}, {"requantize": True}, {"verbatim": True})
 @pytest.mark.parametrize("g", GRANULARITIES)
 def test_int8_handles_into_floats_dequantise(g):
     for dtype in FLOATS:
-        assert check_dequant([handle(torch.int8, g)] * 2, torch.zeros(4, 4, dtype=dtype)) == {"w"}
+        assert check_dequant([scaled_handle(torch.int8, g)] * 2, torch.zeros(4, 4, dtype=dtype)) == {"w"}
 
 
 @pytest.mark.parametrize("g", GRANULARITIES)
 def test_int8_handles_into_named_int8_move_verbatim_only(g):
-    h = [handle(torch.int8, g)] * 2
+    h = [scaled_handle(torch.int8, g)] * 2
     assert check_scales(h, fake_dest(torch.int8), g, verbatim=True)["w"][3] == "verbatim"
     with pytest.raises(TypeError, match="pass verbatim=True"):
         check_scales(h, fake_dest(torch.int8), g)
@@ -287,40 +276,40 @@ def test_int8_handles_into_named_int8_move_verbatim_only(g):
         check_scales(h, fake_dest(torch.int8), g, requantize=True)
     other = "tensor" if g != "tensor" else "channel"
     with pytest.raises(ValueError, match="granularity only"):
-        check_scales([handle(torch.int8, other)], fake_dest(torch.int8), g, verbatim=True)
+        check_scales([scaled_handle(torch.int8, other)], fake_dest(torch.int8), g, verbatim=True)
 
 
 @pytest.mark.parametrize("g", GRANULARITIES)
 def test_int8_handles_into_unnamed_int8_are_bytes(g):
-    assert check_dequant([handle(torch.int8, g)], torch.zeros(4, 4, dtype=torch.int8)) == set()
+    assert check_dequant([scaled_handle(torch.int8, g)], torch.zeros(4, 4, dtype=torch.int8)) == set()
 
 
 @pytest.mark.parametrize("g", GRANULARITIES)
 def test_int8_handles_never_become_fp8(g):
     for kw in FLAGS:
         with pytest.raises(TypeError, match="int8 is not converted to fp8"):
-            check_scales([handle(torch.int8, g)], fake_dest(E4M3), g, **kw)
+            check_scales([scaled_handle(torch.int8, g)], fake_dest(E4M3), g, **kw)
     with pytest.raises(TypeError, match="int8 is not converted to fp8"):
-        check_dequant([handle(torch.int8, g)], torch.zeros(4, 4, dtype=E4M3))
+        check_dequant([scaled_handle(torch.int8, g)], torch.zeros(4, 4, dtype=E4M3))
 
 
 @pytest.mark.parametrize("dtype", (torch.uint8, torch.int16, torch.float64, torch.float8_e5m2), ids=str)
 def test_int8_handles_into_other_dtypes_are_refused(dtype):
     with pytest.raises(TypeError, match="must be bfloat16, float16, float32"):
-        check_dequant([handle(torch.int8, "channel")], torch.zeros(4, 4, dtype=dtype))
+        check_dequant([scaled_handle(torch.int8, "channel")], torch.zeros(4, 4, dtype=dtype))
     with pytest.raises(TypeError, match="must be float8_e4m3fn or int8"):
-        check_scales([handle(torch.int8, "channel")], fake_dest(dtype), "channel", verbatim=True)
+        check_scales([scaled_handle(torch.int8, "channel")], fake_dest(dtype), "channel", verbatim=True)
 
 
 def test_mixed_formats_and_mixed_scaling_are_refused():
-    mixed = [handle(torch.int8, "channel"), handle(E4M3, "channel")]
+    mixed = [scaled_handle(torch.int8, "channel"), scaled_handle(E4M3, "channel")]
     for kw in FLAGS:
         for dest in (fake_dest(torch.int8), fake_dest(E4M3)):
             with pytest.raises(ValueError, match="mix scaled int8 and scaled fp8"):
                 check_scales(mixed, dest, "channel", **kw)
     with pytest.raises(ValueError, match="mix scaled int8 and scaled fp8"):
         check_dequant(mixed, torch.zeros(4, 4))
-    half = [handle(torch.int8, "channel"), handle(torch.int8)]
+    half = [scaled_handle(torch.int8, "channel"), scaled_handle(torch.int8)]
     with pytest.raises(ValueError, match="mix scaled int8 and unscaled"):
         check_dequant(half, torch.zeros(4, 4))
     for kw in FLAGS:
@@ -332,30 +321,15 @@ def test_mixed_formats_and_mixed_scaling_are_refused():
 def test_fp8_verdicts_are_unchanged(g):
     for kw in FLAGS:
         with pytest.raises(TypeError, match="int8 destinations are quantised from bf16, f16 or f32 handles"):
-            check_scales([handle(E4M3, g)], fake_dest(torch.int8), g, **kw)
-    assert check_scales([handle(E4M3, g)], fake_dest(E4M3), g, verbatim=True)["w"][3] == "verbatim"
-    assert check_dequant([handle(E4M3, g)], torch.zeros(4, 4)) == {"w"}
+            check_scales([scaled_handle(E4M3, g)], fake_dest(torch.int8), g, **kw)
+    assert check_scales([scaled_handle(E4M3, g)], fake_dest(E4M3), g, verbatim=True)["w"][3] == "verbatim"
+    assert check_dequant([scaled_handle(E4M3, g)], torch.zeros(4, 4)) == {"w"}
     with pytest.raises(ValueError, match="mix scaled fp8 and unscaled"):
-        check_dequant([handle(E4M3, g), handle(torch.bfloat16)], torch.zeros(4, 4))
+        check_dequant([scaled_handle(E4M3, g), scaled_handle(torch.bfloat16)], torch.zeros(4, 4))
 
 
 # ---- refusals before anything is compiled ---------------------------------------------------------------------------
-class Boom(Exception):
-    pass
-
-
-@pytest.fixture
-def nothing_exported(monkeypatch):
-    from torchstore_b200 import direct_weight_sync as dws
-
-    def boom(*a, **k):
-        raise Boom("exported, allocated or compiled before validation finished")
-
-    monkeypatch.setattr(dws.HbmDescriptor, "from_tensor", staticmethod(boom))
-    monkeypatch.setattr(torch, "empty", boom)
-    for name in ("build", "build_source_quant", "build_dequant_fp8", "build_requant_fp8", "build_block_fp8",
-                 "build_scaled_fp8"):
-        monkeypatch.setattr(dws.Plans, name, classmethod(boom))
+no_export = pytest.fixture(no_export)
 
 
 def _w(*shape, dtype=torch.bfloat16):
@@ -375,7 +349,7 @@ def _w(*shape, dtype=torch.bfloat16):
     ({"block_scales": {"w": torch.zeros(1, 1)}}, TypeError, "must be float8_e4m3fn or int8, not torch.bfloat16"),
     ({"block_scales": {"i": torch.zeros(1, 1)}, "transfer_dtype": torch.float16}, ValueError, "transfer_dtype"),
 ])
-def test_register_validation(nothing_exported, kw, exc, needle):
+def test_register_validation(no_export, kw, exc, needle):
     src = DirectWeightSyncSource()
     with pytest.raises(exc, match=needle):
         src.register({"w": _w(4, 4), "i": _w(4, 4, dtype=torch.int8)}, rank=0, **kw)
@@ -410,14 +384,15 @@ def test_put_state_dict_passes_quant_dtype_through(monkeypatch):
 def test_pull_refusals_come_before_planning(monkeypatch):
     d = DirectWeightSyncDest()
     monkeypatch.setattr(DirectWeightSyncDest, "_build_plan", lambda *a, **k: (_ for _ in ()).throw(Boom("planned")))
-    h = {"w": [handle(torch.int8, "channel")]}
+    h = {"w": [scaled_handle(torch.int8, "channel")]}
     with pytest.raises(TypeError, match="pass verbatim=True"):
         asyncio.run(d.pull(h, {"w": fake_dest(torch.int8)}, channel_scales={"w": scale_for("channel")}))
     with pytest.raises(ValueError, match="does not apply to int8 destinations"):
         asyncio.run(d.pull(h, {"w": fake_dest(torch.int8)}, channel_scales={"w": scale_for("channel")}, verbatim=True,
                            scale_fmt="ue8m0"))
     with pytest.raises(ValueError, match="mix scaled int8 and scaled fp8"):
-        asyncio.run(d.pull({"w": [handle(torch.int8, "channel"), handle(E4M3, "channel")]}, {"w": torch.zeros(4, 4)}))
+        asyncio.run(d.pull({"w": [scaled_handle(torch.int8, "channel"), scaled_handle(E4M3, "channel")]},
+                           {"w": torch.zeros(4, 4)}))
     assert d._plan is None
 
 
@@ -463,7 +438,7 @@ def test_plan_rebuilds_on_a_dtype_flip(monkeypatch, built, now):
     scales = {"w": scale_for("channel")}
     d = DirectWeightSyncDest()
     for dtype, n in ((built, 1), (built, 1), (now, 2), (now, 2)):
-        asyncio.run(d.pull({"w": [handle(dtype, "channel")]}, {"w": fake_dest(dtype)}, channel_scales=scales,
+        asyncio.run(d.pull({"w": [scaled_handle(dtype, "channel")]}, {"w": fake_dest(dtype)}, channel_scales=scales,
                            verbatim=True))
         assert len(plans_built) == n
     d.close()

@@ -13,7 +13,7 @@ import torch
 import workloads
 from oracle import c_oracle
 from oracle import packed_oracle as po
-from tests.packed_harness import HostBuffer, fsdp_handles, pull_args, unfused_args, window
+from tests.helpers import HostBuffer, fsdp_handles, handles_of, pull_args, region, unfused_args
 from torchstore_b200 import _native, api, state_dict_utils
 from torchstore_b200.direct_weight_sync import (DirectWeightSyncDest, PackedPart, RDMAWeightHandle, scale_grid,
                                                 source_scale_shapes)
@@ -21,11 +21,6 @@ from torchstore_b200.planner import StridedMem, build_rects
 from torchstore_b200.transport.types import TensorSlice
 
 E4M3 = torch.float8_e4m3fn
-
-
-def handles_of(shape, n=1, dtype=torch.bfloat16):
-    """Row shards of a ``shape`` tensor with metadata-only buffers."""
-    return fsdp_handles({"s": (shape, None)}, n, lambda _, off, loc: HostBuffer(None, loc, dtype))["s"]
 
 
 def check(dest_shape, packed, handles, match, dests=None):
@@ -171,7 +166,7 @@ def host_sources(layout, names, dtype, seed):
 
 def plan_layout(hf, vl, tp, rank, n, sources):
     handles = fsdp_handles(hf, n, lambda name, off, loc: HostBuffer(
-        window(sources[name], off, loc).contiguous() if name in sources else None, loc, torch.bfloat16))
+        region(sources[name], off, loc).contiguous() if name in sources else None, loc, torch.bfloat16))
     dests, slices, packed = pull_args(vl, tp, rank, lambda name, shape: torch.full(shape, 0x5A, dtype=torch.uint8))
     return handles, dests, slices, packed, DirectWeightSyncDest()._build_plan(handles, dests, slices, packed=packed)
 
@@ -280,7 +275,7 @@ def scaled_sources(g, shapes: dict, n, seed):
         full[name] = torch.from_numpy(rng.integers(0, 256, size=shape, dtype=np.uint8)).view(E4M3)
 
         def make(_, off, loc, name=name):
-            shard = window(full[name], off, loc).contiguous()
+            shard = region(full[name], off, loc).contiguous()
             scale = torch.from_numpy(rng.standard_normal(source_scale_shapes(g, loc, off[-2], off[-1])[0]).astype(np.float32))
             return ScaledHost(shard, scale, g, off[-2], off[-1])
         out.update(fsdp_handles({name: (shape, None)}, n, make))

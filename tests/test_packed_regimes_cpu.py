@@ -10,6 +10,7 @@ import pytest
 import torch
 
 from tests import packed_regimes as pr
+from tests.helpers import cuda_like
 from torchstore_b200 import _native
 from torchstore_b200.direct_weight_sync import DirectWeightSyncDest, PackedPart, _build_named
 from torchstore_b200.launch import Plans
@@ -111,7 +112,7 @@ def test_scaled_sources_into_a_dropped_column_dim_are_refused(route):
     assert match and "part 0 \\(source 's0'\\)" in match
     _, handles, dests, scales, _ = host_setup(spec)
     if ro.kind == "requant":  # the scaled destination's checks read only metadata: claim CUDA
-        dests = {n: pr.cuda_like(t) for n, t in dests.items()}
+        dests = {n: cuda_like(t) for n, t in dests.items()}
     sync = DirectWeightSyncDest()
     with pytest.raises(ValueError, match=match):
         asyncio.run(sync.pull(handles, dests, packed=spec.packed(), requantize=spec.requantize,

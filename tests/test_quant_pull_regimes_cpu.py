@@ -10,8 +10,8 @@ import pytest
 import torch
 
 from oracle import block_fp8_oracle, scaled_fp8_oracle
+from tests.helpers import rand_full, region
 from tests.quant_pull_regimes import REGIMES, WORKLOADS, compile_tables, plan_bytes, scale_shape, spots
-from tests.test_block_fp8_cpu import rand_full, region
 from torchstore_b200.direct_weight_sync import DirectWeightSyncDest, RDMAWeightHandle
 from torchstore_b200.planner import StridedMem
 from torchstore_b200.transport.types import TensorSlice

@@ -13,14 +13,10 @@ import torch
 
 from oracle import c_oracle
 from oracle import reshard_oracle as ro
+from tests.helpers import HostBuffer
 from torchstore_b200.direct_weight_sync import DirectWeightSyncDest, RDMAWeightHandle
 from torchstore_b200.planner import StridedMem, build_rects
 from torchstore_b200.transport.types import TensorSlice
-
-
-class HostBuffer:
-    def __init__(self, tensor):
-        self.tensor = tensor
 
 
 def rand_layout(rng, ndim):
@@ -48,7 +44,7 @@ def test_random_mesh_pairs(seed):
         for rank, coord in enumerate(itertools.product(*(range(m) for m in smesh))):
             sl = ro.make_slice(shape, smesh, coord, spl)
             shard = full[tuple(slice(o, o + s) for o, s in zip(sl.offsets, sl.local_shape))].contiguous()
-            handles.append(RDMAWeightHandle(HostBuffer(shard), to_ts(sl), rank))
+            handles.append(RDMAWeightHandle(HostBuffer(shard, shard.shape, shard.dtype), to_ts(sl), rank))
             np_handles.append((sl, rank))
         for coord in itertools.product(*(range(m) for m in dmesh)):
             dsl = ro.make_slice(shape, dmesh, coord, dpl)
@@ -60,7 +56,7 @@ def test_random_mesh_pairs(seed):
             for op, oop in zip(plan, oracle_plan):
                 assert (op.dest_tensor is None) == oop.exact
                 assert op.src_slices == oop.src_index and op.dest_slices == oop.dest_index
-            pairs = [sync.op_windows(op, StridedMem.from_tensor(op.rdma_buffer.tensor)) for op in plan]
+            pairs = [sync.op_windows(op, StridedMem.from_tensor(op.rdma_buffer.shard)) for op in plan]
             rects, n = build_rects(pairs)
             c_oracle.copy_rects(rects, n)
             want = full[tuple(slice(o, o + s) for o, s in zip(dsl.offsets, dsl.local_shape))]

@@ -15,6 +15,8 @@ import torch
 from oracle.dequant_fp8_oracle import GRANULARITIES, scale_shape
 from oracle.requant_fp8_oracle import (PAIRS, canonical_nan, digest, fixture_inputs, quantize, replay, requantize,
                                        torch_requantize)
+from tests.helpers import (Boom, cuda_like, expect_invalid, no_compile, plan_windows, region, shard_box,
+                           shard_handles)
 from torchstore_b200 import _native
 from torchstore_b200.direct_weight_sync import BLOCK, DirectWeightSyncDest, RDMAWeightHandle
 from torchstore_b200.planner import StridedMem, build_rects
@@ -64,18 +66,6 @@ def test_poisoned_scales_poison_their_destination_groups():
 
 
 # ---- the plan compiler, replayed on host memory ----------------------------------------------------
-def shard_box(shape, n, r, dim):
-    off, loc = [0] * len(shape), list(shape)
-    chunk = -(-shape[dim] // n)
-    start, stop = min(shape[dim], chunk * r), min(shape[dim], chunk * (r + 1))
-    off[dim], loc[dim] = start, max(0, stop - start)
-    return tuple(off), tuple(loc)
-
-
-def region(t, off, loc):
-    return t[tuple(slice(o, o + s) for o, s in zip(off, loc))]
-
-
 def global_scale(g, shape, seed):
     gen = torch.Generator().manual_seed(seed)
     return torch.rand(scale_shape(g, shape), generator=gen) * 0.01 + 1e-4
@@ -108,25 +98,15 @@ class FakeScaledBuffer:
 def compile_pull(q_full, full_scale, sg, src_boxes, dst_box, dg, flags=0):
     """Plan a requantising pull of `q_full`'s `sg`-scaled shards into a `dg`-scaled fp8 window `dst_box` with the
     plan `flags`; returns (dest, dest_scale, tables, keepalive)."""
-    gshape = tuple(q_full.shape)
-    handles, keep = [], []
-    for r, (off, loc) in enumerate(src_boxes):
-        if 0 in loc:
-            continue
-        shard = region(q_full, off, loc).contiguous()
-        scale = local_scale(full_scale, sg, off, loc)
-        keep += [shard, scale]
-        buf = FakeScaledBuffer(shard, scale, sg, off[-2], off[-1])
-        handles.append(RDMAWeightHandle(rdma_buffer=buf, tensor_slice=TensorSlice(off, (r,), gshape, loc, (len(src_boxes),)),
-                                        source_rank=r))
-    off, loc = dst_box
+    handles, keep = shard_handles(q_full, src_boxes, lambda shard, off, loc: FakeScaledBuffer(
+        shard, local_scale(full_scale, sg, off, loc), sg, off[-2], off[-1]))
+    loc = dst_box[1]
     dest = torch.full(loc, 0x55, dtype=torch.uint8).view(E4M3)
     dest_scale = torch.full(dest_scale_shape(dg, loc), -1.0)
-    ops = DirectWeightSyncDest()._build_plan({"w": handles}, {"w": dest}, {"w": TensorSlice(off, (0,), gshape, loc, (1,))})
-    pairs, sources, index = [], [], {}
+    ops, pairs = plan_windows(handles, dest, dst_box)
+    sources, index = [], {}
     for op in ops:
         buf = op.rdma_buffer
-        pairs.append(DirectWeightSyncDest.op_windows(op, StridedMem.from_tensor(buf.shard)))
         if id(buf) not in index:
             index[id(buf)] = len(sources)
             n, k = buf.shard.shape[-2:]
@@ -255,13 +235,6 @@ def test_full_size_llama3_8b_compile():
 
 
 # ---- compiler errors ------------------------------------------------------------------------------
-def expect_invalid(fn):
-    with pytest.raises(_native.TsbError) as e:
-        fn()
-    assert e.value.code == _native.TSB_ERR_INVALID, e.value
-    return str(e.value)
-
-
 def test_compile_errors_name_the_target_group_rect_or_source():
     q = torch.zeros(256, 256, dtype=E4M3)
     s = torch.zeros(2, 2)
@@ -301,25 +274,7 @@ def test_compile_errors_name_the_target_group_rect_or_source():
 
 
 # ---- pull validation (before anything is compiled) --------------------------------------------------
-class Boom(Exception):
-    pass
-
-
-@pytest.fixture
-def no_compile(monkeypatch):
-    import torchstore_b200.direct_weight_sync as dws
-
-    def boom(*a, **k):
-        raise Boom("compiled")
-
-    for name in ("build", "build_dequant_fp8", "build_requant_fp8", "build_block_fp8", "build_scaled_fp8"):
-        monkeypatch.setattr(dws.Plans, name, classmethod(lambda cls, *a: boom()))
-
-
-def cuda_like(t):
-    """A CPU tensor's metadata that claims to be on CUDA (validation reads nothing else)."""
-    return types.SimpleNamespace(dtype=t.dtype, shape=t.shape, dim=t.dim, numel=t.numel, is_contiguous=t.is_contiguous,
-                                 stride=t.stride, is_cuda=True, device=t.device)
+no_compile = pytest.fixture(no_compile)
 
 
 def handles(kinds, dtype=E4M3):

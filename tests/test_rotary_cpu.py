@@ -12,7 +12,7 @@ import torch
 import workloads
 from oracle import c_oracle
 from oracle import rotary_oracle as ro
-from tests.packed_harness import HostBuffer, fsdp_handles, pull_args, window
+from tests.helpers import HostBuffer, fsdp_handles, handles_of, pull_args, region
 from tests.test_packed_cpu import ScaledHost, host_sources
 from torchstore_b200 import _native, state_dict_utils
 from torchstore_b200.direct_weight_sync import (DirectWeightSyncDest, PackedPart, _packed_key, scale_grid,
@@ -21,10 +21,6 @@ from torchstore_b200.planner import StridedMem, build_rects
 
 E4M3 = torch.float8_e4m3fn
 LLAMA = workloads.LLAMA3_8B
-
-
-def handles_of(shape, n=1, dtype=torch.bfloat16):
-    return fsdp_handles({"s": (shape, None)}, n, lambda _, off, loc: HostBuffer(None, loc, dtype))["s"]
 
 
 def check(dest_shape, packed, handles, match):
@@ -127,7 +123,7 @@ def test_field_rides_in_packed_on_get_state_dict():
 def titan_plan(rank, n, sources, layout):
     vl = workloads.vllm_tp_layout(layout, LLAMA, 8, rank, source="torchtitan")
     handles = fsdp_handles(layout, n, lambda name, off, loc: HostBuffer(
-        window(sources[name], off, loc).contiguous() if name in sources else None, loc, sources[name].dtype
+        region(sources[name], off, loc).contiguous() if name in sources else None, loc, sources[name].dtype
         if name in sources else torch.uint8))
     dests, slices, packed = pull_args(vl, 8, rank, lambda name, shape: torch.full(shape, 0x5A, dtype=torch.uint8))
     assert not slices and set(packed) == set(vl)
@@ -182,7 +178,7 @@ def test_scaled_llama_every_rank_every_name_matches_the_oracle():
     np_sources = {k: v.view(torch.int16).numpy() for k, v in sources.items()}
     for rank in range(2):
         vl = workloads.vllm_tp_layout(layout, LLAMA, 2, rank, source="torchtitan")
-        handles = fsdp_handles(layout, 3, lambda name, off, loc: HostBuffer(window(sources[name], off, loc).contiguous(),
+        handles = fsdp_handles(layout, 3, lambda name, off, loc: HostBuffer(region(sources[name], off, loc).contiguous(),
                                                                             loc, torch.bfloat16))
         dests = {k: torch.full(e[0], -3, dtype=torch.int16).view(torch.bfloat16) for k, e in vl.items()}
         packed = {k: e[1] for k, e in vl.items()}
@@ -200,7 +196,7 @@ def rotary_scaled(g, hd, rows, n):
 
     def make(_, off, loc):
         scale = torch.from_numpy(rng.standard_normal(source_scale_shapes(g, loc, off[-2], off[-1])[0]).astype(np.float32))
-        return ScaledHost(window(full, off, loc).contiguous(), scale, g, off[-2], off[-1])
+        return ScaledHost(region(full, off, loc).contiguous(), scale, g, off[-2], off[-1])
     return fsdp_handles({"q": ((rows, 256), None)}, n, make)
 
 

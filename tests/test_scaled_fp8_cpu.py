@@ -12,10 +12,9 @@ import pytest
 import torch
 
 from oracle.scaled_fp8_oracle import GRANULARITIES, bits_of, digest, fixture_inputs, quantize, replay, torch_quantize, widen
+from tests.helpers import HostBuffer, expect_invalid, plan_windows, rand_full, region, shard_box, shard_handles
 from torchstore_b200 import _native
-from torchstore_b200.direct_weight_sync import DirectWeightSyncDest, RDMAWeightHandle
 from torchstore_b200.planner import StridedMem, build_rects
-from torchstore_b200.transport.types import TensorSlice
 
 GOLDEN = os.path.join(os.path.dirname(__file__), "golden", "scaled_fp8_vectors.npz")
 E4M3 = torch.float8_e4m3fn
@@ -107,18 +106,6 @@ def test_torch_rendering_matches_the_oracle_on_finite_data(case):
 
 
 # ---- the plan compiler, replayed on host memory ----------------------------------------------------
-def shard_box(shape, n, r, dim):
-    off, loc = [0] * len(shape), list(shape)
-    chunk = -(-shape[dim] // n)
-    start, stop = min(shape[dim], chunk * r), min(shape[dim], chunk * (r + 1))
-    off[dim], loc[dim] = start, max(0, stop - start)
-    return tuple(off), tuple(loc)
-
-
-def region(t, off, loc):
-    return t[tuple(slice(o, o + s) for o, s in zip(off, loc))]
-
-
 def scale_shape(loc, g):
     *lead, n, _ = loc
     return (*lead, n, 1) if g == "channel" else tuple(lead)
@@ -127,21 +114,12 @@ def scale_shape(loc, g):
 def compile_pull(full, src_boxes, dst_box, g):
     """Plan (product planner, host memory) a pull of `full`'s `src_boxes` shards into the fp8
     destination `dst_box`; returns (dest, scale, (bands, pieces, tiles, n_groups), keepalive)."""
-    gshape = tuple(full.shape)
-    handles, keep = [], []
-    for r, (off, loc) in enumerate(src_boxes):
-        if 0 in loc:
-            continue
-        shard = region(full, off, loc).contiguous()
-        keep.append(shard)
-        handles.append(RDMAWeightHandle(rdma_buffer=shard, tensor_slice=TensorSlice(off, (r,), gshape, loc, (len(src_boxes),)),
-                                        source_rank=r))
-    off, loc = dst_box
+    handles, keep = shard_handles(full, src_boxes, lambda shard, off, loc: HostBuffer(shard, loc, shard.dtype))
+    loc = dst_box[1]
     dest = torch.zeros(loc, dtype=E4M3)
     n, k = loc[-2:]
     scale = torch.zeros(scale_shape(loc, g), dtype=torch.float32)
-    ops = DirectWeightSyncDest()._build_plan({"w": handles}, {"w": dest}, {"w": TensorSlice(off, (0,), gshape, loc, (1,))})
-    pairs = [DirectWeightSyncDest.op_windows(op, StridedMem.from_tensor(op.rdma_buffer)) for op in ops]
+    _, pairs = plan_windows(handles, dest, dst_box)
     rects, nr = build_rects(pairs)
     targets = _native.make_sq_target_array(1)
     targets[0] = _native.SqTarget(dest.data_ptr(), scale.data_ptr(), dest.numel() // (n * k), n, k, CODE[g], 0)
@@ -180,11 +158,6 @@ def run_reshard(full, src_boxes, dst_box, g):
     assert np.array_equal(dest.view(torch.uint8).numpy(), want_q)
     assert np.array_equal(scale.numpy().view(np.uint32), want_s.view(np.uint32))
     return tables
-
-
-def rand_full(shape, dtype, seed):
-    g = torch.Generator().manual_seed(seed)
-    return (torch.randn(shape, generator=g) * 2.0 ** torch.randint(-6, 6, shape, generator=g).float()).to(dtype)
 
 
 @pytest.mark.parametrize("g", GRANULARITIES)
@@ -258,13 +231,6 @@ def test_random_reshards():
             dst = shard_box(shape, n_dst, d, dd)
             if 0 not in dst[1]:
                 run_reshard(full, srcs, dst, GRANULARITIES[i % 2])
-
-
-def expect_invalid(fn):
-    with pytest.raises(_native.TsbError) as e:
-        fn()
-    assert e.value.code == _native.TSB_ERR_INVALID, e.value
-    return str(e.value)
 
 
 @pytest.mark.parametrize("g", GRANULARITIES)

@@ -12,12 +12,13 @@ import torch
 
 from oracle import dequant_fp8_oracle, requant_fp8_oracle
 from oracle.source_quant_oracle import GRANULARITIES, bits_of, element_scales, quantize, replay, synth_f32, widen
+from tests.helpers import plan_windows, region, shard_box
 from tests.source_quant_regimes import REGIMES, WORKLOADS, plan_bytes
-from tests.test_requant_fp8_cpu import CODE, FakeScaledBuffer, dest_scale_shape, region, shard_box
+from tests.test_requant_fp8_cpu import CODE, FakeScaledBuffer, dest_scale_shape
 from tests.test_source_quant_cpu import compile_host, host_shard
 from torchstore_b200 import _native
-from torchstore_b200.direct_weight_sync import DirectWeightSyncDest, RDMAWeightHandle
-from torchstore_b200.planner import StridedMem, build_rects
+from torchstore_b200.direct_weight_sync import RDMAWeightHandle
+from torchstore_b200.planner import build_rects
 from torchstore_b200.transport.types import TensorSlice
 
 E4M3 = torch.float8_e4m3fn
@@ -185,15 +186,14 @@ def compile_consumer(shape, shards, g, consumer, window):
         buf = FakeScaledBuffer(shard, scale, g, off[-2], off[-1])
         handles.append(RDMAWeightHandle(rdma_buffer=buf, tensor_slice=TensorSlice(off, (r,), shape, loc, (len(shards),)),
                                         source_rank=r))
-    off, loc = window
+    loc = window[1]
     requant = consumer in GRANULARITIES
     dest = torch.full(loc, 0x55, dtype=torch.uint8).view(E4M3) if requant else torch.zeros(loc, dtype=getattr(torch, consumer))
     dest_scale = torch.full(dest_scale_shape(consumer, loc), -1.0) if requant else None
-    ops = DirectWeightSyncDest()._build_plan({"w": handles}, {"w": dest}, {"w": TensorSlice(off, (0,), shape, loc, (1,))})
-    pairs, sources, index = [], [], {}
+    ops, pairs = plan_windows(handles, dest, window)
+    sources, index = [], {}
     for op in ops:
         buf = op.rdma_buffer
-        pairs.append(DirectWeightSyncDest.op_windows(op, StridedMem.from_tensor(buf.shard)))
         if id(buf) not in index:
             index[id(buf)] = len(sources)
             n, k = buf.shard.shape[-2:]

@@ -11,7 +11,7 @@ import torch
 
 import workloads
 from oracle import packed_oracle, transpose_oracle as to
-from tests.packed_harness import HostBuffer, fsdp_handles, window
+from tests.helpers import HostBuffer, fsdp_handles, handles_of
 from tests.test_packed_cpu import ScaledHost
 from torchstore_b200 import _native, state_dict_utils
 from torchstore_b200.direct_weight_sync import DirectWeightSyncDest, PackedPart, RDMAWeightHandle, _packed_key
@@ -20,16 +20,6 @@ from torchstore_b200.transport.types import TensorSlice
 
 QWEN = workloads.QWEN3_MOE
 WHAT = r"packed destination 'fused' part 0 \(source 'a'\)"
-
-
-def handles_of(shape, n=1, dtype=torch.bfloat16, dim=0, sources=None):
-    """FSDP(n) handles of one tensor ``a`` cut along ``dim`` (torch.chunk-style, uneven when n does not divide it)."""
-    out = []
-    for r in range(n):
-        off, loc = workloads.shard_box(shape, n, r, ("S", dim)) if n > 1 else ((0,) * len(shape), tuple(shape))
-        shard = None if sources is None else window(sources, off, loc).contiguous()
-        out.append(RDMAWeightHandle(HostBuffer(shard, loc, dtype), TensorSlice(off, (r,), tuple(shape), loc, (n,)), r))
-    return {"a": out}
 
 
 def check(dest_shape, packed, handles, match):
@@ -75,41 +65,40 @@ def test_oracle_matches_torch_transpose(seed):
 @pytest.mark.parametrize("flag", [1, 0, "yes", None])
 def test_transpose_must_be_a_bool(flag):
     check((4, 8), {"fused": (PackedPart("a", (slice(0, 4), slice(0, 8)), (0, 0), transpose=flag),)},
-          handles_of((8, 4)), WHAT + r": transpose must be a bool")
+          {"a": handles_of((8, 4))}, WHAT + r": transpose must be a bool")
 
 
 def test_source_needs_two_dims():
-    check((4, 8), T((0, slice(0, 8)), (0,)), handles_of((8,)), WHAT + r": transpose swaps the source's last two dims, "
-                                                                      "and the source has 1 dim")
+    check((4, 8), T((0, slice(0, 8)), (0,)), {"a": handles_of((8,))},
+          WHAT + r": transpose swaps the source's last two dims, and the source has 1 dim")
 
 
 def test_not_with_rotary():
-    check((4, 8), T((slice(0, 4), slice(0, 8)), (0, 0), rotary_head_dim=4), handles_of((8, 4)),
+    check((4, 8), T((slice(0, 4), slice(0, 8)), (0, 0), rotary_head_dim=4), {"a": handles_of((8, 4))},
           WHAT + r": transpose and rotary_head_dim do not combine")
 
 
 @pytest.mark.parametrize("index", [(slice(0, 2), 1, slice(0, 4)), (slice(0, 2), slice(0, 4), 3)])
 def test_int_index_must_not_drop_the_swapped_dims(index):
-    check((2, 4, 4), T(index, (0, 0)), handles_of((2, 4)), WHAT + r": its int index drops one of the destination's "
-                                                                  "last two dims")
+    check((2, 4, 4), T(index, (0, 0)), {"a": handles_of((2, 4))},
+          WHAT + r": its int index drops one of the destination's last two dims")
 
 
 def test_swapped_box_outside_the_source():
     # box (4, 6) reads a (6, 4) source box: at (0, 0) of an (8, 4) source it fits, at (3, 0) it leaves it
-    check((4, 6), T((slice(0, 4), slice(0, 6)), (3, 0)), handles_of((8, 4)),
+    check((4, 6), T((slice(0, 4), slice(0, 6)), (3, 0)), {"a": handles_of((8, 4))},
           WHAT + r": the source box at \(3, 0\) with extent \(6, 4\) leaves the source's global shape \(8, 4\)")
-    DirectWeightSyncDest._check_packed(handles_of((8, 4)), {"fused": torch.zeros(4, 6)},
+    DirectWeightSyncDest._check_packed({"a": handles_of((8, 4))}, {"fused": torch.zeros(4, 6)},
                                        T((slice(0, 4), slice(0, 6)), (2, 0)))
 
 
 def test_hole_names_the_source_element():
-    hs = handles_of((8, 4), n=2)
-    hs["a"] = hs["a"][:1]  # rows 0..4 only
+    hs = {"a": handles_of((8, 4), n=2)[:1]}  # rows 0..4 only
     check((4, 6), T((slice(0, 4), slice(0, 6)), (0, 0)), hs, WHAT + r": no handle covers global element \(4, 0\)")
 
 
 def test_routes_refuse_scaled_destinations_and_scaled_handles():
-    hs = handles_of((8, 4))
+    hs = {"a": handles_of((8, 4))}
     dests = {"fused": torch.zeros(4, 8, dtype=torch.bfloat16)}
     parts = DirectWeightSyncDest._check_packed(hs, dests, T((slice(0, 4), slice(0, 8)), (0, 0)))
     for kw in ("block_scales", "channel_scales", "tensor_scales"):
@@ -131,7 +120,7 @@ def test_plan_key_tells_transpose_apart():
 
 
 def test_field_rides_in_packed_on_get_state_dict():
-    hs = handles_of((8, 4), n=2)["a"]
+    hs = handles_of((8, 4), n=2)
 
     class Store:
         async def get(self, key):
@@ -169,7 +158,7 @@ def test_ops_fill_what_the_oracle_says(n, dim):
     transposed box (int index on dim 1), an untransposed one and a transposed one at odd offsets."""
     g = torch.Generator().manual_seed(n * 10 + dim)
     full = torch.randint(-2 ** 15, 2 ** 15, (7, 11, 13), generator=g, dtype=torch.int16)
-    hs = handles_of((7, 11, 13), n, torch.int16, dim, full)
+    hs = {"a": handles_of((7, 11, 13), n, torch.int16, dim, full)}
     parts = (PackedPart("a", (slice(0, 3), 0, slice(0, 10), slice(0, 9)), (1, 1, 2), transpose=True),
              PackedPart("a", (slice(0, 3), 1, slice(0, 10), slice(0, 9)), (4, 1, 2)),
              PackedPart("a", (slice(0, 3), 1, slice(0, 10), slice(0, 1)), (2, 10, 3), transpose=True))

@@ -14,6 +14,7 @@ import torch
 from oracle.ue8m0_oracle import (GRANULARITIES, bits_of, digest, edge_amaxes, fixture_inputs, log2_scale_inv, quantize,
                                  replay_block, replay_requant, replay_scaled, replay_source, requantize, scales_of_amax,
                                  synth_f32, torch_quantize, torch_scales_of_amax, widen)
+from tests.helpers import Boom, expect_invalid, no_export
 from torchstore_b200 import _native
 from torchstore_b200.direct_weight_sync import DirectWeightSyncDest, DirectWeightSyncSource
 from torchstore_b200.planner import StridedMem, build_rects
@@ -253,18 +254,12 @@ def test_quantising_kinds_accept_the_flag_with_identical_tables():
         same_tables(compile_(0), compile_(UE8M0))
 
 
-def expect_invalid(fn, needle="flags must be"):
-    with pytest.raises(_native.TsbError, match=needle) as e:
-        fn()
-    assert e.value.code == _native.TSB_ERR_INVALID
-
-
 def test_unknown_bits_and_the_dequantising_kind_are_refused():
     for bad in (2, 1 << 31, UE8M0 | 4):
-        expect_invalid(lambda: block_case(bad))
-        expect_invalid(lambda: scaled_case("channel", 260, bad))
-        expect_invalid(lambda: source_case("block", bad))
-        expect_invalid(lambda: requant_case("block", bad))
+        expect_invalid(lambda: block_case(bad), "flags must be")
+        expect_invalid(lambda: scaled_case("channel", 260, bad), "flags must be")
+        expect_invalid(lambda: source_case("block", bad), "flags must be")
+        expect_invalid(lambda: requant_case("block", bad), "flags must be")
     q = torch.zeros(8, 16, dtype=E4M3)
     s = torch.ones(8, 1)
     y = torch.zeros(8, 16)
@@ -273,10 +268,10 @@ def test_unknown_bits_and_the_dequantising_kind_are_refused():
     src[0] = _native.DqSource(q.data_ptr(), s.data_ptr(), 1, 8, 16, 0, 0, _native.TSB_SCALE_PER_CHANNEL, 0)
     assert len(_native.dequant_fp8_compile_host(0, rects, n, src, 1)) == 1
     for bad in (UE8M0, 2):
-        expect_invalid(lambda: _native.dequant_fp8_compile_host(0, rects, n, src, 1, bad))
+        expect_invalid(lambda: _native.dequant_fp8_compile_host(0, rects, n, src, 1, bad), "flags must be")
         # plan creation checks the flags before it touches a device
-        expect_invalid(lambda: _native.dequant_fp8_plan_create(0, rects, n, [src[0]], flags=bad))
-    expect_invalid(lambda: _native.block_fp8_plan_create(0, rects, n, [], flags=2))
+        expect_invalid(lambda: _native.dequant_fp8_plan_create(0, rects, n, [src[0]], flags=bad), "flags must be")
+    expect_invalid(lambda: _native.block_fp8_plan_create(0, rects, n, [], flags=2), "flags must be")
 
 
 def test_replayed_block_and_scaled_tables_match_the_formula():
@@ -321,24 +316,11 @@ def test_requantising_power_of_two_groups_onto_themselves_is_lossless():
 
 
 # ---- Python validation, before any device work -------------------------------------------------------------------
-class Boom(Exception):
-    pass
-
-
-@pytest.fixture
-def nothing_compiled(monkeypatch):
-    from torchstore_b200 import direct_weight_sync as dws
-
-    def boom(*a, **k):
-        raise Boom("exported or compiled before validation finished")
-
-    monkeypatch.setattr(dws.HbmDescriptor, "from_tensor", staticmethod(boom))
-    for name in ("build", "build_source_quant", "build_dequant_fp8", "build_requant_fp8", "build_block_fp8", "build_scaled_fp8"):
-        monkeypatch.setattr(dws.Plans, name, classmethod(boom))
+no_export = pytest.fixture(no_export)
 
 
 @pytest.mark.parametrize("fmt", ["e8m0", "UE8M0", "", 1, "float32"])
-def test_unknown_scale_fmt_is_refused(nothing_compiled, fmt):
+def test_unknown_scale_fmt_is_refused(no_export, fmt):
     dest = DirectWeightSyncDest()
     with pytest.raises(ValueError, match="scale_fmt must be None or 'ue8m0'"):
         asyncio.run(dest.pull({}, {}, block_scales={"w": torch.zeros(1, 1)}, scale_fmt=fmt))
@@ -348,7 +330,7 @@ def test_unknown_scale_fmt_is_refused(nothing_compiled, fmt):
     assert dest._plan is None and src._handles == {} and not src._quant_plans
 
 
-def test_scale_fmt_without_scaled_names_is_refused(nothing_compiled):
+def test_scale_fmt_without_scaled_names_is_refused(no_export):
     with pytest.raises(ValueError, match="must name at least one"):
         asyncio.run(DirectWeightSyncDest().pull({}, {"w": torch.zeros(4, 4)}, scale_fmt="ue8m0"))
     with pytest.raises(ValueError, match="must name at least one"):
@@ -361,7 +343,7 @@ def test_scale_fmt_without_scaled_names_is_refused(nothing_compiled):
     assert src._handles == {}
 
 
-def test_scale_fmt_is_validated_before_the_quantize_dict(nothing_compiled):
+def test_scale_fmt_is_validated_before_the_quantize_dict(no_export):
     with pytest.raises(ValueError, match="scale_fmt must be"):
         DirectWeightSyncSource().register({"w": torch.zeros(4, 4)}, rank=0, quantize={"nope": "block"}, scale_fmt="x")
 

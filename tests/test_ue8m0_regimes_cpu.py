@@ -21,7 +21,7 @@ from oracle.dequant_fp8_oracle import decode_e4m3, expand
 from tests import fp8_regimes, quant_pull_regimes, source_quant_regimes
 from tests import test_fp8_regimes_cpu as fp8_cpu
 from tests import test_requant_fp8_cpu as rq_cpu
-from tests.test_block_fp8_cpu import region
+from tests.helpers import region
 from tests.test_quant_pull_regimes_cpu import compiled
 from tests.test_source_quant_cpu import compile_host, host_shard
 from tests.test_source_quant_regimes_cpu import workload_inputs as source_inputs
@@ -157,7 +157,7 @@ def test_requant_workload_replays_to_the_ue8m0_oracle(name):
     w = fp8_regimes.WORKLOADS[name]
     q, s, dest, dest_scale, _, _ = requant_catalogue(name)
     off, loc = w.dst
-    args = (rq_cpu.region(q, off, loc), rq_cpu.local_scale(s, w.sg, off, loc), w.sg, off[-2], off[-1], w.out)
+    args = (region(q, off, loc), rq_cpu.local_scale(s, w.sg, off, loc), w.sg, off[-2], off[-1], w.out)
     want_q, want_s = u8.requantize(args[0].view(torch.uint8).numpy(), args[1].numpy(), *args[2:], scale_fmt="ue8m0")
     got_q, got_s = dest.view(torch.uint8).numpy(), dest_scale.numpy()
     assert np.array_equal(got_q, want_q), w.describe()
@@ -195,7 +195,7 @@ def test_lossless_workloads_are_decided_by_geometry():
 
 def assert_lossless(q, s, sg, y, ys, dg, off, loc):
     """f32(q') * s' == f32(q) * s element for element over the window, and s' <= s group by group."""
-    qw = rq_cpu.region(q, off, loc).view(torch.uint8).numpy()
+    qw = region(q, off, loc).view(torch.uint8).numpy()
     sw = rq_cpu.local_scale(s, sg, off, loc).numpy()
     before = decode_e4m3(qw) * expand(sw, loc, sg, off[-2], off[-1])
     after = decode_e4m3(y) * expand(np.asarray(ys, np.float32).reshape(rq_cpu.dest_scale_shape(dg, loc)), loc, dg)

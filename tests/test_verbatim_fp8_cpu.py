@@ -14,6 +14,7 @@ import torch
 
 from oracle import reshard_oracle as ro
 from oracle.verbatim_fp8_oracle import verbatim
+from tests.helpers import Boom, cuda_like, no_export
 from torchstore_b200.direct_weight_sync import (DirectWeightSyncDest, RDMAWeightHandle, scale_grid, source_scale_shapes,
                                                 verbatim_scale_rects)
 from torchstore_b200.transport.types import TensorSlice
@@ -253,26 +254,7 @@ def test_random_layouts(seed):
 
 
 # ---- pull validation (before anything is compiled) --------------------------------------------------
-class Boom(Exception):
-    pass
-
-
-@pytest.fixture
-def no_compile(monkeypatch):
-    import torchstore_b200.direct_weight_sync as dws
-
-    def boom(*a, **k):
-        raise Boom("exported or compiled")
-
-    monkeypatch.setattr(dws.HbmDescriptor, "from_tensor", staticmethod(boom))
-    for name in ("build", "build_dequant_fp8", "build_requant_fp8", "build_block_fp8", "build_scaled_fp8"):
-        monkeypatch.setattr(dws.Plans, name, classmethod(boom))
-
-
-def cuda_like(t):
-    """A CPU tensor's metadata that claims to be on CUDA (validation reads nothing else)."""
-    return types.SimpleNamespace(dtype=t.dtype, shape=t.shape, dim=t.dim, numel=t.numel, is_contiguous=t.is_contiguous,
-                                 stride=t.stride, is_cuda=True, device=t.device)
+no_export = pytest.fixture(no_export)
 
 
 def handles(kinds, dtype=E4M3):
@@ -280,7 +262,7 @@ def handles(kinds, dtype=E4M3):
                              tensor_slice=TensorSlice((0, 0), (r,), (8, 8), (8, 8), (2,))) for r, k in enumerate(kinds)]
 
 
-def test_route_decision(no_compile):
+def test_route_decision(no_export):
     check = DirectWeightSyncDest._check_scales
     dest = {"w": cuda_like(torch.zeros(8, 8, dtype=E4M3))}
     bs = {"block_scales": {"w": torch.zeros(1, 1)}}
@@ -303,7 +285,7 @@ def test_route_decision(no_compile):
         check({"w": handles(["block"])}, dest, bs)
 
 
-def test_pull_errors_raise_before_compile(no_compile):
+def test_pull_errors_raise_before_compile(no_export):
     dest = {"w": cuda_like(torch.zeros(8, 8, dtype=E4M3))}
     cs = {"w": torch.zeros(8, 1)}
     with pytest.raises(ValueError, match="exclusive"):
