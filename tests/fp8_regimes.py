@@ -4,8 +4,8 @@ Every regime is a predicate over the record arrays ``_native.requant_fp8_compile
 tiles, n_groups) or ``_native.dequant_fp8_compile_host`` (tiles) return, plus the destination's geometry,
 and names the workload that reaches it.  A workload is one pull: a global fp8 tensor cut into source
 shards of one scale granularity, and one destination window.  The CPU suite compiles every workload on
-host memory and replays it against the oracles; the H100 suite runs it through ``DirectWeightSyncDest.pull``
-and asserts the regime again from the tables of the live plan's inputs.
+host memory and replays it against the oracles; the H100 suites run it through ``DirectWeightSyncDest.pull``
+(``run_regime``) and assert the regime again from the tables of the live plan's inputs.
 
 Branches (csrc/requant_fp8.cu, csrc/dequant_fp8.cu):
   staged units      block targets (one group per 128x128 block) and per-channel bands of rows of at most
@@ -22,13 +22,25 @@ Branches (csrc/requant_fp8.cu, csrc/dequant_fp8.cu):
 
 from __future__ import annotations
 
+import random
 from dataclasses import dataclass
+from functools import partial
 from typing import Callable
 
 import numpy as np
+import torch
 
-from tests.helpers import shard_box
+from oracle import int8_source_oracle, ue8m0_oracle
+from oracle.dequant_fp8_oracle import DST, GRANULARITIES, dequantize, torch_dequantize
+from oracle.requant_fp8_oracle import SCALE_POISON, requantize, torch_requantize
+from tests.helpers import (DEV, E4M3, assert_same_bits_or_nan, cleanup, guards_intact, named, pull_box, region,
+                           register_boxes, shard_box)
+from tests.test_dequant_fp8_cpu import local_scale as dq_local_scale
+from tests.test_dequant_fp8_cpu import torch_bits
+from tests.test_requant_fp8_cpu import CODE, fp8_full, global_scale, local_scale
 from torchstore_b200 import _native
+from torchstore_b200.direct_weight_sync import DirectWeightSyncDest, _add_dq_source
+from torchstore_b200.planner import build_rects
 
 STAGE_BYTES, TILE_ELEMS, BAND_ROWS, DQ_TILE_ROWS = 32768, 16384, 256, 256
 ES = {"bfloat16": 2, "float16": 2, "float32": 4}
@@ -245,3 +257,189 @@ REGIMES: dict[str, Regime] = {
     "dq_vec_tile_ragged_cols": Regime("dq_wide_rows", _dq_tile(lambda t, g: t["vec"] == 1 and t["cols"] % 16 != 0),
                                       "16-byte tile whose last chunk is partial"),
 }
+
+
+# ---- on the H100 ---------------------------------------------------------------------------------
+def want_bits(q_full, full_scale, g, box, dtype):
+    """The numpy oracle's bits of the `box` of `q_full` dequantised into `dtype`."""
+    dst = str(dtype).replace("torch.", "")
+    return dequantize(region(q_full, *box).view(torch.uint8).numpy(), dq_local_scale(full_scale, g, *box).numpy(), g,
+                      box[0][-2], box[0][-1], dst)
+
+
+def assert_dequant_oracle(y, want):
+    """A dequantised destination y bit for bit the oracle's bits `want` wherever y is not NaN."""
+    got = torch_bits(y.cpu())
+    nan = torch.isnan(y.float()).cpu().numpy()
+    assert np.array_equal(got[~nan], want[~nan])
+
+
+def assert_dequant_torch_cuda(y, q_full, full_scale, g, box):
+    """Bit-exact, NaN bytes included, against the torch CUDA rendering of the same region."""
+    want = torch_dequantize(region(q_full, *box).to(DEV), dq_local_scale(full_scale, g, *box).to(DEV), g, box[0][-2],
+                            box[0][-1], y.dtype)
+    assert torch.equal(y.view(torch.uint8), want.view(torch.uint8))
+
+
+def assert_requant_torch_cuda(q, s, q_full, full_scale, sg, box, dg, scale_fmt=None):
+    """A requantised destination (q, s) bit-exact, NaN bytes included, against the torch CUDA composition of the
+    same window."""
+    args = (region(q_full, *box).to(DEV), local_scale(full_scale, sg, *box).to(DEV), sg, box[0][-2], box[0][-1], dg)
+    want_q, want_s = ue8m0_oracle.torch_requantize(*args, scale_fmt=scale_fmt) if scale_fmt else torch_requantize(*args)
+    if scale_fmt:
+        ue8m0_oracle.assert_pow2_over(s, torch_requantize(*args)[1])
+    assert torch.equal(q.view(torch.uint8), want_q.view(torch.uint8))
+    assert_same_bits_or_nan(s.reshape(-1), want_s.reshape(-1))  # a NaN scale_inv's bits are torch's choice
+
+
+def assert_requant_oracle(q, s, q_full, full_scale, sg, box, dg, scale_fmt=None):
+    """A requantised destination (q, s) bit-exact against the numpy composition wherever it is not NaN."""
+    args = (region(q_full, *box).view(torch.uint8).numpy(), local_scale(full_scale, sg, *box).numpy(), sg, box[0][-2],
+            box[0][-1], dg)
+    want_q, want_s = ue8m0_oracle.requantize(*args, scale_fmt=scale_fmt) if scale_fmt else requantize(*args)
+    got_q = q.view(torch.uint8).cpu().numpy()
+    nan = (want_q & 0x7F) == 0x7F
+    assert np.array_equal(got_q[~nan], want_q[~nan])
+    got_s, want_s = s.cpu().numpy().reshape(-1), np.asarray(want_s, np.float32).reshape(-1)
+    ok = ~np.isnan(want_s)
+    assert np.array_equal(got_s[ok].view(np.uint32), want_s[ok].view(np.uint32))
+
+
+def live_tables(sync, dest, dest_scale=None, dg=None, int8_src=False):
+    """Compile on the host the tables of the plan `sync` built for its one name: the same windows, sources and
+    target it compiled from, with the live device addresses (`int8_src`: a dequantising plan of int8 handles, TSB_I8
+    rects).  Checks their size against plan_info and returns (tables, Geometry)."""
+    dev = dest.device.index
+    pairs, sources = [], {}
+    for op in sync._plan:
+        pairs.append(DirectWeightSyncDest.op_windows(op, op.rdma_buffer.window(dev)))
+        _add_dq_source(sources, op, dev)
+    arr = _native.make_dq_source_array(max(1, len(sources)))
+    for i, (_, s) in enumerate(sources.values()):
+        arr[i] = s
+    rects, n = build_rects(pairs, dequantise=int8_src)
+    *lead, rows, cols = dest.shape
+    if dg is None:
+        tables = _native.dequant_fp8_compile_host(dev, rects, n, arr, len(sources))
+        mine, other = (sync._int8_dequant_plans, sync._dequant_plans) if int8_src else (sync._dequant_plans, sync._int8_dequant_plans)
+        assert not other, "dequantising plans of the other source format"
+        info = _native.plan_info(mine[dev])
+        count, read = len(tables), int((tables["rows"].astype(np.int64) * tables["cols"]).sum())
+    else:
+        for i in range(n):
+            rects[i].src_dtype = rects[i].dst_dtype = _native.TSB_F8E4M3
+        tgt = _native.make_sq_target_array(1)
+        tgt[0] = _native.SqTarget(dest.data_ptr(), dest_scale.data_ptr(), dest.numel() // (rows * cols), rows, cols, CODE[dg], 0)
+        tables = _native.requant_fp8_compile_host(dev, rects, n, arr, len(sources), tgt, 1)
+        units, pieces, tiles, _ = tables
+        info = _native.plan_info(sync._requant_plans[dev])
+        count = len(units) + len(tiles)
+        read = int((pieces["rows"].astype(np.int64) * pieces["cols"]).sum() + (tiles["rows"].astype(np.int64) * tiles["cols"]).sum())
+    assert (info.num_tiles, info.src_bytes) == (count, read)
+    return tables, geometry(dest.data_ptr(), tuple(dest.shape), dest.element_size(), arr, len(sources))
+
+
+POISON = (float(SCALE_POISON[0]), float(SCALE_POISON[1]), 0.0, -0.5)  # Inf, NaN, 0, negative
+
+
+def poison(s, seed):
+    """Inf, NaN, 0 and -0.5 at four spread entries of a source scale (one of them if it has one entry)."""
+    flat = s.reshape(-1)
+    n = flat.numel()
+    for k, i in enumerate(sorted({0, n // 3, 2 * n // 3, n - 1})):
+        flat[i] = POISON[(k + seed) % len(POISON)]
+    return s
+
+
+def zero_first_group(q, w: Workload):
+    """All-zero bytes over the first destination group of `w` (dequantising pulls: its first row)."""
+    off, loc = w.dst
+    *lead, n, k = loc
+    h, kk = {"block": (min(128, n), min(128, k)), "channel": (1, k), "tensor": (n, k)}.get(w.out, (1, k))
+    q.view(torch.uint8)[tuple(off[:-2]) + (slice(off[-2], off[-2] + h), slice(off[-1], off[-1] + kk))] = 0
+    return q
+
+
+def inputs(w: Workload, variant: str, src_dtype=E4M3):
+    """The source weight (fp8 bytes, or int8 ones from int8_of) and its global scale of workload `w` in `variant`."""
+    q = int8_source_oracle.int8_of(w.shape, w.seed) if src_dtype == torch.int8 else fp8_full(w.shape, w.seed)
+    s = global_scale(w.sg, w.shape, w.seed)
+    if variant == "poisoned_scale":
+        s = poison(s, w.seed)
+    elif variant == "zero_group":
+        q = zero_first_group(q, w)
+    return q, s
+
+
+VARIANTS = ("finite", "poisoned_scale", "zero_group")
+
+
+def run_regime(regime, variant, scale_fmt=None, src_dtype=E4M3):
+    """Pull the regime's workload in `variant` (requantising ones with the scale format `scale_fmt`; dequantising
+    ones from handles of `src_dtype`, float8_e4m3fn or int8) and check it."""
+    r = REGIMES[regime]
+    w = WORKLOADS[r.workload]
+    int8 = src_dtype == torch.int8
+    assert not (int8 and w.kind == "requant"), "int8 handles are not requantised"
+    q, s = inputs(w, variant, src_dtype)
+    sources, handles = register_boxes(q, list(w.src), granularity=w.sg, scale_of=partial(dq_local_scale, s, w.sg))
+    where = f"{regime} ({r.doc}), {variant}, scale_fmt={scale_fmt}, {src_dtype}: {w.describe()}"
+    if w.kind == "requant":
+        sync, y, ys, bases = pull_box(handles, w.shape, w.dst, E4M3, granularity=w.out, requantize=True,
+                                      scale_fmt=scale_fmt)
+        tables, geom = live_tables(sync, y, ys, w.out)
+        assert r.holds(tables, geom), f"not reached: {where}"
+        with named(where):
+            assert_requant_oracle(y, ys, q, s, w.sg, w.dst, w.out, scale_fmt)
+            assert_requant_torch_cuda(y, ys, q, s, w.sg, w.dst, w.out, scale_fmt)
+    else:
+        sync, y, _, bases = pull_box(handles, w.shape, w.dst, DST[w.out])
+        tables, geom = live_tables(sync, y, int8_src=int8)
+        assert r.holds(tables, geom), f"not reached: {where}"
+        with named(where):
+            if int8:
+                assert_int8_dequantised(y, q, s, w.sg, w.dst)
+            else:
+                assert_dequant_oracle(y, want_bits(q, s, w.sg, w.dst, DST[w.out]))
+                assert_dequant_torch_cuda(y, q, s, w.sg, w.dst)
+    assert all(guards_intact(b) for b in bases), where
+    sync.close()
+    cleanup(sources)
+
+
+def assert_int8_dequantised(y, q, s, g, box):
+    """A destination y dequantised from the `box` of int8 handles (q, global scale s): bit for bit the numpy oracle
+    (NaN-agnostic) and the torch CUDA rendering (NaN bytes included)."""
+    off, loc = box
+    qr, sr = region(q, off, loc), local_scale(s, g, off, loc)
+    assert_dequant_oracle(y, int8_source_oracle.dequantize(qr.numpy(), sr.numpy(), g, off[-2], off[-1], str(y.dtype)[6:]))
+    want = int8_source_oracle.torch_dequantize(qr.to(DEV), sr.to(DEV), g, off[-2], off[-1], y.dtype)
+    assert torch.equal(y.view(torch.uint8), want.view(torch.uint8))
+
+
+WIDTHS = (16, 48, 64, 100, 128, 130, 260, 16384, 16400, 32768, 32784)
+SRC_DTYPES = (torch.bfloat16, torch.float16, torch.float32)
+
+
+def draw(rng: random.Random, kind: str, seed: int) -> Workload:
+    """One random pull of `kind` ("quant", "dequant" or "requant")."""
+    k = rng.choice(WIDTHS)
+    n = rng.randint(1, max(1, min(400, 300_000 // k)))
+    shape = (rng.randint(2, 4), n, k) if rng.random() < 0.3 else (n, k)
+    layout = rng.choice(["rows", "cols", "replica"] + (["ep"] * (len(shape) == 3)))
+    if layout == "rows":
+        src = split(shape, rng.randint(2, 6), -2)
+    elif layout == "cols":
+        src = split(shape, rng.randint(2, 4), -1)
+    elif layout == "replica":
+        src = split(shape, 2, -2) * 2
+    else:
+        src = split(shape, shape[0], 0)
+    src = tuple(b for b in src if 0 not in b[1])
+    tp = rng.choice(["whole", "rows", "cols"])
+    dst = whole(shape) if tp == "whole" else shard_box(shape, 2, rng.randint(0, 1), len(shape) - (2 if tp == "rows" else 1))
+    if 0 in dst[1]:
+        dst = whole(shape)
+    sg = rng.choice(SRC_DTYPES) if kind == "quant" else rng.choice(GRANULARITIES)
+    out = rng.choice(list(DST)) if kind == "dequant" else rng.choice(GRANULARITIES)
+    return Workload(kind, shape, str(sg).replace("torch.", ""), src, dst, out, seed)

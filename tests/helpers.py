@@ -1,9 +1,12 @@
 """Shared helpers for the test-suite: seeded random rectangle workloads that can be materialised on
-the CPU (for the C oracle) and on CUDA (for the product), Llama-3 layouts, and the host-memory stand-ins,
-shards, handles and plans of the pull suites that run without a GPU."""
+the CPU (for the C oracle) and on CUDA (for the product), Llama-3 layouts, the host-memory stand-ins,
+shards, handles and plans of the pull suites that run without a GPU, and the sources, guarded buffers
+and pulls of the GPU suites (nothing here touches CUDA at import time)."""
 
 from __future__ import annotations
 
+import asyncio
+import contextlib
 import hashlib
 import random
 import types
@@ -14,7 +17,8 @@ import torch
 
 import workloads
 from torchstore_b200 import _native
-from torchstore_b200.direct_weight_sync import DirectWeightSyncDest, RDMAWeightHandle
+from torchstore_b200.direct_weight_sync import (DirectWeightSyncDest, DirectWeightSyncSource, NvlinkBuffer,
+                                                RDMAWeightHandle)
 from torchstore_b200.planner import StridedMem, build_rects
 from torchstore_b200.transport.types import TensorSlice
 
@@ -247,6 +251,53 @@ VECTOR_CAST_MODES = (8, 10, 12, 14, 16, 18)
 KIND_GENERIC, KIND_B16, KIND_F32_BF16, KIND_BF16_E4M3 = 0, 1, 2, 3
 
 
+KNOBS = ("TSB_TILE_BYTES", "TSB_STATIC_SCHED", "TSB_MAX_GRID", "TSB_FORCE_GENERIC", "TSB_LINK", "TSB_LINK_STAGES",
+         "TSB_LINK_STAGE_BYTES", "TSB_CTAS_PER_SM")
+# A covering design over (tile bytes, grid cap, scheduling, TSB_FORCE_GENERIC, TSB_LINK): every value of
+# every axis, and every (tile bytes, grid cap) pair.  Static scheduling only applies to plans without
+# link tiles, so it runs with TSB_LINK=1 on local sources.
+KERNEL_REGIMES = [
+    # tile bytes, grid cap, scheduling, force generic, TSB_LINK
+    (1024, None, "dynamic", False, 2),
+    (1024, 1, "static", True, 1),
+    (1024, 5, "dynamic", False, 1),
+    (4096, None, "static", False, 1),
+    (4096, 1, "dynamic", True, 2),
+    (4096, 5, "static", True, 1),
+    (65536, None, "dynamic", True, 1),
+    (65536, 1, "dynamic", False, 2),
+    (65536, 5, "static", False, 1),
+    (524288, None, "static", True, 1),
+    (524288, 1, "dynamic", False, 1),
+    (524288, 5, "dynamic", True, 2),
+]
+
+
+def set_knobs(monkeypatch, **knobs):
+    for k in KNOBS:
+        monkeypatch.delenv(k, raising=False)
+    for k, v in knobs.items():
+        if v is not None:
+            monkeypatch.setenv(k, str(v))
+
+
+def compiled(pairs):
+    """(rects, n, rect table fields, host PlanInfo) of `pairs` under the current knobs."""
+    rects, n = rects_for(pairs)
+    table, _, info = _native.plan_compile_host(0, rects, n, 0, 0)
+    return rects, n, rect_fields(table), info
+
+
+def run_plan(rects, n):
+    """Compile, run on torch's stream, wait, destroy; returns the plan's PlanInfo."""
+    plan = _native.plan_create(0, rects, n)
+    info = _native.plan_info(plan)
+    _native.plan_run(plan, _native.torch_stream(0))
+    torch.cuda.synchronize()
+    _native.plan_destroy(plan)
+    return info
+
+
 def rect_fields(table: np.ndarray) -> np.ndarray:
     """The rect table of _native.plan_compile_host as a record array with DevRect's field names."""
     return np.ascontiguousarray(table).view(DEV_RECT)
@@ -325,6 +376,16 @@ def assert_equal_modulo_nan(got: torch.Tensor, want: torch.Tensor, cast: bool):
     wn = ((wb & np_t(emask)) == np_t(emask)) & ((wb & np_t(mmask)) != 0)
     assert np.array_equal(gn, wn)
     assert np.array_equal(gb[~wn], wb[~wn])
+
+
+def assert_same_bits_or_nan(got: torch.Tensor, want: torch.Tensor):
+    """On the device: equal bits, or both NaN (the assert_equal_modulo_nan rule)."""
+    assert got.shape == want.shape and got.dtype == want.dtype
+    as_int = {1: torch.uint8, 2: torch.int16, 4: torch.int32, 8: torch.int64}[got.element_size()]
+    same = got.view(as_int) == want.view(as_int)
+    if got.is_floating_point():
+        same |= torch.isnan(got) & torch.isnan(want)
+    assert bool(same.all()), int((~same).sum())
 
 
 # ---- Llama-3 layouts (torchtitan TP plan; SURVEY.md section 8 header) -------------------------------
@@ -521,3 +582,136 @@ def no_export(monkeypatch):
     monkeypatch.setattr(dws.HbmDescriptor, "from_tensor", staticmethod(_boom))
     monkeypatch.setattr(torch, "empty", _boom)
     no_compile(monkeypatch)
+
+
+# ---- device suites: sessions, guarded buffers, sources and pulls on the GPU ------------------------------
+DEV = "cuda:0"
+E4M3 = torch.float8_e4m3fn
+I8 = torch.int8
+KW = {"block": "block_scales", "channel": "channel_scales", "tensor": "tensor_scales"}
+GUARD = 0x5A
+LEAD = 256
+
+needs_two_gpus = pytest.mark.skipif(torch.cuda.device_count() < 2, reason="needs 2 GPUs")
+
+
+def run(coro):
+    return asyncio.run(coro)
+
+
+def native_session():
+    """The native library for one module's tests, and every launch finished and cached block freed after them.  A
+    module binds it as ``_init = pytest.fixture(scope="module", autouse=True)(native_session)``."""
+    _native.init()
+    yield
+    torch.cuda.synchronize()
+    torch.cuda.empty_cache()
+
+
+@contextlib.contextmanager
+def named(what):
+    """Prefix a failing comparison with the layout it ran on."""
+    try:
+        yield
+    except AssertionError as e:
+        raise AssertionError(f"{what}: {e}") from e
+
+
+def skip_unless_free(nbytes):
+    free, _ = torch.cuda.mem_get_info(DEV)
+    if free < 3 * nbytes:
+        pytest.skip(f"needs {3 * nbytes / 2**30:.1f} GiB of free device memory, {free / 2**30:.1f} GiB free")
+
+
+def guarded(shape, dtype, device=DEV):
+    """A contiguous tensor of `shape` inside a GUARD-filled byte buffer (LEAD bytes before, LEAD after)
+    -> (buffer, tensor)."""
+    n = int(np.prod(shape, dtype=np.int64)) * dtype.itemsize
+    base = torch.full((n + 2 * LEAD,), GUARD, dtype=torch.uint8, device=device)
+    return base, base[LEAD: LEAD + n].view(dtype).view(shape)
+
+
+def guards_intact(base):
+    return bool((base[:LEAD] == GUARD).all()) and bool((base[-LEAD:] == GUARD).all())
+
+
+def dest_scale_shape(granularity, local_shape):
+    """The scale_inv shape of a `granularity`-scaled destination of `local_shape`."""
+    *lead, n, k = local_shape
+    return {"block": (*lead, -(-n // 128), -(-k // 128)), "channel": (*lead, n, 1), "tensor": tuple(lead)}[granularity]
+
+
+def register_shards(global_shape, shards, *, name="w", device=DEV, granularity=None, **register_kw):
+    """One DirectWeightSyncSource per entry (offsets, shard, scale or None) of `shards`: rank r publishes shard r on
+    `device` over its box of `global_shape`, with its scale under KW[granularity]; a None entry keeps its rank and
+    publishes nothing -> (sources [(source, device shard, device scale or None)], handles)."""
+    sources, handles = [], []
+    for r, entry in enumerate(shards):
+        if entry is None:
+            continue
+        off, shard, scale = entry
+        shard, kw = shard.to(device), dict(register_kw)
+        if scale is not None:
+            scale = scale.to(device)
+            kw[KW[granularity]] = {name: scale}
+        sl = TensorSlice(tuple(off), (r,), tuple(global_shape), tuple(shard.shape), (len(shards),))
+        src = DirectWeightSyncSource()
+        handles.append(src.register({name: shard}, rank=r, tensor_slices={name: sl}, **kw)[name])
+        sources.append((src, shard, scale))
+    return sources, handles
+
+
+def register_boxes(full, boxes, *, scale_of=None, **kw):
+    """register_shards of the `boxes` (offsets, local shape) of `full`, rank r holding box r (an empty box publishes
+    nothing); ``scale_of(offsets, local shape)`` gives each shard's scale."""
+    shards = [None if 0 in loc else (off, region(full, off, loc).contiguous(), scale_of(off, loc) if scale_of else None)
+              for off, loc in boxes]
+    return register_shards(full.shape, shards, **kw)
+
+
+def cleanup(sources):
+    for source, *_ in sources:
+        run(source.cleanup())
+
+
+def pull_box(handles, full_shape, box, dtype, *, granularity=None, sync=None, device=DEV, name="w", **pull_kw):
+    """Pull `handles` into a guarded `dtype` destination over the `box` (offsets, local shape) of the tensor, with a
+    guarded float32 scale under KW[granularity] when given (``requantize``, ``scale_fmt`` and ``verbatim`` pass
+    through) -> (sync, destination, scale or None, guard buffers)."""
+    off, loc = box
+    base, y = guarded(loc, dtype, device)
+    guards, scale, scales = (base,), None, {}
+    if granularity is not None:
+        sbase, scale = guarded(dest_scale_shape(granularity, loc), torch.float32, device)
+        guards, scales = (base, sbase), {KW[granularity]: {name: scale}}
+    sync = sync or DirectWeightSyncDest()
+    run(sync.pull({name: handles}, {name: y}, {name: TensorSlice(off, (0,), tuple(full_shape), loc, (1,))}, **scales,
+                  **pull_kw))
+    return sync, y, scale, guards
+
+
+# ---- packed destinations on the GPU -------------------------------------------------------------------------
+def masters(layout, seed, device=DEV):
+    g = torch.Generator(device).manual_seed(seed)
+    return {n: (torch.randn(shape, device=device, generator=g) * 0.02).to(torch.bfloat16)
+            for n, (shape, _) in layout.items()}
+
+
+def nv_handles(layout, n, full):
+    return fsdp_handles(layout, n, lambda name, off, loc: NvlinkBuffer(region(full[name], off, loc).contiguous()))
+
+
+def as_np(t):
+    return t.view({1: torch.uint8, 2: torch.int16, 4: torch.int32}[t.element_size()]).cpu().numpy()
+
+
+def whole_handle(t):
+    """One handle over the whole of ``t``."""
+    z = (0,) * t.dim()
+    return [RDMAWeightHandle(NvlinkBuffer(t.contiguous()), TensorSlice(z, (0,), tuple(t.shape), tuple(t.shape), (1,)), 0)]
+
+
+def pull(handles, dests, slices=None, **kw):
+    sync = DirectWeightSyncDest()
+    run(sync.pull(handles, dests, slices, **kw))
+    return sync

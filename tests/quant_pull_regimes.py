@@ -33,15 +33,25 @@ Branches:
 
 from __future__ import annotations
 
+import random
 from collections import defaultdict
 from dataclasses import dataclass
 from typing import Callable
 
 import numpy as np
+import torch
 
-from tests.fp8_regimes import split, whole
+from oracle import block_fp8_oracle, int8_source_oracle, scaled_fp8_oracle, ue8m0_oracle
+from oracle.block_fp8_oracle import synth_f32
+from tests.fp8_regimes import draw, split, whole
+from tests.helpers import (DEV, E4M3, KW, assert_same_bits_or_nan, dest_scale_shape, guarded, guards_intact, named,
+                           rand_full, region, run)
+from tests.source_quant_regimes import on_device
+from tests.test_block_fp8_cpu import assert_block_fp8_equal
+from tests.test_scaled_fp8_cpu import assert_scaled_fp8_equal
 from torchstore_b200 import _native
-from torchstore_b200.direct_weight_sync import DirectWeightSyncDest
+from torchstore_b200.direct_weight_sync import DirectWeightSyncDest, DirectWeightSyncSource
+from torchstore_b200.transport.types import TensorSlice
 from torchstore_b200.planner import build_rects
 
 BLOCK, STAGE_BYTES, TILE_ELEMS, BAND_ROWS = 128, 32768, 16384, 256
@@ -50,7 +60,6 @@ ES = {"bfloat16": 2, "float16": 2, "float32": 4}
 CODE = {"bfloat16": _native.TSB_BF16, "float16": _native.TSB_F16, "float32": _native.TSB_F32}
 NAME = {v: k for k, v in CODE.items()}
 GRANULARITIES = ("block", "channel", "tensor")
-KW = {"block": "block_scales", "channel": "channel_scales", "tensor": "tensor_scales"}
 
 
 @dataclass(frozen=True)
@@ -78,13 +87,6 @@ class Workload:
 
     def describe(self) -> str:
         return "; ".join(f"w{i}: {p.describe()}" for i, p in enumerate(self.pulls))
-
-
-def scale_shape(g: str, loc) -> tuple:
-    *lead, n, k = loc
-    if g == "block":
-        return (*lead, -(-n // BLOCK), -(-k // BLOCK))
-    return (*lead, n, 1) if g == "channel" else tuple(lead)
 
 
 def cut(shape, dim: int, bounds) -> tuple:
@@ -501,3 +503,298 @@ def spots(tables: Tables, geom: Geometry, cap: int = 32) -> dict[int, list]:
         add(t, es, (0, 0))
         add(t, es, (int(t["rows"]) - 1, int(t["cols"]) - 1))
     return {i: (c if len(c) <= cap else c[: cap // 2] + c[-(cap // 2):]) for i, c in out.items()}
+
+
+# ---- on the H100 ---------------------------------------------------------------------------------
+TOP = {d: float(torch.finfo(getattr(torch, d)).max) for d in ES}  # 3.39e38, 65504, 3.40e38
+
+
+def assert_block_torch_cuda(q, s, x):
+    """A block-scaled fp8 destination (q, s) against torch CUDA's quantisation of x: bytes (NaN bytes included) and
+    scale_inv bits (any NaN equal to any NaN)."""
+    want_q, want_s = block_fp8_oracle.torch_quantize(x.to(DEV))
+    assert torch.equal(q.view(torch.uint8), want_q.view(torch.uint8))
+    assert_same_bits_or_nan(s, want_s)
+
+
+def assert_scaled_torch_cuda(q, s, x, g):
+    """A channel- or tensor-scaled fp8 destination (q, s) against torch CUDA's quantisation of x, as
+    assert_block_torch_cuda."""
+    want_q, want_s = scaled_fp8_oracle.torch_quantize(x.to(DEV), g)
+    assert torch.equal(q.view(torch.uint8), want_q.view(torch.uint8))
+    assert_same_bits_or_nan(s, want_s)
+
+
+# ---- groups of a destination window -----------------------------------------------------------------
+def group_of(p: Pull, coord) -> tuple:
+    """The destination group (block, row or matrix of the window) holding global element `coord`."""
+    *lead, r, c = (x - o for x, o in zip(coord, p.dst[0]))
+    if p.g == "block":
+        return (*lead, r // BLOCK, c // BLOCK)
+    return (*lead, r) if p.g == "channel" else tuple(lead)
+
+
+def group_box(p: Pull, key) -> tuple:
+    """Global index of every element of destination group `key`."""
+    (*lo, r0, c0), (*_, n, k) = p.dst
+    lead = tuple(o + i for o, i in zip(lo, key))
+    if p.g == "block":
+        br, bc = key[-2:]
+        return lead + (slice(r0 + br * BLOCK, r0 + min(n, (br + 1) * BLOCK)), slice(c0 + bc * BLOCK, c0 + min(k, (bc + 1) * BLOCK)))
+    if p.g == "channel":
+        return lead + (slice(r0 + key[-1], r0 + key[-1] + 1), slice(c0, c0 + k))
+    return lead + (slice(r0, r0 + n), slice(c0, c0 + k))
+
+
+def n_groups(p: Pull) -> int:
+    *lead, n, k = p.dst[1]
+    m = int(np.prod(lead, dtype=np.int64))
+    return m * -(-n // BLOCK) * -(-k // BLOCK) if p.g == "block" else m * n if p.g == "channel" else m
+
+
+def fill_group(x, p: Pull, key, kind: str, seed: int):
+    box = group_box(p, key)
+    shape = tuple(x[box].shape)
+    if kind == "zero":
+        x[box] = torch.where(synth_f32(shape, seed) < 0, -0.0, 0.0)
+    else:
+        x[box] = synth_f32(shape, seed, spread=0) * torch.finfo(getattr(torch, p.dtype)).tiny * 0.5
+
+
+KINDS = ("nan", "inf", "-inf", "zero", "subnormal")
+
+
+def plant_special(x, p: Pull, coords, seed: int):
+    """NaN, +Inf, -Inf, an all-zero (+-0) group and an all-subnormal group, each in its own destination group
+    at the first spots that lie in one (one group of the window keeps finite data when it has several); -0 and
+    single subnormals at the spots in the other groups."""
+    x = x.float().clone()
+    kinds = {}
+    for j, c in enumerate(coords):
+        key = group_of(p, c)
+        if key not in kinds and len(kinds) < max(1, n_groups(p) - 1):
+            kinds[key] = KINDS[len(kinds) % len(KINDS)]
+            if kinds[key] in ("zero", "subnormal"):
+                fill_group(x, p, key, kinds[key], seed + j)
+        kind = kinds.get(key)
+        if kind in ("nan", "inf", "-inf"):
+            x[c] = float(kind)
+        elif kind is None:
+            x[c] = -0.0 if j % 2 else torch.finfo(getattr(torch, p.dtype)).tiny * 0.25
+    return x.to(getattr(torch, p.dtype))
+
+
+def near_top(x, p: Pull, coords, seed: int):
+    """Values of magnitude [0.25, 1] x the largest finite value of the source dtype, +-that value at the spots."""
+    top = TOP[p.dtype]
+    u = synth_f32(tuple(x.shape), seed, spread=0)
+    y = u.sign() * (0.25 + 0.75 * u.abs()) * top
+    for j, c in enumerate(coords):
+        y[c] = top if j % 2 == 0 else -top
+    return y.to(getattr(torch, p.dtype))
+
+
+def inputs(name: str, variant: str):
+    from tests import test_quant_pull_regimes_cpu as qp_cpu  # the host suite imports this catalogue
+    xs = qp_cpu.workload_inputs(name)
+    if variant not in ("special", "near_top"):
+        return xs
+    w = WORKLOADS[name]
+    tables, geom, *_ = qp_cpu.compiled(name)
+    at = spots(tables, geom)
+    plant = plant_special if variant == "special" else near_top
+    return [plant(x, p, at.get(i, []), w.seed + 100 * i) for i, (p, x) in enumerate(zip(w.pulls, xs))]
+
+
+# ---- one pull of several names ----------------------------------------------------------------------
+class Pulled:
+    """The names w0, w1, ... of `pulls` registered shard by shard (one source each), pulled into guarded
+    destinations of `dst_dtype` (float8_e4m3fn or int8) and scales by one DirectWeightSyncDest with the scale format
+    `scale_fmt`; `extra` handles and destinations join the pull."""
+
+    def __init__(self, pulls, xs, extra_handles=None, extra_dests=None, scale_fmt=None, dst_dtype=E4M3):
+        self.pulls, self.sources, self.shards, self.scale_fmt = tuple(pulls), [], {}, scale_fmt
+        self.dst_dtype = dst_dtype
+        self.handles, self.dests, self.scales, self.slices, self.bases = {}, {}, {}, {}, []
+        try:
+            for i, (p, x) in enumerate(zip(pulls, xs)):
+                n = f"w{i}"
+                self.handles[n], self.shards[n] = [], []
+                for r, (off, loc) in enumerate(p.src):
+                    shard = on_device(region(x, off, loc).contiguous(), p.shift(r))
+                    src = DirectWeightSyncSource()
+                    self.sources.append(src)
+                    sl = TensorSlice(off, (r,), p.shape, loc, (len(p.src),))
+                    self.handles[n].append(src.register({n: shard}, rank=r, tensor_slices={n: sl})[n])
+                    self.shards[n].append(shard)
+                qb, self.dests[n] = guarded(p.dst[1], dst_dtype)
+                sb, self.scales[n] = guarded(dest_scale_shape(p.g, p.dst[1]), torch.float32)
+                self.bases += [qb, sb]
+                self.slices[n] = TensorSlice(p.dst[0], (0,), p.shape, p.dst[1], (1,))
+        except BaseException:
+            self.close()
+            raise
+        self.all_handles = {**self.handles, **(extra_handles or {})}
+        self.all_dests = {**self.dests, **(extra_dests or {})}
+        self.by_kw = {}
+        for i, p in enumerate(self.pulls):
+            self.by_kw.setdefault(KW[p.g], {})[f"w{i}"] = self.scales[f"w{i}"]
+        self.sync = DirectWeightSyncDest()
+
+    def pull(self):
+        run(self.sync.pull(self.all_handles, self.all_dests, self.slices, **self.by_kw, scale_fmt=self.scale_fmt))
+
+    def plan_dicts(self):
+        """The (block, per-channel / per-tensor) plans of the destination format; the other format's stay empty."""
+        fp8, int8 = (self.sync._block_plans, self.sync._scaled_plans), (self.sync._int8_block_plans, self.sync._int8_scaled_plans)
+        mine, other = (int8, fp8) if self.dst_dtype == torch.int8 else (fp8, int8)
+        assert not any(other), "plans of the other destination format"
+        return mine
+
+    def plans(self):
+        return tuple(dict(p) for p in self.plan_dicts())
+
+    def live_tables(self):
+        """The tables of the plans the pull built, compiled on the host from the same windows and targets with
+        the live device addresses; their size checked against plan_info."""
+        tables, geom = compile_tables(self.pulls, self.sync._plan, self.handles, lambda b: b.window(0), self.dests, self.scales)
+        want = plan_bytes(tables)
+        for kind, plans in zip(("block", "scaled"), self.plan_dicts()):
+            if kind in want:
+                info = _native.plan_info(plans[0])
+                assert (info.num_tiles, info.src_bytes) == want[kind], kind
+            else:
+                assert not plans, kind
+        return tables, geom
+
+    def check(self, xs):
+        for i, (p, x) in enumerate(zip(self.pulls, xs)):
+            n = f"w{i}"
+            with named(f"w{i}: {p.describe()}"):
+                assert_quantised(self.dests[n], self.scales[n], region(x, *p.dst), p.g, self.scale_fmt, self.dst_dtype)
+        assert all(guards_intact(b) for b in self.bases)
+
+    def update(self, xs):
+        """New values in every source shard, in place; guard patterns over every destination and scale."""
+        for i, (p, x) in enumerate(zip(self.pulls, xs)):
+            for shard, (off, loc) in zip(self.shards[f"w{i}"], p.src):
+                shard.copy_(region(x, off, loc).to(DEV))
+            self.dests[f"w{i}"].view(torch.uint8).fill_(0xA5)
+            self.scales[f"w{i}"].fill_(-3.0)
+
+    def close(self):
+        if hasattr(self, "sync"):
+            self.sync.close()
+        for src in self.sources:
+            run(src.cleanup())
+
+
+def assert_quantised(y, ys, x, g, scale_fmt=None, dst_dtype=E4M3):
+    """The fp8 weight y and its scale_inv ys against the numpy oracle of the source region x (bit-exact in
+    finite groups, NaN-agnostic in the others) and the torch CUDA composition (bit-exact, NaN bytes included),
+    both in the scale format `scale_fmt`.  An int8 y: int8_source_oracle.assert_exact."""
+    from tests import test_quant_pull_regimes_cpu as qp_cpu  # the host suite imports this catalogue
+    if dst_dtype == torch.int8:
+        int8_source_oracle.assert_exact(y, ys, x, g)
+        return
+    if scale_fmt is None:
+        want_q, want_s = qp_cpu.oracle_quantize(x.float().numpy(), g)
+    else:
+        want_q, want_s = ue8m0_oracle.quantize(x.float().numpy(), g, scale_fmt=scale_fmt)
+    q, s = y.view(torch.uint8).cpu().numpy(), ys.cpu().numpy()
+    if g == "block":
+        assert_block_fp8_equal(q, s, want_q, want_s)
+    else:
+        assert_scaled_fp8_equal(q, s, want_q, np.asarray(want_s, np.float32), g)
+    if scale_fmt is not None:
+        want_q, want_s = ue8m0_oracle.torch_quantize(x.to(DEV), g, scale_fmt=scale_fmt)
+        want_s = want_s.reshape(ys.shape)
+        assert torch.equal(y.view(torch.uint8), want_q.view(torch.uint8))  # NaN bytes included
+        assert_same_bits_or_nan(ys, want_s)
+        ue8m0_oracle.assert_pow2_over(ys, ue8m0_oracle.torch_quantize(x.to(DEV), g)[1])
+    elif g == "block":
+        assert_block_torch_cuda(y, ys, x)
+    else:
+        assert_scaled_torch_cuda(y, ys, x, g)
+
+
+# ---- the regimes ------------------------------------------------------------------------------------
+VARIANTS = ("finite", "special", "near_top", "update")
+
+
+def run_regime(regime, variant, scale_fmt=None, dst_dtype=E4M3):
+    """Pull the regime's workload in `variant` with the scale format `scale_fmt` into `dst_dtype` destinations,
+    and check it (module doc)."""
+    r = REGIMES[regime]
+    w = WORKLOADS[r.workload]
+    xs = inputs(r.workload, variant)
+    where = f"{regime} ({r.doc}), {variant}, scale_fmt={scale_fmt}, {dst_dtype}: {w.describe()}"
+    pulled = Pulled(w.pulls, xs, scale_fmt=scale_fmt, dst_dtype=dst_dtype)
+    try:
+        pulled.pull()
+        tables, geom = pulled.live_tables()
+        assert r.holds(tables, geom), f"not reached: {where}"
+        with named(where):
+            pulled.check(xs)
+            if variant == "update":
+                xs = [(rand_full(p.shape, getattr(torch, p.dtype), w.seed + 50 + i) * -0.5) for i, p in enumerate(w.pulls)]
+                pulled.update(xs)
+                before = pulled.plans()
+                pulled.pull()
+                assert pulled.plans() == before  # replayed, not rebuilt
+                pulled.check(xs)
+    finally:
+        pulled.close()
+
+
+# ---- random layouts with special values -------------------------------------------------------------
+def boundary_spots(p: Pull, rng: random.Random, k: int = 8):
+    """`k` global coordinates of the window drawn from the corners of every shard inside it, the rows and
+    columns around block edges, and the ends and starts of consecutive rows."""
+    (doff, dloc) = p.dst
+    cands = []
+    for off, loc in p.src:
+        lo = [max(a, b) for a, b in zip(off, doff)]
+        hi = [min(a + m, b + n) for a, m, b, n in zip(off, loc, doff, dloc)]
+        if any(a >= b for a, b in zip(lo, hi)):
+            continue
+        lead = tuple(lo[:-2])
+        for r in (lo[-2], hi[-2] - 1):
+            for c in (lo[-1], hi[-1] - 1):
+                cands.append(lead + (r, c))
+    *lo, r0, c0 = doff
+    *ln, n, kk = dloc
+    for rr in (BLOCK - 1, BLOCK, rng.randrange(n)):
+        for cc in (BLOCK - 1, BLOCK, 15, 16, kk - 1, 0):
+            if rr < n and cc < kk:
+                cands.append(tuple(o + rng.randrange(m) for o, m in zip(lo, ln)) + (r0 + rr, c0 + cc))
+    return rng.sample(cands, min(k, len(cands)))
+
+
+def plant_random(x, p: Pull, rng: random.Random, seed: int):
+    """NaN, +-Inf, -0, a subnormal and the dtype's top at boundary spots; one group all zero, one subnormal."""
+    x = x.float().clone()
+    tiny = torch.finfo(getattr(torch, p.dtype)).tiny
+    values = (float("nan"), float("inf"), float("-inf"), -0.0, tiny * 0.25, TOP[p.dtype])
+    for j, c in enumerate(boundary_spots(p, rng)):
+        x[c] = values[(j + seed) % len(values)]
+    for j, kind in enumerate(("zero", "subnormal")):
+        c = tuple(o + rng.randrange(m) for o, m in zip(*p.dst))
+        fill_group(x, p, group_of(p, c), kind, seed + j)
+    return x.to(getattr(torch, p.dtype))
+
+
+def run_random_layout(seed, dst_dtype=E4M3):
+    """Pull the layout drawn from `seed`, with special values, into a `dst_dtype` destination and check it."""
+    rng = random.Random(19000 + seed)
+    w = draw(rng, "quant", seed)
+    p = Pull(("bfloat16", "float16", "float32")[seed % 3], w.shape, w.src, w.dst, w.out)
+    x = plant_random(torch.randn(w.shape, generator=torch.Generator().manual_seed(seed)) * 0.05, p, rng, seed)
+    pulled = Pulled((p,), [x], dst_dtype=dst_dtype)
+    try:
+        with named(f"seed {seed}: {p.describe()}"):
+            pulled.pull()
+            pulled.live_tables()
+            pulled.check([x])
+    finally:
+        pulled.close()

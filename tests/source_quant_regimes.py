@@ -6,7 +6,7 @@ n_groups), plus the targets they were compiled from, and names the workload that
 one ``register(quantize=...)`` call: a list of targets, each a bf16/f16/f32 shard with its shape (leading dims
 make a stack), granularity, global offset (row0, col0) and a misalignment of its source address in elements.
 The CPU suite compiles every workload on host memory and replays it against the oracle; the H100 suite
-registers it and asserts the regime again from the tables of the live addresses.
+registers it (``run_regime``) and asserts the regime again from the tables of the live addresses.
 
 Branches:
   units             blocks (one group: the part of a global 128x128 block inside the shard) and per-channel bands
@@ -26,8 +26,17 @@ from dataclasses import dataclass
 from typing import Callable
 
 import numpy as np
+import torch
 
+from oracle import int8_source_oracle, ue8m0_oracle
+from oracle.source_quant_oracle import bits_of, element_scales, quantize, synth_f32, torch_quantize, widen
+from tests.helpers import DEV, E4M3, guarded, guards_intact, named, run
+from tests.test_source_quant_cpu import CODE as GCODE
+from tests.test_source_quant_cpu import compile_host
 from torchstore_b200 import _native
+from torchstore_b200.direct_weight_sync import DirectWeightSyncSource, source_scale_shapes
+from torchstore_b200.launch import Plans
+from torchstore_b200.transport.types import TensorSlice
 
 STAGE_BYTES, TILE_ELEMS, BAND_ROWS, UNIT_CHUNKS = 32768, 16384, 256, 1024
 ES = {"bfloat16": 2, "float16": 2, "float32": 4}
@@ -229,3 +238,177 @@ def plan_bytes(tables) -> tuple[int, int]:
     read = int((units["rows"].astype(np.int64) * units["cols"] * es(units)).sum()) if len(units) else 0
     read += int((tiles["cols"].astype(np.int64) * es(tiles)).sum()) if len(tiles) else 0
     return len(units) + len(tiles), read
+
+
+# ---- on the H100 ---------------------------------------------------------------------------------
+def assert_exact(q: torch.Tensor, s: torch.Tensor, x: torch.Tensor, g: str, r0: int, c0: int, scale_fmt=None):
+    """Bit-exact against torch CUDA everywhere (NaN bytes included) and against the numpy oracle on finite groups,
+    both in the scale format `scale_fmt`."""
+    tq, tsc = ue8m0_oracle.torch_quantize(x.to(q.device), g, r0, c0, scale_fmt=scale_fmt)
+    assert torch.equal(q.view(torch.uint8), tq.view(torch.uint8))
+    assert torch.equal(s.view(torch.int32), tsc.reshape(s.shape).view(torch.int32))
+    xf = widen(bits_of(x.cpu()), str(x.dtype)[6:])
+    want_q, want_s = ue8m0_oracle.quantize(xf, g, r0, c0, scale_fmt=scale_fmt) if scale_fmt else quantize(xf, g, r0, c0)
+    want_s = np.asarray(want_s, np.float32).reshape(tuple(s.shape))
+    if scale_fmt:
+        ue8m0_oracle.assert_pow2_over(s, torch_quantize(x.to(q.device), g, r0, c0)[1])
+    got_q, got_s = q.view(torch.uint8).cpu().numpy(), s.cpu().numpy()
+    fin = np.isfinite(element_scales(want_s, g, want_q.shape, r0, c0))
+    assert np.array_equal(got_q[fin], want_q[fin])
+    fs = np.isfinite(want_s)
+    assert np.array_equal(got_s[fs].view(np.uint32), want_s[fs].view(np.uint32))
+
+
+def on_device(x: torch.Tensor, misalign: int = 0) -> torch.Tensor:
+    """`x` on the GPU, starting `misalign` elements into a fresh allocation (not 16-byte aligned if > 0) with
+    4096 elements of slack after it, so that reads past a shard's end stay inside the allocation."""
+    flat = torch.zeros(x.numel() + 4096, dtype=x.dtype, device=DEV)
+    out = flat[misalign: misalign + x.numel()].view(x.shape)
+    out.copy_(x.to(DEV))
+    return out
+
+
+def local_slice(shape, row0, col0, global_shape=None, rank=0, ranks=1):
+    lead = tuple(shape[:-2])
+    gshape = global_shape or lead + (row0 + shape[-2], col0 + shape[-1])
+    offsets = (0,) * len(lead) + (row0, col0)
+    return TensorSlice(offsets, (rank,), tuple(gshape), tuple(shape), (ranks,))
+
+
+# ---- the regimes ------------------------------------------------------------------------------------
+def group_boxes(t: Target):
+    """Index tuples of the first and the last group of a target's shard."""
+    *lead, n, k = t.shape
+    first_m, last_m = (0,) * len(lead), tuple(e - 1 for e in lead)
+    if t.granularity == "block":
+        r1, c1 = min(n, 128 - t.row0 % 128), min(k, 128 - t.col0 % 128)
+        lr, lc = max(0, (t.row0 + n - 1) // 128 * 128 - t.row0), max(0, (t.col0 + k - 1) // 128 * 128 - t.col0)
+        return first_m + (slice(0, r1), slice(0, c1)), last_m + (slice(lr, n), slice(lc, k))
+    if t.granularity == "channel":
+        return first_m + (slice(0, 1), slice(None)), last_m + (slice(n - 1, n), slice(None))
+    return first_m + (slice(None), slice(None)), last_m + (slice(None), slice(None))
+
+
+def plant(x: torch.Tensor, t: Target, kind: str, seed: int) -> torch.Tensor:
+    """Special values in the first and the last group of `x` (in its dtype): +Inf and -Inf, or NaN, at the
+    first element of the first group and the last element of the last; or both groups all zero or subnormal."""
+    x = x.float().clone()
+    first, last = group_boxes(t)
+    first_elem, last_elem = (0,) * len(t.shape), tuple(e - 1 for e in t.shape)
+    if kind in ("inf", "nan"):
+        x[first_elem] = float("inf") if kind == "inf" else float("nan")
+        x[last_elem] = float("-inf") if kind == "inf" else float("nan")
+    elif kind == "zero":
+        x[first] = 0
+        x[last] = 0
+    elif kind == "subnormal":
+        tiny = torch.finfo(getattr(torch, t.dtype)).tiny
+        for box in (first, last):
+            x[box] = synth_f32(tuple(x[box].shape), seed, spread=0) * tiny * 0.5
+    return x.to(getattr(torch, t.dtype))
+
+
+def register_workload(name, xs, scale_fmt=None, quant_dtype=None):
+    """One register() of every target of workload `name` (values `xs`), in the scale format `scale_fmt` and the
+    staging dtype `quant_dtype` -> (source, handles, device shards)."""
+    w = WORKLOADS[name]
+    src = DirectWeightSyncSource()
+    sd, slices, quant = {}, {}, {}
+    for i, (t, x) in enumerate(zip(w.targets, xs)):
+        sd[f"t{i}"] = on_device(x, t.misalign)
+        slices[f"t{i}"] = local_slice(t.shape, t.row0, t.col0)
+        quant[f"t{i}"] = t.granularity
+    handles = src.register(sd, rank=0, tensor_slices=slices, quantize=quant, scale_fmt=scale_fmt, quant_dtype=quant_dtype)
+    return src, handles, sd
+
+
+def live_tables(src, handles, w, quant_dtype=None):
+    """Compile on the host the targets register() built, from the staging it allocated and the handles'
+    offsets (for int8 staging with TSB_I8); check their size against plan_info -> (tables, targets)."""
+    targets = []
+    for i, t in enumerate(w.targets):
+        fp8, scale, local = src._quantized[f"t{i}"]
+        buf = handles[f"t{i}"].rdma_buffer
+        rows, cols = local.shape[-2:]
+        targets.append(_native.SourceQuantTarget(local.data_ptr(), fp8.data_ptr(), scale.data_ptr(), local.numel() // (rows * cols),
+                                                 rows, cols, buf.row0, buf.col0, CODE[t.dtype], GCODE[t.granularity]))
+    if quant_dtype == torch.int8:
+        arr = _native.make_source_quant_target_array(len(targets))
+        for i, t in enumerate(targets):
+            arr[i] = t
+        tables = _native.source_quant_compile_host(0, arr, len(targets), dst_dtype=_native.TSB_I8)
+    else:
+        tables = compile_host(targets)
+    info = _native.plan_info(src._quant_plans[0])
+    assert (info.num_tiles, info.src_bytes) == plan_bytes(tables)
+    return tables, targets
+
+
+def check_staging(src, w, xs, scale_fmt=None, quant_dtype=None):
+    for i, (t, x) in enumerate(zip(w.targets, xs)):
+        q, s, _ = src._quantized[f"t{i}"]
+        with named(t.describe()):
+            if quant_dtype == torch.int8:
+                int8_source_oracle.assert_exact(q, s, x, t.granularity, t.row0, t.col0)
+            else:
+                assert_exact(q, s, x, t.granularity, t.row0, t.col0, scale_fmt)
+
+
+VARIANTS = ("finite", "inf", "nan", "zero", "subnormal", "refresh")
+
+
+def run_regime(regime, variant, scale_fmt=None, quant_dtype=None):
+    """Register the regime's workload in `variant` with the scale format `scale_fmt` and the staging dtype
+    `quant_dtype`, and check it (module doc)."""
+    from tests import test_source_quant_regimes_cpu as sq_cpu  # the host suite imports this catalogue
+    r = REGIMES[regime]
+    w = WORKLOADS[r.workload]
+    xs = sq_cpu.workload_inputs(r.workload)
+    if variant not in ("finite", "refresh"):
+        xs = [plant(x, t, variant, w.seed + i) for i, (t, x) in enumerate(zip(w.targets, xs))]
+    src, handles, sd = register_workload(r.workload, xs, scale_fmt, quant_dtype)
+    where = f"{regime} ({r.doc}), {variant}, scale_fmt={scale_fmt}, quant_dtype={quant_dtype}: {w.describe()}"
+    try:
+        tables, targets = live_tables(src, handles, w, quant_dtype)
+        assert r.holds(tables, targets), f"not reached: {where}"
+        with named(where):
+            check_staging(src, w, xs, scale_fmt, quant_dtype)
+            if variant == "refresh":
+                xs = [synth_f32(t.shape, w.seed + 50 + i).to(x.dtype) * 0.25 for i, (t, x) in enumerate(zip(w.targets, xs))]
+                for i, x in enumerate(xs):
+                    sd[f"t{i}"].copy_(x.to(DEV))
+                assert src.refresh() == len(w.targets)
+                check_staging(src, w, xs, scale_fmt, quant_dtype)
+    finally:
+        run(src.cleanup())
+
+
+def run_guarded(name, scale_fmt=None, quant_dtype=None):
+    from tests import test_source_quant_regimes_cpu as sq_cpu  # the host suite imports this catalogue
+    w = WORKLOADS[name]
+    xs = sq_cpu.workload_inputs(name)
+    targets, outs = [], []
+    for t, x in zip(w.targets, xs):
+        sv = on_device(x, t.misalign)
+        sshape = source_scale_shapes(t.granularity, t.shape, t.row0, t.col0)[0]
+        qbase, q = guarded(t.shape, quant_dtype or E4M3)
+        sbase, s = guarded(sshape, torch.float32)
+        rows, cols = t.shape[-2:]
+        targets.append(_native.SourceQuantTarget(sv.data_ptr(), q.data_ptr(), s.data_ptr(), x.numel() // (rows * cols), rows, cols,
+                                                 t.row0, t.col0, CODE[t.dtype], GCODE[t.granularity]))
+        outs.append((sv, q, s, qbase, sbase))
+    plans = Plans.build_source_quant({0: targets}, _native.TSB_QUANT_UE8M0 if scale_fmt else 0,
+                                     _native.TSB_I8 if quant_dtype == torch.int8 else _native.TSB_F8E4M3)
+    try:
+        for _ in range(2):
+            plans.launch()
+            plans.synchronize()
+    finally:
+        plans.close()
+    for t, x, (_, q, s, qbase, sbase) in zip(w.targets, xs, outs):
+        with named(f"{name}: {t.describe()}"):
+            if quant_dtype == torch.int8:
+                int8_source_oracle.assert_exact(q, s, x, t.granularity, t.row0, t.col0)
+            else:
+                assert_exact(q, s, x, t.granularity, t.row0, t.col0, scale_fmt)
+            assert guards_intact(qbase) and guards_intact(sbase)

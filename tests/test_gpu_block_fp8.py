@@ -4,94 +4,28 @@ numpy oracle (finite data) and against a torch-CUDA tensor/tensor rendering of t
 values, NaN bytes included); reshards, mixed dicts, plan replay and invalidation, the public
 state-dict API, validation before any launch, and peer-mapped sources on a second GPU."""
 
-import asyncio
-
 import numpy as np
 import pytest
 import torch
 
 import torchstore_b200 as ts
-from oracle.block_fp8_oracle import quantize, torch_quantize
-from tests.helpers import rand_full, region, shard_box
+from oracle.block_fp8_oracle import quantize
+from tests.helpers import (DEV, E4M3, cleanup, guards_intact, native_session, needs_two_gpus, pull_box, rand_full, region,
+                           register_boxes, run, shard_box)
+from tests.quant_pull_regimes import assert_block_torch_cuda
 from tests.test_block_fp8_cpu import fixture_cases
 from torchstore_b200 import _native
 from torchstore_b200.direct_weight_sync import DirectWeightSyncDest, DirectWeightSyncSource
 from torchstore_b200.transport.types import TensorSlice
 
 pytestmark = pytest.mark.gpu
-DEV = "cuda:0"
-E4M3 = torch.float8_e4m3fn
-GUARD = 0x5A
-LEAD = 256
-
-
-@pytest.fixture(scope="module", autouse=True)
-def _init():
-    _native.init()
-    yield
-
-
-def run(coro):
-    return asyncio.run(coro)
-
-
-def scale_shape(shape):
-    *lead, n, k = shape
-    return (*lead, -(-n // 128), -(-k // 128))
-
-
-def guarded(shape, dtype, device=DEV):
-    """A contiguous tensor of `shape` inside a guard-filled byte buffer (LEAD bytes before, LEAD after)."""
-    n = int(np.prod(shape)) * dtype.itemsize
-    base = torch.full((n + 2 * LEAD,), GUARD, dtype=torch.uint8, device=device)
-    return base, base[LEAD: LEAD + n].view(dtype).view(shape)
-
-
-def guards_intact(base):
-    return bool((base[:LEAD] == GUARD).all()) and bool((base[-LEAD:] == GUARD).all())
-
-
-def register(full, boxes, device=DEV, **kw):
-    """One DirectWeightSyncSource per box of `full` (plain shards with tensor_slices)."""
-    sources, handles = [], []
-    for r, (off, loc) in enumerate(boxes):
-        if 0 in loc:
-            continue
-        src = DirectWeightSyncSource()
-        shard = region(full, off, loc).contiguous().to(device)
-        sl = TensorSlice(off, (r,), tuple(full.shape), loc, (len(boxes),))
-        handles.append(src.register({"w": shard}, rank=r, tensor_slices={"w": sl}, **kw)["w"])
-        sources.append((src, shard))
-    return sources, handles
-
-
-def cleanup(sources):
-    for src, _ in sources:
-        run(src.cleanup())
-
-
-def pull_into(handles, full_shape, dst_box, sync=None):
-    off, loc = dst_box
-    qb, q = guarded(loc, E4M3)
-    sb, s = guarded(scale_shape(loc), torch.float32)
-    sync = sync or DirectWeightSyncDest()
-    dsl = TensorSlice(off, (0,), tuple(full_shape), loc, (1,))
-    run(sync.pull({"w": handles}, {"w": q}, {"w": dsl}, block_scales={"w": s}))
-    return sync, q, s, qb, sb
+_init = pytest.fixture(scope="module", autouse=True)(native_session)
 
 
 def assert_oracle(q, s, x_f32):
     want_q, want_s = quantize(x_f32)
     assert np.array_equal(q.view(torch.uint8).cpu().numpy(), want_q)
     assert np.array_equal(s.cpu().numpy().view(np.uint32), want_s.view(np.uint32))
-
-
-def assert_torch_cuda(q, s, x):
-    want_q, want_s = torch_quantize(x.to(DEV))
-    assert torch.equal(q.view(torch.uint8), want_q.view(torch.uint8))  # NaN bytes included
-    both_nan = torch.isnan(s) & torch.isnan(want_s)
-    assert torch.equal(torch.isnan(s), torch.isnan(want_s))
-    assert torch.equal(s.view(torch.int32)[~both_nan], want_s.view(torch.int32)[~both_nan])
 
 
 FINITE = [c for c in fixture_cases() if "nonfinite" not in c[0]]
@@ -102,8 +36,8 @@ def test_exact_match_pull_of_the_fixture_shapes(case):
     _, dtype, x, _, _ = case
     full = torch.from_numpy(x).to(getattr(torch, dtype))
     shape = tuple(full.shape)
-    sources, handles = register(full, [((0,) * len(shape), shape)])
-    sync, q, s, qb, sb = pull_into(handles, shape, ((0,) * len(shape), shape))
+    sources, handles = register_boxes(full, [((0,) * len(shape), shape)])
+    sync, q, s, (qb, sb) = pull_box(handles, shape, ((0,) * len(shape), shape), E4M3, granularity="block")
     assert_oracle(q, s, x)
     assert guards_intact(qb) and guards_intact(sb)
     sync.close()
@@ -113,8 +47,8 @@ def test_exact_match_pull_of_the_fixture_shapes(case):
 @pytest.mark.parametrize("dtype", [torch.bfloat16, torch.float16, torch.float32])
 def test_exact_match_pull_4096(dtype):
     full = rand_full((4096, 4096), dtype, 1)
-    sources, handles = register(full, [((0, 0), (4096, 4096))])
-    sync, q, s, qb, sb = pull_into(handles, full.shape, ((0, 0), (4096, 4096)))
+    sources, handles = register_boxes(full, [((0, 0), (4096, 4096))])
+    sync, q, s, (qb, sb) = pull_box(handles, full.shape, ((0, 0), (4096, 4096)), E4M3, granularity="block")
     assert_oracle(q, s, full.float().numpy())
     assert guards_intact(qb) and guards_intact(sb)
     assert sync._block_plans and _native.plan_info(sync._block_plans[0]).num_tiles == 32 * 32
@@ -127,9 +61,9 @@ def test_exact_match_pull_4096(dtype):
 def test_special_value_blocks_match_torch_cuda_bit_for_bit(case):
     _, dtype, x, _, _ = case
     full = torch.from_numpy(x).to(getattr(torch, dtype))
-    sources, handles = register(full, [((0, 0), tuple(full.shape))])
-    sync, q, s, qb, sb = pull_into(handles, full.shape, ((0, 0), tuple(full.shape)))
-    assert_torch_cuda(q, s, full)
+    sources, handles = register_boxes(full, [((0, 0), tuple(full.shape))])
+    sync, q, s, (qb, sb) = pull_box(handles, full.shape, ((0, 0), tuple(full.shape)), E4M3, granularity="block")
+    assert_block_torch_cuda(q, s, full)
     assert guards_intact(qb) and guards_intact(sb)
     sync.close()
     cleanup(sources)
@@ -138,10 +72,10 @@ def test_special_value_blocks_match_torch_cuda_bit_for_bit(case):
 @pytest.mark.parametrize("dtype", [torch.bfloat16, torch.float32])
 def test_fsdp_rows_of_75_to_tp_columns(dtype):
     full = rand_full((300, 520), dtype, 2)
-    sources, handles = register(full, [shard_box(full.shape, 4, r, 0) for r in range(4)])
+    sources, handles = register_boxes(full, [shard_box(full.shape, 4, r, 0) for r in range(4)])
     for d in range(4):
         dst = shard_box(full.shape, 4, d, 1)
-        sync, q, s, qb, sb = pull_into(handles, full.shape, dst)
+        sync, q, s, (qb, sb) = pull_box(handles, full.shape, dst, E4M3, granularity="block")
         assert_oracle(q, s, region(full, *dst).float().numpy())
         assert guards_intact(qb) and guards_intact(sb)
         sync.close()
@@ -150,10 +84,10 @@ def test_fsdp_rows_of_75_to_tp_columns(dtype):
 
 def test_moe_stack_reshard():
     full = rand_full((3, 130, 260), torch.bfloat16, 3)
-    sources, handles = register(full, [shard_box(full.shape, 3, r, 1) for r in range(3)])
+    sources, handles = register_boxes(full, [shard_box(full.shape, 3, r, 1) for r in range(3)])
     for d in range(2):
         dst = shard_box(full.shape, 2, d, 2)
-        sync, q, s, _, _ = pull_into(handles, full.shape, dst)
+        sync, q, s, _ = pull_box(handles, full.shape, dst, E4M3, granularity="block")
         assert_oracle(q, s, region(full, *dst).float().numpy())
         sync.close()
     cleanup(sources)
@@ -189,9 +123,9 @@ def test_mixed_dict_leaves_the_other_names_as_a_plain_pull():
 
 def test_replay_refresh_and_invalidation():
     full = rand_full((300, 260), torch.bfloat16, 5)
-    sources, handles = register(full, [shard_box(full.shape, 4, r, 0) for r in range(4)])
+    sources, handles = register_boxes(full, [shard_box(full.shape, 4, r, 0) for r in range(4)])
     dst = shard_box(full.shape, 2, 1, 1)
-    sync, q, s, _, _ = pull_into(handles, full.shape, dst)
+    sync, q, s, _ = pull_box(handles, full.shape, dst, E4M3, granularity="block")
     plan = sync._block_plans[0]
     dsl = TensorSlice(dst[0], (0,), tuple(full.shape), dst[1], (1,))
     dest, scales = {"w": q}, {"w": s}
@@ -199,7 +133,7 @@ def test_replay_refresh_and_invalidation():
     run(sync.pull({"w": handles}, dest, {"w": dsl}, block_scales=scales))
     run(sync.pull({"w": handles}, dest, {"w": dsl}, block_scales=scales))
     assert _native.launch_count() == before + 2 and sync._block_plans[0] == plan  # replayed
-    for _, shard in sources:
+    for _, shard, _ in sources:
         shard.mul_(-7.0)
     new_full = (full.to(DEV) * -7.0).to(torch.bfloat16).cpu()
     run(sync.pull({"w": handles}, dest, {"w": dsl}, block_scales=scales))
@@ -246,8 +180,8 @@ def test_put_and_get_state_dict_with_block_scales():
 
 def test_every_validation_error_raises_before_any_launch():
     full = rand_full((300, 260), torch.bfloat16, 6)
-    sources, handles = register(full, [shard_box(full.shape, 4, r, 0) for r in range(4)])
-    fp8_sources, fp8_handles = register(full.to(E4M3), [((0, 0), (300, 260))])
+    sources, handles = register_boxes(full, [shard_box(full.shape, 4, r, 0) for r in range(4)])
+    fp8_sources, fp8_handles = register_boxes(full.to(E4M3), [((0, 0), (300, 260))])
     q = torch.zeros(300, 260, dtype=E4M3, device=DEV)
     s = torch.zeros(3, 3, device=DEV)
     cases = [
@@ -277,18 +211,18 @@ def test_every_validation_error_raises_before_any_launch():
     cleanup(fp8_sources)
 
 
-@pytest.mark.skipif(not torch.cuda.is_available() or torch.cuda.device_count() < 2, reason="needs 2 GPUs")
+@needs_two_gpus
 def test_pieces_read_over_peer_mappings():
     full = rand_full((300, 520), torch.bfloat16, 8)
     boxes = [shard_box(full.shape, 4, r, 0) for r in range(4)]
     sources, handles = [], []
     for r, b in enumerate(boxes):  # shards alternate between cuda:1 and cuda:0
-        s_, h_ = register(full, [b], device=f"cuda:{1 - r % 2}")
+        s_, h_ = register_boxes(full, [b], device=f"cuda:{1 - r % 2}")
         sources += s_
         handles += h_
     for d in range(2):
         dst = shard_box(full.shape, 2, d, 1)
-        sync, q, s, qb, sb = pull_into(handles, full.shape, dst)
+        sync, q, s, (qb, sb) = pull_box(handles, full.shape, dst, E4M3, granularity="block")
         assert _native.plan_info(sync._block_plans[0]).remote_src_bytes > 0
         assert_oracle(q, s, region(full, *dst).float().numpy())
         assert guards_intact(qb) and guards_intact(sb)

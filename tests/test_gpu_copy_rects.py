@@ -10,17 +10,13 @@ import pytest
 import torch
 
 from oracle import c_oracle
-from tests.helpers import (CAST_PAIRS, assert_equal_modulo_nan, bytes_of, materialise, random_case, rects_for)
+from tests.helpers import (CAST_PAIRS, assert_equal_modulo_nan, bytes_of, materialise, native_session, random_case,
+                           rects_for)
 from torchstore_b200 import _native
 from torchstore_b200.planner import StridedMem, build_rects
 
 pytestmark = pytest.mark.gpu
-
-
-@pytest.fixture(scope="module", autouse=True)
-def _init():
-    _native.init()
-    yield
+_init = pytest.fixture(scope="module", autouse=True)(native_session)
 
 
 def run_product(pairs, device=0, flags=0):

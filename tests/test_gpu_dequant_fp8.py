@@ -3,7 +3,7 @@ destinations, bit-exact against the numpy oracle on every non-NaN output and aga
 rendering (q.float() * s).to(dst) with NaN bytes included; guard bytes, mixed pulls, plan replay and
 rebuild, the state-dict API, the quantise -> dequantise round trip and peer-mapped sources."""
 
-import asyncio
+from functools import partial
 
 import numpy as np
 import pytest
@@ -11,91 +11,18 @@ import torch
 
 import torchstore_b200 as ts
 from oracle.block_fp8_oracle import quantize as block_quantize
-from oracle.dequant_fp8_oracle import GRANULARITIES, SCALE_SET, dequantize, scale_shape, torch_dequantize
-from tests.helpers import region, shard_box
-from tests.test_dequant_fp8_cpu import fp8_full, global_scale, local_scale, torch_bits
+from oracle.dequant_fp8_oracle import GRANULARITIES, SCALE_SET, scale_shape, torch_dequantize
+from tests.fp8_regimes import assert_dequant_oracle, assert_dequant_torch_cuda, want_bits
+from tests.helpers import (DEV, E4M3, KW, cleanup, guards_intact, native_session, needs_two_gpus, pull_box, region,
+                           register_boxes, run, shard_box)
+from tests.test_dequant_fp8_cpu import fp8_full, global_scale, local_scale
 from torchstore_b200 import _native
 from torchstore_b200.direct_weight_sync import DirectWeightSyncDest, DirectWeightSyncSource, ScaledNvlinkBuffer
 from torchstore_b200.transport.types import TensorSlice
 
 pytestmark = pytest.mark.gpu
-DEV = "cuda:0"
-E4M3 = torch.float8_e4m3fn
-GUARD = 0x5A
-LEAD = 256
-KW = {"block": "block_scales", "channel": "channel_scales", "tensor": "tensor_scales"}
 DTYPES = [torch.bfloat16, torch.float16, torch.float32]
-
-
-@pytest.fixture(scope="module", autouse=True)
-def _init():
-    _native.init()
-    yield
-
-
-def run(coro):
-    return asyncio.run(coro)
-
-
-def guarded(shape, dtype, device=DEV):
-    n = int(np.prod(shape, dtype=np.int64)) * dtype.itemsize
-    base = torch.full((n + 2 * LEAD,), GUARD, dtype=torch.uint8, device=device)
-    return base, base[LEAD: LEAD + n].view(dtype).view(shape)
-
-
-def guards_intact(base):
-    return bool((base[:LEAD] == GUARD).all()) and bool((base[-LEAD:] == GUARD).all())
-
-
-def register(q_full, full_scale, g, boxes, name="w", device=DEV):
-    """One source per box of `q_full`, each publishing its shard with the groups it touches."""
-    sources, handles = [], []
-    for r, (off, loc) in enumerate(boxes):
-        if 0 in loc:
-            continue
-        src = DirectWeightSyncSource()
-        shard = region(q_full, off, loc).contiguous().to(device)
-        scale = local_scale(full_scale, g, off, loc).to(device)
-        sl = TensorSlice(off, (r,), tuple(q_full.shape), loc, (len(boxes),))
-        handles.append(src.register({name: shard}, rank=r, tensor_slices={name: sl}, **{KW[g]: {name: scale}})[name])
-        sources.append((src, shard, scale))
-    return sources, handles
-
-
-def cleanup(sources):
-    for src, *_ in sources:
-        run(src.cleanup())
-
-
-def want_bits(q_full, full_scale, g, box, dtype):
-    dst = str(dtype).replace("torch.", "")
-    return dequantize(region(q_full, *box).view(torch.uint8).numpy(), local_scale(full_scale, g, *box).numpy(), g,
-                      box[0][-2], box[0][-1], dst)
-
-
-def nan_mask(y):
-    return torch.isnan(y.float()).cpu().numpy()
-
-
-def assert_oracle(y, want):
-    got = torch_bits(y.cpu())
-    nan = nan_mask(y)
-    assert np.array_equal(got[~nan], want[~nan])
-
-
-def assert_torch_cuda(y, q_full, full_scale, g, box):
-    """Bit-exact, NaN bytes included, against the torch CUDA rendering of the same region."""
-    want = torch_dequantize(region(q_full, *box).to(DEV), local_scale(full_scale, g, *box).to(DEV), g, box[0][-2],
-                            box[0][-1], y.dtype)
-    assert torch.equal(y.view(torch.uint8), want.view(torch.uint8))
-
-
-def pull_into(handles, full_shape, box, dtype, sync=None):
-    off, loc = box
-    base, y = guarded(loc, dtype)
-    sync = sync or DirectWeightSyncDest()
-    run(sync.pull({"w": handles}, {"w": y}, {"w": TensorSlice(off, (0,), tuple(full_shape), loc, (1,))}))
-    return sync, y, base
+_init = pytest.fixture(scope="module", autouse=True)(native_session)
 
 
 @pytest.mark.parametrize("g", GRANULARITIES)
@@ -105,13 +32,14 @@ def test_fsdp_to_tp_reshard(g, dtype, n, dst_dim):
     """FSDP(n) shards starting mid-block into column- and row-parallel TP destinations."""
     q = fp8_full((700, 520), 10 * n + dst_dim)
     s = global_scale(g, q.shape, n)
-    sources, handles = register(q, s, g, [shard_box(q.shape, n, r, 0) for r in range(n)])
+    sources, handles = register_boxes(q, [shard_box(q.shape, n, r, 0) for r in range(n)], granularity=g,
+                                      scale_of=partial(local_scale, s, g))
     for d in range(2):
         box = shard_box(q.shape, 2, d, dst_dim)
-        sync, y, base = pull_into(handles, q.shape, box, dtype)
+        sync, y, _, (base,) = pull_box(handles, q.shape, box, dtype)
         assert sync._dequant_plans and not sync._block_plans and not sync._scaled_plans
-        assert_oracle(y, want_bits(q, s, g, box, dtype))
-        assert_torch_cuda(y, q, s, g, box)
+        assert_dequant_oracle(y, want_bits(q, s, g, box, dtype))
+        assert_dequant_torch_cuda(y, q, s, g, box)
         assert guards_intact(base)
         sync.close()
     cleanup(sources)
@@ -123,10 +51,11 @@ def test_every_byte_against_the_scale_set(dtype):
     0, a negative scale, Inf and NaN: torch CUDA bit for bit, NaN bytes included."""
     q = torch.arange(256, dtype=torch.uint8).repeat(len(SCALE_SET), 1).view(E4M3)
     s = torch.from_numpy(SCALE_SET.copy()).reshape(-1, 1)
-    sources, handles = register(q, s, "channel", [((0, 0), tuple(q.shape))])
-    sync, y, base = pull_into(handles, q.shape, ((0, 0), tuple(q.shape)), dtype)
-    assert_torch_cuda(y, q, s, "channel", ((0, 0), tuple(q.shape)))
-    assert_oracle(y, want_bits(q, s, "channel", ((0, 0), tuple(q.shape)), dtype))
+    sources, handles = register_boxes(q, [((0, 0), tuple(q.shape))], granularity="channel",
+                                      scale_of=partial(local_scale, s, "channel"))
+    sync, y, _, (base,) = pull_box(handles, q.shape, ((0, 0), tuple(q.shape)), dtype)
+    assert_dequant_torch_cuda(y, q, s, "channel", ((0, 0), tuple(q.shape)))
+    assert_dequant_oracle(y, want_bits(q, s, "channel", ((0, 0), tuple(q.shape)), dtype))
     assert guards_intact(base)
     sync.close()
     cleanup(sources)
@@ -137,10 +66,10 @@ def test_ep_moe_stack_and_replicas(g):
     q = fp8_full((4, 130, 260), 5)
     s = global_scale(g, q.shape, 5)
     boxes = [shard_box(q.shape, 2, r % 2, 0) for r in range(4)]  # EP(2) x replicated(2)
-    sources, handles = register(q, s, g, boxes)
+    sources, handles = register_boxes(q, boxes, granularity=g, scale_of=partial(local_scale, s, g))
     box = ((0, 0, 0), (4, 130, 260))
-    sync, y, base = pull_into(handles, q.shape, box, torch.bfloat16)
-    assert_torch_cuda(y, q, s, g, box)
+    sync, y, _, (base,) = pull_box(handles, q.shape, box, torch.bfloat16)
+    assert_dequant_torch_cuda(y, q, s, g, box)
     sync.close()
     cleanup(sources)
 
@@ -150,7 +79,8 @@ def test_strided_windows_leave_the_rest_alone():
     q = fp8_full((256, 512), 7)
     s = global_scale("block", q.shape, 7)
     box = ((0, 0), (256, 384))
-    sources, handles = register(q, s, "block", [box])  # columns 384.. are published by no handle
+    sources, handles = register_boxes(q, [box], granularity="block",
+                                      scale_of=partial(local_scale, s, "block"))  # columns 384.. are published by no handle
     dest = torch.full((256, 512), 3.0, dtype=torch.bfloat16, device=DEV)
     dsl = TensorSlice((0, 0), (0,), (256, 512), (256, 512), (1,))
     sync = DirectWeightSyncDest()
@@ -165,7 +95,8 @@ def test_mixed_pull_dequant_plain_cast_and_quantise():
     """One pull: a block-dequantised name, a plain bf16 name, an unscaled fp8 -> bf16 cast and a block-quantising name."""
     q = fp8_full((300, 260), 9)
     s = global_scale("block", q.shape, 9)
-    dq_sources, dq_handles = register(q, s, "block", [shard_box(q.shape, 3, r, 0) for r in range(3)], name="dq")
+    dq_sources, dq_handles = register_boxes(q, [shard_box(q.shape, 3, r, 0) for r in range(3)], granularity="block",
+                                            scale_of=partial(local_scale, s, "block"), name="dq")
     plain = (torch.randn(128, 64) * 0.1).to(torch.bfloat16)
     raw = fp8_full((128, 96), 10)
     master = (torch.randn(256, 256) * 0.1).to(torch.bfloat16)
@@ -194,8 +125,9 @@ def test_scaled_handles_never_take_the_unscaled_cast():
     """Regression: a scaled handle pulled into bf16 is dequantised, never cast as raw e4m3fn bytes."""
     q = fp8_full((128, 128), 11)
     s = torch.full((1, 1), 0.25)
-    sources, handles = register(q, s, "block", [((0, 0), (128, 128))])
-    sync, y, _ = pull_into(handles, q.shape, ((0, 0), (128, 128)), torch.bfloat16)
+    sources, handles = register_boxes(q, [((0, 0), (128, 128))], granularity="block",
+                                      scale_of=partial(local_scale, s, "block"))
+    sync, y, _, _ = pull_box(handles, q.shape, ((0, 0), (128, 128)), torch.bfloat16)
     assert not sync._native_plans and len(sync._dequant_plans) == 1
     assert torch.equal(y, (q.to(DEV).float() * 0.25).to(torch.bfloat16))
     assert not torch.equal(y, q.to(DEV).to(torch.bfloat16))
@@ -210,7 +142,8 @@ def test_scaled_handles_never_take_the_unscaled_cast():
 def test_replay_after_source_change_and_rebuild_after_destination_change():
     q = fp8_full((256, 256), 12)
     s = global_scale("channel", q.shape, 12)
-    sources, handles = register(q, s, "channel", [shard_box(q.shape, 2, r, 0) for r in range(2)])
+    sources, handles = register_boxes(q, [shard_box(q.shape, 2, r, 0) for r in range(2)], granularity="channel",
+                                      scale_of=partial(local_scale, s, "channel"))
     dest = {"w": torch.zeros(256, 256, dtype=torch.float16, device=DEV)}
     sync = DirectWeightSyncDest()
     run(sync.pull({"w": handles}, dest))
@@ -308,10 +241,12 @@ def test_put_and_get_state_dict_with_scaled_sources():
 def test_validation_raises_before_any_launch():
     q = fp8_full((256, 256), 17)
     s = global_scale("block", q.shape, 17)
-    sources, handles = register(q, s, "block", [((0, 0), (256, 256))])
+    sources, handles = register_boxes(q, [((0, 0), (256, 256))], granularity="block",
+                                      scale_of=partial(local_scale, s, "block"))
     psrc = DirectWeightSyncSource()
     plain = psrc.register({"w": q.to(DEV)}, rank=1)["w"]
-    csources, chandles = register(q, global_scale("channel", q.shape, 1), "channel", [((0, 0), (256, 256))])
+    csources, chandles = register_boxes(q, [((0, 0), (256, 256))], granularity="channel",
+                                        scale_of=partial(local_scale, global_scale("channel", q.shape, 1), "channel"))
     before = _native.launch_count()
     cases = [
         (ValueError, handles + [plain], torch.zeros(256, 256, dtype=torch.bfloat16, device=DEV)),
@@ -341,21 +276,21 @@ def test_validation_raises_before_any_launch():
     run(psrc.cleanup())
 
 
-@pytest.mark.skipif(not torch.cuda.is_available() or torch.cuda.device_count() < 2, reason="needs 2 GPUs")
+@needs_two_gpus
 @pytest.mark.parametrize("g", GRANULARITIES)
 def test_weight_and_scale_read_over_peer_mappings(g):
     q = fp8_full((300, 520), 18)
     s = global_scale(g, q.shape, 18)
     sources, handles = [], []
     for r, b in enumerate([shard_box(q.shape, 4, r, 0) for r in range(4)]):  # shards alternate between cuda:1 and cuda:0
-        s_, h_ = register(q, s, g, [b], device=f"cuda:{1 - r % 2}")
+        s_, h_ = register_boxes(q, [b], granularity=g, scale_of=partial(local_scale, s, g), device=f"cuda:{1 - r % 2}")
         sources += s_
         handles += h_
     for d in range(2):
         box = shard_box(q.shape, 2, d, 1)
-        sync, y, base = pull_into(handles, q.shape, box, torch.bfloat16)
+        sync, y, _, (base,) = pull_box(handles, q.shape, box, torch.bfloat16)
         assert _native.plan_info(sync._dequant_plans[0]).remote_src_bytes > 0
-        assert_torch_cuda(y, q, s, g, box)
+        assert_dequant_torch_cuda(y, q, s, g, box)
         assert guards_intact(base)
         sync.close()
     cleanup(sources)

@@ -3,7 +3,6 @@
 the second replays the golden plans recorded from the reference; the third checks a scaled
 Llama-3 FSDP->TP sync against the numpy oracle."""
 
-import asyncio
 import itertools
 import json
 import os
@@ -13,18 +12,13 @@ import pytest
 import torch
 
 from oracle import reshard_oracle as ro
-from tests.helpers import llama_layout, sha256_of
+from tests.helpers import DEV, llama_layout, run, sha256_of
 from torchstore_b200.direct_weight_sync import (DirectWeightSyncDest, DirectWeightSyncSource, NvlinkBuffer,
                                                 RDMAWeightHandle)
 from torchstore_b200.transport.types import TensorSlice
 
 pytestmark = pytest.mark.gpu
 GOLDEN = os.path.join(os.path.dirname(__file__), "golden")
-DEV = "cuda:0"
-
-
-def run(coro):
-    return asyncio.run(coro)
 
 
 def _make_sharded_handles(original, num_shards, shard_dim, keep):

@@ -3,7 +3,6 @@ bit for bit like torch's CUDA .to() (NaN encodings included), every fp8 pattern 
 multi-rect fp8 workloads against the C oracle, direct weight sync with fp8 staging and fp8
 destinations, and the store path's fused fp8 gets."""
 
-import asyncio
 import json
 import os
 import random
@@ -14,7 +13,8 @@ import torch
 import torchstore_b200 as ts
 import workloads
 from oracle import fp8_oracle
-from tests.helpers import assert_equal_modulo_nan, rect_fields, sha256_of
+from tests.helpers import (DEV, E4M3, GUARD, assert_equal_modulo_nan, assert_same_bits_or_nan, cleanup, named,
+                           native_session, rect_fields, register_boxes, run, sha256_of, shard_box)
 from tests.test_fp8_cast_cpu import SHORT as SHORT_NAMES
 from tests.test_fp8_cast_cpu import VECTOR_MODE, fp8_case, host_bases
 from torchstore_b200 import _native
@@ -23,37 +23,16 @@ from torchstore_b200.planner import StridedMem, build_rects
 from torchstore_b200.transport.types import TensorSlice
 
 pytestmark = pytest.mark.gpu
-DEV = "cuda:0"
-E4M3, E5M2 = torch.float8_e4m3fn, torch.float8_e5m2
-GUARD = 0x5A
+E5M2 = torch.float8_e5m2
 GOLDEN = os.path.join(os.path.dirname(__file__), "golden", "direct_fp8.json")
-
-
-@pytest.fixture(scope="module", autouse=True)
-def _init():
-    _native.init()
-    yield
-
-
-def run(coro):
-    return asyncio.run(coro)
+_init = pytest.fixture(scope="module", autouse=True)(native_session)
 
 
 def u8(t: torch.Tensor) -> torch.Tensor:
     return t.contiguous().view(torch.uint8)
 
 
-def same_or_nan(got: torch.Tensor, want: torch.Tensor) -> bool:
-    """Bit-exact, except that any NaN equals any NaN (widened outputs)."""
-    if got.dtype in (E4M3, E5M2):
-        return torch.equal(u8(got), u8(want))
-    g, w = got.float(), want.float()
-    both_nan = torch.isnan(g) & torch.isnan(w)
-    return bool(torch.equal(torch.isnan(g), torch.isnan(w))) and torch.equal(
-        u8(got).view(-1, got.element_size())[~both_nan.reshape(-1)], u8(want).view(-1, want.element_size())[~both_nan.reshape(-1)])
-
-
-def guarded(shape, dtype, lead: int, pitch_pad: int = 0):
+def guarded_pitched(shape, dtype, lead: int, pitch_pad: int = 0):
     """A destination window of `shape` inside a guard-filled buffer: `lead` elements before the window's
     first element, rows `pitch_pad` elements longer than the window's."""
     rows, cols = shape
@@ -68,9 +47,9 @@ def layouts(src_flat: torch.Tensor, dst_dtype):
     same one element off alignment (scalar), strided narrow rows and strided wide rows."""
     n = src_flat.numel()
     out = []
-    base, win = guarded((1, n), dst_dtype, 16 // dst_dtype.itemsize * 2 if dst_dtype.itemsize < 16 else 2)
+    base, win = guarded_pitched((1, n), dst_dtype, 16 // dst_dtype.itemsize * 2 if dst_dtype.itemsize < 16 else 2)
     out.append(("vector", src_flat.view(1, n), win, base))
-    base, win = guarded((1, n), dst_dtype, 1)
+    base, win = guarded_pitched((1, n), dst_dtype, 1)
     out.append(("scalar", src_flat.view(1, n), win, base))
     for name, cols in (("narrow", 64), ("wide", 65536)):
         if n % cols:
@@ -80,7 +59,7 @@ def layouts(src_flat: torch.Tensor, dst_dtype):
         sbase = torch.empty(rows * (cols + spad), dtype=src_flat.dtype, device=DEV)
         swin = sbase.view(rows, cols + spad)[:, :cols]
         swin.copy_(src_flat.view(rows, cols))
-        base, win = guarded((rows, cols), dst_dtype, 16, pitch_pad=16)
+        base, win = guarded_pitched((rows, cols), dst_dtype, 16, pitch_pad=16)
         out.append((name, swin, win, base))
     return out
 
@@ -139,7 +118,7 @@ def test_every_f32_pattern_narrows_like_torch(dst_dtype):
     vmode = VECTOR_MODE[(torch.float32, dst_dtype)]
     plans = []
     for name, lead in (("vector", 16), ("scalar", 1)):
-        base, win = guarded((1, chunk), dst_dtype, lead)
+        base, win = guarded_pitched((1, chunk), dst_dtype, lead)
         rects, n = build_rects([(StridedMem.from_tensor(src.view(1, chunk)), StridedMem.from_tensor(win))])
         table, _, _ = _native.plan_compile_host(0, rects, n)
         assert set(rect_fields(table)["mode"].tolist()) == ({vmode} if name == "vector" else {vmode + 1})
@@ -170,7 +149,8 @@ def test_every_fp8_pattern_widens_like_torch(src_dtype, dst_dtype):
     vmode = VECTOR_MODE[(src_dtype, dst_dtype)]
     for name, swin, dwin, dbase in layouts(src, dst_dtype):
         run_pairs([(swin, dwin)], expect_modes={vmode + 1} if name == "scalar" else {vmode})
-        assert same_or_nan(dwin.reshape(-1), want), name
+        with named(name):
+            assert_same_bits_or_nan(dwin.reshape(-1), want)
         check_guards(dbase, dwin)
 
 
@@ -222,19 +202,6 @@ def box(t, ts_):
     return t[tuple(slice(o, o + s) for o, s in zip(ts_.offsets, ts_.local_shape))]
 
 
-def register_fsdp(full, n_src, **kw):
-    sources, handles = [], []
-    for r in range(n_src):
-        sl = tslice(full.shape, n_src, r, ("S", 0))
-        if 0 in sl.local_shape:
-            continue
-        src = DirectWeightSyncSource()
-        shard = box(full, sl).contiguous().to(DEV)
-        handles.append(src.register({"w": shard}, rank=r, tensor_slices={"w": sl}, **kw)["w"])
-        sources.append((src, shard))
-    return sources, handles
-
-
 def test_register_fp8_transfer_dtype_and_pull_matches_torch_and_the_reference():
     with open(GOLDEN) as f:
         cases = json.load(f)["cases"]
@@ -242,7 +209,8 @@ def test_register_fp8_transfer_dtype_and_pull_matches_torch_and_the_reference():
     for c in cases:
         full = direct_fp8_full(tuple(c["global_shape"]), c["src_dtype"], c["seed"])
         fdt = getattr(torch, c["transfer_dtype"])
-        sources, handles = register_fsdp(full, c["n_src"], transfer_dtype=fdt)
+        sources, handles = register_boxes(full, [shard_box(full.shape, c["n_src"], r, 0) for r in range(c["n_src"])],
+                                          transfer_dtype=fdt)
         want_full = full.to(DEV).to(fdt)
         for drank, rec in c["dest"].items():
             dsl = tslice(full.shape, c["n_dst"], int(drank), tuple(c["dst_placement"]))
@@ -252,19 +220,18 @@ def test_register_fp8_transfer_dtype_and_pull_matches_torch_and_the_reference():
             assert torch.equal(u8(dest), u8(box(want_full, dsl))), (c, drank)
             assert sha256_of(dest) == rec["sha256"], (c, drank)
             sync.close()
-        for src, _ in sources:
-            run(src.cleanup())
+        cleanup(sources)
 
 
 @pytest.mark.parametrize("src_dtype", [torch.bfloat16, torch.float32])
 def test_refresh_after_an_in_place_update(src_dtype):
     full = direct_fp8_full((128, 96), str(src_dtype).replace("torch.", ""), 7)
-    sources, handles = register_fsdp(full, 4, transfer_dtype=E4M3)
+    sources, handles = register_boxes(full, [shard_box(full.shape, 4, r, 0) for r in range(4)], transfer_dtype=E4M3)
     dsl = tslice(full.shape, 2, 1, ("S", 1))
     dest = torch.zeros(dsl.local_shape, dtype=E4M3, device=DEV)
     sync = DirectWeightSyncDest()
     run(sync.pull({"w": handles}, {"w": dest}, {"w": dsl}))
-    for src, shard in sources:
+    for src, shard, _ in sources:
         shard.mul_(-3.0)
         assert src.refresh() == 1
     run(sync.pull({"w": handles}, {"w": dest}, {"w": dsl}))
@@ -276,7 +243,7 @@ def test_refresh_after_an_in_place_update(src_dtype):
 @pytest.mark.parametrize("dst_dtype", [E4M3, E5M2])
 def test_bf16_handles_into_fp8_destinations_fuse_the_cast_into_the_gather(dst_dtype):
     full = direct_fp8_full((256, 128), "bfloat16", 11)
-    _, handles = register_fsdp(full, 4)
+    _, handles = register_boxes(full, [shard_box(full.shape, 4, r, 0) for r in range(4)])
     for drank in range(2):
         dsl = tslice(full.shape, 2, drank, ("S", 1))
         dest = torch.zeros(dsl.local_shape, dtype=dst_dtype, device=DEV)
@@ -291,12 +258,12 @@ def test_bf16_handles_into_fp8_destinations_fuse_the_cast_into_the_gather(dst_dt
 @pytest.mark.parametrize("src_fp8", [E4M3, E5M2])
 def test_fp8_handles_into_bf16_destinations(src_fp8):
     full = direct_fp8_full((256, 128), "bfloat16", 12).to(src_fp8)
-    _, handles = register_fsdp(full, 4)
+    _, handles = register_boxes(full, [shard_box(full.shape, 4, r, 0) for r in range(4)])
     dsl = tslice(full.shape, 2, 0, ("S", 1))
     dest = torch.zeros(dsl.local_shape, dtype=torch.bfloat16, device=DEV)
     sync = DirectWeightSyncDest()
     run(sync.pull({"w": handles}, {"w": dest}, {"w": dsl}))
-    assert same_or_nan(dest.reshape(-1), box(full.to(DEV).to(torch.bfloat16), dsl).reshape(-1))
+    assert_same_bits_or_nan(dest.reshape(-1), box(full.to(DEV).to(torch.bfloat16), dsl).reshape(-1))
     sync.close()
 
 

@@ -9,8 +9,6 @@ fp8 oracle or torch's CUDA .to() -- fp8 outputs byte for byte, widened outputs w
 any NaN -- and asserts from plan_info and the compiled rect table that it reached the regime it is
 named for."""
 
-import asyncio
-
 import numpy as np
 import pytest
 import torch
@@ -18,28 +16,20 @@ import torch
 from oracle import fp8_oracle
 from oracle import reshard_oracle as ro
 from tests import fp8_cast_regimes as fr
-from tests.helpers import (KIND_BF16_E4M3, KIND_GENERIC, MODE_B16, assert_equal_modulo_nan, edge_coverage,
-                           llama_layout, plan_kind, rect_fields, rects_for)
+from tests.helpers import (DEV, E4M3, KERNEL_REGIMES, KIND_BF16_E4M3, KIND_GENERIC, MODE_B16, assert_equal_modulo_nan,
+                           assert_same_bits_or_nan, compiled, edge_coverage, llama_layout, native_session, plan_kind,
+                           rect_fields, rects_for, run, run_plan, set_knobs)
 from tests.test_fp8_cast_cpu import VECTOR_MODE
-from tests.test_gpu_kernel_regimes import REGIMES, assert_same_bits_or_nan, compiled, run_plan, set_knobs
 from torchstore_b200 import _native
 from torchstore_b200.direct_weight_sync import DirectWeightSyncDest, DirectWeightSyncSource
 from torchstore_b200.planner import StridedMem, build_rects
 from torchstore_b200.transport.types import TensorSlice
 
 pytestmark = pytest.mark.gpu
-DEV = "cuda:0"
-E4M3, E5M2 = torch.float8_e4m3fn, torch.float8_e5m2
+E5M2 = torch.float8_e5m2
 BF16, F16, F32 = torch.bfloat16, torch.float16, torch.float32
 GUARD = fr.GUARD
-
-
-@pytest.fixture(scope="module", autouse=True)
-def _init():
-    _native.init()
-    yield
-    torch.cuda.synchronize()
-    torch.cuda.empty_cache()
+_init = pytest.fixture(scope="module", autouse=True)(native_session)
 
 
 def assert_same(got: torch.Tensor, want: torch.Tensor):
@@ -51,7 +41,7 @@ def assert_same(got: torch.Tensor, want: torch.Tensor):
         assert_same_bits_or_nan(got, want)
 
 
-def guarded(n: int, dtype) -> torch.Tensor:
+def guarded_flat(n: int, dtype) -> torch.Tensor:
     """A flat destination allocation of n elements, every byte GUARD."""
     return torch.full((n * dtype.itemsize,), GUARD, dtype=torch.uint8, device=DEV).view(dtype)
 
@@ -106,7 +96,7 @@ def test_fp8_edge_workloads_match_oracle_across_regimes(tile_bytes, workload, mo
     fp8_oracle.copy_rects(hrects, hn, nan_mode=1)
     dev = fr.materialise(cases, DEV, seed, T)
     initial = [d[2].clone() for d in dev]
-    regimes = [r for r in REGIMES if r[0] == tile_bytes]
+    regimes = [r for r in KERNEL_REGIMES if r[0] == tile_bytes]
     assert {r[1] for r in regimes} == {None, 1, 5}
     for _, cap, sched, generic, link in regimes:
         set_knobs(monkeypatch, TSB_TILE_BYTES=tile_bytes, TSB_MAX_GRID=cap, TSB_LINK=link,
@@ -152,9 +142,9 @@ def _boundary_plan(plan, ntiles, g):
         (wide_s, wide_d), (nd_s, nd_d), nd_w, (s0, d0) = (F32, E5M2), (E4M3, BF16), 8, (1, 3)
     a = torch.randint(0, 256, (L * wide_s.itemsize + 64 + SLACK,), dtype=torch.uint8, device=DEV, generator=g)
     a = a.view(wide_s)
-    out_a = guarded(L + 64 + SLACK, wide_d)
+    out_a = guarded_flat(L + 64 + SLACK, wide_d)
     b, bstack = _stack(nd_s, 2 * m, m, nd_w + 16, g)
-    out_b = guarded((2 * m * (m + 1) * (nd_w + 32) * nd_d.itemsize + SLACK) // nd_d.itemsize, nd_d)
+    out_b = guarded_flat((2 * m * (m + 1) * (nd_w + 32) * nd_d.itemsize + SLACK) // nd_d.itemsize, nd_d)
     bdst = lambda o: o[: 2 * m * (m + 1) * (nd_w + 32)].view(2 * m, m + 1, nd_w + 32)
     # the wide row 16 bytes in on both sides; the N-D window: 2 of the stack's outer rows, m of m + 1
     sa = 16 // wide_s.itemsize
@@ -196,7 +186,7 @@ def _slacked(shape, dtype, guard: bool):
     """(flat allocation, alloc -> [shape] view of its front) with SLACK bytes behind; GUARD-filled or empty."""
     n = int(np.prod(shape))
     count = n + SLACK // dtype.itemsize
-    a = guarded(count, dtype) if guard else torch.empty(count, dtype=dtype, device=DEV)
+    a = guarded_flat(count, dtype) if guard else torch.empty(count, dtype=dtype, device=DEV)
     return a, lambda o: o[:n].view(shape)
 
 
@@ -306,7 +296,7 @@ def test_fp8_windows_beyond_4_gib(monkeypatch):
         w = win.shape[1]
         for vector in (True, False):
             start = 16 // ddt.itemsize if vector else 1
-            out = guarded(rows * (w + 2 * start + 16), ddt).view(rows, w + 2 * start + 16)
+            out = guarded_flat(rows * (w + 2 * start + 16), ddt).view(rows, w + 2 * start + 16)
             rects, n, fields, _ = compiled([(win, out[:, start:start + w])])
             assert len(fields) == 1
             assert int(fields["mode"][0]) == VECTOR_MODE[(sdt, ddt)] + (0 if vector else 1)
@@ -314,7 +304,7 @@ def test_fp8_windows_beyond_4_gib(monkeypatch):
             assert int(fields["src_stride"][0][0]) * int(fields["rows"][0]) > 1 << 32
             if vector:
                 assert int(fields["src_unit_bytes"][0]) == 16 * sdt.itemsize
-            full = guarded(out.numel(), ddt).view(out.shape)
+            full = guarded_flat(out.numel(), ddt).view(out.shape)
             full[:, start:start + w] = want
             run_plan(rects, n)
             assert_same(out, full)
@@ -325,10 +315,6 @@ def test_fp8_windows_beyond_4_gib(monkeypatch):
 
 
 # ---- at model scale -----------------------------------------------------------------------------------
-def _run(coro):
-    return asyncio.run(coro)
-
-
 def _box(t, sl):
     return t[tuple(slice(o, o + s) for o, s in zip(sl.offsets, sl.local_shape))]
 
@@ -370,9 +356,9 @@ def test_llama_bf16_fsdp_refresh_into_e4m3_and_tp_pulls_match_torch(n):
                     dslices[name] = TensorSlice(dsl.offsets, dsl.coordinates, dsl.global_shape, dsl.local_shape, dsl.mesh_shape)
                 boxes[name] = dsl
             sync = DirectWeightSyncDest()
-            _run(sync.pull(handles, dest, dslices or None))
+            run(sync.pull(handles, dest, dslices or None))
             for name in layout:
                 assert_same(dest[name], _box(want[name], boxes[name]).to(dtype))
             sync.close()
     for src in sources:
-        _run(src.cleanup())
+        run(src.cleanup())

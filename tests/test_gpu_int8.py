@@ -4,26 +4,19 @@ partial edge blocks, the two-pass paths, NaN / Inf / zero groups, mixed pulls, r
 refusals, FSDP -> TP over peer mappings (two GPUs), and the full-size Llama-3-8B linear weights against the
 torch-CUDA rendering.  Several "ranks" are emulated as several sources on cuda:0."""
 
-import asyncio
-
 import numpy as np
 import pytest
 import torch
 
 from oracle.int8_oracle import (GRANULARITIES, SPECIALS, bits_of, quantize, same_scales, scale_shape, special_stack,
                                 synth_f32, torch_quantize, widen)
+from tests.fp8_regimes import whole
+from tests.helpers import DEV, E4M3, I8, KW, cleanup, needs_two_gpus, pull_box, run
 from torchstore_b200.direct_weight_sync import DirectWeightSyncDest, DirectWeightSyncSource
 from torchstore_b200.transport.types import TensorSlice
 
 pytestmark = pytest.mark.gpu
-DEV = "cuda:0"
-E4M3 = torch.float8_e4m3fn
 DTYPES = (torch.bfloat16, torch.float16, torch.float32)
-KW = {"block": "block_scales", "channel": "channel_scales", "tensor": "tensor_scales"}
-
-
-def run(coro):
-    return asyncio.run(coro)
 
 
 def publish(full: torch.Tensor, boxes, name="w", device=DEV, **register_kw):
@@ -36,11 +29,6 @@ def publish(full: torch.Tensor, boxes, name="w", device=DEV, **register_kw):
         handles.append(src.register({name: shard}, rank=r, tensor_slices={name: ts}, **register_kw)[name])
         sources.append((src, shard))
     return sources, handles
-
-
-def cleanup(sources):
-    for src, _ in sources:
-        run(src.cleanup())
 
 
 def rows(shape, k):
@@ -68,14 +56,6 @@ def assert_exact(q, s, x, g):
     assert same_scales(s.cpu().numpy().reshape(want_s.shape), want_s)
 
 
-def pull_into(handles, shape, g, **kw):
-    q, s = int8_dest(g, shape)
-    d = DirectWeightSyncDest()
-    run(d.pull({"w": handles}, {"w": q}, **{KW[g]: {"w": s}}, **kw))
-    d.close()
-    return q, s
-
-
 LAYOUTS = {
     "exact_300x520": ((300, 520), lambda s: [((0, 0), s)]),
     "fsdp4_rows_ragged_300x200": ((300, 200), lambda s: rows(s, 4)),
@@ -93,7 +73,8 @@ def test_quantising_pull_is_exact(g, dtype, layout):
     shape, boxes = LAYOUTS[layout]
     full = synth_f32(shape, 201 + len(layout)).to(dtype)
     sources, handles = publish(full, boxes(shape))
-    q, s = pull_into(handles, shape, g)
+    sync, q, s, _ = pull_box(handles, shape, whole(shape), I8, granularity=g)
+    sync.close()
     assert_exact(q, s, full, g)
     cleanup(sources)
 
@@ -104,7 +85,8 @@ def test_long_channel_rows_and_tensors_take_the_two_pass_path(dtype):
     full = synth_f32(shape, 7).to(dtype)
     sources, handles = publish(full, cols(shape, (shape[1] // 2,)))
     for g in ("channel", "tensor"):
-        q, s = pull_into(handles, shape, g)
+        sync, q, s, _ = pull_box(handles, shape, whole(shape), I8, granularity=g)
+        sync.close()
         assert_exact(q, s, full, g)
     cleanup(sources)
 
@@ -117,7 +99,8 @@ def test_nan_inf_zero_ties_max_and_subnormal_groups(g, dtype):
     full = special_stack(dtype)
     shape = tuple(full.shape)
     sources, handles = publish(full, rows(shape, 2))
-    q, s = pull_into(handles, shape, g)
+    sync, q, s, _ = pull_box(handles, shape, whole(shape), I8, granularity=g)
+    sync.close()
     assert_exact(q, s, full, g)
     qc, sc = q.cpu(), s.cpu()
     for k, kind in enumerate(SPECIALS):
@@ -236,7 +219,7 @@ def test_refusals_on_the_device():
     cleanup(sources)
 
 
-@pytest.mark.skipif(torch.cuda.device_count() < 2, reason="needs two GPUs")
+@needs_two_gpus
 @pytest.mark.parametrize("g", GRANULARITIES)
 def test_fsdp_to_tp_over_peer_mappings(g):
     """FSDP(2) row shards on cuda:0 and cuda:1 pulled into TP(2) column shards on both devices."""

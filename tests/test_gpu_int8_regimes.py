@@ -19,9 +19,9 @@ the INT8 golden fixtures, past byte 2^32 and across random layouts.
 * Random layouts: the quantising pull's random layouts with special values into int8 destinations, and the
   dequantising draws from int8 handles."""
 
-import asyncio
 import os
 import random
+from functools import partial
 
 import numpy as np
 import pytest
@@ -30,57 +30,42 @@ import torch
 from oracle import int8_oracle as i8
 from oracle import int8_source_oracle as i8s
 from tests import fp8_regimes, quant_pull_regimes, source_quant_regimes
-from tests import test_gpu_fp8_regimes as fp8_gpu
-from tests import test_gpu_quant_pull_regimes as qp_gpu
-from tests import test_gpu_source_quant_regimes as sq_gpu
+from tests.helpers import (DEV, I8, KW, cleanup, dest_scale_shape, guarded, guards_intact, named, native_session, pull_box,
+                           register_boxes, run, skip_unless_free)
 from tests.quant_pull_regimes import Pull, split, whole
-from tests.test_gpu_dequant_fp8 import cleanup, guarded, guards_intact, register
-from tests.test_gpu_fp8_regimes import named, skip_unless_free
+from tests.test_dequant_fp8_cpu import local_scale as dq_local_scale
 from tests.test_requant_fp8_cpu import global_scale
-from torchstore_b200 import _native
 from torchstore_b200.direct_weight_sync import DirectWeightSyncDest, DirectWeightSyncSource
 
 pytestmark = pytest.mark.gpu
-DEV = "cuda:0"
-I8 = torch.int8
 DTYPES = (torch.bfloat16, torch.float16, torch.float32)
-KW = {"block": "block_scales", "channel": "channel_scales", "tensor": "tensor_scales"}
 GOLDEN = os.path.join(os.path.dirname(__file__), "golden")
 DQ_REGIMES = sorted(n for n, r in fp8_regimes.REGIMES.items() if fp8_regimes.WORKLOADS[r.workload].kind == "dequant")
-
-
-@pytest.fixture(scope="module", autouse=True)
-def _init():
-    _native.init()
-    yield
-
-
-def run(coro):
-    return asyncio.run(coro)
+_init = pytest.fixture(scope="module", autouse=True)(native_session)
 
 
 # ---- every regime in int8 ----------------------------------------------------------------------------
-@pytest.mark.parametrize("variant", qp_gpu.VARIANTS)
+@pytest.mark.parametrize("variant", quant_pull_regimes.VARIANTS)
 @pytest.mark.parametrize("regime", sorted(quant_pull_regimes.REGIMES))
 def test_quant_pull_regime(regime, variant):
-    qp_gpu.run_regime(regime, variant, dst_dtype=I8)
+    quant_pull_regimes.run_regime(regime, variant, dst_dtype=I8)
 
 
-@pytest.mark.parametrize("variant", sq_gpu.VARIANTS)
+@pytest.mark.parametrize("variant", source_quant_regimes.VARIANTS)
 @pytest.mark.parametrize("regime", sorted(source_quant_regimes.REGIMES))
 def test_source_regime(regime, variant):
-    sq_gpu.run_regime(regime, variant, quant_dtype=I8)
+    source_quant_regimes.run_regime(regime, variant, quant_dtype=I8)
 
 
 @pytest.mark.parametrize("name", sorted(source_quant_regimes.WORKLOADS))
 def test_source_workload_writes_nothing_outside_its_outputs(name):
-    sq_gpu.run_guarded(name, quant_dtype=I8)
+    source_quant_regimes.run_guarded(name, quant_dtype=I8)
 
 
-@pytest.mark.parametrize("variant", fp8_gpu.VARIANTS)
+@pytest.mark.parametrize("variant", fp8_regimes.VARIANTS)
 @pytest.mark.parametrize("regime", DQ_REGIMES)
 def test_dequant_regime(regime, variant):
-    fp8_gpu.run_regime(regime, variant, src_dtype=I8)
+    fp8_regimes.run_regime(regime, variant, src_dtype=I8)
 
 
 # ---- the rounding edges, route by route ----------------------------------------------------------------
@@ -118,7 +103,7 @@ def test_rounding_edges_of_a_quantising_pull(route, dtype):
     assert_told_apart(x, g)
     name = str(dtype)[6:]
     p = Pull(name, shape, split(shape, 2, -1), whole(shape), g)
-    pulled = qp_gpu.Pulled((p,), [x], dst_dtype=I8)
+    pulled = quant_pull_regimes.Pulled((p,), [x], dst_dtype=I8)
     try:
         pulled.pull()
         tables, _ = pulled.live_tables()
@@ -155,7 +140,7 @@ def test_rounding_edges_of_source_side_quantisation(route, dtype):
     w = source_quant_regimes.Workload((source_quant_regimes.Target(name, shape, g, 37, 70),), 0)
     src, handles, _ = register_one(w, x)
     try:
-        (units, tiles, _), _ = sq_gpu.live_tables(src, handles, w, I8)
+        (units, tiles, _), _ = source_quant_regimes.live_tables(src, handles, w, I8)
         assert (len(units) > 0 and len(tiles) == 0) if kind == "units" else (len(tiles) > 0 and len(units) == 0)
         q, s, _ = src._quantized["t0"]
         with named(f"{route} {name}"):
@@ -169,7 +154,7 @@ def register_one(w, x):
     t = w.targets[0]
     src = DirectWeightSyncSource()
     sd = {"t0": x.to(DEV)}
-    handles = src.register(sd, rank=0, tensor_slices={"t0": sq_gpu.local_slice(t.shape, t.row0, t.col0)},
+    handles = src.register(sd, rank=0, tensor_slices={"t0": source_quant_regimes.local_slice(t.shape, t.row0, t.col0)},
                            quantize={"t0": t.granularity}, quant_dtype=I8)
     return src, handles, sd
 
@@ -181,7 +166,7 @@ def int8_pull(x, g):
     try:
         h = src.register({"w": x.to(DEV)}, rank=0)["w"]
         qb, q = guarded(tuple(x.shape), I8)
-        sb, s = guarded(quant_pull_regimes.scale_shape(g, tuple(x.shape)), torch.float32)
+        sb, s = guarded(dest_scale_shape(g, tuple(x.shape)), torch.float32)
         sync = DirectWeightSyncDest()
         run(sync.pull({"w": [h]}, {"w": q}, **{KW[g]: {"w": s}}))
         assert sync._int8_block_plans or sync._int8_scaled_plans
@@ -214,7 +199,7 @@ def test_int8_source_fixture_as_staging(i):
     name, x, g, r0, c0 = SOURCE_CASES[i]
     src = DirectWeightSyncSource()
     try:
-        src.register({"w": x.to(DEV)}, rank=0, tensor_slices={"w": sq_gpu.local_slice(x.shape, r0, c0)}, quantize={"w": g},
+        src.register({"w": x.to(DEV)}, rank=0, tensor_slices={"w": source_quant_regimes.local_slice(x.shape, r0, c0)}, quantize={"w": g},
                      quant_dtype=I8)
         q, s, _ = src._quantized["w"]
         assert i8s.digest(q.view(torch.uint8).cpu().numpy()) == str(d[f"q_sha{i}"]), name
@@ -227,7 +212,7 @@ def test_int8_source_fixture_as_staging(i):
 def dequant_pull(q, s, g, r0, c0, dtype):
     """An int8 handle q (scale s) at global (r0, c0) pulled whole into a guarded `dtype` destination -> y."""
     src = DirectWeightSyncSource()
-    sl = sq_gpu.local_slice(tuple(q.shape), r0, c0)
+    sl = source_quant_regimes.local_slice(tuple(q.shape), r0, c0)
     try:
         h = src.register({"w": q.to(DEV)}, rank=0, tensor_slices={"w": sl}, **{KW[g]: {"w": s.to(DEV)}})["w"]
         base, y = guarded(tuple(q.shape), dtype)
@@ -300,7 +285,7 @@ def test_int8_quantising_pull_past_byte_2_32():
         h = src.register({"w": x}, rank=0)["w"]
         for g in i8.GRANULARITIES:
             qb, q = guarded(BIG, I8)
-            sb, s = guarded(quant_pull_regimes.scale_shape(g, BIG), torch.float32)
+            sb, s = guarded(dest_scale_shape(g, BIG), torch.float32)
             sync = DirectWeightSyncDest()
             run(sync.pull({"w": [h]}, {"w": q}, **{KW[g]: {"w": s}}))
             for e in (0, 127, 128):
@@ -350,8 +335,9 @@ def test_int8_dequantising_pull_past_byte_2_32():
     for e in range(BIG[0]):
         q[e] = torch.randint(-128, 128, BIG[1:], dtype=I8, device=DEV, generator=gen)
     s = global_scale("channel", BIG, 17).to(DEV)
-    sources, handles = register(q, s, "channel", [whole(BIG)])
-    sync, y, base = fp8_gpu.dq_gpu.pull_into(handles, BIG, whole(BIG), torch.bfloat16)
+    sources, handles = register_boxes(q, [whole(BIG)], granularity="channel",
+                                      scale_of=partial(dq_local_scale, s, "channel"))
+    sync, y, _, (base,) = pull_box(handles, BIG, whole(BIG), torch.bfloat16)
     try:
         assert sync._int8_dequant_plans
         for e in (0, 127, 128):
@@ -367,19 +353,19 @@ def test_int8_dequantising_pull_past_byte_2_32():
 # ---- random layouts ----------------------------------------------------------------------------------
 @pytest.mark.parametrize("seed", range(24, 48))
 def test_random_layouts_with_special_values(seed):
-    qp_gpu.run_random_layout(seed, dst_dtype=I8)
+    quant_pull_regimes.run_random_layout(seed, dst_dtype=I8)
 
 
 @pytest.mark.parametrize("seed", range(24))
 def test_random_dequant_layouts_from_int8_handles(seed):
-    w = fp8_gpu.draw(random.Random(9800 + seed), "dequant", seed)
-    q, s = fp8_gpu.inputs(w, "finite", I8)
-    sources, handles = register(q, s, w.sg, list(w.src))
-    sync, y, base = fp8_gpu.dq_gpu.pull_into(handles, w.shape, w.dst, fp8_gpu.DST[w.out])
+    w = fp8_regimes.draw(random.Random(9800 + seed), "dequant", seed)
+    q, s = fp8_regimes.inputs(w, "finite", I8)
+    sources, handles = register_boxes(q, list(w.src), granularity=w.sg, scale_of=partial(dq_local_scale, s, w.sg))
+    sync, y, _, (base,) = pull_box(handles, w.shape, w.dst, fp8_regimes.DST[w.out])
     try:
         with named(f"seed {seed}: {w.describe()}"):
-            fp8_gpu.live_tables(sync, y, int8_src=True)
-            fp8_gpu.assert_int8_dequantised(y, q, s, w.sg, w.dst)
+            fp8_regimes.live_tables(sync, y, int8_src=True)
+            fp8_regimes.assert_int8_dequantised(y, q, s, w.sg, w.dst)
             assert guards_intact(base)
     finally:
         sync.close()

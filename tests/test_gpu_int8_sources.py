@@ -7,8 +7,6 @@ that need no oracle: source-side int8 + verbatim pull equals the destination-sid
 the groups coincide, and source-side int8 of an unsharded tensor equals the destination-side pull from it.  Several
 "ranks" are emulated as several sources on cuda:0."""
 
-import asyncio
-
 import numpy as np
 import pytest
 import torch
@@ -16,18 +14,12 @@ import torch
 from oracle.int8_oracle import SPECIALS, same_scales, special_stack
 from oracle.int8_source_oracle import (GRANULARITIES, bits_of, int8_of, quantize, scale_of, scale_shape, synth_f32,
                                        torch_dequantize, torch_quantize, widen)
+from tests.helpers import DEV, E4M3, I8, KW, cleanup, needs_two_gpus, register_boxes, register_shards, run
 from torchstore_b200.direct_weight_sync import DirectWeightSyncDest, DirectWeightSyncSource
 from torchstore_b200.transport.types import TensorSlice
 
 pytestmark = pytest.mark.gpu
-DEV = "cuda:0"
-E4M3 = torch.float8_e4m3fn
 DTYPES = (torch.bfloat16, torch.float16, torch.float32)
-KW = {"block": "block_scales", "channel": "channel_scales", "tensor": "tensor_scales"}
-
-
-def run(coro):
-    return asyncio.run(coro)
 
 
 def rows(shape, cuts):
@@ -44,37 +36,6 @@ def cols(shape, cuts):
 
 def box(full, off, loc):
     return full[tuple(slice(o, o + e) for o, e in zip(off, loc))]
-
-
-def quantise_sources(full, boxes, g, name="w", device=DEV, quant_dtype=torch.int8):
-    """One source per box of `full`, each quantised on its device -> (sources, handles, shards)."""
-    sources, handles, shards = [], [], []
-    for r, (off, loc) in enumerate(boxes):
-        shard = box(full, off, loc).contiguous().to(device)
-        ts = TensorSlice(tuple(off), (r,), tuple(full.shape), tuple(loc), (len(boxes),))
-        src = DirectWeightSyncSource()
-        handles.append(src.register({name: shard}, rank=r, tensor_slices={name: ts}, quantize={name: g},
-                                    quant_dtype=quant_dtype)[name])
-        sources.append(src)
-        shards.append(shard)
-    return sources, handles, shards
-
-
-def checkpoint_sources(q, scales, boxes, g, name="w"):
-    """One source per box of an int8 checkpoint `q`, registered with its shard-local scale -> (sources, handles)."""
-    sources, handles = [], []
-    for r, ((off, loc), s) in enumerate(zip(boxes, scales)):
-        shard = box(q, off, loc).contiguous().to(DEV)
-        ts = TensorSlice(tuple(off), (r,), tuple(q.shape), tuple(loc), (len(boxes),))
-        src = DirectWeightSyncSource()
-        handles.append(src.register({name: shard}, rank=r, tensor_slices={name: ts}, **{KW[g]: {name: s.to(DEV)}})[name])
-        sources.append(src)
-    return sources, handles
-
-
-def cleanup(sources):
-    for src in sources:
-        run(src.cleanup())
 
 
 def staging(src, name="w"):
@@ -107,8 +68,8 @@ LAYOUTS = {  # shape, boxes: FSDP row shards cut mid-block, unaligned column sha
 def test_source_side_int8_is_exact(g, dtype, layout):
     shape, boxes = LAYOUTS[layout]
     full = synth_f32(shape, 301 + len(layout)).to(dtype)
-    sources, handles, shards = quantise_sources(full, boxes(shape), g)
-    for src, shard, (off, _) in zip(sources, shards, boxes(shape)):
+    sources, handles = register_boxes(full, boxes(shape), quantize={"w": g}, quant_dtype=I8)
+    for (src, shard, _), (off, _) in zip(sources, boxes(shape)):
         assert_staging_exact(src, shard, g, off[-2], off[-1])
         assert src._handles["w"].rdma_buffer.dtype == torch.int8
     cleanup(sources)
@@ -118,9 +79,10 @@ def test_source_side_int8_is_exact(g, dtype, layout):
 @pytest.mark.parametrize("g", GRANULARITIES)
 def test_nan_inf_zero_and_tie_groups(g, dtype):
     full = special_stack(dtype)
-    sources, _, shards = quantise_sources(full, [((0, 0, 0), tuple(full.shape))], g)
-    assert_staging_exact(sources[0], shards[0], g, 0, 0)
-    q, s = staging(sources[0])
+    sources, _ = register_boxes(full, [((0, 0, 0), tuple(full.shape))], quantize={"w": g}, quant_dtype=I8)
+    src, shard, _ = sources[0]
+    assert_staging_exact(src, shard, g, 0, 0)
+    q, s = staging(src)
     for k, kind in enumerate(SPECIALS):
         if kind in ("nan", "inf", "nan_inf"):
             assert (q[k] == 0).all() and (torch.isinf(s[k]) if kind == "inf" else torch.isnan(s[k])).all()
@@ -132,8 +94,8 @@ def test_two_pass_paths(dtype):
     shape = (3, 16400 if dtype != torch.float32 else 8200)  # rows over the 32 KiB stage
     full = synth_f32(shape, 9).to(dtype)
     for g in ("channel", "tensor"):
-        sources, _, shards = quantise_sources(full, rows(shape, (1,)), g)
-        for src, shard, off in zip(sources, shards, (0, 1)):
+        sources, _ = register_boxes(full, rows(shape, (1,)), quantize={"w": g}, quant_dtype=I8)
+        for (src, shard, _), off in zip(sources, (0, 1)):
             assert_staging_exact(src, shard, g, off, 0)
         cleanup(sources)
 
@@ -142,13 +104,13 @@ def test_refresh_after_the_weights_change():
     shape = (300, 260)
     full = synth_f32(shape, 12).to(torch.bfloat16)
     for g in GRANULARITIES:
-        sources, _, shards = quantise_sources(full, rows(shape, (100,)), g)
+        sources, _ = register_boxes(full, rows(shape, (100,)), quantize={"w": g}, quant_dtype=I8)
         for k in range(2):
-            for shard in shards:
+            for _, shard, _ in sources:
                 shard.mul_(3.0 if k else 0.25)
-            for src in sources:
+            for src, *_ in sources:
                 assert src.refresh() == 1
-            for src, shard, r0 in zip(sources, shards, (0, 100)):
+            for (src, shard, _), r0 in zip(sources, (0, 100)):
                 assert_staging_exact(src, shard, g, r0, 0)
         cleanup(sources)
 
@@ -162,7 +124,8 @@ def test_int8_checkpoints_dequantise_across_reshards(g, dst):
     q = int8_of(shape, 21)
     boxes = rows(shape, (75, 200))
     scales = [scale_of(scale_shape(g, loc, off[-2], off[-1]), 30 + i) for i, (off, loc) in enumerate(boxes)]
-    sources, handles = checkpoint_sources(q, scales, boxes, g)
+    shards = [(off, box(q, off, loc).contiguous(), s) for (off, loc), s in zip(boxes, scales)]
+    sources, handles = register_shards(shape, shards, granularity=g)
     want = torch.cat([torch_dequantize(box(q, off, loc).to(DEV), s.to(DEV), g, off[-2], off[-1], dst)
                       for (off, loc), s in zip(boxes, scales)], dim=-2)
     for c0, c1 in ((0, 200), (200, 520)):
@@ -206,9 +169,9 @@ def test_verbatim_int8_chain(g):
         src_boxes, tp = cols(shape, ()), ((0, 128), (128, 384))
     else:
         src_boxes, tp = rows(shape, (128, 384)), ((0, 256), (256, 384))
-    sources, handles, _ = quantise_sources(full, src_boxes, g)
+    sources, handles = register_boxes(full, src_boxes, quantize={"w": g}, quant_dtype=I8)
     want = torch.cat([torch_dequantize(*staging(src), g, off[0], off[1], torch.bfloat16)
-                      for src, (off, _) in zip(sources, src_boxes)])
+                      for (src, *_), (off, _) in zip(sources, src_boxes)])
     for c0, c1 in tp:
         ts = TensorSlice((0, c0), (0,), shape, (512, c1 - c0), (2,))
         q, s = verbatim_pull(handles, (512, c1 - c0), g, ts)
@@ -228,15 +191,15 @@ def test_unsharded_source_side_int8_equals_the_destination_side_pull(g):
     """Cross-check (b): with one group layout on both sides the two quantisers write the same bytes and scales."""
     shape = (3, 300, 260)
     full = synth_f32(shape, 51).to(torch.bfloat16)
-    sources, handles, _ = quantise_sources(full, [((0, 0, 0), shape)], g)
+    sources, handles = register_boxes(full, [((0, 0, 0), shape)], quantize={"w": g}, quant_dtype=I8)
     plain = DirectWeightSyncSource()
     ph = plain.register({"w": full.to(DEV)}, rank=0)["w"]
     dq, ds = quantising_pull([ph], shape, g)
-    sq, ss = staging(sources[0])
+    sq, ss = staging(sources[0][0])
     assert torch.equal(sq, dq) and torch.equal(ss.view(torch.int32), ds.reshape(ss.shape).view(torch.int32))
     vq, vs = verbatim_pull(handles, shape, g)
     assert torch.equal(vq, dq) and torch.equal(vs.view(torch.int32), ds.view(torch.int32))
-    cleanup(sources + [plain])
+    cleanup(sources + [(plain,)])
 
 
 def test_mixed_pull_of_fp8_int8_quantising_and_plain_names():
@@ -244,12 +207,13 @@ def test_mixed_pull_of_fp8_int8_quantising_and_plain_names():
     fulls = {n: synth_f32(shape, 60 + i).to(torch.bfloat16) for i, n in enumerate(("f8", "i8", "i8v", "qz", "plain"))}
     sources, handles, by_name = [], {}, {}
     for n, qd in (("f8", E4M3), ("i8", torch.int8), ("i8v", torch.int8)):
-        by_name[n], handles[n], _ = quantise_sources(fulls[n], rows(shape, (128,)), "block", name=n, quant_dtype=qd)
+        by_name[n], handles[n] = register_boxes(fulls[n], rows(shape, (128,)), name=n, quantize={n: "block"},
+                                                quant_dtype=qd)
         sources += by_name[n]
     for n in ("qz", "plain"):
         src = DirectWeightSyncSource()
         handles[n] = [src.register({n: fulls[n].to(DEV)}, rank=0)[n]]
-        sources.append(src)
+        sources.append((src,))
     dests = {"f8": torch.zeros(shape, dtype=torch.bfloat16, device=DEV),
              "i8": torch.zeros(shape, dtype=torch.float32, device=DEV),
              "i8v": torch.zeros(shape, dtype=torch.int8, device=DEV),
@@ -263,9 +227,9 @@ def test_mixed_pull_of_fp8_int8_quantising_and_plain_names():
 
         for n, dt in (("f8", torch.bfloat16), ("i8", torch.float32)):
             want = torch.cat([(fp8_dequantize if n == "f8" else torch_dequantize)(*staging(src, n), "block", r0, 0, dt)
-                              for src, r0 in zip(by_name[n], (0, 128))])
+                              for (src, *_), r0 in zip(by_name[n], (0, 128))])
             assert torch.equal(dests[n].view(torch.uint8), want.view(torch.uint8)), n
-        vq = torch.cat([staging(src, "i8v")[0] for src in by_name["i8v"]])
+        vq = torch.cat([staging(src, "i8v")[0] for src, *_ in by_name["i8v"]])
         assert torch.equal(dests["i8v"], vq)
         tq, ts = torch_quantize(fulls["qz"].to(DEV), "block")
         assert torch.equal(dests["qz"], tq) and torch.equal(bs["qz"].view(torch.int32), ts.view(torch.int32))
@@ -313,7 +277,7 @@ def test_state_dict_api():
 def test_refusals_on_the_device():
     shape = (128, 256)
     full = synth_f32(shape, 81).to(torch.bfloat16)
-    sources, handles, _ = quantise_sources(full, [((0, 0), shape)], "channel")
+    sources, handles = register_boxes(full, [((0, 0), shape)], quantize={"w": "channel"}, quant_dtype=I8)
     s = torch.zeros(128, 1, device=DEV)
     for kw in ({}, {"requantize": True}):
         with pytest.raises(TypeError, match="verbatim=True"):
@@ -325,8 +289,8 @@ def test_refusals_on_the_device():
                                             channel_scales={"w": s}, **kw))
     raw = torch.zeros(shape, dtype=torch.int8, device=DEV)  # not in a scale dict: the raw int8 bytes
     run(DirectWeightSyncDest().pull({"w": handles}, {"w": raw}))
-    assert torch.equal(raw, staging(sources[0])[0])
-    f8s, f8h, _ = quantise_sources(full, [((0, 0), shape)], "channel", quant_dtype=E4M3)
+    assert torch.equal(raw, staging(sources[0][0])[0])
+    f8s, f8h = register_boxes(full, [((0, 0), shape)], quantize={"w": "channel"}, quant_dtype=E4M3)
     with pytest.raises(ValueError, match="mix scaled int8 and scaled fp8"):
         run(DirectWeightSyncDest().pull({"w": handles + f8h}, {"w": torch.zeros(shape, device=DEV)}))
     with pytest.raises(ValueError, match="int8 staging"):
@@ -335,7 +299,7 @@ def test_refusals_on_the_device():
     cleanup(sources + f8s)
 
 
-@pytest.mark.skipif(torch.cuda.device_count() < 2, reason="needs two GPUs")
+@needs_two_gpus
 @pytest.mark.parametrize("g", GRANULARITIES)
 def test_fsdp_to_tp_over_peer_mappings(g):
     """Int8 staging quantised on cuda:0 and cuda:1 (FSDP(2) row shards), dequantised into TP(2) bf16 column shards
@@ -344,11 +308,11 @@ def test_fsdp_to_tp_over_peer_mappings(g):
     full = synth_f32(shape, 91).to(torch.bfloat16)
     sources, handles = [], []
     for r, (off, loc) in enumerate(rows(shape, (256,))):
-        s, h, _ = quantise_sources(full, [(off, loc)], g, device=f"cuda:{r}")
+        s, h = register_boxes(full, [(off, loc)], device=f"cuda:{r}", quantize={"w": g}, quant_dtype=I8)
         sources += s
         handles += h
     want = torch.cat([torch_dequantize(*staging(src), g, r0, 0, torch.bfloat16).to(DEV)
-                      for src, r0 in zip(sources, (0, 256))])
+                      for (src, *_), r0 in zip(sources, (0, 256))])
     for t in range(2):
         dev = f"cuda:{t}"
         c0, c1 = t * 384, (t + 1) * 384
@@ -360,7 +324,7 @@ def test_fsdp_to_tp_over_peer_mappings(g):
         d.close()
         if g == "block":
             q, s = verbatim_pull(handles, (512, 384), g, ts, device=dev)
-            want_q = torch.cat([staging(src)[0].to(DEV) for src in sources])[:, c0:c1]
+            want_q = torch.cat([staging(src)[0].to(DEV) for src, *_ in sources])[:, c0:c1]
             assert torch.equal(q.cpu(), want_q.cpu())
     cleanup(sources)
 
@@ -404,8 +368,8 @@ def test_llama3_8b_fsdp8_to_tp8_full_size(g):
         for n in names:
             quant_h[n].append(qh[n])
             plain_h[n].append(ph[n])
-        sources += [qs, ps]
-    staged = {n: torch.cat([src._quantized[n][0] for src in sources[::2]]) for n in names}
+        sources += [(qs,), (ps,)]
+    staged = {n: torch.cat([src._quantized[n][0] for (src,) in sources[::2]]) for n in names}
     for t in range(8):
         dests, scales, ref_d, ref_s, tsl = {}, {}, {}, {}, {}
         for n, shape in names.items():
@@ -424,7 +388,7 @@ def test_llama3_8b_fsdp8_to_tp8_full_size(g):
         d.close()
         ref.close()
     for n in names:  # the staging itself against the torch-CUDA rendering, shard by shard
-        for r, src in enumerate(sources[::2]):
+        for r, (src,) in enumerate(sources[::2]):
             (r0, c0), _ = fsdp_boxes(names[n])[r]
             tq, ts = torch_quantize(box(fulls[n], *fsdp_boxes(names[n])[r]), g, r0, c0)
             q, s = src._quantized[n][:2]

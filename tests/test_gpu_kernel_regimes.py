@@ -14,82 +14,18 @@ import pytest
 import torch
 
 from oracle import c_oracle
-from tests.helpers import (KIND_B16, KIND_F32_BF16, KIND_GENERIC, MODE_B16, MODE_F32_BF16_V8, VECTOR_CAST_MODES,
-                           assert_equal_modulo_nan, edge_coverage, edge_workload, materialise, plan_kind,
-                           rect_fields, rects_for)
+from tests.helpers import (KERNEL_REGIMES, KIND_B16, KIND_F32_BF16, KIND_GENERIC, MODE_B16, MODE_F32_BF16_V8,
+                           VECTOR_CAST_MODES, assert_equal_modulo_nan, assert_same_bits_or_nan, compiled, edge_coverage,
+                           edge_workload, materialise, native_session, plan_kind, rects_for, run_plan, set_knobs)
 from torchstore_b200 import _native
 
 pytestmark = pytest.mark.gpu
 
-KNOBS = ("TSB_TILE_BYTES", "TSB_STATIC_SCHED", "TSB_MAX_GRID", "TSB_FORCE_GENERIC", "TSB_LINK", "TSB_LINK_STAGES",
-         "TSB_LINK_STAGE_BYTES", "TSB_CTAS_PER_SM")
 GUARD = 0xA5
-
-
-@pytest.fixture(scope="module", autouse=True)
-def _init():
-    _native.init()
-    yield
-    torch.cuda.synchronize()
-    torch.cuda.empty_cache()
-
-
-def set_knobs(monkeypatch, **knobs):
-    for k in KNOBS:
-        monkeypatch.delenv(k, raising=False)
-    for k, v in knobs.items():
-        if v is not None:
-            monkeypatch.setenv(k, str(v))
-
-
-def compiled(pairs):
-    """(rects, n, rect table fields, host PlanInfo) of `pairs` under the current knobs."""
-    rects, n = rects_for(pairs)
-    table, _, info = _native.plan_compile_host(0, rects, n, 0, 0)
-    return rects, n, rect_fields(table), info
-
-
-def run_plan(rects, n):
-    """Compile, run on torch's stream, wait, destroy; returns the plan's PlanInfo."""
-    plan = _native.plan_create(0, rects, n)
-    info = _native.plan_info(plan)
-    _native.plan_run(plan, _native.torch_stream(0))
-    torch.cuda.synchronize()
-    _native.plan_destroy(plan)
-    return info
-
-
-def assert_same_bits_or_nan(got: torch.Tensor, want: torch.Tensor):
-    """On the device: equal bits, or both NaN (the assert_equal_modulo_nan rule)."""
-    assert got.shape == want.shape and got.dtype == want.dtype
-    as_int = {1: torch.uint8, 2: torch.int16, 4: torch.int32, 8: torch.int64}[got.element_size()]
-    same = got.view(as_int) == want.view(as_int)
-    if got.is_floating_point():
-        same |= torch.isnan(got) & torch.isnan(want)
-    assert bool(same.all()), int((~same).sum())
+_init = pytest.fixture(scope="module", autouse=True)(native_session)
 
 
 # ---- regime matrix ------------------------------------------------------------------------------------
-# A covering design over (tile bytes, grid cap, scheduling, TSB_FORCE_GENERIC, TSB_LINK): every value of
-# every axis, and every (tile bytes, grid cap) pair.  Static scheduling only applies to plans without
-# link tiles, so it runs with TSB_LINK=1 on local sources.
-REGIMES = [
-    # tile bytes, grid cap, scheduling, force generic, TSB_LINK
-    (1024, None, "dynamic", False, 2),
-    (1024, 1, "static", True, 1),
-    (1024, 5, "dynamic", False, 1),
-    (4096, None, "static", False, 1),
-    (4096, 1, "dynamic", True, 2),
-    (4096, 5, "static", True, 1),
-    (65536, None, "dynamic", True, 1),
-    (65536, 1, "dynamic", False, 2),
-    (65536, 5, "static", False, 1),
-    (524288, None, "static", True, 1),
-    (524288, 1, "dynamic", False, 1),
-    (524288, 5, "dynamic", True, 2),
-]
-
-
 def _check_regime(workload, tile_bytes, cap, sched, link, fields, hinfo, info):
     T = tile_bytes // 16
     assert (info.num_tiles, info.num_link_tiles) == (hinfo.num_tiles, hinfo.num_link_tiles)
@@ -131,7 +67,7 @@ def test_edge_workloads_match_oracle_across_regimes(tile_bytes, workload, monkey
     c_oracle.copy_rects(hrects, hn, nan_mode=1)
     dev = materialise(cases, "cuda:0", seed)
     initial = [d[2].clone() for d in dev]
-    regimes = [r for r in REGIMES if r[0] == tile_bytes]
+    regimes = [r for r in KERNEL_REGIMES if r[0] == tile_bytes]
     assert {r[1] for r in regimes} == {None, 1, 5}
     for _, cap, sched, generic, link in regimes:
         set_knobs(monkeypatch, TSB_TILE_BYTES=tile_bytes, TSB_MAX_GRID=cap, TSB_LINK=link,

@@ -12,6 +12,8 @@ import pytest
 import torch
 import torch.multiprocessing as mp
 
+from tests.helpers import run
+
 pytestmark = pytest.mark.gpu
 
 
@@ -20,10 +22,6 @@ def _ngpu():
 
 
 needs2 = pytest.mark.skipif(_ngpu() < 2, reason="needs 2 GPUs")
-
-
-def run(coro):
-    return asyncio.run(coro)
 
 
 @needs2

@@ -3,42 +3,20 @@ fused qkv_proj / gate_up_proj and stacked MoE experts, checked bit for bit again
 rule and against the unfused pull of the same bytes, through every route (byte copy, fused casts, quantising,
 dequantising, requantising, verbatim), the plan cache and the public state-dict path."""
 
-import asyncio
-
 import numpy as np
 import pytest
 import torch
 
 import workloads
 from oracle import packed_oracle as po
-from tests.helpers import fsdp_handles, pull_args, region, unfused_args
-from torchstore_b200.direct_weight_sync import (DirectWeightSyncDest, DirectWeightSyncSource, NvlinkBuffer, PackedPart,
-                                                RDMAWeightHandle, source_scale_shapes)
+from tests.helpers import (DEV, E4M3, as_np, masters, needs_two_gpus, nv_handles, pull, pull_args, region, run,
+                           unfused_args, whole_handle)
+from torchstore_b200.direct_weight_sync import DirectWeightSyncDest, DirectWeightSyncSource, PackedPart, source_scale_shapes
 from torchstore_b200.transport.types import TensorSlice
 
 pytestmark = pytest.mark.gpu
-DEV = "cuda:0"
-E4M3 = torch.float8_e4m3fn
 LLAMA = workloads.LLAMA3_8B
 QWEN = workloads.QWEN3_MOE
-
-
-def run(coro):
-    return asyncio.run(coro)
-
-
-def masters(layout, seed, device=DEV):
-    g = torch.Generator(device).manual_seed(seed)
-    return {n: (torch.randn(shape, device=device, generator=g) * 0.02).to(torch.bfloat16)
-            for n, (shape, _) in layout.items()}
-
-
-def nv_handles(layout, n, full):
-    return fsdp_handles(layout, n, lambda name, off, loc: NvlinkBuffer(region(full[name], off, loc).contiguous()))
-
-
-def as_np(t):
-    return t.view({1: torch.uint8, 2: torch.int16, 4: torch.int32}[t.element_size()]).cpu().numpy()
 
 
 def fused(spec, shape, sources, dtype=None):
@@ -48,18 +26,6 @@ def fused(spec, shape, sources, dtype=None):
         box = out[p.dest_index]
         box.copy_(sources[p.source][tuple(slice(o, o + e) for o, e in zip(p.source_offsets, box.shape))])
     return out
-
-
-def whole_handle(t):
-    """One handle over the whole of ``t``."""
-    z = (0,) * t.dim()
-    return [RDMAWeightHandle(NvlinkBuffer(t.contiguous()), TensorSlice(z, (0,), tuple(t.shape), tuple(t.shape), (1,)), 0)]
-
-
-def pull(handles, dests, slices=None, **kw):
-    sync = DirectWeightSyncDest()
-    run(sync.pull(handles, dests, slices, **kw))
-    return sync
 
 
 # -- Llama-3 HF -> vLLM ---------------------------------------------------------------------------------------------
@@ -387,7 +353,7 @@ def test_get_state_dict_with_packed():
     run(main())
 
 
-@pytest.mark.skipif(not torch.cuda.is_available() or torch.cuda.device_count() < 2, reason="needs 2 GPUs")
+@needs_two_gpus
 def test_parts_read_over_peer_mappings():
     """Parts whose handles live on cuda:1 are read over NVLink by cuda:0's copy plan (the link queue)."""
     hf = workloads.hf_llama_layout(LLAMA, n_layers=1, scale=8, with_embeddings=False)

@@ -5,24 +5,18 @@ scales, sentinels outside every part untouched); random specs with special value
 a grouped pull refused for a hole and the same puller pulling the corrected spec; and parts landing past byte 2^32 of
 their destination."""
 
-import asyncio
-
 import numpy as np
 import pytest
 import torch
 
 from oracle import block_fp8_oracle, dequant_fp8_oracle, packed_oracle
 from tests import packed_regimes as pr
+from tests.helpers import DEV, needs_two_gpus, run
 from torchstore_b200.direct_weight_sync import (DirectWeightSyncDest, DirectWeightSyncSource, NvlinkBuffer, PackedPart,
                                                 RDMAWeightHandle, ScaledNvlinkBuffer, source_scale_shapes)
 from torchstore_b200.transport.types import TensorSlice
 
 pytestmark = pytest.mark.gpu
-DEV = "cuda:0"
-
-
-def run(coro):
-    return asyncio.run(coro)
 
 
 def make_buffer(device):
@@ -243,7 +237,7 @@ def test_block_quantising_part_past_4_gib():
 
 
 # ---- peer handles ---------------------------------------------------------------------------------------------------
-@pytest.mark.skipif(not torch.cuda.is_available() or torch.cuda.device_count() < 2, reason="needs 2 GPUs")
+@needs_two_gpus
 @pytest.mark.parametrize("route", ["copy_bf16", "quant_fp8_block_bfloat16", "dq_e4m3_block_bfloat16"])
 def test_sharded_sources_on_a_peer(route):
     """sharded_sources with every handle on cuda:1, read over the peer mapping by cuda:0's plans."""

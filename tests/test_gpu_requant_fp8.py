@@ -5,73 +5,26 @@ two-step product route (a dequantising pull into an f32 temporary, then a quanti
 bytes, aligned identity, a mixed pull with replay and rebuild, the state-dict API, peer-mapped sources and a
 full-size Llama-3-8B w1."""
 
-import asyncio
+from functools import partial
 
 import numpy as np
 import pytest
 import torch
 
 import torchstore_b200 as ts
-from oracle import ue8m0_oracle
 from oracle.dequant_fp8_oracle import GRANULARITIES, SCALE_SET, scale_shape, torch_dequantize
-from oracle.requant_fp8_oracle import PAIRS, quantize, requantize, torch_requantize
-from tests.helpers import region, shard_box
-from tests.test_gpu_dequant_fp8 import KW, cleanup, guarded, guards_intact, register
-from tests.test_requant_fp8_cpu import dest_scale_shape, fp8_full, global_scale, local_scale
+from oracle.requant_fp8_oracle import PAIRS, quantize, torch_requantize
+from tests.fp8_regimes import assert_requant_oracle, assert_requant_torch_cuda
+from tests.helpers import (DEV, E4M3, KW, cleanup, dest_scale_shape, guards_intact, native_session, needs_two_gpus,
+                           pull_box, register_boxes, run, shard_box)
+from tests.test_dequant_fp8_cpu import local_scale as dq_local_scale
+from tests.test_requant_fp8_cpu import fp8_full, global_scale
 from torchstore_b200 import _native
 from torchstore_b200.direct_weight_sync import DirectWeightSyncDest, DirectWeightSyncSource
 from torchstore_b200.transport.types import TensorSlice
 
 pytestmark = pytest.mark.gpu
-DEV = "cuda:0"
-E4M3 = torch.float8_e4m3fn
-
-
-@pytest.fixture(scope="module", autouse=True)
-def _init():
-    _native.init()
-    yield
-
-
-def run(coro):
-    return asyncio.run(coro)
-
-
-def pull_into(handles, full_shape, box, dg, sync=None, device=DEV, scale_fmt=None):
-    """Requantising pull of `handles` into a guarded `dg`-scaled fp8 window `box` in the scale format `scale_fmt`
-    -> (sync, q, scale, guards)."""
-    off, loc = box
-    qbase, q = guarded(loc, E4M3, device)
-    sbase, s = guarded(dest_scale_shape(dg, loc), torch.float32, device)
-    sync = sync or DirectWeightSyncDest()
-    run(sync.pull({"w": handles}, {"w": q}, {"w": TensorSlice(off, (0,), tuple(full_shape), loc, (1,))},
-                  **{KW[dg]: {"w": s}}, requantize=True, scale_fmt=scale_fmt))
-    return sync, q, s, (qbase, sbase)
-
-
-def assert_torch_cuda(q, s, q_full, full_scale, sg, box, dg, scale_fmt=None):
-    """Bit-exact, NaN bytes included, against the torch CUDA composition of the same window."""
-    args = (region(q_full, *box).to(DEV), local_scale(full_scale, sg, *box).to(DEV), sg, box[0][-2], box[0][-1], dg)
-    want_q, want_s = ue8m0_oracle.torch_requantize(*args, scale_fmt=scale_fmt) if scale_fmt else torch_requantize(*args)
-    if scale_fmt:
-        ue8m0_oracle.assert_pow2_over(s, torch_requantize(*args)[1])
-    assert torch.equal(q.view(torch.uint8), want_q.view(torch.uint8))
-    got_s, want_s = s.reshape(-1), want_s.reshape(-1)
-    nan = torch.isnan(want_s)  # a NaN scale_inv's bits are torch's choice
-    assert torch.equal(torch.isnan(got_s), nan) and torch.equal(got_s[~nan].view(torch.int32), want_s[~nan].view(torch.int32))
-
-
-def assert_oracle(q, s, q_full, full_scale, sg, box, dg, scale_fmt=None):
-    """Bit-exact against the numpy composition wherever it is not NaN."""
-    args = (region(q_full, *box).view(torch.uint8).numpy(), local_scale(full_scale, sg, *box).numpy(), sg, box[0][-2],
-            box[0][-1], dg)
-    want_q, want_s = ue8m0_oracle.requantize(*args, scale_fmt=scale_fmt) if scale_fmt else requantize(*args)
-    got_q = q.view(torch.uint8).cpu().numpy()
-    nan = (want_q & 0x7F) == 0x7F
-    assert np.array_equal(got_q[~nan], want_q[~nan])
-    got_s, want_s = s.cpu().numpy().reshape(-1), np.asarray(want_s, np.float32).reshape(-1)
-    ok = ~np.isnan(want_s)
-    assert np.array_equal(got_s[ok].view(np.uint32), want_s[ok].view(np.uint32))
+_init = pytest.fixture(scope="module", autouse=True)(native_session)
 
 
 @pytest.mark.parametrize("sg,dg", PAIRS)
@@ -80,14 +33,15 @@ def test_reshard_matrix(sg, dg):
     columns each: not 128-aligned)."""
     q = fp8_full((700, 520), 31)
     s = global_scale(sg, q.shape, 31)
-    sources, handles = register(q, s, sg, [shard_box(q.shape, 6, r, 0) for r in range(6)])
+    sources, handles = register_boxes(q, [shard_box(q.shape, 6, r, 0) for r in range(6)], granularity=sg,
+                                      scale_of=partial(dq_local_scale, s, sg))
     for dst_dim in (0, 1):
         for d in range(2):
             box = shard_box(q.shape, 2, d, dst_dim)
-            sync, y, ys, bases = pull_into(handles, q.shape, box, dg)
+            sync, y, ys, bases = pull_box(handles, q.shape, box, E4M3, granularity=dg, requantize=True)
             assert sync._requant_plans and not (sync._dequant_plans or sync._block_plans or sync._scaled_plans)
-            assert_oracle(y, ys, q, s, sg, box, dg)
-            assert_torch_cuda(y, ys, q, s, sg, box, dg)
+            assert_requant_oracle(y, ys, q, s, sg, box, dg)
+            assert_requant_torch_cuda(y, ys, q, s, sg, box, dg)
             assert all(guards_intact(b) for b in bases)
             sync.close()
     cleanup(sources)
@@ -113,8 +67,8 @@ def test_differential_against_the_two_step_route(sg, dg):
     for q, s in (scale_set_input(sg), (fp8_full((3, 300, 260), 41), None)):
         s = s if s is not None else global_scale(sg, q.shape, 41)
         box = ((0,) * q.dim(), tuple(q.shape))
-        sources, handles = register(q, s, sg, [box])
-        sync, y, ys, _ = pull_into(handles, q.shape, box, dg)
+        sources, handles = register_boxes(q, [box], granularity=sg, scale_of=partial(dq_local_scale, s, sg))
+        sync, y, ys, _ = pull_box(handles, q.shape, box, E4M3, granularity=dg, requantize=True)
         tmp = torch.zeros(q.shape, device=DEV)
         run(DirectWeightSyncDest().pull({"w": handles}, {"w": tmp}))  # dequantising pull into f32
         back = DirectWeightSyncSource()
@@ -124,7 +78,7 @@ def test_differential_against_the_two_step_route(sg, dg):
         run(DirectWeightSyncDest().pull({"w": [h["w"]]}, {"w": y2}, **{KW[dg]: {"w": ys2}}))  # quantising pull
         assert torch.equal(y.view(torch.uint8), y2.view(torch.uint8))
         assert torch.equal(ys.view(torch.int32), ys2.view(torch.int32))
-        assert_torch_cuda(y, ys, q, s, sg, box, dg)
+        assert_requant_torch_cuda(y, ys, q, s, sg, box, dg)
         sync.close()
         run(back.cleanup())
         cleanup(sources)
@@ -137,8 +91,9 @@ def test_aligned_identity(g):
     q_np, s_np = quantize(x.numpy(), g)
     q = torch.from_numpy(q_np).view(E4M3)
     s = torch.from_numpy(np.asarray(s_np, np.float32).copy()).reshape(scale_shape(g, q.shape))
-    sources, handles = register(q, s, g, [shard_box(q.shape, 4, r, 1) for r in range(4)])
-    sync, y, ys, _ = pull_into(handles, q.shape, ((0, 0, 0), tuple(q.shape)), g)
+    sources, handles = register_boxes(q, [shard_box(q.shape, 4, r, 1) for r in range(4)], granularity=g,
+                                      scale_of=partial(dq_local_scale, s, g))
+    sync, y, ys, _ = pull_box(handles, q.shape, ((0, 0, 0), tuple(q.shape)), E4M3, granularity=g, requantize=True)
     assert torch.equal(y.view(torch.uint8).cpu(), q.view(torch.uint8))
     sync.close()
     cleanup(sources)
@@ -149,8 +104,10 @@ def test_mixed_pull_replay_and_rebuild():
     no rebuild; a new scale dict or a flipped requantize rebuilds."""
     q = fp8_full((300, 260), 51)
     s = global_scale("block", q.shape, 51)
-    dq_sources, dq_handles = register(q, s, "block", [shard_box(q.shape, 3, r, 0) for r in range(3)], name="dq")
-    rq_sources, rq_handles = register(q, s, "block", [shard_box(q.shape, 3, r, 0) for r in range(3)], name="rq")
+    dq_sources, dq_handles = register_boxes(q, [shard_box(q.shape, 3, r, 0) for r in range(3)], granularity="block",
+                                            scale_of=partial(dq_local_scale, s, "block"), name="dq")
+    rq_sources, rq_handles = register_boxes(q, [shard_box(q.shape, 3, r, 0) for r in range(3)], granularity="block",
+                                            scale_of=partial(dq_local_scale, s, "block"), name="rq")
     plain = (torch.randn(128, 64) * 0.1).to(torch.bfloat16)
     cast = (torch.randn(128, 96) * 0.1)
     master = (torch.randn(256, 256) * 0.1).to(torch.bfloat16)
@@ -232,21 +189,22 @@ def test_put_and_get_state_dict_requantise():
     run(main())
 
 
-@pytest.mark.skipif(not torch.cuda.is_available() or torch.cuda.device_count() < 2, reason="needs 2 GPUs")
+@needs_two_gpus
 @pytest.mark.parametrize("sg,dg", [("block", "channel"), ("channel", "block"), ("tensor", "tensor")])
 def test_weight_and_scale_read_over_peer_mappings(sg, dg):
     q = fp8_full((300, 520), 71)
     s = global_scale(sg, q.shape, 71)
     sources, handles = [], []
     for r, b in enumerate([shard_box(q.shape, 4, r, 0) for r in range(4)]):  # shards alternate between cuda:1 and cuda:0
-        s_, h_ = register(q, s, sg, [b], device=f"cuda:{1 - r % 2}")
+        s_, h_ = register_boxes(q, [b], granularity=sg, scale_of=partial(dq_local_scale, s, sg),
+                                device=f"cuda:{1 - r % 2}")
         sources += s_
         handles += h_
     for d in range(2):
         box = shard_box(q.shape, 2, d, 1)
-        sync, y, ys, bases = pull_into(handles, q.shape, box, dg)
+        sync, y, ys, bases = pull_box(handles, q.shape, box, E4M3, granularity=dg, requantize=True)
         assert _native.plan_info(sync._requant_plans[0]).remote_src_bytes > 0
-        assert_torch_cuda(y, ys, q, s, sg, box, dg)
+        assert_requant_torch_cuda(y, ys, q, s, sg, box, dg)
         assert all(guards_intact(b) for b in bases)
         sync.close()
     cleanup(sources)
@@ -262,8 +220,9 @@ def test_full_size_llama3_8b_w1():
     q, s = torch_quantize(x)
     del x
     boxes = [shard_box((rows, cols), 6, r, 0) for r in range(6)]
-    sources, handles = register(q, s, "block", boxes)
-    sync, y, ys, bases = pull_into(handles, (rows, cols), ((0, 0), (rows, cols)), "channel")
+    sources, handles = register_boxes(q, boxes, granularity="block", scale_of=partial(dq_local_scale, s, "block"))
+    sync, y, ys, bases = pull_box(handles, (rows, cols), ((0, 0), (rows, cols)), E4M3, granularity="channel",
+                                  requantize=True)
     want_q, want_s = torch_requantize(q, s, "block", 0, 0, "channel")
     assert torch.equal(y.view(torch.uint8), want_q.view(torch.uint8)) and torch.equal(ys, want_s)
     assert all(guards_intact(b) for b in bases)

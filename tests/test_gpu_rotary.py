@@ -11,15 +11,13 @@ import torch
 import workloads
 from oracle import packed_oracle as po
 from oracle import rotary_oracle as ro
-from tests.helpers import pull_args, region
-from tests.test_gpu_packed import as_np, masters, nv_handles, pull, run, whole_handle
+from tests.helpers import (DEV, E4M3, as_np, masters, needs_two_gpus, nv_handles, pull, pull_args, region, run,
+                           whole_handle)
 from torchstore_b200.direct_weight_sync import (DirectWeightSyncDest, DirectWeightSyncSource, PackedPart,
                                                 RDMAWeightHandle, source_scale_shapes)
 from torchstore_b200.transport.types import TensorSlice
 
 pytestmark = pytest.mark.gpu
-DEV = "cuda:0"
-E4M3 = torch.float8_e4m3fn
 LLAMA = workloads.LLAMA3_8B
 
 
@@ -262,7 +260,7 @@ def test_full_size_llama3_8b_one_rank():
     sync.close()
 
 
-@pytest.mark.skipif(not torch.cuda.is_available() or torch.cuda.device_count() < 2, reason="needs 2 GPUs")
+@needs_two_gpus
 def test_rotary_parts_read_over_peer_mappings():
     layout = titan(layout_scale=8, n_layers=1, with_embeddings=False)
     full = masters(layout, 81, device="cuda:1")

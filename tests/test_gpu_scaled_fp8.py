@@ -5,91 +5,29 @@ the formula (special values, NaN bytes included); both kernel paths, reshards, m
 and invalidation, the public state-dict API, validation before any launch, and peer-mapped sources on a
 second GPU."""
 
-import asyncio
-
 import numpy as np
 import pytest
 import torch
 
 import torchstore_b200 as ts
 from oracle.block_fp8_oracle import quantize as block_quantize
-from oracle.scaled_fp8_oracle import GRANULARITIES, quantize, torch_quantize
-from tests.helpers import rand_full, region, shard_box
-from tests.test_scaled_fp8_cpu import fixture_cases, scale_shape
+from oracle.scaled_fp8_oracle import GRANULARITIES, quantize
+from tests.helpers import (DEV, E4M3, cleanup, guards_intact, native_session, needs_two_gpus, pull_box, rand_full, region,
+                           register_boxes, run, shard_box)
+from tests.quant_pull_regimes import assert_scaled_torch_cuda
+from tests.test_scaled_fp8_cpu import fixture_cases
 from torchstore_b200 import _native
 from torchstore_b200.direct_weight_sync import DirectWeightSyncDest, DirectWeightSyncSource
 from torchstore_b200.transport.types import TensorSlice
 
 pytestmark = pytest.mark.gpu
-DEV = "cuda:0"
-E4M3 = torch.float8_e4m3fn
-GUARD = 0x5A
-LEAD = 256
-KW = {"channel": "channel_scales", "tensor": "tensor_scales"}
-
-
-@pytest.fixture(scope="module", autouse=True)
-def _init():
-    _native.init()
-    yield
-
-
-def run(coro):
-    return asyncio.run(coro)
-
-
-def guarded(shape, dtype, device=DEV):
-    """A contiguous tensor of `shape` inside a guard-filled byte buffer (LEAD bytes before, LEAD after)."""
-    n = int(np.prod(shape, dtype=np.int64)) * dtype.itemsize
-    base = torch.full((n + 2 * LEAD,), GUARD, dtype=torch.uint8, device=device)
-    return base, base[LEAD: LEAD + n].view(dtype).view(shape)
-
-
-def guards_intact(base):
-    return bool((base[:LEAD] == GUARD).all()) and bool((base[-LEAD:] == GUARD).all())
-
-
-def register(full, boxes, device=DEV, **kw):
-    """One DirectWeightSyncSource per box of `full` (plain shards with tensor_slices)."""
-    sources, handles = [], []
-    for r, (off, loc) in enumerate(boxes):
-        if 0 in loc:
-            continue
-        src = DirectWeightSyncSource()
-        shard = region(full, off, loc).contiguous().to(device)
-        sl = TensorSlice(off, (r,), tuple(full.shape), loc, (len(boxes),))
-        handles.append(src.register({"w": shard}, rank=r, tensor_slices={"w": sl}, **kw)["w"])
-        sources.append((src, shard))
-    return sources, handles
-
-
-def cleanup(sources):
-    for src, _ in sources:
-        run(src.cleanup())
-
-
-def pull_into(handles, full_shape, dst_box, g, sync=None):
-    off, loc = dst_box
-    qb, q = guarded(loc, E4M3)
-    sb, s = guarded(scale_shape(loc, g), torch.float32)
-    sync = sync or DirectWeightSyncDest()
-    dsl = TensorSlice(off, (0,), tuple(full_shape), loc, (1,))
-    run(sync.pull({"w": handles}, {"w": q}, {"w": dsl}, **{KW[g]: {"w": s}}))
-    return sync, q, s, qb, sb
+_init = pytest.fixture(scope="module", autouse=True)(native_session)
 
 
 def assert_oracle(q, s, x_f32, g):
     want_q, want_s = quantize(x_f32, g)
     assert np.array_equal(q.view(torch.uint8).cpu().numpy(), want_q)
     assert np.array_equal(s.cpu().numpy().view(np.uint32), want_s.view(np.uint32))
-
-
-def assert_torch_cuda(q, s, x, g):
-    want_q, want_s = torch_quantize(x.to(DEV), g)
-    assert torch.equal(q.view(torch.uint8), want_q.view(torch.uint8))  # NaN bytes included
-    both_nan = torch.isnan(s) & torch.isnan(want_s)
-    assert torch.equal(torch.isnan(s), torch.isnan(want_s))
-    assert torch.equal(s.view(torch.int32)[~both_nan], want_s.view(torch.int32)[~both_nan])
 
 
 FINITE = [c for c in fixture_cases() if "nonfinite" not in c[0]]
@@ -100,8 +38,8 @@ def test_exact_match_pull_of_the_fixture_shapes(case):
     _, g, dtype, x, _, _ = case
     full = torch.from_numpy(x).to(getattr(torch, dtype))
     shape = tuple(full.shape)
-    sources, handles = register(full, [(tuple(0 for _ in shape), shape)])
-    sync, q, s, qb, sb = pull_into(handles, shape, (tuple(0 for _ in shape), shape), g)
+    sources, handles = register_boxes(full, [(tuple(0 for _ in shape), shape)])
+    sync, q, s, (qb, sb) = pull_box(handles, shape, (tuple(0 for _ in shape), shape), E4M3, granularity=g)
     assert_oracle(q, s, x, g)
     assert guards_intact(qb) and guards_intact(sb)
     sync.close()
@@ -114,9 +52,9 @@ def test_special_value_groups_match_torch_cuda_bit_for_bit(case):
     _, g, dtype, x, _, _ = case
     full = torch.from_numpy(x).to(getattr(torch, dtype))
     shape = tuple(full.shape)
-    sources, handles = register(full, [((0, 0), shape)])
-    sync, q, s, _, _ = pull_into(handles, shape, ((0, 0), shape), g)
-    assert_torch_cuda(q, s, full, g)
+    sources, handles = register_boxes(full, [((0, 0), shape)])
+    sync, q, s, _ = pull_box(handles, shape, ((0, 0), shape), E4M3, granularity=g)
+    assert_scaled_torch_cuda(q, s, full, g)
     sync.close()
     cleanup(sources)
 
@@ -127,8 +65,8 @@ def test_rows_inside_and_beyond_the_stage_bound(dtype, cols):
     """Rows of at most 32 KiB take the row-staged kernel, longer ones the two-pass one; 16401 is ragged."""
     full = rand_full((12, cols), dtype, cols)
     boxes = [shard_box(full.shape, 3, r, 1) for r in range(3)]  # unaligned column shards
-    sources, handles = register(full, boxes)
-    sync, q, s, qb, sb = pull_into(handles, full.shape, ((0, 0), tuple(full.shape)), "channel")
+    sources, handles = register_boxes(full, boxes)
+    sync, q, s, (qb, sb) = pull_box(handles, full.shape, ((0, 0), tuple(full.shape)), E4M3, granularity="channel")
     info = _native.plan_info(sync._scaled_plans[0])
     staged = cols * full.element_size() <= 32768
     assert (info.num_tiles <= 12) == staged  # at most one band per row vs a tile per row and shard
@@ -142,10 +80,10 @@ def test_rows_inside_and_beyond_the_stage_bound(dtype, cols):
 @pytest.mark.parametrize("n,dst_dim", [(4, 0), (4, 1), (3, 1)])
 def test_fsdp_to_tp_reshard(g, n, dst_dim):
     full = rand_full((1000, 520), torch.bfloat16, 10 * n + dst_dim)  # per tensor: several tiles per shard
-    sources, handles = register(full, [shard_box(full.shape, n, r, 0) for r in range(n)])
+    sources, handles = register_boxes(full, [shard_box(full.shape, n, r, 0) for r in range(n)])
     for d in range(n):
         dst = shard_box(full.shape, n, d, dst_dim)
-        sync, q, s, qb, sb = pull_into(handles, full.shape, dst, g)
+        sync, q, s, (qb, sb) = pull_box(handles, full.shape, dst, E4M3, granularity=g)
         assert_oracle(q, s, region(full, *dst).float().numpy(), g)
         assert guards_intact(qb) and guards_intact(sb)
         sync.close()
@@ -155,10 +93,10 @@ def test_fsdp_to_tp_reshard(g, n, dst_dim):
 @pytest.mark.parametrize("g", GRANULARITIES)
 def test_moe_stack(g):
     full = rand_full((3, 130, 260), torch.float32, 5)
-    sources, handles = register(full, [shard_box(full.shape, 3, r, 1) for r in range(3)])
+    sources, handles = register_boxes(full, [shard_box(full.shape, 3, r, 1) for r in range(3)])
     for d in range(2):
         dst = shard_box(full.shape, 2, d, 2)
-        sync, q, s, _, _ = pull_into(handles, full.shape, dst, g)
+        sync, q, s, _ = pull_box(handles, full.shape, dst, E4M3, granularity=g)
         assert_oracle(q, s, region(full, *dst).float().numpy(), g)
         sync.close()
     cleanup(sources)
@@ -166,7 +104,7 @@ def test_moe_stack(g):
 
 def test_per_tensor_scale_shapes_with_a_trailing_one():
     full = rand_full((2, 300, 200), torch.bfloat16, 9)
-    sources, handles = register(full, [((0, 0, 0), (2, 300, 200))])
+    sources, handles = register_boxes(full, [((0, 0, 0), (2, 300, 200))])
     q = torch.zeros(2, 300, 200, dtype=E4M3, device=DEV)
     s = torch.zeros(2, 1, device=DEV)  # compressed-tensors keeps [E, 1]; vLLM [E]
     sync = DirectWeightSyncDest()
@@ -205,9 +143,9 @@ def test_mixed_dict_of_plain_block_channel_and_tensor_names():
 
 def test_replay_refresh_and_invalidation():
     full = rand_full((300, 260), torch.bfloat16, 5)
-    sources, handles = register(full, [shard_box(full.shape, 4, r, 0) for r in range(4)])
+    sources, handles = register_boxes(full, [shard_box(full.shape, 4, r, 0) for r in range(4)])
     dst = shard_box(full.shape, 2, 1, 1)
-    sync, q, s, _, _ = pull_into(handles, full.shape, dst, "tensor")
+    sync, q, s, _ = pull_box(handles, full.shape, dst, E4M3, granularity="tensor")
     plan = sync._scaled_plans[0]
     dsl = TensorSlice(dst[0], (0,), tuple(full.shape), dst[1], (1,))
     dest, scales = {"w": q}, {"w": s}
@@ -215,12 +153,12 @@ def test_replay_refresh_and_invalidation():
     run(sync.pull({"w": handles}, dest, {"w": dsl}, tensor_scales=scales))
     run(sync.pull({"w": handles}, dest, {"w": dsl}, tensor_scales=scales))
     assert _native.launch_count() == before + 4 and sync._scaled_plans[0] == plan  # replayed: two passes each
-    for _, shard in sources:
+    for _, shard, _ in sources:
         shard.mul_(-7.0)
     new_full = (full.to(DEV) * -7.0).to(torch.bfloat16).cpu()
     run(sync.pull({"w": handles}, dest, {"w": dsl}, tensor_scales=scales))  # amax words re-armed: a smaller amax is seen
     assert_oracle(q, s, region(new_full, *dst).float().numpy(), "tensor")
-    for _, shard in sources:
+    for _, shard, _ in sources:
         shard.mul_(0.25)
     full = (new_full.to(DEV) * 0.25).to(torch.bfloat16).cpu()
     run(sync.pull({"w": handles}, dest, {"w": dsl}, tensor_scales=scales))  # a smaller amax than the last run's
@@ -279,8 +217,8 @@ def test_put_and_get_state_dict_with_channel_and_tensor_scales():
 
 def test_every_validation_error_raises_before_any_launch():
     full = rand_full((300, 260), torch.bfloat16, 6)
-    sources, handles = register(full, [shard_box(full.shape, 4, r, 0) for r in range(4)])
-    fp8_sources, fp8_handles = register(full.to(E4M3), [((0, 0), (300, 260))])
+    sources, handles = register_boxes(full, [shard_box(full.shape, 4, r, 0) for r in range(4)])
+    fp8_sources, fp8_handles = register_boxes(full.to(E4M3), [((0, 0), (300, 260))])
     q = torch.zeros(300, 260, dtype=E4M3, device=DEV)
     c, t = torch.zeros(300, 1, device=DEV), torch.zeros((), device=DEV)
     cases = [
@@ -320,19 +258,19 @@ def test_every_validation_error_raises_before_any_launch():
     cleanup(fp8_sources)
 
 
-@pytest.mark.skipif(not torch.cuda.is_available() or torch.cuda.device_count() < 2, reason="needs 2 GPUs")
+@needs_two_gpus
 @pytest.mark.parametrize("g", GRANULARITIES)
 def test_pieces_read_over_peer_mappings(g):
     full = rand_full((300, 520), torch.bfloat16, 8)
     boxes = [shard_box(full.shape, 4, r, 0) for r in range(4)]
     sources, handles = [], []
     for r, b in enumerate(boxes):  # shards alternate between cuda:1 and cuda:0
-        s_, h_ = register(full, [b], device=f"cuda:{1 - r % 2}")
+        s_, h_ = register_boxes(full, [b], device=f"cuda:{1 - r % 2}")
         sources += s_
         handles += h_
     for d in range(2):
         dst = shard_box(full.shape, 2, d, 1)
-        sync, q, s, qb, sb = pull_into(handles, full.shape, dst, g)
+        sync, q, s, (qb, sb) = pull_box(handles, full.shape, dst, E4M3, granularity=g)
         assert _native.plan_info(sync._scaled_plans[0]).remote_src_bytes > 0
         assert_oracle(q, s, region(full, *dst).float().numpy(), g)
         assert guards_intact(qb) and guards_intact(sb)

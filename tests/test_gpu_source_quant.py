@@ -3,15 +3,15 @@ the numpy oracle (finite groups) and torch CUDA (NaN bytes included), full-tenso
 shard boundaries, refresh replay, guard bytes around the kernel's outputs, the three existing consumers of scaled
 handles, mixed registers and the state-dict API.  Several "ranks" are emulated as several sources on cuda:0."""
 
-import asyncio
-
 import numpy as np
 import pytest
 import torch
 
 import torchstore_b200 as ts
-from oracle import block_fp8_oracle, ue8m0_oracle
-from oracle.source_quant_oracle import GRANULARITIES, bits_of, element_scales, quantize, synth_f32, torch_quantize, widen
+from oracle import block_fp8_oracle
+from oracle.source_quant_oracle import GRANULARITIES, element_scales, synth_f32, torch_quantize
+from tests.helpers import DEV, E4M3, cleanup, needs_two_gpus, register_boxes, run
+from tests.source_quant_regimes import assert_exact
 from tests.test_source_quant_cpu import CODE, DT
 from torchstore_b200 import _native
 from torchstore_b200.direct_weight_sync import DirectWeightSyncDest, DirectWeightSyncSource, ScaledNvlinkBuffer
@@ -19,13 +19,7 @@ from torchstore_b200.launch import Plans
 from torchstore_b200.transport.types import TensorSlice
 
 pytestmark = pytest.mark.gpu
-DEV = "cuda:0"
-E4M3 = torch.float8_e4m3fn
 DTYPES = (torch.bfloat16, torch.float16, torch.float32)
-
-
-def run(coro):
-    return asyncio.run(coro)
 
 
 def row_bounds(n: int, k: int) -> list[tuple[int, int]]:
@@ -39,48 +33,16 @@ def row_bounds(n: int, k: int) -> list[tuple[int, int]]:
     return out
 
 
-def register_rows(full: torch.Tensor, g: str, bounds, device=DEV, cols=None):
-    """One source per row shard (optionally a column range too) of `full`, quantised on registration."""
-    c0, c1 = cols or (0, full.shape[-1])
-    sources, handles = [], []
-    for r, (r0, r1) in enumerate(bounds):
-        shard = full[..., r0:r1, c0:c1].contiguous().to(device)
-        lead = tuple(full.shape[:-2])
-        tslice = TensorSlice(tuple(0 for _ in lead) + (r0, c0), (r,), tuple(full.shape), lead + (r1 - r0, c1 - c0),
-                             (len(bounds),))
-        src = DirectWeightSyncSource()
-        h = src.register({"w": shard}, rank=r, tensor_slices={"w": tslice}, quantize={"w": g})["w"]
-        sources.append((src, shard))
-        handles.append(h)
-    return sources, handles
+def row_boxes(shape, bounds, cols=None):
+    """(offsets, local shape) of each row range of `bounds` (within the column range `cols`, all columns without)."""
+    c0, c1 = cols or (0, shape[-1])
+    lead = tuple(shape[:-2])
+    return [((0,) * len(lead) + (r0, c0), lead + (r1 - r0, c1 - c0)) for r0, r1 in bounds]
 
 
 def staging(src: DirectWeightSyncSource, name="w"):
     q, s, _ = src._quantized[name]
     return q, s
-
-
-def assert_exact(q: torch.Tensor, s: torch.Tensor, x: torch.Tensor, g: str, r0: int, c0: int, scale_fmt=None):
-    """Bit-exact against torch CUDA everywhere (NaN bytes included) and against the numpy oracle on finite groups,
-    both in the scale format `scale_fmt`."""
-    tq, tsc = ue8m0_oracle.torch_quantize(x.to(q.device), g, r0, c0, scale_fmt=scale_fmt)
-    assert torch.equal(q.view(torch.uint8), tq.view(torch.uint8))
-    assert torch.equal(s.view(torch.int32), tsc.reshape(s.shape).view(torch.int32))
-    xf = widen(bits_of(x.cpu()), str(x.dtype)[6:])
-    want_q, want_s = ue8m0_oracle.quantize(xf, g, r0, c0, scale_fmt=scale_fmt) if scale_fmt else quantize(xf, g, r0, c0)
-    want_s = np.asarray(want_s, np.float32).reshape(tuple(s.shape))
-    if scale_fmt:
-        ue8m0_oracle.assert_pow2_over(s, torch_quantize(x.to(q.device), g, r0, c0)[1])
-    got_q, got_s = q.view(torch.uint8).cpu().numpy(), s.cpu().numpy()
-    fin = np.isfinite(element_scales(want_s, g, want_q.shape, r0, c0))
-    assert np.array_equal(got_q[fin], want_q[fin])
-    fs = np.isfinite(want_s)
-    assert np.array_equal(got_s[fs].view(np.uint32), want_s[fs].view(np.uint32))
-
-
-def cleanup(sources):
-    for src, _ in sources:
-        run(src.cleanup())
 
 
 LAYOUTS = {"aligned_4x128": ((512, 384), row_bounds(512, 4), None),
@@ -95,9 +57,9 @@ def test_staging_is_exact(g, dtype, layout):
     shape, bounds, cols = LAYOUTS[layout]
     full = synth_f32(shape, 11 + len(bounds)).to(dtype)
     full[bounds[-1][0] + 3, 5] = float("nan")  # a NaN group in the last shard
-    sources, handles = register_rows(full, g, bounds, cols=cols)
+    sources, handles = register_boxes(full, row_boxes(full.shape, bounds, cols), quantize={"w": g})
     c0 = cols[0] if cols else 0
-    for (src, shard), (r0, _), h in zip(sources, bounds, handles):
+    for (src, shard, _), (r0, _), h in zip(sources, bounds, handles):
         q, s = staging(src)
         assert isinstance(h.rdma_buffer, ScaledNvlinkBuffer) and (h.rdma_buffer.row0, h.rdma_buffer.col0) == (r0, c0)
         assert h.rdma_buffer.granularity == g and h.rdma_buffer.dtype == E4M3
@@ -109,13 +71,13 @@ def test_staging_is_exact(g, dtype, layout):
 def test_moe_stack_and_long_rows(dtype):
     x = synth_f32((3, 130, 260), 21).to(dtype)
     for g in GRANULARITIES:
-        sources, _ = register_rows(x, g, [(0, 130)])
+        sources, _ = register_boxes(x, row_boxes(x.shape, [(0, 130)]), quantize={"w": g})
         q, s = staging(sources[0][0])
         assert_exact(q, s, sources[0][1], g, 0, 0)
         cleanup(sources)
     long = synth_f32((4, 16400 if dtype != torch.float32 else 8200), 22).to(dtype)  # rows over the 32 KiB stage
     long[2, 7] = float("inf")
-    sources, _ = register_rows(long, "channel", [(0, 4)])
+    sources, _ = register_boxes(long, row_boxes(long.shape, [(0, 4)]), quantize={"w": "channel"})
     q, s = staging(sources[0][0])
     assert_exact(q, s, sources[0][1], "channel", 0, 0)
     cleanup(sources)
@@ -124,9 +86,9 @@ def test_moe_stack_and_long_rows(dtype):
 @pytest.mark.parametrize("g", ("block", "channel"))
 def test_group_aligned_shards_equal_the_full_tensor(g):
     full = synth_f32((1024, 640), 31).to(torch.bfloat16)
-    sources, _ = register_rows(full, g, row_bounds(1024, 8))
-    q = torch.cat([staging(src)[0].view(torch.uint8) for src, _ in sources])
-    s = torch.cat([staging(src)[1] for src, _ in sources])
+    sources, _ = register_boxes(full, row_boxes(full.shape, row_bounds(1024, 8)), quantize={"w": g})
+    q = torch.cat([staging(src)[0].view(torch.uint8) for src, *_ in sources])
+    s = torch.cat([staging(src)[1] for src, *_ in sources])
     fq, fs = torch_quantize(full.to(DEV), g)
     assert torch.equal(q, fq.view(torch.uint8)) and torch.equal(s.view(torch.int32), fs.view(torch.int32))
     cleanup(sources)
@@ -135,9 +97,9 @@ def test_group_aligned_shards_equal_the_full_tensor(g):
 @pytest.mark.parametrize("g", GRANULARITIES)
 def test_refresh_after_an_in_place_update(g):
     full = synth_f32((300, 520), 41).to(torch.bfloat16)
-    sources, _ = register_rows(full, g, row_bounds(300, 3))
+    sources, _ = register_boxes(full, row_boxes(full.shape, row_bounds(300, 3)), quantize={"w": g})
     for step in range(2):
-        for src, shard in sources:
+        for src, shard, _ in sources:
             shard.mul_(0.25)
             before = staging(src)[1].clone()
             assert src.refresh() == 1
@@ -182,7 +144,7 @@ def assemble(sources, shape, bounds):
     """The published fp8 bytes and per-element f32 scales of all shards, assembled into the full tensor."""
     q = torch.zeros(shape, dtype=torch.uint8)
     es = torch.zeros(shape, dtype=torch.float32)
-    for (src, _), (r0, r1) in zip(sources, bounds):
+    for (src, *_), (r0, r1) in zip(sources, bounds):
         sq, ss = staging(src)
         g = src._handles["w"].rdma_buffer.granularity
         q[r0:r1] = sq.view(torch.uint8).cpu()
@@ -194,7 +156,7 @@ def assemble(sources, shape, bounds):
 def test_consumers_dequantise_requantise_and_raw_bytes(g):
     shape, bounds = (300, 520), row_bounds(300, 4)
     full = synth_f32(shape, 61).to(torch.bfloat16)
-    sources, handles = register_rows(full, g, bounds)
+    sources, handles = register_boxes(full, row_boxes(full.shape, bounds), quantize={"w": g})
     q, es = assemble(sources, shape, bounds)
     x32 = q.view(E4M3).float() * es  # what a dequantising pull into f32 writes
     for d in range(2):  # a TP(2) column split
@@ -305,12 +267,12 @@ def test_put_and_get_state_dict_with_quantize():
     run(main())
 
 
-@pytest.mark.skipif(not torch.cuda.is_available() or torch.cuda.device_count() < 2, reason="needs 2 GPUs")
+@needs_two_gpus
 @pytest.mark.parametrize("g", GRANULARITIES)
 def test_quantised_handles_read_over_peer_mappings(g):
     shape, bounds = (300, 520), row_bounds(300, 2)
     full = synth_f32(shape, 91).to(torch.bfloat16)
-    sources, handles = register_rows(full, g, bounds, device="cuda:1")
+    sources, handles = register_boxes(full, row_boxes(full.shape, bounds), device="cuda:1", quantize={"w": g})
     q, es = assemble(sources, shape, bounds)
     y = torch.zeros(shape, dtype=torch.bfloat16, device=DEV)
     sync = DirectWeightSyncDest()

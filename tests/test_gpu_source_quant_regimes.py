@@ -15,210 +15,39 @@ carry their own scales.
 * Seeded random round trips (a layout, a dtype, a granularity and a consumer with its window), and mixed
   registers of several quantised names and a transfer_dtype name refreshed with changed weights."""
 
-import asyncio
 import random
 
 import numpy as np
 import pytest
 import torch
 
-from oracle import int8_source_oracle
 from oracle.source_quant_oracle import GRANULARITIES, fixture_inputs, synth_f32, torch_quantize
-from tests import test_gpu_dequant_fp8 as dq_gpu
-from tests import test_gpu_requant_fp8 as rq_gpu
 from tests.fp8_regimes import split, whole
-from tests.helpers import region, shard_box
-from tests.source_quant_regimes import CODE, REGIMES, WORKLOADS, Target, plan_bytes
-from tests.test_gpu_dequant_fp8 import guarded, guards_intact
-from tests.test_gpu_fp8_regimes import named, skip_unless_free
-from tests.test_gpu_source_quant import assert_exact
-from tests.test_source_quant_cpu import CODE as GCODE
-from tests.test_source_quant_cpu import assert_source_quant_equal, compile_host, fixture_cases
+from tests.helpers import (DEV, E4M3, cleanup, guarded, guards_intact, named, native_session, pull_box, region, register_boxes, run,
+                           shard_box, skip_unless_free)
+from tests.source_quant_regimes import (REGIMES, VARIANTS, WORKLOADS, assert_exact, local_slice, run_guarded,
+                                        run_regime)
+from tests.test_source_quant_cpu import assert_source_quant_equal, fixture_cases
 from tests.test_source_quant_regimes_cpu import (CONSUMERS, SHARD_LAYOUTS, assert_shared_groups_differ, layout_shards,
-                                                 oracle_shards, want_consumer, windows, workload_inputs)
-from torchstore_b200 import _native
-from torchstore_b200.direct_weight_sync import DirectWeightSyncDest, DirectWeightSyncSource, source_scale_shapes
-from torchstore_b200.launch import Plans
+                                                 oracle_shards, want_consumer, windows)
+from torchstore_b200.direct_weight_sync import DirectWeightSyncDest, DirectWeightSyncSource
 from torchstore_b200.transport.types import TensorSlice
 
 pytestmark = pytest.mark.gpu
-DEV = "cuda:0"
-E4M3 = torch.float8_e4m3fn
-
-
-@pytest.fixture(scope="module", autouse=True)
-def _init():
-    _native.init()
-    yield
-
-
-def run(coro):
-    return asyncio.run(coro)
-
-
-def on_device(x: torch.Tensor, misalign: int = 0) -> torch.Tensor:
-    """`x` on the GPU, starting `misalign` elements into a fresh allocation (not 16-byte aligned if > 0) with
-    4096 elements of slack after it, so that reads past a shard's end stay inside the allocation."""
-    flat = torch.zeros(x.numel() + 4096, dtype=x.dtype, device=DEV)
-    out = flat[misalign: misalign + x.numel()].view(x.shape)
-    out.copy_(x.to(DEV))
-    return out
-
-
-def local_slice(shape, row0, col0, global_shape=None, rank=0, ranks=1):
-    lead = tuple(shape[:-2])
-    gshape = global_shape or lead + (row0 + shape[-2], col0 + shape[-1])
-    offsets = (0,) * len(lead) + (row0, col0)
-    return TensorSlice(offsets, (rank,), tuple(gshape), tuple(shape), (ranks,))
+_init = pytest.fixture(scope="module", autouse=True)(native_session)
 
 
 # ---- the regimes ------------------------------------------------------------------------------------
-def group_boxes(t: Target):
-    """Index tuples of the first and the last group of a target's shard."""
-    *lead, n, k = t.shape
-    first_m, last_m = (0,) * len(lead), tuple(e - 1 for e in lead)
-    if t.granularity == "block":
-        r1, c1 = min(n, 128 - t.row0 % 128), min(k, 128 - t.col0 % 128)
-        lr, lc = max(0, (t.row0 + n - 1) // 128 * 128 - t.row0), max(0, (t.col0 + k - 1) // 128 * 128 - t.col0)
-        return first_m + (slice(0, r1), slice(0, c1)), last_m + (slice(lr, n), slice(lc, k))
-    if t.granularity == "channel":
-        return first_m + (slice(0, 1), slice(None)), last_m + (slice(n - 1, n), slice(None))
-    return first_m + (slice(None), slice(None)), last_m + (slice(None), slice(None))
-
-
-def plant(x: torch.Tensor, t: Target, kind: str, seed: int) -> torch.Tensor:
-    """Special values in the first and the last group of `x` (in its dtype): +Inf and -Inf, or NaN, at the
-    first element of the first group and the last element of the last; or both groups all zero or subnormal."""
-    x = x.float().clone()
-    first, last = group_boxes(t)
-    first_elem, last_elem = (0,) * len(t.shape), tuple(e - 1 for e in t.shape)
-    if kind in ("inf", "nan"):
-        x[first_elem] = float("inf") if kind == "inf" else float("nan")
-        x[last_elem] = float("-inf") if kind == "inf" else float("nan")
-    elif kind == "zero":
-        x[first] = 0
-        x[last] = 0
-    elif kind == "subnormal":
-        tiny = torch.finfo(getattr(torch, t.dtype)).tiny
-        for box in (first, last):
-            x[box] = synth_f32(tuple(x[box].shape), seed, spread=0) * tiny * 0.5
-    return x.to(getattr(torch, t.dtype))
-
-
-def register_workload(name, xs, scale_fmt=None, quant_dtype=None):
-    """One register() of every target of workload `name` (values `xs`), in the scale format `scale_fmt` and the
-    staging dtype `quant_dtype` -> (source, handles, device shards)."""
-    w = WORKLOADS[name]
-    src = DirectWeightSyncSource()
-    sd, slices, quant = {}, {}, {}
-    for i, (t, x) in enumerate(zip(w.targets, xs)):
-        sd[f"t{i}"] = on_device(x, t.misalign)
-        slices[f"t{i}"] = local_slice(t.shape, t.row0, t.col0)
-        quant[f"t{i}"] = t.granularity
-    handles = src.register(sd, rank=0, tensor_slices=slices, quantize=quant, scale_fmt=scale_fmt, quant_dtype=quant_dtype)
-    return src, handles, sd
-
-
-def live_tables(src, handles, w, quant_dtype=None):
-    """Compile on the host the targets register() built, from the staging it allocated and the handles'
-    offsets (for int8 staging with TSB_I8); check their size against plan_info -> (tables, targets)."""
-    targets = []
-    for i, t in enumerate(w.targets):
-        fp8, scale, local = src._quantized[f"t{i}"]
-        buf = handles[f"t{i}"].rdma_buffer
-        rows, cols = local.shape[-2:]
-        targets.append(_native.SourceQuantTarget(local.data_ptr(), fp8.data_ptr(), scale.data_ptr(), local.numel() // (rows * cols),
-                                                 rows, cols, buf.row0, buf.col0, CODE[t.dtype], GCODE[t.granularity]))
-    if quant_dtype == torch.int8:
-        arr = _native.make_source_quant_target_array(len(targets))
-        for i, t in enumerate(targets):
-            arr[i] = t
-        tables = _native.source_quant_compile_host(0, arr, len(targets), dst_dtype=_native.TSB_I8)
-    else:
-        tables = compile_host(targets)
-    info = _native.plan_info(src._quant_plans[0])
-    assert (info.num_tiles, info.src_bytes) == plan_bytes(tables)
-    return tables, targets
-
-
-def check_staging(src, w, xs, scale_fmt=None, quant_dtype=None):
-    for i, (t, x) in enumerate(zip(w.targets, xs)):
-        q, s, _ = src._quantized[f"t{i}"]
-        with named(t.describe()):
-            if quant_dtype == torch.int8:
-                int8_source_oracle.assert_exact(q, s, x, t.granularity, t.row0, t.col0)
-            else:
-                assert_exact(q, s, x, t.granularity, t.row0, t.col0, scale_fmt)
-
-
-VARIANTS = ("finite", "inf", "nan", "zero", "subnormal", "refresh")
-
-
 @pytest.mark.parametrize("variant", VARIANTS)
 @pytest.mark.parametrize("regime", sorted(REGIMES))
 def test_regime_on_the_h100(regime, variant):
     run_regime(regime, variant)
 
 
-def run_regime(regime, variant, scale_fmt=None, quant_dtype=None):
-    """Register the regime's workload in `variant` with the scale format `scale_fmt` and the staging dtype
-    `quant_dtype`, and check it (module doc)."""
-    r = REGIMES[regime]
-    w = WORKLOADS[r.workload]
-    xs = workload_inputs(r.workload)
-    if variant not in ("finite", "refresh"):
-        xs = [plant(x, t, variant, w.seed + i) for i, (t, x) in enumerate(zip(w.targets, xs))]
-    src, handles, sd = register_workload(r.workload, xs, scale_fmt, quant_dtype)
-    where = f"{regime} ({r.doc}), {variant}, scale_fmt={scale_fmt}, quant_dtype={quant_dtype}: {w.describe()}"
-    try:
-        tables, targets = live_tables(src, handles, w, quant_dtype)
-        assert r.holds(tables, targets), f"not reached: {where}"
-        with named(where):
-            check_staging(src, w, xs, scale_fmt, quant_dtype)
-            if variant == "refresh":
-                xs = [synth_f32(t.shape, w.seed + 50 + i).to(x.dtype) * 0.25 for i, (t, x) in enumerate(zip(w.targets, xs))]
-                for i, x in enumerate(xs):
-                    sd[f"t{i}"].copy_(x.to(DEV))
-                assert src.refresh() == len(w.targets)
-                check_staging(src, w, xs, scale_fmt, quant_dtype)
-    finally:
-        run(src.cleanup())
-
-
 @pytest.mark.parametrize("name", sorted(WORKLOADS))
 def test_workload_writes_nothing_outside_its_outputs(name):
     """The workload's plan driven directly on guarded fp8 and scale buffers, launched twice."""
     run_guarded(name)
-
-
-def run_guarded(name, scale_fmt=None, quant_dtype=None):
-    w = WORKLOADS[name]
-    xs = workload_inputs(name)
-    targets, outs = [], []
-    for t, x in zip(w.targets, xs):
-        sv = on_device(x, t.misalign)
-        sshape = source_scale_shapes(t.granularity, t.shape, t.row0, t.col0)[0]
-        qbase, q = guarded(t.shape, quant_dtype or E4M3)
-        sbase, s = guarded(sshape, torch.float32)
-        rows, cols = t.shape[-2:]
-        targets.append(_native.SourceQuantTarget(sv.data_ptr(), q.data_ptr(), s.data_ptr(), x.numel() // (rows * cols), rows, cols,
-                                                 t.row0, t.col0, CODE[t.dtype], GCODE[t.granularity]))
-        outs.append((sv, q, s, qbase, sbase))
-    plans = Plans.build_source_quant({0: targets}, _native.TSB_QUANT_UE8M0 if scale_fmt else 0,
-                                     _native.TSB_I8 if quant_dtype == torch.int8 else _native.TSB_F8E4M3)
-    try:
-        for _ in range(2):
-            plans.launch()
-            plans.synchronize()
-    finally:
-        plans.close()
-    for t, x, (_, q, s, qbase, sbase) in zip(w.targets, xs, outs):
-        with named(f"{name}: {t.describe()}"):
-            if quant_dtype == torch.int8:
-                int8_source_oracle.assert_exact(q, s, x, t.granularity, t.row0, t.col0)
-            else:
-                assert_exact(q, s, x, t.granularity, t.row0, t.col0, scale_fmt)
-            assert guards_intact(qbase) and guards_intact(sbase)
 
 
 # ---- the torch CPU fixture on the device ------------------------------------------------------------
@@ -237,20 +66,8 @@ def test_fixture_on_the_h100(case):
 
 
 # ---- consumers of shard-local scales ----------------------------------------------------------------
-def register_boxes(x_full, g, boxes, name="w"):
-    """One source per box of `x_full`, quantised on registration -> (sources, handles)."""
-    sources, handles = [], []
-    for r, (off, loc) in enumerate(boxes):
-        src = DirectWeightSyncSource()
-        sl = TensorSlice(off, (r,), tuple(x_full.shape), loc, (len(boxes),))
-        handles.append(src.register({name: region(x_full, off, loc).contiguous().to(DEV)}, rank=r, tensor_slices={name: sl},
-                                    quantize={name: g})[name])
-        sources.append(src)
-    return sources, handles
-
-
 def assert_staging_is_the_oracle(sources, shards, name="w"):
-    for src, (off, loc, want_q, want_s) in zip(sources, shards):
+    for (src, *_), (off, loc, want_q, want_s) in zip(sources, shards):
         q, s, _ = src._quantized[name]
         assert np.array_equal(q.view(torch.uint8).cpu().numpy(), want_q), off
         assert np.array_equal(s.cpu().numpy().view(np.uint32), want_s.view(np.uint32)), off
@@ -259,7 +76,7 @@ def assert_staging_is_the_oracle(sources, shards, name="w"):
 def pull_consumer(handles, shape, g, consumer, window):
     """One pull of `handles` into a guarded window -> (result, want) as comparable numpy arrays, guards intact."""
     if consumer in GRANULARITIES:
-        sync, y, ys, bases = rq_gpu.pull_into(handles, shape, window, consumer)
+        sync, y, ys, bases = pull_box(handles, shape, window, E4M3, granularity=consumer, requantize=True)
         got = (y.view(torch.uint8).cpu().numpy(), ys.cpu().numpy().reshape(-1).view(np.uint32))
     elif consumer == "raw":
         base, y = guarded(window[1], E4M3)
@@ -267,8 +84,7 @@ def pull_consumer(handles, shape, g, consumer, window):
         run(sync.pull({"w": handles}, {"w": y}, {"w": TensorSlice(window[0], (0,), shape, window[1], (1,))}))
         got = y.view(torch.uint8).cpu().numpy()
     else:
-        sync, y, base = dq_gpu.pull_into(handles, shape, window, getattr(torch, consumer))
-        bases = (base,)
+        sync, y, _, bases = pull_box(handles, shape, window, getattr(torch, consumer))
         got = y.view(torch.int16 if y.element_size() == 2 else torch.int32).cpu().numpy()
     assert all(guards_intact(b) for b in bases)
     sync.close()
@@ -288,7 +104,7 @@ def assert_consumer(got, want, consumer):
 def test_consumers_of_shard_local_scales(layout, g):
     shape, boxes, x, shards = layout_shards(layout, g, 300 + len(layout))
     assert_shared_groups_differ(shards, g)
-    sources, handles = register_boxes(x, g, boxes)
+    sources, handles = register_boxes(x, boxes, quantize={"w": g})
     try:
         assert_staging_is_the_oracle(sources, shards)
         for consumer, win in CONSUMERS:
@@ -297,8 +113,7 @@ def test_consumers_of_shard_local_scales(layout, g):
                 assert_consumer(pull_consumer(handles, shape, g, consumer, window),
                                 want_consumer(shape, shards, g, consumer, window), consumer)
     finally:
-        for src in sources:
-            run(src.cleanup())
+        cleanup(sources)
 
 
 # ---- seeded random round trips ----------------------------------------------------------------------
@@ -338,17 +153,16 @@ def test_random_round_trips(seed):
     shape, dtype, g, layout, boxes, consumer, window = draw(rng)
     x = (torch.randn(shape, generator=torch.Generator().manual_seed(seed)) * 0.05).to(dtype)
     shards = oracle_shards(x, g, boxes)
-    sources, handles = register_boxes(x, g, boxes)
+    sources, handles = register_boxes(x, boxes, quantize={"w": g})
     try:
         with named(f"seed {seed}: {str(dtype)[6:]}{list(shape)} {g} {layout} {[b for b in boxes]} -> {consumer} {window}"):
-            for src, (off, loc) in zip(sources, boxes):
+            for (src, *_), (off, loc) in zip(sources, boxes):
                 q, s, _ = src._quantized["w"]
                 assert_exact(q, s, region(x, off, loc).contiguous(), g, off[-2], off[-1])
             assert_consumer(pull_consumer(handles, shape, g, consumer, window), want_consumer(shape, shards, g, consumer, window),
                             consumer)
     finally:
-        for src in sources:
-            run(src.cleanup())
+        cleanup(sources)
 
 
 @pytest.mark.parametrize("seed", range(6))

@@ -2,7 +2,6 @@
 fixtures recorded from the reference's LocalClient + SharedMemory transport, plus the behaviours the
 reference's integration tests pin (tests/test_store.py, test_tensor_slice.py, test_state_dict.py)."""
 
-import asyncio
 import itertools
 import json
 import os
@@ -14,17 +13,12 @@ import torch
 import torchstore_b200 as ts
 from torchstore_b200 import _native
 from oracle import reshard_oracle as ro
-from tests.helpers import sha256_of
+from tests.helpers import DEV, run, sha256_of
 from torchstore_b200.transport import create_transport_buffer
 from torchstore_b200.transport.types import Request, TensorSlice
 
 pytestmark = pytest.mark.gpu
 GOLDEN = os.path.join(os.path.dirname(__file__), "golden")
-DEV = "cuda:0"
-
-
-def run(coro):
-    return asyncio.run(coro)
 
 
 @pytest.fixture(autouse=True)

@@ -4,24 +4,19 @@ converting destinations on the CPU and on the GPU, medium shapes that reach both
 kernel, TORCHSTORE_B200_GET_DEVICE=cuda, and fast-lane replays after in-place overwrites and layout
 changes."""
 
-import asyncio
 import random
 
 import pytest
 import torch
 
 import torchstore_b200 as ts
+from tests.helpers import DEV, run
 from tests.store_harness import (DTYPES, TORCH_CAST_PAIRS, Layout, StoreHarness, _strided_copy, fill, run_differential,
                                  store_layout, to_np)
 from tests.test_random_layouts import to_ts
 
 pytestmark = pytest.mark.gpu
-DEV = "cuda:0"
 NVOL = 3
-
-
-def run(coro):
-    return asyncio.run(coro)
 
 
 @pytest.fixture(autouse=True)

@@ -9,15 +9,14 @@ import torch
 
 import workloads
 from oracle import transpose_oracle as to
-from tests.helpers import fsdp_handles, pull_args, region
-from tests.test_gpu_packed import as_np, masters, nv_handles, pull, run, whole_handle
+from tests.helpers import (DEV, E4M3, as_np, fsdp_handles, masters, needs_two_gpus, nv_handles, pull, pull_args, region,
+                           run, whole_handle)
 from torchstore_b200.direct_weight_sync import DirectWeightSyncDest, NvlinkBuffer, PackedPart, RDMAWeightHandle
 from torchstore_b200.transport.types import TensorSlice
 
 pytestmark = pytest.mark.gpu
-DEV = "cuda:0"
 QWEN = workloads.QWEN3_MOE
-E4M3, E5M2 = torch.float8_e4m3fn, torch.float8_e5m2
+E5M2 = torch.float8_e5m2
 
 
 def i16(shape):
@@ -237,7 +236,7 @@ def test_get_state_dict_with_transposed_parts():
     run(main())
 
 
-@pytest.mark.skipif(not torch.cuda.is_available() or torch.cuda.device_count() < 2, reason="needs 2 GPUs")
+@needs_two_gpus
 def test_transposed_parts_read_over_peer_mappings():
     layout = grouped(scale=8)
     full = masters(layout, 81, device="cuda:1")

@@ -4,26 +4,19 @@ scale_inv included) and against the numpy oracle on finite groups; non-finite gr
 changes; and the lossless round trip of power-of-two groups requantised onto themselves.  Several "ranks" are
 emulated as several sources on cuda:0."""
 
-import asyncio
-
 import numpy as np
 import pytest
 import torch
 
 from oracle.dequant_fp8_oracle import expand
 from oracle.ue8m0_oracle import GRANULARITIES, bits_of, quantize, synth_f32, torch_quantize, torch_requantize, widen
+from tests.fp8_regimes import whole
+from tests.helpers import DEV, E4M3, KW, cleanup, pull_box, run
 from torchstore_b200.direct_weight_sync import DirectWeightSyncDest, DirectWeightSyncSource, ScaledNvlinkBuffer
 from torchstore_b200.transport.types import TensorSlice
 
 pytestmark = pytest.mark.gpu
-DEV = "cuda:0"
-E4M3 = torch.float8_e4m3fn
 DTYPES = (torch.bfloat16, torch.float16, torch.float32)
-KW = {"block": "block_scales", "channel": "channel_scales", "tensor": "tensor_scales"}
-
-
-def run(coro):
-    return asyncio.run(coro)
 
 
 def dest_scale(g: str, shape) -> torch.Tensor:
@@ -42,11 +35,6 @@ def publish(full: torch.Tensor, boxes, **register_kw):
         handles.append(src.register({"w": shard}, rank=r, tensor_slices={"w": ts}, **register_kw)["w"])
         sources.append((src, shard))
     return sources, handles
-
-
-def cleanup(sources):
-    for src, _ in sources:
-        run(src.cleanup())
 
 
 def rows(shape, k):
@@ -78,15 +66,6 @@ def assert_exact(q, s, x, g, r0=0, c0=0):
     assert (got_s[fs].view(np.uint32) & 0x7FFFFF == 0).all()  # powers of two
 
 
-def pull_into(handles, shape, g, **kw):
-    q = torch.full(shape, 0x55, dtype=torch.uint8, device=DEV).view(E4M3)
-    s = dest_scale(g, shape)
-    d = DirectWeightSyncDest()
-    run(d.pull({"w": handles}, {"w": q}, **{KW[g]: {"w": s}}, **kw))
-    d.close()
-    return q, s
-
-
 # ---- quantising pulls ------------------------------------------------------------------------------------------
 LAYOUTS = {
     "exact_300x520": ((300, 520), lambda s: [((0, 0), s)]),
@@ -106,7 +85,8 @@ def test_quantising_pull_is_exact(g, dtype, layout):
     shape, boxes = LAYOUTS[layout]
     full = synth_f32(shape, 101 + len(layout)).to(dtype)
     sources, handles = publish(full, boxes(shape))
-    q, s = pull_into(handles, shape, g, scale_fmt="ue8m0")
+    sync, q, s, _ = pull_box(handles, shape, whole(shape), E4M3, granularity=g, scale_fmt="ue8m0")
+    sync.close()
     assert_exact(q, s, full, g)
     cleanup(sources)
 
@@ -116,7 +96,9 @@ def test_long_channel_rows_take_the_two_pass_path(dtype):
     shape = (3, 16400 if dtype != torch.float32 else 8200)  # over the 32 KiB row stage
     full = synth_f32(shape, 7).to(dtype)
     sources, handles = publish(full, cols(shape, (shape[1] // 2,)))
-    q, s = pull_into(handles, shape, "channel", scale_fmt="ue8m0")
+    sync, q, s, _ = pull_box(handles, shape, whole(shape), E4M3, granularity="channel",
+                             scale_fmt="ue8m0")
+    sync.close()
     assert_exact(q, s, full, "channel")
     cleanup(sources)
 
@@ -128,7 +110,9 @@ def test_non_finite_groups(g):
     full[3, 5] = float("inf")
     full[200, 140] = float("nan")
     sources, handles = publish(full, rows(full.shape, 2))
-    q, s = pull_into(handles, tuple(full.shape), g, scale_fmt="ue8m0")
+    sync, q, s, _ = pull_box(handles, tuple(full.shape), whole(tuple(full.shape)), E4M3, granularity=g,
+                             scale_fmt="ue8m0")
+    sync.close()
     assert_exact(q, s, full, g)
     sc = s.cpu()
     assert torch.isnan(sc).any()
@@ -188,7 +172,9 @@ def test_requantising_pull_is_the_torch_composition(sg, dg):
         src = DirectWeightSyncSource()
         handles.append(src.register({"w": shard}, rank=r, tensor_slices={"w": ts}, **{KW[sg]: {"w": scale}})["w"])
         sources.append((src, shard))
-    q, s = pull_into(handles, tuple(x.shape), dg, requantize=True, scale_fmt="ue8m0")
+    sync, q, s, _ = pull_box(handles, tuple(x.shape), whole(tuple(x.shape)), E4M3, granularity=dg, requantize=True,
+                             scale_fmt="ue8m0")
+    sync.close()
     tq, ts_ = torch_requantize(q_full, s_full, sg, 0, 0, dg, scale_fmt="ue8m0")
     assert torch.equal(q.view(torch.uint8), tq.view(torch.uint8))
     assert torch.equal(s.view(torch.int32), ts_.reshape(s.shape).view(torch.int32))
@@ -239,7 +225,9 @@ def test_power_of_two_groups_requantised_onto_themselves_keep_every_value(g):
     full = synth_f32((512, 640), 13, spread=12).to(torch.bfloat16)
     boxes = rows(full.shape, 4)  # 128-row shards: block rows and channel rows coincide on both sides
     sources, handles = publish(full, boxes, quantize={"w": g}, scale_fmt="ue8m0")
-    q, s = pull_into(handles, tuple(full.shape), g, requantize=True, scale_fmt="ue8m0")
+    sync, q, s, _ = pull_box(handles, tuple(full.shape), whole(tuple(full.shape)), E4M3, granularity=g,
+                             requantize=True, scale_fmt="ue8m0")
+    sync.close()
     src_q = torch.cat([src._quantized["w"][0].view(torch.uint8) for src, _ in sources]).view(E4M3)
     src_s = torch.cat([src._quantized["w"][1] for src, _ in sources])
     before = src_q.float() * torch.from_numpy(np.ascontiguousarray(expand(src_s.cpu().numpy(), tuple(full.shape), g))).to(DEV)

@@ -15,7 +15,7 @@ every route, over the torch CPU fixture and over the lossless-requantise domain.
   overflow at amax >= 248 * 2^120, and source scales under 2^-22.
 * One state-dict round trip with ``quantize=`` and ``scale_fmt="ue8m0"``."""
 
-import asyncio
+from functools import partial
 
 import numpy as np
 import pytest
@@ -26,37 +26,19 @@ from oracle import ue8m0_oracle as u8
 from oracle.dequant_fp8_oracle import decode_e4m3, expand, torch_dequantize
 from tests import fp8_regimes, quant_pull_regimes, source_quant_regimes
 from tests import test_fp8_regimes_cpu as fp8_cpu
-from tests import test_gpu_fp8_regimes as fp8_gpu
-from tests import test_gpu_quant_pull_regimes as qp_gpu
-from tests import test_gpu_requant_fp8 as rq_gpu
-from tests import test_gpu_source_quant_regimes as sq_gpu
-from tests.helpers import region
+from tests.helpers import (DEV, E4M3, KW, cleanup, dest_scale_shape, guarded, guards_intact, named, native_session,
+                           pull_box, region, register_boxes, run)
 from tests.quant_pull_regimes import Pull
-from tests.test_gpu_dequant_fp8 import cleanup, guarded, guards_intact, register
-from tests.test_gpu_fp8_regimes import named
-from tests.test_gpu_source_quant import assert_exact
+from tests.source_quant_regimes import assert_exact
+from tests.test_dequant_fp8_cpu import local_scale as dq_local_scale
 from tests.test_ue8m0_cpu import fixture_cases, is_pow2, u32
 from tests.test_ue8m0_regimes_cpu import LOSSLESS, RQ_REGIMES, assert_lossless
-from torchstore_b200 import _native
 from torchstore_b200.direct_weight_sync import DirectWeightSyncDest, DirectWeightSyncSource
-from torchstore_b200.transport.types import TensorSlice
 
 pytestmark = pytest.mark.gpu
-DEV = "cuda:0"
-E4M3 = torch.float8_e4m3fn
 UE = "ue8m0"
 DTYPES = (torch.bfloat16, torch.float16, torch.float32)
-KW = {"block": "block_scales", "channel": "channel_scales", "tensor": "tensor_scales"}
-
-
-@pytest.fixture(scope="module", autouse=True)
-def _init():
-    _native.init()
-    yield
-
-
-def run(coro):
-    return asyncio.run(coro)
+_init = pytest.fixture(scope="module", autouse=True)(native_session)
 
 
 def whole(shape):
@@ -64,27 +46,27 @@ def whole(shape):
 
 
 # ---- every regime in UE8M0 ---------------------------------------------------------------------------
-@pytest.mark.parametrize("variant", qp_gpu.VARIANTS)
+@pytest.mark.parametrize("variant", quant_pull_regimes.VARIANTS)
 @pytest.mark.parametrize("regime", sorted(quant_pull_regimes.REGIMES))
 def test_quant_pull_regime(regime, variant):
-    qp_gpu.run_regime(regime, variant, UE)
+    quant_pull_regimes.run_regime(regime, variant, UE)
 
 
-@pytest.mark.parametrize("variant", sq_gpu.VARIANTS)
+@pytest.mark.parametrize("variant", source_quant_regimes.VARIANTS)
 @pytest.mark.parametrize("regime", sorted(source_quant_regimes.REGIMES))
 def test_source_regime(regime, variant):
-    sq_gpu.run_regime(regime, variant, UE)
+    source_quant_regimes.run_regime(regime, variant, UE)
 
 
 @pytest.mark.parametrize("name", sorted(source_quant_regimes.WORKLOADS))
 def test_source_workload_writes_nothing_outside_its_outputs(name):
-    sq_gpu.run_guarded(name, UE)
+    source_quant_regimes.run_guarded(name, UE)
 
 
-@pytest.mark.parametrize("variant", fp8_gpu.VARIANTS)
+@pytest.mark.parametrize("variant", fp8_regimes.VARIANTS)
 @pytest.mark.parametrize("regime", RQ_REGIMES)
 def test_requant_regime(regime, variant):
-    fp8_gpu.run_regime(regime, variant, UE)
+    fp8_regimes.run_regime(regime, variant, UE)
 
 
 # ---- the step's edges, route by route ----------------------------------------------------------------
@@ -115,7 +97,7 @@ def test_edges_of_a_quantising_pull(route, dtype):
     assert_all_branches(branches)
     name = str(dtype)[6:]
     p = Pull(name, shape, quant_pull_regimes.split(shape, 2, -1), whole(shape), g)
-    pulled = qp_gpu.Pulled((p,), [x], scale_fmt=UE)
+    pulled = quant_pull_regimes.Pulled((p,), [x], scale_fmt=UE)
     try:
         pulled.pull()
         tables, _ = pulled.live_tables()
@@ -146,7 +128,7 @@ def test_edges_of_source_side_quantisation(route, dtype):
     assert_all_branches(branches)
     src = DirectWeightSyncSource()
     try:
-        src.register({"w": x.to(DEV)}, rank=0, tensor_slices={"w": sq_gpu.local_slice(shape, 37, 70)}, quantize={"w": g},
+        src.register({"w": x.to(DEV)}, rank=0, tensor_slices={"w": source_quant_regimes.local_slice(shape, 37, 70)}, quantize={"w": g},
                      scale_fmt=UE)
         q, s, _ = src._quantized["w"]
         with named(f"{route} {str(dtype)[6:]}"):
@@ -184,15 +166,15 @@ def test_edges_of_a_requantising_pull(route):
     q, s, branches = edge_source(g)
     assert_all_branches(branches)
     box = whole(tuple(q.shape))
-    sources, handles = register(q, s, g, [box])
-    sync, y, ys, bases = rq_gpu.pull_into(handles, tuple(q.shape), box, g, scale_fmt=UE)
+    sources, handles = register_boxes(q, [box], granularity=g, scale_of=partial(dq_local_scale, s, g))
+    sync, y, ys, bases = pull_box(handles, tuple(q.shape), box, E4M3, granularity=g, requantize=True, scale_fmt=UE)
     try:
-        tables, _ = fp8_gpu.live_tables(sync, y, ys, g)
+        tables, _ = fp8_regimes.live_tables(sync, y, ys, g)
         units, _, tiles, _ = tables
         assert (len(tiles) > 0) == (g == "tensor") and (len(units) > 0) == (g != "tensor")
         with named(route):
-            rq_gpu.assert_oracle(y, ys, q, s, g, box, g, UE)
-            rq_gpu.assert_torch_cuda(y, ys, q, s, g, box, g, UE)
+            fp8_regimes.assert_requant_oracle(y, ys, q, s, g, box, g, UE)
+            fp8_regimes.assert_requant_torch_cuda(y, ys, q, s, g, box, g, UE)
         assert all(guards_intact(b) for b in bases)
     finally:
         sync.close()
@@ -224,13 +206,13 @@ def test_fixture_on_the_h100(case):
         if (r0, c0) == (0, 0):
             h = src.register({"w": x.to(DEV)}, rank=0)["w"]
             qb, q = guarded(tuple(x.shape), E4M3)
-            sb, s = guarded(quant_pull_regimes.scale_shape(g, tuple(x.shape)), torch.float32)
+            sb, s = guarded(dest_scale_shape(g, tuple(x.shape)), torch.float32)
             sync = DirectWeightSyncDest()
             run(sync.pull({"w": [h]}, {"w": q}, **{KW[g]: {"w": s}}, scale_fmt=UE))
             sync.close()
             assert guards_intact(qb) and guards_intact(sb)
         else:
-            src.register({"w": x.to(DEV)}, rank=0, tensor_slices={"w": sq_gpu.local_slice(x.shape, r0, c0)}, quantize={"w": g},
+            src.register({"w": x.to(DEV)}, rank=0, tensor_slices={"w": source_quant_regimes.local_slice(x.shape, r0, c0)}, quantize={"w": g},
                          scale_fmt=UE)
             q, s, _ = src._quantized["w"]
         assert_fixture(q.view(torch.uint8).cpu().numpy(), s.cpu().numpy(), want_q, want_s)
@@ -250,10 +232,10 @@ def test_lossless_requantise_of_a_catalogue_workload(name):
     w = fp8_regimes.WORKLOADS[name]
     q, s = fp8_cpu.inputs(w)
     s = torch.from_numpy(u8.pow2_scales(tuple(s.shape), w.seed))
-    sources, handles = register(q, s, w.sg, list(w.src))
-    sync, y, ys, bases = rq_gpu.pull_into(handles, w.shape, w.dst, w.out, scale_fmt=UE)
+    sources, handles = register_boxes(q, list(w.src), granularity=w.sg, scale_of=partial(dq_local_scale, s, w.sg))
+    sync, y, ys, bases = pull_box(handles, w.shape, w.dst, E4M3, granularity=w.out, requantize=True, scale_fmt=UE)
     try:
-        rq_gpu.assert_torch_cuda(y, ys, q, s, w.sg, w.dst, w.out, UE)
+        fp8_regimes.assert_requant_torch_cuda(y, ys, q, s, w.sg, w.dst, w.out, UE)
         assert_lossless(q, s, w.sg, y.view(torch.uint8).cpu().numpy(), ys.cpu().numpy(), w.out, *w.dst)
         assert all(guards_intact(b) for b in bases)
     finally:
@@ -264,22 +246,11 @@ def test_lossless_requantise_of_a_catalogue_workload(name):
 def source_values(sources, boxes, g, shape):
     """The values f32(q) * s of UE8M0 source-quantised shards, assembled over the global shape."""
     out = torch.full(shape, float("nan"), device=DEV)
-    for src, (off, loc) in zip(sources, boxes):
+    for (src, *_), (off, loc) in zip(sources, boxes):
         q, s, _ = src._quantized["w"]
         e = torch.from_numpy(np.ascontiguousarray(expand(s.cpu().numpy(), tuple(loc), g, off[-2], off[-1]))).to(DEV)
         out[tuple(slice(o, o + n) for o, n in zip(off, loc))] = q.float() * e
     return out
-
-
-def register_quantized(full, boxes, g):
-    sources, handles = [], []
-    for r, (off, loc) in enumerate(boxes):
-        src = DirectWeightSyncSource()
-        sl = TensorSlice(off, (r,), tuple(full.shape), loc, (len(boxes),))
-        handles.append(src.register({"w": region(full, off, loc).contiguous().to(DEV)}, rank=r, tensor_slices={"w": sl},
-                                    quantize={"w": g}, scale_fmt=UE)["w"])
-        sources.append(src)
-    return sources, handles
 
 
 CONTAINED = {  # name -> (source granularity, source boxes of a [300, 512] tensor, destination window, granularity)
@@ -294,37 +265,37 @@ CONTAINED = {  # name -> (source granularity, source boxes of a [300, 512] tenso
 def test_lossless_requantise_of_contained_groups(case):
     sg, boxes, (off, loc), dg = CONTAINED[case]
     full = u8.synth_f32((300, 512), 40 + len(case), spread=12).to(torch.bfloat16)
-    sources, handles = register_quantized(full, boxes, sg)
+    sources, handles = register_boxes(full, boxes, quantize={"w": sg}, scale_fmt=UE)
     try:
         before = source_values(sources, boxes, sg, (300, 512))[tuple(slice(o, o + n) for o, n in zip(off, loc))]
-        sync, y, ys, bases = rq_gpu.pull_into(handles, (300, 512), (off, loc), dg, scale_fmt=UE)
+        sync, y, ys, bases = pull_box(handles, (300, 512), (off, loc), E4M3, granularity=dg, requantize=True,
+                                      scale_fmt=UE)
         e = torch.from_numpy(np.ascontiguousarray(expand(ys.cpu().numpy(), tuple(loc), dg))).to(DEV)
         after = y.float() * e
         assert torch.isfinite(before).all() and torch.equal(after.view(torch.int32), before.view(torch.int32))
-        s_src = torch.cat([src._quantized["w"][1].reshape(-1) for src in sources])
+        s_src = torch.cat([src._quantized["w"][1].reshape(-1) for src, *_ in sources])
         assert ys.max() <= s_src.max()
         assert all(guards_intact(b) for b in bases)
         sync.close()
     finally:
-        for src in sources:
-            run(src.cleanup())
+        cleanup(sources)
 
 
 @pytest.mark.parametrize("g", u8.GRANULARITIES)
 def test_published_ue8m0_handles_requantised_into_their_own_layout_keep_their_values(g):
     full = u8.synth_f32((300, 512), 44, spread=12).to(torch.bfloat16)
     boxes = (((0, 0), (300, 256)), ((0, 256), (300, 256)))  # column shards cut on a block boundary
-    sources, handles = register_quantized(full, boxes, g)
+    sources, handles = register_boxes(full, boxes, quantize={"w": g}, scale_fmt=UE)
     try:
         want = source_values(sources, boxes, g, (300, 512))
         for off, loc in boxes:
-            sync, y, ys, _ = rq_gpu.pull_into(handles, (300, 512), (off, loc), g, scale_fmt=UE)
+            sync, y, ys, _ = pull_box(handles, (300, 512), (off, loc), E4M3, granularity=g, requantize=True,
+                                      scale_fmt=UE)
             e = torch.from_numpy(np.ascontiguousarray(expand(ys.cpu().numpy(), tuple(loc), g))).to(DEV)
             assert torch.equal((y.float() * e).view(torch.int32), region(want, off, loc).view(torch.int32)), off
             sync.close()
     finally:
-        for src in sources:
-            run(src.cleanup())
+        cleanup(sources)
 
 
 # ---- both ends of the domain -------------------------------------------------------------------------
@@ -348,7 +319,8 @@ def test_amax_at_the_dtype_top_reads_back_as_inf(dtype):
         sync.close()
         assert torch.equal(y, torch_dequantize(q, s, "block", 0, 0, dtype))
         assert y[5, 9] == float("inf") and torch.isfinite(y[:, 128:]).all()
-        sync, yq, ys, bases = rq_gpu.pull_into([h], tuple(x.shape), whole(tuple(x.shape)), "block", scale_fmt=UE)
+        sync, yq, ys, bases = pull_box([h], tuple(x.shape), whole(tuple(x.shape)), E4M3, granularity="block",
+                                       requantize=True, scale_fmt=UE)
         sync.close()
         want_q, want_s = u8.torch_requantize(q, s, "block", 0, 0, "block", scale_fmt=UE)
         assert torch.equal(yq.view(torch.uint8), want_q.view(torch.uint8))
@@ -365,10 +337,12 @@ def test_source_scale_under_2_pow_22_loses_low_bits_as_torch_does():
     subnormal bytes lose their low bit, exactly as the torch composition does."""
     q = torch.arange(0, 128, dtype=torch.uint8).repeat(128, 2)[:, :256] & 0x8F  # +-subnormal and small normal bytes
     s = torch.tensor([[2.0 ** -23, 2.0 ** -3]])
-    sources, handles = register(q.view(E4M3), s, "block", [whole((128, 256))])
-    sync, y, ys, _ = rq_gpu.pull_into(handles, (128, 256), whole((128, 256)), "block", scale_fmt=UE)
+    sources, handles = register_boxes(q.view(E4M3), [whole((128, 256))], granularity="block",
+                                      scale_of=partial(dq_local_scale, s, "block"))
+    sync, y, ys, _ = pull_box(handles, (128, 256), whole((128, 256)), E4M3, granularity="block", requantize=True,
+                              scale_fmt=UE)
     try:
-        rq_gpu.assert_torch_cuda(y, ys, q.view(E4M3), s, "block", whole((128, 256)), "block", UE)
+        fp8_regimes.assert_requant_torch_cuda(y, ys, q.view(E4M3), s, "block", whole((128, 256)), "block", UE)
         assert float(ys[0, 0]) == 2.0 ** -22
         before = q.view(E4M3).float()[:, :128] * 2.0 ** -23
         after = y.cpu().float()[:, :128] * 2.0 ** -22

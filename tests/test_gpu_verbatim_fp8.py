@@ -5,8 +5,6 @@ subnormal scales); source-side quantisation followed by a verbatim pull and refr
 the destination; one mixed pull; the errors; the state-dict API; peer mappings and the full-size Llama-3-8B
 linear weights."""
 
-import asyncio
-
 import numpy as np
 import pytest
 import torch
@@ -15,53 +13,15 @@ import torchstore_b200 as ts
 import workloads
 from oracle.dequant_fp8_oracle import torch_dequantize
 from oracle.verbatim_fp8_oracle import verbatim
-from tests.test_gpu_dequant_fp8 import guarded, guards_intact
+from tests.helpers import (DEV, E4M3, cleanup, guards_intact, native_session, needs_two_gpus, pull_box, register_shards,
+                           run)
 from tests.test_verbatim_fp8_cpu import GRANULARITIES, KW, LAYOUTS, fp8_full, make_sources, rows
 from torchstore_b200 import _native
 from torchstore_b200.direct_weight_sync import DirectWeightSyncDest, DirectWeightSyncSource, source_scale_shapes
 from torchstore_b200.transport.types import TensorSlice
 
 pytestmark = pytest.mark.gpu
-DEV = "cuda:0"
-E4M3 = torch.float8_e4m3fn
-
-
-@pytest.fixture(scope="module", autouse=True)
-def _init():
-    _native.init()
-    yield
-
-
-def run(coro):
-    return asyncio.run(coro)
-
-
-def register(g, gshape, sources, name="w", device=DEV):
-    """One DirectWeightSyncSource per (shard, scale, offset), publishing it with its scale -> (sources, handles)."""
-    out, handles = [], []
-    for r, (shard, scale, off) in enumerate(sources):
-        src = DirectWeightSyncSource()
-        shard, scale = shard.to(device), scale.to(device)
-        sl = TensorSlice(off, (r,), tuple(gshape), tuple(shard.shape), (len(sources),))
-        handles.append(src.register({name: shard}, rank=r, tensor_slices={name: sl}, **{KW[g]: {name: scale}})[name])
-        out.append((src, shard, scale))
-    return out, handles
-
-
-def cleanup(sources):
-    for src, *_ in sources:
-        run(src.cleanup())
-
-
-def pull_into(g, handles, gshape, box, sync=None, device=DEV, **kw):
-    """Verbatim pull of `handles` into a guarded `g`-scaled fp8 window `box` -> (sync, q, scale, guards)."""
-    off, loc = box
-    qbase, q = guarded(loc, E4M3, device)
-    sbase, s = guarded(source_scale_shapes(g, loc, 0, 0)[0], torch.float32, device)
-    sync = sync or DirectWeightSyncDest()
-    run(sync.pull({"w": handles}, {"w": q}, {"w": TensorSlice(off, (0,), tuple(gshape), loc, (1,))}, **{KW[g]: {"w": s}},
-                  verbatim=True, **kw))
-    return sync, q, s, (qbase, sbase)
+_init = pytest.fixture(scope="module", autouse=True)(native_session)
 
 
 def assert_oracle(g, sources, box, q, s):
@@ -79,8 +39,8 @@ def test_layout_table_bit_exact(g):
         if g not in lines_up:
             continue
         sources = make_sources(g, fp8_full(gshape, len(name)), boxes, len(name) + 1)
-        dev_sources, handles = register(g, gshape, sources)
-        sync, q, s, bases = pull_into(g, handles, gshape, box)
+        dev_sources, handles = register_shards(gshape, [(off, sh, sc) for sh, sc, off in sources], granularity=g)
+        sync, q, s, bases = pull_box(handles, gshape, box, E4M3, granularity=g, verbatim=True)
         assert sync._native_plans and not any(sync._fp8_plans), name
         assert_oracle(g, sources, box, q, s)
         assert all(guards_intact(b) for b in bases), name
@@ -112,9 +72,9 @@ def hard_sources(g):
 @pytest.mark.parametrize("g", GRANULARITIES)
 def test_data_a_requantising_pull_would_change(g):
     sources = hard_sources(g)
-    dev_sources, handles = register(g, (2, 256, 512), sources)
+    dev_sources, handles = register_shards((2, 256, 512), [(off, sh, sc) for sh, sc, off in sources], granularity=g)
     box = ((0, 128, 0), (2, 128, 512)) if g == "tensor" else ((0, 0, 256), (2, 256, 256))
-    sync, q, s, bases = pull_into(g, handles, (2, 256, 512), box)
+    sync, q, s, bases = pull_box(handles, (2, 256, 512), box, E4M3, granularity=g, verbatim=True)
     assert_oracle(g, sources, box, q, s)
     # f32(q_dst) * s_dst is the source's, bit for bit: the dequantised values of both sides agree
     want = torch_dequantize(q, s, g, 0, 0, torch.float32)
@@ -169,9 +129,9 @@ def test_source_quantised_chain_and_refresh(g, scale_fmt):
 def test_dequantising_from_the_destination_equals_the_source(g):
     gshape = (384, 512)
     sources = make_sources(g, fp8_full(gshape, 21), rows(gshape, 3), 22)
-    dev_sources, handles = register(g, gshape, sources)
+    dev_sources, handles = register_shards(gshape, [(off, sh, sc) for sh, sc, off in sources], granularity=g)
     box = ((128, 0), (128, 512)) if g == "tensor" else ((0, 256), (384, 256))
-    sync, q, s, _ = pull_into(g, handles, gshape, box)
+    sync, q, s, _ = pull_box(handles, gshape, box, E4M3, granularity=g, verbatim=True)
     from_dest = torch.zeros(box[1], device=DEV)
     back = DirectWeightSyncSource()
     h = back.register({"w": q}, rank=0, tensor_slices={"w": TensorSlice(box[0], (0,), gshape, box[1], (1,))},
@@ -192,8 +152,10 @@ def test_mixed_pull_replay_and_rebuild():
     gshape = (256, 384)
     vb_sources = make_sources("block", fp8_full(gshape, 31), rows(gshape, 2), 32)
     dq_sources = make_sources("channel", fp8_full(gshape, 33), rows(gshape, 2), 34)
-    vb_dev, vb_handles = register("block", gshape, vb_sources, name="vb")
-    dq_dev, dq_handles = register("channel", gshape, dq_sources, name="dq")
+    vb_dev, vb_handles = register_shards(gshape, [(off, sh, sc) for sh, sc, off in vb_sources], granularity="block",
+                                         name="vb")
+    dq_dev, dq_handles = register_shards(gshape, [(off, sh, sc) for sh, sc, off in dq_sources], granularity="channel",
+                                         name="dq")
     plain = (torch.randn(128, 64) * 0.1).to(torch.bfloat16)
     cast = torch.randn(128, 96) * 0.1
     master = (torch.randn(256, 256) * 0.1).to(torch.bfloat16)
@@ -250,7 +212,7 @@ def test_errors_raise_before_anything_is_compiled():
     gshape = (256, 768)
     q_full = fp8_full(gshape, 41)
     sources = make_sources("block", q_full, rows(gshape, 2) + [((64, 0), (128, 768))], 42)
-    dev_sources, all_handles = register("block", gshape, sources)
+    dev_sources, all_handles = register_shards(gshape, [(off, sh, sc) for sh, sc, off in sources], granularity="block")
     handles, overlapping = all_handles[:2], all_handles[2]
     bf16 = DirectWeightSyncSource()
     hb = bf16.register({"w": torch.zeros(256, 768, dtype=torch.bfloat16, device=DEV)}, rank=0)["w"]
@@ -263,7 +225,7 @@ def test_errors_raise_before_anything_is_compiled():
         before = _native.launch_count()
         sync = DirectWeightSyncDest()
         with pytest.raises(exc, match=match):
-            pull_into(g, hs, gshape, box, sync, **kw)
+            pull_box(hs, gshape, box, E4M3, granularity=g, sync=sync, verbatim=True, **kw)
         assert _native.launch_count() == before and sync._plan is None and not sync._native_plans
 
     refuses(ValueError, r"verbatim pull of 'w' \(block_scales\): destination block \(0, 0\).*requantize=True", handles, box)
@@ -312,18 +274,19 @@ def test_put_and_get_state_dict_verbatim():
     run(main())
 
 
-@pytest.mark.skipif(not torch.cuda.is_available() or torch.cuda.device_count() < 2, reason="needs 2 GPUs")
+@needs_two_gpus
 @pytest.mark.parametrize("g", GRANULARITIES)
 def test_weight_and_scale_read_over_peer_mappings(g):
     gshape = (512, 512)
     sources = make_sources(g, fp8_full(gshape, 51), rows(gshape, 4), 52)
     dev_sources, handles = [], []
     for r, sh in enumerate(sources):  # shards alternate between cuda:1 and cuda:0
-        d, h = register(g, gshape, [sh], device=f"cuda:{1 - r % 2}")
+        d, h = register_shards(gshape, [(off, sh, sc) for sh, sc, off in [sh]], granularity=g,
+                               device=f"cuda:{1 - r % 2}")
         dev_sources += d
         handles += h
     box = rows(gshape, 4)[1] if g == "tensor" else ((0, 256), (512, 256))
-    sync, q, s, bases = pull_into(g, handles, gshape, box)
+    sync, q, s, bases = pull_box(handles, gshape, box, E4M3, granularity=g, verbatim=True)
     assert _native.plan_info(sync._native_plans[0]).remote_src_bytes > 0
     assert_oracle(g, sources, box, q, s)
     assert all(guards_intact(b) for b in bases)

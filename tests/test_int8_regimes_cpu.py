@@ -22,7 +22,7 @@ from oracle.ue8m0_oracle import group_amax, group_ids
 from tests import fp8_regimes, quant_pull_regimes, source_quant_regimes
 from tests import test_dequant_fp8_cpu as dq_cpu
 from tests import test_requant_fp8_cpu as rq_cpu
-from tests.helpers import region
+from tests.helpers import dest_scale_shape, region
 from tests.test_quant_pull_regimes_cpu import host_shard, workload_inputs
 from tests.test_source_quant_cpu import host_shard as source_shard
 from tests.test_source_quant_regimes_cpu import workload_inputs as source_inputs
@@ -90,7 +90,7 @@ def quant_pull(name):
                       for r, (off, loc) in enumerate(p.src)]
         off, loc = p.dst
         dests[n] = torch.full(loc, 0x55, dtype=torch.int8)
-        scales[n] = torch.full(quant_pull_regimes.scale_shape(p.g, loc), -1.0)
+        scales[n] = torch.full(dest_scale_shape(p.g, loc), -1.0)
         slices[n] = TensorSlice(off, (0,), p.shape, loc, (1,))
     ops = DirectWeightSyncDest()._build_plan(handles, dests, slices)
     with fp8_compared("dst_dtype") as seen:

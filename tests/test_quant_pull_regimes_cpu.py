@@ -10,8 +10,8 @@ import pytest
 import torch
 
 from oracle import block_fp8_oracle, scaled_fp8_oracle
-from tests.helpers import rand_full, region
-from tests.quant_pull_regimes import REGIMES, WORKLOADS, compile_tables, plan_bytes, scale_shape, spots
+from tests.helpers import dest_scale_shape, rand_full, region
+from tests.quant_pull_regimes import REGIMES, WORKLOADS, compile_tables, plan_bytes, spots
 from torchstore_b200.direct_weight_sync import DirectWeightSyncDest, RDMAWeightHandle
 from torchstore_b200.planner import StridedMem
 from torchstore_b200.transport.types import TensorSlice
@@ -76,7 +76,7 @@ def compiled(name, flags=0):
                       for r, (off, loc) in enumerate(p.src)]
         off, loc = p.dst
         dests[n] = torch.zeros(loc, dtype=E4M3)
-        scales[n] = torch.zeros(scale_shape(p.g, loc), dtype=torch.float32)
+        scales[n] = torch.zeros(dest_scale_shape(p.g, loc), dtype=torch.float32)
         slices[n] = TensorSlice(off, (0,), p.shape, loc, (1,))
     ops = DirectWeightSyncDest()._build_plan(handles, dests, slices)
     tables, geom = compile_tables(w.pulls, ops, handles, StridedMem.from_tensor, dests, scales, flags)

@@ -15,8 +15,8 @@ import torch
 from oracle.dequant_fp8_oracle import GRANULARITIES, scale_shape
 from oracle.requant_fp8_oracle import (PAIRS, canonical_nan, digest, fixture_inputs, quantize, replay, requantize,
                                        torch_requantize)
-from tests.helpers import (Boom, cuda_like, expect_invalid, no_compile, plan_windows, region, shard_box,
-                           shard_handles)
+from tests.helpers import (Boom, cuda_like, dest_scale_shape, expect_invalid, no_compile, plan_windows, region,
+                           shard_box, shard_handles)
 from torchstore_b200 import _native
 from torchstore_b200.direct_weight_sync import BLOCK, DirectWeightSyncDest, RDMAWeightHandle
 from torchstore_b200.planner import StridedMem, build_rects
@@ -80,11 +80,6 @@ def local_scale(full_scale, g, off, loc):
     if g == "channel":
         return full_scale[lead_idx + (slice(r0, r0 + n),)].contiguous().reshape(*lead, n, 1)
     return full_scale[lead_idx].contiguous()
-
-
-def dest_scale_shape(g, loc):
-    *lead, n, k = loc
-    return {"block": (*lead, -(-n // BLOCK), -(-k // BLOCK)), "channel": (*lead, n, 1), "tensor": tuple(lead)}[g]
 
 
 class FakeScaledBuffer:

@@ -12,7 +12,8 @@ import pytest
 import torch
 
 from oracle.scaled_fp8_oracle import GRANULARITIES, bits_of, digest, fixture_inputs, quantize, replay, torch_quantize, widen
-from tests.helpers import HostBuffer, expect_invalid, plan_windows, rand_full, region, shard_box, shard_handles
+from tests.helpers import (HostBuffer, dest_scale_shape, expect_invalid, plan_windows, rand_full, region, shard_box,
+                           shard_handles)
 from torchstore_b200 import _native
 from torchstore_b200.planner import StridedMem, build_rects
 
@@ -106,11 +107,6 @@ def test_torch_rendering_matches_the_oracle_on_finite_data(case):
 
 
 # ---- the plan compiler, replayed on host memory ----------------------------------------------------
-def scale_shape(loc, g):
-    *lead, n, _ = loc
-    return (*lead, n, 1) if g == "channel" else tuple(lead)
-
-
 def compile_pull(full, src_boxes, dst_box, g):
     """Plan (product planner, host memory) a pull of `full`'s `src_boxes` shards into the fp8
     destination `dst_box`; returns (dest, scale, (bands, pieces, tiles, n_groups), keepalive)."""
@@ -118,7 +114,7 @@ def compile_pull(full, src_boxes, dst_box, g):
     loc = dst_box[1]
     dest = torch.zeros(loc, dtype=E4M3)
     n, k = loc[-2:]
-    scale = torch.zeros(scale_shape(loc, g), dtype=torch.float32)
+    scale = torch.zeros(dest_scale_shape(g, loc), dtype=torch.float32)
     _, pairs = plan_windows(handles, dest, dst_box)
     rects, nr = build_rects(pairs)
     targets = _native.make_sq_target_array(1)

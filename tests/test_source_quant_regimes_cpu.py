@@ -12,9 +12,9 @@ import torch
 
 from oracle import dequant_fp8_oracle, requant_fp8_oracle
 from oracle.source_quant_oracle import GRANULARITIES, bits_of, element_scales, quantize, replay, synth_f32, widen
-from tests.helpers import plan_windows, region, shard_box
+from tests.helpers import dest_scale_shape, plan_windows, region, shard_box
 from tests.source_quant_regimes import REGIMES, WORKLOADS, plan_bytes
-from tests.test_requant_fp8_cpu import CODE, FakeScaledBuffer, dest_scale_shape
+from tests.test_requant_fp8_cpu import CODE, FakeScaledBuffer
 from tests.test_source_quant_cpu import compile_host, host_shard
 from torchstore_b200 import _native
 from torchstore_b200.direct_weight_sync import RDMAWeightHandle
